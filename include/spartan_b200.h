@@ -61,9 +61,6 @@ int sp_comm_export(sp_ctx* ctx, uint8_t* handle_out);
 int sp_comm_connect(sp_ctx* ctx, int rank, int world, const uint8_t* handles /* world x sp_comm_handle_bytes() */);
 int sp_comm_info(const sp_ctx* ctx, int* rank, int* world);
 int sp_comm_set_enabled(sp_ctx* ctx, int enabled);   /* 0: the next prove calls run on this rank's GPU alone (all ranks must switch together) */
-/* self-test of the host helper threads that share the single-point commitments of a ZK sumcheck round (engine.hpp: HostPool; SP_HOST_THREADS=0 disables
- * them): runs `iterations` small jobs sets, returns the number of jobs that did not run exactly once; *helpers = number of helper threads.  No GPU needed. */
-int sp_host_pool_selftest(int iterations, int* helpers);
 /* 1 (default): SNARK::prove commits to the dereferenced SPARK values on a background stream underneath the latency-bound rounds that precede the
  * commitment in the transcript (same bytes, shorter proof); 0: every kernel on the context's stream, one after the other (per-kernel profiling) */
 int sp_ctx_set_overlap(sp_ctx* ctx, int enabled);

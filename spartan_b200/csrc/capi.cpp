@@ -78,21 +78,6 @@ int sp_comm_connect(sp_ctx* ctx, int rank, int world, const uint8_t* handles) {
   SP_CATCH(ctx)
 }
 int sp_comm_set_enabled(sp_ctx* ctx, int enabled) { ctx->c.shard_enabled = enabled != 0; return SP_OK; }
-int sp_host_pool_selftest(int iterations, int* helpers) {   // runs on the CPU: every job of every run must execute exactly once
-  HostPool& p = HostPool::get();
-  if (helpers) *helpers = p.helpers();
-  int bad = 0;
-  for (int it = 0; it < iterations; it++) {
-    const int n = 1 + it % 6;
-    std::atomic<int> sum{0};
-    int hit[8] = {0};
-    p.run(n, [&](int i) { hit[i]++; sum.fetch_add(i + 1); });
-    if (sum.load() != n * (n + 1) / 2) bad++;
-    for (int i = 0; i < n; i++) if (hit[i] != 1) bad++;
-    if (it % 20000 == 19999) std::this_thread::sleep_for(std::chrono::milliseconds(1));   // lets the helpers fall asleep once in a while
-  }
-  return bad;
-}
 int sp_ctx_set_overlap(sp_ctx* ctx, int enabled) { ctx->c.overlap = enabled != 0; return SP_OK; }
 int sp_comm_info(const sp_ctx* ctx, int* rank, int* world) { *rank = ctx->c.rank(); *world = ctx->c.world(); return SP_OK; }
 

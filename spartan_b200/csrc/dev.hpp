@@ -20,8 +20,6 @@ int device_count();
 void set_device(int dev);
 cudaStream_t stream_create();
 cudaStream_t stream_create_prio(int level);   // > 0: greatest priority of the device, < 0: least
-// a stream confined to `sms` SMs (green context); nullptr when unsupported; *sms_granted = the SM count of the partition
-cudaStream_t stream_create_partition(int sms, int level, int* sms_granted);
 void stream_wait_event(cudaStream_t s, void* ev);
 void stream_destroy(cudaStream_t s);
 void stream_sync(cudaStream_t s);
@@ -107,17 +105,6 @@ void sc_fold_eval_g(const ScInst* d_insts, int ninst, size_t len, const u256& r,
 // levels[k-1] (k = 1..K, back to back, n0 >> k entries each) = eq(tau[k+1..], .) from E0 = eq(tau[1..], .) of n0 entries
 size_t eq_suffix_entries(size_t n0, int K);
 void eq_suffix(u256* levels, const u256* E0, size_t n0, int K, cudaStream_t s);
-// ---- persistent tail of a batched cubic sumcheck (prove_cubic_batched, sumcheck.rs:254-424, once the tables are small): ONE launch runs all the
-// remaining rounds.  CTA i owns instance i (tables A, B and a private copy of C); after every bind it publishes the instance's evaluations to
-// the host (HostSig, sequence numbers sig.seq, sig.seq+1, ...), then spins on a mailbox in mapped pinned host memory until the host has derived
-// the next challenge from the transcript.  After the last bind it publishes the bound heads A[0], B[0], C[0] instead.  No launch, no cold
-// caches and no kernel drain between rounds: a round costs the PCIe round trip plus a few microseconds of arithmetic.
-struct PersistMail { u256 r; unsigned int seq; unsigned int pad[7]; };
-// One CTA (one SM) per instance: worth it only while a round is latency, not throughput (<= 256 entries: one bind task per thread)
-#define SC_PERSIST_MAX_LEN 256
-// dmail: a device-memory copy of the mailbox (zero-initialised, reused across launches): only CTA 0 polls the host over PCIe and forwards the challenge
-void sc_persist(const ScInst* insts, int ninst, int n_shared_c /* instances [0, n_shared_c) read the shared C table */, u256* c_scratch /* n_shared_c * len */,
-                size_t len, const u256& r0, const PersistMail* mail, PersistMail* dmail, unsigned int mail_seq0, u256* out, cudaStream_t s, HostSig sig);
 // fold only (bound_poly_var_top, dense_mlpoly.rs:215-223): tables[k][i] += r*(tables[k][i+len/2]-tables[k][i])
 void fold_top(u256* const* d_tables, int ntables, size_t len, const u256& r, cudaStream_t s);
 void fold_top_single(u256* table, size_t len, const u256& r, cudaStream_t s);
@@ -197,11 +184,10 @@ void sum_points(ge* out, const ge* in, int n, cudaStream_t s);   // out[0] = in[
 // scratch >= ipa_msm_scratch_points(n_full, wbits) points; ticket: one zero-initialised word (self-resetting)
 size_t ipa_msm_scratch_points(size_t n_full, int wbits);
 void ipa_msm(ge* out, const ge_niels* table, int wbits, const u256* a, const u256* svec, size_t n_cur, size_t n_full, void* scratch, unsigned int* ticket,
-             cudaStream_t s, HostSig sig = HostSig(), int max_ctas = 0 /* > 0: cap on the blocks of the quad-lane kernel (both sides together) */,
-             // b != null (only when ipa_msm_fuses_dots()): the same launch also computes c_out[0] = <a_L, b_R>, c_out[1] = <a_R, b_L> of the round and
+             cudaStream_t s, HostSig sig = HostSig(),
+             // b != null: the same launch also computes c_out[0] = <a_L, b_R>, c_out[1] = <a_R, b_L> of the round and
              // publishes them through sigc (its own flag word and completion counter), instead of a separate dot_pairs launch in front of the MSM
              const u256* b = nullptr, u256* c_out = nullptr, HostSig sigc = HostSig());
-bool ipa_msm_fuses_dots();
 
 // ---- variable-base MSM on arbitrary points (bucket method; kernels_pip.cu).  pts: affine-niels form of the caller's points.
 struct PipPlan { size_t n = 0; int c = 0, nwin = 0, G = 32; uint32_t nb = 0; size_t tile = 0, ntiles = 0, S = 0, max_items = 0; };

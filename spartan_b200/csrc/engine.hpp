@@ -1,10 +1,5 @@
 // spartan_b200 — device context, buffers and generator sets shared by the host prover.
 #pragma once
-#include <atomic>
-#include <condition_variable>
-#include <functional>
-#include <mutex>
-#include <thread>
 #include <chrono>
 #include <cstdlib>
 #include <map>
@@ -87,8 +82,6 @@ struct Ctx {
   // to the dereferenced SPARK values runs there under the second sumcheck phase and the witness evaluation proof (snark.cpp)
   cudaStream_t stream2 = nullptr;
   bool overlap = true;                 // sp_ctx_set_overlap: 0 keeps every kernel on the prover's stream (profiling: per-kernel event times free of concurrent work)
-  bool bg_busy = false;                // between fork and join of background work (snark.cpp): latency kernels shape their grids for the free SMs
-  int stream2_sms = 0;                 // > 0: stream2 is confined to that many SMs (green context); 0: it shares every SM with the prover's stream
   void* ev_fork = nullptr; void* ev_join = nullptr;
   DevBuf<uint8_t> scratch2;        // MSM partial sums of the background stream
   uint8_t* pinned = nullptr;       // staging for small host<->device exchanges
@@ -113,15 +106,6 @@ struct Ctx {
   unsigned int sigc_seq = 0;           // sequence of the second flag word (host_flag + 16)
   dev::HostSig next_sig() { dev::HostSig s; s.host_out = host_res; s.flag = host_flag; s.done = sig_done.p; s.seq = ++sig_seq; return s; }
   void wait_sig(const dev::HostSig& s);   // spins on the flag; falls back to a stream synchronise to surface CUDA errors
-  // host -> persistent-kernel mailbox (dev::sc_persist): the next challenge and its sequence number, in mapped pinned memory
-  dev::PersistMail* mail = nullptr;
-  DevBuf<dev::PersistMail> dmail;      // device-side copy the polling CTA forwards the challenge through
-  unsigned int mail_seq = 0;
-  void post_challenge(const Fq& r) {
-    memcpy((void*)&mail->r, &r.m, sizeof(u256));
-    std::atomic_thread_fence(std::memory_order_release);
-    *((volatile unsigned int*)&mail->seq) = ++mail_seq;
-  }
   void sync() { dev::stream_sync(stream); }
   void ensure_scratch(size_t bytes) { if (scratch.n < bytes) { sync(); scratch.alloc(bytes); } }
   // upload k scalars to small[slot..]
@@ -182,33 +166,6 @@ struct GenSet {
 struct CommitKey {
   const GenSet* set = nullptr;
   size_t off = 0, n = 0, h = 0;
-};
-
-// A few helper threads for the host's single-point commitments (process-wide, created on first use).  The ZK sumcheck rounds are host-bound: between a
-// round's evaluations and its challenge the prover thread commits to the four coefficients of the round polynomial — four independent fixed-base scalar
-// multiplications of ~4 us each.  run(n, fn) executes fn(0) .. fn(n-1), fn(0) on the caller and the rest on helpers that spin for work while proofs are in
-// flight (they fall asleep on a condition variable after ~200 us without any).  SP_HOST_THREADS=<n> switches them on (default 0: the
-// hand-over costs about what the parallel scalar multiplications save); results do not depend on it (group addition is commutative, encodings are canonical).
-class HostPool {
- public:
-  static HostPool& get();
-  int helpers() const { return (int)th_.size(); }
-  void run(int njobs, const std::function<void(int)>& fn);
-  ~HostPool();
- private:
-  HostPool();
-  void worker();
-  std::vector<std::thread> th_;
-  std::atomic<uint64_t> epoch_{0};
-  // next_ = (run tag << 32) | next job index, desc_ = (run tag << 32) | job count: a helper that drew an index from an earlier run's counter sees the
-  // tag mismatch and drops it (index and job count are never read from two different runs)
-  std::atomic<uint64_t> next_{0}, desc_{0};
-  std::atomic<int> pending_{0}, sleepers_{0};
-  std::atomic<bool> stop_{false};
-  std::atomic<const std::function<void(int)>*> fn_{nullptr};
-  uint64_t tag_ = 0;                   // caller side only
-  std::mutex mu_;
-  std::condition_variable cv_;
 };
 
 struct Term { size_t base; Fq k; };

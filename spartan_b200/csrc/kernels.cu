@@ -13,8 +13,6 @@
 //   K7     eq_evals, dot, bound_rows, lincomb3, hadamard, spmv, SPARK hash layer, IPA helpers.
 // All arithmetic is exact 256-bit integer work on the INT32 pipe; no tensor-core formulation exists (DESIGN.md).
 #include <cuda_runtime.h>
-#include <cstdio>
-#include <cuda.h>
 #include <stdexcept>
 #include <string>
 #include <map>
@@ -83,50 +81,6 @@ cudaStream_t stream_create_prio(int level) {
   cudaStream_t s;
   ck(cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, level > 0 ? greatest : (level < 0 ? least : (least + greatest) / 2)), "cudaStreamCreateWithPriority");
   return s;
-}
-// A stream whose kernels run on a fixed subset of `sms` SMs (a CUDA green context carved out of the device's SM resource; driver entry points are
-// resolved at run time so that the library has no link-time dependency on libcuda).  The remaining SMs are never touched by work on this stream, so
-// the short kernels of the prover's stream find idle SMs however long the background MSMs run.  Returns nullptr when the driver cannot do it.
-cudaStream_t stream_create_partition(int sms, int level, int* sms_granted) {
-  typedef CUresult (*GetRes)(CUdevice, CUdevResource*, CUdevResourceType);
-  typedef CUresult (*Split)(CUdevResource*, unsigned int*, const CUdevResource*, CUdevResource*, unsigned int, unsigned int);
-  typedef CUresult (*GenDesc)(CUdevResourceDesc*, CUdevResource*, unsigned int);
-  typedef CUresult (*GreenCreate)(CUgreenCtx*, CUdevResourceDesc, CUdevice, unsigned int);
-  typedef CUresult (*GreenStream)(CUstream*, CUgreenCtx, unsigned int, int);
-  typedef CUresult (*DevGet)(CUdevice*, int);
-  auto ep = [](const char* name) -> void* {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult st;
-    if (cudaGetDriverEntryPoint(name, &f, cudaEnableDefault, &st) != cudaSuccess || st != cudaDriverEntryPointSuccess) { cudaGetLastError(); return nullptr; }
-    return f;
-  };
-  GetRes get_res = (GetRes)ep("cuDeviceGetDevResource");
-  Split split = (Split)ep("cuDevSmResourceSplitByCount");
-  GenDesc gen = (GenDesc)ep("cuDevResourceGenerateDesc");
-  GreenCreate gcreate = (GreenCreate)ep("cuGreenCtxCreate");
-  GreenStream gstream = (GreenStream)ep("cuGreenCtxStreamCreate");
-  DevGet devget = (DevGet)ep("cuDeviceGet");
-  if (!get_res || !split || !gen || !gcreate || !gstream || !devget) return nullptr;
-  int ord = 0;
-  cudaGetDevice(&ord);
-  cudaFree(0);   // the primary context must exist
-  CUdevice dev;
-  if (devget(&dev, ord) != CUDA_SUCCESS) return nullptr;
-  CUdevResource all, grp, rem;
-  if (get_res(dev, &all, CU_DEV_RESOURCE_TYPE_SM) != CUDA_SUCCESS) return nullptr;
-  if (sms < 8 || (unsigned)sms >= all.sm.smCount) return nullptr;
-  unsigned int nb = 1;
-  if (split(&grp, &nb, &all, &rem, 0, (unsigned)sms) != CUDA_SUCCESS || nb < 1) return nullptr;
-  CUdevResourceDesc desc;
-  if (gen(&desc, &grp, 1) != CUDA_SUCCESS) return nullptr;
-  CUgreenCtx g;
-  if (gcreate(&g, desc, dev, CU_GREEN_CTX_DEFAULT_STREAM) != CUDA_SUCCESS) return nullptr;   // lives as long as the process (one per prover context)
-  int least = 0, greatest = 0;
-  cudaDeviceGetStreamPriorityRange(&least, &greatest);
-  CUstream st;
-  if (gstream(&st, g, CU_STREAM_NON_BLOCKING, level > 0 ? greatest : least) != CUDA_SUCCESS) return nullptr;
-  if (sms_granted) *sms_granted = (int)grp.sm.smCount;
-  return (cudaStream_t)st;
 }
 void stream_wait_event(cudaStream_t s, void* ev) { ck(cudaStreamWaitEvent(s, (cudaEvent_t)ev, 0), "cudaStreamWaitEvent"); }
 void stream_destroy(cudaStream_t s) { cudaStreamDestroy(s); }
@@ -722,88 +676,6 @@ void sum_points(ge* out, const ge* in, int n, cudaStream_t s) {
   k_msm_reduce_small<<<1, 32, 0, s>>>(out, in, n);
   SP_LAUNCHED(); check("sum_points");
 }
-// ---- the two MSMs of one inner-product round in a single launch (bullet.rs:83-97 with unfolded generators, see k_ipa_lr):
-// every generator j carries exactly one non-zero scalar, a[.]*s[j], for L (j in the right half of its n_cur-block) or for R (left half).
-// grid = (chunks, 2 sides); the last block to finish sums the partial points of both sides and publishes L, R to the host.
-// (latency-bound: 256 CTAs of which each thread makes <= 3 mixed additions and then two point-addition trees; no register cap, so that ptxas can
-//  keep the four independent field products of a point addition in flight together)
-#ifndef SP_IPA_LB
-#define SP_IPA_LB 1
-#endif
-template <int WBITS, int GROUPS>
-__global__ void __launch_bounds__(128, SP_IPA_LB) k_ipa_msm(ge* partial, const ge_niels* __restrict__ table, const u256* __restrict__ a, const u256* __restrict__ sv,
-                                                           size_t n_cur, size_t n_full, unsigned int* ticket, ge* out, HostSig sig) {
-  constexpr int NWIN = (253 + WBITS - 1) / WBITS;
-  constexpr int WPT = (NWIN + GROUPS - 1) / GROUPS;
-  constexpr int COLS = 128 / GROUPS;
-  constexpr uint32_t HALF = 1u << (WBITS - 1);
-  constexpr size_t DEPTH = (size_t)1 << (WBITS - 1);
-  const int side = blockIdx.y;
-  const size_t half = n_cur >> 1, total = n_full >> 1;
-  const int g = threadIdx.x % GROUPS;
-  const size_t t = (size_t)blockIdx.x * COLS + threadIdx.x / GROUPS;
-  ge acc = ge_identity();
-  if (t < total) {
-    const size_t blk = t / half, off = t - blk * half;
-    const size_t j = blk * n_cur + off + (side == 0 ? half : 0);
-    u256 k = fq_mul(ld256_ro(a + (side == 0 ? off : off + half)), ld256_ro(sv + j));
-    if (!fq_is_zero(k)) {
-      k = fq_from_mont(k);
-      uint32_t carry = 0;
-      for (int w = 0; w < g * WPT; w++) carry = (msm_window<WBITS>(k, w) + carry) > HALF ? 1u : 0u;
-      const int w_end = (g + 1) * WPT < NWIN ? (g + 1) * WPT : NWIN;
-      const ge_niels* tb = table + (j * NWIN + (size_t)g * WPT) * DEPTH;
-#pragma unroll 1
-      for (int w = g * WPT; w < w_end; w++, tb += DEPTH) {
-        uint32_t v = msm_window<WBITS>(k, w) + carry;
-        int d;
-        if (v > HALF) { d = (int)v - (int)(2 * HALF); carry = 1; } else { d = (int)v; carry = 0; }
-        if (d == 0) continue;
-        int ad = d < 0 ? -d : d;
-        const ge_niels* e = tb + (ad - 1);
-        ge_niels nl;
-        nl.ypx = ld256_ro(&e->ypx); nl.ymx = ld256_ro(&e->ymx); nl.t2d = ld256_ro(&e->t2d);
-        acc = ge_madd(acc, nl, d < 0);
-      }
-    }
-  }
-  acc = block_sum_ge_128(acc);
-  __shared__ bool is_last;
-  if (threadIdx.x == 0) {
-    st_ge(partial + (size_t)side * gridDim.x + blockIdx.x, acc);
-    __threadfence();
-    is_last = atomicAdd(ticket, 1u) == 2 * gridDim.x - 1;
-  }
-  __syncthreads();
-  if (!is_last) return;
-  __threadfence();
-  const int s2 = threadIdx.x >> 6, tt = threadIdx.x & 63;   // threads 0..63 finish L, 64..127 finish R
-  ge r = ge_identity();
-  for (unsigned int c = tt; c < gridDim.x; c += 64) {
-    const ge* p = partial + (size_t)s2 * gridDim.x + c;
-    ge x;
-    x.X = ld256_cg(&p->X); x.Y = ld256_cg(&p->Y); x.Z = ld256_cg(&p->Z); x.T = ld256_cg(&p->T);
-    r = ge_add(r, x);
-  }
-#pragma unroll 1
-  for (int d = 16; d > 0; d >>= 1) r = ge_add(r, shfl_down_ge(r, d));
-  __shared__ ge fin[4];
-  if ((threadIdx.x & 31) == 0) fin[threadIdx.x >> 5] = r;
-  __syncthreads();
-  if (tt == 0) {
-    r = ge_add(fin[2 * s2], fin[2 * s2 + 1]);
-    st_ge(out + s2, r);
-    if (sig.host_out) {
-      st256(sig.host_out + 4 * s2, r.X); st256(sig.host_out + 4 * s2 + 1, r.Y); st256(sig.host_out + 4 * s2 + 2, r.Z); st256(sig.host_out + 4 * s2 + 3, r.T);
-      __threadfence_system();
-    }
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    *ticket = 0;
-    if (sig.flag) { __threadfence_system(); *((volatile unsigned int*)sig.flag) = sig.seq; }
-  }
-}
 // ---- quad-lane point arithmetic for latency-bound reductions.
 // A lone warp gains nothing from the four independent field products of a point addition (9 products
 // back to back), so a reduction tree of point additions costs 9 product latencies per level.  Here FOUR LANES share one point — lane c of a quad holds coordinate
@@ -868,7 +740,9 @@ __device__ __forceinline__ u256 quad_warp_sum(u256 P, int c, int lane) {
   for (int d = 16; d >= 4; d >>= 1) P = quad_add(P, shfl_down_256(P, d), c, lane);
   return P;
 }
-// Both MSMs of an inner-product round, quad-lane formulation of k_ipa_msm (same inputs, same outputs).  grid = (chunks, 2 sides), IPAQ_THREADS
+// ---- the two MSMs of one inner-product round in a single launch (bullet.rs:83-97 with unfolded generators, see k_ipa_lr):
+// every generator j carries exactly one non-zero scalar, a[.]*s[j], for L (j in the right half of its n_cur-block) or for R (left half).
+// Quad-lane formulation: grid = (chunks, 2 sides), IPAQ_THREADS
 // threads = IPAQ_THREADS/4 quads; a quad owns WPQ adjacent windows of one scalar and chains their table entries by mixed additions (two product
 // latencies each), then 3 tree levels inside the warp, one gather + 3 levels across the warps, and the last block to finish sums the blocks' partial
 // points of both sides.  WPQ balances the two costs: a lone warp already keeps much of its
@@ -921,17 +795,9 @@ __global__ void __launch_bounds__(IPAQ_THREADS, 2) k_ipa_msm_quad(ge* partial, c
   const int side = blockIdx.y, tid = threadIdx.x, lane = tid & 31, c = lane & 3, warp = tid >> 5;
   const size_t half = n_cur >> 1, total = n_full >> 1;
   const size_t total_quads = total * QPS, stride = (size_t)gridDim.x * QPB;
-#ifdef SP_IPA_TIMELINE
-  unsigned long long tl[10];
-  int tli = 0;
-#define SP_TL() do { if (tid == 0) tl[tli++] = global_timer_ns(); } while (0)
-#else
-#define SP_TL() do { } while (0)
-#endif
-  SP_TL();
   u256 P = quad_identity(c);
   // grid-stride over the (scalar, window group) work items with the same trip count in every quad (the shuffles inside quad_madd need the whole
-  // warp): a launch may be capped to fewer blocks than work items (the prover does that while a background MSM occupies most SMs)
+  // warp)
   for (size_t g0 = (size_t)blockIdx.x * QPB; g0 < total_quads; g0 += stride) {
     const size_t gq = g0 + (tid >> 2);
     const size_t t = gq / QPS;
@@ -945,7 +811,6 @@ __global__ void __launch_bounds__(IPAQ_THREADS, 2) k_ipa_msm_quad(ge* partial, c
       k = fq_mul(ld256_ro(a + (side == 0 ? off : off + half)), ld256_ro(sv + j));
       if (!fq_is_zero(k)) k = fq_from_mont(k);
     }
-    SP_TL();
     uint32_t carry = 0;
     for (int w = 0; w < w0; w++) carry = (msm_window<WBITS>(k, w) + carry) > HALF ? 1u : 0u;
     const ge_niels* tb = table + (j * NWIN + (size_t)w0) * DEPTH;
@@ -967,13 +832,10 @@ __global__ void __launch_bounds__(IPAQ_THREADS, 2) k_ipa_msm_quad(ge* partial, c
         }
       }
     }
-    SP_TL();
 #pragma unroll
     for (int h = 0; h < WPQ; h++) P = quad_madd(P, x[h], c, lane);
   }
-  SP_TL();
   P = quad_warp_sum(P, c, lane);
-  SP_TL();
   __shared__ u256 sm[NWARP][4];
   __shared__ bool is_last;
   if (lane < 4) sm[warp][c] = P;
@@ -987,12 +849,6 @@ __global__ void __launch_bounds__(IPAQ_THREADS, 2) k_ipa_msm_quad(ge* partial, c
     if (lane == 0) is_last = atomicAdd(ticket, 1u) == 2 * gridDim.x - 1;
   }
   __syncthreads();
-  SP_TL();
-#ifdef SP_IPA_TIMELINE
-  if (tid == 0 && !is_last && blockIdx.x == 0 && blockIdx.y == 0 && n_cur == n_full)
-    printf("ipa_tl %s blk(%d,%d) n=%llu: prep %llu loads+digits %llu madds %llu warp_tree %llu cross+ticket %llu ns (start %llu)\n", is_last ? "LAST" : "first", blockIdx.x, blockIdx.y,
-           (unsigned long long)n_full, tl[1] - tl[0], tl[2] - tl[1], tl[3] - tl[2], tl[4] - tl[3], tl[5] - tl[4], tl[0]);
-#endif
   if (!is_last) return;
   __threadfence();
   // last block: the first half of its quads finishes L, the second half R
@@ -1019,64 +875,33 @@ __global__ void __launch_bounds__(IPAQ_THREADS, 2) k_ipa_msm_quad(ge* partial, c
     }
   }
   __syncthreads();
-#ifdef SP_IPA_TIMELINE
-  if (tid == 0 && n_cur == n_full) {
-    unsigned long long te = global_timer_ns();
-    printf("ipa_tl LAST blk(%d,%d) n=%llu: prep %llu loads+digits %llu madds %llu warp_tree %llu cross+ticket %llu final %llu ns, span %llu ns\n", blockIdx.x, blockIdx.y, (unsigned long long)n_full,
-           tl[1] - tl[0], tl[2] - tl[1], tl[3] - tl[2], tl[4] - tl[3], tl[5] - tl[4], te - tl[5], te - tl[0]);
-  }
-#endif
   if (tid == 0) {
     *ticket = 0;
     if (sig.flag) { __threadfence_system(); *((volatile unsigned int*)sig.flag) = sig.seq; }
   }
 }
-#undef SP_TL
 // windows per quad: the window count split into three groups (17 -> 6, 20 -> 7, 32 -> 11)
 template <int WBITS> struct IpaQ { static constexpr int NWIN = (253 + WBITS - 1) / WBITS, WPQ = (NWIN + SP_IPAQ_SPLIT - 1) / SP_IPAQ_SPLIT, QPS = (NWIN + WPQ - 1) / WPQ; };
 template <int WBITS>
 static void ipa_msm_quad_launch(ge* out, const ge_niels* table, const u256* a, const u256* svec, size_t n_cur, size_t n_full, void* scratch, unsigned int* ticket,
-                                cudaStream_t s, HostSig sig, int max_ctas, const u256* b, u256* c_out, HostSig sigc) {
+                                cudaStream_t s, HostSig sig, const u256* b, u256* c_out, HostSig sigc) {
   const size_t quads = (n_full / 2) * IpaQ<WBITS>::QPS, qpb = IPAQ_THREADS / 4;
   dim3 grid((unsigned)((quads + qpb - 1) / qpb), 2);
-  if (max_ctas >= 2 && grid.x > (unsigned)max_ctas / 2) grid.x = (unsigned)max_ctas / 2;   // the kernel strides over the work items
   if (b) { grid.y = 3; if (grid.x < 2) grid.x = 2; }        // a third row of blocks, of which two compute the round's dot products
   k_ipa_msm_quad<WBITS, IpaQ<WBITS>::WPQ><<<grid, IPAQ_THREADS, 0, s>>>((ge*)scratch, table, a, svec, n_cur, n_full, ticket, out, sig, b, c_out, sigc);
 }
-#ifndef SP_IPA_QUAD_DEFAULT
-#define SP_IPA_QUAD_DEFAULT 1
-#endif
-bool ipa_msm_fuses_dots() {   // true when ipa_msm can compute the round's two dot products in the same launch (quad-lane kernel)
-  static const bool quad = [] { const char* e = getenv("SP_IPA_QUAD"); return e ? atoi(e) != 0 : SP_IPA_QUAD_DEFAULT != 0; }();
-  static const bool fuse = getenv("SP_IPA_NO_FUSED_DOT") == nullptr;
-  return quad && fuse;
-}
-size_t ipa_msm_scratch_points(size_t n_full, int wbits) {   // partial points of either formulation
+size_t ipa_msm_scratch_points(size_t n_full, int wbits) {   // partial points of the quad-lane kernel (>= 2 blocks per side when the dots are fused)
   const size_t nwin = (size_t)msm_nwin(wbits), total = n_full / 2, wpq = (nwin + SP_IPAQ_SPLIT - 1) / SP_IPAQ_SPLIT, qps = (nwin + wpq - 1) / wpq;
-  const size_t quad_chunks = (total * qps + IPAQ_THREADS / 4 - 1) / (IPAQ_THREADS / 4), plain_chunks = (total + 15) / 16;
-  return 2 * std::max(quad_chunks, plain_chunks);
+  return 2 * std::max<size_t>((total * qps + IPAQ_THREADS / 4 - 1) / (IPAQ_THREADS / 4), 2);
 }
 void ipa_msm(ge* out, const ge_niels* table, int wbits, const u256* a, const u256* svec, size_t n_cur, size_t n_full, void* scratch, unsigned int* ticket,
-             cudaStream_t s, HostSig sig, int max_ctas, const u256* b, u256* c_out, HostSig sigc) {
+             cudaStream_t s, HostSig sig, const u256* b, u256* c_out, HostSig sigc) {
   ProfScope ps("ipa_msm", 64.0 * (double)n_full, s);
-  static const bool quad = [] { const char* e = getenv("SP_IPA_QUAD"); return e ? atoi(e) != 0 : SP_IPA_QUAD_DEFAULT != 0; }();
-  if (quad) {
-    if (wbits == 8) ipa_msm_quad_launch<8>(out, table, a, svec, n_cur, n_full, scratch, ticket, s, sig, max_ctas, b, c_out, sigc);
-    else if (wbits == 13) ipa_msm_quad_launch<13>(out, table, a, svec, n_cur, n_full, scratch, ticket, s, sig, max_ctas, b, c_out, sigc);
-    else if (wbits == 15) ipa_msm_quad_launch<15>(out, table, a, svec, n_cur, n_full, scratch, ticket, s, sig, max_ctas, b, c_out, sigc);
-    else throw std::runtime_error("spartan_b200: unsupported MSM window width");
-    SP_LAUNCHED(); check("ipa_msm_quad");
-    return;
-  }
-  if (b) throw std::runtime_error("spartan_b200: the fused dot products need the quad-lane inner-product kernel");
-  constexpr int GROUPS = 8;
-  const size_t cols = 128 / GROUPS, total = n_full / 2;
-  dim3 grid((unsigned)((total + cols - 1) / cols), 2);
-  if (wbits == 8) k_ipa_msm<8, GROUPS><<<grid, 128, 0, s>>>((ge*)scratch, table, a, svec, n_cur, n_full, ticket, out, sig);
-  else if (wbits == 13) k_ipa_msm<13, GROUPS><<<grid, 128, 0, s>>>((ge*)scratch, table, a, svec, n_cur, n_full, ticket, out, sig);
-  else if (wbits == 15) k_ipa_msm<15, GROUPS><<<grid, 128, 0, s>>>((ge*)scratch, table, a, svec, n_cur, n_full, ticket, out, sig);
+  if (wbits == 8) ipa_msm_quad_launch<8>(out, table, a, svec, n_cur, n_full, scratch, ticket, s, sig, b, c_out, sigc);
+  else if (wbits == 13) ipa_msm_quad_launch<13>(out, table, a, svec, n_cur, n_full, scratch, ticket, s, sig, b, c_out, sigc);
+  else if (wbits == 15) ipa_msm_quad_launch<15>(out, table, a, svec, n_cur, n_full, scratch, ticket, s, sig, b, c_out, sigc);
   else throw std::runtime_error("spartan_b200: unsupported MSM window width");
-  SP_LAUNCHED(); check("ipa_msm");
+  SP_LAUNCHED(); check("ipa_msm_quad");
 }
 
 static int msm_pick_groups(size_t L, size_t R) {

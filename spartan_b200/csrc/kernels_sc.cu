@@ -1,6 +1,4 @@
 // spartan_b200 — sumcheck-round kernels (K1/K2 of SURVEY.md §2b), their own translation unit so the two .cu files build in parallel.
-#include <cstdlib>
-#include <algorithm>
 #include "kcommon.cuh"
 
 #ifndef SP_SC_LB
@@ -63,10 +61,10 @@ __global__ void __launch_bounds__(256, SP_SC_LB) k_sc_eval(ScBatch batch, size_t
 
 // Fused: bind the top variable with r (len -> len/2) and evaluate the next round's polynomial on the folded table.
 // Thread i owns elements {i, i+len/4, i+len/2, i+3len/4} of every table: in-place update is race-free.
-// CF: bind with the constant-multiplier fold (fq_fold_const: table of r*2^(32j) mod q in uniform registers, 72 wide products and no separate
-// modular addition) instead of sub + Montgomery product + add; same canonical values either way.
-template <int KIND, bool CF>
-__global__ void __launch_bounds__(256, SP_SC_LB) k_sc_fold_eval(ScBatch batch, size_t len, const u256 r, const __grid_constant__ FqConst rc, u256* partials,
+// The bind is the constant-multiplier fold (fq_fold_const: table of r*2^(32j) mod q in uniform registers, 72 wide products and no separate
+// modular addition) instead of sub + Montgomery product + add; same canonical values.
+template <int KIND>
+__global__ void __launch_bounds__(256, SP_SC_LB) k_sc_fold_eval(ScBatch batch, size_t len, const __grid_constant__ FqConst rc, u256* partials,
                                                        unsigned int* counters, u256* out, HostSig sig, const __grid_constant__ XRank xr) {
   constexpr int NT = KIND == SC_QUAD ? 2 : (KIND == SC_CUBIC3 ? 3 : 4);
   const ScInst& in = batch.inst[blockIdx.y];
@@ -80,11 +78,8 @@ __global__ void __launch_bounds__(256, SP_SC_LB) k_sc_fold_eval(ScBatch batch, s
     for (int t = 0; t < NT; t++) {
       u256 a0 = ld256(in.t[t] + i), a1 = ld256(in.t[t] + i + half);
       u256 b0 = ld256(in.t[t] + i + quarter), b1 = ld256(in.t[t] + i + quarter + half);
-      if (CF) { lo[t] = fq_fold_const(a0, a1, rc); hi[t] = fq_fold_const(b0, b1, rc); }
-      else {
-        lo[t] = fq_add(a0, fq_mul(r, fq_sub(a1, a0)));   // dense_mlpoly.rs:218
-        hi[t] = fq_add(b0, fq_mul(r, fq_sub(b1, b0)));
-      }
+      lo[t] = fq_fold_const(a0, a1, rc);   // dense_mlpoly.rs:218
+      hi[t] = fq_fold_const(b0, b1, rc);
       if (t == 2) {
         if (in.write_c) { st256(in.c_out + i, lo[t]); st256(in.c_out + i + quarter, hi[t]); }
       } else {
@@ -155,186 +150,13 @@ __global__ void __launch_bounds__(256) k_eq_suffix(u256* levels, const u256* __r
   }
 }
 
-// ---- register-lean formulation of the fused round (3 CTAs of 256 threads per SM instead of 2).
-// The tables of an index are visited one after the other: bind (lo, hi), store, form the three evaluation arguments lo, 2hi-lo, 3hi-2lo and
-// fold them straight into three running products, so that only ONE table's values are live at a time; the three per-thread sums live in
-// shared memory ([point][limb][thread]: conflict-free) because they are touched once per index.  Same values as k_sc_fold_eval, same layout.
-// Order of the factors: A*B, A*B*C as stored; A*(B*C-D) as B, C, D, A.
-#ifndef SC_V2_THREADS
-#define SC_V2_THREADS 128   // 5 CTAs x 4 warps per SM at <= 96 registers (6 CTAs: 80 registers)
-#endif
-#ifndef SC_V2_BLOCKS
-#define SC_V2_BLOCKS 5
-#endif
-template <int KIND>
-__global__ void __launch_bounds__(SC_V2_THREADS, SC_V2_BLOCKS) k_sc_fold_eval_v2(ScBatch batch, size_t len, const __grid_constant__ FqConst rc, u256* partials,
-                                                            unsigned int* counters, u256* out, HostSig sig, const __grid_constant__ XRank xr) {
-  constexpr int NT = KIND == SC_QUAD ? 2 : (KIND == SC_CUBIC3 ? 3 : 4);
-  constexpr int NP = KIND == SC_QUAD ? 2 : 3;
-  __shared__ uint32_t accs[3][8][SC_V2_THREADS];
-  const ScInst& in = batch.inst[blockIdx.y];
-  const size_t half = len >> 1, quarter = len >> 2;
-  const int tid = threadIdx.x;
-#pragma unroll
-  for (int k = 0; k < 3; k++)
-#pragma unroll
-    for (int l = 0; l < 8; l++) accs[k][l][tid] = 0;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + tid; i < quarter; i += (size_t)gridDim.x * blockDim.x) {
-    u256 P0, P2, P3;
-#pragma unroll
-    for (int step = 0; step < NT; step++) {
-      const int t = KIND == SC_CUBIC4 ? (step + 1) & 3 : step;     // B, C, D, A for A*(B*C-D)
-      u256* T = in.t[t];
-      u256 lo, hi;
-      {
-        u256 a0 = ld256(T + i), a1 = ld256(T + i + half), b0 = ld256(T + i + quarter), b1 = ld256(T + i + quarter + half);
-        lo = fq_fold_const(a0, a1, rc);   // dense_mlpoly.rs:218
-        hi = fq_fold_const(b0, b1, rc);
-      }
-      if (t == 2) { if (in.write_c) { st256(in.c_out + i, lo); st256(in.c_out + i + quarter, hi); } }
-      else { st256(T + i, lo); st256(T + i + quarter, hi); }
-      const u256 dl = fq_sub(hi, lo);
-      const u256 x2 = fq_add(hi, dl);                              // 2*hi - lo      (sumcheck.rs:466-468 / :630-639)
-      if (step == 0) {
-        P0 = lo; P2 = x2;
-        if (NP == 3) P3 = fq_add(x2, dl);                          // 3*hi - 2*lo    (sumcheck.rs:642-651)
-      } else if (KIND == SC_CUBIC4 && step == 2) {                 // ... - D
-        P0 = fq_sub(P0, lo); P2 = fq_sub(P2, x2); P3 = fq_sub(P3, fq_add(x2, dl));
-      } else {
-        P0 = fq_mul(P0, lo); P2 = fq_mul(P2, x2);
-        if (NP == 3) P3 = fq_mul(P3, fq_add(x2, dl));
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < NP; k++) {
-      u256 a;
-#pragma unroll
-      for (int l = 0; l < 8; l++) a.v[l] = accs[k][l][tid];
-      a = fq_add(a, k == 0 ? P0 : (k == 1 ? P2 : P3));
-#pragma unroll
-      for (int l = 0; l < 8; l++) accs[k][l][tid] = a.v[l];
-    }
-  }
-  u256 acc[3];
-#pragma unroll
-  for (int k = 0; k < 3; k++)
-#pragma unroll
-    for (int l = 0; l < 8; l++) acc[k].v[l] = accs[k][l][tid];
-  block_reduce_finish<3>(acc, partials, counters, out, 3, sig, xr);
-}
-
-// ---- TMA-staged formulation of the fused round (north_star: "TMA-staged into shared memory"; A/B against the register-resident ones:
-// DESIGN.md's switch table).  A CTA walks tiles of SC_TMA_TI indices; one elected thread issues the 4*NT bulk copies of the NEXT tile
-// (cp.async.bulk global -> shared, completion counted in bytes on an mbarrier) while all 256 threads work on the current one in two phases:
-//   A (bind)     : 2*NT*TI independent tasks (table, half, index): read the pair from shared memory, constant-multiplier fold, write the bound value
-//                  back to shared memory and out to HBM — no thread ever holds more than one pair, loads occupy no registers and no issue slots;
-//   B (evaluate) : NP*TI tasks (point, index): form the point's argument per table from (lo, hi) in shared memory, running product, one
-//                  accumulator per thread (a thread always serves the same evaluation point).
-// Two stages of shared memory (32 KiB each for four tables), <= 80 registers: 3 CTAs per SM.
-#ifndef SC_TMA_TI
-#define SC_TMA_TI 64
-#endif
-#ifndef SC_TMA_BLOCKS
-#define SC_TMA_BLOCKS 3
-#endif
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile("{\n\t.reg .pred p;\n\tSP_MBAR_WAIT:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra SP_MBAR_DONE;\n\tbra SP_MBAR_WAIT;\n\tSP_MBAR_DONE:\n\t}" ::"r"(
-                   smem_u32(bar)),
-               "r"(parity)
-               : "memory");
-}
-template <int KIND>
-__global__ void __launch_bounds__(256, SC_TMA_BLOCKS) k_sc_fold_eval_tma(ScBatch batch, size_t len, const __grid_constant__ FqConst rc, u256* partials, unsigned int* counters,
-                                                             u256* out, HostSig sig, const __grid_constant__ XRank xr) {
-  constexpr int NT = KIND == SC_QUAD ? 2 : (KIND == SC_CUBIC3 ? 3 : 4);
-  constexpr int NP = KIND == SC_QUAD ? 2 : 3;
-  constexpr int TI = SC_TMA_TI;
-  constexpr uint32_t SEG_BYTES = TI * 32, STAGE_BYTES = NT * 4 * SEG_BYTES;
-  extern __shared__ __align__(128) uint8_t smem_raw[];
-  u256* buf = reinterpret_cast<u256*>(smem_raw);                                    // [stage][table][segment][TI]
-  uint64_t* mbar = reinterpret_cast<uint64_t*>(smem_raw + 2 * STAGE_BYTES);         // [2]
-  const ScInst& in = batch.inst[blockIdx.y];
-  const size_t half = len >> 1, quarter = len >> 2;
-  const size_t ntiles = quarter / TI;
-  const int tid = threadIdx.x;
-  auto slot = [&](int stage, int t, int seg) { return buf + ((size_t)(stage * NT + t) * 4 + seg) * TI; };
-  auto issue = [&](int stage, size_t tile) {   // one thread: arm the barrier with the byte count, then the 4*NT bulk copies
-    mbar_expect_tx(&mbar[stage], STAGE_BYTES);
-#pragma unroll
-    for (int t = 0; t < NT; t++) {
-      const u256* T = in.t[t] + tile * TI;
-      bulk_g2s(slot(stage, t, 0), T, SEG_BYTES, &mbar[stage]);
-      bulk_g2s(slot(stage, t, 1), T + half, SEG_BYTES, &mbar[stage]);
-      bulk_g2s(slot(stage, t, 2), T + quarter, SEG_BYTES, &mbar[stage]);
-      bulk_g2s(slot(stage, t, 3), T + quarter + half, SEG_BYTES, &mbar[stage]);
-    }
-  };
-  if (tid == 0) {
-    mbar_init(&mbar[0], 1); mbar_init(&mbar[1], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (tid == 0 && blockIdx.x < ntiles) issue(0, blockIdx.x);
-  u256 acc = fq_zero();
-  int k = 0;
-  for (size_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, k++) {
-    const int s = k & 1;
-    if (tid == 0 && tile + gridDim.x < ntiles) issue(s ^ 1, tile + gridDim.x);   // stage s^1 was released by the barrier that ended iteration k-1
-    mbar_wait(&mbar[s], (k >> 1) & 1);
-    // ---- phase A: bind
-#pragma unroll 1
-    for (int task = tid; task < NT * 2 * TI; task += 256) {
-      const int t = task / (2 * TI), h = (task / TI) & 1, e = task % TI;
-      u256* pa = slot(s, t, 2 * h) + e;
-      const u256 v = fq_fold_const(ld256(pa), ld256(slot(s, t, 2 * h + 1) + e), rc);   // dense_mlpoly.rs:218
-      st256(pa, v);
-      const size_t g = tile * TI + e + (h ? quarter : 0);
-      if (t == 2) { if (in.write_c) st256(in.c_out + g, v); }
-      else st256(in.t[t] + g, v);
-    }
-    __syncthreads();
-    // ---- phase B: evaluate at t = 0, 2 (, 3)
-    if (tid < NP * TI) {
-      const int p = tid / TI, e = tid % TI;
-      u256 P = fq_zero();
-#pragma unroll
-      for (int step = 0; step < NT; step++) {
-        const int t = KIND == SC_CUBIC4 ? (step + 1) & 3 : step;     // B, C, D, A for A*(B*C-D)
-        const u256 lo = ld256(slot(s, t, 0) + e), hi = ld256(slot(s, t, 2) + e);
-        u256 x = lo;
-        if (p > 0) { const u256 dl = fq_sub(hi, lo); x = fq_add(hi, dl); if (p == 2) x = fq_add(x, dl); }
-        if (step == 0) P = x;
-        else if (KIND == SC_CUBIC4 && step == 2) P = fq_sub(P, x);
-        else P = fq_mul(P, x);
-      }
-      acc = fq_add(acc, P);
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // this iteration's generic-proxy accesses to stage s before the bulk copy that refills it
-    __syncthreads();
-  }
-  u256 acc3[3];
-  const int p = tid / TI;
-#pragma unroll
-  for (int q = 0; q < 3; q++) acc3[q] = (tid < NP * TI && p == q) ? acc : fq_zero();
-  block_reduce_finish<3>(acc3, partials, counters, out, 3, sig, xr);
-}
-
 // Small tables (len/4 <= SC_SMALL_MAX): the round's latency, not its throughput, is what the prover waits for, so the work of one index is
 // spread over 2*NT threads for the bind step (one multiplication deep) and 3 threads for the evaluations (two deep), exchanging the bound
 // values through shared memory, instead of one thread running all 14 multiplications back to back.  Same arithmetic, same results.
 #define SC_SMALL_Q 64
 #define SC_SMALL_MAX 1024
-template <int KIND, bool CF>
-__global__ void __launch_bounds__(SC_SMALL_Q * 8) k_sc_fold_eval_small(ScBatch batch, size_t len, const u256 r, const __grid_constant__ FqConst rc, u256* partials,
+template <int KIND>
+__global__ void __launch_bounds__(SC_SMALL_Q * 8) k_sc_fold_eval_small(ScBatch batch, size_t len, const __grid_constant__ FqConst rc, u256* partials,
                                                                      unsigned int* counters, u256* out, HostSig sig) {
   constexpr int NT = KIND == SC_QUAD ? 2 : (KIND == SC_CUBIC3 ? 3 : 4);
   constexpr int NP = KIND == SC_QUAD ? 2 : 3;   // evaluation points 0, 2 (, 3)
@@ -348,7 +170,7 @@ __global__ void __launch_bounds__(SC_SMALL_Q * 8) k_sc_fold_eval_small(ScBatch b
     const int t = th >> 1, h = th & 1;
     const size_t idx = i + (h ? quarter : 0);
     u256 x0 = ld256(in.t[t] + idx), x1 = ld256(in.t[t] + idx + half);
-    u256 v = CF ? fq_fold_const(x0, x1, rc) : fq_add(x0, fq_mul(r, fq_sub(x1, x0)));   // dense_mlpoly.rs:218
+    u256 v = fq_fold_const(x0, x1, rc);   // dense_mlpoly.rs:218
     if (t == 2) { if (in.write_c) st256(in.c_out + idx, v); }
     else st256(in.t[t] + idx, v);
     sh[t][h][e] = v;
@@ -416,115 +238,15 @@ __global__ void __launch_bounds__(SC_SMALL_Q * 8) k_sc_fold_eval_small(ScBatch b
   }
 }
 
-// ---- persistent tail (dev.hpp: sc_persist)
-__device__ __forceinline__ u256 ld256_sys(const u256* p) {   // mapped host memory: two 16-byte volatile loads (two PCIe reads), never cached
-  u256 r;
-  asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%8];\n\tld.volatile.global.v4.u32 {%4, %5, %6, %7}, [%8+16];"
-               : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]), "=r"(r.v[7])
-               : "l"(p)
-               : "memory");
-  return r;
-}
-__device__ __forceinline__ unsigned int ld_acquire_gpu(const unsigned int* p) {
-  unsigned int v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__global__ void __launch_bounds__(512) k_sc_persist(ScBatch batch, int n_shared_c, u256* c_scratch, size_t len, const u256 r0, const PersistMail* mail,
-                                                    PersistMail* dmail, unsigned int mail_seq0, u256* out, HostSig sig) {
-  __shared__ u256 ws[16][3];
-  __shared__ u256 s_r;
-  const int inst = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  u256* T[3] = {batch.inst[inst].t[0], batch.inst[inst].t[1], batch.inst[inst].t[2]};
-  if (inst < n_shared_c) {   // private copy of the shared eq table: the instances then never touch common data
-    u256* mine = c_scratch + (size_t)inst * len;
-    for (size_t i = tid; i < len; i += blockDim.x) st256(mine + i, ld256(T[2] + i));
-    T[2] = mine;
-    __syncthreads();
-  }
-  int nfold = 0;
-  while (((size_t)1 << nfold) < len) nfold++;
-  u256 r = r0;
-  size_t L = len;
-  for (int f = 0; f < nfold; f++) {
-    const size_t half = L >> 1, quarter = L >> 2;
-    if (f + 1 < nfold) {
-      // bind: entries idx in [0, half) of every table, idx + half being the partner             (dense_mlpoly.rs:218)
-      for (size_t task = tid; task < 3 * half; task += blockDim.x) {
-        const int t = (int)(task / half);
-        const size_t idx = task - (size_t)t * half;
-        const u256 x0 = ld256(T[t] + idx), x1 = ld256(T[t] + idx + half);
-        st256(T[t] + idx, fq_add(x0, fq_mul(r, fq_sub(x1, x0))));
-      }
-      __syncthreads();
-      // evaluate the next round polynomial on the bound tables (length half): points 0, 2, 3 of A*B*C      (sumcheck.rs:296-355)
-      u256 acc0 = fq_zero(), acc2 = fq_zero(), acc3 = fq_zero();
-      for (size_t task = tid; task < 3 * quarter; task += blockDim.x) {
-        const int p = (int)(task / quarter);
-        const size_t e = task - (size_t)p * quarter;
-        u256 x[3];
-#pragma unroll
-        for (int t = 0; t < 3; t++) {
-          const u256 lo = ld256(T[t] + e), hi = ld256(T[t] + e + quarter);
-          if (p == 0) x[t] = lo;
-          else { const u256 dl = fq_sub(hi, lo); x[t] = fq_add(hi, dl); if (p == 2) x[t] = fq_add(x[t], dl); }
-        }
-        const u256 v = fq_mul(fq_mul(x[0], x[1]), x[2]);
-        if (p == 0) acc0 = fq_add(acc0, v); else if (p == 1) acc2 = fq_add(acc2, v); else acc3 = fq_add(acc3, v);
-      }
-      acc0 = warp_sum_fq(acc0); acc2 = warp_sum_fq(acc2); acc3 = warp_sum_fq(acc3);
-      if (lane == 0) { ws[warp][0] = acc0; ws[warp][1] = acc2; ws[warp][2] = acc3; }
-      __syncthreads();
-      if (warp < 3) {   // warp k finishes value k
-        u256 v = lane < (int)(blockDim.x >> 5) ? ws[lane][warp] : fq_zero();
-        v = warp_sum_fq(v);
-        if (lane == 0) { st256(&out[(size_t)inst * 3 + warp], v); st256(&sig.host_out[(size_t)inst * 3 + warp], v); __threadfence_system(); }
-      }
-    } else {
-      // last bind (L = 2): the heads are the layer's claims (product_tree.rs:330-347)
-      if (tid < 3) {
-        const u256 x0 = ld256(T[tid]), x1 = ld256(T[tid] + 1);
-        const u256 v = fq_add(x0, fq_mul(r, fq_sub(x1, x0)));
-        st256(T[tid], v);
-        st256(&out[(size_t)inst * 3 + tid], v); st256(&sig.host_out[(size_t)inst * 3 + tid], v);
-        __threadfence_system();
-      }
-    }
-    __syncthreads();
-    if (tid == 0) {
-      __threadfence_system();
-      const unsigned int done = atomicAdd(sig.done, 1u) + 1;
-      if (done == gridDim.x) { *sig.done = 0; __threadfence_system(); *((volatile unsigned int*)sig.flag) = sig.seq + (unsigned int)f; }
-      if (f + 1 < nfold) {   // wait for the host's next challenge: CTA 0 polls the host mailbox over PCIe and forwards it through device memory
-        const unsigned int want = mail_seq0 + (unsigned int)f + 1;
-        if (inst == 0) {
-          wait_flag_sys(&mail->seq, want);
-          s_r = ld256_sys(&mail->r);
-          if (gridDim.x > 1) { st256(&dmail->r, s_r); __threadfence(); *((volatile unsigned int*)&dmail->seq) = want; }
-        } else {
-          const unsigned long long t0 = global_timer_ns();
-          unsigned int spins = 0;
-          while ((int)(ld_acquire_gpu(&dmail->seq) - want) < 0)
-            if ((++spins & 0x3ff) == 0 && global_timer_ns() - t0 > 30000000000ull) __trap();
-          s_r = ld256_cg(&dmail->r);
-        }
-      }
-    }
-    __syncthreads();
-    if (f + 1 < nfold) r = s_r;
-    L = half;
-  }
-}
 struct FoldBatch {
   u256* t[64];
 };
-template <bool CF>
-__global__ void __launch_bounds__(256) k_fold_top(FoldBatch tabs, size_t len, const u256 r, const __grid_constant__ FqConst rc) {
+__global__ void __launch_bounds__(256) k_fold_top(FoldBatch tabs, size_t len, const __grid_constant__ FqConst rc) {
   const size_t half = len >> 1;
   u256* T = tabs.t[blockIdx.y];
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < half; i += (size_t)gridDim.x * blockDim.x) {
     u256 a0 = ld256(T + i), a1 = ld256(T + i + half);
-    st256(T + i, CF ? fq_fold_const(a0, a1, rc) : fq_add(a0, fq_mul(r, fq_sub(a1, a0))));   // dense_mlpoly.rs:218
+    st256(T + i, fq_fold_const(a0, a1, rc));   // dense_mlpoly.rs:218
   }
 }
 
@@ -532,29 +254,6 @@ __global__ void __launch_bounds__(256) k_fold_top(FoldBatch tabs, size_t len, co
 static const size_t SC_MAX_BLOCKS = 132 * 6 + 64;   // 6 CTAs on each of an H100's 132 SMs; larger grids are capped to it
 size_t sc_scratch_bytes(int ninst) { return 256 + (size_t)ninst * SC_MAX_BLOCKS * 3 * sizeof(u256); }
 
-// A/B switch for the constant-multiplier fold (tools/bench_kernels.py): SP_SC_CONSTFOLD=0/1 overrides the default
-#ifndef SP_SC_CONSTFOLD_DEFAULT
-#define SP_SC_CONSTFOLD_DEFAULT 1   // 72 wide products instead of a Montgomery product per bind; same canonical values, parity suite green
-#endif
-// which streaming formulation of the fused round: 0 = register-resident (k_sc_fold_eval), 1 = register-lean (k_sc_fold_eval_v2), 2 = TMA-staged
-// (k_sc_fold_eval_tma); SP_SC_VARIANT overrides the default (SP_SC_V2 / SP_SC_TMA are shorthands); 1 and 2 need the constant-multiplier fold
-#ifndef SP_SC_VARIANT_DEFAULT
-#define SP_SC_VARIANT_DEFAULT 0
-#endif
-static bool sc_constfold();
-static int sc_variant() {
-  static const int v = [] {
-    if (const char* e = getenv("SP_SC_VARIANT")) return atoi(e);
-    if (getenv("SP_SC_TMA")) return 2;
-    if (getenv("SP_SC_V2")) return 1;
-    return SP_SC_VARIANT_DEFAULT;
-  }();
-  return sc_constfold() ? v : 0;
-}
-static bool sc_constfold() {
-  static const bool on = [] { const char* e = getenv("SP_SC_CONSTFOLD"); return e ? atoi(e) != 0 : SP_SC_CONSTFOLD_DEFAULT != 0; }();
-  return on;
-}
 // algorithmic bytes of one launch: every DISTINCT table is streamed once (a C table shared by several instances of a batched sumcheck counts
 // once, not once per instance): `per_elem` bytes per entry (32 for an evaluation pass, 48 for the fused bind + evaluate: read 32, write 16 per input entry)
 static double sc_bytes(const ScInst* insts, int ninst, ScKind kind, size_t len, double per_elem) {
@@ -591,70 +290,30 @@ void sc_eval(ScKind kind, const ScInst* insts, int ninst, size_t len, u256* out,
 }
 void sc_fold_eval(ScKind kind, const ScInst* insts, int ninst, size_t len, const u256& r, u256* out, void* scratch, cudaStream_t s, HostSig sig, const XRank& xr) {
   if (xr.world > 1 && (len / 4 <= SC_SMALL_MAX || !sig.done)) throw std::runtime_error("spartan_b200: a sharded sumcheck round needs a streaming-size table and a completion counter");
-  static const bool small_ok = getenv("SP_SC_NO_SMALL") == nullptr;
   // two kernels, two profiler families: the streaming kernel (HBM roofline) and the latency-bound small-table kernel (k_sc_fold_eval_small)
-  const bool small = small_ok && len / 4 <= SC_SMALL_MAX && len >= 4;
+  const bool small = len / 4 <= SC_SMALL_MAX && len >= 4;
   ProfScope ps(small ? "sc_fold_eval_small" : "sc_fold_eval", sc_bytes(insts, ninst, kind, len, 48.0), s);
   ScBatch b; fill_batch(b, insts, ninst);
   unsigned int* counters = (unsigned int*)scratch;
   u256* partials = (u256*)((char*)scratch + 256);
-  static const bool cf = sc_constfold();
-  const FqConst rc = cf ? fq_const_table(r) : FqConst();
-#define SP_SC_LAUNCH(KERNEL, K, THREADS, ...) \
-  do { if (cf) KERNEL<K, true><<<grid, THREADS, 0, s>>>(b, len, r, rc, partials, counters, out, sig, ##__VA_ARGS__); \
-       else KERNEL<K, false><<<grid, THREADS, 0, s>>>(b, len, r, rc, partials, counters, out, sig, ##__VA_ARGS__); } while (0)
+  const FqConst rc = fq_const_table(r);
   if (small) {
     dim3 grid((unsigned)((len / 4 + SC_SMALL_Q - 1) / SC_SMALL_Q), ninst);
     switch (kind) {
-      case SC_QUAD: SP_SC_LAUNCH(k_sc_fold_eval_small, SC_QUAD, SC_SMALL_Q * 4); break;
-      case SC_CUBIC3: SP_SC_LAUNCH(k_sc_fold_eval_small, SC_CUBIC3, SC_SMALL_Q * 6); break;
-      default: SP_SC_LAUNCH(k_sc_fold_eval_small, SC_CUBIC4, SC_SMALL_Q * 8); break;
+      case SC_QUAD: k_sc_fold_eval_small<SC_QUAD><<<grid, SC_SMALL_Q * 4, 0, s>>>(b, len, rc, partials, counters, out, sig); break;
+      case SC_CUBIC3: k_sc_fold_eval_small<SC_CUBIC3><<<grid, SC_SMALL_Q * 6, 0, s>>>(b, len, rc, partials, counters, out, sig); break;
+      default: k_sc_fold_eval_small<SC_CUBIC4><<<grid, SC_SMALL_Q * 8, 0, s>>>(b, len, rc, partials, counters, out, sig); break;
     }
     SP_LAUNCHED(); check("sc_fold_eval_small");
-    return;
-  }
-  const bool tma = sc_variant() == 2;   // TMA-staged two-phase formulation
-  if (tma && len / 4 >= 64 * SC_TMA_TI) {
-    const int nt = kind == SC_QUAD ? 2 : kind == SC_CUBIC3 ? 3 : 4;
-    const size_t smem = (size_t)2 * nt * 4 * SC_TMA_TI * 32 + 64;
-    static bool attr_set = false;
-    if (!attr_set) {
-      cudaFuncSetAttribute(k_sc_fold_eval_tma<SC_QUAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2 * 4 * SC_TMA_TI * 32 + 64);
-      cudaFuncSetAttribute(k_sc_fold_eval_tma<SC_CUBIC3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 3 * 4 * SC_TMA_TI * 32 + 64);
-      cudaFuncSetAttribute(k_sc_fold_eval_tma<SC_CUBIC4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 4 * 4 * SC_TMA_TI * 32 + 64);
-      attr_set = true;
-    }
-    size_t ntiles = len / 4 / SC_TMA_TI;
-    dim3 grid((unsigned)std::min<size_t>(ntiles, (size_t)sm_count() * SC_TMA_BLOCKS), ninst);
-    if (grid.x > SC_MAX_BLOCKS) grid.x = SC_MAX_BLOCKS;
-    switch (kind) {
-      case SC_QUAD: k_sc_fold_eval_tma<SC_QUAD><<<grid, 256, smem, s>>>(b, len, rc, partials, counters, out, sig, xr); break;
-      case SC_CUBIC3: k_sc_fold_eval_tma<SC_CUBIC3><<<grid, 256, smem, s>>>(b, len, rc, partials, counters, out, sig, xr); break;
-      default: k_sc_fold_eval_tma<SC_CUBIC4><<<grid, 256, smem, s>>>(b, len, rc, partials, counters, out, sig, xr); break;
-    }
-    SP_LAUNCHED(); check("sc_fold_eval_tma");
-    return;
-  }
-  const bool v2 = sc_variant() == 1;   // register-lean formulation
-  if (v2) {
-    dim3 grid(grid_for(len / 4, SC_V2_THREADS, SC_V2_BLOCKS), ninst);
-    if (grid.x > SC_MAX_BLOCKS) grid.x = SC_MAX_BLOCKS;
-    switch (kind) {
-      case SC_QUAD: k_sc_fold_eval_v2<SC_QUAD><<<grid, SC_V2_THREADS, 0, s>>>(b, len, rc, partials, counters, out, sig, xr); break;
-      case SC_CUBIC3: k_sc_fold_eval_v2<SC_CUBIC3><<<grid, SC_V2_THREADS, 0, s>>>(b, len, rc, partials, counters, out, sig, xr); break;
-      default: k_sc_fold_eval_v2<SC_CUBIC4><<<grid, SC_V2_THREADS, 0, s>>>(b, len, rc, partials, counters, out, sig, xr); break;
-    }
-    SP_LAUNCHED(); check("sc_fold_eval_v2");
     return;
   }
   dim3 grid(grid_for(len / 4, 256, SP_SC_LB), ninst);
   if (grid.x > SC_MAX_BLOCKS) grid.x = SC_MAX_BLOCKS;
   switch (kind) {
-    case SC_QUAD: SP_SC_LAUNCH(k_sc_fold_eval, SC_QUAD, 256, xr); break;
-    case SC_CUBIC3: SP_SC_LAUNCH(k_sc_fold_eval, SC_CUBIC3, 256, xr); break;
-    default: SP_SC_LAUNCH(k_sc_fold_eval, SC_CUBIC4, 256, xr); break;
+    case SC_QUAD: k_sc_fold_eval<SC_QUAD><<<grid, 256, 0, s>>>(b, len, rc, partials, counters, out, sig, xr); break;
+    case SC_CUBIC3: k_sc_fold_eval<SC_CUBIC3><<<grid, 256, 0, s>>>(b, len, rc, partials, counters, out, sig, xr); break;
+    default: k_sc_fold_eval<SC_CUBIC4><<<grid, 256, 0, s>>>(b, len, rc, partials, counters, out, sig, xr); break;
   }
-#undef SP_SC_LAUNCH
   SP_LAUNCHED(); check("sc_fold_eval");
 }
 void sc_eval_g(const ScInst* insts, int ninst, size_t len, const u256* E, u256* out, void* scratch, cudaStream_t s, HostSig sig, const XRank& xr) {
@@ -689,30 +348,17 @@ void eq_suffix(u256* levels, const u256* E0, size_t n0, int K, cudaStream_t s) {
 }
 void fold_top(u256* const* tables, int ntables, size_t len, const u256& r, cudaStream_t s) {
   ProfScope ps("fold_top", (double)ntables * len * 48.0, s);
-  const bool cf = sc_constfold();
-  const FqConst rc = cf ? fq_const_table(r) : FqConst();
+  const FqConst rc = fq_const_table(r);
   for (int base = 0; base < ntables; base += 64) {
     FoldBatch fb; int n = ntables - base < 64 ? ntables - base : 64;
     for (int i = 0; i < n; i++) fb.t[i] = tables[base + i];
     dim3 grid(grid_for(len / 2, 256, 4), n);
-    if (cf) k_fold_top<true><<<grid, 256, 0, s>>>(fb, len, r, rc);
-    else k_fold_top<false><<<grid, 256, 0, s>>>(fb, len, r, rc);
+    k_fold_top<<<grid, 256, 0, s>>>(fb, len, rc);
     SP_LAUNCHED();
   }
   check("fold_top");
 }
 void fold_top_single(u256* table, size_t len, const u256& r, cudaStream_t s) { u256* t[1] = {table}; fold_top(t, 1, len, r, s); }
-
-
-void sc_persist(const ScInst* insts, int ninst, int n_shared_c, u256* c_scratch, size_t len, const u256& r0, const PersistMail* mail, PersistMail* dmail,
-                unsigned int mail_seq0, u256* out, cudaStream_t s, HostSig sig) {
-  ProfScope ps("sc_persist", sc_bytes(insts, ninst, SC_CUBIC3, len, 96.0), s);
-  if (len < 4 || len > SC_PERSIST_MAX_LEN || (len & (len - 1)) || !sig.flag || !sig.done || !sig.host_out) throw std::runtime_error("spartan_b200: sc_persist: bad arguments");
-  ScBatch b; fill_batch(b, insts, ninst);
-  k_sc_persist<<<ninst, 512, 0, s>>>(b, n_shared_c, c_scratch, len, r0, mail, dmail, mail_seq0, out, sig);
-  SP_LAUNCHED(); check("sc_persist");
-}
-
 
 }  // namespace dev
 }  // namespace sp

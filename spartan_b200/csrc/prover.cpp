@@ -29,20 +29,11 @@ void shake256(uint8_t* out, size_t outlen, const uint8_t* in, size_t inlen) {
   }
 }
 
-#ifndef SP_BG_SMS_DEFAULT
-#define SP_BG_SMS_DEFAULT 0
-#endif
 Ctx::Ctx(int dev_) : device(dev_) {
   if (dev::device_count() <= dev_) throw std::runtime_error("spartan_b200: no CUDA device " + std::to_string(dev_) + " (the prover has no CPU fallback)");
   dev::set_device(dev_);
   stream = dev::stream_create_prio(+1);
-  {
-    // SP_BG_SMS: SMs of the background partition (0: no partition, the background stream shares all SMs at the least priority)
-    const char* e = getenv("SP_BG_SMS");
-    const int want = e ? atoi(e) : SP_BG_SMS_DEFAULT;
-    if (want > 0) stream2 = dev::stream_create_partition(want, -1, &stream2_sms);
-    if (!stream2) { stream2_sms = 0; stream2 = dev::stream_create_prio(-1); }
-  }
+  stream2 = dev::stream_create_prio(-1);
   ev_fork = dev::event_create(); ev_join = dev::event_create();
   pinned_bytes = 1 << 20;
   pinned = (uint8_t*)dev::hmalloc_pinned(pinned_bytes);
@@ -50,10 +41,6 @@ Ctx::Ctx(int dev_) : device(dev_) {
   host_flag = reinterpret_cast<unsigned int*>(pinned + (768 << 10));
   *host_flag = 0;
   host_flag[16] = 0;   // second flag word (its own cache line): the dot products fused into the inner-product MSM launch
-  mail = reinterpret_cast<dev::PersistMail*>(pinned + (900 << 10));
-  memset(mail, 0, sizeof(dev::PersistMail));
-  dmail.alloc(1);
-  dev::dzero(dmail.p, sizeof(dev::PersistMail), stream);
   sig_done.alloc(4);
   dev::dzero(sig_done.p, 16, stream);
   small.alloc(4096);
@@ -73,7 +60,7 @@ void Ctx::comm_create() {
 Ctx::~Ctx() {
   try { sync(); } catch (...) {}
   try { dev::stream_sync(stream2); } catch (...) {}
-  scratch.release(); scratch2.release(); red.release(); small.release(); dmail.release();
+  scratch.release(); scratch2.release(); red.release(); small.release();
   dev::event_destroy(ev_fork); dev::event_destroy(ev_join);
   dev::stream_destroy(stream2);
   if (ev_a) { dev::event_destroy(ev_a); dev::event_destroy(ev_b); }
@@ -208,87 +195,7 @@ hge GenSet::host_point(size_t base) const {
   hge acc = hge_identity();
   return hge_madd(acc, tab(base).e[0], false);
 }
-// ---- HostPool
-HostPool& HostPool::get() { static HostPool p; return p; }
-HostPool::HostPool() {
-  int n = 0;   // off by default: the helpers spin on host cores that the ZK rounds' single-threaded host work also needs
-  if (const char* e = getenv("SP_HOST_THREADS")) n = atoi(e);
-  if (std::thread::hardware_concurrency() < 8) n = 0;
-  if (n < 0) n = 0;
-  if (n > 7) n = 7;
-  for (int i = 0; i < n; i++) th_.emplace_back([this] { worker(); });
-}
-HostPool::~HostPool() {
-  stop_.store(true);
-  { std::lock_guard<std::mutex> lk(mu_); cv_.notify_all(); }
-  for (auto& t : th_) t.join();
-}
-void HostPool::worker() {
-  uint64_t seen = 0;
-  auto last_work = std::chrono::steady_clock::now();
-  unsigned spins = 0;
-  while (!stop_.load(std::memory_order_relaxed)) {
-    const uint64_t e = epoch_.load(std::memory_order_acquire);
-    if (e != seen) {
-      seen = e;
-      for (;;) {
-        const uint64_t v = next_.fetch_add(1, std::memory_order_acq_rel);
-        const uint64_t d = desc_.load(std::memory_order_acquire);
-        if ((v >> 32) != (d >> 32) || (uint32_t)v >= (uint32_t)d) break;
-        (*fn_.load(std::memory_order_acquire))((int)(uint32_t)v);
-        pending_.fetch_sub(1, std::memory_order_acq_rel);
-      }
-      last_work = std::chrono::steady_clock::now();
-      spins = 0;
-      continue;
-    }
-#if defined(__x86_64__)
-    __builtin_ia32_pause();
-#endif
-    if ((++spins & 0x3ff) == 0 && std::chrono::steady_clock::now() - last_work > std::chrono::microseconds(200)) {
-      std::unique_lock<std::mutex> lk(mu_);
-      sleepers_.fetch_add(1);
-      cv_.wait_for(lk, std::chrono::milliseconds(50), [&] { return stop_.load() || epoch_.load(std::memory_order_acquire) != seen; });
-      sleepers_.fetch_sub(1);
-      last_work = std::chrono::steady_clock::now();
-    }
-  }
-}
-void HostPool::run(int njobs, const std::function<void(int)>& fn) {
-  if (njobs <= 1 || th_.empty()) { for (int i = 0; i < njobs; i++) fn(i); return; }
-  const uint64_t tag = ++tag_ & 0xffffffu;
-  fn_.store(&fn, std::memory_order_relaxed);
-  pending_.store(njobs - 1, std::memory_order_relaxed);
-  desc_.store(tag << 32 | (uint32_t)njobs, std::memory_order_release);
-  next_.store(tag << 32 | 1u, std::memory_order_release);
-  epoch_.fetch_add(1, std::memory_order_release);
-  if (sleepers_.load(std::memory_order_acquire) > 0) { std::lock_guard<std::mutex> lk(mu_); cv_.notify_all(); }
-  fn(0);
-  for (;;) {   // the caller takes whatever the helpers have not started
-    const uint64_t v = next_.fetch_add(1, std::memory_order_acq_rel);
-    if ((uint32_t)v >= (uint32_t)njobs) break;
-    fn((int)(uint32_t)v);
-    pending_.fetch_sub(1, std::memory_order_acq_rel);
-  }
-  while (pending_.load(std::memory_order_acquire) > 0) {
-#if defined(__x86_64__)
-    __builtin_ia32_pause();
-#endif
-  }
-}
-
 hge host_commit(const GenSet& gs, const Term* terms, size_t nterms) {
-  if (nterms >= 3 && HostPool::get().helpers() > 0) {   // one fixed-base scalar multiplication per job, partial points added here
-    hge part[8];
-    const int n = (int)std::min<size_t>(nterms, 8);
-    const HostBaseTable* tb[8];
-    for (int i = 0; i < n; i++) tb[i] = &gs.tab(terms[i].base);   // look-ups (and their exceptions) stay on this thread
-    HostPool::get().run(n, [&](int i) { part[i] = hge_identity(); host_fixed_mul_acc(part[i], *tb[i], terms[i].k); });
-    hge acc = part[0];
-    for (int i = 1; i < n; i++) acc = hge_add(acc, part[i]);
-    for (size_t i = (size_t)n; i < nterms; i++) host_fixed_mul_acc(acc, gs.tab(terms[i].base), terms[i].k);
-    return acc;
-  }
   hge acc = hge_identity();
   for (size_t i = 0; i < nterms; i++) host_fixed_mul_acc(acc, gs.tab(terms[i].base), terms[i].k);
   return acc;
@@ -662,26 +569,13 @@ static void bullet_prove(Ctx& ctx, Transcript& T, const PolyCommitmentGens& gens
   while (cur != 1) {
     size_t half = cur / 2;
     FineTimer f1(ctx, "ipa launch");
-    const u256* da[2] = {d_a, d_a + half};
-    const u256* db[2] = {d_b + half, d_b};
     // c_L = <a_L, b_R>, c_R = <a_R, b_L> (bullet.rs:78-79) and L = <a_L, G_R>, R = <a_R, G_L> over the unfolded generators (scalars a[.]*s[j] formed
-    // inside the kernel), all published to the host.  With the quad-lane kernel the dot products ride in the MSM's launch (two extra blocks with
-    // their own flag word); otherwise a dot_pairs launch precedes the MSM.
+    // inside the kernel), all published to the host.  The dot products ride in the MSM's launch (two extra blocks with their own flag word).
     dev::HostSig sig, sig2;
-    // while a background MSM owns most SMs (partitioned stream2), two blocks per free SM is all that can start at once: cap the grid, the kernel strides
-    const int ipa_cap = ctx.bg_busy && ctx.stream2_sms > 0 ? 2 * std::max(4, dev::sm_count() - ctx.stream2_sms) : 0;
-    if (dev::ipa_msm_fuses_dots()) {
-      sig.host_out = ctx.host_res; sig.flag = ctx.host_flag + 16; sig.done = ctx.sig_done.p + 2; sig.seq = ++ctx.sigc_seq;
-      sig2 = ctx.next_sig();
-      sig2.host_out = ctx.host_res + 8;
-      dev::ipa_msm(pts.p, gs.table.p, gs.wbits, d_a, svec.p, cur, n, ctx.scratch.p, ctx.sig_done.p + 1, ctx.stream, sig2, ipa_cap, d_b, d_c, sig);
-    } else {
-      sig = ctx.next_sig();
-      dev::dot_pairs(d_c, da, db, 2, half, ctx.red.p, ctx.stream, sig);
-      sig2 = ctx.next_sig();
-      sig2.host_out = ctx.host_res + 8;
-      dev::ipa_msm(pts.p, gs.table.p, gs.wbits, d_a, svec.p, cur, n, ctx.scratch.p, ctx.sig_done.p + 1, ctx.stream, sig2, ipa_cap);
-    }
+    sig.host_out = ctx.host_res; sig.flag = ctx.host_flag + 16; sig.done = ctx.sig_done.p + 2; sig.seq = ++ctx.sigc_seq;
+    sig2 = ctx.next_sig();
+    sig2.host_out = ctx.host_res + 8;
+    dev::ipa_msm(pts.p, gs.table.p, gs.wbits, d_a, svec.p, cur, n, ctx.scratch.p, ctx.sig_done.p + 1, ctx.stream, sig2, d_b, d_c, sig);
     f1.stop();
     // the transcript work that precedes the first round (absorbing a_vec, deriving r) runs while the device computes round 0
     if (k == 0) r_scale = get_r_scale();

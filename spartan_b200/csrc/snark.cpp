@@ -179,18 +179,7 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
   DevBuf<u256> cpar_a(std::max<size_t>(max_half / 2, 1)), cpar_b(std::max<size_t>(max_half / 2, 1)), d_rand(64), eq_small(2 * ((size_t)1 << ((num_layers + 1) / 2)) + 8);
   DevBuf<u256> cpar0(std::max<size_t>(max_half, 1));
   std::vector<Fq> rand;
-  // persistent tail (dev::sc_persist): once a layer's tables are small, one launch runs all its remaining rounds; A/B switch
-#ifndef SP_SC_PERSIST_DEFAULT
-#define SP_SC_PERSIST_DEFAULT 0
-#endif
-#ifndef SP_SC_EQFACTOR_DEFAULT
-#define SP_SC_EQFACTOR_DEFAULT 1   // 4 instead of 6 field products per index in the streaming rounds, parity suite green
-#endif
-  static const bool eqfactor_on = [] { const char* e = getenv("SP_SC_EQFACTOR"); return e ? atoi(e) != 0 : SP_SC_EQFACTOR_DEFAULT != 0; }();
   const size_t G_MIN = 2 * Ctx::SHARD_MIN_LOCAL;   // 16384 entries per table: the fused G kernel then always streams >= 32768
-  static const bool persist_on = [] { const char* e = getenv("SP_SC_PERSIST"); return e ? atoi(e) != 0 : SP_SC_PERSIST_DEFAULT != 0; }();
-  DevBuf<u256> persist_c;
-  if (persist_on) persist_c.alloc(np * (size_t)SC_PERSIST_MAX_LEN);
   u256* d_out = ctx.small.p + 64;   // ninst * 3 scalars
   DevBuf<u256> d_heads(64);
   for (size_t layer_id = num_layers; layer_id-- > 0;) {
@@ -206,9 +195,9 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
     const Fq c_rank = sh ? shard_eq_scale(rand, W, rk) : Fq::one();   // factor of eq(rand, .) that this rank's low index bits fix (cyclic shards)
     // eq-factored streaming rounds (kernels_sc.cu: k_sc_eval_g): rounds 0 .. jG-1, i.e. those whose evaluation streams >= G_MIN entries per table;
     // the suffix tables E_j = eq(rand[j+1..], .) live in cpar0 (E_0, then the levels 1 .. jG-1); from round jG on the standard kernels run on
-    // C = prefix * eq(rand[jG..], .), built at the switch.  Off / not applicable: the standard method from round 0.
+    // C = prefix * eq(rand[jG..], .), built at the switch.  Not applicable: the standard method from round 0.
     size_t jG = 0;
-    if (eqfactor_on && num_rounds >= 2) {
+    if (num_rounds >= 2) {
       while (jG + 1 < num_rounds && (lhalf >> jG) >= G_MIN) jG++;
       for (size_t j = 0; j < jG; j++) if (rand[j].is_zero()) jG = 0;   // q(1) is recovered by a division by tau_j
     }
@@ -329,9 +318,6 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
     u256* cin = cpar0.p;
     u256* cpp[2] = {cpar_a.p, cpar_b.p};
     int flip = 0;
-    bool persist = false;
-    unsigned int persist_seq0 = 0;
-    size_t persist_j0 = 0;
     for (size_t j = jG; j < num_rounds; j++) {
       std::vector<Fq> ev(3 * ninst);
       FineTimer fw(ctx, "batched wait evals");
@@ -345,28 +331,8 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
       poly.append_to_transcript("poly", T);
       Fq r_j = T.challenge_scalar("challenge_nextround");
       rand_prod.push_back(r_j);
-      if (persist) {   // the persistent kernel binds (and evaluates the next round) as soon as it sees the challenge
-        ctx.post_challenge(r_j);
-        sig.seq = persist_seq0 + (unsigned int)(j - persist_j0);
-        cur >>= 1;
-        e = poly.evaluate(r_j);
-        lp.proof.compressed_polys.push_back(poly.compress());
-        continue;
-      }
       // bind every table (shared C written once, through a ping-pong buffer)
       for (size_t i = 0; i < np; i++) { insts[i].t[2] = cin; insts[i].c_out = cpp[flip]; }
-      if (persist_on && !sh && j + 1 < num_rounds && cur >= 4 && cur <= SC_PERSIST_MAX_LEN) {
-        // small tables from here on: one launch for all the remaining rounds of this layer, its first bind with r_j
-        const unsigned int nfold = (unsigned int)log2_ceil(cur);
-        sig = ctx.next_sig();
-        ctx.sig_seq += nfold - 1;        // one sequence number per publication: nfold-1 round evaluations, then the bound heads
-        dev::sc_persist(insts.data(), (int)ninst, (int)np, persist_c.p, cur, r_j.m, ctx.mail, ctx.dmail.p, ctx.mail_seq, d_out, ctx.stream, sig);
-        persist = true; persist_seq0 = sig.seq; persist_j0 = j;
-        cur >>= 1;
-        e = poly.evaluate(r_j);
-        lp.proof.compressed_polys.push_back(poly.compress());
-        continue;
-      }
       if (j + 1 < num_rounds && sh && cur < Ctx::SHARD_MIN_LOCAL) {
         // leave the sharded stage: bind locally, all-gather every table into replicated copies (in the window), evaluate the next round there
         std::vector<u256*> tabs;
@@ -406,8 +372,7 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
     }
     // final claims: first element of every A / B (and C for the dot-product circuits)
     FineTimer fl(ctx, "batched layer tail (claims d2h + transcript)");
-    if (persist) ctx.wait_sig(sig);   // the heads arrive with the persistent kernel's last publication, in the layout of the gather below
-    else {  // one gather kernel that also publishes the values to the host (instead of 2-3 tiny copies per instance and a stream synchronise)
+    {  // one gather kernel that also publishes the values to the host (instead of 2-3 tiny copies per instance and a stream synchronise)
       std::vector<const u256*> hp(3 * ninst);
       for (size_t i = 0; i < ninst; i++) { hp[3 * i] = insts[i].t[0]; hp[3 * i + 1] = insts[i].t[1]; hp[3 * i + 2] = i >= np ? insts[i].t[2] : insts[i].t[0]; }
       dev::HostSig hs = ctx.next_sig();
@@ -459,7 +424,6 @@ static std::vector<Fq> bound_bot_all(std::vector<Fq> v, const std::vector<Fq>& c
 void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const u256* d_vars, const std::vector<Fq>& input, const SnarkGens& gens,
                  Transcript& T, const Fq& tape_seed, Writer& w) {
   ctx.timings.clear();
-  ctx.timings.push_back({"info:background_stream_sms", (double)ctx.stream2_sms});
   ShardScope shard(ctx);   // on a connected multi-GPU context every rank runs this same function on the same inputs (see DESIGN.md "Multi-GPU")
   auto t_start = std::chrono::steady_clock::now();
   auto mark = [&](const char* name, std::chrono::steady_clock::time_point t0) {
@@ -501,15 +465,15 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
   DevBuf<uint8_t> early_comp;
   struct ForkGuard {   // an exception between fork and join must not release buffers the background stream still works on
     Ctx& c; bool forked = false;
-    ~ForkGuard() { c.bg_busy = false; if (forked) { try { dev::stream_sync(c.stream2); } catch (...) {} } }
+    ~ForkGuard() { if (forked) { try { dev::stream_sync(c.stream2); } catch (...) {} } }
   } fork_guard{ctx};
   dev::MsmTune early_tune;
   {
-    // Shared SMs (the default; DESIGN.md's switch table has the H100 A/B): three resident MSM CTAs per SM instead of four leave a quarter of every
-    // register file to the prover's stream.  Partitioned (ctx.stream2_sms > 0): the background stream owns its SMs, full occupancy there.
+    // three resident MSM CTAs per SM instead of four leave a quarter of every register file to the prover's stream (DESIGN.md's switch table
+    // has the H100 A/B)
     static const char* e_cpt = getenv("SP_EARLY_MSM_CPT");
     static const char* e_smem = getenv("SP_EARLY_MSM_SMEM");
-    early_tune.smem_pad = ctx.stream2_sms > 0 ? 0 : (60 << 10);
+    early_tune.smem_pad = 60 << 10;
     if (e_cpt) early_tune.cpt = atoi(e_cpt);
     if (e_smem) early_tune.smem_pad = (size_t)atol(e_smem);
   }
@@ -526,7 +490,6 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
     dev::event_record(ctx.ev_fork, ctx.stream);
     dev::stream_wait_event(ctx.stream2, ctx.ev_fork);
     fork_guard.forked = true;
-    ctx.bg_busy = true;
     cudaStream_t s2 = ctx.stream2;
     u256* chal = d_chal2.p + 32 * part;
     u256* mem = part ? mem_ry.p : mem_rx.p;
@@ -582,7 +545,6 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
       else dev::d2h(hb.data(), early_comp.p, hb.size(), ctx.stream);
       ctx.sync();
       fork_guard.forked = false;
-      ctx.bg_busy = false;
       ep.comm_derefs.C.assign(L_d, Cp{});                                  // value-initialised: 32 zero bytes = the identity's encoding
       for (size_t r = 0; r < (shard_rows ? Wd : 1); r++)
         for (int part = 0; part < 2; part++)

@@ -85,7 +85,7 @@ def first_diff(a, b):
 def test_snark_bench_configuration_bytes_match_oracle(sb, logn):
     """BASELINE.json configs[1] — exactly what bench.py times (2^20 constraints / variables / non-zeros, 10 inputs, instance seed 0, tape
     seed 0, transcript label b"example") — and the 2^16 sample: computation commitment and proof bytes identical to the oracle's, which runs
-    on all host cores.  This puts k_msm_rows<13,1,4>, k_ipa_msm<13,8> (4098-generator sets) and the streaming sumcheck kernels under a byte
+    on all host cores.  This puts k_msm_rows<13,1,4>, k_ipa_msm_quad<13,5> (4098-generator sets) and the streaming sumcheck kernels under a byte
     diff inside a whole proof.  Also the reference's published structure at 2^20: 47,024 / 64,712 / 133,720 bytes (README.md:362,371,374)."""
     n = 1 << logn
     oc.lib.oracle_set_threads(max(1, (os.cpu_count() or 2) // 2))
@@ -192,13 +192,13 @@ def test_snark_caller_owned_transcript(sb):
 
 
 def test_scheduling_switches_do_not_change_bytes():
-    """The background-stream commitment of the dereferenced values (snark.cpp) and the quad-lane inner-product MSM (kernels.cu) only change WHEN and
-    HOW things are computed: the proof bytes with either switched off must equal the default build's (each variant is its own process: the
-    switches are read once per process)."""
+    """The background-stream commitment of the dereferenced values (snark.cpp) and its launch shape (column passes per CTA, shared-memory pad) only
+    change WHEN and HOW things are computed: the proof bytes with the commitment on the prover's stream, or with another launch shape, must equal
+    the default's (each variant is its own process: the switches are read once per process)."""
     import json, subprocess, sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     shas = {}
-    for name, env in [("default", {}), ("no_early", {"SP_NO_EARLY_DEREFS": "1"}), ("no_quad", {"SP_IPA_QUAD": "0"}), ("cpt1_smem", {"SP_EARLY_MSM_CPT": "1", "SP_EARLY_MSM_SMEM": "61440"})]:
+    for name, env in [("default", {}), ("no_early", {"SP_NO_EARLY_DEREFS": "1"}), ("cpt1_smem", {"SP_EARLY_MSM_CPT": "1", "SP_EARLY_MSM_SMEM": "61440"})]:
         e = dict(os.environ); e.update(env)
         out = subprocess.run([sys.executable, os.path.join(root, "tools", "ab_prove.py"), name, "12", "1"], env=e, capture_output=True, text=True, timeout=600)
         assert out.returncode == 0, out.stderr[-2000:]

@@ -11,7 +11,7 @@ tag = os.environ.get("SP_LIB_TAG", "")
 try:
     peak = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"]
 except Exception:
-    peak = 6650.0
+    peak = 3350.0   # H100 SXM data sheet (bench.py's fallback)
 ctx = sb.default_context()
 n = 1 << logn
 rng = np.random.default_rng(0)
@@ -23,7 +23,7 @@ def rand_table(n):
     return t
 
 
-res = {"tag": tag, "logn": logn, "constfold": os.environ.get("SP_SC_CONSTFOLD"), "v2": bool(os.environ.get("SP_SC_V2")), "tma": bool(os.environ.get("SP_SC_TMA")), "persist": bool(os.environ.get("SP_SC_PERSIST"))}
+res = {"tag": tag, "logn": logn}
 for kind, nt, name in [(2, 4, "cubic4"), (0, 2, "quad"), (1, 3, "cubic3")]:
     polys = [sb.DensePolynomial(rand_table(n)) for _ in range(nt)]
     r = sb.prg_scalars("r", 1)[0]
