@@ -486,7 +486,7 @@ int sp_ipa_finish(sp_ctx* ctx, sp_ipa* h, uint64_t a_hat[4], uint64_t b_hat[4], 
   SP_TRY(ctx)
   Ctx& c = ctx->c;
   if (h->cur != 1) throw SpError(SP_ERR_INVALID_ARG, "ipa: rounds remain");
-  dev::msm_rows(h->pts.p, h->gs->table.p, h->gs->wbits, h->svec.p, h->n, 1, h->n, nullptr, 0, c.scratch.p, c.stream);
+  dev::msm_rows(h->pts.p, h->gs->table.p, h->gs->wbits, h->gs->rows(), h->svec.p, h->n, 1, h->n, nullptr, 0, c.scratch.p, c.stream);
   DevBuf<uint8_t> comp(32);
   dev::compress_batch(comp.p, h->pts.p, 1, c.stream);
   dev::d2h(a_hat, h->a.p, 32, c.stream);

@@ -111,6 +111,22 @@ SP_HD ge ge_scalarmul(const u256& k, const ge& p) {
   return acc;
 }
 
+// Signed W-bit recoding of a canonical scalar k < 2^253 (W <= 24): k = sum_w d_w * 2^(W*w) over ceil(253/W) windows, d_w in (-2^(W-1), 2^(W-1)].
+// A window value above 2^(W-1) becomes v - 2^W and carries one into the next window; the top window never carries (its value is < 2^(W-1)).
+SP_HD uint32_t scalar_window(const u256& k, int w, int wbits) {
+  const int b = w * wbits, limb = b >> 5, sh = b & 31;
+  if (limb >= 8) return 0;
+  uint32_t v = k.v[limb] >> sh;
+  if (sh + wbits > 32 && limb + 1 < 8) v |= k.v[limb + 1] << (32 - sh);
+  return v & ((1u << wbits) - 1u);
+}
+SP_HD int signed_digit(const u256& k, int w, int wbits, uint32_t& carry) {   // the digit of window w, given the carry out of window w-1; updates carry
+  const uint32_t half = 1u << (wbits - 1);
+  const uint32_t v = scalar_window(k, w, wbits) + carry;
+  carry = v > half ? 1u : 0u;
+  return carry ? (int)v - (int)(2 * half) : (int)v;
+}
+
 // ---------------------------------------------------------------------------------------------- ristretto255
 SP_HD u256 bytes_to_u256(const uint8_t* b) {
   u256 r;

@@ -149,6 +149,8 @@ struct GenSet {
   DevBuf<ge> G;
   DevBuf<ge_niels> table;
   int wbits = 8;               // window width of `table` (host_tab is always 8-bit)
+  DevBuf<ge_niels> row_table;  // d * G_j for the row MSM of large sets (dev::build_row_table); empty for small sets
+  const ge_niels* rows() const { return row_table.n ? row_table.p : nullptr; }
   std::map<size_t, HostBaseTable> host_tab;
   std::vector<Cp> compressed;  // lazily filled export
   GenSet(Ctx* c, const std::string& label, size_t nbases, const std::vector<size_t>& host_bases);

@@ -97,6 +97,43 @@ int spt_fixed_base_mul(const uint8_t* k_mont, const uint8_t* a32, uint8_t* out32
   memcpy(out32, c.b, 32);
   return 1;
 }
+// signed W-bit recoding of the row MSM (curve.cuh signed_digit) of a canonical scalar; returns the window count
+int spt_signed_digits(const uint8_t* k_canonical, int wbits, int* out) {
+  const u256 k = in256(k_canonical);
+  const int nwin = (253 + wbits - 1) / wbits;
+  uint32_t carry = 0;
+  for (int w = 0; w < nwin; w++) out[w] = signed_digit(k, w, wbits, carry);
+  return nwin;
+}
+// the row MSM's arithmetic on one row: per-window sums S_w = sum_j d_{j,w} * P_j (|d| * P_j standing in for the row-table entry), then
+// out = sum_w 2^(W*w) S_w by Horner's rule with W doublings per window.  k_mont: n Montgomery scalars, pts: n encodings
+int spt_row_msm(const uint8_t* k_mont, const uint8_t* pts, size_t n, int wbits, uint8_t* out32) {
+  const int nwin = (253 + wbits - 1) / wbits;
+  std::vector<ge> P(n);
+  for (size_t j = 0; j < n; j++) if (!ristretto_decode(P[j], in256(pts + 32 * j))) return 0;
+  std::vector<ge> S(nwin, ge_identity());
+  for (size_t j = 0; j < n; j++) {
+    const u256 km = in256(k_mont + 32 * j);
+    if (fq_is_zero(km)) continue;
+    const u256 k = fq_from_mont(km);
+    uint32_t carry = 0;
+    for (int w = 0; w < nwin; w++) {
+      const int d = signed_digit(k, w, wbits, carry);
+      if (d == 0) continue;
+      u256 ad = fq_zero();
+      ad.v[0] = (uint32_t)(d < 0 ? -d : d);
+      const ge e = ge_scalarmul(ad, P[j]);
+      S[w] = ge_add(S[w], d < 0 ? ge_neg(e) : e);
+    }
+  }
+  ge acc = S[nwin - 1];
+  for (int w = nwin - 2; w >= 0; w--) {
+    for (int i = 0; i < wbits; i++) acc = ge_dbl(acc);
+    acc = ge_add(acc, S[w]);
+  }
+  out256(out32, ristretto_encode(acc));
+  return 1;
+}
 // radix-2^51 host arithmetic (host_fe51.hpp) against the 8x32-limb field code: mul, sqr, add, sub, freeze on raw 256-bit inputs
 void spt_fe51_ops(const uint8_t* a32, const uint8_t* b32, uint8_t* out160) {
   fe51 a = fe_from_u256(in256(a32)), b = fe_from_u256(in256(b32));

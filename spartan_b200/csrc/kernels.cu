@@ -8,7 +8,8 @@
 //   K3/K4  msm_rows : Pedersen commitments sum_j s_j*G_j (+ blind*h) for L rows sharing one generator set
 //          (reference: dalek vartime_multiscalar_mul behind src/group.rs:98-117, called from src/commitments.rs:80-92 and
 //           src/dense_mlpoly.rs:165-177).  Generators are fixed per `Gens`, so the kernel is a fixed-base comb: 8-bit signed
-//           windows, 128-entry affine-niels tables per (generator, window) resident in HBM, 7M mixed additions.
+//           windows, 128-entry affine-niels tables per (generator, window) resident in HBM, 7M mixed additions.  Many long rows
+//           use 16-bit row tables (d * G_j only) instead: per-window sums, then a doubling tail per row.
 //   K6     compress_batch / decompress_batch / gens_from_uniform (RFC 9496).
 //   K7     eq_evals, dot, bound_rows, lincomb3, hadamard, spmv, SPARK hash layer, IPA helpers.
 // All arithmetic is exact 256-bit integer work on the INT32 pipe; no tensor-core formulation exists (DESIGN.md).
@@ -573,6 +574,37 @@ void build_tables(ge_niels* table, const ge* G, size_t nbases, int wbits, cudaSt
   k_build_tables<<<(unsigned)((threads + 63) / 64), 64, 0, s>>>(table, G, nbases, wbits, msm_nwin(wbits), (int)msm_depth(wbits));
   SP_LAUNCHED(); check("build_tables");
 }
+// ---- row tables: entry (j, d-1) = d * G_j, d = 1 .. 2^(ROW_W-1), affine niels, no per-window copies (3.1 MB per generator at ROW_W = 16).  The row MSM
+// sums the entries of each window separately and pays the window shift once per row (k_msm_horner).  One thread per (generator, run of 64 entries).
+#ifndef SP_ROW_WBITS
+#define SP_ROW_WBITS 16
+#endif
+static_assert(SP_ROW_WBITS >= 14 && SP_ROW_WBITS <= 17, "row-table window width");
+constexpr int ROW_W = SP_ROW_WBITS, ROW_NWIN = (253 + ROW_W - 1) / ROW_W;
+constexpr size_t ROW_DEPTH = (size_t)1 << (ROW_W - 1);
+constexpr int ROW_BUILD_RUN = 64;
+size_t row_table_entries(size_t nbases) { return nbases * ROW_DEPTH; }
+__global__ void __launch_bounds__(64) k_build_row_table(ge_niels* rt, const ge* __restrict__ G, size_t nbases) {
+  constexpr size_t RUNS = ROW_DEPTH / ROW_BUILD_RUN;
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nbases * RUNS) return;
+  const size_t j = t / RUNS, d0 = (t % RUNS) * ROW_BUILD_RUN;
+  const ge P = ld_ge(G + j);
+  u256 k = fq_zero();
+  k.v[0] = (uint32_t)(d0 + 1);
+  ge acc = ge_scalarmul(k, P);
+  ge_niels* dst = rt + j * ROW_DEPTH + d0;
+  for (int i = 0; i < ROW_BUILD_RUN; i++) {
+    const ge_niels nl = ge_to_niels(acc);
+    st256(&dst[i].ypx, nl.ypx); st256(&dst[i].ymx, nl.ymx); st256(&dst[i].t2d, nl.t2d);
+    acc = ge_add(acc, P);
+  }
+}
+void build_row_table(ge_niels* rt, const ge* G, size_t nbases, cudaStream_t s) {
+  const size_t threads = nbases * (ROW_DEPTH / ROW_BUILD_RUN);
+  k_build_row_table<<<(unsigned)((threads + 63) / 64), 64, 0, s>>>(rt, G, nbases);
+  SP_LAUNCHED(); check("build_row_table");
+}
 
 // ---- multi-row fixed-base MSM
 // grid = (chunks, L); block = 128 threads = COLS columns x GROUPS window-groups of one row.  A thread owns one scalar and the windows
@@ -904,6 +936,112 @@ void ipa_msm(ge* out, const ge_niels* table, int wbits, const u256* a, const u25
   SP_LAUNCHED(); check("ipa_msm_quad");
 }
 
+// ---- row MSM over the row tables, for many long rows (the witness commitment, the dereferenced SPARK values).  Per term it does ROW_NWIN mixed
+// additions instead of the per-window tables' 20 (13-bit windows), at the price of (ROW_NWIN - 1) * ROW_W doublings per row:
+//   k_msm_digits   signed ROW_W-bit digits of every scalar, once: digits[(row * ROW_NWIN + w) * ncols + col]
+//   k_msm_win      four lanes own window w of one row and one chunk of ROW_CHUNK columns; lane i adds the table entries of columns i, i + 4, ...
+//                  of the chunk into one accumulator, then two shuffle levels give the chunk's part of S[row, w] = sum_col d[row, w, col] * G_col
+//   k_msm_chunks   S[row, w] = the sum over the chunks
+//   k_msm_horner   out[row] = sum_w 2^(ROW_W * w) S[row, w] by Horner's rule, four lanes per row (quad_dbl / quad_add)
+// A CTA makes ROW_CHUNK / 4 = 64 mixed additions per lane and retires, about as many as a CTA of k_msm_rows makes.  Short-lived CTAs matter when the
+// MSM runs on the background stream: a kernel of the prover's stream that does not fit beside the resident MSM CTAs starts only when some of them
+// retire, and one lane owning a whole 4096-column row (256 additions) delayed the inner-product rounds running beside it by 2 ms per proof.
+// doubling: dbl-2008-hwcd (ge_dbl) on a quad, lane c holding coordinate c: one round of squarings (X^2 | Y^2 | Z^2 | (X+Y)^2), one of products
+static __device__ __noinline__ u256 quad_dbl(u256 p, int c, int lane) {
+  const int base = lane & ~3;
+  const u256 x = shfl_idx_256(p, base), y = shfl_idx_256(p, base + 1);
+  const u256 m = fp_sqr(sel256(c == 3, fp_add(x, y), p));
+  const u256 A = shfl_idx_256(m, base), B = shfl_idx_256(m, base + 1), Z2 = shfl_idx_256(m, base + 2), S = shfl_idx_256(m, base + 3);
+  const u256 C = fp_add(Z2, Z2), D = fp_neg(A);
+  const u256 E = fp_sub(fp_sub(S, A), B), G = fp_add(D, B), F = fp_sub(G, C), H = fp_sub(D, B);
+  // lane 0: X3 = E F, lane 1: Y3 = G H, lane 2: Z3 = F G, lane 3: T3 = E H
+  return fp_mul(sel256(c == 1, G, sel256(c == 2, F, E)), sel256(c == 0, F, sel256(c == 2, G, H)));
+}
+__global__ void __launch_bounds__(128) k_msm_digits(int* digits, const u256* __restrict__ scalars, size_t stride, size_t L, size_t R, const u256* __restrict__ blinds) {
+  const size_t ncols = R + (blinds ? 1 : 0);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < L * ncols; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t row = i / ncols, col = i - row * ncols;
+    u256 k = col < R ? ld256_ro(scalars + row * stride + col) : ld256_ro(blinds + row);
+    int* dst = digits + row * ROW_NWIN * ncols + col;
+    const bool zero = fq_is_zero(k);
+    if (!zero) k = fq_from_mont(k);  // group.rs:110-113: scalars leave Montgomery form before the MSM
+    uint32_t carry = 0;
+#pragma unroll
+    for (int w = 0; w < ROW_NWIN; w++) {
+      const int d = signed_digit(k, w, ROW_W, carry);
+      dst[(size_t)w * ncols] = zero ? 0 : d;
+    }
+  }
+}
+#ifndef SP_ROW_CHUNK
+#define SP_ROW_CHUNK 256
+#endif
+constexpr size_t ROW_CHUNK = SP_ROW_CHUNK;
+// grid = (groups / 32, chunks): CTA (x, y) sums columns [y * ROW_CHUNK, (y + 1) * ROW_CHUNK) of the 32 (row, window) groups [32 x, 32 x + 32)
+__global__ void __launch_bounds__(128, SP_MSM_LB) k_msm_win(ge* part, const ge_niels* __restrict__ rt, const int* __restrict__ digits, size_t groups, size_t ncols,
+                                                            size_t R, size_t blind_base) {
+  const size_t g = (size_t)blockIdx.x * 32 + threadIdx.x / 4;   // (row, window) = (g / ROW_NWIN, g % ROW_NWIN)
+  const int lane = threadIdx.x % 4;
+  const size_t c0 = (size_t)blockIdx.y * ROW_CHUNK, c1 = c0 + ROW_CHUNK < ncols ? c0 + ROW_CHUNK : ncols;
+  ge acc = ge_identity();
+  if (g < groups) {
+    const int* dg = digits + g * ncols;
+#pragma unroll 1
+    for (size_t col = c0 + lane; col < c1; col += 4) {
+      const int d = __ldg(dg + col);
+      if (d == 0) continue;
+      const size_t base = col < R ? col : blind_base;
+      const ge_niels* e = rt + base * ROW_DEPTH + ((d < 0 ? -d : d) - 1);
+      ge_niels nl;
+      nl.ypx = ld256_ro(&e->ypx); nl.ymx = ld256_ro(&e->ymx); nl.t2d = ld256_ro(&e->t2d);
+      acc = ge_madd(acc, nl, d < 0);
+    }
+  }
+  acc = ge_add(acc, shfl_down_ge(acc, 2));   // the four lanes of a group are adjacent and 4-aligned in the warp
+  acc = ge_add(acc, shfl_down_ge(acc, 1));
+  if (lane == 0 && g < groups) st_ge(part + g * gridDim.y + blockIdx.y, acc);
+}
+__global__ void __launch_bounds__(128) k_msm_chunks(ge* sums, const ge* __restrict__ part, size_t groups, int chunks) {
+  const size_t g = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= groups) return;
+  ge acc = ld_ge(part + g * chunks);
+  for (int c = 1; c < chunks; c++) acc = ge_add(acc, ld_ge(part + g * chunks + c));
+  st_ge(sums + g, acc);
+}
+__global__ void __launch_bounds__(32) k_msm_horner(ge* out, const ge* __restrict__ sums, size_t L) {
+  const int lane = threadIdx.x & 31, c = lane & 3;
+  const size_t row = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 2;
+  const bool live = row < L;                                 // every lane takes part in the shuffles; rows past L carry the identity
+  const u256* S = reinterpret_cast<const u256*>(sums + (live ? row : 0) * ROW_NWIN) + c;   // coordinate c of S[row, w] at S[4 w]
+  u256 P = live ? ld256(S + 4 * (ROW_NWIN - 1)) : quad_identity(c);
+#pragma unroll 1
+  for (int w = ROW_NWIN - 2; w >= 0; w--) {
+#pragma unroll 1
+    for (int i = 0; i < ROW_W; i++) P = quad_dbl(P, c, lane);
+    P = quad_add(P, live ? ld256(S + 4 * w) : quad_identity(c), c, lane);
+  }
+  if (live) st256(reinterpret_cast<u256*>(out + row) + c, P);
+}
+static size_t row_msm_chunks(size_t ncols) { return (ncols + ROW_CHUNK - 1) / ROW_CHUNK; }
+static size_t row_msm_points_bytes(size_t L, size_t ncols) { return (L * ROW_NWIN * (row_msm_chunks(ncols) + 1) * sizeof(ge) + 255) / 256 * 256; }
+static size_t row_msm_scratch_bytes(size_t L, size_t ncols) { return row_msm_points_bytes(L, ncols) + L * ROW_NWIN * ncols * sizeof(int); }
+static void msm_rows_win(ge* out, const ge_niels* rt, const u256* scalars, size_t stride, size_t L, size_t R, const u256* blinds, size_t blind_base,
+                         void* scratch, cudaStream_t s, size_t smem_pad) {
+  const size_t ncols = R + (blinds ? 1 : 0), groups = L * ROW_NWIN, chunks = row_msm_chunks(ncols);
+  ge* sums = (ge*)scratch;
+  ge* part = sums + groups;
+  int* digits = (int*)((char*)scratch + row_msm_points_bytes(L, ncols));
+  k_msm_digits<<<grid_for(L * ncols, 128, 16), 128, 0, s>>>(digits, scalars, stride, L, R, blinds);
+  if (smem_pad > (48u << 10)) cudaFuncSetAttribute(k_msm_win, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pad);
+  k_msm_win<<<dim3((unsigned)((groups + 31) / 32), (unsigned)chunks), 128, smem_pad, s>>>(part, rt, digits, groups, ncols, R, blind_base);
+  k_msm_chunks<<<(unsigned)((groups + 127) / 128), 128, 0, s>>>(sums, part, groups, (int)chunks);
+  k_msm_horner<<<(unsigned)((L * 4 + 31) / 32), 32, 0, s>>>(out, sums, L);
+  SP_LAUNCHED(); SP_LAUNCHED(); SP_LAUNCHED(); SP_LAUNCHED(); check("msm_rows_win");
+}
+// many rows of many terms: the doubling tail is shared by a row's terms and runs beside the other rows.  Short rows, few rows (the blind and delta
+// batches of the ZK sumchecks, single-row commitments) stay on the per-window tables, which need no doublings.
+static bool msm_rows_use_row_table(size_t L, size_t R) { return L >= 64 && R >= 512; }
+
 static int msm_pick_groups(size_t L, size_t R) {
   // enough threads to fill the chip: one thread per scalar once L*R is large (least reduction work), else split the windows
   size_t cols = L * (R + 1);
@@ -919,7 +1057,10 @@ static int msm_pick_cpt(size_t L, size_t ncols, int groups) {
   return (ncols >= 4 * cols && blocks4 >= (size_t)sm_count() * 4) ? 4 : 1;
 }
 static size_t msm_chunks(size_t R1, int groups, int cpt) { size_t cols = (128 / groups) * (size_t)cpt; return (R1 + cols - 1) / cols; }
-size_t msm_scratch_bytes(size_t L, size_t R) { return L * msm_chunks(R + 1, 8, 1) * sizeof(ge); }
+size_t msm_scratch_bytes(size_t L, size_t R) {
+  const size_t per_window = L * msm_chunks(R + 1, 8, 1) * sizeof(ge);
+  return msm_rows_use_row_table(L, R) ? std::max(per_window, row_msm_scratch_bytes(L, R + 1)) : per_window;
+}
 template <int WBITS, int GROUPS>
 static void msm_launch2(int cpt, dim3 grid, cudaStream_t s, ge* pp, const ge_niels* table, const u256* sc, size_t stride, size_t R, const u256* bl,
                         size_t blind_base, size_t smem_pad) {
@@ -940,9 +1081,13 @@ static void msm_launch(int groups, int cpt, dim3 grid, cudaStream_t s, ge* pp, c
   else if (groups == 4) msm_launch2<WBITS, 4>(cpt, grid, s, pp, table, sc, stride, R, bl, blind_base, smem_pad);
   else msm_launch2<WBITS, 8>(cpt, grid, s, pp, table, sc, stride, R, bl, blind_base, smem_pad);
 }
-void msm_rows(ge* out, const ge_niels* table, int wbits, const u256* scalars, size_t stride, size_t L, size_t R, const u256* blinds, size_t blind_base,
-              void* scratch, cudaStream_t s, const MsmTune& tune) {
+void msm_rows(ge* out, const ge_niels* table, int wbits, const ge_niels* row_table, const u256* scalars, size_t stride, size_t L, size_t R,
+              const u256* blinds, size_t blind_base, void* scratch, cudaStream_t s, const MsmTune& tune) {
   ProfScope ps("msm_rows", 32.0 * (double)L * (double)R + 32.0 * (double)R, s);
+  if (row_table && msm_rows_use_row_table(L, R)) {
+    msm_rows_win(out, row_table, scalars, stride, L, R, blinds, blind_base, scratch, s, tune.smem_pad);
+    return;
+  }
   const size_t ncols = R + (blinds ? 1 : 0);
   int groups = msm_pick_groups(L, R);
   int cpt = tune.cpt ? tune.cpt : msm_pick_cpt(L, ncols, groups);

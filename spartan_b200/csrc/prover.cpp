@@ -154,8 +154,18 @@ GenSet::GenSet(Ctx* c, const ge* d_points, size_t nbases_, const std::vector<siz
   finish(host_bases);
 }
 void GenSet::finish(const std::vector<size_t>& host_bases) {
-  // large generator sets get 13-bit windows (20 additions per term instead of 32; 7.9 MB of table per generator); SP_MSM_WINDOW=15 trades
-  // 26.7 MB per generator for 17 additions per term (110 GB for the 4098 generators of a 2^20 SNARK: more than an 80 GB H100 holds)
+  // large sets first get a row table (d * G_j only, 3.1 MB per generator at 16 bits): the big row commitments run on it with 16 additions per
+  // term and a doubling tail per row.  It comes first because it serves the largest MSMs; it is skipped only when it would not fit.
+  if (nbases >= 512) {
+    size_t free_b = 0, total_b = 0;
+    dev::mem_info(&free_b, &total_b);
+    if ((double)dev::row_table_entries(nbases) * sizeof(ge_niels) <= 0.65 * (double)free_b) {
+      row_table.alloc(dev::row_table_entries(nbases));
+      dev::build_row_table(row_table.p, G.p, nbases, ctx->stream);
+    }
+  }
+  // the per-window table serves the inner-product rounds and the small commitments.  Large generator sets get 13-bit windows (20 additions per
+  // term instead of 32; 7.9 MB of table per generator); SP_MSM_WINDOW=15 trades 26.7 MB per generator for 17 additions per term
   const char* wenv = getenv("SP_MSM_WINDOW");
   if (nbases < 512) wbits = 8;
   else if (wenv) wbits = atoi(wenv);
@@ -361,11 +371,11 @@ struct ZkPre {
     dev::h2d(d_b.p + 3 * num_rounds, blinds_evals.data(), num_rounds * sizeof(u256), ctx.stream);
     if (ctx.scratch.n < dev::msm_scratch_bytes(num_rounds, nco) + 64) ctx.ensure_scratch(dev::msm_scratch_bytes(num_rounds, nco) + 64);
     const GenSet& gs = *gn.set;
-    dev::msm_rows(d_pts.p, gs.table.p, gs.wbits, d_s.p, nco, num_rounds, nco, d_b.p, gn.h, ctx.scratch.p, ctx.stream);                    // delta_j
+    dev::msm_rows(d_pts.p, gs.table.p, gs.wbits, gs.rows(), d_s.p, nco, num_rounds, nco, d_b.p, gn.h, ctx.scratch.p, ctx.stream);                    // delta_j
     dev::compress_batch(d_c.p, d_pts.p, num_rounds, ctx.stream);
-    dev::msm_rows(d_pts.p + num_rounds, gs.table.p, gs.wbits, d_s.p, 0, num_rounds, 0, d_b.p + num_rounds, g1.h, ctx.scratch.p, ctx.stream);      // r_beta_j * h
-    dev::msm_rows(d_pts.p + 2 * num_rounds, gs.table.p, gs.wbits, d_s.p, 0, num_rounds, 0, d_b.p + 2 * num_rounds, gn.h, ctx.scratch.p, ctx.stream);  // blinds_poly[j] * h
-    dev::msm_rows(d_pts.p + 3 * num_rounds, gs.table.p, gs.wbits, d_s.p, 0, num_rounds, 0, d_b.p + 3 * num_rounds, g1.h, ctx.scratch.p, ctx.stream);  // blinds_evals[j] * h
+    dev::msm_rows(d_pts.p + num_rounds, gs.table.p, gs.wbits, gs.rows(), d_s.p, 0, num_rounds, 0, d_b.p + num_rounds, g1.h, ctx.scratch.p, ctx.stream);      // r_beta_j * h
+    dev::msm_rows(d_pts.p + 2 * num_rounds, gs.table.p, gs.wbits, gs.rows(), d_s.p, 0, num_rounds, 0, d_b.p + 2 * num_rounds, gn.h, ctx.scratch.p, ctx.stream);  // blinds_poly[j] * h
+    dev::msm_rows(d_pts.p + 3 * num_rounds, gs.table.p, gs.wbits, gs.rows(), d_s.p, 0, num_rounds, 0, d_b.p + 3 * num_rounds, g1.h, ctx.scratch.p, ctx.stream);  // blinds_evals[j] * h
     dev::d2h(stage, d_c.p, 32 * num_rounds, ctx.stream);
     dev::d2h(stage + 32 * num_rounds, d_pts.p + num_rounds, 3 * num_rounds * sizeof(ge), ctx.stream);
     enqueued = true;
@@ -521,12 +531,12 @@ Cp commit_rows_and_compress(Ctx& ctx, const CommitKey& key, const u256* d_scalar
   // rows are independent MSMs over the same generators: when sharded, rank r commits rows [r*L/W, (r+1)*L/W) and the 32-byte encodings are all-gathered
   const bool split = W > 1 && L >= 2 * W && L % W == 0;
   const size_t Lr = split ? L / W : L, row0 = split ? (size_t)ctx.rank() * Lr : 0;
-  dev::msm_rows(rows.p, key.set->table.p, key.set->wbits, d_scalars + row0 * stride, stride, Lr, R, blinds ? d_bl.p + row0 : nullptr, key.h, ctx.scratch.p, ctx.stream);
+  dev::msm_rows(rows.p, key.set->table.p, key.set->wbits, key.set->rows(), d_scalars + row0 * stride, stride, Lr, R, blinds ? d_bl.p + row0 : nullptr, key.h, ctx.scratch.p, ctx.stream);
   if (!blinds && blinds_late) {
     const Fq* bl = blinds_late();
     d_bl.alloc(L); bh.alloc(Lr);
     dev::h2d(d_bl.p, bl, L * sizeof(u256), ctx.stream);
-    dev::msm_rows(bh.p, key.set->table.p, key.set->wbits, d_scalars, 0, Lr, 0, d_bl.p + row0, key.h, ctx.scratch.p, ctx.stream);   // blinds[i]*h (rows without generator terms)
+    dev::msm_rows(bh.p, key.set->table.p, key.set->wbits, key.set->rows(), d_scalars, 0, Lr, 0, d_bl.p + row0, key.h, ctx.scratch.p, ctx.stream);   // blinds[i]*h (rows without generator terms)
     dev::add_points(rows.p, bh.p, Lr, ctx.stream);
   }
   dev::compress_batch(comp.p, rows.p, Lr, ctx.stream);
@@ -559,7 +569,7 @@ static void bullet_prove(Ctx& ctx, Transcript& T, const PolyCommitmentGens& gens
     std::vector<Fq> bl(2 * rounds);
     for (size_t k = 0; k < rounds; k++) { bl[2 * k] = blinds_vec[k].first; bl[2 * k + 1] = blinds_vec[k].second; }
     dev::h2d(d_bl.p, bl.data(), bl.size() * sizeof(u256), ctx.stream);
-    dev::msm_rows(d_bh.p, gs.table.p, gs.wbits, lr.p, 0, 2 * rounds, 0, d_bl.p, gens.gens_n.h, ctx.scratch.p, ctx.stream);
+    dev::msm_rows(d_bh.p, gs.table.p, gs.wbits, gs.rows(), lr.p, 0, 2 * rounds, 0, d_bl.p, gens.gens_n.h, ctx.scratch.p, ctx.stream);
     dev::d2h(bh.data(), d_bh.p, bh.size() * sizeof(ge), ctx.stream);   // pageable target: completes before the call returns
   }
   u256* d_c = ctx.small.p + 16;  // c_L, c_R
@@ -627,7 +637,7 @@ static void bullet_prove(Ctx& ctx, Transcript& T, const PolyCommitmentGens& gens
     memcpy(&odd, ctx.host_res + 8, sizeof(ge)); memcpy(&even, ctx.host_res + 12, sizeof(ge));
     g_hat = hge_add(to_hge(odd), to_hge(even));
   } else {
-    dev::msm_rows(pts.p, gs.table.p, gs.wbits, svec.p, n, 1, n, nullptr, 0, ctx.scratch.p, ctx.stream);
+    dev::msm_rows(pts.p, gs.table.p, gs.wbits, gs.rows(), svec.p, n, 1, n, nullptr, 0, ctx.scratch.p, ctx.stream);
     dev::d2h(ctx.pinned + 64, pts.p, sizeof(ge), ctx.stream);
     ctx.sync();
     ge g;

@@ -498,7 +498,7 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
     for (int m = 0; m < 3; m++) dev::gather(part ? col_val[m] : row_val[m], mem, (part ? enc.col : enc.row).ops_addr_idx[m].p, N, s2);
     const size_t first = (size_t)part * n_part + (shard_rows ? (size_t)ctx.rank() * cnt : 0);
     const CommitKey& key = gens.gens_derefs.gens_n;
-    dev::msm_rows(early_rows.p + (size_t)part * cnt, key.set->table.p, key.set->wbits, derefs.p + first * R_d, R_d, cnt, R_d, nullptr, key.h, ctx.scratch2.p, s2, early_tune);
+    dev::msm_rows(early_rows.p + (size_t)part * cnt, key.set->table.p, key.set->wbits, key.set->rows(), derefs.p + first * R_d, R_d, cnt, R_d, nullptr, key.h, ctx.scratch2.p, s2, early_tune);
     dev::compress_batch(early_comp.p + 32 * (size_t)part * cnt, early_rows.p + (size_t)part * cnt, cnt, s2);
   };
   R1csHooks hooks;
