@@ -85,8 +85,10 @@ def first_diff(a, b):
 def test_snark_bench_configuration_bytes_match_oracle(sb, logn):
     """BASELINE.json configs[1] — exactly what bench.py times (2^20 constraints / variables / non-zeros, 10 inputs, instance seed 0, tape
     seed 0, transcript label b"example") — and the 2^16 sample: computation commitment and proof bytes identical to the oracle's, which runs
-    on all host cores.  This puts k_msm_rows<13,1,4>, k_ipa_msm_quad<13,5> (4098-generator sets) and the streaming sumcheck kernels under a byte
-    diff inside a whole proof.  Also the reference's published structure at 2^20: 47,024 / 64,712 / 133,720 bytes (README.md:362,371,374)."""
+    on all host cores.  This puts the row-table MSM (k_msm_digits, k_msm_win, k_msm_chunks, k_msm_horner) of the big row commitments,
+    k_ipa_msm_quad<13,5> (4098-generator sets) and the streaming sumcheck kernels under a byte diff inside a whole proof; every k_msm_rows instance
+    is checked directly by test_gpu_msm_instances.py.  Also the reference's published structure at 2^20: 47,024 / 64,712 / 133,720 bytes
+    (README.md:362,371,374)."""
     n = 1 << logn
     oc.lib.oracle_set_threads(max(1, (os.cpu_count() or 2) // 2))
     oi, ovars, oinputs = r1cs.Instance.produce_synthetic_r1cs(n, n, 10, 0)

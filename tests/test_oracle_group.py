@@ -4,6 +4,8 @@ The reference holds no group-level known answers (its group is curve25519-dalek,
 import ctypes as C
 import glob
 import hashlib
+import json
+import os
 import site
 
 import numpy as np
@@ -11,14 +13,10 @@ import pytest
 
 from oracle.spartan_ref import core as oc
 
-# RFC 9496 A.1: multiples 0..4 of the generator
-RFC_MULTIPLES = [
-    "0000000000000000000000000000000000000000000000000000000000000000",
-    "e2f2ae0a6abc4e71a884a961c500515f58e30b6aa582dd8db6a65945e08d2d76",
-    "6a493210f7499cd17fecb510ae0cea23a110e8d5b901f8acadd3095c73a3b919",
-    "94741f5d5d52755ece4f23f044ee27d5d1ea1e2bd196b462166b16152a9d0259",
-    "da80862773358b466ffadfe0b3293ab3d9fd53c5ea6c955358f568322daf6a57",
-]
+# RFC 9496 A.1 (multiples 0..4 of the generator) and A.2 (bad encodings), shared with the device tests
+with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "rfc9496.json")) as _f:
+    RFC = json.load(_f)
+RFC_MULTIPLES = RFC["multiples"]
 
 
 def _sodium():
@@ -39,14 +37,7 @@ def test_rfc9496_basepoint_multiples():
 
 def test_decode_rejects_bad_encodings():
     # RFC 9496 A.2: non-canonical field encodings and negative field elements
-    bad = [
-        "00ffffffffffffffffffffffffffffffffffffffffffffffffffffffffffffff",
-        "ffffffffffffffffffffffffffffffffffffffffffffffffffffffffffffff7f",
-        "f3ffffffffffffffffffffffffffffffffffffffffffffffffffffffffffff7f",
-        "edffffffffffffffffffffffffffffffffffffffffffffffffffffffffffff7f",
-        "0100000000000000000000000000000000000000000000000000000000000000",
-        "01ffffffffffffffffffffffffffffffffffffffffffffffffffffffffffff7f",
-    ]
+    bad = RFC["bad_encodings"]
     for h in bad:
         assert oc.Point.decompress(bytes.fromhex(h)) is None
 
