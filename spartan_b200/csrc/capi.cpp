@@ -166,65 +166,48 @@ static dev::ScInst make_inst(sp_poly* const* polys, int nt) {
   in.write_c = 1;
   return in;
 }
-int sp_sumcheck_eval(sp_ctx* ctx, int kind, sp_poly* const* polys, uint64_t out[3][4]) {
-  SP_TRY(ctx)
-  if (kind < 0 || kind > 2) throw SpError(SP_ERR_INVALID_ARG, "bad sumcheck kind");
-  int nt = kind_tables(kind);
-  check_same_len(polys, nt);
-  dev::ScInst in = make_inst(polys, nt);
-  dev::sc_eval((dev::ScKind)kind, &in, 1, polys[0]->len, ctx->c.small.p, ctx->c.red.p, ctx->c.stream);
-  Fq e[3];
-  ctx->c.get_small(0, e, 3);
-  memcpy(out, e, 96);
-  SP_CATCH(ctx)
-}
-int sp_sumcheck_fold_eval(sp_ctx* ctx, int kind, sp_poly* const* polys, const uint64_t r[4], uint64_t out[3][4]) {
-  SP_TRY(ctx)
-  if (kind < 0 || kind > 2) throw SpError(SP_ERR_INVALID_ARG, "bad sumcheck kind");
-  int nt = kind_tables(kind);
-  check_same_len(polys, nt);
-  if (polys[0]->len < 4) throw SpError(SP_ERR_INVALID_ARG, "fold_eval needs length >= 4");
-  Fq rr = fq_in(r);
-  dev::ScInst in = make_inst(polys, nt);
-  dev::sc_fold_eval((dev::ScKind)kind, &in, 1, polys[0]->len, rr.m, ctx->c.small.p, ctx->c.red.p, ctx->c.stream);
-  Fq e[3];
-  ctx->c.get_small(0, e, 3);
-  memcpy(out, e, 96);
-  for (int i = 0; i < nt; i++) polys[i]->len /= 2;
-  SP_CATCH(ctx)
-}
-// The same two calls on a connected context (sp_comm_connect), every rank passing its CYCLIC SHARDS of the tables (rank r holds the entries
+// sharded: the same calls on a connected context (sp_comm_connect), every rank passing its CYCLIC SHARDS of the tables (rank r holds the entries
 // r, r+W, r+2W, ...): the kernels exchange their partial sums over NVLink and every rank receives the evaluations of the whole tables.
 // Binding the top variable stays local as long as the local length is >= 2; shards must be of streaming size (>= 8192 entries) for fold_eval.
-static dev::HostSig xr_sig(Ctx& c) { dev::HostSig s; s.done = c.sig_done.p; return s; }
-int sp_sumcheck_eval_sharded(sp_ctx* ctx, int kind, sp_poly* const* polys, uint64_t out[3][4]) {
-  SP_TRY(ctx)
-  if (ctx->c.world() < 2) throw SpError(SP_ERR_INVALID_ARG, "not a connected multi-GPU context");
+static int sumcheck_tables(Ctx& c, int kind, sp_poly* const* polys, bool sharded) {
+  if (sharded && c.world() < 2) throw SpError(SP_ERR_INVALID_ARG, "not a connected multi-GPU context");
   if (kind < 0 || kind > 2) throw SpError(SP_ERR_INVALID_ARG, "bad sumcheck kind");
-  int nt = kind_tables(kind);
+  const int nt = kind_tables(kind);
   check_same_len(polys, nt);
+  return nt;
+}
+// sharded: the kernel's cross-rank completion counter and the next exchange (every rank issues it in the same order)
+static dev::HostSig xr_sig(Ctx& c, bool sharded) { dev::HostSig s; if (sharded) s.done = c.sig_done.p; return s; }
+static int sumcheck_eval(sp_ctx* ctx, int kind, sp_poly* const* polys, uint64_t out[3][4], bool sharded) {
+  SP_TRY(ctx)
+  Ctx& c = ctx->c;
+  const int nt = sumcheck_tables(c, kind, polys, sharded);
   dev::ScInst in = make_inst(polys, nt);
-  dev::sc_eval((dev::ScKind)kind, &in, 1, polys[0]->len, ctx->c.small.p, ctx->c.red.p, ctx->c.stream, xr_sig(ctx->c), ctx->c.comm->next_xr());
-  Fq e[3];
-  ctx->c.get_small(0, e, 3);
-  memcpy(out, e, 96);
+  dev::sc_eval((dev::ScKind)kind, &in, 1, polys[0]->len, c.small.p, c.red.p, c.stream, xr_sig(c, sharded), sharded ? c.comm->next_xr() : dev::XRank());
+  c.get_small(0, reinterpret_cast<Fq*>(out), 3);
   SP_CATCH(ctx)
 }
-int sp_sumcheck_fold_eval_sharded(sp_ctx* ctx, int kind, sp_poly* const* polys, const uint64_t r[4], uint64_t out[3][4]) {
+static int sumcheck_fold_eval(sp_ctx* ctx, int kind, sp_poly* const* polys, const uint64_t r[4], uint64_t out[3][4], bool sharded) {
   SP_TRY(ctx)
-  if (ctx->c.world() < 2) throw SpError(SP_ERR_INVALID_ARG, "not a connected multi-GPU context");
-  if (kind < 0 || kind > 2) throw SpError(SP_ERR_INVALID_ARG, "bad sumcheck kind");
-  int nt = kind_tables(kind);
-  check_same_len(polys, nt);
-  if (polys[0]->len < Ctx::SHARD_MIN_LOCAL) throw SpError(SP_ERR_INVALID_ARG, "sharded fold_eval needs shards of at least 8192 entries (gather the shards and finish on one GPU)");
+  Ctx& c = ctx->c;
+  const int nt = sumcheck_tables(c, kind, polys, sharded);
+  if (polys[0]->len < (sharded ? Ctx::SHARD_MIN_LOCAL : 4))
+    throw SpError(SP_ERR_INVALID_ARG, sharded ? "sharded fold_eval needs shards of at least 8192 entries (gather the shards and finish on one GPU)"
+                                              : "fold_eval needs length >= 4");
   Fq rr = fq_in(r);
   dev::ScInst in = make_inst(polys, nt);
-  dev::sc_fold_eval((dev::ScKind)kind, &in, 1, polys[0]->len, rr.m, ctx->c.small.p, ctx->c.red.p, ctx->c.stream, xr_sig(ctx->c), ctx->c.comm->next_xr());
-  Fq e[3];
-  ctx->c.get_small(0, e, 3);
-  memcpy(out, e, 96);
+  dev::sc_fold_eval((dev::ScKind)kind, &in, 1, polys[0]->len, rr.m, c.small.p, c.red.p, c.stream, xr_sig(c, sharded), sharded ? c.comm->next_xr() : dev::XRank());
+  c.get_small(0, reinterpret_cast<Fq*>(out), 3);
   for (int i = 0; i < nt; i++) polys[i]->len /= 2;
   SP_CATCH(ctx)
+}
+int sp_sumcheck_eval(sp_ctx* ctx, int kind, sp_poly* const* polys, uint64_t out[3][4]) { return sumcheck_eval(ctx, kind, polys, out, false); }
+int sp_sumcheck_fold_eval(sp_ctx* ctx, int kind, sp_poly* const* polys, const uint64_t r[4], uint64_t out[3][4]) {
+  return sumcheck_fold_eval(ctx, kind, polys, r, out, false);
+}
+int sp_sumcheck_eval_sharded(sp_ctx* ctx, int kind, sp_poly* const* polys, uint64_t out[3][4]) { return sumcheck_eval(ctx, kind, polys, out, true); }
+int sp_sumcheck_fold_eval_sharded(sp_ctx* ctx, int kind, sp_poly* const* polys, const uint64_t r[4], uint64_t out[3][4]) {
+  return sumcheck_fold_eval(ctx, kind, polys, r, out, true);
 }
 // prove_cubic_batched's evaluation loops (sumcheck.rs:290-357): ninst instances of A*B*C; an sp_poly may serve as C of several instances
 // (the shared eq table poly_C_par) — it is then bound once, through a temporary, and copied back
@@ -342,18 +325,24 @@ int sp_gens_create(sp_ctx* ctx, const uint8_t* label, size_t label_len, size_t n
   *out = g.release();
   SP_CATCH(ctx)
 }
+// n ristretto255 encodings -> device points.  ok == null: an encoding that is not a point is an SP_ERR_INVALID_POINT naming its index
+// (`what`); otherwise ok[i] tells whether encoding i is a point.
+static DevBuf<ge> decode_points(Ctx& c, const uint8_t* in32, size_t n, const char* what, int* ok = nullptr) {
+  DevBuf<uint8_t> d_in(32 * n + 1);
+  DevBuf<ge> pts(n + 1);
+  DevBuf<int> d_ok(n + 1);
+  std::vector<int> h_ok(ok ? 0 : n);
+  dev::h2d(d_in.p, in32, 32 * n, c.stream);
+  dev::decompress_batch(pts.p, d_ok.p, d_in.p, n, c.stream);
+  dev::d2h(ok ? ok : h_ok.data(), d_ok.p, sizeof(int) * n, c.stream);
+  c.sync();
+  for (size_t i = 0; i < h_ok.size(); i++)
+    if (!h_ok[i]) throw SpError(SP_ERR_INVALID_POINT, std::string(what) + ": encoding " + std::to_string(i) + " is not a ristretto255 point");
+  return pts;
+}
 int sp_gens_upload(sp_ctx* ctx, const uint8_t* compressed32, size_t n, sp_gens** out) {
   SP_TRY(ctx)
-  DevBuf<uint8_t> d_in(32 * (n + 1));
-  DevBuf<ge> g(n + 1);
-  DevBuf<int> ok(n + 1);
-  dev::h2d(d_in.p, compressed32, 32 * (n + 1), ctx->c.stream);
-  dev::decompress_batch(g.p, ok.p, d_in.p, n + 1, ctx->c.stream);
-  std::vector<int> h_ok(n + 1);
-  dev::d2h(h_ok.data(), ok.p, sizeof(int) * (n + 1), ctx->c.stream);
-  ctx->c.sync();
-  for (size_t i = 0; i <= n; i++)
-    if (!h_ok[i]) throw SpError(SP_ERR_INVALID_POINT, "gens_upload: encoding " + std::to_string(i) + " is not a ristretto255 point");
+  DevBuf<ge> g = decode_points(ctx->c, compressed32, n + 1, "gens_upload");
   std::unique_ptr<sp_gens> G(new sp_gens);
   G->n = n;
   G->set.reset(new GenSet(&ctx->c, g.p, n + 1, {}));
@@ -393,13 +382,7 @@ int sp_commit_rows(sp_ctx* ctx, const sp_gens* g, const sp_poly* p, size_t L, si
 }
 int sp_point_decompress_check(sp_ctx* ctx, const uint8_t* in32, size_t n, int* ok) {
   SP_TRY(ctx)
-  DevBuf<uint8_t> d_in(32 * n);
-  DevBuf<ge> pts(n);
-  DevBuf<int> d_ok(n);
-  dev::h2d(d_in.p, in32, 32 * n, ctx->c.stream);
-  dev::decompress_batch(pts.p, d_ok.p, d_in.p, n, ctx->c.stream);
-  dev::d2h(ok, d_ok.p, sizeof(int) * n, ctx->c.stream);
-  ctx->c.sync();
+  decode_points(ctx->c, in32, n, nullptr, ok);
   SP_CATCH(ctx)
 }
 int sp_point_roundtrip(sp_ctx* ctx, const uint8_t* in32, size_t n, uint8_t* out32) {
@@ -437,29 +420,26 @@ int sp_ipa_begin(sp_ctx* ctx, const sp_gens* gens, const sp_poly* a_vec, const s
   dev::d2d(h->a.p, a_vec->d.p, n * sizeof(u256), ctx->c.stream);
   dev::d2d(h->b.p, b_vec->d.p, n * sizeof(u256), ctx->c.stream);
   dev::fill_one(h->svec.p, n, ctx->c.stream);
-  ctx->c.ensure_scratch(std::max(dev::msm_scratch_bytes(4, n), dev::ipa_msm_scratch_points(n, gens->set->wbits) * sizeof(sp::ge)) + 64);
+  // the fused round launch and, for n >= 2, the one-row sum of sp_ipa_finish run on ipa_msm scratch; n = 1 runs msm_rows
+  ctx->c.ensure_scratch(std::max(dev::msm_scratch_bytes(1, n), dev::ipa_msm_scratch_points(n, gens->set->wbits) * sizeof(sp::ge)) + 64);
   ctx->c.sync();
   *out = h.release();
   SP_CATCH(ctx)
 }
 void sp_ipa_free(sp_ipa* h) { delete h; }
+static IpaRound ipa_round(sp_ipa* h) { return IpaRound{*h->ctx, *h->gs, h->a.p, h->b.p, h->svec.p, h->n, h->pts.p}; }
 // L = <a_L, G_R> + c_L*Q + blind_L*H,  R = <a_R, G_L> + c_R*Q + blind_R*H  with c_L = <a_L, b_R>, c_R = <a_R, b_L>   (bullet.rs:74-97)
 int sp_ipa_round_LR(sp_ctx* ctx, sp_ipa* h, const uint8_t Q32[32], const uint8_t H32[32], const uint64_t blind_L[4], const uint64_t blind_R[4], uint8_t L32[32],
                     uint8_t R32[32]) {
   SP_TRY(ctx)
-  Ctx& c = ctx->c;
   if (h->cur < 2) throw SpError(SP_ERR_INVALID_ARG, "ipa: the reduction is complete");
-  const size_t half = h->cur / 2;
-  const u256* da[2] = {h->a.p, h->a.p + half};
-  const u256* db[2] = {h->b.p + half, h->b.p};
-  dev::dot_pairs(c.small.p + 16, da, db, 2, half, c.red.p, c.stream);
-  dev::ipa_msm(h->pts.p, h->gs->table.p, h->gs->wbits, h->a.p, h->svec.p, h->cur, h->n, c.scratch.p, c.sig_done.p + 1, c.stream);
-  Fq cc[2];
-  c.get_small(16, cc, 2);
-  ge lr[2];
-  dev::d2h(lr, h->pts.p, 2 * sizeof(ge), c.stream);
-  c.sync();
   const hge Q = point_in(Q32, "Q"), H = point_in(H32, "H");
+  IpaRound rd = ipa_round(h);
+  rd.launch(h->cur);
+  Fq cc[2];
+  rd.wait_c(cc[0], cc[1]);
+  ge lr[2];
+  rd.wait_LR(lr[0], lr[1]);
   const Fq bl[2] = {fq_in(blind_L), fq_in(blind_R)};
   Cp outp[2];
   hge full[2];
@@ -474,10 +454,8 @@ int sp_ipa_fold(sp_ctx* ctx, sp_ipa* h, const uint64_t u[4], const uint64_t u_in
   if (h->cur < 2) throw SpError(SP_ERR_INVALID_ARG, "ipa: the reduction is complete");
   const Fq uu = fq_in(u), ui = fq_in(u_inv);
   if (!(uu * ui == Fq::one())) throw SpError(SP_ERR_INVALID_SCALAR, "ipa: u_inv is not the inverse of u");
-  const size_t half = h->cur / 2;
-  dev::ipa_fold_ab(h->a.p, h->b.p, half, uu.m, ui.m, ctx->c.stream);
-  dev::ipa_update_s(h->svec.p, half, h->n, uu.m, ui.m, ctx->c.stream);
-  h->cur = half;
+  ipa_round(h).fold(h->cur, uu, ui);
+  h->cur /= 2;
   ctx->c.sync();
   SP_CATCH(ctx)
 }
@@ -486,13 +464,10 @@ int sp_ipa_finish(sp_ctx* ctx, sp_ipa* h, uint64_t a_hat[4], uint64_t b_hat[4], 
   SP_TRY(ctx)
   Ctx& c = ctx->c;
   if (h->cur != 1) throw SpError(SP_ERR_INVALID_ARG, "ipa: rounds remain");
-  dev::msm_rows(h->pts.p, h->gs->table.p, h->gs->wbits, h->gs->rows(), h->svec.p, h->n, 1, h->n, nullptr, 0, c.scratch.p, c.stream);
-  DevBuf<uint8_t> comp(32);
-  dev::compress_batch(comp.p, h->pts.p, 1, c.stream);
   dev::d2h(a_hat, h->a.p, 32, c.stream);
   dev::d2h(b_hat, h->b.p, 32, c.stream);
-  dev::d2h(G_hat32, comp.p, 32, c.stream);
-  c.sync();
+  const Cp G = compress(RowSum(c, *h->gs, h->svec.p, h->n).collect());
+  memcpy(G_hat32, G.b, 32);
   SP_CATCH(ctx)
 }
 
@@ -504,16 +479,7 @@ static void points_from_ge(sp_ctx* ctx, sp_points* P, const ge* d_ge, size_t n) 
 }
 int sp_points_upload(sp_ctx* ctx, const uint8_t* in32, size_t n, sp_points** out) {
   SP_TRY(ctx)
-  DevBuf<uint8_t> d_in(32 * n + 1);
-  DevBuf<ge> g(n + 1);
-  DevBuf<int> ok(n + 1);
-  dev::h2d(d_in.p, in32, 32 * n, ctx->c.stream);
-  dev::decompress_batch(g.p, ok.p, d_in.p, n, ctx->c.stream);
-  std::vector<int> h_ok(n);
-  dev::d2h(h_ok.data(), ok.p, sizeof(int) * n, ctx->c.stream);
-  ctx->c.sync();
-  for (size_t i = 0; i < n; i++)
-    if (!h_ok[i]) throw SpError(SP_ERR_INVALID_POINT, "points_upload: encoding " + std::to_string(i) + " is not a ristretto255 point");
+  DevBuf<ge> g = decode_points(ctx->c, in32, n, "points_upload");
   std::unique_ptr<sp_points> P(new sp_points);
   points_from_ge(ctx, P.get(), g.p, n);
   ctx->c.sync();
@@ -560,60 +526,47 @@ int sp_points_export(sp_ctx* ctx, const sp_points* p, size_t offset, size_t n, u
   ctx->c.sync();
   SP_CATCH(ctx)
 }
-static void msm_var_run(sp_ctx* ctx, const sp_points* p, size_t offset, const u256* d_scalars, size_t n, uint8_t out32[32]) {
+// sharded: the MSM split over the ranks of a connected context.  Every rank passes ITS slice of the points (offset, scalars->len) and of the
+// scalars; the partial sums meet in a point-add all-reduce (all-gather of the W extended points into every window, W-term sum) and every rank
+// returns the same encoding of the sum over all ranks.
+static void msm_var_run(Ctx& c, const sp_points* p, size_t offset, const u256* d_scalars, size_t n, uint8_t out32[32], bool sharded) {
+  if (sharded && c.world() < 2) throw SpError(SP_ERR_INVALID_ARG, "not a connected multi-GPU context");
   if (offset + n > p->n) throw SpError(SP_ERR_INVALID_ARG, "msm_var: range outside the point set");
-  DevBuf<ge> out(1);
+  DevBuf<ge> out(1), total;
   DevBuf<uint8_t> comp(32);
   if (n == 0) {
     ge id = ge_identity();
-    dev::h2d(out.p, &id, sizeof(ge), ctx->c.stream);
+    dev::h2d(out.p, &id, sizeof(ge), c.stream);
   } else {
     const char* cenv = getenv("SP_PIP_WINDOW");
     dev::PipPlan plan = dev::pip_plan(n, cenv ? atoi(cenv) : 0);
     const size_t need = dev::pip_scratch_bytes(plan);
     if (need > p->scratch_bytes) { p->scratch.alloc(need); p->scratch_bytes = need; }   // the sort workspace stays with the point set
-    dev::msm_var(out.p, p->pts.p + offset, d_scalars, plan, p->scratch.p, ctx->c.stream);
+    dev::msm_var(out.p, p->pts.p + offset, d_scalars, plan, p->scratch.p, c.stream);
   }
-  dev::compress_batch(comp.p, out.p, 1, ctx->c.stream);
-  dev::d2h(out32, comp.p, 32, ctx->c.stream);
-  ctx->c.sync();
-}
-// MSM split over the ranks of a connected context: every rank passes ITS slice of the points (offset, scalars->len) and of the scalars; the
-// partial sums meet in a point-add all-reduce (all-gather of the W extended points into every window, W-term sum) and every rank returns the
-// same encoding of sum over all ranks.
-int sp_msm_var_sharded(sp_ctx* ctx, const sp_points* p, size_t offset, const sp_poly* scalars, uint8_t out32[32]) {
-  SP_TRY(ctx)
-  Ctx& c = ctx->c;
-  if (c.world() < 2) throw SpError(SP_ERR_INVALID_ARG, "not a connected multi-GPU context");
-  const size_t n = scalars->len;
-  if (offset + n > p->n) throw SpError(SP_ERR_INVALID_ARG, "msm_var: range outside the point set");
-  DevBuf<ge> part(1), total(1);
-  DevBuf<uint8_t> comp(32);
-  if (n == 0) { ge id = ge_identity(); dev::h2d(part.p, &id, sizeof(ge), c.stream); }
-  else {
-    const char* cenv = getenv("SP_PIP_WINDOW");
-    dev::PipPlan plan = dev::pip_plan(n, cenv ? atoi(cenv) : 0);
-    const size_t need = dev::pip_scratch_bytes(plan);
-    if (need > p->scratch_bytes) { p->scratch.alloc(need); p->scratch_bytes = need; }
-    dev::msm_var(part.p, p->pts.p + offset, scalars->d.p, plan, p->scratch.p, c.stream);
+  if (sharded) {
+    total.alloc(1);
+    dev::sum_points(total.p, reinterpret_cast<const ge*>(c.allgather_block(out.p, sizeof(ge))), c.world(), c.stream);
   }
-  const ge* all = reinterpret_cast<const ge*>(c.allgather_block(part.p, sizeof(ge)));
-  dev::sum_points(total.p, all, c.world(), c.stream);
-  dev::compress_batch(comp.p, total.p, 1, c.stream);
+  dev::compress_batch(comp.p, sharded ? total.p : out.p, 1, c.stream);
   dev::d2h(out32, comp.p, 32, c.stream);
   c.sync();
+}
+int sp_msm_var_sharded(sp_ctx* ctx, const sp_points* p, size_t offset, const sp_poly* scalars, uint8_t out32[32]) {
+  SP_TRY(ctx)
+  msm_var_run(ctx->c, p, offset, scalars->d.p, scalars->len, out32, true);
   SP_CATCH(ctx)
 }
 int sp_msm_var(sp_ctx* ctx, const sp_points* p, size_t offset, const uint64_t* scalars, size_t n, uint8_t out32[32]) {
   SP_TRY(ctx)
   DevBuf<u256> d(n ? n : 1);
   dev::h2d(d.p, scalars, n * 32, ctx->c.stream);
-  msm_var_run(ctx, p, offset, d.p, n, out32);
+  msm_var_run(ctx->c, p, offset, d.p, n, out32, false);
   SP_CATCH(ctx)
 }
 int sp_msm_var_resident(sp_ctx* ctx, const sp_points* p, size_t offset, const sp_poly* scalars, uint8_t out32[32]) {
   SP_TRY(ctx)
-  msm_var_run(ctx, p, offset, scalars->d.p, scalars->len, out32);
+  msm_var_run(ctx->c, p, offset, scalars->d.p, scalars->len, out32, false);
   SP_CATCH(ctx)
 }
 
@@ -754,7 +707,9 @@ int sp_instance_is_sat(sp_ctx* ctx, const sp_instance* inst, const uint64_t* var
   u256* outs[3] = {Az.p, Bz.p, Cz.p};
   for (int m = 0; m < 3; m++) dev::spmv(outs[m], I.num_cons, I.M[m].csr_ptr.p, I.M[m].csr_idx.p, I.M[m].csr_val.p, z.p, c.stream);
   DevBuf<u256> prod(I.num_cons);
-  dev::hadamard(prod.p, Az.p, Bz.p, I.num_cons, c.stream);
+  u256* prods[1] = {prod.p};
+  const u256 *as[1] = {Az.p}, *bs[1] = {Bz.p};
+  dev::hadamard_many(prods, as, bs, 1, I.num_cons, c.stream);
   std::vector<Fq> p = c.download(prod.p, I.num_cons), cz = c.download(Cz.p, I.num_cons);
   *sat = 1;
   for (size_t i = 0; i < I.num_cons; i++) if (!(p[i] == cz[i])) { *sat = 0; break; }   // r1cs.rs:265
@@ -773,15 +728,28 @@ int sp_nizk_gens_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t nu
 }
 void sp_nizk_gens_free(sp_nizk_gens* g) { delete g; }
 
-// the caller's transcript: either a fresh Transcript::new(label) (state == NULL) or the caller-owned STROBE state, updated in place
+// the caller's transcript: either a fresh Transcript::new(label) or (the _t entry points) the caller-owned STROBE state, updated in place
 struct TranscriptArg {
-  const uint8_t* label; size_t label_len; uint8_t* state;
-  Transcript open() const { return state ? Transcript(Transcript::FromState(), state) : Transcript(std::string((const char*)label, label_len)); }
-  void close(const Transcript& T) const { if (state) T.export_state(state); }
+  const uint8_t* label; size_t label_len; uint8_t* state; bool from_state;
+  static TranscriptArg fresh(const uint8_t* label, size_t label_len) { return {label, label_len, nullptr, false}; }
+  static TranscriptArg caller(uint8_t* state) { return {nullptr, 0, state, true}; }
+  void check() const { if (from_state && !state) throw SpError(SP_ERR_INVALID_ARG, "transcript state is NULL"); }
+  Transcript open() const { return from_state ? Transcript(Transcript::FromState(), state) : Transcript(std::string((const char*)label, label_len)); }
+  void close(const Transcript& T) const { if (from_state) T.export_state(state); }
 };
-static int nizk_prove_common(sp_ctx* ctx, const sp_instance* inst, const u256* d_vars, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens,
+// the witness of a prove call: the caller's host limbs, padded on upload (Assignment::pad), or a resident poly already padded to num_vars
+struct VarsArg { const uint64_t* host; size_t nvars; const sp_poly* resident; };
+static const u256* vars_on_device(Ctx& c, const Instance& I, const VarsArg& v, DevBuf<u256>& upload) {
+  if (!v.resident) { upload = upload_padded_vars(c, I, v.host, v.nvars); return upload.p; }
+  if (v.resident->len != I.num_vars) throw SpError(SP_ERR_INVALID_INPUTS, "resident vars must already be padded to num_vars");
+  return v.resident->d.p;
+}
+static int nizk_prove_common(sp_ctx* ctx, const sp_instance* inst, const VarsArg& vars, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens,
                              const TranscriptArg& ta, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
   SP_TRY(ctx)
+  ta.check();
+  DevBuf<u256> upload;
+  const u256* d_vars = vars_on_device(ctx->c, inst->inst, vars, upload);
   if (ninputs != inst->inst.num_inputs) throw SpError(SP_ERR_INVALID_INPUTS, "R1CSError::InvalidNumberOfInputs");
   if (!seed) throw SpError(SP_ERR_INVALID_ARG, "tape seed is NULL: draw it from the OS RNG (random.rs:13-15); a fixed seed makes every blind public");
   require_reduced(inputs, ninputs, "inputs"); require_reduced(seed, 1, "tape seed");
@@ -796,26 +764,16 @@ static int nizk_prove_common(sp_ctx* ctx, const sp_instance* inst, const u256* d
 }
 int sp_nizk_prove(sp_ctx* ctx, const sp_instance* inst, const uint64_t* vars, size_t nvars, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens,
                   const uint8_t* label, size_t label_len, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  DevBuf<u256> d_vars;
-  try { d_vars = upload_padded_vars(ctx->c, inst->inst, vars, nvars); }
-  catch (const SpError& e) { ctx->c.last_error = e.what(); return e.code; }
-  catch (const std::exception& e) { ctx->c.last_error = e.what(); return SP_ERR_CUDA; }
-  return nizk_prove_common(ctx, inst, d_vars.p, inputs, ninputs, gens, TranscriptArg{label, label_len, nullptr}, seed, proof, proof_len);
+  return nizk_prove_common(ctx, inst, {vars, nvars, nullptr}, inputs, ninputs, gens, TranscriptArg::fresh(label, label_len), seed, proof, proof_len);
 }
 // NIZK::prove(&inst, vars, &inputs, &gens, transcript: &mut Transcript) with the caller's transcript state in / out (lib.rs:501-508)
 int sp_nizk_prove_t(sp_ctx* ctx, const sp_instance* inst, const uint64_t* vars, size_t nvars, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens,
                     uint8_t* strobe_state, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  if (!strobe_state) { ctx->c.last_error = "transcript state is NULL"; return SP_ERR_INVALID_ARG; }
-  DevBuf<u256> d_vars;
-  try { d_vars = upload_padded_vars(ctx->c, inst->inst, vars, nvars); }
-  catch (const SpError& e) { ctx->c.last_error = e.what(); return e.code; }
-  catch (const std::exception& e) { ctx->c.last_error = e.what(); return SP_ERR_CUDA; }
-  return nizk_prove_common(ctx, inst, d_vars.p, inputs, ninputs, gens, TranscriptArg{nullptr, 0, strobe_state}, seed, proof, proof_len);
+  return nizk_prove_common(ctx, inst, {vars, nvars, nullptr}, inputs, ninputs, gens, TranscriptArg::caller(strobe_state), seed, proof, proof_len);
 }
 int sp_nizk_prove_resident(sp_ctx* ctx, const sp_instance* inst, const sp_poly* vars, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens,
                            const uint8_t* label, size_t label_len, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  if (vars->len != inst->inst.num_vars) { ctx->c.last_error = "resident vars must already be padded to num_vars"; return SP_ERR_INVALID_INPUTS; }
-  return nizk_prove_common(ctx, inst, vars->d.p, inputs, ninputs, gens, TranscriptArg{label, label_len, nullptr}, seed, proof, proof_len);
+  return nizk_prove_common(ctx, inst, {nullptr, 0, vars}, inputs, ninputs, gens, TranscriptArg::fresh(label, label_len), seed, proof, proof_len);
 }
 
 // ---- SNARK
@@ -862,9 +820,12 @@ int sp_snark_commitment_load(sp_ctx* ctx, const uint8_t* bytes, size_t len, sp_s
   *out = E.release();
   SP_CATCH(ctx)
 }
-static int snark_prove_common(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const u256* d_vars, const uint64_t* inputs, size_t ninputs,
+static int snark_prove_common(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const VarsArg& vars, const uint64_t* inputs, size_t ninputs,
                               const sp_snark_gens* gens, const TranscriptArg& ta, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
   SP_TRY(ctx)
+  ta.check();
+  DevBuf<u256> upload;
+  const u256* d_vars = vars_on_device(ctx->c, inst->inst, vars, upload);
   if (ninputs != inst->inst.num_inputs) throw SpError(SP_ERR_INVALID_INPUTS, "R1CSError::InvalidNumberOfInputs");
   if (!enc->e->comb_ops.p) throw SpError(SP_ERR_INVALID_ARG, "this handle holds a commitment only (sp_snark_commitment_load): proving needs sp_snark_encode");
   if (!seed) throw SpError(SP_ERR_INVALID_ARG, "tape seed is NULL: draw it from the OS RNG (random.rs:13-15); a fixed seed makes every blind public");
@@ -878,66 +839,56 @@ static int snark_prove_common(sp_ctx* ctx, const sp_instance* inst, const sp_sna
 }
 int sp_snark_prove(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const uint64_t* vars, size_t nvars, const uint64_t* inputs, size_t ninputs,
                    const sp_snark_gens* gens, const uint8_t* label, size_t label_len, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  DevBuf<u256> d_vars;
-  try { d_vars = upload_padded_vars(ctx->c, inst->inst, vars, nvars); }
-  catch (const SpError& e) { ctx->c.last_error = e.what(); return e.code; }
-  catch (const std::exception& e) { ctx->c.last_error = e.what(); return SP_ERR_CUDA; }
-  return snark_prove_common(ctx, inst, enc, d_vars.p, inputs, ninputs, gens, TranscriptArg{label, label_len, nullptr}, seed, proof, proof_len);
+  return snark_prove_common(ctx, inst, enc, {vars, nvars, nullptr}, inputs, ninputs, gens, TranscriptArg::fresh(label, label_len), seed, proof, proof_len);
 }
 // SNARK::prove(..., transcript: &mut Transcript) with the caller's transcript state in / out (lib.rs:339-347)
 int sp_snark_prove_t(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const uint64_t* vars, size_t nvars, const uint64_t* inputs, size_t ninputs,
                      const sp_snark_gens* gens, uint8_t* strobe_state, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  if (!strobe_state) { ctx->c.last_error = "transcript state is NULL"; return SP_ERR_INVALID_ARG; }
-  DevBuf<u256> d_vars;
-  try { d_vars = upload_padded_vars(ctx->c, inst->inst, vars, nvars); }
-  catch (const SpError& e) { ctx->c.last_error = e.what(); return e.code; }
-  catch (const std::exception& e) { ctx->c.last_error = e.what(); return SP_ERR_CUDA; }
-  return snark_prove_common(ctx, inst, enc, d_vars.p, inputs, ninputs, gens, TranscriptArg{nullptr, 0, strobe_state}, seed, proof, proof_len);
+  return snark_prove_common(ctx, inst, enc, {vars, nvars, nullptr}, inputs, ninputs, gens, TranscriptArg::caller(strobe_state), seed, proof, proof_len);
 }
 int sp_snark_prove_resident(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const sp_poly* vars, const uint64_t* inputs, size_t ninputs,
                             const sp_snark_gens* gens, const uint8_t* label, size_t label_len, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  if (vars->len != inst->inst.num_vars) { ctx->c.last_error = "resident vars must already be padded to num_vars"; return SP_ERR_INVALID_INPUTS; }
-  return snark_prove_common(ctx, inst, enc, vars->d.p, inputs, ninputs, gens, TranscriptArg{label, label_len, nullptr}, seed, proof, proof_len);
+  return snark_prove_common(ctx, inst, enc, {nullptr, 0, vars}, inputs, ninputs, gens, TranscriptArg::fresh(label, label_len), seed, proof, proof_len);
 }
 
-// ---- verifiers
-int sp_nizk_verify(sp_ctx* ctx, const sp_instance* inst, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens, const uint8_t* label, size_t label_len,
-                   const uint8_t* proof, size_t proof_len) {
+// ---- verifiers.  The _t forms verify on the caller's transcript state (lib.rs:423-429, :549-555), which is updated in place whether or not the
+// proof is accepted (a _t prove writes it back only on success).
+struct TranscriptClose { const TranscriptArg& ta; const Transcript& T; ~TranscriptClose() { ta.close(T); } };
+static int nizk_verify_common(sp_ctx* ctx, const sp_instance* inst, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens, const TranscriptArg& ta,
+                              const uint8_t* proof, size_t proof_len) {
   SP_TRY(ctx)
+  ta.check();
   require_reduced(inputs, ninputs, "inputs");
-  Transcript T(std::string((const char*)label, label_len));
+  Transcript T = ta.open();
+  TranscriptClose close{ta, T};
   nizk_verify(ctx->c, inst->inst, fq_vec(inputs, ninputs), *gens->g, T, proof, proof_len);
   SP_CATCH(ctx)
+}
+static int snark_verify_common(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t* inputs, size_t ninputs, const sp_snark_gens* gens,
+                               const TranscriptArg& ta, const uint8_t* proof, size_t proof_len) {
+  SP_TRY(ctx)
+  ta.check();
+  require_reduced(inputs, ninputs, "inputs");
+  Transcript T = ta.open();
+  TranscriptClose close{ta, T};
+  snark_verify(ctx->c, *comm->e, fq_vec(inputs, ninputs), *gens->g, T, proof, proof_len);
+  SP_CATCH(ctx)
+}
+int sp_nizk_verify(sp_ctx* ctx, const sp_instance* inst, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens, const uint8_t* label, size_t label_len,
+                   const uint8_t* proof, size_t proof_len) {
+  return nizk_verify_common(ctx, inst, inputs, ninputs, gens, TranscriptArg::fresh(label, label_len), proof, proof_len);
 }
 int sp_snark_verify(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t* inputs, size_t ninputs, const sp_snark_gens* gens, const uint8_t* label,
                     size_t label_len, const uint8_t* proof, size_t proof_len) {
-  SP_TRY(ctx)
-  require_reduced(inputs, ninputs, "inputs");
-  Transcript T(std::string((const char*)label, label_len));
-  snark_verify(ctx->c, *comm->e, fq_vec(inputs, ninputs), *gens->g, T, proof, proof_len);
-  SP_CATCH(ctx)
+  return snark_verify_common(ctx, comm, inputs, ninputs, gens, TranscriptArg::fresh(label, label_len), proof, proof_len);
 }
-
-// verify(..., transcript: &mut Transcript) on the caller's transcript state (lib.rs:423-429, :549-555); the state is updated in place either way
 int sp_nizk_verify_t(sp_ctx* ctx, const sp_instance* inst, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens, uint8_t* strobe_state,
                      const uint8_t* proof, size_t proof_len) {
-  SP_TRY(ctx)
-  if (!strobe_state) throw SpError(SP_ERR_INVALID_ARG, "transcript state is NULL");
-  require_reduced(inputs, ninputs, "inputs");
-  Transcript T(Transcript::FromState(), strobe_state);
-  struct Out { Transcript& T; uint8_t* s; ~Out() { T.export_state(s); } } out{T, strobe_state};
-  nizk_verify(ctx->c, inst->inst, fq_vec(inputs, ninputs), *gens->g, T, proof, proof_len);
-  SP_CATCH(ctx)
+  return nizk_verify_common(ctx, inst, inputs, ninputs, gens, TranscriptArg::caller(strobe_state), proof, proof_len);
 }
 int sp_snark_verify_t(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t* inputs, size_t ninputs, const sp_snark_gens* gens, uint8_t* strobe_state,
                       const uint8_t* proof, size_t proof_len) {
-  SP_TRY(ctx)
-  if (!strobe_state) throw SpError(SP_ERR_INVALID_ARG, "transcript state is NULL");
-  require_reduced(inputs, ninputs, "inputs");
-  Transcript T(Transcript::FromState(), strobe_state);
-  struct Out { Transcript& T; uint8_t* s; ~Out() { T.export_state(s); } } out{T, strobe_state};
-  snark_verify(ctx->c, *comm->e, fq_vec(inputs, ninputs), *gens->g, T, proof, proof_len);
-  SP_CATCH(ctx)
+  return snark_verify_common(ctx, comm, inputs, ninputs, gens, TranscriptArg::caller(strobe_state), proof, proof_len);
 }
 // merlin::Transcript for hosts without merlin (tests, C callers): the state buffer is the whole object
 int sp_transcript_new(const uint8_t* label, size_t label_len, uint8_t* strobe_state) {

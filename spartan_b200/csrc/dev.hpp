@@ -18,18 +18,14 @@ namespace dev {
 void check(const char* what);  // throws std::runtime_error on a pending CUDA error
 int device_count();
 void set_device(int dev);
-cudaStream_t stream_create();
 cudaStream_t stream_create_prio(int level);   // > 0: greatest priority of the device, < 0: least
 void stream_wait_event(cudaStream_t s, void* ev);
 void stream_destroy(cudaStream_t s);
 void stream_sync(cudaStream_t s);
-void* dmalloc(size_t bytes);
-void dfree(void* p);
 // size-bucketed caching allocator on top of cudaMalloc: a prove call allocates the same multi-hundred-MB buffers every time, and
 // cudaMalloc / cudaFree (which synchronises the device) would otherwise cost milliseconds per proof
 void* pool_alloc(size_t bytes);
 void pool_free(void* p);
-void pool_trim();   // return every cached block to the driver
 void* hmalloc_pinned(size_t bytes);
 void hfree_pinned(void* p);
 void h2d(void* d, const void* h, size_t bytes, cudaStream_t s);
@@ -91,7 +87,6 @@ struct XRank {
 
 // scratch: >= sc_scratch_bytes(); out: ninst*3 scalars [e0,e2,e3] (e3 = 0 for SC_QUAD), device memory
 size_t sc_scratch_bytes(int ninst);
-void dot_pairs(u256* out, const u256* const* a_list, const u256* const* b_list, int count, size_t n, void* scratch, cudaStream_t s, HostSig sig = HostSig());
 void heads(u256* out, const u256* const* tables, int count, cudaStream_t s, HostSig sig = HostSig());
 void sc_eval(ScKind kind, const ScInst* d_insts, int ninst, size_t len, u256* out, void* scratch, cudaStream_t s, HostSig sig = HostSig(), const XRank& xr = XRank());
 // fold every table of every instance by r (len -> len/2, in place) and evaluate the next round on the result; r travels as a kernel argument
@@ -103,11 +98,9 @@ void sc_eval_g(const ScInst* d_insts, int ninst, size_t len, const u256* E, u256
 void sc_fold_eval_g(const ScInst* d_insts, int ninst, size_t len, const u256& r, const u256* E, u256* out, void* scratch, cudaStream_t s, HostSig sig = HostSig(),
                     const XRank& xr = XRank());
 // levels[k-1] (k = 1..K, back to back, n0 >> k entries each) = eq(tau[k+1..], .) from E0 = eq(tau[1..], .) of n0 entries
-size_t eq_suffix_entries(size_t n0, int K);
 void eq_suffix(u256* levels, const u256* E0, size_t n0, int K, cudaStream_t s);
 // fold only (bound_poly_var_top, dense_mlpoly.rs:215-223): tables[k][i] += r*(tables[k][i+len/2]-tables[k][i])
 void fold_top(u256* const* d_tables, int ntables, size_t len, const u256& r, cudaStream_t s);
-void fold_top_single(u256* table, size_t len, const u256& r, cudaStream_t s);
 
 // ---- dense polynomial helpers (K7)
 void eq_evals(u256* out, const u256* d_r, int ell, u256* scratch_small /* >= 2*2^ceil(ell/2) */, cudaStream_t s);
@@ -116,22 +109,16 @@ void dot_many(u256* out, const u256* const* a_list, int count, const u256* b, si
 void dot3(u256* out, const u256* a, const u256* b, const u256* c, size_t n, void* scratch, cudaStream_t s);
 void bound_rows(u256* out, const u256* Z, const u256* L, size_t L_size, size_t R_size, u256* scratch /* >= 64*R_size */, cudaStream_t s);
 void lincomb3(u256* out, const u256* A, const u256* B, const u256* C, const u256* d_rabc /*3*/, size_t n, cudaStream_t s);
-void hadamard(u256* out, const u256* a, const u256* b, size_t n, cudaStream_t s);
 void hadamard_many(u256* const* outs, const u256* const* as, const u256* const* bs, int count, size_t n, cudaStream_t s);
 void from_u64(u256* out, const uint64_t* v, size_t n, cudaStream_t s);
-void from_bytes_wide(u256* out, const uint8_t* in64, size_t n, cudaStream_t s);
-void batch_invert_elems(u256* inout, size_t n, cudaStream_t s);
 void to_canonical(u256* out, const u256* in, size_t n, cudaStream_t s);   // Montgomery -> canonical little-endian integers (transcript bytes)
 void gather(u256* out, const u256* mem, const uint32_t* idx, size_t n, cudaStream_t s);
 // hash layer of the SPARK memory check: out = ts*r^2 + val*r + addr - g  (sparse_mlpoly.rs:545-600)
 // addr == null: addr = index i;  ts == null: ts = 0;  ts_plus_one adds one.   d_rg = [r_hash, r_multiset]
 void spark_hash(u256* out, size_t n, const u256* addr, const u256* val, const u256* ts, int ts_plus_one, const u256* d_rg, cudaStream_t s);
-// IPA vector folds (bullet.rs:105-107): a[i] = a[i]*u + uinv*a[i+n];  b[i] = b[i]*uinv + u*b[i+n]   d_u = [u, uinv]
-void ipa_fold_ab(u256* a, u256* b, size_t n, const u256& u, const u256& uinv, cudaStream_t s);
-// scalars for the L / R commitments against the UNFOLDED generators: see DESIGN.md "IPA without folding G"
-void ipa_lr_scalars(u256* outL, u256* outR, const u256* a, const u256* svec, size_t n_cur, size_t n_full, cudaStream_t s);
-void ipa_update_s(u256* svec, size_t n_cur_half, size_t n_full, const u256& u, const u256& uinv, cudaStream_t s);
-void ipa_fold_update(u256* a, u256* b, u256* svec, size_t n_cur_half, size_t n_full, const u256& u, const u256& uinv, cudaStream_t s);   // ipa_fold_ab + ipa_update_s in one launch
+// the folds of an inner-product round (bullet.rs:105-108) in one launch: a[i] = a[i]*u + uinv*a[i+half], b[i] = b[i]*uinv + u*b[i+half], and the
+// running scalars s[j] of the unfolded generators (DESIGN.md "IPA without folding G") times uinv (left half of their block) or u (right half)
+void ipa_fold_update(u256* a, u256* b, u256* svec, size_t n_cur_half, size_t n_full, const u256& u, const u256& uinv, cudaStream_t s);
 void fill_one(u256* out, size_t n, cudaStream_t s);
 
 // windows: IPC-exportable device allocations and their mappings in the peers
@@ -190,7 +177,7 @@ size_t ipa_msm_scratch_points(size_t n_full, int wbits);
 void ipa_msm(ge* out, const ge_niels* table, int wbits, const u256* a, const u256* svec, size_t n_cur, size_t n_full, void* scratch, unsigned int* ticket,
              cudaStream_t s, HostSig sig = HostSig(),
              // b != null: the same launch also computes c_out[0] = <a_L, b_R>, c_out[1] = <a_R, b_L> of the round and
-             // publishes them through sigc (its own flag word and completion counter), instead of a separate dot_pairs launch in front of the MSM
+             // publishes them through sigc (its own flag word and completion counter), long before the MSM finishes
              const u256* b = nullptr, u256* c_out = nullptr, HostSig sigc = HostSig());
 
 // ---- variable-base MSM on arbitrary points (bucket method; kernels_pip.cu).  pts: affine-niels form of the caller's points.

@@ -75,7 +75,6 @@ static void ck(cudaError_t e, const char* what) {
 }
 int device_count() { int n = 0; if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; } return n; }
 void set_device(int d) { ck(cudaSetDevice(d), "cudaSetDevice"); }
-cudaStream_t stream_create() { cudaStream_t s; ck(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking), "cudaStreamCreate"); return s; }
 // level > 0: the device's greatest priority (the transcript-serialised stream of small kernels), level < 0: its least (background MSMs)
 cudaStream_t stream_create_prio(int level) {
   int least = 0, greatest = 0;
@@ -87,8 +86,6 @@ cudaStream_t stream_create_prio(int level) {
 void stream_wait_event(cudaStream_t s, void* ev) { ck(cudaStreamWaitEvent(s, (cudaEvent_t)ev, 0), "cudaStreamWaitEvent"); }
 void stream_destroy(cudaStream_t s) { cudaStreamDestroy(s); }
 void stream_sync(cudaStream_t s) { ck(cudaStreamSynchronize(s), "cudaStreamSynchronize"); }
-void* dmalloc(size_t b) { void* p = nullptr; ck(cudaMalloc(&p, b ? b : 16), "cudaMalloc"); return p; }
-void dfree(void* p) { if (p) cudaFree(p); }
 namespace {
 std::mutex g_pool_mu;
 std::multimap<std::pair<int, size_t>, void*> g_pool_free;  // (device, rounded size) -> cached block
@@ -131,12 +128,6 @@ void pool_free(void* p) {
   if (it->second.second > ((size_t)8 << 30)) cudaFree(p);
   else g_pool_free.insert({it->second, p});
   g_pool_live.erase(it);
-}
-void pool_trim() {
-  std::lock_guard<std::mutex> lk(g_pool_mu);
-  cudaDeviceSynchronize();
-  for (auto& kv : g_pool_free) cudaFree(kv.second);
-  g_pool_free.clear();
 }
 void* hmalloc_pinned(size_t b) { void* p = nullptr; ck(cudaMallocHost(&p, b ? b : 16), "cudaMallocHost"); return p; }
 void hfree_pinned(void* p) { if (p) cudaFreeHost(p); }
@@ -245,28 +236,6 @@ void dot_many(u256* out, const u256* const* a_list, int count, const u256* b, si
   SP_LAUNCHED(); check("dot_many");
 }
 
-// out[k] = <a_k, b_k> for up to 8 independent pairs in one launch; the results can also be published to the host (HostSig)
-struct DotPairs { const u256* a[8]; const u256* b[8]; };
-__global__ void __launch_bounds__(256) k_dot_pairs(DotPairs dp, size_t n, u256* partials, unsigned int* counters, u256* out, HostSig sig) {
-  const u256* a = dp.a[blockIdx.y];
-  const u256* b = dp.b[blockIdx.y];
-  u256 acc[1] = {fq_zero()};
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    acc[0] = fq_add(acc[0], fq_mul(ld256_ro(a + i), ld256_ro(b + i)));
-  block_reduce_finish<1>(acc, partials, counters, out, 1, sig);
-}
-void dot_pairs(u256* out, const u256* const* a_list, const u256* const* b_list, int count, size_t n, void* scratch, cudaStream_t s, HostSig sig) {
-  ProfScope ps("dot", 64.0 * (double)n * count, s);
-  if (count > 8) throw std::runtime_error("spartan_b200: dot_pairs supports at most 8 pairs");
-  DotPairs dp;
-  for (int i = 0; i < count; i++) { dp.a[i] = a_list[i]; dp.b[i] = b_list[i]; }
-  unsigned int* counters = (unsigned int*)scratch;
-  u256* partials = (u256*)((char*)scratch + 256);
-  dim3 grid(grid_for(n, 256, 1), count);
-  k_dot_pairs<<<grid, 256, 0, s>>>(dp, n, partials, counters, out, sig);
-  SP_LAUNCHED(); check("dot_pairs");
-}
-
 // first elements of up to 64 tables -> one contiguous array (+ the host, through HostSig): the layer claims of the batched product proofs
 struct HeadBatch { const u256* p[64]; };
 __global__ void __launch_bounds__(64) k_heads(HeadBatch hb, int count, u256* out, HostSig sig) {
@@ -330,15 +299,6 @@ void lincomb3(u256* out, const u256* A, const u256* B, const u256* C, const u256
   k_lincomb3<<<grid_for(n, 256, 4), 256, 0, s>>>(out, A, B, C, d_rabc, n);
   SP_LAUNCHED(); check("lincomb3");
 }
-__global__ void k_hadamard(u256* out, const u256* a, const u256* b, size_t n) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    st256(out + i, fq_mul(ld256(a + i), ld256(b + i)));
-}
-void hadamard(u256* out, const u256* a, const u256* b, size_t n, cudaStream_t s) {
-  ProfScope ps("hadamard", 96.0 * (double)n, s);
-  k_hadamard<<<grid_for(n, 256, 8), 256, 0, s>>>(out, a, b, n);
-  SP_LAUNCHED(); check("hadamard");
-}
 // one product-tree layer of up to 16 circuits of equal size in one launch (blockIdx.y = circuit)
 struct HadBatch { u256* out[16]; const u256* a[16]; const u256* b[16]; };
 __global__ void k_hadamard_many(HadBatch hb, size_t n) {
@@ -362,29 +322,12 @@ void from_u64(u256* out, const uint64_t* v, size_t n, cudaStream_t s) {
   k_from_u64<<<grid_for(n, 256, 8), 256, 0, s>>>(out, v, n);
   SP_LAUNCHED(); check("from_u64");
 }
-__global__ void k_from_wide(u256* out, const uint8_t* __restrict__ in, size_t n) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const u256* p = reinterpret_cast<const u256*>(in + 64 * i);
-    st256(out + i, fq_from_wide(ld256_ro(p), ld256_ro(p + 1)));
-  }
-}
-void from_bytes_wide(u256* out, const uint8_t* in64, size_t n, cudaStream_t s) {
-  k_from_wide<<<grid_for(n, 256, 8), 256, 0, s>>>(out, in64, n);
-  SP_LAUNCHED(); check("from_bytes_wide");
-}
 __global__ void k_to_canonical(u256* out, const u256* __restrict__ in, size_t n) {   // Scalar::to_bytes (ristretto255.rs:419) for a whole vector
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) st256(out + i, fq_from_mont(ld256_ro(in + i)));
 }
 void to_canonical(u256* out, const u256* in, size_t n, cudaStream_t s) {
   k_to_canonical<<<grid_for(n, 128, 8), 128, 0, s>>>(out, in, n);
   SP_LAUNCHED(); check("to_canonical");
-}
-__global__ void k_invert(u256* x, size_t n) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) st256(x + i, fq_inv(ld256(x + i)));
-}
-void batch_invert_elems(u256* x, size_t n, cudaStream_t s) {
-  k_invert<<<grid_for(n, 128, 16), 128, 0, s>>>(x, n);
-  SP_LAUNCHED(); check("invert");
 }
 __global__ void k_gather(u256* out, const u256* __restrict__ mem, const uint32_t* __restrict__ idx, size_t n) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) st256(out + i, ld256_ro(mem + idx[i]));
@@ -419,39 +362,6 @@ void fill_one(u256* out, size_t n, cudaStream_t s) {
 }
 
 // ---- IPA helpers (nizk/bullet.rs:72-119)
-__global__ void k_ipa_fold_ab(u256* a, u256* b, size_t n, const u256 u, const u256 ui) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    u256 aL = ld256(a + i), aR = ld256(a + i + n), bL = ld256(b + i), bR = ld256(b + i + n);
-    st256(a + i, fq_add(fq_mul(aL, u), fq_mul(ui, aR)));   // bullet.rs:106
-    st256(b + i, fq_add(fq_mul(bL, ui), fq_mul(u, bR)));   // bullet.rs:107
-  }
-}
-void ipa_fold_ab(u256* a, u256* b, size_t n, const u256& u, const u256& uinv, cudaStream_t s) {
-  ProfScope ps("ipa_fold_ab", 192.0 * (double)n, s);
-  k_ipa_fold_ab<<<grid_for(n, 128, 8), 128, 0, s>>>(a, b, n, u, uinv);
-  SP_LAUNCHED(); check("ipa_fold_ab");
-}
-// G is never folded on the device: after k rounds G_k[i] = sum_{j = i mod n_k} s[j]*G[j], so the round's
-// L = <a_L, G_R> and R = <a_R, G_L> are full-length fixed-base MSMs with scalars a[.]*s[j] (zero on the other half).
-__global__ void k_ipa_lr(u256* outL, u256* outR, const u256* __restrict__ a, const u256* __restrict__ sv, size_t n_cur, size_t n_full) {
-  size_t half = n_cur >> 1;
-  for (size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x; j < n_full; j += (size_t)gridDim.x * blockDim.x) {
-    size_t ip = j & (n_cur - 1);
-    u256 sj = ld256_ro(sv + j);
-    if (ip >= half) { st256(outL + j, fq_mul(ld256_ro(a + ip - half), sj)); st256(outR + j, fq_zero()); }
-    else { st256(outL + j, fq_zero()); st256(outR + j, fq_mul(ld256_ro(a + ip + half), sj)); }
-  }
-}
-void ipa_lr_scalars(u256* outL, u256* outR, const u256* a, const u256* svec, size_t n_cur, size_t n_full, cudaStream_t s) {
-  k_ipa_lr<<<grid_for(n_full, 128, 8), 128, 0, s>>>(outL, outR, a, svec, n_cur, n_full);
-  SP_LAUNCHED(); check("ipa_lr");
-}
-__global__ void k_ipa_update_s(u256* sv, size_t half, size_t n_full, const u256 u, const u256 ui) {
-  for (size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x; j < n_full; j += (size_t)gridDim.x * blockDim.x) {
-    bool right = (j & (2 * half - 1)) >= half;
-    st256(sv + j, fq_mul(ld256(sv + j), right ? u : ui));   // G_L[i] <- u^-1 G_L[i] + u G_R[i], bullet.rs:108
-  }
-}
 // both updates of an inner-product round in one launch: rows of blocks y = 0: s[j] *= u^(+-1); y = 1: fold a; y = 2: fold b (one or two products per thread)
 __global__ void k_ipa_fold_update(u256* a, u256* b, u256* sv, size_t half, size_t n_full, const u256 u, const u256 ui) {
   const size_t t0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
@@ -471,10 +381,6 @@ void ipa_fold_update(u256* a, u256* b, u256* svec, size_t half, size_t n_full, c
   dim3 grid(grid_for(n_full, 128, 8), 3);
   k_ipa_fold_update<<<grid, 128, 0, s>>>(a, b, svec, half, n_full, u, uinv);
   SP_LAUNCHED(); check("ipa_fold_update");
-}
-void ipa_update_s(u256* svec, size_t half, size_t n_full, const u256& u, const u256& uinv, cudaStream_t s) {
-  k_ipa_update_s<<<grid_for(n_full, 128, 8), 128, 0, s>>>(svec, half, n_full, u, uinv);
-  SP_LAUNCHED(); check("ipa_update_s");
 }
 
 // ---- sparse
@@ -702,7 +608,8 @@ void sum_points(ge* out, const ge* in, int n, cudaStream_t s) {
   k_msm_reduce_small<<<1, 32, 0, s>>>(out, in, n);
   SP_LAUNCHED(); check("sum_points");
 }
-// ---- the two MSMs of one inner-product round in a single launch (bullet.rs:83-97 with unfolded generators, see k_ipa_lr):
+// ---- the two MSMs of one inner-product round in a single launch (bullet.rs:83-97 with unfolded generators).  G is never folded on the device:
+// after k rounds G_k[i] = sum_{j = i mod n_k} s[j]*G[j], so the round's L = <a_L, G_R> and R = <a_R, G_L> are full-length fixed-base MSMs in which
 // every generator j carries exactly one non-zero scalar, a[.]*s[j], for L (j in the right half of its n_cur-block) or for R (left half).
 // Quad-lane formulation: grid = (chunks, 2 sides), IPAQ_THREADS
 // threads = IPAQ_THREADS/4 quads; a quad owns WPQ adjacent windows of one scalar and chains their table entries by mixed additions (two product

@@ -339,7 +339,7 @@ void sc_fold_eval_g(const ScInst* insts, int ninst, size_t len, const u256& r, c
   k_sc_fold_eval_g<<<grid, 256, 0, s>>>(b, len, rc, E, partials, counters, out, sig, xr);
   SP_LAUNCHED(); check("sc_fold_eval_g");
 }
-size_t eq_suffix_entries(size_t n0, int K) { size_t t = 0; for (int k = 1; k <= K; k++) t += n0 >> k; return t; }
+static size_t eq_suffix_entries(size_t n0, int K) { size_t t = 0; for (int k = 1; k <= K; k++) t += n0 >> k; return t; }
 void eq_suffix(u256* levels, const u256* E0, size_t n0, int K, cudaStream_t s) {
   if (K < 1) return;
   ProfScope ps("eq_evals", 64.0 * (double)n0, s);
@@ -358,7 +358,6 @@ void fold_top(u256* const* tables, int ntables, size_t len, const u256& r, cudaS
   }
   check("fold_top");
 }
-void fold_top_single(u256* table, size_t len, const u256& r, cudaStream_t s) { u256* t[1] = {table}; fold_top(t, 1, len, r, s); }
 
 }  // namespace dev
 }  // namespace sp

@@ -504,21 +504,14 @@ Cp commit_rows_and_compress(Ctx& ctx, const CommitKey& key, const u256* d_scalar
   if (key.off != 0 || R > key.n) throw std::runtime_error("spartan_b200: commit_rows key mismatch");
   const bool blind_on_host = !blinds || blinds[0].is_zero() || key.set->host_tab.count(key.h) != 0;   // the blind term needs the host copy of h's table
   if (L == 1 && R >= 2 && R % 2 == 0 && !blinds_late && ctx.shard_world() == 1 && blind_on_host) {
-    // one row (the Cx commitment of DotProductProofLog, nizk/mod.rs:466): a latency problem.  The inner-product round kernel with a = (1, 1) and
-    // blocks of two generators returns sum_{j odd} x_j G_j and sum_{j even} x_j G_j straight to the host; the blind term, the two additions and the
-    // encoding happen there instead of in a 265-product chain on one GPU thread, and the msm_rows + reduce + k_compress + copy sequence is avoided
+    // one row (the Cx commitment of DotProductProofLog, nizk/mod.rs:466): a latency problem.  The row's sum reaches the host, which adds the
+    // blind term and encodes, instead of a 265-product chain on one GPU thread; the blind term is computed while the kernel runs
     ctx.ensure_scratch(std::max(dev::msm_scratch_bytes(1, R), dev::ipa_msm_scratch_points(R, key.set->wbits) * sizeof(ge)) + 64);
-    dev::HostSig sg = ctx.next_sig();
-    sg.host_out = ctx.host_res + 8;
-    DevBuf<ge> pts(2);   // the kernel's device-side copy of the two sums (the host reads its own copy); released after the wait below
-    dev::ipa_msm(pts.p, key.set->table.p, key.set->wbits, ctx.ones(), d_scalars, 2, R, ctx.scratch.p, ctx.sig_done.p + 1, ctx.stream, sg);
+    RowSum row(ctx, *key.set, d_scalars, R);
     hge acc = hge_identity();
     if (blinds && !blinds[0].is_zero()) { Term t[1] = {{key.h, blinds[0]}}; acc = host_commit(*key.set, t, 1); }
-    ctx.wait_sig(sg);
-    ge odd, even;
-    memcpy(&odd, ctx.host_res + 8, sizeof(ge)); memcpy(&even, ctx.host_res + 12, sizeof(ge));
     out.resize(1);
-    out[0] = compress(hge_add(hge_add(to_hge(odd), to_hge(even)), acc));
+    out[0] = compress(hge_add(row.collect(), acc));
     return out[0];
   }
   ctx.ensure_scratch(dev::msm_scratch_bytes(L, R) + 64);
@@ -552,8 +545,47 @@ void append_poly_commitment(Transcript& T, const char* label, const PolyCommitme
   T.append_message(label, "poly_commitment_end");
 }
 
+void IpaRound::launch(size_t cur) {
+  // the dot products ride in the MSM's launch (two extra blocks with their own flag word, host_flag + 16, and completion counter)
+  sig_c.host_out = ctx.host_res; sig_c.flag = ctx.host_flag + 16; sig_c.done = ctx.sig_done.p + 2; sig_c.seq = ++ctx.sigc_seq;
+  sig_lr = ctx.next_sig();
+  sig_lr.host_out = ctx.host_res + 8;
+  dev::ipa_msm(pts, gs.table.p, gs.wbits, a, svec, cur, n, ctx.scratch.p, ctx.sig_done.p + 1, ctx.stream, sig_lr, b, ctx.small.p + 16, sig_c);
+}
+void IpaRound::wait_c(Fq& c_L, Fq& c_R) {
+  ctx.wait_sig(sig_c);
+  memcpy(&c_L, ctx.host_res, 32); memcpy(&c_R, ctx.host_res + 1, 32);
+}
+void IpaRound::wait_LR(ge& L, ge& R) {
+  ctx.wait_sig(sig_lr);
+  memcpy(&L, ctx.host_res + 8, sizeof(ge)); memcpy(&R, ctx.host_res + 12, sizeof(ge));
+}
+void IpaRound::fold(size_t cur, const Fq& u, const Fq& u_inv) { dev::ipa_fold_update(a, b, svec, cur / 2, n, u.m, u_inv.m, ctx.stream); }
+
+RowSum::RowSum(Ctx& c, const GenSet& gs, const u256* d_x, size_t n_) : ctx(c), n(n_), pts(2) {
+  if (n >= 2) {
+    sig = ctx.next_sig();
+    sig.host_out = ctx.host_res + 8;
+    dev::ipa_msm(pts.p, gs.table.p, gs.wbits, ctx.ones(), d_x, 2, n, ctx.scratch.p, ctx.sig_done.p + 1, ctx.stream, sig);
+  } else {
+    dev::msm_rows(pts.p, gs.table.p, gs.wbits, gs.rows(), d_x, n, 1, n, nullptr, 0, ctx.scratch.p, ctx.stream);
+    dev::d2h(ctx.host_res + 8, pts.p, sizeof(ge), ctx.stream);
+  }
+}
+hge RowSum::collect() {
+  ge p[2];
+  if (n < 2) {
+    ctx.sync();
+    memcpy(&p[0], ctx.host_res + 8, sizeof(ge));
+    return to_hge(p[0]);
+  }
+  ctx.wait_sig(sig);
+  memcpy(p, ctx.host_res + 8, 2 * sizeof(ge));
+  return hge_add(to_hge(p[0]), to_hge(p[1]));
+}
+
 // BulletReductionProof::prove (nizk/bullet.rs:32-132) with Q = r*G1 and H = h folded into host fixed-base terms, and the
-// generator vector left unfolded (see k_ipa_lr in kernels.cu).  d_a / d_b are consumed (folded in place).
+// generator vector left unfolded (DESIGN.md "IPA without folding G").  d_a / d_b are consumed (folded in place).
 static void bullet_prove(Ctx& ctx, Transcript& T, const PolyCommitmentGens& gens, const std::function<Fq()>& get_r_scale, u256* d_a, u256* d_b, size_t n,
                          const Fq& blind, const std::vector<std::pair<Fq, Fq>>& blinds_vec, BulletReductionProof& proof, Fq& a_hat, Fq& b_hat, hge& g_hat,
                          Fq& blind_final) {
@@ -572,29 +604,21 @@ static void bullet_prove(Ctx& ctx, Transcript& T, const PolyCommitmentGens& gens
     dev::msm_rows(d_bh.p, gs.table.p, gs.wbits, gs.rows(), lr.p, 0, 2 * rounds, 0, d_bl.p, gens.gens_n.h, ctx.scratch.p, ctx.stream);
     dev::d2h(bh.data(), d_bh.p, bh.size() * sizeof(ge), ctx.stream);   // pageable target: completes before the call returns
   }
-  u256* d_c = ctx.small.p + 16;  // c_L, c_R
+  IpaRound rd{ctx, gs, d_a, d_b, svec.p, n, pts.p};
   blind_final = blind;
   Fq r_scale = Fq::zero();
   size_t cur = n, k = 0;
   while (cur != 1) {
-    size_t half = cur / 2;
     FineTimer f1(ctx, "ipa launch");
-    // c_L = <a_L, b_R>, c_R = <a_R, b_L> (bullet.rs:78-79) and L = <a_L, G_R>, R = <a_R, G_L> over the unfolded generators (scalars a[.]*s[j] formed
-    // inside the kernel), all published to the host.  The dot products ride in the MSM's launch (two extra blocks with their own flag word).
-    dev::HostSig sig, sig2;
-    sig.host_out = ctx.host_res; sig.flag = ctx.host_flag + 16; sig.done = ctx.sig_done.p + 2; sig.seq = ++ctx.sigc_seq;
-    sig2 = ctx.next_sig();
-    sig2.host_out = ctx.host_res + 8;
-    dev::ipa_msm(pts.p, gs.table.p, gs.wbits, d_a, svec.p, cur, n, ctx.scratch.p, ctx.sig_done.p + 1, ctx.stream, sig2, d_b, d_c, sig);
+    rd.launch(cur);
     f1.stop();
     // the transcript work that precedes the first round (absorbing a_vec, deriving r) runs while the device computes round 0
     if (k == 0) r_scale = get_r_scale();
     FineTimer f2(ctx, "ipa wait c");
-    ctx.wait_sig(sig);
+    Fq c_L, c_R;
+    rd.wait_c(c_L, c_R);
     f2.stop();
     FineTimer f3(ctx, "ipa host c*Q (overlaps MSM)");
-    Fq c_L, c_R;
-    memcpy(&c_L, ctx.host_res, 32); memcpy(&c_R, ctx.host_res + 1, 32);
     // + c_L*Q + blind_L*H with Q = r*G1 (nizk/mod.rs:479-480), H = gens_n.h   (bullet.rs:83-97)
     Term tl[1] = {{gens.gens_1.off, c_L * r_scale}};
     Term tr[1] = {{gens.gens_1.off, c_R * r_scale}};
@@ -602,11 +626,10 @@ static void bullet_prove(Ctx& ctx, Transcript& T, const PolyCommitmentGens& gens
     hge hr = hge_add(host_commit(gs, tr, 1), to_hge(bh[2 * k + 1]));
     f3.stop();
     FineTimer f4(ctx, "ipa wait MSM");
-    ctx.wait_sig(sig2);
+    ge Lg, Rg;
+    rd.wait_LR(Lg, Rg);
     f4.stop();
     FineTimer f5(ctx, "ipa host compress+transcript");
-    ge Lg, Rg;
-    memcpy(&Lg, ctx.host_res + 8, sizeof(ge)); memcpy(&Rg, ctx.host_res + 12, sizeof(ge));
     Cp Lc, Rc;
     compress2(hge_add(to_hge(Lg), hl), hge_add(to_hge(Rg), hr), Lc, Rc);
     T.append_point("L", Lc.b);
@@ -614,11 +637,11 @@ static void bullet_prove(Ctx& ctx, Transcript& T, const PolyCommitmentGens& gens
     Fq u = T.challenge_scalar("u");
     Fq u_inv = u.inv();
     f5.stop();
-    dev::ipa_fold_update(d_a, d_b, svec.p, half, n, u.m, u_inv.m, ctx.stream);
+    rd.fold(cur, u, u_inv);
     blind_final = blind_final + blinds_vec[k].first * u * u + blinds_vec[k].second * u_inv * u_inv;  // bullet.rs:111
     proof.L_vec.push_back(Lc);
     proof.R_vec.push_back(Rc);
-    cur = half;
+    cur /= 2;
     k++;
   }
   if (k == 0) r_scale = get_r_scale();
@@ -626,24 +649,8 @@ static void bullet_prove(Ctx& ctx, Transcript& T, const PolyCommitmentGens& gens
   FineTimer f6(ctx, "ipa final");
   dev::d2h(ctx.pinned, d_a, 32, ctx.stream);
   dev::d2h(ctx.pinned + 32, d_b, 32, ctx.stream);
-  if (n >= 2) {
-    // the round kernel with a = (1, 1) and blocks of two generators: "L" = sum over the odd j of s[j] G_j, "R" = over the even j; both reach the host
-    // through the kernel's own publication and are added there (one launch instead of msm_rows + reduce + copy)
-    dev::HostSig sg = ctx.next_sig();
-    sg.host_out = ctx.host_res + 8;
-    dev::ipa_msm(pts.p, gs.table.p, gs.wbits, ctx.ones(), svec.p, 2, n, ctx.scratch.p, ctx.sig_done.p + 1, ctx.stream, sg);
-    ctx.sync();
-    ge odd, even;
-    memcpy(&odd, ctx.host_res + 8, sizeof(ge)); memcpy(&even, ctx.host_res + 12, sizeof(ge));
-    g_hat = hge_add(to_hge(odd), to_hge(even));
-  } else {
-    dev::msm_rows(pts.p, gs.table.p, gs.wbits, gs.rows(), svec.p, n, 1, n, nullptr, 0, ctx.scratch.p, ctx.stream);
-    dev::d2h(ctx.pinned + 64, pts.p, sizeof(ge), ctx.stream);
-    ctx.sync();
-    ge g;
-    memcpy(&g, ctx.pinned + 64, sizeof(ge));
-    g_hat = to_hge(g);
-  }
+  g_hat = RowSum(ctx, gs, svec.p, n).collect();
+  ctx.sync();   // a_hat, b_hat
   memcpy(&a_hat, ctx.pinned, 32); memcpy(&b_hat, ctx.pinned + 32, 32);
 }
 

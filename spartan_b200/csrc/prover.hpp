@@ -171,6 +171,37 @@ void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt
 // exposed pieces (C-ABI operator level and tests)
 Cp commit_rows_and_compress(Ctx& ctx, const CommitKey& key, const u256* d_scalars, size_t stride, size_t L, size_t R, const Fq* blinds,
                             std::vector<Cp>& out, const std::function<const Fq*()>& blinds_late = nullptr);
+
+// The device side of one inner-product round (bullet.rs:74-111) over the unfolded generators of `gs` (DESIGN.md "IPA without folding G"), run by
+// bullet_prove and by the operator-level sp_ipa_*.  launch() computes c_L = <a_L, b_R>, c_R = <a_R, b_L> and L' = <a_L, G_R>, R' = <a_R, G_L> in one
+// kernel that publishes the two pairs to the host through separate flag words, so the host can work on c*Q while the MSM still runs.
+// Scratch: >= ipa_msm_scratch_points(n, gs.wbits) points.
+struct IpaRound {
+  Ctx& ctx;
+  const GenSet& gs;
+  u256* a; u256* b;    // the current a, b (folded in place)
+  u256* svec;          // the n running scalars of the unfolded generators
+  size_t n;
+  ge* pts;             // device copy of L', R'
+  dev::HostSig sig_c, sig_lr;
+  void launch(size_t cur);
+  void wait_c(Fq& c_L, Fq& c_R);
+  void wait_LR(ge& L, ge& R);
+  void fold(size_t cur, const Fq& u, const Fq& u_inv);   // a, b, svec of the next round (bullet.rs:105-108)
+};
+
+// <x, G[0..n)> of one row of n scalars against the per-window table of `gs`, for latency.  For n >= 2 (even) it is the inner-product round kernel
+// with a = (1, 1) and blocks of two generators: its "L" (odd j) and "R" (even j) reach the host through the kernel's own publication and are added
+// there, one launch instead of msm_rows + reduce + compress + copy.  n = 1 runs msm_rows.  The constructor launches, collect() waits.
+// Scratch: >= ipa_msm_scratch_points(n, gs.wbits) points, or msm_scratch_bytes(1, 1) bytes for n = 1.
+struct RowSum {
+  Ctx& ctx;
+  size_t n;
+  DevBuf<ge> pts;
+  dev::HostSig sig;
+  RowSum(Ctx& ctx, const GenSet& gs, const u256* d_x, size_t n);
+  hge collect();
+};
 std::vector<Fq> host_eq_evals(const std::vector<Fq>& r);
 
 }  // namespace sp

@@ -202,7 +202,8 @@ def test_sumcheck_batched(sb, logn):
 @pytest.mark.parametrize("n", [2, 32, 1024, 4096])
 def test_bullet_reduction_operator_level(sb, n):
     """BulletReductionProof::prove (nizk/bullet.rs:32-132) driven from the host through sp_ipa_begin / sp_ipa_round_LR / sp_ipa_fold /
-    sp_ipa_finish with the oracle's transcript: every L, R, the final a, b and G[0] equal the oracle's.  n >= 512 runs the 13-bit-window
+    sp_ipa_finish with the oracle's transcript: every L, R, the final a, b and G[0] equal the oracle's.  The rounds run the prover's own launches
+    (IpaRound: k_ipa_msm_quad with its fused dot products, then k_ipa_fold_update; RowSum for G[0]).  n >= 512 runs the 13-bit-window
     instance of k_ipa_msm_quad (the generator set of the 2^20 proofs), n = 32 the 8-bit one."""
     from spartan_b200 import api
     from oracle.spartan_ref import protocol as pr
