@@ -89,9 +89,11 @@ struct XRank {
 size_t sc_scratch_bytes(int ninst);
 void heads(u256* out, const u256* const* tables, int count, cudaStream_t s, HostSig sig = HostSig());
 void sc_eval(ScKind kind, const ScInst* d_insts, int ninst, size_t len, u256* out, void* scratch, cudaStream_t s, HostSig sig = HostSig(), const XRank& xr = XRank());
-// fold every table of every instance by r (len -> len/2, in place) and evaluate the next round on the result; r travels as a kernel argument
+// fold every table of every instance by r (len -> len/2, in place) and evaluate the next round on the result; r travels as a kernel argument.
+// host_bound (len == 4, signalled launch): the bound two-entry tables also go to the host, host_bound[i * 2 NT + 2 t + h] = entry h of table t of
+// instance i (NT = 2, 3 or 4 tables per instance), published with the evaluations
 void sc_fold_eval(ScKind kind, const ScInst* d_insts, int ninst, size_t len, const u256& r, u256* out, void* scratch, cudaStream_t s,
-                  HostSig sig = HostSig(), const XRank& xr = XRank());
+                  HostSig sig = HostSig(), const XRank& xr = XRank(), u256* host_bound = nullptr);
 // ---- eq-factored streaming rounds of a batched A*B*eq sumcheck (kernels_sc.cu: k_sc_eval_g): instances use t[0] = A, t[1] = B; E: the suffix eq table
 // of the round (len/2 entries for sc_eval_g, len/4 for sc_fold_eval_g); out[3*i + 0] = q(0), out[3*i + 1] = q(inf) of instance i
 void sc_eval_g(const ScInst* d_insts, int ninst, size_t len, const u256* E, u256* out, void* scratch, cudaStream_t s, HostSig sig = HostSig(), const XRank& xr = XRank());
@@ -104,6 +106,8 @@ void fold_top(u256* const* d_tables, int ntables, size_t len, const u256& r, cud
 
 // ---- dense polynomial helpers (K7)
 void eq_evals(u256* out, const u256* d_r, int ell, u256* scratch_small /* >= 2*2^ceil(ell/2) */, cudaStream_t s);
+// out[n .. 2n) holds E = eq(r', .); rewrite out[0 .. 2n) as eq((r, r'), .) = [(1 - r) E | r E] in one pass
+void eq_extend_top(u256* out, size_t n, const u256& r, cudaStream_t s);
 void dot(u256* out, const u256* a, const u256* b, size_t n, void* scratch, cudaStream_t s);
 void dot_many(u256* out, const u256* const* a_list, int count, const u256* b, size_t n, void* scratch, cudaStream_t s);
 void dot3(u256* out, const u256* a, const u256* b, const u256* c, size_t n, void* scratch, cudaStream_t s);

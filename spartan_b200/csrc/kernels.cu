@@ -194,6 +194,18 @@ void eq_evals(u256* out, const u256* d_r, int ell, u256* small, cudaStream_t s) 
   k_eq_combine<<<grid_for(n, 256, 8), 256, 0, s>>>(out, thi, tlo, nlo, n);
   SP_LAUNCHED(); SP_LAUNCHED(); SP_LAUNCHED(); check("eq_evals");
 }
+__global__ void k_eq_extend_top(u256* out, size_t n, const u256 r) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const u256 e = ld256(out + n + i), hi = fq_mul(e, r);
+    st256(out + i, fq_sub(e, hi));   // (1 - r) e as e - r e: the same canonical residue
+    st256(out + n + i, hi);
+  }
+}
+void eq_extend_top(u256* out, size_t n, const u256& r, cudaStream_t s) {
+  ProfScope ps("eq_evals", 96.0 * (double)n, s);
+  k_eq_extend_top<<<grid_for(n, 256, 8), 256, 0, s>>>(out, n, r);
+  SP_LAUNCHED(); check("eq_extend_top");
+}
 
 __global__ void __launch_bounds__(256) k_dot(const u256* __restrict__ a, const u256* __restrict__ b, const u256* __restrict__ c, size_t n,
                                             u256* partials, unsigned int* counters, u256* out) {

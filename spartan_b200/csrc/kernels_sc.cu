@@ -155,9 +155,11 @@ __global__ void __launch_bounds__(256) k_eq_suffix(u256* levels, const u256* __r
 // values through shared memory, instead of one thread running all 14 multiplications back to back.  Same arithmetic, same results.
 #define SC_SMALL_Q 64
 #define SC_SMALL_MAX 1024
+// host_bound (len == 4 only): the bound two-entry tables also go to the host, host_bound[inst * 2 NT + 2 t + h] = table t's entry h, ordered before
+// the flag like the evaluations, so the host can bind the last variable itself and skip a fold and a gather launch and their round trip.
 template <int KIND>
 __global__ void __launch_bounds__(SC_SMALL_Q * 8) k_sc_fold_eval_small(ScBatch batch, size_t len, const __grid_constant__ FqConst rc, u256* partials,
-                                                                     unsigned int* counters, u256* out, HostSig sig) {
+                                                                     unsigned int* counters, u256* out, HostSig sig, u256* host_bound) {
   constexpr int NT = KIND == SC_QUAD ? 2 : (KIND == SC_CUBIC3 ? 3 : 4);
   constexpr int NP = KIND == SC_QUAD ? 2 : 3;   // evaluation points 0, 2 (, 3)
   __shared__ u256 sh[NT][2][SC_SMALL_Q];
@@ -173,6 +175,7 @@ __global__ void __launch_bounds__(SC_SMALL_Q * 8) k_sc_fold_eval_small(ScBatch b
     u256 v = fq_fold_const(x0, x1, rc);   // dense_mlpoly.rs:218
     if (t == 2) { if (in.write_c) st256(in.c_out + idx, v); }
     else st256(in.t[t] + idx, v);
+    if (host_bound) st256(&host_bound[(size_t)blockIdx.y * 2 * NT + 2 * t + h], v);
     sh[t][h][e] = v;
   }
   __syncthreads();
@@ -288,8 +291,10 @@ void sc_eval(ScKind kind, const ScInst* insts, int ninst, size_t len, u256* out,
   }
   SP_LAUNCHED(); check("sc_eval");
 }
-void sc_fold_eval(ScKind kind, const ScInst* insts, int ninst, size_t len, const u256& r, u256* out, void* scratch, cudaStream_t s, HostSig sig, const XRank& xr) {
+void sc_fold_eval(ScKind kind, const ScInst* insts, int ninst, size_t len, const u256& r, u256* out, void* scratch, cudaStream_t s, HostSig sig, const XRank& xr,
+                  u256* host_bound) {
   if (xr.world > 1 && (len / 4 <= SC_SMALL_MAX || !sig.done)) throw std::runtime_error("spartan_b200: a sharded sumcheck round needs a streaming-size table and a completion counter");
+  if (host_bound && (len != 4 || !sig.flag)) throw std::runtime_error("spartan_b200: only a signalled fold to two-entry tables publishes them");
   // two kernels, two profiler families: the streaming kernel (HBM roofline) and the latency-bound small-table kernel (k_sc_fold_eval_small)
   const bool small = len / 4 <= SC_SMALL_MAX && len >= 4;
   ProfScope ps(small ? "sc_fold_eval_small" : "sc_fold_eval", sc_bytes(insts, ninst, kind, len, 48.0), s);
@@ -300,9 +305,9 @@ void sc_fold_eval(ScKind kind, const ScInst* insts, int ninst, size_t len, const
   if (small) {
     dim3 grid((unsigned)((len / 4 + SC_SMALL_Q - 1) / SC_SMALL_Q), ninst);
     switch (kind) {
-      case SC_QUAD: k_sc_fold_eval_small<SC_QUAD><<<grid, SC_SMALL_Q * 4, 0, s>>>(b, len, rc, partials, counters, out, sig); break;
-      case SC_CUBIC3: k_sc_fold_eval_small<SC_CUBIC3><<<grid, SC_SMALL_Q * 6, 0, s>>>(b, len, rc, partials, counters, out, sig); break;
-      default: k_sc_fold_eval_small<SC_CUBIC4><<<grid, SC_SMALL_Q * 8, 0, s>>>(b, len, rc, partials, counters, out, sig); break;
+      case SC_QUAD: k_sc_fold_eval_small<SC_QUAD><<<grid, SC_SMALL_Q * 4, 0, s>>>(b, len, rc, partials, counters, out, sig, host_bound); break;
+      case SC_CUBIC3: k_sc_fold_eval_small<SC_CUBIC3><<<grid, SC_SMALL_Q * 6, 0, s>>>(b, len, rc, partials, counters, out, sig, host_bound); break;
+      default: k_sc_fold_eval_small<SC_CUBIC4><<<grid, SC_SMALL_Q * 8, 0, s>>>(b, len, rc, partials, counters, out, sig, host_bound); break;
     }
     SP_LAUNCHED(); check("sc_fold_eval_small");
     return;

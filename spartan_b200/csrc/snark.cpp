@@ -4,6 +4,7 @@
 #include "snark.hpp"
 #include <cstdlib>
 #include <algorithm>
+#include <optional>
 #include "../../include/spartan_b200.h"
 
 namespace sp {
@@ -182,42 +183,65 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
   const size_t G_MIN = 2 * Ctx::SHARD_MIN_LOCAL;   // 16384 entries per table: the fused G kernel then always streams >= 32768
   u256* d_out = ctx.small.p + 64;   // ninst * 3 scalars
   DevBuf<u256> d_heads(64);
-  for (size_t layer_id = num_layers; layer_id-- > 0;) {
-    const size_t len = prods[0]->layer_len(layer_id);  // left + right
-    const size_t half = len / 2;                       // table length of this layer's sumcheck (global)
-    const size_t num_rounds = log2_ceil(half);
-    bool sh = prods[0]->sharded(layer_id);             // this layer's tables are cyclic shards: the first rounds run sharded
-    const size_t lhalf = sh ? half / W : half;         // ... of this many entries per rank
-    // poly_C_par = eq(rand)                                                  (product_tree.rs:279-280)
-    if (!rand.empty()) dev::h2d(d_rand.p, rand.data(), rand.size() * sizeof(u256), ctx.stream);
-    int logW = 0;
-    if (sh) while ((1 << logW) < W) logW++;
-    const Fq c_rank = sh ? shard_eq_scale(rand, W, rk) : Fq::one();   // factor of eq(rand, .) that this rank's low index bits fix (cyclic shards)
-    // eq-factored streaming rounds (kernels_sc.cu: k_sc_eval_g): rounds 0 .. jG-1, i.e. those whose evaluation streams >= G_MIN entries per table;
-    // the suffix tables E_j = eq(rand[j+1..], .) live in cpar0 (E_0, then the levels 1 .. jG-1); from round jG on the standard kernels run on
-    // C = prefix * eq(rand[jG..], .), built at the switch.  Not applicable: the standard method from round 0.
+  int logW = 0;
+  while ((1 << logW) < W) logW++;
+  // a layer's sumcheck runs on tables of half = len/2 entries (num_rounds variables), lhalf of them on this rank while the layer is sharded
+  struct Shape { size_t half, num_rounds, lhalf; bool sh; int logW; };
+  auto shape_of = [&](size_t layer_id) {
+    Shape s;
+    s.half = prods[0]->layer_len(layer_id) / 2;
+    s.num_rounds = log2_ceil(s.half);
+    s.sh = prods[0]->sharded(layer_id);
+    s.lhalf = s.sh ? s.half / W : s.half;
+    s.logW = s.sh ? logW : 0;
+    return s;
+  };
+  // eq-factored streaming rounds (kernels_sc.cu: k_sc_eval_g): rounds 0 .. jG-1, i.e. those whose evaluation streams >= G_MIN entries per table,
+  // when no tau_j of them is zero (q(1) is recovered by a division by tau_j); rand[0] = r_layer is checked when the layer starts
+  auto plan_jG = [&](const Shape& s, const Fq* rand_tail /* rand[1..] */) {
     size_t jG = 0;
-    if (num_rounds >= 2) {
-      while (jG + 1 < num_rounds && (lhalf >> jG) >= G_MIN) jG++;
-      for (size_t j = 0; j < jG; j++) if (rand[j].is_zero()) jG = 0;   // q(1) is recovered by a division by tau_j
+    if (s.num_rounds >= 2) {
+      while (jG + 1 < s.num_rounds && (s.lhalf >> jG) >= G_MIN) jG++;
+      for (size_t j = 1; j < jG; j++) if (rand_tail[j - 1].is_zero()) jG = 0;
     }
-    std::vector<const u256*> Elev(jG);
+    return jG;
+  };
+  // poly_C_par = eq(rand) with rand = [r_layer | rand_tail] (product_tree.rs:279-280).  Everything but the top variable is known once the layer
+  // above has drawn its last challenge, so this builds E = eq(rand_tail, .) (times c_rank, leaving out the last logW variables, when sharded)
+  // into cpar0 + lhalf/2 then, and the suffix levels of an eq-factored layer below it, all while the host still runs the layer above's tail
+  // transcript; once r_layer is drawn, a layer without eq-factoring needs one eq_extend_top launch and an eq-factored one none.
+  auto build_eq = [&](const Shape& s, const std::vector<Fq>& rand_tail) {
+    const size_t n0 = s.lhalf / 2;
+    if (!rand_tail.empty()) dev::h2d(d_rand.p, rand_tail.data(), rand_tail.size() * sizeof(u256), ctx.stream);
+    dev::eq_evals(cpar0.p + n0, d_rand.p, (int)rand_tail.size() - s.logW, eq_small.p, ctx.stream);
+    if (s.sh) dev::scale(cpar0.p + n0, shard_eq_scale(rand_tail, W, rk).m, n0, ctx.stream);   // c_rank: fixed by rand's last logW entries
+    const size_t jG = plan_jG(s, rand_tail.data());
+    if (jG > 1) dev::eq_suffix(cpar0.p, cpar0.p + n0, n0, (int)jG - 1, ctx.stream);
+  };
+  for (size_t layer_id = num_layers; layer_id-- > 0;) {
+    const Shape shp = shape_of(layer_id);
+    const size_t num_rounds = shp.num_rounds, lhalf = shp.lhalf;
+    bool sh = shp.sh;                                  // this layer's tables are cyclic shards: the first rounds run sharded
+    std::optional<FineTimer> fhead(std::in_place, ctx, "batched layer head");   // r_layer drawn .. round 0's evaluations on the host
+    std::optional<FineTimer> fswitch;                                             // switch of an eq-factored layer .. its evaluations on the host
+    if (num_rounds > 0 && rand.size() != num_rounds) throw SpError(SP_ERR_INTERNAL, "product layer sizes are not powers of two");
+    // the suffix tables E_j = eq(rand[j+1..], .) of an eq-factored layer (E_0 at cpar0 + lhalf/2, the levels 1 .. jG-1 from cpar0 on, built by
+    // build_eq); from round jG on the standard kernels run on C = eq(rand[jG..], .) = E_{jG-1} (times c_rank) and the host multiplies the product
+    // instances' evaluations by prefix = prod_{j<jG} eq(tau_j, r_j).  Not applicable: the standard method from round 0 on C = [(1 - r_layer) E_0 | r_layer E_0].
+    size_t jG = num_rounds > 0 ? plan_jG(shp, rand.data() + 1) : 0;
+    if (jG && rand[0].is_zero()) jG = 0;
+    std::vector<u256*> Elev(jG);
     if (jG) {
       const size_t n0 = lhalf / 2;
-      dev::eq_evals(cpar0.p, d_rand.p + 1, (int)rand.size() - 1 - logW, eq_small.p, ctx.stream);
-      if (sh) dev::scale(cpar0.p, c_rank.m, n0, ctx.stream);
-      if (jG > 1) dev::eq_suffix(cpar0.p + n0, cpar0.p, n0, (int)jG - 1, ctx.stream);
-      Elev[0] = cpar0.p;
-      size_t off = n0;
+      Elev[0] = cpar0.p + n0;
+      size_t off = 0;
       for (size_t k = 1; k < jG; k++) { Elev[k] = cpar0.p + off; off += n0 >> k; }
-    } else if (sh) {
-      dev::eq_evals(cpar0.p, d_rand.p, (int)rand.size() - logW, eq_small.p, ctx.stream);
-      dev::scale(cpar0.p, c_rank.m, lhalf, ctx.stream);
-    } else dev::eq_evals(cpar0.p, d_rand.p, (int)rand.size(), eq_small.p, ctx.stream);
+    } else if (num_rounds > 0) dev::eq_extend_top(cpar0.p, lhalf / 2, rand[0].m, ctx.stream);
+    u256* const C0 = jG ? Elev[jG - 1] : cpar0.p;   // the shared C of the first standard round (read, never written)
     std::vector<dev::ScInst> insts;
     for (size_t i = 0; i < np; i++) {
       dev::ScInst in;
-      in.t[0] = prods[i]->layer(layer_id); in.t[1] = prods[i]->layer(layer_id) + lhalf; in.t[2] = cpar0.p; in.t[3] = nullptr;
+      in.t[0] = prods[i]->layer(layer_id); in.t[1] = prods[i]->layer(layer_id) + lhalf; in.t[2] = C0; in.t[3] = nullptr;
       in.c_out = cpar_a.p; in.write_c = i == 0;
       insts.push_back(in);
     }
@@ -233,27 +257,34 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
       }
     }
     const size_t ninst = insts.size();
+    size_t cur = lhalf;                                // current length of the tables this rank holds
+    dev::HostSig sig;
+    auto xr_next = [&]() { return sh ? ctx.comm->next_xr() : dev::XRank(); };
+    // eq-factored rounds: the np product instances through the G kernels (2 values each), the dot-product circuits (their third table is not an
+    // eq table) through the standard kernels in a second launch whose results land behind the first's
+    const size_t ndi = ninst - np;
+    auto launch_dotp = [&](bool first, const Fq& r) {
+      if (!ndi) return;
+      sig = ctx.next_sig();
+      sig.host_out = ctx.host_res + 3 * np;
+      if (first) dev::sc_eval(dev::SC_CUBIC3, insts.data() + np, (int)ndi, cur, d_out + 3 * np, ctx.red.p, ctx.stream, sig, xr_next());
+      else dev::sc_fold_eval(dev::SC_CUBIC3, insts.data() + np, (int)ndi, cur, r.m, d_out + 3 * np, ctx.red.p, ctx.stream, sig, xr_next());
+    };
+    // round 0's evaluations do not depend on the batching coefficients: launch them first, draw the coefficients while they run
+    if (jG) {
+      sig = ctx.next_sig();
+      dev::sc_eval_g(insts.data(), (int)np, cur, Elev[0], d_out, ctx.red.p, ctx.stream, sig, xr_next());
+      launch_dotp(true, Fq::zero());
+    } else if (num_rounds > 0) { sig = ctx.next_sig(); dev::sc_eval(dev::SC_CUBIC3, insts.data(), (int)ninst, cur, d_out, ctx.red.p, ctx.stream, sig, xr_next()); }
     std::vector<Fq> coeff_vec = T.challenge_vector("rand_coeffs_next_layer", claims_to_verify.size());
     Fq claim = Fq::zero();
     for (size_t i = 0; i < claims_to_verify.size(); i++) claim += claims_to_verify[i] * coeff_vec[i];
 
+    std::vector<Fq> coeff_std = coeff_vec;            // the standard rounds' weights: after an eq-factored switch, prefix * coeff for the product instances
     LayerProofBatched lp;
     std::vector<Fq> rand_prod;
     Fq e = claim;
-    size_t cur = lhalf;                                // current length of the tables this rank holds
-    dev::HostSig sig;
-    auto xr_next = [&]() { return sh ? ctx.comm->next_xr() : dev::XRank(); };
     if (jG) {
-      // ---- eq-factored rounds: the np product instances through the G kernels (2 values each), the dot-product circuits (their third table is not an
-      // eq table) through the standard kernels in a second launch whose results land behind the first's
-      const size_t ndi = ninst - np;
-      auto launch_dotp = [&](bool first, const Fq& r) {
-        if (!ndi) return;
-        sig = ctx.next_sig();
-        sig.host_out = ctx.host_res + 3 * np;
-        if (first) dev::sc_eval(dev::SC_CUBIC3, insts.data() + np, (int)ndi, cur, d_out + 3 * np, ctx.red.p, ctx.stream, sig, xr_next());
-        else dev::sc_fold_eval(dev::SC_CUBIC3, insts.data() + np, (int)ndi, cur, r.m, d_out + 3 * np, ctx.red.p, ctx.stream, sig, xr_next());
-      };
       std::vector<Fq> tau_inv(jG);   // batch inversion of tau_0 .. tau_{jG-1}
       {
         std::vector<Fq> pre(jG);
@@ -265,15 +296,13 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
       Fq cP = Fq::zero(), eD = Fq::zero(), prefix = Fq::one();
       for (size_t i = 0; i < np; i++) cP += claims_to_verify[i] * coeff_vec[i];
       for (size_t i = np; i < ninst; i++) eD += claims_to_verify[i] * coeff_vec[i];
-      sig = ctx.next_sig();
-      dev::sc_eval_g(insts.data(), (int)np, cur, Elev[0], d_out, ctx.red.p, ctx.stream, sig, xr_next());
-      launch_dotp(true, Fq::zero());
       const Fq one = Fq::one();
       for (size_t j = 0; j < jG; j++) {
         std::vector<Fq> ev(3 * ninst);
         FineTimer fw(ctx, "batched wait evals");
         ctx.wait_sig(sig);
         fw.stop();
+        fhead.reset();
         FineTimer fh(ctx, "batched host round");
         memcpy(ev.data(), ctx.host_res, 3 * ninst * sizeof(u256));
         Fq Q0 = Fq::zero(), Qinf = Fq::zero(), D0 = Fq::zero(), D2 = Fq::zero(), D3 = Fq::zero();
@@ -303,30 +332,36 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
           launch_dotp(false, r_j);
           cur >>= 1;
         } else {
-          // switch: bind with r_j, build C = prefix * eq(rand[jG..], .) (this rank's slice when sharded) and evaluate round jG the standard way
+          // switch: bind with r_j and evaluate round jG the standard way on C = E_{jG-1} = eq(rand[jG..], .) (this rank's slice, times c_rank, when
+          // sharded); the factor prefix, the same on every rank, is applied to the product instances' evaluations on the host
+          fswitch.emplace(ctx, "batched switch");
           std::vector<u256*> tabs;
           for (size_t i = 0; i < ninst; i++) { tabs.push_back(insts[i].t[0]); tabs.push_back(insts[i].t[1]); if (i >= np) tabs.push_back(insts[i].t[2]); }
           dev::fold_top(tabs.data(), (int)tabs.size(), cur, r_j.m, ctx.stream);
           cur >>= 1;
-          dev::eq_evals(cpar0.p, d_rand.p + jG, (int)rand.size() - (int)jG - logW, eq_small.p, ctx.stream);
-          dev::scale(cpar0.p, (prefix * c_rank).m, cur, ctx.stream);
           sig = ctx.next_sig();
           dev::sc_eval(dev::SC_CUBIC3, insts.data(), (int)ninst, cur, d_out, ctx.red.p, ctx.stream, sig, xr_next());
+          for (size_t i = 0; i < np; i++) coeff_std[i] = coeff_vec[i] * prefix;
         }
       }
-    } else if (num_rounds > 0) { sig = ctx.next_sig(); dev::sc_eval(dev::SC_CUBIC3, insts.data(), (int)ninst, cur, d_out, ctx.red.p, ctx.stream, sig, xr_next()); }
-    u256* cin = cpar0.p;
+    }
+    u256* cin = C0;
     u256* cpp[2] = {cpar_a.p, cpar_b.p};
     int flip = 0;
+    // the fold to two-entry tables (the last round's launch) publishes them, and the host binds the last variable itself (lp claims below)
+    bool bound_on_host = false;
+    std::vector<Fq> bound(6 * ninst);
     for (size_t j = jG; j < num_rounds; j++) {
       std::vector<Fq> ev(3 * ninst);
       FineTimer fw(ctx, "batched wait evals");
       ctx.wait_sig(sig);
       fw.stop();
+      fhead.reset(); fswitch.reset();
       FineTimer fh(ctx, "batched host round");
       memcpy(ev.data(), ctx.host_res, 3 * ninst * sizeof(u256));
+      if (bound_on_host) memcpy(bound.data(), ctx.host_res + 3 * ninst, 6 * ninst * sizeof(u256));
       Fq c0 = Fq::zero(), c2 = Fq::zero(), c3 = Fq::zero();
-      for (size_t i = 0; i < ninst; i++) { c0 += ev[3 * i] * coeff_vec[i]; c2 += ev[3 * i + 1] * coeff_vec[i]; c3 += ev[3 * i + 2] * coeff_vec[i]; }  // sumcheck.rs:359-361
+      for (size_t i = 0; i < ninst; i++) { c0 += ev[3 * i] * coeff_std[i]; c2 += ev[3 * i + 1] * coeff_std[i]; c3 += ev[3 * i + 2] * coeff_std[i]; }  // sumcheck.rs:359-361
       UniPoly poly = UniPoly::from_evals({c0, e - c0, c2, c3});
       poly.append_to_transcript("poly", T);
       Fq r_j = T.challenge_scalar("challenge_nextround");
@@ -357,8 +392,12 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
         lp.proof.compressed_polys.push_back(poly.compress());
         continue;
       }
-      if (j + 1 < num_rounds) { sig = ctx.next_sig(); dev::sc_fold_eval(dev::SC_CUBIC3, insts.data(), (int)ninst, cur, r_j.m, d_out, ctx.red.p, ctx.stream, sig, sh ? ctx.comm->next_xr() : dev::XRank()); }
-      else {
+      if (j + 1 < num_rounds) {
+        bound_on_host = j + 2 == num_rounds;
+        sig = ctx.next_sig();
+        dev::sc_fold_eval(dev::SC_CUBIC3, insts.data(), (int)ninst, cur, r_j.m, d_out, ctx.red.p, ctx.stream, sig, sh ? ctx.comm->next_xr() : dev::XRank(),
+                          bound_on_host ? ctx.host_res + 3 * ninst : nullptr);
+      } else if (!bound_on_host) {
         std::vector<u256*> tabs;
         for (size_t i = 0; i < ninst; i++) { tabs.push_back(insts[i].t[0]); tabs.push_back(insts[i].t[1]); if (i >= np) tabs.push_back(insts[i].t[2]); }
         dev::fold_top(tabs.data(), (int)tabs.size(), cur, r_j.m, ctx.stream);
@@ -371,17 +410,24 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
       lp.proof.compressed_polys.push_back(poly.compress());
     }
     // final claims: first element of every A / B (and C for the dot-product circuits)
+    fhead.reset();
     FineTimer fl(ctx, "batched layer tail (claims d2h + transcript)");
-    {  // one gather kernel that also publishes the values to the host (instead of 2-3 tiny copies per instance and a stream synchronise)
+    std::vector<Fq> heads(3 * ninst);
+    if (bound_on_host) {   // a0 + r (a1 - a0): what the fold computes (fq_fold_const), on the two entries the last launch published
+      const Fq& r = rand_prod.back();
+      for (size_t k = 0; k < 3 * ninst; k++) heads[k] = bound[2 * k] + r * (bound[2 * k + 1] - bound[2 * k]);
+      if (layer_id > 0) build_eq(shape_of(layer_id - 1), rand_prod);
+    } else {  // layers of fewer than two rounds: one gather kernel that also publishes the values to the host
       std::vector<const u256*> hp(3 * ninst);
       for (size_t i = 0; i < ninst; i++) { hp[3 * i] = insts[i].t[0]; hp[3 * i + 1] = insts[i].t[1]; hp[3 * i + 2] = i >= np ? insts[i].t[2] : insts[i].t[0]; }
       dev::HostSig hs = ctx.next_sig();
       dev::heads(d_heads.p, hp.data(), (int)hp.size(), ctx.stream, hs);
+      if (layer_id > 0) build_eq(shape_of(layer_id - 1), rand_prod);
       ctx.wait_sig(hs);
+      memcpy(heads.data(), ctx.host_res, 3 * ninst * sizeof(u256));
     }
-    const uint8_t* heads_h = reinterpret_cast<const uint8_t*>(ctx.host_res);
     lp.claims_prod_left.resize(np); lp.claims_prod_right.resize(np);
-    for (size_t i = 0; i < np; i++) { memcpy(&lp.claims_prod_left[i], heads_h + 96 * i, 32); memcpy(&lp.claims_prod_right[i], heads_h + 96 * i + 32, 32); }
+    for (size_t i = 0; i < np; i++) { lp.claims_prod_left[i] = heads[3 * i]; lp.claims_prod_right[i] = heads[3 * i + 1]; }
     for (size_t i = 0; i < np; i++) {
       T.append_scalar("claim_prod_left", lp.claims_prod_left[i]);
       T.append_scalar("claim_prod_right", lp.claims_prod_right[i]);
@@ -389,9 +435,9 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
     if (with_dotp) {
       out.dotp_left.resize(nd); out.dotp_right.resize(nd); out.dotp_weight.resize(nd);
       for (size_t i = 0; i < nd; i++) {
-        memcpy(&out.dotp_left[i], heads_h + 96 * (np + i), 32);
-        memcpy(&out.dotp_right[i], heads_h + 96 * (np + i) + 32, 32);
-        memcpy(&out.dotp_weight[i], heads_h + 96 * (np + i) + 64, 32);
+        out.dotp_left[i] = heads[3 * (np + i)];
+        out.dotp_right[i] = heads[3 * (np + i) + 1];
+        out.dotp_weight[i] = heads[3 * (np + i) + 2];
         T.append_scalar("claim_dotp_left", out.dotp_left[i]);
         T.append_scalar("claim_dotp_right", out.dotp_right[i]);
         T.append_scalar("claim_dotp_weight", out.dotp_weight[i]);
