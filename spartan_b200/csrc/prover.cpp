@@ -328,6 +328,58 @@ std::vector<Fq> host_eq_evals(const std::vector<Fq>& r) {  // EqPolynomial::eval
   return ev;
 }
 
+// ================================================================================================ sumcheck rounds on the device
+// the tables fold_top binds, in instance order: every set t[k] but a t[2] the instance only reads; with shared_c, that shared C follows once
+static std::vector<u256*> owned_tables(const std::vector<dev::ScInst>& insts, bool shared_c) {
+  std::vector<u256*> tabs;
+  u256* shared = nullptr;
+  for (const dev::ScInst& in : insts)
+    for (int k = 0; k < 4; k++)
+      if (k == 2 && in.c_out != in.t[2]) shared = in.t[2];
+      else if (in.t[k]) tabs.push_back(in.t[k]);
+  if (shared_c && shared) tabs.push_back(shared);
+  return tabs;
+}
+dev::XRank ScRounds::xr() { return sharded ? ctx.comm->next_xr() : dev::XRank(); }
+void ScRounds::eval() {
+  sig = ctx.next_sig();
+  dev::sc_eval(kind, insts.data(), (int)insts.size(), len, d_out, ctx.red.p, ctx.stream, sig, xr());
+}
+void ScRounds::fold_eval(const Fq& r, u256* host_bound) {
+  if (sharded && len < Ctx::SHARD_MIN_LOCAL) {
+    // leave the sharded stage: bind locally, all-gather every table into replicated copies (in the window), evaluate the next round there
+    std::vector<u256*> tabs = owned_tables(insts, true);
+    dev::fold_top(tabs.data(), (int)tabs.size(), len, r.m, ctx.stream);
+    const size_t glen = (len / 2) * (size_t)ctx.shard_world();
+    u256* g = ctx.allgather_cyclic(tabs.data(), (int)tabs.size(), len / 2);
+    for (dev::ScInst& in : insts) {
+      const bool own_c = in.c_out == in.t[2];
+      for (int k = 0; k < 4; k++)
+        if (in.t[k]) in.t[k] = g + (size_t)(std::find(tabs.begin(), tabs.end(), in.t[k]) - tabs.begin()) * glen;
+      if (own_c) in.c_out = in.t[2];
+    }
+    sharded = false;
+    len = glen;
+    eval();
+    return;
+  }
+  sig = ctx.next_sig();
+  dev::sc_fold_eval(kind, insts.data(), (int)insts.size(), len, r.m, d_out, ctx.red.p, ctx.stream, sig, xr(), host_bound);
+  len >>= 1;
+  for (dev::ScInst& in : insts) in.t[2] = in.c_out;   // a shared C is read from where it was folded to
+}
+void ScRounds::fold(const Fq& r) {
+  std::vector<u256*> tabs = owned_tables(insts, false);
+  dev::fold_top(tabs.data(), (int)tabs.size(), len, r.m, ctx.stream);
+  len >>= 1;
+}
+std::vector<Fq> ScRounds::wait() {
+  ctx.wait_sig(sig);
+  std::vector<Fq> ev(3 * insts.size());
+  memcpy(static_cast<void*>(ev.data()), ctx.host_res, ev.size() * sizeof(u256));
+  return ev;
+}
+
 // ================================================================================================ ZK sumcheck on the device
 // prove_quad (sumcheck.rs:428-586) and prove_cubic_with_additive_term (sumcheck.rs:588-776).
 // tables: NT device arrays of length 2^num_rounds, folded in place (their first element holds the final evaluation).
@@ -393,15 +445,13 @@ struct ZkPre {
   }
 };
 
-// sharded: `tables_in` are this rank's cyclic shards (length 2^num_rounds / world).  The first rounds then run on the shards — the fused
+// sharded: `tables` are this rank's cyclic shards (length 2^num_rounds / world).  The first rounds then run on the shards — the fused
 // kernels exchange their partial sums over NVLink before handing the round's evaluations to the host — until the local tables drop below
 // streaming size; the shards are then all-gathered into replicated tables (in the window) and the latency-bound tail runs on every rank alike.
-static void zk_sumcheck_prove(Ctx& ctx, dev::ScKind kind, const Fq& claim, const Fq& blind_claim, size_t num_rounds, u256* const* tables_in, int nt,
+static void zk_sumcheck_prove(Ctx& ctx, dev::ScKind kind, const Fq& claim, const Fq& blind_claim, size_t num_rounds, u256* const* tables, int nt,
                               const CommitKey& g1, const CommitKey& gn, Transcript& T, RandomTape& tape, ZKSumcheckInstanceProof& proof,
                               std::vector<Fq>& r, std::vector<Fq>& finals, Fq& blind_post, bool sharded = false, ZkPre* pre_in = nullptr) {
-  std::vector<u256*> tabs(tables_in, tables_in + nt);
-  u256* const* tables = tabs.data();
-  bool sh = sharded && ctx.shard_world() > 1;
+  const bool sh = sharded && ctx.shard_world() > 1;
   const int W = sh ? ctx.shard_world() : 1;
   const int degree = kind == dev::SC_QUAD ? 2 : 3;
   ZkPre pre_local;
@@ -425,17 +475,13 @@ static void zk_sumcheck_prove(Ctx& ctx, dev::ScKind kind, const Fq& claim, const
   for (int t = 0; t < 4; t++) inst.t[t] = t < nt ? tables[t] : nullptr;
   inst.c_out = inst.t[2];
   inst.write_c = 1;
-  u256* d_out = ctx.small.p + 0;     // 3 result scalars
-  size_t len = ((size_t)1 << num_rounds) / W;   // current length of the tables this rank holds
-  dev::HostSig sig = ctx.next_sig();
-  dev::sc_eval(kind, &inst, 1, len, d_out, ctx.red.p, ctx.stream, sig, sh ? ctx.comm->next_xr() : dev::XRank());
+  ScRounds sc{ctx, kind, {inst}, ((size_t)1 << num_rounds) / W, sh, ctx.small.p + 0};
+  sc.eval();
   for (size_t j = 0; j < num_rounds; j++) {
-    Fq e[3];
     FineTimer fw(ctx, "zk wait evals");
-    ctx.wait_sig(sig);
+    const std::vector<Fq> e = sc.wait();
     fw.stop();
     FineTimer fh(ctx, "zk host commit_poly+challenge");
-    memcpy(e, ctx.host_res, sizeof e);
     std::vector<Fq> evals = {e[0], claim_per_round - e[0], e[1]};
     if (degree == 3) evals.push_back(e[2]);
     UniPoly poly = UniPoly::from_evals(evals);
@@ -445,22 +491,8 @@ static void zk_sumcheck_prove(Ctx& ctx, dev::ScKind kind, const Fq& claim, const
     Fq r_j = T.challenge_scalar("challenge_nextround");
     // bind the tables to r_j on the device right away (fused with the next round's evaluation); the host continues with the
     // sigma protocol of this round while the kernel runs
-    if (j + 1 < num_rounds && sh && len < Ctx::SHARD_MIN_LOCAL) {
-      // leave the sharded stage: bind locally, all-gather the shards into replicated tables, evaluate the next round there
-      dev::fold_top(tables, nt, len, r_j.m, ctx.stream);
-      const size_t glen = (len / 2) * W;
-      u256* g = ctx.allgather_cyclic(tables, nt, len / 2);
-      for (int t = 0; t < nt; t++) { tabs[t] = g + (size_t)t * glen; inst.t[t] = tabs[t]; }
-      inst.c_out = inst.t[2];
-      sh = false;
-      len = glen;
-      sig = ctx.next_sig();
-      dev::sc_eval(kind, &inst, 1, len, d_out, ctx.red.p, ctx.stream, sig);
-    } else {
-      if (j + 1 < num_rounds) { sig = ctx.next_sig(); dev::sc_fold_eval(kind, &inst, 1, len, r_j.m, d_out, ctx.red.p, ctx.stream, sig, sh ? ctx.comm->next_xr() : dev::XRank()); }
-      else dev::fold_top(tables, nt, len, r_j.m, ctx.stream);
-      len >>= 1;
-    }
+    if (j + 1 < num_rounds) sc.fold_eval(r_j);
+    else sc.fold(r_j);
     fh.stop();
     FineTimer fs(ctx, "zk host sigma (overlaps kernel)");
 
@@ -489,7 +521,7 @@ static void zk_sumcheck_prove(Ctx& ctx, dev::ScKind kind, const Fq& claim, const
     proof.comm_evals.push_back(comm_claim_per_round);
   }
   finals.resize(nt);
-  for (int t = 0; t < nt; t++) dev::d2h(ctx.pinned + 32 * t, tables[t], 32, ctx.stream);
+  for (int t = 0; t < nt; t++) dev::d2h(ctx.pinned + 32 * t, sc.insts[0].t[t], 32, ctx.stream);   // the replicated copies after a shard exit
   ctx.sync();
   memcpy(finals.data(), ctx.pinned, 32 * nt);
   blind_post = blinds_evals[num_rounds - 1];

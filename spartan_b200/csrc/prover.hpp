@@ -190,6 +190,25 @@ struct IpaRound {
   void fold(size_t cur, const Fq& u, const Fq& u_inv);   // a, b, svec of the next round (bullet.rs:105-108)
 };
 
+// The device side of one sumcheck, or of a batch of instances proved together (prove_cubic_batched), run by zk_sumcheck_prove and batched_prove.
+// An instance owns the tables t[0..4) that are set, except a t[2] it only reads (c_out != t[2]): a C shared by the batch, which one instance
+// folds into c_out, where they all read it next round.  Sharded, the tables are this rank's cyclic shards until fold_eval leaves the sharded
+// stage (DESIGN.md §6): once they are shorter than Ctx::SHARD_MIN_LOCAL it binds them, all-gathers them into replicated copies and evaluates there.
+struct ScRounds {
+  Ctx& ctx;
+  dev::ScKind kind;
+  std::vector<dev::ScInst> insts;
+  size_t len;            // current length of the tables this rank holds
+  bool sharded;
+  u256* d_out;           // device result slot, 3 scalars per instance
+  dev::HostSig sig;      // of the last launch that publishes evaluations
+  void eval();                                              // evaluations of the current round
+  void fold_eval(const Fq& r, u256* host_bound = nullptr);  // bind with r, evaluate the next round (host_bound: dev::sc_fold_eval)
+  void fold(const Fq& r);                                   // bind the owned tables with r only
+  std::vector<Fq> wait();                                   // the 3 ninst evaluations of the last launch
+  dev::XRank xr();                                          // the cross-rank exchange of the next launch (none once replicated)
+};
+
 // <x, G[0..n)> of one row of n scalars against the per-window table of `gs`, for latency.  For n >= 2 (even) it is the inner-product round kernel
 // with a = (1, 1) and blocks of two generators: its "L" (odd j) and "R" (even j) reach the host through the kernel's own publication and are added
 // there, one launch instead of msm_rows + reduce + compress + copy.  n = 1 runs msm_rows.  The constructor launches, collect() waits.

@@ -221,7 +221,6 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
   for (size_t layer_id = num_layers; layer_id-- > 0;) {
     const Shape shp = shape_of(layer_id);
     const size_t num_rounds = shp.num_rounds, lhalf = shp.lhalf;
-    bool sh = shp.sh;                                  // this layer's tables are cyclic shards: the first rounds run sharded
     std::optional<FineTimer> fhead(std::in_place, ctx, "batched layer head");   // r_layer drawn .. round 0's evaluations on the host
     std::optional<FineTimer> fswitch;                                             // switch of an eq-factored layer .. its evaluations on the host
     if (num_rounds > 0 && rand.size() != num_rounds) throw SpError(SP_ERR_INTERNAL, "product layer sizes are not powers of two");
@@ -238,44 +237,43 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
       for (size_t k = 1; k < jG; k++) { Elev[k] = cpar0.p + off; off += n0 >> k; }
     } else if (num_rounds > 0) dev::eq_extend_top(cpar0.p, lhalf / 2, rand[0].m, ctx.stream);
     u256* const C0 = jG ? Elev[jG - 1] : cpar0.p;   // the shared C of the first standard round (read, never written)
-    std::vector<dev::ScInst> insts;
+    ScRounds sc{ctx, dev::SC_CUBIC3, {}, lhalf, shp.sh, d_out};
     for (size_t i = 0; i < np; i++) {
       dev::ScInst in;
       in.t[0] = prods[i]->layer(layer_id); in.t[1] = prods[i]->layer(layer_id) + lhalf; in.t[2] = C0; in.t[3] = nullptr;
       in.c_out = cpar_a.p; in.write_c = i == 0;
-      insts.push_back(in);
+      sc.insts.push_back(in);
     }
     const bool with_dotp = layer_id == 0 && nd > 0;
     if (with_dotp) {
       for (size_t i = 0; i < nd; i++) {
-        if (dotps[i].sharded != sh) throw SpError(SP_ERR_INTERNAL, "dot-product circuits and product circuits disagree on sharding");
+        if (dotps[i].sharded != shp.sh) throw SpError(SP_ERR_INTERNAL, "dot-product circuits and product circuits disagree on sharding");
         dev::ScInst in;
         in.t[0] = dotps[i].left; in.t[1] = dotps[i].right; in.t[2] = dotps[i].weight; in.t[3] = nullptr;
         in.c_out = dotps[i].weight; in.write_c = 1;
-        insts.push_back(in);
+        sc.insts.push_back(in);
         claims_to_verify.push_back(dotps[i].claim);   // DotProductCircuit::evaluate, taken on the unsharded tables by the caller
       }
     }
-    const size_t ninst = insts.size();
-    size_t cur = lhalf;                                // current length of the tables this rank holds
-    dev::HostSig sig;
-    auto xr_next = [&]() { return sh ? ctx.comm->next_xr() : dev::XRank(); };
+    const size_t ninst = sc.insts.size();
     // eq-factored rounds: the np product instances through the G kernels (2 values each), the dot-product circuits (their third table is not an
     // eq table) through the standard kernels in a second launch whose results land behind the first's
     const size_t ndi = ninst - np;
-    auto launch_dotp = [&](bool first, const Fq& r) {
-      if (!ndi) return;
-      sig = ctx.next_sig();
-      sig.host_out = ctx.host_res + 3 * np;
-      if (first) dev::sc_eval(dev::SC_CUBIC3, insts.data() + np, (int)ndi, cur, d_out + 3 * np, ctx.red.p, ctx.stream, sig, xr_next());
-      else dev::sc_fold_eval(dev::SC_CUBIC3, insts.data() + np, (int)ndi, cur, r.m, d_out + 3 * np, ctx.red.p, ctx.stream, sig, xr_next());
+    auto launch_g = [&](size_t j, const Fq* r) {   // round j; r: bind with r first
+      sc.sig = ctx.next_sig();
+      if (!r) dev::sc_eval_g(sc.insts.data(), (int)np, sc.len, Elev[j], d_out, ctx.red.p, ctx.stream, sc.sig, sc.xr());
+      else dev::sc_fold_eval_g(sc.insts.data(), (int)np, sc.len, r->m, Elev[j], d_out, ctx.red.p, ctx.stream, sc.sig, sc.xr());
+      if (ndi) {
+        sc.sig = ctx.next_sig();
+        sc.sig.host_out = ctx.host_res + 3 * np;
+        if (!r) dev::sc_eval(dev::SC_CUBIC3, sc.insts.data() + np, (int)ndi, sc.len, d_out + 3 * np, ctx.red.p, ctx.stream, sc.sig, sc.xr());
+        else dev::sc_fold_eval(dev::SC_CUBIC3, sc.insts.data() + np, (int)ndi, sc.len, r->m, d_out + 3 * np, ctx.red.p, ctx.stream, sc.sig, sc.xr());
+      }
+      if (r) sc.len >>= 1;
     };
     // round 0's evaluations do not depend on the batching coefficients: launch them first, draw the coefficients while they run
-    if (jG) {
-      sig = ctx.next_sig();
-      dev::sc_eval_g(insts.data(), (int)np, cur, Elev[0], d_out, ctx.red.p, ctx.stream, sig, xr_next());
-      launch_dotp(true, Fq::zero());
-    } else if (num_rounds > 0) { sig = ctx.next_sig(); dev::sc_eval(dev::SC_CUBIC3, insts.data(), (int)ninst, cur, d_out, ctx.red.p, ctx.stream, sig, xr_next()); }
+    if (jG) launch_g(0, nullptr);
+    else if (num_rounds > 0) sc.eval();
     std::vector<Fq> coeff_vec = T.challenge_vector("rand_coeffs_next_layer", claims_to_verify.size());
     Fq claim = Fq::zero();
     for (size_t i = 0; i < claims_to_verify.size(); i++) claim += claims_to_verify[i] * coeff_vec[i];
@@ -284,142 +282,91 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
     LayerProofBatched lp;
     std::vector<Fq> rand_prod;
     Fq e = claim;
+    std::vector<Fq> tau_inv(jG);   // batch inversion of tau_0 .. tau_{jG-1}
+    Fq cP = Fq::zero(), eD = Fq::zero(), prefix = Fq::one();
     if (jG) {
-      std::vector<Fq> tau_inv(jG);   // batch inversion of tau_0 .. tau_{jG-1}
-      {
-        std::vector<Fq> pre(jG);
-        Fq acc = Fq::one();
-        for (size_t j = 0; j < jG; j++) { pre[j] = acc; acc *= rand[j]; }
-        Fq inv = acc.inv();
-        for (size_t j = jG; j-- > 0;) { tau_inv[j] = inv * pre[j]; inv *= rand[j]; }
-      }
-      Fq cP = Fq::zero(), eD = Fq::zero(), prefix = Fq::one();
+      std::vector<Fq> pre(jG);
+      Fq acc = Fq::one();
+      for (size_t j = 0; j < jG; j++) { pre[j] = acc; acc *= rand[j]; }
+      Fq inv = acc.inv();
+      for (size_t j = jG; j-- > 0;) { tau_inv[j] = inv * pre[j]; inv *= rand[j]; }
       for (size_t i = 0; i < np; i++) cP += claims_to_verify[i] * coeff_vec[i];
       for (size_t i = np; i < ninst; i++) eD += claims_to_verify[i] * coeff_vec[i];
-      const Fq one = Fq::one();
-      for (size_t j = 0; j < jG; j++) {
-        std::vector<Fq> ev(3 * ninst);
-        FineTimer fw(ctx, "batched wait evals");
-        ctx.wait_sig(sig);
-        fw.stop();
-        fhead.reset();
-        FineTimer fh(ctx, "batched host round");
-        memcpy(ev.data(), ctx.host_res, 3 * ninst * sizeof(u256));
-        Fq Q0 = Fq::zero(), Qinf = Fq::zero(), D0 = Fq::zero(), D2 = Fq::zero(), D3 = Fq::zero();
-        for (size_t i = 0; i < np; i++) { Q0 += ev[3 * i] * coeff_vec[i]; Qinf += ev[3 * i + 1] * coeff_vec[i]; }
-        for (size_t i = np; i < ninst; i++) { D0 += ev[3 * i] * coeff_vec[i]; D2 += ev[3 * i + 1] * coeff_vec[i]; D3 += ev[3 * i + 2] * coeff_vec[i]; }
-        const Fq& tau = rand[j];
-        const Fq omt = one - tau;
-        const Fq Q1 = (cP - omt * Q0) * tau_inv[j];            // c_j = (1 - tau_j) q(0) + tau_j q(1)
-        const Fq qb = Q1 - Q0 - Qinf;
-        auto q_at = [&](const Fq& t) { return (Qinf * t + qb) * t + Q0; };
-        const Fq slope = tau - omt;                              // eq(tau_j, t) = (1 - tau_j) + t (2 tau_j - 1)
-        std::vector<Fq> sD = {D0, eD - D0, D2, D3}, evals(4);
-        Fq t = Fq::zero(), lin = omt;
-        for (int k = 0; k < 4; k++) { evals[k] = prefix * lin * q_at(t) + (ndi ? sD[k] : Fq::zero()); t += one; lin += slope; }
-        UniPoly poly = UniPoly::from_evals(evals);             // the same cubic the reference interpolates from its evaluations at 0, 1, 2, 3
-        poly.append_to_transcript("poly", T);
-        Fq r_j = T.challenge_scalar("challenge_nextround");
-        rand_prod.push_back(r_j);
-        cP = q_at(r_j);
-        prefix *= omt + r_j * slope;
-        if (ndi) eD = UniPoly::from_evals(sD).evaluate(r_j);
-        e = poly.evaluate(r_j);
-        lp.proof.compressed_polys.push_back(poly.compress());
-        if (j + 1 < jG) {
-          sig = ctx.next_sig();
-          dev::sc_fold_eval_g(insts.data(), (int)np, cur, r_j.m, Elev[j + 1], d_out, ctx.red.p, ctx.stream, sig, xr_next());
-          launch_dotp(false, r_j);
-          cur >>= 1;
-        } else {
-          // switch: bind with r_j and evaluate round jG the standard way on C = E_{jG-1} = eq(rand[jG..], .) (this rank's slice, times c_rank, when
-          // sharded); the factor prefix, the same on every rank, is applied to the product instances' evaluations on the host
-          fswitch.emplace(ctx, "batched switch");
-          std::vector<u256*> tabs;
-          for (size_t i = 0; i < ninst; i++) { tabs.push_back(insts[i].t[0]); tabs.push_back(insts[i].t[1]); if (i >= np) tabs.push_back(insts[i].t[2]); }
-          dev::fold_top(tabs.data(), (int)tabs.size(), cur, r_j.m, ctx.stream);
-          cur >>= 1;
-          sig = ctx.next_sig();
-          dev::sc_eval(dev::SC_CUBIC3, insts.data(), (int)ninst, cur, d_out, ctx.red.p, ctx.stream, sig, xr_next());
-          for (size_t i = 0; i < np; i++) coeff_std[i] = coeff_vec[i] * prefix;
-        }
-      }
     }
-    u256* cin = C0;
-    u256* cpp[2] = {cpar_a.p, cpar_b.p};
-    int flip = 0;
+    const Fq one = Fq::one();
     // the fold to two-entry tables (the last round's launch) publishes them, and the host binds the last variable itself (lp claims below)
     bool bound_on_host = false;
-    std::vector<Fq> bound(6 * ninst);
-    for (size_t j = jG; j < num_rounds; j++) {
-      std::vector<Fq> ev(3 * ninst);
+    for (size_t j = 0; j < num_rounds; j++) {
       FineTimer fw(ctx, "batched wait evals");
-      ctx.wait_sig(sig);
+      const std::vector<Fq> ev = sc.wait();
       fw.stop();
       fhead.reset(); fswitch.reset();
       FineTimer fh(ctx, "batched host round");
-      memcpy(ev.data(), ctx.host_res, 3 * ninst * sizeof(u256));
-      if (bound_on_host) memcpy(bound.data(), ctx.host_res + 3 * ninst, 6 * ninst * sizeof(u256));
-      Fq c0 = Fq::zero(), c2 = Fq::zero(), c3 = Fq::zero();
-      for (size_t i = 0; i < ninst; i++) { c0 += ev[3 * i] * coeff_std[i]; c2 += ev[3 * i + 1] * coeff_std[i]; c3 += ev[3 * i + 2] * coeff_std[i]; }  // sumcheck.rs:359-361
-      UniPoly poly = UniPoly::from_evals({c0, e - c0, c2, c3});
+      const bool eqf = j < jG;
+      std::vector<Fq> evals(4), sD;
+      Fq Q0 = Fq::zero(), Qinf = Fq::zero(), qb = Fq::zero(), omt = Fq::zero(), slope = Fq::zero();
+      auto q_at = [&](const Fq& t) { return (Qinf * t + qb) * t + Q0; };
+      if (eqf) {
+        Fq D0 = Fq::zero(), D2 = Fq::zero(), D3 = Fq::zero();
+        for (size_t i = 0; i < np; i++) { Q0 += ev[3 * i] * coeff_vec[i]; Qinf += ev[3 * i + 1] * coeff_vec[i]; }
+        for (size_t i = np; i < ninst; i++) { D0 += ev[3 * i] * coeff_vec[i]; D2 += ev[3 * i + 1] * coeff_vec[i]; D3 += ev[3 * i + 2] * coeff_vec[i]; }
+        const Fq& tau = rand[j];
+        omt = one - tau;
+        const Fq Q1 = (cP - omt * Q0) * tau_inv[j];            // c_j = (1 - tau_j) q(0) + tau_j q(1)
+        qb = Q1 - Q0 - Qinf;
+        slope = tau - omt;                                       // eq(tau_j, t) = (1 - tau_j) + t (2 tau_j - 1)
+        sD = {D0, eD - D0, D2, D3};
+        Fq t = Fq::zero(), lin = omt;
+        for (int k = 0; k < 4; k++) { evals[k] = prefix * lin * q_at(t) + (ndi ? sD[k] : Fq::zero()); t += one; lin += slope; }
+      } else {
+        Fq c0 = Fq::zero(), c2 = Fq::zero(), c3 = Fq::zero();
+        for (size_t i = 0; i < ninst; i++) { c0 += ev[3 * i] * coeff_std[i]; c2 += ev[3 * i + 1] * coeff_std[i]; c3 += ev[3 * i + 2] * coeff_std[i]; }  // sumcheck.rs:359-361
+        evals = {c0, e - c0, c2, c3};
+      }
+      UniPoly poly = UniPoly::from_evals(evals);               // eq-factored: the same cubic the reference interpolates from its evaluations at 0, 1, 2, 3
       poly.append_to_transcript("poly", T);
       Fq r_j = T.challenge_scalar("challenge_nextround");
       rand_prod.push_back(r_j);
-      // bind every table (shared C written once, through a ping-pong buffer)
-      for (size_t i = 0; i < np; i++) { insts[i].t[2] = cin; insts[i].c_out = cpp[flip]; }
-      if (j + 1 < num_rounds && sh && cur < Ctx::SHARD_MIN_LOCAL) {
-        // leave the sharded stage: bind locally, all-gather every table into replicated copies (in the window), evaluate the next round there
-        std::vector<u256*> tabs;
-        for (size_t i = 0; i < ninst; i++) { tabs.push_back(insts[i].t[0]); tabs.push_back(insts[i].t[1]); if (i >= np) tabs.push_back(insts[i].t[2]); }
-        tabs.push_back(cin);
-        dev::fold_top(tabs.data(), (int)tabs.size(), cur, r_j.m, ctx.stream);
-        const size_t glen = (cur / 2) * (size_t)W;
-        std::vector<const u256*> src(tabs.begin(), tabs.end());
-        u256* g = ctx.allgather_cyclic(src.data(), (int)src.size(), cur / 2);
-        size_t k = 0;
-        for (size_t i = 0; i < ninst; i++) {
-          insts[i].t[0] = g + (k++) * glen; insts[i].t[1] = g + (k++) * glen;
-          if (i >= np) { insts[i].t[2] = g + (k++) * glen; insts[i].c_out = insts[i].t[2]; }
-        }
-        cin = g + k * glen;
-        for (size_t i = 0; i < np; i++) insts[i].t[2] = cin;
-        sh = false;
-        cur = glen;
-        sig = ctx.next_sig();
-        dev::sc_eval(dev::SC_CUBIC3, insts.data(), (int)ninst, cur, d_out, ctx.red.p, ctx.stream, sig);
-        e = poly.evaluate(r_j);
-        lp.proof.compressed_polys.push_back(poly.compress());
-        continue;
-      }
-      if (j + 1 < num_rounds) {
+      if (j + 1 < jG) {
+        launch_g(j + 1, &r_j);
+      } else if (j + 1 == jG) {
+        // switch: bind with r_j and evaluate round jG the standard way on C = E_{jG-1} = eq(rand[jG..], .) (this rank's slice, times c_rank, when
+        // sharded); the factor prefix, the same on every rank, is applied to the product instances' evaluations on the host
+        fswitch.emplace(ctx, "batched switch");
+        sc.fold(r_j);
+        sc.eval();
+      } else if (j + 1 < num_rounds) {
         bound_on_host = j + 2 == num_rounds;
-        sig = ctx.next_sig();
-        dev::sc_fold_eval(dev::SC_CUBIC3, insts.data(), (int)ninst, cur, r_j.m, d_out, ctx.red.p, ctx.stream, sig, sh ? ctx.comm->next_xr() : dev::XRank(),
-                          bound_on_host ? ctx.host_res + 3 * ninst : nullptr);
+        sc.fold_eval(r_j, bound_on_host ? ctx.host_res + 3 * ninst : nullptr);
+        // the product instances now read the shared C where instance 0 folded it, so the next fold writes it into the other ping-pong half;
+        // after the shard exit they read its gathered copy instead and both halves are free
+        for (size_t i = 0; i < np; i++)
+          if (sc.insts[i].t[2] == sc.insts[i].c_out) sc.insts[i].c_out = sc.insts[i].c_out == cpar_a.p ? cpar_b.p : cpar_a.p;
       } else if (!bound_on_host) {
-        std::vector<u256*> tabs;
-        for (size_t i = 0; i < ninst; i++) { tabs.push_back(insts[i].t[0]); tabs.push_back(insts[i].t[1]); if (i >= np) tabs.push_back(insts[i].t[2]); }
-        dev::fold_top(tabs.data(), (int)tabs.size(), cur, r_j.m, ctx.stream);
-        // the shared C's final value is never used by the prover (claims_prod.2 is dropped, product_tree.rs:336)
+        sc.fold(r_j);   // the shared C's final value is never used by the prover (claims_prod.2 is dropped, product_tree.rs:336)
       }
-      cin = cpp[flip];
-      flip ^= 1;
-      cur >>= 1;
       e = poly.evaluate(r_j);
       lp.proof.compressed_polys.push_back(poly.compress());
+      if (eqf) {
+        cP = q_at(r_j);
+        prefix *= omt + r_j * slope;
+        if (ndi) eD = UniPoly::from_evals(sD).evaluate(r_j);
+        if (j + 1 == jG) for (size_t i = 0; i < np; i++) coeff_std[i] = coeff_vec[i] * prefix;
+      }
     }
     // final claims: first element of every A / B (and C for the dot-product circuits)
     fhead.reset();
     FineTimer fl(ctx, "batched layer tail (claims d2h + transcript)");
     std::vector<Fq> heads(3 * ninst);
     if (bound_on_host) {   // a0 + r (a1 - a0): what the fold computes (fq_fold_const), on the two entries the last launch published
+      std::vector<Fq> bound(6 * ninst);
+      memcpy(bound.data(), ctx.host_res + 3 * ninst, 6 * ninst * sizeof(u256));
       const Fq& r = rand_prod.back();
       for (size_t k = 0; k < 3 * ninst; k++) heads[k] = bound[2 * k] + r * (bound[2 * k + 1] - bound[2 * k]);
       if (layer_id > 0) build_eq(shape_of(layer_id - 1), rand_prod);
     } else {  // layers of fewer than two rounds: one gather kernel that also publishes the values to the host
-      std::vector<const u256*> hp(3 * ninst);
-      for (size_t i = 0; i < ninst; i++) { hp[3 * i] = insts[i].t[0]; hp[3 * i + 1] = insts[i].t[1]; hp[3 * i + 2] = i >= np ? insts[i].t[2] : insts[i].t[0]; }
+      std::vector<const u256*> hp;
+      for (size_t i = 0; i < ninst; i++) { const dev::ScInst& in = sc.insts[i]; hp.insert(hp.end(), {in.t[0], in.t[1], i >= np ? in.t[2] : in.t[0]}); }
       dev::HostSig hs = ctx.next_sig();
       dev::heads(d_heads.p, hp.data(), (int)hp.size(), ctx.stream, hs);
       if (layer_id > 0) build_eq(shape_of(layer_id - 1), rand_prod);
