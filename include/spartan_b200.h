@@ -49,6 +49,9 @@ int sp_ctx_create(int device, sp_ctx** out);
 void sp_ctx_destroy(sp_ctx* ctx);
 const char* sp_last_error(const sp_ctx* ctx);  /* ctx may be NULL: message of the last failed sp_ctx_create */
 unsigned long long sp_kernel_launches(void);   /* kernels launched by this library since load */
+/* device blocks freed by the library are kept for reuse by later proofs of this process; this returns them to the driver (e.g. before another
+ * process on the same GPU needs the memory) and gives their size in bytes.  Buffers still held by live objects are not touched. */
+unsigned long long sp_release_cached_memory(void);
 
 /* ---- one proof over several GPUs (SURVEY.md 8(e); the reference is single-process, the loops being sharded are dense_mlpoly.rs:215-223,
  * sumcheck.rs:290-357 / :460-469 / :625-652, dense_mlpoly.rs:165-177, product_tree.rs:18-56).  One process per GPU, one context per process.

@@ -34,6 +34,7 @@ def _load():
 lib = _load()
 lib.sp_last_error.restype = C.c_char_p
 lib.sp_kernel_launches.restype = C.c_ulonglong
+lib.sp_release_cached_memory.restype = C.c_ulonglong
 lib.sp_poly_len.restype = C.c_size_t
 lib.sp_points_len.restype = C.c_size_t
 _vp, _sz = C.c_void_p, C.c_size_t
@@ -41,6 +42,11 @@ _vp, _sz = C.c_void_p, C.c_size_t
 
 def kernel_launches():
     return int(lib.sp_kernel_launches())
+
+
+def release_cached_memory():
+    """return the device blocks this process keeps for reuse to the driver (drop the Python objects first); bytes released"""
+    return int(lib.sp_release_cached_memory())
 
 
 def _p(a):

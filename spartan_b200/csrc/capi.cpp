@@ -53,6 +53,7 @@ int sp_ctx_create(int device, sp_ctx** out) {
 void sp_ctx_destroy(sp_ctx* ctx) { delete ctx; }
 const char* sp_last_error(const sp_ctx* ctx) { return ctx ? ctx->c.last_error.c_str() : g_create_error.c_str(); }
 unsigned long long sp_kernel_launches(void) { return dev::launch_count(); }
+unsigned long long sp_release_cached_memory(void) { return dev::pool_release_cached(); }
 int sp_timings(sp_ctx* ctx, char* buf, size_t buflen) {
   std::ostringstream os;
   for (auto& t : ctx->c.timings) os << t.first << "=" << t.second << ";";

@@ -26,6 +26,7 @@ void stream_sync(cudaStream_t s);
 // cudaMalloc / cudaFree (which synchronises the device) would otherwise cost milliseconds per proof
 void* pool_alloc(size_t bytes);
 void pool_free(void* p);
+size_t pool_release_cached();   // cudaFree every cached free block; returns their bytes
 void* hmalloc_pinned(size_t bytes);
 void hfree_pinned(void* p);
 void h2d(void* d, const void* h, size_t bytes, cudaStream_t s);

@@ -96,7 +96,17 @@ size_t pool_round(size_t b) {
   const size_t g = 2u << 20;                   // 2 MiB granularity above 1 MiB
   return (b + g - 1) / g * g;
 }
+size_t drop_cached_locked() {   // caller holds g_pool_mu
+  size_t bytes = 0;
+  for (auto& kv : g_pool_free) { bytes += kv.first.second; cudaFree(kv.second); }
+  g_pool_free.clear();
+  return bytes;
+}
 }  // namespace
+size_t pool_release_cached() {
+  std::lock_guard<std::mutex> lk(g_pool_mu);
+  return drop_cached_locked();
+}
 void* pool_alloc(size_t bytes) {
   size_t r = pool_round(bytes);
   int dev = 0;
@@ -109,8 +119,7 @@ void* pool_alloc(size_t bytes) {
     cudaError_t e = cudaMalloc(&p, r);
     if (e != cudaSuccess) {  // out of memory: drop the cache and retry once
       cudaGetLastError();
-      for (auto& kv : g_pool_free) cudaFree(kv.second);
-      g_pool_free.clear();
+      drop_cached_locked();
       ck(cudaMalloc(&p, r), "cudaMalloc");
     }
   }

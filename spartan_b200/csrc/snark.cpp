@@ -54,6 +54,9 @@ void snark_encode(Ctx& ctx, const Instance& inst, const SnarkGens& gens, SnarkEn
   e.batch_size = 3;
   size_t N = 1;
   for (int m = 0; m < 3; m++) N = std::max(N, next_pow2(inst.M[m].row.size()));
+  // every product circuit of the memory check has log2(N) layers and the proof binds its last one: with at most one entry per matrix there is
+  // none (the reference panics in ProductCircuit::evaluate)
+  if (N < 2) throw SpError(SP_ERR_INVALID_ARG, "SNARK::encode needs a matrix with at least two entries (num_ops = 1 leaves the product circuits without layers)");
   size_t x = log2_ceil(inst.num_cons), y = log2_ceil(2 * inst.num_vars);
   size_t cells = (size_t)1 << std::max(x, y);
   e.num_ops = N; e.num_mem_cells = cells;

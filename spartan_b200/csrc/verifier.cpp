@@ -553,9 +553,11 @@ void nizk_verify(Ctx& ctx, const Instance& inst, const std::vector<Fq>& input, c
 // SNARK::verify (lib.rs:423-465); `comm` supplies the ComputationCommitment
 void snark_verify(Ctx& ctx, const SnarkEncoding& comm, const std::vector<Fq>& input, const SnarkGens& gens, Transcript& T, const uint8_t* proof, size_t len) {
   check_dims(comm.num_cons, comm.num_vars, comm.num_inputs);
-  {  // SparseMatPolyCommitment consistency (sparse_mlpoly.rs:366-420): 3 matrices, power-of-two op count, cells = max(num_cons, 2*num_vars)
+  {  // SparseMatPolyCommitment consistency (sparse_mlpoly.rs:366-420): 3 matrices, power-of-two op count of at least 2 (what snark_encode
+     // produces: one op leaves the product circuits without layers), cells = max(num_cons, 2*num_vars)
     const size_t cells = std::max(comm.num_cons, 2 * comm.num_vars);
-    if (comm.batch_size != 3 || !pow2(comm.num_ops) || comm.num_mem_cells != cells) throw SpError(SP_ERR_INVALID_ARG, "verifier: inconsistent computation commitment");
+    if (comm.batch_size != 3 || !pow2(comm.num_ops) || comm.num_ops < 2 || comm.num_mem_cells != cells)
+      throw SpError(SP_ERR_INVALID_ARG, "verifier: inconsistent computation commitment");
   }
   Reader r(proof, len);
   R1CSProof sat;
