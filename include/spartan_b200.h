@@ -91,6 +91,10 @@ int sp_scalar_invert(const uint64_t a[4], uint64_t out[4]);                     
 /* ---- dense multilinear polynomials on the device */
 int sp_poly_upload(sp_ctx* ctx, const uint64_t* limbs_mont, size_t len, sp_poly** out);   /* DensePolynomial::new   dense_mlpoly.rs:121 */
 int sp_poly_download(sp_ctx* ctx, const sp_poly* p, uint64_t* limbs_mont, size_t len);
+/* n canonical little-endian 32-byte scalars in DEVICE memory of the context's GPU (e.g. a witness computed there) -> a polynomial in Montgomery
+ * form, for sp_*_prove_resident.  SP_ERR_INVALID_SCALAR if a value is >= q, SP_ERR_INVALID_ARG if the pointer is not device memory of the
+ * context's device.  Same synchronisation rules as sp_instance_create_device. */
+int sp_poly_from_canonical_device(sp_ctx* ctx, const uint8_t* d_canonical32, size_t n, sp_poly** out);
 size_t sp_poly_len(const sp_poly* p);
 void sp_poly_free(sp_poly* p);
 /* bound_poly_var_top on k polynomials of equal length                                      dense_mlpoly.rs:215-223 */
@@ -163,6 +167,14 @@ int sp_ipa_finish(sp_ctx* ctx, sp_ipa* h, uint64_t a_hat_mont[4], uint64_t b_hat
 int sp_instance_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, const uint64_t* A_row, const uint64_t* A_col, const uint8_t* A_val32,
                        size_t nA, const uint64_t* B_row, const uint64_t* B_col, const uint8_t* B_val32, size_t nB, const uint64_t* C_row, const uint64_t* C_col,
                        const uint8_t* C_val32, size_t nC, sp_instance** out);
+/* the same with every array in DEVICE memory on the context's GPU (e.g. CUDA tensors, a Rust caller's own device buffers): same padding, input-column
+ * remap, error codes and messages; the first bad entry in (matrix, entry) order is reported, row before column before scalar.  A pointer that is
+ * not device memory of the context's device (an array with zero entries is not looked at) gives SP_ERR_INVALID_ARG.  The arrays must be fully
+ * written before the call (synchronise the stream that wrote them); the call returns only after it has finished reading them.  The instance
+ * keeps no host copy of the matrices until sp_instance_bincode / sp_instance_digest / sp_instance_export asks for one. */
+int sp_instance_create_device(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, const uint64_t* A_row, const uint64_t* A_col,
+                              const uint8_t* A_val32, size_t nA, const uint64_t* B_row, const uint64_t* B_col, const uint8_t* B_val32, size_t nB,
+                              const uint64_t* C_row, const uint64_t* C_col, const uint8_t* C_val32, size_t nC, sp_instance** out);
 /* Instance::produce_synthetic_r1cs with the OsRng replaced by the seeded SHAKE256 generator of DESIGN.md.
  * vars_out: num_vars*4 limbs, inputs_out: num_inputs*4 limbs (Montgomery) */
 int sp_instance_synthetic(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, uint64_t seed, sp_instance** out, uint64_t* vars_out,

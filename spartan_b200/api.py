@@ -173,6 +173,32 @@ def random_tape_seed():
     return out
 
 
+# ----------------------------------------------------------------------------- device arrays from torch
+def _torch():
+    import torch   # only the tensor entry points need torch: the module imports without it
+    return torch
+
+
+def _device_tensor(t, ctx, name, dtype, width=None):
+    """t as a contiguous tensor of `dtype` on ctx.device: 1-D, or (n, width) when width is given"""
+    torch = _torch()
+    if not isinstance(t, torch.Tensor):
+        raise SpartanB200Error("%s: expected a torch.Tensor, got %s" % (name, type(t).__name__))
+    if t.device.type != "cuda" or t.device.index != ctx.device:
+        raise SpartanB200Error("%s: expected a tensor on cuda:%d, got one on %s" % (name, ctx.device, t.device))
+    if t.dtype != dtype:
+        raise SpartanB200Error("%s: expected dtype %s, got %s" % (name, dtype, t.dtype))
+    if (width is None and t.dim() != 1) or (width is not None and (t.dim() != 2 or t.shape[1] != width)):
+        raise SpartanB200Error("%s: expected shape %s, got %s" % (name, "(n,)" if width is None else "(n, %d)" % width, tuple(t.shape)))
+    return t.contiguous()
+
+
+def _sync_torch(ctx):
+    """the library reads the tensors on its own stream: whatever torch queued to write them must have finished"""
+    torch = _torch()
+    torch.cuda.current_stream(ctx.device).synchronize()
+
+
 # ----------------------------------------------------------------------------- operator level
 class DensePolynomial:
     """dense_mlpoly.rs:18-22 with Z resident on the device"""
@@ -189,6 +215,17 @@ class DensePolynomial:
         o = cls.__new__(cls)
         o.ctx, o.h = ctx, h
         return o
+
+    @classmethod
+    def from_tensor(cls, vals, ctx=None):
+        """Z from a (n, 32) uint8 CUDA tensor of canonical little-endian scalars on ctx.device (e.g. a witness computed by torch), converted to
+        Montgomery form on the device; raises R1CSError (InvalidScalar) if a value is >= q"""
+        ctx = ctx or default_context()
+        vals = _device_tensor(vals, ctx, "vals", _torch().uint8, 32)
+        _sync_torch(ctx)
+        h = _vp()
+        ctx.check(lib.sp_poly_from_canonical_device(ctx.h, _vp(vals.data_ptr()), _sz(vals.shape[0]), C.byref(h)))
+        return cls._wrap(ctx, h)
 
     def len(self):
         return int(lib.sp_poly_len(self.h))
@@ -511,6 +548,31 @@ class Instance:
         h = _vp()
         ctx.check(lib.sp_instance_create(ctx.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), _p(a[0]), _p(a[1]), C.c_char_p(a[2]), _sz(a[3]),
                                          _p(b[0]), _p(b[1]), C.c_char_p(b[2]), _sz(b[3]), _p(c[0]), _p(c[1]), C.c_char_p(c[2]), _sz(c[3]), C.byref(h)))
+        return Instance(ctx, h)
+
+    @staticmethod
+    def from_tensors(num_cons, num_vars, num_inputs, A, B, Cm, ctx=None):
+        """Instance::new from CUDA tensors on ctx.device, built there: A/B/C are (rows, cols, vals) with rows and cols int64 of length nnz and vals
+        uint8 of shape (nnz, 32), canonical little-endian scalars.  Same checks, padding, errors and instance as Instance.new; the matrices stay
+        on the device (bincode / digest / export download them on first use)."""
+        ctx = ctx or default_context()
+        torch = _torch()
+        mats = []
+        for mname, M in zip("ABC", (A, B, Cm)):
+            if not isinstance(M, (tuple, list)) or len(M) != 3:
+                raise SpartanB200Error("%s: expected a (rows, cols, vals) triple" % mname)
+            rows = _device_tensor(M[0], ctx, mname + " rows", torch.int64)
+            cols = _device_tensor(M[1], ctx, mname + " cols", torch.int64)
+            vals = _device_tensor(M[2], ctx, mname + " vals", torch.uint8, 32)
+            if not rows.shape[0] == cols.shape[0] == vals.shape[0]:
+                raise SpartanB200Error("%s: rows, cols and vals differ in length (%d, %d, %d)" % (mname, rows.shape[0], cols.shape[0], vals.shape[0]))
+            mats.append((rows, cols, vals))
+        _sync_torch(ctx)
+        args = []
+        for rows, cols, vals in mats:
+            args += [_vp(rows.data_ptr()), _vp(cols.data_ptr()), _vp(vals.data_ptr()), _sz(rows.shape[0])]
+        h = _vp()
+        ctx.check(lib.sp_instance_create_device(ctx.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), *args, C.byref(h)))
         return Instance(ctx, h)
 
     @staticmethod

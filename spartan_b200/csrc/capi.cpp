@@ -574,38 +574,96 @@ int sp_msm_var_resident(sp_ctx* ctx, const sp_points* p, size_t offset, const sp
 // ---- instances
 static size_t next_pow2(size_t x) { size_t p = 1; while (p < x) p <<= 1; return p; }
 
-int sp_instance_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, const uint64_t* A_row, const uint64_t* A_col, const uint8_t* A_val,
-                       size_t nA, const uint64_t* B_row, const uint64_t* B_col, const uint8_t* B_val, size_t nB, const uint64_t* C_row, const uint64_t* C_col,
-                       const uint8_t* C_val, size_t nC, sp_instance** out) {
-  SP_TRY(ctx)
-  // Instance::new padding rules (lib.rs:129-198)
+// Instance::new (lib.rs:129-198) from arrays in device memory: padding rules, checks, input-column remap and Montgomery form on the device, then
+// the CSR / CSC copies.  The caller's arrays are read by the ingestion kernel only, which has finished when this returns or throws.
+static sp_instance* instance_from_device(Ctx& c, size_t num_cons, size_t num_vars, size_t num_inputs, const dev::CooIn& in) {
   size_t num_vars_padded = next_pow2(std::max(num_vars, num_inputs + 1));
   size_t num_cons_padded = num_cons;
   if (num_cons_padded == 0 || num_cons_padded == 1) num_cons_padded = 2;
   if (next_pow2(num_cons) != num_cons) num_cons_padded = next_pow2(num_cons);
   std::unique_ptr<sp_instance> I(new sp_instance);
   I->inst.num_cons = num_cons_padded; I->inst.num_vars = num_vars_padded; I->inst.num_inputs = num_inputs;
+  const bool pad = num_cons == 0 || num_cons == 1;   // lib.rs: fewer than two constraints get padding entries (row i, column num_vars, 0)
+  dev::CooOut co;
+  for (int m = 0; m < 3; m++) {
+    SparseMatDev& M = I->inst.M[m];
+    M.nnz = in.n[m] + (pad && in.n[m] < num_cons_padded ? num_cons_padded - in.n[m] : 0);
+    M.coo_row.alloc(M.nnz); M.coo_col.alloc(M.nnz); M.coo_val.alloc(M.nnz);
+    co.row[m] = M.coo_row.p; co.col[m] = M.coo_col.p; co.val[m] = M.coo_val.p;
+  }
+  DevBuf<unsigned long long> err(1);
+  dev::set_max_u64(err.p, c.stream);
+  dev::inst_ingest(in, co, num_cons, num_vars, num_inputs, num_vars_padded, err.p, c.stream);
+  unsigned long long first = 0;
+  dev::d2h(&first, err.p, sizeof(first), c.stream);
+  c.sync();
+  if (first != ~0ull) {   // the first bad entry in (matrix, entry) order; within it row, then column, then scalar
+    const unsigned code = (unsigned)(first & 3);
+    if (code == dev::INGEST_ROW) throw SpError(SP_ERR_INVALID_INDEX, "R1CSError::InvalidIndex (row)");
+    if (code == dev::INGEST_COL) throw SpError(SP_ERR_INVALID_INDEX, "R1CSError::InvalidIndex (col)");
+    throw SpError(SP_ERR_INVALID_SCALAR, "R1CSError::InvalidScalar");
+  }
+  for (int m = 0; m < 3; m++)
+    if (pad) dev::inst_pad_rows(co.row[m], co.col[m], co.val[m], in.n[m], I->inst.M[m].nnz, (uint32_t)num_vars, c.stream);
+  I->inst.finalize(&c);
+  return I.release();
+}
+
+int sp_instance_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, const uint64_t* A_row, const uint64_t* A_col, const uint8_t* A_val,
+                       size_t nA, const uint64_t* B_row, const uint64_t* B_col, const uint8_t* B_val, size_t nB, const uint64_t* C_row, const uint64_t* C_col,
+                       const uint8_t* C_val, size_t nC, sp_instance** out) {
+  SP_TRY(ctx)
+  // the host arrays go to the device as they are and meet the same checks as sp_instance_create_device's
   const uint64_t* rows[3] = {A_row, B_row, C_row};
   const uint64_t* cols[3] = {A_col, B_col, C_col};
   const uint8_t* vals[3] = {A_val, B_val, C_val};
-  size_t nn[3] = {nA, nB, nC};
+  const size_t nn[3] = {nA, nB, nC};
+  DevBuf<uint64_t> d_row[3], d_col[3];
+  DevBuf<uint8_t> d_val[3];
+  dev::CooIn in;
   for (int m = 0; m < 3; m++) {
-    SparseMatDev& M = I->inst.M[m];
-    for (size_t k = 0; k < nn[m]; k++) {
-      size_t row = rows[m][k], col = cols[m][k];
-      if (row >= num_cons) throw SpError(SP_ERR_INVALID_INDEX, "R1CSError::InvalidIndex (row)");
-      if (col >= num_vars + 1 + num_inputs) throw SpError(SP_ERR_INVALID_INDEX, "R1CSError::InvalidIndex (col)");
-      const uint8_t* vb = vals[m] + 32 * k;
-      if (!fq_bytes_canonical(vb)) throw SpError(SP_ERR_INVALID_SCALAR, "R1CSError::InvalidScalar");
-      M.row.push_back((uint32_t)row);
-      M.col.push_back((uint32_t)(col >= num_vars ? col + num_vars_padded - num_vars : col));
-      M.val.push_back(Fq(fq_to_mont(bytes_to_u256(vb))));
-    }
-    if (num_cons == 0 || num_cons == 1)
-      for (size_t i = nn[m]; i < num_cons_padded; i++) { M.row.push_back((uint32_t)i); M.col.push_back((uint32_t)num_vars); M.val.push_back(Fq::zero()); }
+    d_row[m].alloc(nn[m]); d_col[m].alloc(nn[m]); d_val[m].alloc(32 * nn[m]);
+    dev::h2d(d_row[m].p, rows[m], nn[m] * sizeof(uint64_t), ctx->c.stream);
+    dev::h2d(d_col[m].p, cols[m], nn[m] * sizeof(uint64_t), ctx->c.stream);
+    dev::h2d(d_val[m].p, vals[m], 32 * nn[m], ctx->c.stream);
+    in.row[m] = d_row[m].p; in.col[m] = d_col[m].p; in.val[m] = d_val[m].p; in.n[m] = nn[m];
   }
-  I->inst.finalize(&ctx->c);
-  *out = I.release();
+  *out = instance_from_device(ctx->c, num_cons, num_vars, num_inputs, in);
+  SP_CATCH(ctx)
+}
+
+static void require_device(const Ctx& c, const void* p, size_t n, const char* what) {
+  if (n && !dev::is_device_pointer(p, c.device))
+    throw SpError(SP_ERR_INVALID_ARG, std::string(what) + ": not device memory of the context's GPU (device " + std::to_string(c.device) + ")");
+}
+int sp_instance_create_device(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, const uint64_t* A_row, const uint64_t* A_col,
+                              const uint8_t* A_val, size_t nA, const uint64_t* B_row, const uint64_t* B_col, const uint8_t* B_val, size_t nB,
+                              const uint64_t* C_row, const uint64_t* C_col, const uint8_t* C_val, size_t nC, sp_instance** out) {
+  SP_TRY(ctx)
+  const dev::CooIn in = {{A_row, B_row, C_row}, {A_col, B_col, C_col}, {A_val, B_val, C_val}, {nA, nB, nC}};
+  static const char* names[3][3] = {{"A_row", "A_col", "A_val"}, {"B_row", "B_col", "B_val"}, {"C_row", "C_col", "C_val"}};
+  for (int m = 0; m < 3; m++) {
+    require_device(ctx->c, in.row[m], in.n[m], names[m][0]);
+    require_device(ctx->c, in.col[m], in.n[m], names[m][1]);
+    require_device(ctx->c, in.val[m], in.n[m], names[m][2]);
+  }
+  *out = instance_from_device(ctx->c, num_cons, num_vars, num_inputs, in);
+  SP_CATCH(ctx)
+}
+
+int sp_poly_from_canonical_device(sp_ctx* ctx, const uint8_t* d_canonical32, size_t n, sp_poly** out) {
+  SP_TRY(ctx)
+  Ctx& c = ctx->c;
+  require_device(c, d_canonical32, n, "poly_from_canonical_device");
+  std::unique_ptr<sp_poly> p(new sp_poly{&c, DevBuf<u256>(n), n});
+  DevBuf<unsigned long long> err(1);
+  dev::set_max_u64(err.p, c.stream);
+  dev::canonical_to_mont(p->d.p, d_canonical32, n, err.p, c.stream);
+  unsigned long long first = 0;
+  dev::d2h(&first, err.p, sizeof(first), c.stream);
+  c.sync();
+  if (first != ~0ull) throw SpError(SP_ERR_INVALID_SCALAR, "R1CSError::InvalidScalar (entry " + std::to_string(first) + ")");
+  *out = p.release();
   SP_CATCH(ctx)
 }
 
@@ -649,6 +707,7 @@ int sp_instance_synthetic(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t 
   }
   // the COO column index space is [vars | 1 | inputs] padded to 2*num_vars: columns >= num_vars need no shift here because
   // produce_synthetic_r1cs requires num_vars to be a power of two already (r1cs.rs:172-176)
+  I->inst.upload_coo(&ctx->c);
   I->inst.finalize(&ctx->c);
   memcpy(vars_out, Z.data(), 32 * num_vars);
   memcpy(inputs_out, Z.data() + num_vars + 1, 32 * num_inputs);
@@ -662,9 +721,11 @@ int sp_instance_dims(const sp_instance* inst, size_t* nc, size_t* nv, size_t* ni
 }
 int sp_instance_set_digest(sp_instance* inst, const uint8_t* digest, size_t len) { inst->inst.digest.assign(digest, digest + len); return SP_OK; }
 int sp_instance_bincode(const sp_instance* inst, uint8_t** out, size_t* len) {
-  std::vector<uint8_t> raw = inst->inst.shape_bincode();
-  *out = dup_bytes(raw); *len = raw.size();
-  return SP_OK;
+  try {
+    std::vector<uint8_t> raw = inst->inst.shape_bincode();
+    *out = dup_bytes(raw); *len = raw.size();
+    return SP_OK;
+  } catch (...) { return SP_ERR_INTERNAL; }
 }
 // R1CSShape::get_digest (r1cs.rs:154-158): the bytes NIZK::prove / verify absorb (lib.rs:514) — the caller's (sp_instance_set_digest) or, by
 // default, this library's miniz-level-6 zlib stream of bincode(shape), computed on first use
@@ -675,13 +736,16 @@ int sp_instance_digest(const sp_instance* inst, uint8_t** out, size_t* len) {
     return SP_OK;
   } catch (...) { return SP_ERR_INTERNAL; }
 }
-int sp_instance_nnz(const sp_instance* inst, int m, size_t* nnz) { if (m < 0 || m > 2) return SP_ERR_INVALID_ARG; *nnz = inst->inst.M[m].row.size(); return SP_OK; }
+int sp_instance_nnz(const sp_instance* inst, int m, size_t* nnz) { if (m < 0 || m > 2) return SP_ERR_INVALID_ARG; *nnz = inst->inst.M[m].nnz; return SP_OK; }
 int sp_instance_export(const sp_instance* inst, int m, uint64_t* row, uint64_t* col, uint64_t* val) {
   if (m < 0 || m > 2) return SP_ERR_INVALID_ARG;
-  const SparseMatDev& M = inst->inst.M[m];
-  for (size_t k = 0; k < M.row.size(); k++) { row[k] = M.row[k]; col[k] = M.col[k]; }
-  memcpy(val, M.val.data(), 32 * M.val.size());
-  return SP_OK;
+  try {
+    inst->inst.host_coo();
+    const SparseMatDev& M = inst->inst.M[m];
+    for (size_t k = 0; k < M.nnz; k++) { row[k] = M.row[k]; col[k] = M.col[k]; }
+    if (M.nnz) memcpy(val, M.val.data(), 32 * M.nnz);
+    return SP_OK;
+  } catch (...) { return SP_ERR_INTERNAL; }
 }
 
 static DevBuf<u256> upload_padded_vars(Ctx& c, const Instance& I, const uint64_t* vars, size_t nvars) {

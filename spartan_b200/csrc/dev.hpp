@@ -115,7 +115,6 @@ void dot3(u256* out, const u256* a, const u256* b, const u256* c, size_t n, void
 void bound_rows(u256* out, const u256* Z, const u256* L, size_t L_size, size_t R_size, u256* scratch /* >= 64*R_size */, cudaStream_t s);
 void lincomb3(u256* out, const u256* A, const u256* B, const u256* C, const u256* d_rabc /*3*/, size_t n, cudaStream_t s);
 void hadamard_many(u256* const* outs, const u256* const* as, const u256* const* bs, int count, size_t n, cudaStream_t s);
-void from_u64(u256* out, const uint64_t* v, size_t n, cudaStream_t s);
 void to_canonical(u256* out, const u256* in, size_t n, cudaStream_t s);   // Montgomery -> canonical little-endian integers (transcript bytes)
 void gather(u256* out, const u256* mem, const uint32_t* idx, size_t n, cudaStream_t s);
 // hash layer of the SPARK memory check: out = ts*r^2 + val*r + addr - g  (sparse_mlpoly.rs:545-600)
@@ -153,6 +152,32 @@ void wait_peers(const CommDev& c, unsigned int seq, cudaStream_t s);   // return
 void spmv(u256* out, size_t nrows, const uint32_t* ptr, const uint32_t* idx, const u256* val, const u256* x, cudaStream_t s);
 // sum_k trx[row_k]*try[col_k]*val_k
 void sparse_eval3(u256* out, const uint32_t* row, const uint32_t* col, const u256* val, size_t nnz, const u256* trx, const u256* try_, void* scratch, cudaStream_t s);
+
+// ---- instance ingestion (kernels_inst.cu)
+bool is_device_pointer(const void* p, int device);   // memory allocated on `device` (cudaMemoryTypeDevice)
+void set_max_u64(unsigned long long* w, cudaStream_t s);
+void d2h_sync(void* h, const void* d, size_t bytes);  // blocking copy outside any stream's order (data no pending work writes)
+// Instance::new (lib.rs:129-198) entries of A, B, C from caller arrays: row < num_cons, col < num_vars + 1 + num_inputs, value < q; columns from
+// num_vars on move up by num_vars_padded - num_vars; values to Montgomery form.  The first bad entry in (matrix, entry, row/col/scalar) order
+// wins: *err = min over bad entries of ((m << 40 | k) << 2) | code (*err = ~0 beforehand: none)
+enum { INGEST_ROW = 0, INGEST_COL = 1, INGEST_SCALAR = 2 };
+struct CooIn { const uint64_t* row[3]; const uint64_t* col[3]; const uint8_t* val[3]; size_t n[3]; };
+struct CooOut { uint32_t* row[3]; uint32_t* col[3]; u256* val[3]; };
+void inst_ingest(const CooIn& in, const CooOut& out, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_vars_padded, unsigned long long* err,
+                 cudaStream_t s);
+// entries [from, to) = (row i, column pad_col, value 0): the padding of an instance with fewer than two constraints
+void inst_pad_rows(uint32_t* row, uint32_t* col, u256* val, size_t from, size_t to, uint32_t pad_col, cudaStream_t s);
+// n canonical 32-byte scalars -> Montgomery form; *err = smallest index of a value >= q (*err = ~0 beforehand: none)
+void canonical_to_mont(u256* out, const uint8_t* in32, size_t n, unsigned long long* err, cudaStream_t s);
+// CSR (major = row) or CSC (major = column) copy of a COO matrix: ptr[nmajor + 1], idx / v[nnz] in stable order of the major index
+size_t compress_scratch_bytes(size_t nmajor, size_t nnz);
+void build_compressed(uint32_t* ptr, uint32_t* idx, u256* v, size_t nmajor, const uint32_t* major, const uint32_t* minor, const u256* val, size_t nnz,
+                      void* scratch, cudaStream_t s);
+// AddrTimestamps::new (sparse_mlpoly.rs:220-254), one side: the addresses src[m][0..nnz[m]) zero-padded to N -> idx[m] (N each) and, as field
+// elements over the 3N positions (matrix-major), addr_f, ts_f (read_ts) and audit_f (cells); *bad |= 1 when an address is >= cells
+struct SparkAddrs { const uint32_t* src[3]; size_t nnz[3]; uint32_t* idx[3]; };
+size_t spark_ts_scratch_bytes(size_t N, size_t cells);
+void spark_timestamps(const SparkAddrs& sa, u256* addr_f, u256* ts_f, u256* audit_f, size_t N, size_t cells, void* scratch, unsigned int* bad, cudaStream_t s);
 
 // ---- group: generators, fixed-base window tables, multi-row MSM, compression (K3/K4/K6)
 void gens_from_uniform(ge* out, const uint8_t* d_uniform64, size_t n, cudaStream_t s);

@@ -336,13 +336,6 @@ void hadamard_many(u256* const* outs, const u256* const* as, const u256* const* 
   k_hadamard_many<<<grid, 256, 0, s>>>(hb, n);
   SP_LAUNCHED(); check("hadamard_many");
 }
-__global__ void k_from_u64(u256* out, const uint64_t* __restrict__ v, size_t n) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) st256(out + i, fq_from_u64(v[i]));
-}
-void from_u64(u256* out, const uint64_t* v, size_t n, cudaStream_t s) {
-  k_from_u64<<<grid_for(n, 256, 8), 256, 0, s>>>(out, v, n);
-  SP_LAUNCHED(); check("from_u64");
-}
 __global__ void k_to_canonical(u256* out, const u256* __restrict__ in, size_t n) {   // Scalar::to_bytes (ristretto255.rs:419) for a whole vector
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) st256(out + i, fq_from_mont(ld256_ro(in + i)));
 }

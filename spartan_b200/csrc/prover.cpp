@@ -762,22 +762,34 @@ void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt
 }
 
 // ================================================================================================ instance
-static void build_compressed(size_t nmajor, const std::vector<uint32_t>& major, const std::vector<uint32_t>& minor, const std::vector<Fq>& val,
-                             std::vector<uint32_t>& ptr, std::vector<uint32_t>& idx, std::vector<Fq>& v) {
-  size_t nnz = major.size();
-  ptr.assign(nmajor + 1, 0);
-  for (size_t k = 0; k < nnz; k++) ptr[major[k] + 1]++;
-  for (size_t i = 0; i < nmajor; i++) ptr[i + 1] += ptr[i];
-  std::vector<uint32_t> fill(ptr.begin(), ptr.end() - 1);
-  idx.resize(nnz); v.resize(nnz);
-  for (size_t k = 0; k < nnz; k++) { uint32_t p = fill[major[k]]++; idx[p] = minor[k]; v[p] = val[k]; }
-}
 template <class T>
 static void up(Ctx* ctx, DevBuf<T>& d, const std::vector<T>& h) { d.alloc(h.size()); dev::h2d(d.p, h.data(), h.size() * sizeof(T), ctx->stream); }
 static void up(Ctx* ctx, DevBuf<u256>& d, const std::vector<Fq>& h) { d.alloc(h.size()); dev::h2d(d.p, h.data(), h.size() * sizeof(u256), ctx->stream); }
 
+void Instance::host_coo() const {
+  std::lock_guard<std::mutex> lk(host_mu);
+  if (host_ready) return;
+  for (int m = 0; m < 3; m++) {   // finalize has synchronised the stream that wrote the COO: a blocking copy outside its order is safe
+    const SparseMatDev& S = M[m];
+    S.row.resize(S.nnz); S.col.resize(S.nnz); S.val.resize(S.nnz);
+    dev::d2h_sync(S.row.data(), S.coo_row.p, S.nnz * sizeof(uint32_t));
+    dev::d2h_sync(S.col.data(), S.coo_col.p, S.nnz * sizeof(uint32_t));
+    dev::d2h_sync(S.val.data(), S.coo_val.p, S.nnz * sizeof(u256));
+  }
+  host_ready = true;
+}
+void Instance::upload_coo(Ctx* ctx) {
+  for (int m = 0; m < 3; m++) {
+    SparseMatDev& S = M[m];
+    S.nnz = S.row.size();
+    up(ctx, S.coo_row, S.row); up(ctx, S.coo_col, S.col); up(ctx, S.coo_val, S.val);
+  }
+  host_ready = true;
+}
+
 std::vector<uint8_t> Instance::shape_bincode() const {
   // bincode(R1CSShape{num_cons,num_vars,num_inputs,A,B,C}), SparseMatPolynomial{num_vars_x,num_vars_y,M:Vec<{row,col,val}>} (r1cs.rs:19-26, sparse_mlpoly.rs:19-37)
+  host_coo();
   Writer w;
   w.u64(num_cons); w.u64(num_vars); w.u64(num_inputs);
   size_t nx = 0, ny = 0;
@@ -796,18 +808,19 @@ const std::vector<uint8_t>& Instance::shape_digest() const {
 }
 
 void Instance::finalize(Ctx* ctx) {
-  size_t ncols = 2 * num_vars;
+  const size_t ncols = 2 * num_vars;
+  size_t scratch = 0;
+  for (int m = 0; m < 3; m++)
+    scratch = std::max(scratch, std::max(dev::compress_scratch_bytes(num_cons, M[m].nnz), dev::compress_scratch_bytes(ncols, M[m].nnz)));
+  DevBuf<uint8_t> tmp(scratch);
   for (int m = 0; m < 3; m++) {
-    SparseMatDev& M_ = M[m];
-    std::vector<uint32_t> ptr, idx;
-    std::vector<Fq> v;
-    build_compressed(num_cons, M_.row, M_.col, M_.val, ptr, idx, v);
-    up(ctx, M_.csr_ptr, ptr); up(ctx, M_.csr_idx, idx); up(ctx, M_.csr_val, v);
-    build_compressed(ncols, M_.col, M_.row, M_.val, ptr, idx, v);
-    up(ctx, M_.csc_ptr, ptr); up(ctx, M_.csc_idx, idx); up(ctx, M_.csc_val, v);
-    up(ctx, M_.coo_row, M_.row); up(ctx, M_.coo_col, M_.col); up(ctx, M_.coo_val, M_.val);
-    ctx->sync();
+    SparseMatDev& S = M[m];
+    S.csr_ptr.alloc(num_cons + 1); S.csr_idx.alloc(S.nnz); S.csr_val.alloc(S.nnz);
+    S.csc_ptr.alloc(ncols + 1); S.csc_idx.alloc(S.nnz); S.csc_val.alloc(S.nnz);
+    dev::build_compressed(S.csr_ptr.p, S.csr_idx.p, S.csr_val.p, num_cons, S.coo_row.p, S.coo_col.p, S.coo_val.p, S.nnz, tmp.p, ctx->stream);
+    dev::build_compressed(S.csc_ptr.p, S.csc_idx.p, S.csc_val.p, ncols, S.coo_col.p, S.coo_row.p, S.coo_val.p, S.nnz, tmp.p, ctx->stream);
   }
+  ctx->sync();
 }
 
 // ================================================================================================ R1CSProof::prove

@@ -3,6 +3,7 @@
 #pragma once
 #include <functional>
 #include <array>
+#include <mutex>
 #include "engine.hpp"
 
 namespace sp {
@@ -94,11 +95,12 @@ struct R1CSGens {  // r1csproof.rs:39-74
 };
 
 // ---- instance
-struct SparseMatDev {  // one of A, B, C: COO on host (reference order), CSR + CSC on device
-  std::vector<uint32_t> row, col;
-  std::vector<Fq> val;
+struct SparseMatDev {  // one of A, B, C: COO (reference order), CSR and CSC on the device; a host copy of the COO only when asked for
+  size_t nnz = 0;
   DevBuf<uint32_t> csr_ptr, csr_idx, csc_ptr, csc_idx, coo_row, coo_col;
   DevBuf<u256> csr_val, csc_val, coo_val;
+  mutable std::vector<uint32_t> row, col;   // host COO: see Instance::host_coo
+  mutable std::vector<Fq> val;
 };
 struct Instance {  // lib.rs:111-114 (R1CSShape + digest)
   size_t num_cons = 0, num_vars = 0, num_inputs = 0;
@@ -108,7 +110,14 @@ struct Instance {  // lib.rs:111-114 (R1CSShape + digest)
   mutable std::vector<uint8_t> digest;
   std::vector<uint8_t> shape_bincode() const;
   const std::vector<uint8_t>& shape_digest() const;
-  void finalize(Ctx* ctx);  // build the device copies
+  // The device COO is authoritative.  The host copy is filled by one download on first use (the digest, export): a caller that only proves
+  // SNARKs never moves the matrices to the host.  An instance built on the host (upload_coo) keeps its host copy from the start.
+  void host_coo() const;
+  void upload_coo(Ctx* ctx);   // host row / col / val -> device COO, nnz
+  void finalize(Ctx* ctx);     // CSR and CSC from the device COO (returns once they are built)
+ private:
+  mutable bool host_ready = false;
+  mutable std::mutex host_mu;
 };
 
 std::vector<uint8_t> miniz_zlib_level6(const uint8_t* data, size_t len);   // deflate.cpp

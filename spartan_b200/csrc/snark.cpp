@@ -53,7 +53,7 @@ void snark_encode(Ctx& ctx, const Instance& inst, const SnarkGens& gens, SnarkEn
   e.num_cons = inst.num_cons; e.num_vars = inst.num_vars; e.num_inputs = inst.num_inputs;
   e.batch_size = 3;
   size_t N = 1;
-  for (int m = 0; m < 3; m++) N = std::max(N, next_pow2(inst.M[m].row.size()));
+  for (int m = 0; m < 3; m++) N = std::max(N, next_pow2(inst.M[m].nnz));
   // every product circuit of the memory check has log2(N) layers and the proof binds its last one: with at most one entry per matrix there is
   // none (the reference panics in ProductCircuit::evaluate)
   if (N < 2) throw SpError(SP_ERR_INVALID_ARG, "SNARK::encode needs a matrix with at least two entries (num_ops = 1 leaves the product circuits without layers)");
@@ -63,40 +63,28 @@ void snark_encode(Ctx& ctx, const Instance& inst, const SnarkGens& gens, SnarkEn
   e.comb_ops.alloc(16 * N);   // row.ops_addr[3] | row.read_ts[3] | col.ops_addr[3] | col.read_ts[3] | val[3] | zero pad  (DensePolynomial::merge)
   e.comb_mem.alloc(2 * cells);
   dev::dzero(e.comb_ops.p, 16 * N * sizeof(u256), ctx.stream);
-  DevBuf<uint64_t> tmp64(std::max(N, cells));
-  std::vector<uint64_t> audit(cells), rts(N), addr64(N);
+  DevBuf<uint8_t> scratch(dev::spark_ts_scratch_bytes(N, cells));
+  DevBuf<unsigned int> bad(1);
+  dev::dzero(bad.p, sizeof(unsigned int), ctx.stream);
   for (int side = 0; side < 2; side++) {  // AddrTimestamps::new (sparse_mlpoly.rs:220-254), row then col
-    std::fill(audit.begin(), audit.end(), 0);
     AddrTimestampsDev& at = side == 0 ? e.row : e.col;
     at.ops_addr_idx.resize(3);
+    dev::SparkAddrs sa;
     for (int m = 0; m < 3; m++) {
-      const std::vector<uint32_t>& src = side == 0 ? inst.M[m].row : inst.M[m].col;
-      std::vector<uint32_t> a32(N, 0);
-      std::copy(src.begin(), src.end(), a32.begin());
-      for (size_t i = 0; i < N; i++) {
-        size_t a = a32[i];
-        if (a >= cells) throw SpError(SP_ERR_INVALID_INDEX, "address out of range");
-        rts[i] = audit[a];
-        audit[a] += 1;
-        addr64[i] = a;
-      }
       at.ops_addr_idx[m].alloc(N);
-      dev::h2d(at.ops_addr_idx[m].p, a32.data(), N * sizeof(uint32_t), ctx.stream);
-      u256* d_addr = e.comb_ops.p + (size_t)(side * 6 + m) * N;
-      u256* d_rts = e.comb_ops.p + (size_t)(side * 6 + 3 + m) * N;
-      dev::h2d(tmp64.p, addr64.data(), N * 8, ctx.stream);
-      dev::from_u64(d_addr, tmp64.p, N, ctx.stream);
-      dev::h2d(tmp64.p, rts.data(), N * 8, ctx.stream);
-      dev::from_u64(d_rts, tmp64.p, N, ctx.stream);
-      ctx.sync();
+      sa.src[m] = side == 0 ? inst.M[m].coo_row.p : inst.M[m].coo_col.p;
+      sa.nnz[m] = inst.M[m].nnz;
+      sa.idx[m] = at.ops_addr_idx[m].p;
     }
-    dev::h2d(tmp64.p, audit.data(), cells * 8, ctx.stream);
-    dev::from_u64(e.comb_mem.p + (size_t)side * cells, tmp64.p, cells, ctx.stream);
-    ctx.sync();
+    // ops_addr[3] | read_ts[3] of this side are contiguous in comb_ops: position m*N + i of the loop's order is element m*N + i of each block
+    dev::spark_timestamps(sa, e.comb_ops.p + (size_t)side * 6 * N, e.comb_ops.p + (size_t)(side * 6 + 3) * N, e.comb_mem.p + (size_t)side * cells, N, cells,
+                          scratch.p, bad.p, ctx.stream);
   }
-  for (int m = 0; m < 3; m++)
-    dev::h2d(e.comb_ops.p + (size_t)(12 + m) * N, inst.M[m].val.data(), inst.M[m].val.size() * sizeof(u256), ctx.stream);
+  for (int m = 0; m < 3; m++) dev::d2d(e.comb_ops.p + (size_t)(12 + m) * N, inst.M[m].coo_val.p, inst.M[m].nnz * sizeof(u256), ctx.stream);
+  unsigned int out_of_range = 0;
+  dev::d2h(&out_of_range, bad.p, sizeof(unsigned int), ctx.stream);
   ctx.sync();
+  if (out_of_range) throw SpError(SP_ERR_INVALID_INDEX, "address out of range");
   commit_poly(ctx, e.comb_ops.p, 16 * N, gens.gens_ops, e.comm_comb_ops);
   commit_poly(ctx, e.comb_mem.p, 2 * cells, gens.gens_mem, e.comm_comb_mem);
 }
@@ -517,7 +505,7 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
     dev::h2d(d_chal.p + 32, ry.data(), ry.size() * sizeof(u256), ctx.stream);
     dev::eq_evals(try_.p, d_chal.p + 32, (int)ry.size(), eq_small.p, ctx.stream);
     for (int m = 0; m < 3; m++)
-      dev::sparse_eval3(ctx.small.p + 40 + m, inst.M[m].coo_row.p, inst.M[m].coo_col.p, inst.M[m].coo_val.p, inst.M[m].row.size(), trx.p, try_.p, ctx.red.p, ctx.stream);
+      dev::sparse_eval3(ctx.small.p + 40 + m, inst.M[m].coo_row.p, inst.M[m].coo_col.p, inst.M[m].coo_val.p, inst.M[m].nnz, trx.p, try_.p, ctx.red.p, ctx.stream);
     ctx.get_small(40, inst_evals, 3);
   }
   T.append_scalar("Ar_claim", inst_evals[0]);

@@ -518,7 +518,7 @@ void instance_evaluate(Ctx& ctx, const Instance& inst, const std::vector<Fq>& rx
   dev::h2d(d_chal.p + rx.size(), ry.data(), ry.size() * sizeof(u256), ctx.stream);
   dev::eq_evals(try_.p, d_chal.p + rx.size(), (int)ry.size(), eq_small.p, ctx.stream);
   for (int m = 0; m < 3; m++)
-    dev::sparse_eval3(ctx.small.p + 40 + m, inst.M[m].coo_row.p, inst.M[m].coo_col.p, inst.M[m].coo_val.p, inst.M[m].row.size(), trx.p, try_.p, ctx.red.p, ctx.stream);
+    dev::sparse_eval3(ctx.small.p + 40 + m, inst.M[m].coo_row.p, inst.M[m].coo_col.p, inst.M[m].coo_val.p, inst.M[m].nnz, trx.p, try_.p, ctx.red.p, ctx.stream);
   ctx.get_small(40, out, 3);
 }
 
