@@ -276,7 +276,7 @@ int sp_eq_evals(sp_ctx* ctx, const uint64_t* r, size_t ell, sp_poly** out) {
   SP_TRY(ctx)
   size_t n = (size_t)1 << ell;
   std::unique_ptr<sp_poly> p(new sp_poly{&ctx->c, DevBuf<u256>(n), n});
-  DevBuf<u256> d_r(ell + 1), small(2 * ((size_t)1 << ((ell + 1) / 2)) + 8);
+  DevBuf<u256> d_r(ell + 1), small(dev::eq_evals_scratch(ell));
   dev::h2d(d_r.p, r, ell * 32, ctx->c.stream);
   dev::eq_evals(p->d.p, d_r.p, (int)ell, small.p, ctx->c.stream);
   ctx->c.sync();
@@ -286,7 +286,7 @@ int sp_eq_evals(sp_ctx* ctx, const uint64_t* r, size_t ell, sp_poly** out) {
 int sp_poly_evaluate(sp_ctx* ctx, const sp_poly* p, const uint64_t* r, size_t ell, uint64_t out[4]) {
   SP_TRY(ctx)
   if (p->len != (size_t)1 << ell) throw SpError(SP_ERR_INVALID_ARG, "evaluate: |r| != num_vars");
-  DevBuf<u256> d_r(ell + 1), small(2 * ((size_t)1 << ((ell + 1) / 2)) + 8), eq(p->len);
+  DevBuf<u256> d_r(ell + 1), small(dev::eq_evals_scratch(ell)), eq(p->len);
   dev::h2d(d_r.p, r, ell * 32, ctx->c.stream);
   dev::eq_evals(eq.p, d_r.p, (int)ell, small.p, ctx->c.stream);
   dev::dot(ctx->c.small.p + 32, p->d.p, eq.p, p->len, ctx->c.red.p, ctx->c.stream);
@@ -572,8 +572,6 @@ int sp_msm_var_resident(sp_ctx* ctx, const sp_points* p, size_t offset, const sp
 }
 
 // ---- instances
-static size_t next_pow2(size_t x) { size_t p = 1; while (p < x) p <<= 1; return p; }
-
 // Instance::new (lib.rs:129-198) from arrays in device memory: padding rules, checks, input-column remap and Montgomery form on the device, then
 // the CSR / CSC copies.  The caller's arrays are read by the ingestion kernel only, which has finished when this returns or throws.
 static sp_instance* instance_from_device(Ctx& c, size_t num_cons, size_t num_vars, size_t num_inputs, const dev::CooIn& in) {
@@ -822,9 +820,8 @@ static int nizk_prove_common(sp_ctx* ctx, const sp_instance* inst, const VarsArg
   NizkProof P;
   nizk_prove(ctx->c, inst->inst, d_vars, fq_vec(inputs, ninputs), *gens->g, T, fq_in(seed), P);
   ta.close(T);
-  Writer w;
-  P.ser(w);
-  *proof = dup_bytes(w.out); *proof_len = w.out.size();
+  const std::vector<uint8_t> bytes = to_bincode(P);
+  *proof = dup_bytes(bytes); *proof_len = bytes.size();
   SP_CATCH(ctx)
 }
 int sp_nizk_prove(sp_ctx* ctx, const sp_instance* inst, const uint64_t* vars, size_t nvars, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens,
@@ -860,28 +857,16 @@ int sp_snark_encode(sp_ctx* ctx, const sp_instance* inst, const sp_snark_gens* g
 }
 void sp_snark_encoding_free(sp_snark_encoding* e) { delete e; }
 int sp_snark_commitment_bytes(const sp_snark_encoding* e, uint8_t** out, size_t* len) {
-  Writer w;
-  e->e->ser_commitment(w);
-  *out = dup_bytes(w.out); *len = w.out.size();
+  const std::vector<uint8_t> bytes = to_bincode(e->e->comm);
+  *out = dup_bytes(bytes); *len = bytes.size();
   return SP_OK;
 }
 // a verifier holds only the ComputationCommitment: bincode(ComputationCommitment) -> a handle usable with sp_snark_verify (not with sp_snark_prove)
 int sp_snark_commitment_load(sp_ctx* ctx, const uint8_t* bytes, size_t len, sp_snark_encoding** out) {
   SP_TRY(ctx)
-  size_t pos = 0;
-  auto u64 = [&]() { if (len - pos < 8) throw SpError(SP_ERR_INVALID_ARG, "commitment truncated"); uint64_t x = 0; for (int i = 0; i < 8; i++) x |= (uint64_t)bytes[pos + i] << (8 * i); pos += 8; return x; };
-  auto pts = [&](PolyCommitment& c) {
-    uint64_t k = u64();
-    if (k > (len - pos) / 32) throw SpError(SP_ERR_INVALID_ARG, "commitment truncated");
-    c.C.resize(k);
-    for (auto& p : c.C) { memcpy(p.b, bytes + pos, 32); pos += 32; }
-  };
   std::unique_ptr<sp_snark_encoding> E(new sp_snark_encoding);
   E->e.reset(new SnarkEncoding);
-  SnarkEncoding& e = *E->e;
-  e.num_cons = u64(); e.num_vars = u64(); e.num_inputs = u64(); e.batch_size = u64(); e.num_ops = u64(); e.num_mem_cells = u64();
-  pts(e.comm_comb_ops); pts(e.comm_comb_mem);
-  if (pos != len) throw SpError(SP_ERR_INVALID_ARG, "trailing bytes after the commitment");
+  E->e->comm = from_bincode<ComputationCommitment>(bytes, len, SP_ERR_INVALID_ARG, "computation commitment");
   *out = E.release();
   SP_CATCH(ctx)
 }
@@ -896,10 +881,11 @@ static int snark_prove_common(sp_ctx* ctx, const sp_instance* inst, const sp_sna
   if (!seed) throw SpError(SP_ERR_INVALID_ARG, "tape seed is NULL: draw it from the OS RNG (random.rs:13-15); a fixed seed makes every blind public");
   require_reduced(inputs, ninputs, "inputs"); require_reduced(seed, 1, "tape seed");
   Transcript T = ta.open();
-  Writer w;
-  snark_prove(ctx->c, inst->inst, *enc->e, d_vars, fq_vec(inputs, ninputs), *gens->g, T, fq_in(seed), w);
+  SnarkProof P;
+  snark_prove(ctx->c, inst->inst, *enc->e, d_vars, fq_vec(inputs, ninputs), *gens->g, T, fq_in(seed), P);
   ta.close(T);
-  *proof = dup_bytes(w.out); *proof_len = w.out.size();
+  const std::vector<uint8_t> bytes = to_bincode(P);
+  *proof = dup_bytes(bytes); *proof_len = bytes.size();
   SP_CATCH(ctx)
 }
 int sp_snark_prove(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const uint64_t* vars, size_t nvars, const uint64_t* inputs, size_t ninputs,

@@ -106,7 +106,8 @@ void eq_suffix(u256* levels, const u256* E0, size_t n0, int K, cudaStream_t s);
 void fold_top(u256* const* d_tables, int ntables, size_t len, const u256& r, cudaStream_t s);
 
 // ---- dense polynomial helpers (K7)
-void eq_evals(u256* out, const u256* d_r, int ell, u256* scratch_small /* >= 2*2^ceil(ell/2) */, cudaStream_t s);
+void eq_evals(u256* out, const u256* d_r, int ell, u256* scratch_small /* >= eq_evals_scratch(ell) */, cudaStream_t s);
+inline size_t eq_evals_scratch(size_t ell) { return 2 * ((size_t)1 << ((ell + 1) / 2)) + 8; }   // scalars
 // out[n .. 2n) holds E = eq(r', .); rewrite out[0 .. 2n) as eq((r, r'), .) = [(1 - r) E | r E] in one pass
 void eq_extend_top(u256* out, size_t n, const u256& r, cudaStream_t s);
 void dot(u256* out, const u256* a, const u256* b, size_t n, void* scratch, cudaStream_t s);

@@ -122,8 +122,7 @@ struct ShardScope {   // RAII: sharded proving for the duration of one prove cal
 };
 // eq(r, j*W + rank) = c * eq(r[0 .. ell-log2 W), j): the factor contributed by the last log2(W) variables, which the rank fixes
 inline Fq shard_eq_scale(const std::vector<Fq>& r, int W, int rank) {
-  int logW = 0;
-  while ((1 << logW) < W) logW++;
+  const int logW = (int)log2_ceil(W);
   Fq c = Fq::one();
   for (int k = 0; k < logW; k++) {
     const Fq& rj = r[r.size() - logW + k];

@@ -16,6 +16,9 @@
 
 namespace sp {
 
+inline size_t log2_ceil(size_t x) { size_t l = 0; while (((size_t)1 << l) < x) l++; return l; }   // 0 for x <= 1
+inline size_t next_pow2(size_t x) { return (size_t)1 << log2_ceil(x); }
+
 // ------------------------------------------------------------------------------------------------ scalars
 struct Fq {  // Montgomery-form element, same bytes as the reference's Scalar([u64;4])
   u256 m;

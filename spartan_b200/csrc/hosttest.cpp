@@ -3,6 +3,7 @@
 // Not linked into libspartan_b200.so.
 #include "host.hpp"
 #include "engine.hpp"
+#include "wire.hpp"
 using namespace sp;
 
 namespace sp { void shake256(uint8_t* out, size_t outlen, const uint8_t* in, size_t inlen); }
@@ -166,6 +167,21 @@ void spt_transcript_run(const uint8_t* label, size_t llen, const uint8_t* msgs, 
   t.challenge_bytes("c", out64, 64);
 }
 void spt_shake256(uint8_t* out, size_t outlen, const uint8_t* in, size_t inlen) { sp::shake256(out, outlen, in, inlen); }
+// wire format (wire.hpp): parse one input with Reader under the status code the library uses for it, re-encode it with Writer.  kind 0: a NIZK
+// proof, 1: a SNARK proof, 2: a ComputationCommitment.  *out_len: the capacity of out, then the length of the re-encoding.
+int spt_wire_roundtrip(int kind, const uint8_t* in, size_t len, uint8_t* out, size_t* out_len) {
+  try {
+    std::vector<uint8_t> b;
+    if (kind == 0) b = to_bincode(from_bincode<NizkProof>(in, len, SP_ERR_VERIFY, "proof"));
+    else if (kind == 1) b = to_bincode(from_bincode<SnarkProof>(in, len, SP_ERR_VERIFY, "proof"));
+    else if (kind == 2) b = to_bincode(from_bincode<ComputationCommitment>(in, len, SP_ERR_INVALID_ARG, "computation commitment"));
+    else return SP_ERR_INVALID_ARG;
+    if (b.size() > *out_len) return SP_ERR_INVALID_ARG;
+    memcpy(out, b.data(), b.size());
+    *out_len = b.size();
+    return SP_OK;
+  } catch (const SpError& e) { return e.code; }
+}
 }
 
 namespace sp {

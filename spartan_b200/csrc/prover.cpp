@@ -214,8 +214,7 @@ hge host_commit(const GenSet& gs, const Term* terms, size_t nterms) {
 R1CSGens::R1CSGens(Ctx* ctx, const std::string& label, size_t num_vars) {
   // R1CSGens::new (r1csproof.rs:68-73) -> PolyCommitmentGens::new(log2 num_vars) (dense_mlpoly.rs:31-35) ->
   // DotProductProofGens::new(2^ceil(ell/2)) = MultiCommitGens::new(n+1).split_at(n) (nizk/mod.rs:414-418)
-  size_t ell = 0;
-  while (((size_t)1 << ell) < num_vars) ell++;
+  const size_t ell = log2_ceil(num_vars);
   size_t n = (size_t)1 << (ell - ell / 2);
   set.reset(new GenSet(ctx, label, std::max<size_t>(n + 2, 5), {0, 1, 2, 3, 4, n, n + 1}));  // gens_4 draws 5 points of the same stream
   gens_pc.n = n;
@@ -227,24 +226,44 @@ R1CSGens::R1CSGens(Ctx* ctx, const std::string& label, size_t num_vars) {
 }
 
 // ================================================================================================ small host protocol pieces
-static Cp commit1(const CommitKey& k, const Fq& x, const Fq& blind) {  // impl Commitments for Scalar (commitments.rs:73-78)
+hge commit1(const CommitKey& k, const Fq& x, const Fq& blind) {
   Term t[2] = {{k.off, x}, {k.h, blind}};
-  return compress(host_commit(*k.set, t, 2));
+  return host_commit(*k.set, t, 2);
 }
-static Cp commitv(const CommitKey& k, const std::vector<Fq>& x, const Fq& blind) {  // impl Commitments for [Scalar] (:80-92), small n only
+hge commitv(const CommitKey& k, const std::vector<Fq>& x, const Fq& blind) {
   std::vector<Term> t;
   for (size_t i = 0; i < x.size(); i++) t.push_back({k.off + i, x[i]});
   t.push_back({k.h, blind});
-  return compress(host_commit(*k.set, t.data(), t.size()));
+  return host_commit(*k.set, t.data(), t.size());
+}
+std::vector<Fq> zk_round_weights(const std::vector<Fq>& w, const Fq& r_j, size_t degree) {
+  std::vector<Fq> a(degree + 1);
+  Fq rpow = Fq::one();
+  for (size_t k = 0; k <= degree; k++) {
+    a[k] = w[0] * (k == 0 ? Fq::from_u64(2) : Fq::one()) + w[1] * rpow;
+    rpow *= r_j;
+  }
+  return a;
+}
+void append_claims_phase2(Transcript& T, const std::array<Cp, 4>& c) {
+  T.append_point("comm_Az_claim", c[0].b);
+  T.append_point("comm_Bz_claim", c[1].b);
+  T.append_point("comm_Cz_claim", c[2].b);
+  T.append_point("comm_prod_Az_Bz_claims", c[3].b);
+}
+void append_nizk_head(Transcript& T, const Instance& inst) {
+  T.append_protocol_name("Spartan NIZK proof");
+  const std::vector<uint8_t>& digest = inst.shape_digest();   // computed here unless the caller supplied its own (r1cs.rs:154-158)
+  T.append_message("R1CSShapeDigest", digest.data(), digest.size());
 }
 
 static KnowledgeProof knowledge_prove(const CommitKey& g, Transcript& T, RandomTape& tape, const Fq& x, const Fq& r, Cp& C_out) {  // nizk/mod.rs:27-52
   T.append_protocol_name("knowledge proof");
   Fq t1 = tape.random_scalar("t1"), t2 = tape.random_scalar("t2");
-  C_out = commit1(g, x, r);
+  C_out = compress(commit1(g, x, r));
   T.append_point("C", C_out.b);
   KnowledgeProof p;
-  p.alpha = commit1(g, t1, t2);
+  p.alpha = compress(commit1(g, t1, t2));
   T.append_point("alpha", p.alpha.b);
   Fq c = T.challenge_scalar("c");
   p.z1 = x * c + t1;
@@ -254,8 +273,8 @@ static KnowledgeProof knowledge_prove(const CommitKey& g, Transcript& T, RandomT
 static EqualityProof equality_prove(const CommitKey& g, Transcript& T, RandomTape& tape, const Fq& v1, const Fq& s1, const Fq& v2, const Fq& s2) {  // :88-116
   T.append_protocol_name("equality proof");
   Fq r = tape.random_scalar("r");
-  Cp C1 = commit1(g, v1, s1); T.append_point("C1", C1.b);
-  Cp C2 = commit1(g, v2, s2); T.append_point("C2", C2.b);
+  Cp C1 = compress(commit1(g, v1, s1)); T.append_point("C1", C1.b);
+  Cp C2 = compress(commit1(g, v2, s2)); T.append_point("C2", C2.b);
   EqualityProof p;
   Term t[1] = {{g.h, r}};
   p.alpha = compress(host_commit(*g.set, t, 1));  // r * h
@@ -268,14 +287,14 @@ static ProductProof product_prove(const CommitKey& g, Transcript& T, RandomTape&
                                   const Fq& rZ, Cp& X, Cp& Y, Cp& Z) {  // nizk/mod.rs:159-229
   T.append_protocol_name("product proof");
   Fq b1 = tape.random_scalar("b1"), b2 = tape.random_scalar("b2"), b3 = tape.random_scalar("b3"), b4 = tape.random_scalar("b4"), b5 = tape.random_scalar("b5");
-  X = commit1(g, x, rX); T.append_point("X", X.b);
-  Y = commit1(g, y, rY); T.append_point("Y", Y.b);
-  Z = commit1(g, z, rZ); T.append_point("Z", Z.b);
+  X = compress(commit1(g, x, rX)); T.append_point("X", X.b);
+  Y = compress(commit1(g, y, rY)); T.append_point("Y", Y.b);
+  Z = compress(commit1(g, z, rZ)); T.append_point("Z", Z.b);
   ProductProof p;
-  p.alpha = commit1(g, b1, b2); T.append_point("alpha", p.alpha.b);
-  p.beta = commit1(g, b3, b4); T.append_point("beta", p.beta.b);
+  p.alpha = compress(commit1(g, b1, b2)); T.append_point("alpha", p.alpha.b);
+  p.beta = compress(commit1(g, b3, b4)); T.append_point("beta", p.beta.b);
   // delta = b3*X + b5*h with X = x*G + rX*h (nizk/mod.rs:199-206): same group element as (b3*x)*G + (b3*rX + b5)*h
-  p.delta = commit1(g, b3 * x, b3 * rX + b5);
+  p.delta = compress(commit1(g, b3 * x, b3 * rX + b5));
   T.append_point("delta", p.delta.b);
   Fq c = T.challenge_scalar("c");
   p.z = {b1 + c * x, b2 + c * rX, b3 + c * y, b4 + c * rY, b5 + c * (rZ - rX * y)};
@@ -291,18 +310,18 @@ static DotProductProof dotproduct_prove(const CommitKey& g1, const CommitKey& gn
   size_t n = x_vec.size();
   std::vector<Fq> d_vec = pre ? pre->d_vec : tape.random_vector("d_vec", n);
   Fq r_delta = pre ? pre->r_delta : tape.random_scalar("r_delta"), r_beta = pre ? pre->r_beta : tape.random_scalar("r_beta");
-  Cp Cx = Cx_known ? *Cx_known : commitv(gn, x_vec, blind_x);
+  Cp Cx = Cx_known ? *Cx_known : compress(commitv(gn, x_vec, blind_x));
   T.append_point("Cx", Cx.b);
-  Cp Cy = commit1(g1, y, blind_y);
+  Cp Cy = compress(commit1(g1, y, blind_y));
   T.append_point("Cy", Cy.b);
   T.append_scalars("a", a_vec);
   DotProductProof p;
-  p.delta = pre ? pre->delta : commitv(gn, d_vec, r_delta);
+  p.delta = pre ? pre->delta : compress(commitv(gn, d_vec, r_delta));
   T.append_point("delta", p.delta.b);
   Fq dot = Fq::zero();
   for (size_t i = 0; i < n; i++) dot += a_vec[i] * d_vec[i];
   if (pre) { Term t1[1] = {{g1.off, dot}}; p.beta = compress(hge_add(host_commit(*g1.set, t1, 1), pre->r_beta_h)); }
-  else p.beta = commit1(g1, dot, r_beta);
+  else p.beta = compress(commit1(g1, dot, r_beta));
   T.append_point("beta", p.beta.b);
   Fq c = T.challenge_scalar("c");
   p.z.resize(n);
@@ -465,7 +484,7 @@ static void zk_sumcheck_prove(Ctx& ctx, dev::ScKind kind, const Fq& claim, const
   const std::vector<hge>& bp_h = zp.bp_h;
   const std::vector<hge>& be_h = zp.be_h;
   Fq claim_per_round = claim;
-  Cp comm_claim_per_round = commit1(g1, claim_per_round, blind_claim);
+  Cp comm_claim_per_round = compress(commit1(g1, claim_per_round, blind_claim));
   auto commit_poly_pre = [&](const std::vector<Fq>& coeffs, size_t j) {   // commit(coeffs; blinds_poly[j]; gens_n) = sum coeff_i*G_i + (blinds_poly[j]*h)
     std::vector<Term> t;
     for (size_t i = 0; i < coeffs.size(); i++) t.push_back({gn.off + i, coeffs[i]});
@@ -507,13 +526,7 @@ static void zk_sumcheck_prove(Ctx& ctx, dev::ScKind kind, const Fq& claim, const
     Fq blind = w[0] * blind_sc + w[1] * blinds_evals[j];
     // (the reference also recomputes comm_target from the two decompressed commitments and asserts equality, sumcheck.rs:531/:722;
     //  it is a self-check with no effect on the transcript)
-    std::vector<Fq> a(degree + 1);
-    Fq rpow = Fq::one();
-    for (int i = 0; i <= degree; i++) {
-      Fq a_sc = i == 0 ? Fq::from_u64(2) : Fq::one();
-      a[i] = w[0] * a_sc + w[1] * rpow;
-      rpow *= r_j;
-    }
+    const std::vector<Fq> a = zk_round_weights(w, r_j, degree);
     proof.proofs.push_back(dotproduct_prove(g1, gn, T, tape, poly.coeffs, blinds_poly[j], a, target, blind, &comm_poly, &pre[j]));
     claim_per_round = eval;
     comm_claim_per_round = comm_eval;
@@ -698,15 +711,14 @@ static void dotproduct_log_prove(Ctx& ctx, const PolyCommitmentGens& gens, Trans
   Fq d = tape.random_scalar("d");
   Fq r_delta = tape.random_scalar("r_delta");
   Fq r_beta = tape.random_scalar("r_delta");  // sic: the reference reuses the label (nizk/mod.rs:459)
-  size_t lg_n = 0;
-  while (((size_t)1 << lg_n) < n) lg_n++;
+  const size_t lg_n = log2_ceil(n);
   std::vector<Fq> v1 = tape.random_vector("blinds_vec_1", lg_n), v2 = tape.random_vector("blinds_vec_2", lg_n);
   std::vector<std::pair<Fq, Fq>> blinds_vec;
   for (size_t i = 0; i < lg_n; i++) blinds_vec.push_back({v1[i], v2[i]});
   std::vector<Cp> cx;
   commit_rows_and_compress(ctx, gens.gens_n, d_x, n, 1, n, &blind_x, cx);
   T.append_point("Cx", cx[0].b);
-  Cy_out = commit1(gens.gens_1, y, blind_y);
+  Cy_out = compress(commit1(gens.gens_1, y, blind_y));
   T.append_point("Cy", Cy_out.b);
   Fq r = Fq::zero();
   auto absorb_a = [&]() {   // called by bullet_prove once round 0 is in flight on the device (same transcript order as nizk/mod.rs:475-477)
@@ -727,7 +739,7 @@ static void dotproduct_log_prove(Ctx& ctx, const PolyCommitmentGens& gens, Trans
   proof.delta = compress(hge_add(hge_scalarmul(d.canonical(), g_hat), host_commit(gs, th, 1)));
   T.append_point("delta", proof.delta.b);
   // beta = d*(r*G1) + r_beta*h (gens_1_scaled, nizk/mod.rs:507)
-  proof.beta = commit1(gens.gens_1, d * r, r_beta);
+  proof.beta = compress(commit1(gens.gens_1, d * r, r_beta));
   T.append_point("beta", proof.beta.b);
   Fq c = T.challenge_scalar("c");
   proof.z1 = d + c * y_hat;
@@ -742,7 +754,7 @@ void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt
   size_t ell = r.size(), lv = ell / 2;
   size_t L_size = (size_t)1 << lv, R_size = (size_t)1 << (ell - lv);
   // compute_factored_evals (dense_mlpoly.rs:90-98) on the device; the R half is also needed as canonical bytes (the transcript absorbs a_vec)
-  DevBuf<u256> d_r(r.size() + 1), d_L(L_size), d_R(R_size), d_Rc(R_size), d_LZ(R_size), tmp(64 * R_size), eqs(2 * ((size_t)1 << ((ell - lv + 1) / 2)) + 8);
+  DevBuf<u256> d_r(r.size() + 1), d_L(L_size), d_R(R_size), d_Rc(R_size), d_LZ(R_size), tmp(64 * R_size), eqs(dev::eq_evals_scratch(ell - lv));
   dev::h2d(d_r.p, r.data(), r.size() * sizeof(u256), ctx.stream);
   dev::eq_evals(d_L.p, d_r.p, (int)lv, eqs.p, ctx.stream);
   dev::eq_evals(d_R.p, d_r.p + lv, (int)(ell - lv), eqs.p, ctx.stream);
@@ -792,9 +804,7 @@ std::vector<uint8_t> Instance::shape_bincode() const {
   host_coo();
   Writer w;
   w.u64(num_cons); w.u64(num_vars); w.u64(num_inputs);
-  size_t nx = 0, ny = 0;
-  while (((size_t)1 << nx) < num_cons) nx++;
-  while (((size_t)1 << ny) < 2 * num_vars) ny++;
+  const size_t nx = log2_ceil(num_cons), ny = log2_ceil(2 * num_vars);
   for (int m = 0; m < 3; m++) {
     w.out.reserve(w.out.size() + 24 + 48 * M[m].row.size());
     w.u64(nx); w.u64(ny); w.u64(M[m].row.size());
@@ -838,8 +848,7 @@ void r1cs_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::v
   if (!(input.size() < num_vars)) throw std::runtime_error("spartan_b200: |input| + 1 must be at most the number of variables");  // r1csproof.rs:156
   T.append_scalars("input", input);
 
-  size_t ell = 0;
-  while (((size_t)1 << ell) < num_vars) ell++;
+  const size_t ell = log2_ceil(num_vars);
   const size_t L_size = (size_t)1 << (ell / 2), R_size = (size_t)1 << (ell - ell / 2);
   std::vector<Fq> blinds_vars;
   {
@@ -855,15 +864,11 @@ void r1cs_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::v
   // z = vars || 1 || input || 0...                                          (r1csproof.rs:177-185)
   const size_t zlen = 2 * num_vars;
   DevBuf<u256> d_z(zlen);
-  size_t num_rounds_x = 0, num_rounds_y = 0;
-  while (((size_t)1 << num_rounds_x) < num_cons) num_rounds_x++;
-  while (((size_t)1 << num_rounds_y) < zlen) num_rounds_y++;
-  const int W = ctx.shard_world(), rk = ctx.rank();
-  int logW = 0;
-  while ((1 << logW) < W) logW++;
+  const size_t num_rounds_x = log2_ceil(num_cons), num_rounds_y = log2_ceil(zlen);
+  const int W = ctx.shard_world(), rk = ctx.rank(), logW = (int)log2_ceil(W);
   const bool sh1 = ctx.shard_table(num_cons), sh2 = ctx.shard_table(zlen);   // sumcheck tables as cyclic shards (rank r holds the indices = r mod W)
   const size_t n1 = sh1 ? num_cons / W : num_cons, n2 = sh2 ? zlen / W : zlen;
-  DevBuf<u256> d_tau(num_cons), d_Az(n1), d_Bz(n1), d_Cz(n1), d_chal(64), eq_small(2 * ((size_t)1 << ((std::max(num_rounds_x, num_rounds_y) + 1) / 2)) + 8);
+  DevBuf<u256> d_tau(num_cons), d_Az(n1), d_Bz(n1), d_Cz(n1), d_chal(64), eq_small(dev::eq_evals_scratch(std::max(num_rounds_x, num_rounds_y)));
   Fq blind_claim_postsc1;
   std::vector<Fq> claims1;
   {
@@ -899,11 +904,8 @@ void r1cs_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::v
   proof.pok_Cz = knowledge_prove(gens.gens_1, T, tape, Cz_claim, Cz_blind, comm_Cz_claim);
   Fq prod = Az_claim * Bz_claim;
   proof.proof_prod = product_prove(gens.gens_1, T, tape, Az_claim, Az_blind, Bz_claim, Bz_blind, prod, prod_Az_Bz_blind, comm_Az_claim, comm_Bz_claim, comm_prod);
-  T.append_point("comm_Az_claim", comm_Az_claim.b);
-  T.append_point("comm_Bz_claim", comm_Bz_claim.b);
-  T.append_point("comm_Cz_claim", comm_Cz_claim.b);
-  T.append_point("comm_prod_Az_Bz_claims", comm_prod.b);
   proof.claims_phase2 = {comm_Az_claim, comm_Bz_claim, comm_Cz_claim, comm_prod};
+  append_claims_phase2(T, proof.claims_phase2);
   Fq blind_expected_claim_postsc1 = tau_claim * (prod_Az_Bz_blind - Cz_blind);
   Fq claim_post_phase1 = (Az_claim * Bz_claim - Cz_claim) * tau_claim;
   proof.proof_eq_sc_phase1 = equality_prove(gens.gens_1, T, tape, claim_post_phase1, blind_expected_claim_postsc1, claim_post_phase1, blind_claim_postsc1);
@@ -957,9 +959,7 @@ void nizk_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::v
   ShardScope shard(ctx);
   PhaseTimer t(ctx, "NIZK::prove");
   RandomTape tape("proof", tape_seed);                                   // lib.rs:511
-  T.append_protocol_name("Spartan NIZK proof");                          // lib.rs:513
-  const std::vector<uint8_t>& digest = inst.shape_digest();                // r1cs.rs:154-158; never empty: the transcript always binds the shape
-  T.append_message("R1CSShapeDigest", digest.data(), digest.size());       // lib.rs:514
+  append_nizk_head(T, inst);
   r1cs_prove(ctx, inst, d_vars, input, gens, T, tape, out.r1cs_sat_proof, out.rx, out.ry);
 }
 

@@ -1,86 +1,12 @@
-// spartan_b200 — host prover: the reference's proof structs (wire order) and the GPU-driven provers.
-// Struct and field names follow /root/reference/src so the bincode layout (SURVEY.md Appendix B) can be checked line by line.
+// spartan_b200 — host prover: the GPU-driven R1CS / NIZK provers, and the protocol steps of theirs that the verifiers (verifier.cpp) run too.
+// The proof structs and their bincode layout are in wire.hpp.
 #pragma once
 #include <functional>
 #include <array>
 #include <mutex>
-#include "engine.hpp"
+#include "wire.hpp"
 
 namespace sp {
-
-struct Writer {  // bincode 1.x default config
-  std::vector<uint8_t> out;
-  void u64(uint64_t x) { for (int i = 0; i < 8; i++) out.push_back((uint8_t)(x >> (8 * i))); }
-  void scalar(const Fq& s) { uint8_t b[32]; u256_to_bytes(b, s.m); out.insert(out.end(), b, b + 32); }  // Montgomery limbs, not canonical bytes
-  void point(const Cp& c) { out.insert(out.end(), c.b, c.b + 32); }
-  void scalars(const std::vector<Fq>& v) { u64(v.size()); for (auto& s : v) scalar(s); }
-  void points(const std::vector<Cp>& v) { u64(v.size()); for (auto& p : v) point(p); }
-};
-
-// ---- nizk/mod.rs
-struct KnowledgeProof { Cp alpha; Fq z1, z2; void ser(Writer& w) const { w.point(alpha); w.scalar(z1); w.scalar(z2); } };
-struct EqualityProof { Cp alpha; Fq z; void ser(Writer& w) const { w.point(alpha); w.scalar(z); } };
-struct ProductProof { Cp alpha, beta, delta; std::array<Fq, 5> z; void ser(Writer& w) const { w.point(alpha); w.point(beta); w.point(delta); for (auto& s : z) w.scalar(s); } };
-struct DotProductProof { Cp delta, beta; std::vector<Fq> z; Fq z_delta, z_beta; void ser(Writer& w) const { w.point(delta); w.point(beta); w.scalars(z); w.scalar(z_delta); w.scalar(z_beta); } };
-struct BulletReductionProof { std::vector<Cp> L_vec, R_vec; void ser(Writer& w) const { w.points(L_vec); w.points(R_vec); } };
-struct DotProductProofLog { BulletReductionProof bullet_reduction_proof; Cp delta, beta; Fq z1, z2;
-  void ser(Writer& w) const { bullet_reduction_proof.ser(w); w.point(delta); w.point(beta); w.scalar(z1); w.scalar(z2); } };
-// ---- dense_mlpoly.rs
-struct PolyCommitment { std::vector<Cp> C; void ser(Writer& w) const { w.points(C); } };
-struct PolyEvalProof { DotProductProofLog proof; void ser(Writer& w) const { proof.ser(w); } };
-// ---- sumcheck.rs
-struct ZKSumcheckInstanceProof { std::vector<Cp> comm_polys, comm_evals; std::vector<DotProductProof> proofs;
-  void ser(Writer& w) const { w.points(comm_polys); w.points(comm_evals); w.u64(proofs.size()); for (auto& p : proofs) p.ser(w); } };
-struct CompressedUniPoly { std::vector<Fq> coeffs_except_linear_term; void ser(Writer& w) const { w.scalars(coeffs_except_linear_term); } };
-struct SumcheckInstanceProof { std::vector<CompressedUniPoly> compressed_polys; void ser(Writer& w) const { w.u64(compressed_polys.size()); for (auto& p : compressed_polys) p.ser(w); } };
-// ---- r1csproof.rs:21-37
-struct R1CSProof {
-  PolyCommitment comm_vars;
-  ZKSumcheckInstanceProof sc_proof_phase1;
-  std::array<Cp, 4> claims_phase2;
-  KnowledgeProof pok_Cz; ProductProof proof_prod;  // pok_claims_phase2
-  EqualityProof proof_eq_sc_phase1;
-  ZKSumcheckInstanceProof sc_proof_phase2;
-  Cp comm_vars_at_ry;
-  PolyEvalProof proof_eval_vars_at_ry;
-  EqualityProof proof_eq_sc_phase2;
-  void ser(Writer& w) const {
-    comm_vars.ser(w); sc_proof_phase1.ser(w); for (auto& c : claims_phase2) w.point(c); pok_Cz.ser(w); proof_prod.ser(w);
-    proof_eq_sc_phase1.ser(w); sc_proof_phase2.ser(w); w.point(comm_vars_at_ry); proof_eval_vars_at_ry.ser(w); proof_eq_sc_phase2.ser(w);
-  }
-};
-// ---- product_tree.rs / sparse_mlpoly.rs (SNARK only)
-struct LayerProofBatched { SumcheckInstanceProof proof; std::vector<Fq> claims_prod_left, claims_prod_right;
-  void ser(Writer& w) const { proof.ser(w); w.scalars(claims_prod_left); w.scalars(claims_prod_right); } };
-struct ProductCircuitEvalProofBatched { std::vector<LayerProofBatched> proof; std::vector<Fq> dotp_left, dotp_right, dotp_weight;
-  void ser(Writer& w) const { w.u64(proof.size()); for (auto& l : proof) l.ser(w); w.scalars(dotp_left); w.scalars(dotp_right); w.scalars(dotp_weight); } };
-struct ProductLayerProof {
-  Fq row_init; std::vector<Fq> row_read, row_write; Fq row_audit;
-  Fq col_init; std::vector<Fq> col_read, col_write; Fq col_audit;
-  std::vector<Fq> eval_dotp_left, eval_dotp_right;
-  ProductCircuitEvalProofBatched proof_mem, proof_ops;
-  void ser(Writer& w) const {
-    w.scalar(row_init); w.scalars(row_read); w.scalars(row_write); w.scalar(row_audit);
-    w.scalar(col_init); w.scalars(col_read); w.scalars(col_write); w.scalar(col_audit);
-    w.scalars(eval_dotp_left); w.scalars(eval_dotp_right); proof_mem.ser(w); proof_ops.ser(w);
-  }
-};
-struct HashLayerProof {
-  std::vector<Fq> row_addr, row_read_ts; Fq row_audit_ts;
-  std::vector<Fq> col_addr, col_read_ts; Fq col_audit_ts;
-  std::vector<Fq> eval_val, derefs_row, derefs_col;
-  PolyEvalProof proof_ops, proof_mem, proof_derefs;
-  void ser(Writer& w) const {
-    w.scalars(row_addr); w.scalars(row_read_ts); w.scalar(row_audit_ts); w.scalars(col_addr); w.scalars(col_read_ts); w.scalar(col_audit_ts);
-    w.scalars(eval_val); w.scalars(derefs_row); w.scalars(derefs_col); proof_ops.ser(w); proof_mem.ser(w); proof_derefs.ser(w);
-  }
-};
-struct SparseMatPolyEvalProof {  // = R1CSEvalProof.proof
-  PolyCommitment comm_derefs;    // DerefsCommitment.comm_ops_val
-  ProductLayerProof proof_prod_layer;
-  HashLayerProof proof_hash_layer;
-  void ser(Writer& w) const { comm_derefs.ser(w); proof_prod_layer.ser(w); proof_hash_layer.ser(w); }
-};
 
 // ---- generator bundles
 struct PolyCommitmentGens {  // dense_mlpoly.rs:24-36 -> DotProductProofGens (nizk/mod.rs:407-419)
@@ -121,9 +47,6 @@ struct Instance {  // lib.rs:111-114 (R1CSShape + digest)
 };
 
 std::vector<uint8_t> miniz_zlib_level6(const uint8_t* data, size_t len);   // deflate.cpp
-
-struct NizkProof { R1CSProof r1cs_sat_proof; std::vector<Fq> rx, ry;
-  void ser(Writer& w) const { r1cs_sat_proof.ser(w); w.scalars(rx); w.scalars(ry); } };
 
 // R1CSProof::prove (r1csproof.rs:144-349).  d_vars: device array of num_vars Montgomery scalars (consumed read-only).
 // hooks: called (when set) as soon as the first / the second sumcheck phase has produced its point, so that the caller can start work that
@@ -173,6 +96,15 @@ struct UniPoly {  // unipoly.rs
 };
 
 void append_poly_commitment(Transcript& T, const char* label, const PolyCommitment& c);
+// impl Commitments for Scalar / [Scalar] (commitments.rs:73-92): x*G + blind*h, sum x_i*G_i + blind*h, through the host tables (small n only)
+hge commit1(const CommitKey& k, const Fq& x, const Fq& blind);
+hge commitv(const CommitKey& k, const std::vector<Fq>& x, const Fq& blind);
+// the weights a of round j's DotProductProof in a ZK sumcheck (sumcheck.rs:138-157, :535-554, :726-745): a_k = w0 * (k == 0 ? 2 : 1) + w1 * r_j^k, k = 0..degree
+std::vector<Fq> zk_round_weights(const std::vector<Fq>& w, const Fq& r_j, size_t degree);
+// the commitments to Az, Bz, Cz and Az*Bz at rx, absorbed after their sigma proofs (r1csproof.rs:245-248, :400-403)
+void append_claims_phase2(Transcript& T, const std::array<Cp, 4>& c);
+// NIZK::prove / verify before the R1CS proof: protocol name and R1CSShapeDigest (lib.rs:513-514, :558-559)
+void append_nizk_head(Transcript& T, const Instance& inst);
 // PolyEvalProof::prove (dense_mlpoly.rs:312-365) on a device-resident table
 void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt, const std::vector<Fq>& r, const Fq& Zr, const Fq* blind_Zr_opt,
                     const PolyCommitmentGens& gens, Transcript& T, RandomTape& tape, PolyEvalProof& proof, Cp& C_Zr);

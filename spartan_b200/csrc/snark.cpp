@@ -9,9 +9,6 @@
 
 namespace sp {
 
-static size_t log2_ceil(size_t x) { size_t l = 0; while (((size_t)1 << l) < x) l++; return l; }
-static size_t next_pow2(size_t x) { return (size_t)1 << log2_ceil(x); }
-
 static PolyCommitmentGens pc_view(const GenSet* set, size_t num_vars) {  // PolyCommitmentGens::new (dense_mlpoly.rs:31-35)
   PolyCommitmentGens g;
   g.n = (size_t)1 << (num_vars - num_vars / 2);
@@ -34,12 +31,6 @@ SnarkGens::SnarkGens(Ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inpu
   gens_derefs = pc_view(eval_set.get(), v_derefs);
 }
 
-void SnarkEncoding::ser_commitment(Writer& w) const {  // ComputationCommitment { R1CSCommitment { .., SparseMatPolyCommitment } } (r1cs.rs:49-55, sparse_mlpoly.rs:319-327)
-  w.u64(num_cons); w.u64(num_vars); w.u64(num_inputs);
-  w.u64(batch_size); w.u64(num_ops); w.u64(num_mem_cells);
-  comm_comb_ops.ser(w); comm_comb_mem.ser(w);
-}
-
 static void commit_poly(Ctx& ctx, const u256* d_Z, size_t len, const PolyCommitmentGens& gens, PolyCommitment& out) {  // DensePolynomial::commit, no blinds
   size_t ell = log2_ceil(len);
   size_t L = (size_t)1 << (ell / 2), R = (size_t)1 << (ell - ell / 2);
@@ -50,8 +41,9 @@ static void commit_poly(Ctx& ctx, const u256* d_Z, size_t len, const PolyCommitm
 // ================================================================================================ SNARK::encode
 void snark_encode(Ctx& ctx, const Instance& inst, const SnarkGens& gens, SnarkEncoding& e) {
   // SparseMatPolynomial::multi_commit -> multi_sparse_to_dense_rep (sparse_mlpoly.rs:366-420, :483-503)
-  e.num_cons = inst.num_cons; e.num_vars = inst.num_vars; e.num_inputs = inst.num_inputs;
-  e.batch_size = 3;
+  ComputationCommitment& c = e.comm;
+  c.num_cons = inst.num_cons; c.num_vars = inst.num_vars; c.num_inputs = inst.num_inputs;
+  c.batch_size = 3;
   size_t N = 1;
   for (int m = 0; m < 3; m++) N = std::max(N, next_pow2(inst.M[m].nnz));
   // every product circuit of the memory check has log2(N) layers and the proof binds its last one: with at most one entry per matrix there is
@@ -59,7 +51,7 @@ void snark_encode(Ctx& ctx, const Instance& inst, const SnarkGens& gens, SnarkEn
   if (N < 2) throw SpError(SP_ERR_INVALID_ARG, "SNARK::encode needs a matrix with at least two entries (num_ops = 1 leaves the product circuits without layers)");
   size_t x = log2_ceil(inst.num_cons), y = log2_ceil(2 * inst.num_vars);
   size_t cells = (size_t)1 << std::max(x, y);
-  e.num_ops = N; e.num_mem_cells = cells;
+  c.num_ops = N; c.num_mem_cells = cells;
   e.comb_ops.alloc(16 * N);   // row.ops_addr[3] | row.read_ts[3] | col.ops_addr[3] | col.read_ts[3] | val[3] | zero pad  (DensePolynomial::merge)
   e.comb_mem.alloc(2 * cells);
   dev::dzero(e.comb_ops.p, 16 * N * sizeof(u256), ctx.stream);
@@ -85,15 +77,15 @@ void snark_encode(Ctx& ctx, const Instance& inst, const SnarkGens& gens, SnarkEn
   dev::d2h(&out_of_range, bad.p, sizeof(unsigned int), ctx.stream);
   ctx.sync();
   if (out_of_range) throw SpError(SP_ERR_INVALID_INDEX, "address out of range");
-  commit_poly(ctx, e.comb_ops.p, 16 * N, gens.gens_ops, e.comm_comb_ops);
-  commit_poly(ctx, e.comb_mem.p, 2 * cells, gens.gens_mem, e.comm_comb_mem);
+  commit_poly(ctx, e.comb_ops.p, 16 * N, gens.gens_ops, c.comm_comb_ops);
+  commit_poly(ctx, e.comb_mem.p, 2 * cells, gens.gens_mem, c.comm_comb_mem);
 }
 
 // views into the dense representation
 struct DenseView {
   size_t N, cells;
   const u256 *row_addr[3], *row_ts[3], *col_addr[3], *col_ts[3], *val[3], *row_audit, *col_audit;
-  explicit DenseView(const SnarkEncoding& e) : N(e.num_ops), cells(e.num_mem_cells) {
+  explicit DenseView(const SnarkEncoding& e) : N(e.comm.num_ops), cells(e.comm.num_mem_cells) {
     for (int m = 0; m < 3; m++) {
       row_addr[m] = e.comb_ops.p + (size_t)m * N; row_ts[m] = e.comb_ops.p + (size_t)(3 + m) * N;
       col_addr[m] = e.comb_ops.p + (size_t)(6 + m) * N; col_ts[m] = e.comb_ops.p + (size_t)(9 + m) * N;
@@ -168,14 +160,13 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
   const size_t Ks = prods[0]->Ks;
   // the shared eq table and its two ping-pong halves: local sizes while a layer is sharded, full sizes for the replicated layers
   const size_t max_half = std::max(prods[0]->local_len(0) / 2, Ks < num_layers ? prods[0]->local_len(Ks) / 2 : 1);
-  DevBuf<u256> cpar_a(std::max<size_t>(max_half / 2, 1)), cpar_b(std::max<size_t>(max_half / 2, 1)), d_rand(64), eq_small(2 * ((size_t)1 << ((num_layers + 1) / 2)) + 8);
+  DevBuf<u256> cpar_a(std::max<size_t>(max_half / 2, 1)), cpar_b(std::max<size_t>(max_half / 2, 1)), d_rand(64), eq_small(dev::eq_evals_scratch(num_layers));
   DevBuf<u256> cpar0(std::max<size_t>(max_half, 1));
   std::vector<Fq> rand;
   const size_t G_MIN = 2 * Ctx::SHARD_MIN_LOCAL;   // 16384 entries per table: the fused G kernel then always streams >= 32768
   u256* d_out = ctx.small.p + 64;   // ninst * 3 scalars
   DevBuf<u256> d_heads(64);
-  int logW = 0;
-  while ((1 << logW) < W) logW++;
+  const int logW = (int)log2_ceil(W);
   // a layer's sumcheck runs on tables of half = len/2 entries (num_rounds variables), lhalf of them on this rank while the layer is sharded
   struct Shape { size_t half, num_rounds, lhalf; bool sh; int logW; };
   auto shape_of = [&](size_t layer_id) {
@@ -392,21 +383,84 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
   rand_out = rand;
 }
 
-static void append_scalar_vec(Transcript& T, const char* label, const std::vector<Fq>& v) { T.append_scalars(label, v); }
-
-static std::vector<Fq> bound_bot_all(std::vector<Fq> v, const std::vector<Fq>& ch) {  // repeated bound_poly_var_bot (dense_mlpoly.rs:225-233), last challenge first
-  for (size_t k = ch.size(); k-- > 0;) {
-    size_t n = v.size() / 2;
-    std::vector<Fq> o(n);
-    for (size_t i = 0; i < n; i++) o[i] = v[2 * i] + ch[k] * (v[2 * i + 1] - v[2 * i]);
-    v = o;
+// ================================================================================================ steps SNARK::verify shares
+void append_computation_commitment(Transcript& T, const ComputationCommitment& c) {
+  T.append_u64("num_cons", c.num_cons); T.append_u64("num_vars", c.num_vars); T.append_u64("num_inputs", c.num_inputs);
+  T.append_u64("batch_size", c.batch_size); T.append_u64("num_ops", c.num_ops); T.append_u64("num_mem_cells", c.num_mem_cells);
+  append_poly_commitment(T, "comm_comb_ops", c.comm_comb_ops);
+  append_poly_commitment(T, "comm_comb_mem", c.comm_comb_mem);
+}
+void append_derefs_commitment(Transcript& T, const PolyCommitment& c) {
+  T.append_message("derefs_commitment", "begin_derefs_commitment");
+  append_poly_commitment(T, "comm_poly_row_col_ops_val", c);
+  T.append_message("derefs_commitment", "end_derefs_commitment");
+}
+bool append_memory_claims(Transcript& T, const ProductLayerProof& pl) {
+  for (int side = 0; side < 2; side++) {
+    const Fq& init = side ? pl.col_init : pl.row_init;
+    const Fq& audit = side ? pl.col_audit : pl.row_audit;
+    const std::vector<Fq>& read = side ? pl.col_read : pl.row_read;
+    const std::vector<Fq>& write = side ? pl.col_write : pl.row_write;
+    Fq ws = Fq::one(), rs = Fq::one();
+    for (auto& w : write) ws *= w;
+    for (auto& r : read) rs *= r;
+    if (!(init * ws == rs * audit)) return false;
+    T.append_scalar(side ? "claim_col_eval_init" : "claim_row_eval_init", init);
+    T.append_scalars(side ? "claim_col_eval_read" : "claim_row_eval_read", read);
+    T.append_scalars(side ? "claim_col_eval_write" : "claim_row_eval_write", write);
+    T.append_scalar(side ? "claim_col_eval_audit" : "claim_row_eval_audit", audit);
   }
-  return v;
+  return true;
+}
+void equalize(std::vector<Fq>& rx, std::vector<Fq>& ry) {
+  if (rx.size() < ry.size()) rx.insert(rx.begin(), ry.size() - rx.size(), Fq::zero());
+  if (ry.size() < rx.size()) ry.insert(ry.begin(), rx.size() - ry.size(), Fq::zero());
+}
+static std::vector<Fq> combine_to_one(Transcript& T, std::vector<Fq> evals, const std::vector<Fq>& rand, const char* label_evals,
+                                      const char* label_challenge, const char* label_joint, Fq& joint) {
+  evals.resize(next_pow2(evals.size()), Fq::zero());
+  T.append_scalars(label_evals, evals);
+  std::vector<Fq> r_joint = T.challenge_vector(label_challenge, log2_ceil(evals.size()));
+  for (size_t k = r_joint.size(); k-- > 0;) {   // bound_poly_var_bot (dense_mlpoly.rs:225-233), last challenge first
+    const size_t n = evals.size() / 2;
+    for (size_t i = 0; i < n; i++) evals[i] = evals[2 * i] + r_joint[k] * (evals[2 * i + 1] - evals[2 * i]);
+    evals.resize(n);
+  }
+  joint = evals[0];
+  T.append_scalar(label_joint, joint);
+  r_joint.insert(r_joint.end(), rand.begin(), rand.end());
+  return r_joint;
+}
+std::vector<Fq> combine_to_one(Transcript& T, const HashLayerProof& hl, HashOpening which, const std::vector<Fq>& rand, Fq& joint) {
+  const char* n_to_one = "challenge_combine_n_to_one";
+  std::vector<Fq> evals;
+  switch (which) {
+    case HashOpening::derefs:   // DerefsEvalProof (sparse_mlpoly.rs:80-123)
+      for (auto* v : {&hl.derefs_row, &hl.derefs_col}) evals.insert(evals.end(), v->begin(), v->end());
+      return combine_to_one(T, evals, rand, "evals_ops_val", n_to_one, "joint_claim_eval", joint);
+    case HashOpening::ops:
+      for (auto* v : {&hl.row_addr, &hl.row_read_ts, &hl.col_addr, &hl.col_read_ts, &hl.eval_val}) evals.insert(evals.end(), v->begin(), v->end());
+      return combine_to_one(T, evals, rand, "claim_evals_ops", n_to_one, "joint_claim_eval_ops", joint);
+    case HashOpening::mem:
+      return combine_to_one(T, {hl.row_audit_ts, hl.col_audit_ts}, rand, "claim_evals_mem", "challenge_combine_two_to_one", "joint_claim_eval_mem", joint);
+  }
+  throw SpError(SP_ERR_INTERNAL, "unknown hash-layer opening");
+}
+void instance_evaluate(Ctx& ctx, const Instance& inst, const std::vector<Fq>& rx, const std::vector<Fq>& ry, Fq out[3]) {
+  DevBuf<u256> d_chal(rx.size() + ry.size() + 2), trx((size_t)1 << rx.size()), try_((size_t)1 << ry.size());
+  DevBuf<u256> eq_small(dev::eq_evals_scratch(std::max(rx.size(), ry.size())));
+  dev::h2d(d_chal.p, rx.data(), rx.size() * sizeof(u256), ctx.stream);
+  dev::eq_evals(trx.p, d_chal.p, (int)rx.size(), eq_small.p, ctx.stream);
+  dev::h2d(d_chal.p + rx.size(), ry.data(), ry.size() * sizeof(u256), ctx.stream);
+  dev::eq_evals(try_.p, d_chal.p + rx.size(), (int)ry.size(), eq_small.p, ctx.stream);
+  for (int m = 0; m < 3; m++)
+    dev::sparse_eval3(ctx.small.p + 40 + m, inst.M[m].coo_row.p, inst.M[m].coo_col.p, inst.M[m].coo_val.p, inst.M[m].nnz, trx.p, try_.p, ctx.red.p, ctx.stream);
+  ctx.get_small(40, out, 3);
 }
 
 // ================================================================================================ SNARK::prove
 void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const u256* d_vars, const std::vector<Fq>& input, const SnarkGens& gens,
-                 Transcript& T, const Fq& tape_seed, Writer& w) {
+                 Transcript& T, const Fq& tape_seed, SnarkProof& out) {
   ctx.timings.clear();
   ShardScope shard(ctx);   // on a connected multi-GPU context every rank runs this same function on the same inputs (see DESIGN.md "Multi-GPU")
   auto t_start = std::chrono::steady_clock::now();
@@ -415,16 +469,12 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
   };
   RandomTape tape("proof", tape_seed);                    // lib.rs:352
   T.append_protocol_name("Spartan SNARK proof");          // lib.rs:354
-  // comm.comm.append_to_transcript (r1cs.rs:58-65, sparse_mlpoly.rs:329-341)
-  T.append_u64("num_cons", enc.num_cons); T.append_u64("num_vars", enc.num_vars); T.append_u64("num_inputs", enc.num_inputs);
-  T.append_u64("batch_size", enc.batch_size); T.append_u64("num_ops", enc.num_ops); T.append_u64("num_mem_cells", enc.num_mem_cells);
-  append_poly_commitment(T, "comm_comb_ops", enc.comm_comb_ops);
-  append_poly_commitment(T, "comm_comb_mem", enc.comm_comb_mem);
+  append_computation_commitment(T, enc.comm);
 
   const DenseView dv(enc);
   const size_t N = dv.N, cells = dv.cells;
   const size_t lgN = log2_ceil(N), lgC = log2_ceil(cells);
-  DevBuf<u256> d_chal(64), eq_small(2 * ((size_t)1 << ((std::max(lgN + 4, lgC + 1) + 1) / 2)) + 8);
+  DevBuf<u256> d_chal(64), eq_small(dev::eq_evals_scratch(std::max(lgN + 4, lgC + 1)));
 
   // ---- dereferenced values and their commitment (sparse_mlpoly.rs:507-512, :213-219), started EARLY on the background stream.
   // comb = row_ops_val[3] | col_ops_val[3] | zero pad, committed as an L x R matrix (dense_mlpoly.rs:165-177).  row_ops_val depends only on rx
@@ -491,23 +541,12 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
     hooks.on_ry = [&](const std::vector<Fq>& p) { early_part(1, p); };
   }
 
-  R1CSProof sat;
   std::vector<Fq> rx, ry;
-  r1cs_prove(ctx, inst, d_vars, input, *gens.gens_r1cs_sat, T, tape, sat, rx, ry, early ? &hooks : nullptr);
+  r1cs_prove(ctx, inst, d_vars, input, *gens.gens_r1cs_sat, T, tape, out.r1cs_sat_proof, rx, ry, early ? &hooks : nullptr);
 
-  // ---- inst.evaluate(rx, ry) (r1cs.rs:300-303 -> multi_evaluate sparse_mlpoly.rs:440-452)
   auto t0 = std::chrono::steady_clock::now();
-  Fq inst_evals[3];
-  {
-    DevBuf<u256> trx((size_t)1 << rx.size()), try_((size_t)1 << ry.size());
-    dev::h2d(d_chal.p, rx.data(), rx.size() * sizeof(u256), ctx.stream);
-    dev::eq_evals(trx.p, d_chal.p, (int)rx.size(), eq_small.p, ctx.stream);
-    dev::h2d(d_chal.p + 32, ry.data(), ry.size() * sizeof(u256), ctx.stream);
-    dev::eq_evals(try_.p, d_chal.p + 32, (int)ry.size(), eq_small.p, ctx.stream);
-    for (int m = 0; m < 3; m++)
-      dev::sparse_eval3(ctx.small.p + 40 + m, inst.M[m].coo_row.p, inst.M[m].coo_col.p, inst.M[m].coo_val.p, inst.M[m].nnz, trx.p, try_.p, ctx.red.p, ctx.stream);
-    ctx.get_small(40, inst_evals, 3);
-  }
+  const std::array<Fq, 3>& inst_evals = out.inst_evals;
+  instance_evaluate(ctx, inst, rx, ry, out.inst_evals.data());
   T.append_scalar("Ar_claim", inst_evals[0]);
   T.append_scalar("Br_claim", inst_evals[1]);
   T.append_scalar("Cr_claim", inst_evals[2]);
@@ -515,7 +554,7 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
 
   // ---- R1CSEvalProof::prove -> SparseMatPolyEvalProof::prove (sparse_mlpoly.rs:1447-1514)
   auto t_eval = std::chrono::steady_clock::now();
-  SparseMatPolyEvalProof ep;
+  SparseMatPolyEvalProof& ep = out.r1cs_eval_proof;
   T.append_protocol_name("Sparse polynomial evaluation proof");
   if (nx != rx.size() || ny != ry.size()) throw std::runtime_error("spartan_b200: unexpected sumcheck point lengths");
   {
@@ -534,10 +573,8 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
         for (int part = 0; part < 2; part++)
           memcpy(ep.comm_derefs.C[(size_t)part * n_part + r * cnt].b, hb.data() + (r * 2 + part) * 32 * cnt, 32 * cnt);
     } else {
-      // equalize (sparse_mlpoly.rs:1429-1445): left-pad the shorter point with zeros
       std::vector<Fq> rx_ext = rx, ry_ext = ry;
-      if (rx.size() < ry.size()) rx_ext.insert(rx_ext.begin(), ry.size() - rx.size(), Fq::zero());
-      if (ry.size() < rx.size()) ry_ext.insert(ry_ext.begin(), rx.size() - ry.size(), Fq::zero());
+      equalize(rx_ext, ry_ext);
       dev::h2d(d_chal.p, rx_ext.data(), rx_ext.size() * sizeof(u256), ctx.stream);
       dev::eq_evals(mem_rx.p, d_chal.p, (int)rx_ext.size(), eq_small.p, ctx.stream);
       dev::h2d(d_chal.p + 32, ry_ext.data(), ry_ext.size() * sizeof(u256), ctx.stream);
@@ -548,9 +585,7 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
       }
       commit_poly(ctx, derefs.p, 8 * N, gens.gens_derefs, ep.comm_derefs);
     }
-    T.append_message("derefs_commitment", "begin_derefs_commitment");  // sparse_mlpoly.rs:213-219
-    append_poly_commitment(T, "comm_poly_row_col_ops_val", ep.comm_derefs);
-    T.append_message("derefs_commitment", "end_derefs_commitment");
+    append_derefs_commitment(T, ep.comm_derefs);
     mark("commit_nondet_witness", tc);
   }
   std::vector<Fq> r_mem_check = T.challenge_vector("challenge_r_hash", 2);
@@ -608,19 +643,11 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
     memcpy(v, ctx.host_res, sizeof v);
     for (int side = 0; side < 2; side++) for (int c = 0; c < 8; c++) roots[side][c] = v[16 * side + 2 * c] * v[16 * side + 2 * c + 1];
   }
-  for (int side = 0; side < 2; side++) {
-    Fq init = roots[side][0], audit = roots[side][1];
-    std::vector<Fq> read = {roots[side][2], roots[side][3], roots[side][4]}, write = {roots[side][5], roots[side][6], roots[side][7]};
-    Fq ws = write[0] * write[1] * write[2], rs = read[0] * read[1] * read[2];
-    if (!(init * ws == rs * audit)) throw SpError(SP_ERR_INTERNAL, "memory-check subset test failed (sparse_mlpoly.rs:1060)");
-    const char* li = side == 0 ? "claim_row_eval_init" : "claim_col_eval_init";
-    const char* lr = side == 0 ? "claim_row_eval_read" : "claim_col_eval_read";
-    const char* lw = side == 0 ? "claim_row_eval_write" : "claim_col_eval_write";
-    const char* la = side == 0 ? "claim_row_eval_audit" : "claim_col_eval_audit";
-    T.append_scalar(li, init); append_scalar_vec(T, lr, read); append_scalar_vec(T, lw, write); T.append_scalar(la, audit);
-    if (side == 0) { pl.row_init = init; pl.row_read = read; pl.row_write = write; pl.row_audit = audit; }
-    else { pl.col_init = init; pl.col_read = read; pl.col_write = write; pl.col_audit = audit; }
-  }
+  const Fq* rr = roots[0];
+  pl.row_init = rr[0]; pl.row_audit = rr[1]; pl.row_read = {rr[2], rr[3], rr[4]}; pl.row_write = {rr[5], rr[6], rr[7]};
+  const Fq* rc = roots[1];
+  pl.col_init = rc[0]; pl.col_audit = rc[1]; pl.col_read = {rc[2], rc[3], rc[4]}; pl.col_write = {rc[5], rc[6], rc[7]};
+  if (!append_memory_claims(T, pl)) throw SpError(SP_ERR_INTERNAL, "memory-check subset test failed (sparse_mlpoly.rs:1060)");
   // dot-product circuits: clones of (row_ops_val, col_ops_val, val), split in halves (sparse_mlpoly.rs:1090-1117).  Their claims are taken on the
   // full tables; the copies the sumcheck binds are this rank's cyclic shards when the ops circuits are sharded.
   const bool sh_dotp = S[0].read[0].sharded(0);
@@ -696,43 +723,22 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
   mark("  hash_layer_evaluations", th);
   th = std::chrono::steady_clock::now();
   Cp dummy;
+  Fq joint;
   {  // DerefsEvalProof::prove (sparse_mlpoly.rs:125-149, prove_single :80-123)
     T.append_protocol_name("Derefs evaluation proof");
-    std::vector<Fq> evals = hl.derefs_row;
-    evals.insert(evals.end(), hl.derefs_col.begin(), hl.derefs_col.end());
-    evals.resize(next_pow2(evals.size()), Fq::zero());
-    T.append_scalars("evals_ops_val", evals);
-    std::vector<Fq> ch = T.challenge_vector("challenge_combine_n_to_one", log2_ceil(evals.size()));
-    Fq joint = bound_bot_all(evals, ch)[0];
-    std::vector<Fq> r_joint = ch;
-    r_joint.insert(r_joint.end(), rand_ops.begin(), rand_ops.end());
-    T.append_scalar("joint_claim_eval", joint);
+    const std::vector<Fq> r_joint = combine_to_one(T, hl, HashOpening::derefs, rand_ops, joint);
     polyeval_prove(ctx, derefs.p, nullptr, r_joint, joint, nullptr, gens.gens_derefs, T, tape, hl.proof_derefs, dummy);
   }
   mark("  polyeval_derefs(2^23)", th);
   th = std::chrono::steady_clock::now();
   {  // ops decommitment (sparse_mlpoly.rs:766-797)
-    std::vector<Fq> evals;
-    for (auto* v : {&hl.row_addr, &hl.row_read_ts, &hl.col_addr, &hl.col_read_ts, &hl.eval_val}) evals.insert(evals.end(), v->begin(), v->end());
-    evals.resize(next_pow2(evals.size()), Fq::zero());
-    T.append_scalars("claim_evals_ops", evals);
-    std::vector<Fq> ch = T.challenge_vector("challenge_combine_n_to_one", log2_ceil(evals.size()));
-    Fq joint = bound_bot_all(evals, ch)[0];
-    std::vector<Fq> r_joint = ch;
-    r_joint.insert(r_joint.end(), rand_ops.begin(), rand_ops.end());
-    T.append_scalar("joint_claim_eval_ops", joint);
+    const std::vector<Fq> r_joint = combine_to_one(T, hl, HashOpening::ops, rand_ops, joint);
     polyeval_prove(ctx, enc.comb_ops.p, nullptr, r_joint, joint, nullptr, gens.gens_ops, T, tape, hl.proof_ops, dummy);
   }
   mark("  polyeval_ops(2^24)", th);
   th = std::chrono::steady_clock::now();
   {  // mem decommitment (sparse_mlpoly.rs:799-824)
-    std::vector<Fq> evals = {hl.row_audit_ts, hl.col_audit_ts};
-    T.append_scalars("claim_evals_mem", evals);
-    std::vector<Fq> ch = T.challenge_vector("challenge_combine_two_to_one", 1);
-    Fq joint = bound_bot_all(evals, ch)[0];
-    std::vector<Fq> r_joint = ch;
-    r_joint.insert(r_joint.end(), rand_mem.begin(), rand_mem.end());
-    T.append_scalar("joint_claim_eval_mem", joint);
+    const std::vector<Fq> r_joint = combine_to_one(T, hl, HashOpening::mem, rand_mem, joint);
     polyeval_prove(ctx, enc.comb_mem.p, nullptr, r_joint, joint, nullptr, gens.gens_mem, T, tape, hl.proof_mem, dummy);
   }
   mark("  polyeval_mem(2^22)", th);
@@ -741,11 +747,6 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
   mark("SNARK::prove", t_start);
   for (auto& f : ctx.fine) ctx.timings.push_back({"fine:" + f.first, f.second});
   ctx.fine.clear();
-
-  // bincode(SNARK { r1cs_sat_proof, inst_evals, r1cs_eval_proof }) (lib.rs:313-317)
-  sat.ser(w);
-  for (int m = 0; m < 3; m++) w.scalar(inst_evals[m]);
-  ep.ser(w);
 }
 
 }  // namespace sp

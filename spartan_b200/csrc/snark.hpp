@@ -18,22 +18,34 @@ struct AddrTimestampsDev {  // sparse_mlpoly.rs:213-272
   DevBuf<u256> audit_ts;
 };
 struct SnarkEncoding {  // ComputationCommitment + ComputationDecommitment (lib.rs:44-55; sparse_mlpoly.rs:274-327)
-  size_t num_cons = 0, num_vars = 0, num_inputs = 0;
-  size_t batch_size = 0, num_ops = 0, num_mem_cells = 0;
-  PolyCommitment comm_comb_ops, comm_comb_mem;
+  ComputationCommitment comm;     // alone in an encoding loaded from commitment bytes, which can verify but not prove
   std::vector<DevBuf<u256>> val;  // dense.val
   AddrTimestampsDev row, col;
   DevBuf<u256> comb_ops, comb_mem;
-  void ser_commitment(Writer& w) const;
 };
 
 void snark_encode(Ctx& ctx, const Instance& inst, const SnarkGens& gens, SnarkEncoding& out);
 void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const u256* d_vars, const std::vector<Fq>& input, const SnarkGens& gens,
-                 Transcript& T, const Fq& tape_seed, Writer& out);
+                 Transcript& T, const Fq& tape_seed, SnarkProof& out);
+
+// ---- protocol steps SNARK::prove and SNARK::verify share
+void append_computation_commitment(Transcript& T, const ComputationCommitment& c);   // r1cs.rs:58-65, sparse_mlpoly.rs:329-341
+void append_derefs_commitment(Transcript& T, const PolyCommitment& c);              // sparse_mlpoly.rs:204-210
+// ProductLayerProof's memory-check claims, row side then column side (sparse_mlpoly.rs:1060-1088, :1246-1277): a side is absorbed only when
+// init * prod(writes) == prod(reads) * audit; returns false, with that side not absorbed, at the first side where it does not hold
+bool append_memory_claims(Transcript& T, const ProductLayerProof& pl);
+// left-pad the shorter of rx, ry with zeros (sparse_mlpoly.rs:1429-1445)
+void equalize(std::vector<Fq>& rx, std::vector<Fq>& ry);
+// HashLayerProof opens three committed polynomials at one point each (sparse_mlpoly.rs:80-123, :766-824).  The claims it makes about one of
+// them, padded with zeros to a power of two, are absorbed, combined into one joint claim by the challenges drawn next, and the joint claim is
+// absorbed.  Sets `joint`; returns the point it is claimed at: the challenges followed by `rand` (rand_ops for derefs and ops, rand_mem for mem).
+enum class HashOpening { derefs, ops, mem };
+std::vector<Fq> combine_to_one(Transcript& T, const HashLayerProof& hl, HashOpening which, const std::vector<Fq>& rand, Fq& joint);
+// inst.evaluate(rx, ry) (r1cs.rs:300-303 -> sparse_mlpoly.rs:440-452) on the device
+void instance_evaluate(Ctx& ctx, const Instance& inst, const std::vector<Fq>& rx, const std::vector<Fq>& ry, Fq out[3]);
 
 // ---- verifiers (verifier.cpp): throw SpError with code SP_ERR_VERIFY / SP_ERR_DECOMPRESS when the proof is rejected
-void instance_evaluate(Ctx& ctx, const Instance& inst, const std::vector<Fq>& rx, const std::vector<Fq>& ry, Fq out[3]);
 void nizk_verify(Ctx& ctx, const Instance& inst, const std::vector<Fq>& input, const R1CSGens& gens, Transcript& T, const uint8_t* proof, size_t len);
-void snark_verify(Ctx& ctx, const SnarkEncoding& comm, const std::vector<Fq>& input, const SnarkGens& gens, Transcript& T, const uint8_t* proof, size_t len);
+void snark_verify(Ctx& ctx, const SnarkEncoding& enc, const std::vector<Fq>& input, const SnarkGens& gens, Transcript& T, const uint8_t* proof, size_t len);
 
 }  // namespace sp

@@ -17,68 +17,6 @@ namespace {
 struct Reject : SpError { explicit Reject(const std::string& what) : SpError(SP_ERR_VERIFY, "proof rejected: " + what) {} };
 struct BadPoint : SpError { explicit BadPoint(const std::string& what) : SpError(SP_ERR_DECOMPRESS, "proof rejected: " + what + " does not decompress") {} };
 
-// ---- bincode reader (inverse of Writer in prover.hpp)
-struct Reader {
-  const uint8_t* p; size_t n, pos = 0;
-  Reader(const uint8_t* b, size_t len) : p(b), n(len) {}
-  void need(size_t k) { if (n - pos < k) throw Reject("truncated proof"); }
-  uint64_t u64() { need(8); uint64_t x = 0; for (int i = 0; i < 8; i++) x |= (uint64_t)p[pos + i] << (8 * i); pos += 8; return x; }
-  // a Scalar on the wire is its four Montgomery limbs (serde derive on `Scalar([u64;4])`): the reference accepts any limbs, but every host
-  // routine here assumes a reduced residue, so limbs >= q are rejected instead of being carried into fq_mul / fq_eq (no malleability either)
-  Fq scalar() { need(32); if (!fq_bytes_canonical(p + pos)) throw Reject("scalar limbs are not reduced modulo q"); Fq f; memcpy(&f.m, p + pos, 32); pos += 32; return f; }
-  Cp point() { need(32); Cp c; memcpy(c.b, p + pos, 32); pos += 32; return c; }
-  size_t len(size_t item) { uint64_t k = u64(); if (k > (n - pos) / item) throw Reject("vector length exceeds the proof"); return (size_t)k; }
-  std::vector<Fq> scalars() { size_t k = len(32); std::vector<Fq> v(k); for (auto& s : v) s = scalar(); return v; }
-  std::vector<Cp> points() { size_t k = len(32); std::vector<Cp> v(k); for (auto& s : v) s = point(); return v; }
-};
-void rd(Reader& r, KnowledgeProof& p) { p.alpha = r.point(); p.z1 = r.scalar(); p.z2 = r.scalar(); }
-void rd(Reader& r, EqualityProof& p) { p.alpha = r.point(); p.z = r.scalar(); }
-void rd(Reader& r, ProductProof& p) { p.alpha = r.point(); p.beta = r.point(); p.delta = r.point(); for (auto& z : p.z) z = r.scalar(); }
-void rd(Reader& r, DotProductProof& p) { p.delta = r.point(); p.beta = r.point(); p.z = r.scalars(); p.z_delta = r.scalar(); p.z_beta = r.scalar(); }
-void rd(Reader& r, DotProductProofLog& p) {
-  p.bullet_reduction_proof.L_vec = r.points(); p.bullet_reduction_proof.R_vec = r.points();
-  p.delta = r.point(); p.beta = r.point(); p.z1 = r.scalar(); p.z2 = r.scalar();
-}
-void rd(Reader& r, ZKSumcheckInstanceProof& p) {
-  p.comm_polys = r.points(); p.comm_evals = r.points();
-  size_t k = r.len(32 * 5);
-  p.proofs.resize(k);
-  for (auto& d : p.proofs) rd(r, d);
-}
-void rd(Reader& r, R1CSProof& p) {
-  p.comm_vars.C = r.points();
-  rd(r, p.sc_proof_phase1);
-  for (auto& c : p.claims_phase2) c = r.point();
-  rd(r, p.pok_Cz); rd(r, p.proof_prod); rd(r, p.proof_eq_sc_phase1);
-  rd(r, p.sc_proof_phase2);
-  p.comm_vars_at_ry = r.point();
-  rd(r, p.proof_eval_vars_at_ry.proof);
-  rd(r, p.proof_eq_sc_phase2);
-}
-void rd(Reader& r, SumcheckInstanceProof& p) {
-  size_t k = r.len(8);
-  p.compressed_polys.resize(k);
-  for (auto& c : p.compressed_polys) c.coeffs_except_linear_term = r.scalars();
-}
-void rd(Reader& r, ProductCircuitEvalProofBatched& p) {
-  size_t k = r.len(8);
-  p.proof.resize(k);
-  for (auto& l : p.proof) { rd(r, l.proof); l.claims_prod_left = r.scalars(); l.claims_prod_right = r.scalars(); }
-  p.dotp_left = r.scalars(); p.dotp_right = r.scalars(); p.dotp_weight = r.scalars();
-}
-void rd(Reader& r, ProductLayerProof& p) {
-  p.row_init = r.scalar(); p.row_read = r.scalars(); p.row_write = r.scalars(); p.row_audit = r.scalar();
-  p.col_init = r.scalar(); p.col_read = r.scalars(); p.col_write = r.scalars(); p.col_audit = r.scalar();
-  p.eval_dotp_left = r.scalars(); p.eval_dotp_right = r.scalars();
-  rd(r, p.proof_mem); rd(r, p.proof_ops);
-}
-void rd(Reader& r, HashLayerProof& p) {
-  p.row_addr = r.scalars(); p.row_read_ts = r.scalars(); p.row_audit_ts = r.scalar();
-  p.col_addr = r.scalars(); p.col_read_ts = r.scalars(); p.col_audit_ts = r.scalar();
-  p.eval_val = r.scalars(); p.derefs_row = r.scalars(); p.derefs_col = r.scalars();
-  rd(r, p.proof_ops.proof); rd(r, p.proof_mem.proof); rd(r, p.proof_derefs.proof);
-}
-
 // ---- group helpers (host, radix 2^51)
 hge unpack(const Cp& c, const char* what) {
   ge g;
@@ -88,16 +26,6 @@ hge unpack(const Cp& c, const char* what) {
 hge mul(const hge& p, const Fq& k) { return hge_scalarmul(k.canonical(), p); }
 hge neg(const hge& p) { hge q = p; q.X = fe_neg(p.X); q.T = fe_neg(p.T); return q; }
 bool same(const hge& a, const hge& b) { return compress(a) == compress(b); }
-hge commit1(const CommitKey& k, const Fq& x, const Fq& blind) {   // x*G + blind*h through the host tables
-  Term t[2] = {{k.off, x}, {k.h, blind}};
-  return host_commit(*k.set, t, 2);
-}
-hge commit_small(const CommitKey& k, const std::vector<Fq>& x, const Fq& blind) {
-  std::vector<Term> t;
-  for (size_t i = 0; i < x.size(); i++) t.push_back({k.off + i, x[i]});
-  t.push_back({k.h, blind});
-  return host_commit(*k.set, t.data(), t.size());
-}
 // sum_i s_i * G[key.off + i] over the device tables (no blind)
 hge msm_gens(Ctx& ctx, const CommitKey& key, const std::vector<Fq>& s) {
   DevBuf<u256> d(s.size());
@@ -140,17 +68,6 @@ Fq eq_eval(const std::vector<Fq>& a, const std::vector<Fq>& b) {   // EqPolynomi
   for (size_t i = 0; i < a.size(); i++) acc *= a[i] * b[i] + (Fq::one() - a[i]) * (Fq::one() - b[i]);
   return acc;
 }
-std::vector<Fq> bound_bot(std::vector<Fq> v, const std::vector<Fq>& ch) {   // bound_poly_var_bot for each challenge, last first
-  for (size_t k = ch.size(); k-- > 0;) {
-    size_t n = v.size() / 2;
-    std::vector<Fq> o(n);
-    for (size_t i = 0; i < n; i++) o[i] = v[2 * i] + ch[k] * (v[2 * i + 1] - v[2 * i]);
-    v = o;
-  }
-  return v;
-}
-size_t log2c(size_t x) { size_t l = 0; while (((size_t)1 << l) < x) l++; return l; }
-size_t pow2c(size_t x) { size_t p = 1; while (p < x) p <<= 1; return p; }
 
 // ---- sigma protocols
 void knowledge_verify(const KnowledgeProof& p, const CommitKey& g, Transcript& T, const Cp& C) {   // nizk/mod.rs:54-75
@@ -193,7 +110,7 @@ void dotproduct_verify(const DotProductProof& p, const CommitKey& g1, const Comm
   T.append_point("beta", p.beta.b);
   Fq c = T.challenge_scalar("c");
   if (p.z.size() != a.size() || a.size() != gn.n) throw Reject("DotProductProof shape");
-  bool ok = same(hge_add(mul(unpack(Cx, "Cx"), c), unpack(p.delta, "delta")), commit_small(gn, p.z, p.z_delta));
+  bool ok = same(hge_add(mul(unpack(Cx, "Cx"), c), unpack(p.delta, "delta")), commitv(gn, p.z, p.z_delta));
   Fq dz = Fq::zero();
   for (size_t i = 0; i < a.size(); i++) dz += p.z[i] * a[i];
   ok = ok && same(hge_add(mul(Cy, c), unpack(p.beta, "beta")), commit1(g1, dz, p.z_beta));
@@ -214,13 +131,7 @@ Cp zk_sumcheck_verify(const ZKSumcheckInstanceProof& p, const Cp& comm_claim, si
     T.append_point("comm_eval", p.comm_evals[i].b);
     std::vector<Fq> w = T.challenge_vector("combine_two_claims_to_one", 2);
     hge target = hge_add(mul(unpack(claim_c, "comm_claim_per_round"), w[0]), mul(unpack(p.comm_evals[i], "comm_eval"), w[1]));
-    std::vector<Fq> a(degree + 1);
-    Fq rpow = Fq::one();
-    for (size_t k = 0; k <= degree; k++) {
-      Fq a_sc = k == 0 ? Fq::from_u64(2) : Fq::one();
-      a[k] = w[0] * a_sc + w[1] * rpow;
-      rpow *= r_i;
-    }
+    const std::vector<Fq> a = zk_round_weights(w, r_i, degree);
     dotproduct_verify(p.proofs[i], g1, gn, T, a, p.comm_polys[i], target, compress(target));
     r.push_back(r_i);
   }
@@ -313,17 +224,14 @@ void r1cs_verify(Ctx& ctx, const R1CSProof& p, size_t num_vars, size_t num_cons,
   T.append_protocol_name("R1CS proof");
   T.append_scalars("input", input);
   append_poly_commitment(T, "poly_commitment", p.comm_vars);
-  const size_t num_rounds_x = log2c(num_cons), num_rounds_y = log2c(2 * num_vars);
+  const size_t num_rounds_x = log2_ceil(num_cons), num_rounds_y = log2_ceil(2 * num_vars);
   std::vector<Fq> tau = T.challenge_vector("challenge_tau", num_rounds_x);
   Cp claim_phase1 = compress(commit1(gens.gens_1, Fq::zero(), Fq::zero()));
   Cp comm_claim_post_phase1 = zk_sumcheck_verify(p.sc_proof_phase1, claim_phase1, num_rounds_x, 3, gens.gens_1, gens.gens_4, T, rx);
   const Cp &comm_Az = p.claims_phase2[0], &comm_Bz = p.claims_phase2[1], &comm_Cz = p.claims_phase2[2], &comm_prod = p.claims_phase2[3];
   knowledge_verify(p.pok_Cz, gens.gens_1, T, comm_Cz);
   product_verify(p.proof_prod, gens.gens_1, T, comm_Az, comm_Bz, comm_prod);
-  T.append_point("comm_Az_claim", comm_Az.b);
-  T.append_point("comm_Bz_claim", comm_Bz.b);
-  T.append_point("comm_Cz_claim", comm_Cz.b);
-  T.append_point("comm_prod_Az_Bz_claims", comm_prod.b);
+  append_claims_phase2(T, p.claims_phase2);
   Fq taus_bound_rx = eq_eval(rx, tau);
   Cp expected1 = compress(mul(hge_add(unpack(comm_prod, "comm_prod"), neg(unpack(comm_Cz, "comm_Cz"))), taus_bound_rx));
   equality_verify(p.proof_eq_sc_phase1, gens.gens_1, T, expected1, comm_claim_post_phase1);
@@ -332,7 +240,7 @@ void r1cs_verify(Ctx& ctx, const R1CSProof& p, size_t num_vars, size_t num_cons,
   Cp comm_claim_post_phase2 = zk_sumcheck_verify(p.sc_proof_phase2, comm_claim_phase2, num_rounds_y, 2, gens.gens_1, gens.gens_3, T, ry);
   polyeval_verify(ctx, p.proof_eval_vars_at_ry, gens.gens_pc, T, std::vector<Fq>(ry.begin() + 1, ry.end()), p.comm_vars_at_ry, p.comm_vars);
   // SparsePolynomial::evaluate over (0, 1), (i+1, input[i])   (r1csproof.rs:454-464, sparse_mlpoly.rs:1577-1593)
-  const size_t nb = log2c(num_vars);
+  const size_t nb = log2_ceil(num_vars);
   Fq poly_input_eval = Fq::zero();
   for (size_t e = 0; e <= input.size(); e++) {
     Fq chi = Fq::one();
@@ -351,7 +259,7 @@ void r1cs_verify(Ctx& ctx, const R1CSProof& p, size_t num_vars, size_t num_cons,
 struct BatchedOut { std::vector<Fq> claims, claims_dotp, rand; };
 // ProductCircuitEvalProofBatched::verify (product_tree.rs:385-485)
 BatchedOut batched_verify(const ProductCircuitEvalProofBatched& p, const std::vector<Fq>& claims_prod, const std::vector<Fq>& claims_dotp, size_t len, Transcript& T) {
-  const size_t num_layers = log2c(len), np = claims_prod.size();
+  const size_t num_layers = log2_ceil(len), np = claims_prod.size();
   if (p.proof.size() != num_layers) throw Reject("product circuit depth");
   BatchedOut o;
   std::vector<Fq> claims = claims_prod;
@@ -415,36 +323,23 @@ void hash_helper(const std::vector<Fq>& rand_mem, const Fq& claim_init, const st
   }
   if (!(h(init_addr, init_val, audit_ts) == claim_audit)) throw Reject("hash layer: audit");
 }
-void append_derefs_comm(Transcript& T, const PolyCommitment& c) {   // sparse_mlpoly.rs:213-219
-  T.append_message("derefs_commitment", "begin_derefs_commitment");
-  append_poly_commitment(T, "comm_poly_row_col_ops_val", c);
-  T.append_message("derefs_commitment", "end_derefs_commitment");
-}
 // SparseMatPolyEvalProof::verify (sparse_mlpoly.rs:1516-1557) -> PolyEvalNetworkProof::verify (:1356-1416)
-void spark_verify(Ctx& ctx, const SparseMatPolyEvalProof& p, const SnarkEncoding& comm, std::vector<Fq> rx, std::vector<Fq> ry, const Fq evals[3],
-                  const SnarkGens& gens, Transcript& T) {
+void spark_verify(Ctx& ctx, const SparseMatPolyEvalProof& p, const ComputationCommitment& comm, std::vector<Fq> rx, std::vector<Fq> ry,
+                  const Fq evals[3], const SnarkGens& gens, Transcript& T) {
   T.append_protocol_name("Sparse polynomial evaluation proof");
-  while (rx.size() < ry.size()) rx.insert(rx.begin(), Fq::zero());   // equalize (sparse_mlpoly.rs:1429-1445)
-  while (ry.size() < rx.size()) ry.insert(ry.begin(), Fq::zero());
+  equalize(rx, ry);
   if (((size_t)1 << rx.size()) != comm.num_mem_cells) throw Reject("memory size");
-  append_derefs_comm(T, p.comm_derefs);
+  append_derefs_commitment(T, p.comm_derefs);
   std::vector<Fq> r_mem = T.challenge_vector("challenge_r_hash", 2);
   const Fq &r_hash = r_mem[0], &r_multiset = r_mem[1];
   T.append_protocol_name("Sparse polynomial evaluation proof");      // PolyEvalNetworkProof::protocol_name is the same string
-  const size_t ni = 3, num_ops = pow2c(comm.num_ops), num_cells = (size_t)1 << rx.size();
+  const size_t ni = 3, num_ops = next_pow2(comm.num_ops), num_cells = (size_t)1 << rx.size();
   // ---- ProductLayerProof::verify (sparse_mlpoly.rs:1228-1305)
   const ProductLayerProof& pl = p.proof_prod_layer;
   T.append_protocol_name("Sparse polynomial product layer proof");
-  auto side = [&](const Fq& init, const std::vector<Fq>& read, const std::vector<Fq>& write, const Fq& audit, const char* li, const char* lr, const char* lw, const char* la) {
-    if (read.size() != ni || write.size() != ni) throw Reject("product layer shape");
-    Fq ws = Fq::one(), rs = Fq::one();
-    for (auto& w : write) ws *= w;
-    for (auto& r_ : read) rs *= r_;
-    if (!(init * ws == rs * audit)) throw Reject("memory check: init * writes != reads * audit");
-    T.append_scalar(li, init); T.append_scalars(lr, read); T.append_scalars(lw, write); T.append_scalar(la, audit);
-  };
-  side(pl.row_init, pl.row_read, pl.row_write, pl.row_audit, "claim_row_eval_init", "claim_row_eval_read", "claim_row_eval_write", "claim_row_eval_audit");
-  side(pl.col_init, pl.col_read, pl.col_write, pl.col_audit, "claim_col_eval_init", "claim_col_eval_read", "claim_col_eval_write", "claim_col_eval_audit");
+  for (auto* v : {&pl.row_read, &pl.row_write, &pl.col_read, &pl.col_write})
+    if (v->size() != ni) throw Reject("product layer shape");
+  if (!append_memory_claims(T, pl)) throw Reject("memory check: init * writes != reads * audit");
   if (pl.eval_dotp_left.size() != ni || pl.eval_dotp_right.size() != ni) throw Reject("dotp shape");
   std::vector<Fq> claims_dotp_circuit;
   for (size_t i = 0; i < ni; i++) {
@@ -465,42 +360,21 @@ void spark_verify(Ctx& ctx, const SparseMatPolyEvalProof& p, const SnarkEncoding
   const HashLayerProof& hl = p.proof_hash_layer;
   T.append_protocol_name("Sparse polynomial hash layer proof");
   if (hl.derefs_row.size() != ni || hl.derefs_col.size() != ni || hl.eval_val.size() != ni) throw Reject("hash layer shape");
+  Fq joint;
   {  // DerefsEvalProof::verify (sparse_mlpoly.rs:151-211)
     T.append_protocol_name("Derefs evaluation proof");
-    std::vector<Fq> ev = hl.derefs_row;
-    ev.insert(ev.end(), hl.derefs_col.begin(), hl.derefs_col.end());
-    ev.resize(pow2c(ev.size()), Fq::zero());
-    T.append_scalars("evals_ops_val", ev);
-    std::vector<Fq> ch = T.challenge_vector("challenge_combine_n_to_one", log2c(ev.size()));
-    Fq joint = bound_bot(ev, ch)[0];
-    std::vector<Fq> r_joint = ch;
-    r_joint.insert(r_joint.end(), rand_ops.begin(), rand_ops.end());
-    T.append_scalar("joint_claim_eval", joint);
+    const std::vector<Fq> r_joint = combine_to_one(T, hl, HashOpening::derefs, rand_ops, joint);
     polyeval_verify_plain(ctx, hl.proof_derefs, gens.gens_derefs, T, r_joint, joint, p.comm_derefs);
   }
   for (size_t i = 0; i < ni; i++)
     if (!(ops.claims_dotp[3 * i] == hl.derefs_row[i]) || !(ops.claims_dotp[3 * i + 1] == hl.derefs_col[i]) || !(ops.claims_dotp[3 * i + 2] == hl.eval_val[i]))
       throw Reject("dot product claims");
   {
-    std::vector<Fq> ev;
-    for (auto* v : {&hl.row_addr, &hl.row_read_ts, &hl.col_addr, &hl.col_read_ts, &hl.eval_val}) ev.insert(ev.end(), v->begin(), v->end());
-    ev.resize(pow2c(ev.size()), Fq::zero());
-    T.append_scalars("claim_evals_ops", ev);
-    std::vector<Fq> ch = T.challenge_vector("challenge_combine_n_to_one", log2c(ev.size()));
-    Fq joint = bound_bot(ev, ch)[0];
-    T.append_scalar("joint_claim_eval_ops", joint);
-    std::vector<Fq> r_joint = ch;
-    r_joint.insert(r_joint.end(), rand_ops.begin(), rand_ops.end());
+    const std::vector<Fq> r_joint = combine_to_one(T, hl, HashOpening::ops, rand_ops, joint);
     polyeval_verify_plain(ctx, hl.proof_ops, gens.gens_ops, T, r_joint, joint, comm.comm_comb_ops);
   }
   {
-    std::vector<Fq> ev = {hl.row_audit_ts, hl.col_audit_ts};
-    T.append_scalars("claim_evals_mem", ev);
-    std::vector<Fq> ch = T.challenge_vector("challenge_combine_two_to_one", 1);
-    Fq joint = bound_bot(ev, ch)[0];
-    T.append_scalar("joint_claim_eval_mem", joint);
-    std::vector<Fq> r_joint = ch;
-    r_joint.insert(r_joint.end(), rand_mem.begin(), rand_mem.end());
+    const std::vector<Fq> r_joint = combine_to_one(T, hl, HashOpening::mem, rand_mem, joint);
     polyeval_verify_plain(ctx, hl.proof_mem, gens.gens_mem, T, r_joint, joint, comm.comm_comb_mem);
   }
   hash_helper(rand_mem, mem.claims[0], row_read, row_write, mem.claims[1], hl.derefs_row, hl.row_addr, hl.row_read_ts, hl.row_audit_ts, rx, r_hash, r_multiset);
@@ -508,19 +382,6 @@ void spark_verify(Ctx& ctx, const SparseMatPolyEvalProof& p, const SnarkEncoding
 }
 
 }  // namespace
-
-// inst.evaluate(rx, ry) (r1cs.rs:300-303 -> sparse_mlpoly.rs:440-452) on the device
-void instance_evaluate(Ctx& ctx, const Instance& inst, const std::vector<Fq>& rx, const std::vector<Fq>& ry, Fq out[3]) {
-  DevBuf<u256> d_chal(rx.size() + ry.size() + 2), trx((size_t)1 << rx.size()), try_((size_t)1 << ry.size());
-  DevBuf<u256> eq_small(2 * ((size_t)1 << ((std::max(rx.size(), ry.size()) + 1) / 2)) + 8);
-  dev::h2d(d_chal.p, rx.data(), rx.size() * sizeof(u256), ctx.stream);
-  dev::eq_evals(trx.p, d_chal.p, (int)rx.size(), eq_small.p, ctx.stream);
-  dev::h2d(d_chal.p + rx.size(), ry.data(), ry.size() * sizeof(u256), ctx.stream);
-  dev::eq_evals(try_.p, d_chal.p + rx.size(), (int)ry.size(), eq_small.p, ctx.stream);
-  for (int m = 0; m < 3; m++)
-    dev::sparse_eval3(ctx.small.p + 40 + m, inst.M[m].coo_row.p, inst.M[m].coo_col.p, inst.M[m].coo_val.p, inst.M[m].nnz, trx.p, try_.p, ctx.red.p, ctx.stream);
-  ctx.get_small(40, out, 3);
-}
 
 static bool pow2(size_t x) { return x && !(x & (x - 1)); }
 // shape sanity shared by both verifiers: the padded dimensions the prover enforces (lib.rs:129-198, r1csproof.rs:156); without it a
@@ -533,16 +394,10 @@ static void check_dims(size_t num_cons, size_t num_vars, size_t num_inputs) {
 // NIZK::verify (lib.rs:549-591)
 void nizk_verify(Ctx& ctx, const Instance& inst, const std::vector<Fq>& input, const R1CSGens& gens, Transcript& T, const uint8_t* proof, size_t len) {
   check_dims(inst.num_cons, inst.num_vars, inst.num_inputs);
-  Reader r(proof, len);
-  NizkProof p;
-  rd(r, p.r1cs_sat_proof);
-  p.rx = r.scalars(); p.ry = r.scalars();
-  if (r.pos != len) throw Reject("trailing bytes");
+  const NizkProof p = from_bincode<NizkProof>(proof, len, SP_ERR_VERIFY, "proof");
   if (input.size() != inst.num_inputs) throw Reject("number of inputs");
-  if (p.rx.size() != log2c(inst.num_cons) || p.ry.size() != log2c(2 * inst.num_vars)) throw Reject("claimed evaluation point");
-  T.append_protocol_name("Spartan NIZK proof");
-  const std::vector<uint8_t>& digest = inst.shape_digest();   // computed here if the caller did not supply its own (r1cs.rs:154-158)
-  T.append_message("R1CSShapeDigest", digest.data(), digest.size());
+  if (p.rx.size() != log2_ceil(inst.num_cons) || p.ry.size() != log2_ceil(2 * inst.num_vars)) throw Reject("claimed evaluation point");
+  append_nizk_head(T, inst);
   Fq evals[3];
   instance_evaluate(ctx, inst, p.rx, p.ry, evals);
   std::vector<Fq> rx, ry;
@@ -550,8 +405,9 @@ void nizk_verify(Ctx& ctx, const Instance& inst, const std::vector<Fq>& input, c
   if (!(rx == p.rx) || !(ry == p.ry)) throw Reject("evaluation point differs from the sumcheck challenges");
 }
 
-// SNARK::verify (lib.rs:423-465); `comm` supplies the ComputationCommitment
-void snark_verify(Ctx& ctx, const SnarkEncoding& comm, const std::vector<Fq>& input, const SnarkGens& gens, Transcript& T, const uint8_t* proof, size_t len) {
+// SNARK::verify (lib.rs:423-465); `enc` supplies the ComputationCommitment
+void snark_verify(Ctx& ctx, const SnarkEncoding& enc, const std::vector<Fq>& input, const SnarkGens& gens, Transcript& T, const uint8_t* proof, size_t len) {
+  const ComputationCommitment& comm = enc.comm;
   check_dims(comm.num_cons, comm.num_vars, comm.num_inputs);
   {  // SparseMatPolyCommitment consistency (sparse_mlpoly.rs:366-420): 3 matrices, power-of-two op count of at least 2 (what snark_encode
      // produces: one op leaves the product circuits without layers), cells = max(num_cons, 2*num_vars)
@@ -559,28 +415,17 @@ void snark_verify(Ctx& ctx, const SnarkEncoding& comm, const std::vector<Fq>& in
     if (comm.batch_size != 3 || !pow2(comm.num_ops) || comm.num_ops < 2 || comm.num_mem_cells != cells)
       throw SpError(SP_ERR_INVALID_ARG, "verifier: inconsistent computation commitment");
   }
-  Reader r(proof, len);
-  R1CSProof sat;
-  rd(r, sat);
-  Fq evals[3];
-  for (auto& e : evals) e = r.scalar();
-  SparseMatPolyEvalProof ep;
-  ep.comm_derefs.C = r.points();
-  rd(r, ep.proof_prod_layer);
-  rd(r, ep.proof_hash_layer);
-  if (r.pos != len) throw Reject("trailing bytes");
+  const SnarkProof p = from_bincode<SnarkProof>(proof, len, SP_ERR_VERIFY, "proof");
   if (input.size() != comm.num_inputs) throw Reject("number of inputs");
   T.append_protocol_name("Spartan SNARK proof");
-  T.append_u64("num_cons", comm.num_cons); T.append_u64("num_vars", comm.num_vars); T.append_u64("num_inputs", comm.num_inputs);
-  T.append_u64("batch_size", comm.batch_size); T.append_u64("num_ops", comm.num_ops); T.append_u64("num_mem_cells", comm.num_mem_cells);
-  append_poly_commitment(T, "comm_comb_ops", comm.comm_comb_ops);
-  append_poly_commitment(T, "comm_comb_mem", comm.comm_comb_mem);
+  append_computation_commitment(T, comm);
+  const Fq* evals = p.inst_evals.data();
   std::vector<Fq> rx, ry;
-  r1cs_verify(ctx, sat, comm.num_vars, comm.num_cons, input, evals, T, *gens.gens_r1cs_sat, rx, ry);
+  r1cs_verify(ctx, p.r1cs_sat_proof, comm.num_vars, comm.num_cons, input, evals, T, *gens.gens_r1cs_sat, rx, ry);
   T.append_scalar("Ar_claim", evals[0]);
   T.append_scalar("Br_claim", evals[1]);
   T.append_scalar("Cr_claim", evals[2]);
-  spark_verify(ctx, ep, comm, rx, ry, evals, gens, T);
+  spark_verify(ctx, p.r1cs_eval_proof, comm, rx, ry, evals, gens, T);
 }
 
 }  // namespace sp
