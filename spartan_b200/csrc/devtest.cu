@@ -1,13 +1,19 @@
 // spartan_b200 — device test hooks, the GPU counterpart of hosttest.cpp.  Built with the kernels' nvcc flags, so the field and curve arithmetic
 // here is the code the kernels run on the device (inline-PTX carry chains, generated multiplications, quad-lane point operations), not the portable
-// formulation the CPU tests check.  Not linked into libspartan_b200.so.
+// formulation the CPU tests check.  Not linked into libspartan_b200.so; linked with the kernel objects of libspartan_b200.so instead, so the
+// kernel hooks below (spd_sc_*, spd_eq_*, ...) launch the library's own kernels through the sp::dev wrappers of dev.hpp.
 //
-// Every entry point takes host arrays of n elements, copies them to the device, runs one elementwise kernel (one thread per element, or one quad of
-// lanes per point for the quad-lane operations), copies the results back and returns the CUDA status (0 = success).
+// Every arithmetic entry point takes host arrays of n elements, copies them to the device, runs one elementwise kernel (one thread per element, or
+// one quad of lanes per point for the quad-lane operations), copies the results back and returns the CUDA status (0 = success).
 //   u256:     8 little-endian 32-bit limbs.  F_q operands are Montgomery limbs, passed and returned unchanged; F_p operands may be any value < 2^256.
 //   ge:       the four coordinates X, Y, Z, T as u256 (any representatives, not necessarily reduced or normalised).
 //   ge_niels: y + x, y - x, 2dxy as u256.
+// Every kernel hook also takes and returns host arrays (F_q values as Montgomery limbs), runs the wrappers on a stream of its own, frees its device
+// and pinned buffers on return and returns 0, a CUDA status, or SPD_REFUSED when a wrapper threw (spd_last_error() then holds its message).
 #include <cuda_runtime.h>
+#include <string.h>
+#include <exception>
+#include <string>
 #include <vector>
 #include "kcommon.cuh"
 #include "quad.cuh"
@@ -42,6 +48,44 @@ struct Call {
   void launched() { if (err == cudaSuccess) err = cudaGetLastError(); }
   ~Call() { for (void* p : bufs) if (p) cudaFree(p); }
 };
+
+// one call of a kernel hook: a Call whose wrappers run on a stream of its own (a blocking stream: ordered after the synchronous copies of in() and
+// before those of out()), drained before the buffers go, plus zeroed device and pinned host buffers for scratch and the HostSig words
+constexpr int SPD_REFUSED = -1;
+std::string g_last_error;
+struct KCall : Call {
+  cudaStream_t s = nullptr;
+  std::vector<void*> pinned;
+  KCall() { err = cudaStreamCreate(&s); }
+  ~KCall() {
+    if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
+    for (void* p : pinned) if (p) cudaFreeHost(p);
+  }
+  template <class T> T* zeros(size_t n) {
+    T* d = alloc<T>(n);
+    if (err == cudaSuccess) err = cudaMemset(d, 0, n * sizeof(T));
+    return d;
+  }
+  template <class T> T* host(size_t n) {
+    void* p = nullptr;
+    if (err == cudaSuccess) err = cudaMallocHost(&p, n * sizeof(T));
+    if (err == cudaSuccess) memset(p, 0, n * sizeof(T));
+    pinned.push_back(p);
+    return (T*)p;
+  }
+  void sync() { if (err == cudaSuccess) err = cudaStreamSynchronize(s); }
+};
+// a wrapper's std::exception (a refused argument, a CUDA error it checked) becomes SPD_REFUSED; the KCall inside `f` is unwound first
+template <class F> int guarded(F&& f) {
+  try {
+    return f();
+  } catch (const std::exception& e) {
+    g_last_error = e.what();
+    return SPD_REFUSED;
+  }
+}
+// reduction scratch of the dot / sparse kernels: [counters][partials], the same layout as the sumcheck kernels' (>= 32 tables)
+size_t red_scratch_bytes() { return sc_scratch_bytes(32); }
 
 enum FqOp { FQ_MUL, FQ_ADD, FQ_SUB, FQ_NEG, FQ_FROM_MONT, FQ_TO_MONT, FQ_FROM_WIDE, FQ_FROM_U64, FQ_INV };
 enum FpOp { FP_MUL, FP_ADD, FP_SUB, FP_NEG, FP_MUL_SMALL, FP_CANON, FP_INV, FP_POW22523 };
@@ -350,5 +394,434 @@ int spd_window_digits(size_t n, const u256* k, int wbits, int* out) {
   c.launched();
   c.out(out, dout, n * nwin);
   return (int)c.err;
+}
+
+// ---------------------------------------------------------------------------------------------------- kernel hooks (the sp::dev wrappers)
+const char* spd_last_error() { return g_last_error.c_str(); }
+unsigned long long spd_launch_count() { return launch_count(); }
+void spd_prof_enable(int on) { prof_enable(on != 0); }
+// "name:launches:total_ms:total_algorithmic_bytes;..." of the kernel families launched since spd_prof_enable(1), truncated to cap - 1 characters
+size_t spd_prof_report(char* buf, size_t cap) {
+  const std::string r = prof_report();
+  if (cap) { const size_t n = r.size() < cap - 1 ? r.size() : cap - 1; memcpy(buf, r.data(), n); buf[n] = 0; }
+  return r.size();
+}
+
+// A chain of batched sumcheck rounds: sc_eval on len entries, then nfold sc_fold_eval rounds with rs[0 .. nfold).  The tables live in nbuf
+// buffers of len entries (`tables`, back to back); table t of instance i is buffer map[4 i + t] (-1: none), its folded C goes to buffer cbuf[i]
+// when write_c[i].  A C shared by several instances is folded by one of them into a buffer of its own (cbuf[i] != map[4 i + 2]); after the round
+// every instance that read it reads the folded copy, and the writer's next fold goes back to the first buffer, as the prover's ping-pong does.
+// use_sig: every launch also publishes through a HostSig (seq = round + 1); host_out[round], flags[round] and dones[round] are the pinned results,
+// the flag word and the device completion counter after the launch.  bound (use_sig, a fold to two-entry tables): the host_bound area of that
+// fold.  On return: out[round] (ninst x 3 each), the buffers (tables_out) and the scratch's 64 ticket counters.
+int spd_sc_chain(int kind, int ninst, size_t len, int nbuf, const u256* tables, const int* map, const int* cbuf, const int* write_c, int nfold,
+                 const u256* rs, int use_sig, u256* out, u256* host_out, unsigned* flags, unsigned* dones, u256* bound, u256* tables_out,
+                 unsigned* counters) {
+  if (kind < SC_QUAD || kind > SC_CUBIC4 || ninst < 1 || ninst > 64 || nbuf < 1 || nfold < 0 || nfold > 40 || (nfold && (len >> nfold) < 2)) return (int)cudaErrorInvalidValue;
+  return guarded([&] {
+    KCall c;
+    const int nt = kind == SC_QUAD ? 2 : kind == SC_CUBIC3 ? 3 : 4;
+    u256* d = c.in(tables, (size_t)nbuf * len);
+    void* scratch = c.zeros<char>(sc_scratch_bytes(ninst));
+    u256* dout = c.zeros<u256>(3 * (size_t)ninst);
+    HostSig sig;
+    if (use_sig) { sig.host_out = c.host<u256>(3 * (size_t)ninst); sig.flag = c.host<unsigned>(1); sig.done = c.zeros<unsigned>(1); }
+    u256* hb = bound ? c.host<u256>(2 * (size_t)nt * ninst) : nullptr;
+    if (!c.ok()) return (int)c.err;
+    std::vector<int> m(map, map + 4 * ninst), co(cbuf, cbuf + ninst);
+    std::vector<ScInst> in(ninst);
+    XRank xr;
+    xr.world = 1;
+    size_t cur = len;
+    for (int k = 0; k <= nfold && c.ok(); k++) {
+      for (int i = 0; i < ninst; i++) {
+        for (int t = 0; t < 4; t++) in[i].t[t] = m[4 * i + t] >= 0 ? d + (size_t)m[4 * i + t] * len : nullptr;
+        in[i].c_out = co[i] >= 0 ? d + (size_t)co[i] * len : nullptr;
+        in[i].write_c = write_c[i];
+      }
+      sig.seq = (unsigned)k + 1;
+      if (k == 0) {
+        sc_eval((ScKind)kind, in.data(), ninst, cur, dout, scratch, c.s, sig, xr);
+      } else {
+        sc_fold_eval((ScKind)kind, in.data(), ninst, cur, rs[k - 1], dout, scratch, c.s, sig, xr, cur == 4 ? hb : nullptr);
+        cur >>= 1;
+      }
+      c.sync();
+      c.out(out + (size_t)k * 3 * ninst, dout, 3 * (size_t)ninst);
+      if (use_sig && c.ok()) {
+        memcpy(host_out + (size_t)k * 3 * ninst, sig.host_out, 3 * (size_t)ninst * sizeof(u256));
+        flags[k] = *(volatile unsigned*)sig.flag;
+        c.out(dones + k, sig.done, 1);
+      }
+      if (k > 0 && cur == 2 && hb && c.ok()) memcpy(bound, hb, 2 * (size_t)nt * ninst * sizeof(u256));
+      if (k > 0 && nt > 2)
+        for (int i = 0; i < ninst; i++) {
+          const int old = m[4 * i + 2], nw = co[i];
+          if (!write_c[i] || nw < 0 || nw == old) continue;
+          for (int j = 0; j < ninst; j++) if (m[4 * j + 2] == old) m[4 * j + 2] = nw;
+          co[i] = old;
+        }
+    }
+    c.out(tables_out, d, (size_t)nbuf * len);
+    c.out(counters, (unsigned*)scratch, 64);
+    return (int)c.err;
+  });
+}
+
+// The eq-factored chain of batched_prove on ninst instances of A * B * eq(tau, .): A_i, B_i of len = 2^n entries (a, b back to back), E0 =
+// eq(tau[1..], .) (len/2 entries).  eq_suffix builds the levels E_1 .. E_{jG-1}; rounds 0 .. jG-1 run sc_eval_g / sc_fold_eval_g(rs[j-1]) on E_j
+// (out[round][i] = q(0), q(inf), 0); round jG binds A and B with rs[jG-1] (fold_top) and runs sc_eval(SC_CUBIC3) on C = E_{jG-1}, instance 0
+// folding the shared C into a ping-pong pair; rounds jG+1 .. n-1 run sc_fold_eval(SC_CUBIC3) down to two-entry tables.  use_sig as spd_sc_chain.
+// On return a, b hold the bound tables (2 entries per instance, the first two of each table).
+int spd_sc_g_chain(int ninst, size_t len, u256* a, u256* b, const u256* E0, int jG, const u256* rs, int use_sig, u256* out, u256* host_out,
+                   unsigned* flags, unsigned* dones) {
+  int n = 0;
+  while (((size_t)1 << n) < len) n++;
+  if (ninst < 1 || ninst > 64 || ((size_t)1 << n) != len || jG < 1 || jG >= n) return (int)cudaErrorInvalidValue;
+  return guarded([&] {
+    KCall c;
+    u256* dA = c.in(a, (size_t)ninst * len);
+    u256* dB = c.in(b, (size_t)ninst * len);
+    const size_t n0 = len / 2;
+    u256* dE0 = c.in(E0, n0);
+    size_t nlev = 0;
+    for (int k = 1; k < jG; k++) nlev += n0 >> k;
+    u256* levels = c.alloc<u256>(nlev ? nlev : 1);
+    const size_t chalf = (len >> jG) / 2;
+    u256* cp[2] = {c.alloc<u256>(chalf), c.alloc<u256>(chalf)};
+    void* scratch = c.zeros<char>(sc_scratch_bytes(ninst));
+    u256* dout = c.zeros<u256>(3 * (size_t)ninst);
+    HostSig sig;
+    if (use_sig) { sig.host_out = c.host<u256>(3 * (size_t)ninst); sig.flag = c.host<unsigned>(1); sig.done = c.zeros<unsigned>(1); }
+    if (!c.ok()) return (int)c.err;
+    std::vector<u256*> E(jG);
+    E[0] = dE0;
+    for (size_t k = 1, off = 0; k < (size_t)jG; k++) { E[k] = levels + off; off += n0 >> k; }
+    if (jG > 1) eq_suffix(levels, dE0, n0, jG - 1, c.s);
+    std::vector<ScInst> in(ninst);
+    std::vector<u256*> ab;
+    for (int i = 0; i < ninst; i++) {
+      in[i].t[0] = dA + (size_t)i * len; in[i].t[1] = dB + (size_t)i * len; in[i].t[2] = in[i].t[3] = nullptr;
+      in[i].c_out = nullptr; in[i].write_c = 0;
+      ab.push_back(in[i].t[0]); ab.push_back(in[i].t[1]);
+    }
+    XRank xr;
+    xr.world = 1;
+    size_t cur = len;
+    for (int j = 0; j < n && c.ok(); j++) {
+      sig.seq = (unsigned)j + 1;
+      if (j == 0) sc_eval_g(in.data(), ninst, cur, E[0], dout, scratch, c.s, sig, xr);
+      else if (j < jG) { sc_fold_eval_g(in.data(), ninst, cur, rs[j - 1], E[j], dout, scratch, c.s, sig, xr); cur >>= 1; }
+      else if (j == jG) {
+        fold_top(ab.data(), (int)ab.size(), cur, rs[j - 1], c.s);
+        cur >>= 1;
+        for (int i = 0; i < ninst; i++) { in[i].t[2] = E[jG - 1]; in[i].c_out = cp[0]; in[i].write_c = i == 0; }
+        sc_eval(SC_CUBIC3, in.data(), ninst, cur, dout, scratch, c.s, sig, xr);
+      } else {
+        sc_fold_eval(SC_CUBIC3, in.data(), ninst, cur, rs[j - 1], dout, scratch, c.s, sig, xr);
+        cur >>= 1;
+        u256* folded = in[0].c_out;
+        for (int i = 0; i < ninst; i++) { in[i].t[2] = folded; in[i].c_out = folded == cp[0] ? cp[1] : cp[0]; }
+      }
+      c.sync();
+      c.out(out + (size_t)j * 3 * ninst, dout, 3 * (size_t)ninst);
+      if (use_sig && c.ok()) {
+        memcpy(host_out + (size_t)j * 3 * ninst, sig.host_out, 3 * (size_t)ninst * sizeof(u256));
+        flags[j] = *(volatile unsigned*)sig.flag;
+        c.out(dones + j, sig.done, 1);
+      }
+    }
+    for (int i = 0; i < ninst; i++) {
+      c.out(a + (size_t)i * len, dA + (size_t)i * len, 2);
+      c.out(b + (size_t)i * len, dB + (size_t)i * len, 2);
+    }
+    return (int)c.err;
+  });
+}
+
+// levels[k-1] (k = 1 .. K, n0 >> k entries each, back to back) from E0 (n0 entries)
+int spd_eq_suffix(size_t n0, int K, const u256* E0, u256* levels) {
+  return guarded([&] {
+    KCall c;
+    size_t total = 0;
+    for (int k = 1; k <= K; k++) total += n0 >> k;
+    const u256* dE = c.in(E0, n0);
+    u256* dl = c.alloc<u256>(total ? total : 1);
+    if (c.ok()) eq_suffix(dl, dE, n0, K, c.s);
+    c.sync();
+    c.out(levels, dl, total);
+    return (int)c.err;
+  });
+}
+// out (2^ell entries) = eq(r, .)
+int spd_eq_evals(int ell, const u256* r, u256* out) {
+  if (ell < 0 || ell > 30) return (int)cudaErrorInvalidValue;
+  return guarded([&] {
+    KCall c;
+    const size_t n = (size_t)1 << ell;
+    const u256* dr = c.in(r, ell ? (size_t)ell : 1);
+    u256* dout = c.alloc<u256>(n);
+    u256* small = c.alloc<u256>(eq_evals_scratch(ell));
+    if (c.ok()) eq_evals(dout, dr, ell, small, c.s);
+    c.sync();
+    c.out(out, dout, n);
+    return (int)c.err;
+  });
+}
+// out (2n entries) = [(1 - r) E | r E] from E (n entries)
+int spd_eq_extend_top(size_t n, const u256* E, const u256* r, u256* out) {
+  return guarded([&] {
+    KCall c;
+    u256* d = c.alloc<u256>(2 * n);
+    if (c.ok()) c.err = cudaMemcpy(d + n, E, n * sizeof(u256), cudaMemcpyHostToDevice);
+    if (c.ok()) eq_extend_top(d, n, *r, c.s);
+    c.sync();
+    c.out(out, d, 2 * n);
+    return (int)c.err;
+  });
+}
+// out[k] = tables[k * n_each] for k < count; use_sig: host_out and *flag (seq 7) are the published copy
+int spd_heads(int count, size_t n_each, const u256* tables, int use_sig, u256* out, u256* host_out, unsigned* flag) {
+  return guarded([&] {
+    KCall c;
+    u256* d = c.in(tables, (size_t)count * n_each);
+    u256* dout = c.zeros<u256>(64);
+    HostSig sig;
+    if (use_sig) { sig.host_out = c.host<u256>(64); sig.flag = c.host<unsigned>(1); sig.seq = 7; }
+    if (!c.ok()) return (int)c.err;
+    std::vector<const u256*> p(count);
+    for (int k = 0; k < count; k++) p[k] = d + (size_t)k * n_each;
+    heads(dout, p.data(), count, c.s, sig);
+    c.sync();
+    c.out(out, dout, (size_t)count);
+    if (use_sig && c.ok()) { memcpy(host_out, sig.host_out, (size_t)count * sizeof(u256)); *flag = *(volatile unsigned*)sig.flag; }
+    return (int)c.err;
+  });
+}
+// fold_top of ntables tables of len entries (back to back, in place: the first len/2 entries of each are the result)
+int spd_fold_top(int ntables, size_t len, u256* tables, const u256* r) {
+  return guarded([&] {
+    KCall c;
+    u256* d = c.in(tables, (size_t)ntables * len);
+    if (!c.ok()) return (int)c.err;
+    std::vector<u256*> p(ntables);
+    for (int k = 0; k < ntables; k++) p[k] = d + (size_t)k * len;
+    fold_top(p.data(), ntables, len, *r, c.s);
+    c.sync();
+    c.out(tables, d, (size_t)ntables * len);
+    return (int)c.err;
+  });
+}
+
+// ---- SPARK layer and dense helpers
+// out = ts * r^2 + val * r + addr - g over n entries; addr / ts null: the index / zero; rg = [r, g]
+int spd_spark_hash(size_t n, const u256* addr, const u256* val, const u256* ts, int ts_plus_one, const u256* rg, u256* out) {
+  return guarded([&] {
+    KCall c;
+    const u256* da = addr ? c.in(addr, n) : nullptr;
+    const u256* dv = c.in(val, n);
+    const u256* dt = ts ? c.in(ts, n) : nullptr;
+    const u256* drg = c.in(rg, 2);
+    u256* dout = c.alloc<u256>(n);
+    if (c.ok()) spark_hash(dout, n, da, dv, dt, ts_plus_one, drg, c.s);
+    c.sync();
+    c.out(out, dout, n);
+    return (int)c.err;
+  });
+}
+// the same on rank `rank` of `world` (n / world local entries, global index j * world + rank) from the unsharded arrays
+int spd_spark_hash_cyclic(size_t n, int rank, int world, const u256* addr, const u256* val, const u256* ts, int ts_plus_one, const u256* rg, u256* out) {
+  if (world < 1 || rank < 0 || rank >= world || n % world) return (int)cudaErrorInvalidValue;
+  return guarded([&] {
+    KCall c;
+    const u256* da = addr ? c.in(addr, n) : nullptr;
+    const u256* dv = c.in(val, n);
+    const u256* dt = ts ? c.in(ts, n) : nullptr;
+    const u256* drg = c.in(rg, 2);
+    u256* dout = c.alloc<u256>(n / world);
+    if (c.ok()) spark_hash_cyclic(dout, n / world, rank, world, da, dv, dt, ts_plus_one, drg, c.s);
+    c.sync();
+    c.out(out, dout, n / world);
+    return (int)c.err;
+  });
+}
+// out[k] = a[k] o b[k] for count circuits of n entries (back to back)
+int spd_hadamard_many(int count, size_t n, const u256* a, const u256* b, u256* out) {
+  return guarded([&] {
+    KCall c;
+    const u256* da = c.in(a, (size_t)count * n);
+    const u256* db = c.in(b, (size_t)count * n);
+    u256* dout = c.alloc<u256>((size_t)count * n);
+    if (!c.ok()) return (int)c.err;
+    std::vector<u256*> po(count);
+    std::vector<const u256*> pa(count), pb(count);
+    for (int k = 0; k < count; k++) { po[k] = dout + (size_t)k * n; pa[k] = da + (size_t)k * n; pb[k] = db + (size_t)k * n; }
+    hadamard_many(po.data(), pa.data(), pb.data(), count, n, c.s);
+    c.sync();
+    c.out(out, dout, (size_t)count * n);
+    return (int)c.err;
+  });
+}
+// out[i] = mem[idx[i]]
+int spd_gather(size_t cells, const u256* mem, size_t n, const uint32_t* idx, u256* out) {
+  return guarded([&] {
+    KCall c;
+    const u256* dm = c.in(mem, cells);
+    const uint32_t* di = c.in(idx, n);
+    u256* dout = c.alloc<u256>(n);
+    if (c.ok()) gather(dout, dm, di, n, c.s);
+    c.sync();
+    c.out(out, dout, n);
+    return (int)c.err;
+  });
+}
+// *out = sum a b (c null: dot) or sum a b c (dot3)
+int spd_dot3(size_t n, const u256* a, const u256* b, const u256* cc, u256* out) {
+  return guarded([&] {
+    KCall c;
+    const u256* da = c.in(a, n);
+    const u256* db = c.in(b, n);
+    const u256* dc = cc ? c.in(cc, n) : nullptr;
+    void* scratch = c.zeros<char>(red_scratch_bytes());
+    u256* dout = c.zeros<u256>(1);
+    if (c.ok()) { if (dc) dot3(dout, da, db, dc, n, scratch, c.s); else dot(dout, da, db, n, scratch, c.s); }
+    c.sync();
+    c.out(out, dout, 1);
+    return (int)c.err;
+  });
+}
+// out[k] = <a[k], b> for count tables of n entries (back to back)
+int spd_dot_many(int count, size_t n, const u256* a, const u256* b, u256* out) {
+  return guarded([&] {
+    KCall c;
+    const u256* da = c.in(a, (size_t)count * n);
+    const u256* db = c.in(b, n);
+    void* scratch = c.zeros<char>(red_scratch_bytes());
+    u256* dout = c.zeros<u256>(count > 0 ? (size_t)count : 1);
+    if (!c.ok()) return (int)c.err;
+    std::vector<const u256*> pa(count);
+    for (int k = 0; k < count; k++) pa[k] = da + (size_t)k * n;
+    dot_many(dout, pa.data(), count, db, n, scratch, c.s);
+    c.sync();
+    c.out(out, dout, (size_t)count);
+    return (int)c.err;
+  });
+}
+// out = ra A + rb B + rc C, rabc = [ra, rb, rc]
+int spd_lincomb3(size_t n, const u256* A, const u256* B, const u256* Cc, const u256* rabc, u256* out) {
+  return guarded([&] {
+    KCall c;
+    const u256* da = c.in(A, n);
+    const u256* db = c.in(B, n);
+    const u256* dc = c.in(Cc, n);
+    const u256* dr = c.in(rabc, 3);
+    u256* dout = c.alloc<u256>(n);
+    if (c.ok()) lincomb3(dout, da, db, dc, dr, n, c.s);
+    c.sync();
+    c.out(out, dout, n);
+    return (int)c.err;
+  });
+}
+// out[i] = sum_j L[j] Z[j R_size + i]
+int spd_bound_rows(size_t L_size, size_t R_size, const u256* Z, const u256* L, u256* out) {
+  return guarded([&] {
+    KCall c;
+    const u256* dz = c.in(Z, L_size * R_size);
+    const u256* dl = c.in(L, L_size);
+    u256* scratch = c.alloc<u256>(64 * R_size);
+    u256* dout = c.alloc<u256>(R_size);
+    if (c.ok()) bound_rows(dout, dz, dl, L_size, R_size, scratch, c.s);
+    c.sync();
+    c.out(out, dout, R_size);
+    return (int)c.err;
+  });
+}
+// Montgomery limbs -> canonical little-endian integers
+int spd_to_canonical(size_t n, const u256* in, u256* out) {
+  return guarded([&] {
+    KCall c;
+    const u256* di = c.in(in, n);
+    u256* dout = c.alloc<u256>(n);
+    if (c.ok()) to_canonical(dout, di, n, c.s);
+    c.sync();
+    c.out(out, dout, n);
+    return (int)c.err;
+  });
+}
+
+// ---- sparse products on caller CSR / COO arrays
+int spd_spmv(size_t nrows, size_t nnz, const uint32_t* ptr, const uint32_t* idx, const u256* val, size_t ncols, const u256* x, u256* out) {
+  return guarded([&] {
+    KCall c;
+    const uint32_t* dp = c.in(ptr, nrows + 1);
+    const uint32_t* di = c.in(idx, nnz);
+    const u256* dv = c.in(val, nnz);
+    const u256* dx = c.in(x, ncols);
+    u256* dout = c.alloc<u256>(nrows);
+    if (c.ok()) spmv(dout, nrows, dp, di, dv, dx, c.s);
+    c.sync();
+    c.out(out, dout, nrows);
+    return (int)c.err;
+  });
+}
+// rows j * world + rank of the CSR (nrows / world of them)
+int spd_spmv_cyclic(size_t nrows, int rank, int world, size_t nnz, const uint32_t* ptr, const uint32_t* idx, const u256* val, size_t ncols, const u256* x,
+                    u256* out) {
+  if (world < 1 || rank < 0 || rank >= world || nrows % world) return (int)cudaErrorInvalidValue;
+  return guarded([&] {
+    KCall c;
+    const uint32_t* dp = c.in(ptr, nrows + 1);
+    const uint32_t* di = c.in(idx, nnz);
+    const u256* dv = c.in(val, nnz);
+    const u256* dx = c.in(x, ncols);
+    u256* dout = c.alloc<u256>(nrows / world);
+    if (c.ok()) spmv_cyclic(dout, nrows / world, rank, world, dp, di, dv, dx, c.s);
+    c.sync();
+    c.out(out, dout, nrows / world);
+    return (int)c.err;
+  });
+}
+// *out = sum_k trx[row[k]] try[col[k]] val[k]
+int spd_sparse_eval3(size_t nnz, const uint32_t* row, const uint32_t* col, const u256* val, size_t nrx, const u256* trx, size_t nry, const u256* try_,
+                     u256* out) {
+  return guarded([&] {
+    KCall c;
+    const uint32_t* dr = c.in(row, nnz);
+    const uint32_t* dc = c.in(col, nnz);
+    const u256* dv = c.in(val, nnz);
+    const u256* dx = c.in(trx, nrx);
+    const u256* dy = c.in(try_, nry);
+    void* scratch = c.zeros<char>(red_scratch_bytes());
+    u256* dout = c.zeros<u256>(1);
+    if (c.ok()) sparse_eval3(dout, dr, dc, dv, nnz, dx, dy, scratch, c.s);
+    c.sync();
+    c.out(out, dout, 1);
+    return (int)c.err;
+  });
+}
+
+// ---- sharded table producers, on one GPU
+int spd_scale(size_t n, u256* inout, const u256* cst) {
+  return guarded([&] {
+    KCall c;
+    u256* d = c.in(inout, n);
+    if (c.ok()) scale(d, *cst, n, c.s);
+    c.sync();
+    c.out(inout, d, n);
+    return (int)c.err;
+  });
+}
+// out[j] = full[j * world + rank], j < n / world
+int spd_take_cyclic(size_t n, const u256* full, int rank, int world, u256* out) {
+  if (world < 1 || rank < 0 || rank >= world || n % world) return (int)cudaErrorInvalidValue;
+  return guarded([&] {
+    KCall c;
+    const u256* df = c.in(full, n);
+    u256* dout = c.alloc<u256>(n / world);
+    if (c.ok()) take_cyclic(dout, df, n / world, rank, world, c.s);
+    c.sync();
+    c.out(out, dout, n / world);
+    return (int)c.err;
+  });
 }
 }

@@ -172,31 +172,38 @@ def test_gens_upload(sb):
         sb.MultiCommitGens.from_points(bad)
 
 
+@pytest.mark.parametrize("ninst", [5, 24])
 @pytest.mark.parametrize("logn", [2, 5, 11, 14, 16])
-def test_sumcheck_batched(sb, logn):
-    """prove_cubic_batched's loops (sumcheck.rs:290-357): 5 instances, three of them sharing one C table (poly_C_par), whole chain of rounds"""
+def test_sumcheck_batched(sb, logn, ninst):
+    """prove_cubic_batched's loops (sumcheck.rs:290-357): 5 or 24 (SC_MAX_INST) instances, several of them sharing one C table (poly_C_par),
+    whole chain of rounds; 25 instances are refused"""
     from spartan_b200 import api
     n = 1 << logn
-    A = [edge_table(n, "ba%d" % i) for i in range(5)]
-    B = [edge_table(n, "bb%d" % i) for i in range(5)]
+    A = [edge_table(n, "ba%d" % i) for i in range(ninst)]
+    B = [edge_table(n, "bb%d" % i) for i in range(ninst)]
     Cs = [edge_table(n, "bc%d" % i) for i in range(3)]
-    cmap = [0, 0, 1, 0, 2]
+    cmap = [0, 0, 1, 0, 2] + [k % 3 for k in range(ninst - 5)]
     dA, dB = [sb.DensePolynomial(t) for t in A], [sb.DensePolynomial(t) for t in B]
     dC = [sb.DensePolynomial(t) for t in Cs]
     got = api.sumcheck_batched_eval(dA, dB, [dC[k] for k in cmap])
-    for i in range(5):
+    for i in range(ninst):
         assert oc.to_ints(got[i]) == oc.sc_eval_cubic(A[i], B[i], Cs[cmap[i]], None)
     for j in range(logn - 1):
         r = oc.arr_get(oc.prg_scalars("br", 1, j), 0)
         A = [oc.bound_top(t, r) for t in A]; B = [oc.bound_top(t, r) for t in B]; Cs = [oc.bound_top(t, r) for t in Cs]
         got = api.sumcheck_batched_fold_eval(dA, dB, [dC[k] for k in cmap], oc.to_arr([r])[0])
-        for i in range(5):
+        for i in range(ninst):
             assert oc.to_ints(got[i]) == oc.sc_eval_cubic(A[i], B[i], Cs[cmap[i]], None), (j, i)
         assert all(p.len() == len(A[0]) for p in dA + dB + dC)
     for t, p in zip(A + B + Cs, dA + dB + dC):
         assert np.array_equal(p.to_numpy(), t)
     with pytest.raises(api.SpartanB200Error):
         api.sumcheck_batched_eval([dA[0], dA[0]], dB[:2], dC[:2])
+    over = [dA[k % ninst] for k in range(25)]
+    with pytest.raises(api.SpartanB200Error):
+        api.sumcheck_batched_eval(over, [dB[k % ninst] for k in range(25)], [dC[k % 3] for k in range(25)])
+    with pytest.raises(api.SpartanB200Error):
+        api.sumcheck_batched_fold_eval(over, [dB[k % ninst] for k in range(25)], [dC[k % 3] for k in range(25)], oc.to_arr([3])[0])
 
 
 @pytest.mark.parametrize("n", [2, 32, 1024, 4096])

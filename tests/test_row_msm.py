@@ -67,10 +67,11 @@ def sb():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("L,R", [(64, 512), (96, 1024), (63, 512), (64, 511)])
+@pytest.mark.parametrize("L,R", [(64, 512), (96, 1024), (63, 512), (64, 511), (65, 600), (97, 767)])
 def test_commit_rows_row_tables(sb, L, R):
     """DensePolynomial::commit_inner on both sides of the row-table selection (64 rows of 512 terms or more take the row tables), with a zero
-    row, a zero column and the recoding's edge scalars planted; with and without blinds"""
+    row, a zero column and the recoding's edge scalars planted; with and without blinds.  65 and 97 rows leave a Horner block with one live row;
+    600 and 767 columns are not a multiple of the 256-column chunk, with the blind column and without"""
     g = sb.MultiCommitGens(R, b"row-msm-test")
     ref = oc.MultiCommitGens.new(R, b"row-msm-test")
     Z = oc.prg_scalars("row-msm%d_%d" % (L, R), L * R)
