@@ -247,6 +247,34 @@ int sp_nizk_verify_t(sp_ctx* ctx, const sp_instance* inst, const uint64_t* input
                      const uint8_t* proof, size_t proof_len);
 int sp_snark_verify_t(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t* inputs_mont, size_t ninputs, const sp_snark_gens* gens,
                       uint8_t* strobe_state /* in, out */, const uint8_t* proof, size_t proof_len);
+
+/* ---- batch verification: k proofs in one call.  Proof i is checked against comms[i] / insts[i] (one handle may repeat; every handle's sizes must
+ * match `gens`), inputs i (ninputs[i] scalars) and a fresh transcript labels[i] (label_lens[i] bytes) or, in the _t forms, the caller's transcript
+ * strobe_states[i] (in, out).  Each proof's group equations are weighted by random scalars and tested together with the other proofs' in one
+ * device pass (DESIGN.md "deferred checks"); a proof that fails any check is re-run as the single call would run it.  So:
+ *   status[i]   = what sp_*_verify / sp_*_verify_t returns for proof i (SP_OK, SP_ERR_VERIFY or SP_ERR_DECOMPRESS);
+ *   strobe_states[i] is left exactly as the single _t call leaves it, whether proof i is accepted or rejected;
+ *   sp_last_error = "proof <i>: " + the single call's message, for the lowest rejected i;
+ *   returns SP_OK when every proof is accepted, SP_ERR_VERIFY when one or more is rejected, or the usual code for bad arguments (NULL arrays,
+ *   a NULL seed, inputs not reduced, an inconsistent commitment) or device errors, in which case `status` and the states are not written.
+ *   k = 0 returns SP_OK.  A batch may hold up to 2^32 - 1 variable-base terms in all (a few hundred per proof); a larger one is refused with
+ *   SP_ERR_INVALID_ARG: split it.
+ * weight_seed: 32 bytes of FRESH OS RANDOMNESS on every call (like tape_seed): the weight of equation e of proof i is
+ * from_bytes_wide(SHAKE256("spartan-b200/v1/batch-verify" || seed || LE64(i) || LE64(e))), and anyone who knows the weights before the call can
+ * build a false proof that passes.  On a connected multi-GPU context the batch runs on this rank's GPU alone (no collectives). */
+int sp_snark_verify_batch(sp_ctx* ctx, size_t k, const sp_snark_encoding* const* comms, const uint64_t* const* inputs_mont, const size_t* ninputs,
+                          const sp_snark_gens* gens, const uint8_t* const* labels, const size_t* label_lens, const uint8_t* const* proofs,
+                          const size_t* proof_lens, const uint8_t weight_seed[32], int* status /* k, out */);
+int sp_nizk_verify_batch(sp_ctx* ctx, size_t k, const sp_instance* const* insts, const uint64_t* const* inputs_mont, const size_t* ninputs,
+                         const sp_nizk_gens* gens, const uint8_t* const* labels, const size_t* label_lens, const uint8_t* const* proofs,
+                         const size_t* proof_lens, const uint8_t weight_seed[32], int* status /* k, out */);
+int sp_snark_verify_batch_t(sp_ctx* ctx, size_t k, const sp_snark_encoding* const* comms, const uint64_t* const* inputs_mont, const size_t* ninputs,
+                            const sp_snark_gens* gens, uint8_t* const* strobe_states /* k x 203, in, out */, const uint8_t* const* proofs,
+                            const size_t* proof_lens, const uint8_t weight_seed[32], int* status /* k, out */);
+int sp_nizk_verify_batch_t(sp_ctx* ctx, size_t k, const sp_instance* const* insts, const uint64_t* const* inputs_mont, const size_t* ninputs,
+                           const sp_nizk_gens* gens, uint8_t* const* strobe_states /* k x 203, in, out */, const uint8_t* const* proofs,
+                           const size_t* proof_lens, const uint8_t weight_seed[32], int* status /* k, out */);
+
 /* merlin::Transcript::{new, append_message, challenge_bytes} on such a state buffer (transcript.rs:13-30), for hosts without merlin and for the tests */
 int sp_transcript_new(const uint8_t* label, size_t label_len, uint8_t* strobe_state /* out */);
 int sp_transcript_append_message(uint8_t* strobe_state, const uint8_t* label, size_t label_len, const uint8_t* msg, size_t msg_len);

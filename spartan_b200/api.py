@@ -18,7 +18,12 @@ class SpartanB200Error(RuntimeError):
 
 
 class ProofVerifyError(SpartanB200Error):
-    """errors.rs:5-12: InternalError (a check failed) or DecompressionError (a point of the proof does not decompress)"""
+    """errors.rs:5-12: InternalError (a check failed) or DecompressionError (a point of the proof does not decompress).  `code`: the C status,
+    SP_ERR_VERIFY or SP_ERR_DECOMPRESS"""
+
+    def __init__(self, msg, code=None):
+        super().__init__(msg)
+        self.code = code
 
 
 class R1CSError(SpartanB200Error):
@@ -81,9 +86,9 @@ class Context:
         if rc == SP_ERR_INVALID_INPUTS:
             raise R1CSError("InvalidNumberOfInputs: " + msg)
         if rc == SP_ERR_VERIFY:
-            raise ProofVerifyError("InternalError: " + msg)
+            raise ProofVerifyError("InternalError: " + msg, rc)
         if rc == SP_ERR_DECOMPRESS:
-            raise ProofVerifyError("DecompressionError: " + msg)
+            raise ProofVerifyError("DecompressionError: " + msg, rc)
         raise SpartanB200Error("spartan_b200 error %d: %s" % (rc, msg))
 
     def connect_peers(self, rank, world, allgather):
@@ -691,6 +696,15 @@ class NIZK:
         ctx.check(lib.sp_nizk_verify(ctx.h, inst.h, _p(inputs.limbs), _sz(len(inputs)), gens.h, C.c_char_p(transcript_label), _sz(len(transcript_label)),
                                      C.c_char_p(bytes(self.bytes)), _sz(len(self.bytes))))
 
+    @staticmethod
+    def verify_batch(proofs, inst, inputs, transcript_label, gens, seed=None):
+        """NIZK::verify for k proofs in one call (sp_nizk_verify_batch): `inst` one Instance or a list of k, `inputs` a list of k assignments,
+        `transcript_label` one label, k labels or k Transcript objects (advanced in place as NIZK.verify advances one).  Returns k entries: None
+        (accepted) or a ProofVerifyError whose `.code` is the status the single verify gives that proof; the lowest rejected proof's error also
+        carries the single verify's message, the others a generic one.  Rejections do not raise, bad arguments do.
+        seed=None (the default) draws the seed of the batch weights from the OS; a known seed lets a false proof pass."""
+        return _verify_batch(gens.ctx, lib.sp_nizk_verify_batch, lib.sp_nizk_verify_batch_t, inst, proofs, inputs, transcript_label, gens, seed)
+
 
 class SNARKGens:
     """lib.rs:277-309"""
@@ -782,6 +796,65 @@ class SNARK:
             return
         ctx.check(lib.sp_snark_verify(ctx.h, comm.h, _p(inputs.limbs), _sz(len(inputs)), gens.h, C.c_char_p(transcript_label), _sz(len(transcript_label)),
                                       C.c_char_p(bytes(self.bytes)), _sz(len(self.bytes))))
+
+    @staticmethod
+    def verify_batch(proofs, comm, inputs, transcript_label, gens, seed=None):
+        """SNARK::verify for k proofs in one call (sp_snark_verify_batch): `comm` one ComputationCommitment or a list of k; otherwise as
+        NIZK.verify_batch"""
+        return _verify_batch(gens.ctx, lib.sp_snark_verify_batch, lib.sp_snark_verify_batch_t, comm, proofs, inputs, transcript_label, gens, seed)
+
+
+def _verify_batch(ctx, entry, entry_t, handles, proofs, inputs, transcript_label, gens, seed):
+    """the shared body of SNARK.verify_batch / NIZK.verify_batch: one sp_*_verify_batch(_t) call, statuses -> [None | ProofVerifyError]"""
+    k = len(proofs)
+    if len(inputs) != k:
+        raise SpartanB200Error("verify_batch: %d proofs but %d input assignments" % (k, len(inputs)))
+    if not isinstance(handles, (list, tuple)):
+        handles = [handles] * k
+    if len(handles) != k:
+        raise SpartanB200Error("verify_batch: %d proofs but %d statements" % (k, len(handles)))
+    if isinstance(transcript_label, (bytes, bytearray)):
+        transcript_label = [bytes(transcript_label)] * k
+    if len(transcript_label) != k:
+        raise SpartanB200Error("verify_batch: %d proofs but %d transcripts" % (k, len(transcript_label)))
+    seed = os.urandom(32) if seed is None else bytes(seed)
+    if len(seed) != 32:
+        raise SpartanB200Error("verify_batch: the weight seed is 32 bytes")
+    datas = [bytes(p.bytes if hasattr(p, "bytes") else p) for p in proofs]
+    limbs = [np.ascontiguousarray(a.limbs, dtype=np.uint64) for a in inputs]
+    hs = (_vp * k)(*[h.h for h in handles])
+    ins = (_vp * k)(*[_p(a) for a in limbs])
+    nins = (_sz * k)(*[len(a) for a in limbs])
+    pbuf = (C.c_char_p * k)(*datas)
+    plens = (_sz * k)(*[len(d) for d in datas])
+    status = (C.c_int * k)()
+    if any(isinstance(t, Transcript) for t in transcript_label) and not all(isinstance(t, Transcript) for t in transcript_label):
+        raise SpartanB200Error("verify_batch: transcript_label mixes Transcript objects and labels")
+    if all(isinstance(t, Transcript) for t in transcript_label):
+        states = (_vp * k)(*[C.cast(t.state, _vp) for t in transcript_label])
+        rc = entry_t(ctx.h, _sz(k), hs, ins, nins, gens.h, states, pbuf, plens, C.c_char_p(seed), status)
+    else:
+        labels = [bytes(t) for t in transcript_label]
+        lbuf = (C.c_char_p * k)(*labels)
+        llens = (_sz * k)(*[len(t) for t in labels])
+        rc = entry(ctx.h, _sz(k), hs, ins, nins, gens.h, lbuf, llens, pbuf, plens, C.c_char_p(seed), status)
+    if rc not in (SP_OK, SP_ERR_VERIFY):
+        ctx.check(rc)
+    out = []
+    for i in range(k):
+        code = status[i]
+        if code == SP_OK:
+            out.append(None)
+        else:
+            kind = "DecompressionError" if code == SP_ERR_DECOMPRESS else "InternalError"
+            out.append(ProofVerifyError("%s: proof %d rejected (status %d)" % (kind, i, code), code))
+    if rc == SP_ERR_VERIFY:   # the message of the lowest rejected proof
+        first = next(i for i in range(k) if status[i] != SP_OK)
+        out[first] = ProofVerifyError(("DecompressionError: " if status[first] == SP_ERR_DECOMPRESS else "InternalError: ") +
+                                      lib.sp_last_error(ctx.h).decode(), status[first])
+    return out
+
+
 
 
 # ----------------------------------------------------------------------------- measurement helpers (bench.py)

@@ -905,6 +905,13 @@ int sp_snark_prove_resident(sp_ctx* ctx, const sp_instance* inst, const sp_snark
 // ---- verifiers.  The _t forms verify on the caller's transcript state (lib.rs:423-429, :549-555), which is updated in place whether or not the
 // proof is accepted (a _t prove writes it back only on success).
 struct TranscriptClose { const TranscriptArg& ta; const Transcript& T; ~TranscriptClose() { ta.close(T); } };
+// SP_FINE_TIMERS=1: the sub-phase timers of the last verify call (single or batch) replace sp_timings, as a prove call's do
+static void flush_fine(Ctx& c) {
+  if (!FineTimer::enabled()) return;
+  c.timings.clear();
+  for (auto& f : c.fine) c.timings.push_back({"fine:" + f.first, f.second});
+  c.fine.clear();
+}
 static int nizk_verify_common(sp_ctx* ctx, const sp_instance* inst, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens, const TranscriptArg& ta,
                               const uint8_t* proof, size_t proof_len) {
   SP_TRY(ctx)
@@ -913,6 +920,7 @@ static int nizk_verify_common(sp_ctx* ctx, const sp_instance* inst, const uint64
   Transcript T = ta.open();
   TranscriptClose close{ta, T};
   nizk_verify(ctx->c, inst->inst, fq_vec(inputs, ninputs), *gens->g, T, proof, proof_len);
+  flush_fine(ctx->c);
   SP_CATCH(ctx)
 }
 static int snark_verify_common(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t* inputs, size_t ninputs, const sp_snark_gens* gens,
@@ -923,6 +931,7 @@ static int snark_verify_common(sp_ctx* ctx, const sp_snark_encoding* comm, const
   Transcript T = ta.open();
   TranscriptClose close{ta, T};
   snark_verify(ctx->c, *comm->e, fq_vec(inputs, ninputs), *gens->g, T, proof, proof_len);
+  flush_fine(ctx->c);
   SP_CATCH(ctx)
 }
 int sp_nizk_verify(sp_ctx* ctx, const sp_instance* inst, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens, const uint8_t* label, size_t label_len,
@@ -941,6 +950,94 @@ int sp_snark_verify_t(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t
                       const uint8_t* proof, size_t proof_len) {
   return snark_verify_common(ctx, comm, inputs, ninputs, gens, TranscriptArg::caller(strobe_state), proof, proof_len);
 }
+// ---- batch verifiers: proof i is checked as the single call would check it (statement i, inputs i, label i or caller transcript i); the group
+// equations of all of them are tested in one device pass (verifier.cpp, DESIGN.md "deferred checks")
+struct BatchArgs {
+  size_t k;
+  const uint64_t* const* inputs; const size_t* ninputs;
+  const uint8_t* const* labels; const size_t* label_lens;   // fresh transcripts, or
+  uint8_t* const* states;                                    // the callers' transcripts (the _t forms)
+  const uint8_t* const* proofs; const size_t* proof_lens;
+  const uint8_t* seed; int* status;
+};
+static std::vector<VerifyJob> batch_jobs(const BatchArgs& a, const void* const* stmts) {
+  const bool bad_transcripts = a.states ? false : (!a.labels || !a.label_lens);
+  if (!stmts || !a.inputs || !a.ninputs || !a.proofs || !a.proof_lens || !a.status || bad_transcripts)
+    throw SpError(SP_ERR_INVALID_ARG, "verify_batch: NULL array");
+  std::vector<VerifyJob> jobs;
+  jobs.reserve(a.k);
+  for (size_t i = 0; i < a.k; i++) {
+    const std::string at = "verify_batch: proof " + std::to_string(i) + ": ";
+    if (!stmts[i]) throw SpError(SP_ERR_INVALID_ARG, at + "NULL statement handle");
+    if (!a.proofs[i] && a.proof_lens[i]) throw SpError(SP_ERR_INVALID_ARG, at + "NULL proof");
+    if (!a.inputs[i] && a.ninputs[i]) throw SpError(SP_ERR_INVALID_ARG, at + "NULL inputs");
+    require_reduced(a.inputs[i], a.ninputs[i], "inputs");
+    if (a.states && !a.states[i]) throw SpError(SP_ERR_INVALID_ARG, at + "transcript state is NULL");
+    Transcript T = a.states ? Transcript(Transcript::FromState(), a.states[i]) : Transcript(std::string((const char*)a.labels[i], a.label_lens[i]));
+    jobs.push_back(VerifyJob{nullptr, nullptr, fq_vec(a.inputs[i], a.ninputs[i]), T, a.proofs[i], a.proof_lens[i]});
+  }
+  return jobs;
+}
+// statuses, transcripts and the first rejection's message out; SP_ERR_VERIFY when any proof is rejected
+static int batch_finish(sp_ctx* ctx, const BatchArgs& a, const std::vector<VerifyJob>& jobs) {
+  int rc = SP_OK;
+  for (size_t i = 0; i < a.k; i++) {
+    a.status[i] = jobs[i].status;
+    if (a.states) jobs[i].T.export_state(a.states[i]);
+    if (jobs[i].status != SP_OK && rc == SP_OK) { rc = SP_ERR_VERIFY; ctx->c.last_error = "proof " + std::to_string(i) + ": " + jobs[i].msg; }
+  }
+  flush_fine(ctx->c);
+  return rc;
+}
+static int nizk_verify_batch_common(sp_ctx* ctx, const sp_instance* const* insts, const sp_nizk_gens* gens, const BatchArgs& a) {
+  int rc = SP_OK;
+  SP_TRY(ctx)
+  if (!a.seed) throw SpError(SP_ERR_INVALID_ARG, "verify_batch: weight seed is NULL: draw 32 bytes from the OS RNG on every call");
+  if (!a.k) return SP_OK;
+  if (!gens) throw SpError(SP_ERR_INVALID_ARG, "verify_batch: NULL gens");
+  std::vector<VerifyJob> jobs = batch_jobs(a, reinterpret_cast<const void* const*>(insts));
+  for (size_t i = 0; i < a.k; i++) jobs[i].inst = &insts[i]->inst;
+  nizk_verify_batch(ctx->c, *gens->g, jobs, a.seed);
+  rc = batch_finish(ctx, a, jobs);
+  if (rc != SP_OK) return rc;
+  SP_CATCH(ctx)
+}
+static int snark_verify_batch_common(sp_ctx* ctx, const sp_snark_encoding* const* comms, const sp_snark_gens* gens, const BatchArgs& a) {
+  int rc = SP_OK;
+  SP_TRY(ctx)
+  if (!a.seed) throw SpError(SP_ERR_INVALID_ARG, "verify_batch: weight seed is NULL: draw 32 bytes from the OS RNG on every call");
+  if (!a.k) return SP_OK;
+  if (!gens) throw SpError(SP_ERR_INVALID_ARG, "verify_batch: NULL gens");
+  std::vector<VerifyJob> jobs = batch_jobs(a, reinterpret_cast<const void* const*>(comms));
+  for (size_t i = 0; i < a.k; i++) jobs[i].enc = comms[i]->e.get();
+  snark_verify_batch(ctx->c, *gens->g, jobs, a.seed);
+  rc = batch_finish(ctx, a, jobs);
+  if (rc != SP_OK) return rc;
+  SP_CATCH(ctx)
+}
+int sp_nizk_verify_batch(sp_ctx* ctx, size_t k, const sp_instance* const* insts, const uint64_t* const* inputs_mont, const size_t* ninputs,
+                         const sp_nizk_gens* gens, const uint8_t* const* labels, const size_t* label_lens, const uint8_t* const* proofs,
+                         const size_t* proof_lens, const uint8_t weight_seed[32], int* status) {
+  return nizk_verify_batch_common(ctx, insts, gens, {k, inputs_mont, ninputs, labels, label_lens, nullptr, proofs, proof_lens, weight_seed, status});
+}
+int sp_snark_verify_batch(sp_ctx* ctx, size_t k, const sp_snark_encoding* const* comms, const uint64_t* const* inputs_mont, const size_t* ninputs,
+                          const sp_snark_gens* gens, const uint8_t* const* labels, const size_t* label_lens, const uint8_t* const* proofs,
+                          const size_t* proof_lens, const uint8_t weight_seed[32], int* status) {
+  return snark_verify_batch_common(ctx, comms, gens, {k, inputs_mont, ninputs, labels, label_lens, nullptr, proofs, proof_lens, weight_seed, status});
+}
+int sp_nizk_verify_batch_t(sp_ctx* ctx, size_t k, const sp_instance* const* insts, const uint64_t* const* inputs_mont, const size_t* ninputs,
+                           const sp_nizk_gens* gens, uint8_t* const* strobe_states, const uint8_t* const* proofs, const size_t* proof_lens,
+                           const uint8_t weight_seed[32], int* status) {
+  if (!strobe_states && k) { if (ctx) ctx->c.last_error = "verify_batch: NULL array"; return SP_ERR_INVALID_ARG; }
+  return nizk_verify_batch_common(ctx, insts, gens, {k, inputs_mont, ninputs, nullptr, nullptr, strobe_states, proofs, proof_lens, weight_seed, status});
+}
+int sp_snark_verify_batch_t(sp_ctx* ctx, size_t k, const sp_snark_encoding* const* comms, const uint64_t* const* inputs_mont, const size_t* ninputs,
+                            const sp_snark_gens* gens, uint8_t* const* strobe_states, const uint8_t* const* proofs, const size_t* proof_lens,
+                            const uint8_t weight_seed[32], int* status) {
+  if (!strobe_states && k) { if (ctx) ctx->c.last_error = "verify_batch: NULL array"; return SP_ERR_INVALID_ARG; }
+  return snark_verify_batch_common(ctx, comms, gens, {k, inputs_mont, ninputs, nullptr, nullptr, strobe_states, proofs, proof_lens, weight_seed, status});
+}
+
 // merlin::Transcript for hosts without merlin (tests, C callers): the state buffer is the whole object
 int sp_transcript_new(const uint8_t* label, size_t label_len, uint8_t* strobe_state) {
   Transcript T(std::string((const char*)label, label_len));

@@ -219,6 +219,20 @@ void points_to_niels(ge_niels* out, const ge* in, size_t n, cudaStream_t s);
 void niels_to_ge(ge* out, const ge_niels* in, size_t n, cudaStream_t s);
 // out = sum_i scalars[i] * pts[i]   (scalars Montgomery-form, device-resident; scratch >= pip_scratch_bytes(p))
 void msm_var(ge* out, const ge_niels* pts, const u256* scalars, const PipPlan& p, void* scratch, cudaStream_t s);
+// out[k] = sum_{seg_start[k] <= i < seg_start[k+1]} scalars[i] * pts[i] for k < K (an empty segment gives the identity).  scalars: canonical
+// integers (not Montgomery form); seg_start: K+1 entries, non-decreasing, seg_start[K] = n; scratch >= n points
+void msm_var_segmented(ge* out, const ge* pts, const u256* scalars, const uint32_t* seg_start, size_t K, size_t n, ge* scratch, cudaStream_t s);
+
+// ---- the generator scalars of an inner-product argument: row[i] (+)= allinv * scale * prod_{bit b of i} u_sq[lg_n - 1 - b] for i < 2^lg_n, the
+// vector s of DotProductProofLog::verify (bullet.rs:190-201) times `scale`.  Montgomery form; add = 0 writes, 1 adds.  The items of one launch
+// must write disjoint entries
+struct IpaSRow {
+  u256* row;
+  uint32_t lg_n, add;
+  u256 allinv, scale;
+  u256 u_sq[32];
+};
+void ipa_srow(const IpaSRow* d_items, size_t nitems, uint32_t max_lg_n, cudaStream_t s);
 
 }  // namespace dev
 }  // namespace sp

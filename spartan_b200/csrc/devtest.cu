@@ -17,6 +17,7 @@
 #include <vector>
 #include "kcommon.cuh"
 #include "quad.cuh"
+#include "snark.hpp"
 
 using namespace sp;
 using namespace sp::dev;
@@ -610,6 +611,73 @@ int spd_fold_top(int ntables, size_t len, u256* tables, const u256* r) {
     c.sync();
     c.out(tables, d, (size_t)ntables * len);
     return (int)c.err;
+  });
+}
+
+// ---- batch verifier
+// out[k] = sum over segment k of scalars[i] * pts[i] (msm_var_segmented); scalars canonical, seg_start: K+1 entries
+int spd_msm_var_segmented(size_t K, size_t n, const ge* pts, const u256* scalars, const uint32_t* seg_start, ge* out) {
+  return guarded([&] {
+    KCall c;
+    const ge* dp = c.in(pts, n ? n : 1);
+    const u256* ds = c.in(scalars, n ? n : 1);
+    const uint32_t* dseg = c.in(seg_start, K + 1);
+    ge* dtmp = c.alloc<ge>(n ? n : 1);
+    ge* dout = c.alloc<ge>(K ? K : 1);
+    if (c.ok()) msm_var_segmented(dout, dp, ds, dseg, K, n, dtmp, c.s);
+    c.sync();
+    c.out(out, dout, K);
+    return (int)c.err;
+  });
+}
+// ipa_srow over `nitems` rows packed back to back in rows[0 .. total) (in, out): item i writes or adds 2^lg_n[i] entries at row_off[i];
+// u_sq: 32 scalars per item
+int spd_ipa_srow(size_t nitems, const uint32_t* lg_n, const uint32_t* add, const u256* allinv, const u256* scale, const u256* u_sq, const uint64_t* row_off,
+                 size_t total, u256* rows) {
+  return guarded([&] {
+    KCall c;
+    u256* drows = c.in(rows, total);
+    std::vector<IpaSRow> items(nitems);
+    uint32_t max_lg = 0;
+    for (size_t i = 0; i < nitems; i++) {
+      memset(&items[i], 0, sizeof(IpaSRow));
+      items[i].row = drows + row_off[i];
+      items[i].lg_n = lg_n[i]; items[i].add = add[i]; items[i].allinv = allinv[i]; items[i].scale = scale[i];
+      for (int j = 0; j < 32; j++) items[i].u_sq[j] = u_sq[32 * i + j];
+      if (lg_n[i] > max_lg) max_lg = lg_n[i];
+    }
+    const IpaSRow* dit = c.in(items.data(), nitems ? nitems : 1);
+    if (c.ok()) ipa_srow(dit, nitems, max_lg, c.s);
+    c.sync();
+    c.out(rows, drows, total);
+    return (int)c.err;
+  });
+}
+
+// the deferred checker of batch verification and its final pass (verifier.cpp deferred_check) on hand-made equations over a generator set of
+// `nbases` points derived from `label`.  Proof i owns equations [eq_start[i], eq_start[i+1]); equation e owns terms [term_start[e],
+// term_start[e+1]); term t: side[t] (0 lhs, 1 rhs), gen[t] (>= 0: that generator; < 0: the point pts[32 t .. 32 t + 32)), k[t] (Montgomery).
+// ok[i] = 1 when the final pass accepts proof i.
+int spd_deferred_check(size_t nproofs, const uint32_t* eq_start, const uint32_t* term_start, const int32_t* side, const int64_t* gen, const uint8_t* pts,
+                       const u256* k, const uint8_t* label, size_t label_len, size_t nbases, const uint8_t* seed32, int* ok) {
+  return guarded([&] {
+    sp::Ctx ctx(0);
+    sp::GenSet gs(&ctx, std::string((const char*)label, label_len), nbases, {});
+    std::vector<std::vector<DeferredEq>> proofs(nproofs);
+    for (size_t i = 0; i < nproofs; i++)
+      for (uint32_t e = eq_start[i]; e < eq_start[i + 1]; e++) {
+        DeferredEq eq;
+        for (uint32_t t = term_start[e]; t < term_start[e + 1]; t++) {
+          DeferredTerm x;
+          x.k = Fq(k[t]); x.gen = (long)gen[t];
+          memcpy(x.pt.b, pts + 32 * (size_t)t, 32);
+          (side[t] ? eq.rhs : eq.lhs).push_back(x);
+        }
+        proofs[i].push_back(eq);
+      }
+    const std::vector<bool> r = deferred_check(ctx, gs, proofs, seed32);
+    for (size_t i = 0; i < nproofs; i++) ok[i] = r[i] ? 1 : 0;
+    return 0;
   });
 }
 

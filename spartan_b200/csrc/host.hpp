@@ -115,6 +115,27 @@ struct Shake256 {  // streaming SHAKE256 XOF (sha3's Shake256 + XofReader as use
   }
 };
 
+// Weight of equation e of proof i in a batch verification: from_bytes_wide(SHAKE256("spartan-b200/v1/batch-verify" || seed || LE64(i) || LE64(e))).
+// Whoever knows the weights can make a bad proof pass, so `seed` must be fresh OS randomness on every call.
+inline Fq batch_weight(const uint8_t seed[32], uint64_t i, uint64_t e) {
+  static const char tag[] = "spartan-b200/v1/batch-verify";
+  uint8_t in[sizeof(tag) - 1 + 32 + 16];
+  memcpy(in, tag, sizeof(tag) - 1);
+  memcpy(in + sizeof(tag) - 1, seed, 32);
+  for (int b = 0; b < 8; b++) { in[sizeof(tag) - 1 + 32 + b] = (uint8_t)(i >> (8 * b)); in[sizeof(tag) - 1 + 40 + b] = (uint8_t)(e >> (8 * b)); }
+  Shake256 x(in, sizeof in);
+  uint8_t w[64];
+  x.squeeze(w, 64);
+  return Fq::from_bytes_wide(w);
+}
+// <eq(r, .), s> for the vector s of an inner-product argument with challenges u (s_i = prod_j u_j^-1 times u_j^2 for each bit j of i, the
+// top bit first: bullet.rs:190-201): prod_j ((1 - r_j) u_j^-1 + r_j u_j), in O(lg n) instead of the n-term sum
+inline Fq ipa_a_hat(const Fq* r, const Fq* u, const Fq* u_inv, size_t lg_n) {
+  Fq acc = Fq::one();
+  for (size_t j = 0; j < lg_n; j++) acc *= (Fq::one() - r[j]) * u_inv[j] + r[j] * u[j];
+  return acc;
+}
+
 class Transcript {  // merlin::Transcript + ProofTranscript (transcript.rs:5-37)
  public:
   explicit Transcript(const std::string& label) {

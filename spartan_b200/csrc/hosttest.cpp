@@ -167,6 +167,35 @@ void spt_transcript_run(const uint8_t* label, size_t llen, const uint8_t* msgs, 
   t.challenge_bytes("c", out64, 64);
 }
 void spt_shake256(uint8_t* out, size_t outlen, const uint8_t* in, size_t inlen) { sp::shake256(out, outlen, in, inlen); }
+// batch verification: the weight of equation e of proof i (batch_weight), Montgomery limbs out
+void spt_batch_weight(const uint8_t* seed32, uint64_t i, uint64_t e, uint8_t* out) { Fq w = batch_weight(seed32, i, e); memcpy(out, &w.m, 32); }
+// <eq(r, .), s> of an inner-product argument two ways: ipa_a_hat's product (out) and the n-term sum over the vector s that
+// DotProductProofLog::verify builds (out + 32); r, u: lg_n Montgomery scalars each
+void spt_ipa_a_hat(const uint8_t* r_mont, const uint8_t* u_mont, size_t lg_n, uint8_t* out64) {
+  std::vector<Fq> r(lg_n), u(lg_n), u_inv(lg_n), u_sq(lg_n);
+  for (size_t j = 0; j < lg_n; j++) { memcpy(&r[j].m, r_mont + 32 * j, 32); memcpy(&u[j].m, u_mont + 32 * j, 32); }
+  Fq allinv = Fq::one();
+  for (size_t j = 0; j < lg_n; j++) { u_inv[j] = u[j].inv(); allinv *= u_inv[j]; u_sq[j] = u[j] * u[j]; }
+  const Fq fast = ipa_a_hat(r.data(), u.data(), u_inv.data(), lg_n);
+  // the reference's loop (bullet.rs:190-201): s[i] = s[i - 2^k] * u_sq[lg_n - 1 - k], k = floor(log2 i)
+  const size_t n = (size_t)1 << lg_n;
+  std::vector<Fq> s(n);
+  s[0] = allinv;
+  for (size_t i = 1; i < n; i++) {
+    size_t lg_i = 0;
+    while (((size_t)2 << lg_i) <= i) lg_i++;
+    s[i] = s[i - ((size_t)1 << lg_i)] * u_sq[(lg_n - 1) - lg_i];
+  }
+  // a = eq(r, .) (EqPolynomial::evals: r[0] is the top bit of the index)
+  Fq slow = Fq::zero();
+  for (size_t i = 0; i < n; i++) {
+    Fq a = Fq::one();
+    for (size_t j = 0; j < lg_n; j++) a *= ((i >> (lg_n - 1 - j)) & 1) ? r[j] : Fq::one() - r[j];
+    slow += a * s[i];
+  }
+  memcpy(out64, &fast.m, 32);
+  memcpy(out64 + 32, &slow.m, 32);
+}
 // wire format (wire.hpp): parse one input with Reader under the status code the library uses for it, re-encode it with Writer.  kind 0: a NIZK
 // proof, 1: a SNARK proof, 2: a ComputationCommitment.  *out_len: the capacity of out, then the length of the re-encoding.
 int spt_wire_roundtrip(int kind, const uint8_t* in, size_t len, uint8_t* out, size_t* out_len) {

@@ -390,5 +390,59 @@ void msm_var(ge* out, const ge_niels* pts, const u256* scalars, const PipPlan& p
   SP_LAUNCHED(); check("msm_var");
 }
 
+// ---- segmented variable-base MSM of the batch verifier: K independent sums over ragged segments of a few hundred points each.  Every point's
+// multiple is one thread's double-and-add (no shared buckets: a segment is too short to fill them), then one block per segment adds its multiples.
+__global__ void __launch_bounds__(128) k_seg_scalarmul(ge* __restrict__ out, const ge* __restrict__ pts, const u256* __restrict__ scalars, size_t n) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  st_ge_p(out + i, ge_scalarmul(ld256_ro(scalars + i), ld_ge_p(pts + i)));
+}
+__global__ void __launch_bounds__(128) k_seg_sum(ge* __restrict__ out, const ge* __restrict__ terms, const uint32_t* __restrict__ seg_start) {
+  __shared__ ge sm[4];
+  const uint32_t k = blockIdx.x, lo = seg_start[k], hi = seg_start[k + 1];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  ge acc = ge_identity();
+#pragma unroll 1
+  for (uint32_t i = lo + threadIdx.x; i < hi; i += blockDim.x) acc = ge_add(acc, ld_ge_p(terms + i));
+  acc = warp_sum_ge(acc);
+  if (lane == 0) sm[warp] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) st_ge_p(out + k, ge_add(ge_add(sm[0], sm[1]), ge_add(sm[2], sm[3])));
+}
+void msm_var_segmented(ge* out, const ge* pts, const u256* scalars, const uint32_t* seg_start, size_t K, size_t n, ge* scratch, cudaStream_t s) {
+  if (!K) return;
+  if (n >= ((size_t)1 << 32)) throw std::runtime_error("spartan_b200: msm_var_segmented supports fewer than 2^32 points");
+  ProfScope ps("msm_var_segmented", 160.0 * (double)n, s);
+  if (n) {
+    k_seg_scalarmul<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(scratch, pts, scalars, n);
+    SP_LAUNCHED();
+  }
+  k_seg_sum<<<(unsigned)K, 128, 0, s>>>(out, scratch, seg_start);
+  SP_LAUNCHED(); check("msm_var_segmented");
+}
+
+// ---- the scalars s_i = allinv * scale * prod_{bit b of i} u_sq[lg_n - 1 - b] of an inner-product argument's unfolded generators
+// (bullet.rs:190-201), one row per item; blockIdx.y = item
+__global__ void __launch_bounds__(256) k_ipa_srow(const IpaSRow* __restrict__ items) {
+  const IpaSRow& it = items[blockIdx.y];
+  const size_t n = (size_t)1 << it.lg_n;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  u256 v = fq_mul(it.allinv, it.scale);
+  for (uint32_t b = 0; b < it.lg_n; b++)
+    if ((i >> b) & 1) v = fq_mul(v, it.u_sq[it.lg_n - 1 - b]);
+  if (it.add) v = fq_add(v, ld256(it.row + i));
+  st256(it.row + i, v);
+}
+void ipa_srow(const IpaSRow* d_items, size_t nitems, uint32_t max_lg_n, cudaStream_t s) {
+  if (max_lg_n >= 32) throw std::runtime_error("spartan_b200: ipa_srow: rows of at most 2^31 entries");
+  for (size_t at = 0; at < nitems; at += 65535) {   // gridDim.y limit
+    dim3 g((unsigned)((((size_t)1 << max_lg_n) + 255) / 256), (unsigned)(nitems - at < 65535 ? nitems - at : 65535));
+    k_ipa_srow<<<g, 256, 0, s>>>(d_items + at);
+    SP_LAUNCHED();
+  }
+  check("ipa_srow");
+}
+
 }  // namespace dev
 }  // namespace sp

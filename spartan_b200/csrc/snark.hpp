@@ -47,5 +47,24 @@ void instance_evaluate(Ctx& ctx, const Instance& inst, const std::vector<Fq>& rx
 // ---- verifiers (verifier.cpp): throw SpError with code SP_ERR_VERIFY / SP_ERR_DECOMPRESS when the proof is rejected
 void nizk_verify(Ctx& ctx, const Instance& inst, const std::vector<Fq>& input, const R1CSGens& gens, Transcript& T, const uint8_t* proof, size_t len);
 void snark_verify(Ctx& ctx, const SnarkEncoding& enc, const std::vector<Fq>& input, const SnarkGens& gens, Transcript& T, const uint8_t* proof, size_t len);
+// Batch verification with deferred group checks (DESIGN.md "deferred checks").  Every job ends as the single verify leaves it: `status`
+// SP_OK / SP_ERR_VERIFY / SP_ERR_DECOMPRESS, `msg` its message, `T` its transcript.  Throws (no job written) on bad arguments or device errors.
+// `seed`: 32 bytes of fresh OS randomness (batch_weight).
+struct VerifyJob {
+  const Instance* inst = nullptr;        // NIZK
+  const SnarkEncoding* enc = nullptr;    // SNARK
+  std::vector<Fq> input;
+  Transcript T;
+  const uint8_t* proof = nullptr;
+  size_t len = 0;
+  int status = SP_OK;
+  std::string msg;
+};
+void nizk_verify_batch(Ctx& ctx, const R1CSGens& gens, std::vector<VerifyJob>& jobs, const uint8_t seed[32]);
+void snark_verify_batch(Ctx& ctx, const SnarkGens& gens, std::vector<VerifyJob>& jobs, const uint8_t seed[32]);
+// the deferred checker on hand-made equations, for the tests: a term is k * (generator `gen` of `gs` if gen >= 0, else the point `pt`)
+struct DeferredTerm { Fq k; long gen = -1; Cp pt; };
+struct DeferredEq { std::vector<DeferredTerm> lhs, rhs; };
+std::vector<bool> deferred_check(Ctx& ctx, const GenSet& gs, const std::vector<std::vector<DeferredEq>>& proofs, const uint8_t seed[32]);
 
 }  // namespace sp
