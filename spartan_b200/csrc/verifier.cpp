@@ -341,7 +341,11 @@ Cp zk_sumcheck_verify(Checker& chk, const ZKSumcheckInstanceProof& p, const hge&
     const hge claim = i == 0 ? comm_claim : chk.point(claim_c, "comm_claim_per_round");
     hge target = hge_add(mul(claim, w[0]), mul(chk.point(p.comm_evals[i], "comm_eval"), w[1]));
     const std::vector<Fq> a = zk_round_weights(w, r_i, degree);
-    dotproduct_verify(chk, p.proofs[i], g1, gn, T, a, p.comm_polys[i], target, compress(target));
+    try {
+      dotproduct_verify(chk, p.proofs[i], g1, gn, T, a, p.comm_polys[i], target, compress(target));
+    } catch (const BadPoint&) {   // the reference turns every error of the round's DotProductProof into InternalError (sumcheck.rs:164-176)
+      throw Reject("DotProductProof");
+    }
     r.push_back(r_i);
   }
   return p.comm_evals.back();
