@@ -209,6 +209,31 @@ int sp_nizk_prove_resident(sp_ctx* ctx, const sp_instance* inst, const sp_poly* 
 /* ---- SNARK                                                                               lib.rs:277-465 */
 int sp_snark_gens_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries, sp_snark_gens** out);
 void sp_snark_gens_free(sp_snark_gens* g);
+
+/* ---- generator tables shared by several gens.  sp_nizk_gens_create / sp_snark_gens_create each build their own generator sets; a NIZKGens
+ * or SNARKGens made from tables is a view into the tables' sets and holds no device memory of its own, so gens for any number of circuits
+ * up to the tables' sizes share one copy.  MultiCommitGens::new(n, label) of any n is a prefix of the label's SHAKE stream
+ * (commitments.rs:15-33): a view proves and verifies byte for byte as the private gens of its circuit do.  Tables, the gens made from them
+ * and encodings may be freed in any order; the device memory goes back to the library's cache when the last holder is freed. */
+typedef struct sp_gen_tables sp_gen_tables;
+/* the gens_r1cs_sat set for circuits up to (num_cons, num_vars, num_inputs) and, if num_nz_entries > 0, the gens_r1cs_eval set up to that
+ * many non-zeros (commitments.rs:15-33, r1csproof.rs:68-73, sparse_mlpoly.rs:292-317); widths chosen as for private gens (DESIGN.md §2) */
+int sp_gen_tables_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries, sp_gen_tables** out);
+void sp_gen_tables_free(sp_gen_tables* t);       /* drops the caller's reference; views keep the tables alive */
+typedef struct { char label[32]; size_t nbases; int window_bits; int has_row_table; size_t device_bytes; } sp_gen_set_info;
+/* one entry per set (gens_r1cs_sat, then gens_r1cs_eval if built); *n = the number of sets; SP_ERR_INVALID_ARG (nothing written) if cap < *n */
+int sp_gen_tables_info(const sp_gen_tables* t, sp_gen_set_info* out, size_t cap, size_t* n);
+/* views for a circuit whose every dimension is <= the tables' (NIZKGens::new lib.rs:475-481, SNARKGens::new lib.rs:288-309).  SP_ERR_INVALID_ARG
+ * when a set is too short (the message gives needed vs available generators per set), when a SNARK view is asked of tables built with
+ * num_nz_entries = 0, or when the tables were built on another context.  Host copies of the few generators the sigma protocols use are added
+ * to the tables if missing; no device memory stays allocated. */
+int sp_nizk_gens_create_from(sp_ctx* ctx, const sp_gen_tables* tables, size_t num_cons, size_t num_vars, size_t num_inputs, sp_nizk_gens** out);
+int sp_snark_gens_create_from(sp_ctx* ctx, const sp_gen_tables* tables, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries,
+                              sp_snark_gens** out);
+/* device bytes in blocks this library holds for live objects, on every device (its cache of freed blocks excluded): a footprint that other
+ * processes on the GPU cannot change, unlike cudaMemGetInfo */
+unsigned long long sp_device_bytes_live(void);
+
 int sp_snark_encode(sp_ctx* ctx, const sp_instance* inst, const sp_snark_gens* gens, sp_snark_encoding** out);   /* SNARK::encode lib.rs:325 */
 void sp_snark_encoding_free(sp_snark_encoding* e);
 /* bincode::serialize(&ComputationCommitment) */

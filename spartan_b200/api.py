@@ -40,6 +40,7 @@ lib = _load()
 lib.sp_last_error.restype = C.c_char_p
 lib.sp_kernel_launches.restype = C.c_ulonglong
 lib.sp_release_cached_memory.restype = C.c_ulonglong
+lib.sp_device_bytes_live.restype = C.c_ulonglong
 lib.sp_poly_len.restype = C.c_size_t
 lib.sp_points_len.restype = C.c_size_t
 _vp, _sz = C.c_void_p, C.c_size_t
@@ -640,13 +641,54 @@ def _take_bytes(out, n):
     return b
 
 
-class NIZKGens:
-    """lib.rs:468-486"""
+class _GenSetInfo(C.Structure):
+    _fields_ = [("label", C.c_char * 32), ("nbases", C.c_size_t), ("window_bits", C.c_int), ("has_row_table", C.c_int), ("device_bytes", C.c_size_t)]
 
-    def __init__(self, num_cons, num_vars, num_inputs, ctx=None):
+
+class GeneratorTables:
+    """Generator tables sized once for the largest circuit a caller proves (sp_gen_tables): the gens_r1cs_sat set for circuits up to
+    (num_cons, num_vars, num_inputs) and, if num_nz_entries > 0, the gens_r1cs_eval set up to that many non-zeros.  NIZKGens(..., tables=t)
+    and SNARKGens(..., tables=t) for any circuit whose every dimension is <= these are views that share the tables' device memory and prove
+    the same bytes as gens of their own.  Views keep the tables alive: `del` this object whenever convenient."""
+
+    def __init__(self, num_cons, num_vars, num_inputs, num_nz_entries=0, ctx=None):
         self.ctx = ctx or default_context()
         h = _vp()
-        self.ctx.check(lib.sp_nizk_gens_create(self.ctx.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), C.byref(h)))
+        self.ctx.check(lib.sp_gen_tables_create(self.ctx.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), _sz(num_nz_entries), C.byref(h)))
+        self.h = h
+
+    def info(self):
+        """one dict per generator set: label, nbases, window_bits, has_row_table, device_bytes"""
+        out, n = (_GenSetInfo * 2)(), _sz()
+        self.ctx.check(lib.sp_gen_tables_info(self.h, out, _sz(2), C.byref(n)))
+        return [{"label": s.label.decode(), "nbases": int(s.nbases), "window_bits": int(s.window_bits), "has_row_table": bool(s.has_row_table),
+                 "device_bytes": int(s.device_bytes)} for s in out[:n.value]]
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None):
+                lib.sp_gen_tables_free(self.h)
+                self.h = None
+        except Exception:
+            pass
+
+
+def device_bytes_live():
+    """device bytes in blocks the library holds for live objects (its cache of freed blocks excluded): unlike the driver's free-memory
+    figure, other processes on the GPU do not change it"""
+    return int(lib.sp_device_bytes_live())
+
+
+class NIZKGens:
+    """lib.rs:468-486.  tables=GeneratorTables: a view into them instead of generator tables of its own"""
+
+    def __init__(self, num_cons, num_vars, num_inputs, ctx=None, tables=None):
+        self.ctx = ctx or (tables.ctx if tables is not None else default_context())
+        h = _vp()
+        if tables is None:
+            self.ctx.check(lib.sp_nizk_gens_create(self.ctx.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), C.byref(h)))
+        else:
+            self.ctx.check(lib.sp_nizk_gens_create_from(self.ctx.h, tables.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), C.byref(h)))
         self.h = h
 
     @staticmethod
@@ -707,12 +749,16 @@ class NIZK:
 
 
 class SNARKGens:
-    """lib.rs:277-309"""
+    """lib.rs:277-309.  tables=GeneratorTables (built with num_nz_entries > 0): a view into them instead of generator tables of its own"""
 
-    def __init__(self, num_cons, num_vars, num_inputs, num_nz_entries, ctx=None):
-        self.ctx = ctx or default_context()
+    def __init__(self, num_cons, num_vars, num_inputs, num_nz_entries, ctx=None, tables=None):
+        self.ctx = ctx or (tables.ctx if tables is not None else default_context())
         h = _vp()
-        self.ctx.check(lib.sp_snark_gens_create(self.ctx.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), _sz(num_nz_entries), C.byref(h)))
+        if tables is None:
+            self.ctx.check(lib.sp_snark_gens_create(self.ctx.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), _sz(num_nz_entries), C.byref(h)))
+        else:
+            self.ctx.check(lib.sp_snark_gens_create_from(self.ctx.h, tables.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), _sz(num_nz_entries),
+                                                         C.byref(h)))
         self.h = h
 
     @staticmethod

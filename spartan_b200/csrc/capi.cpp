@@ -16,6 +16,7 @@ struct sp_instance { Instance inst; };
 struct sp_nizk_gens { std::unique_ptr<R1CSGens> g; };
 struct sp_snark_gens { std::unique_ptr<SnarkGens> g; };
 struct sp_snark_encoding { std::unique_ptr<SnarkEncoding> e; };
+struct sp_gen_tables { std::unique_ptr<GenTables> t; };
 
 static std::string g_create_error;
 
@@ -780,12 +781,20 @@ int sp_instance_is_sat(sp_ctx* ctx, const sp_instance* inst, const uint64_t* var
 }
 
 // ---- NIZK
+// private gens: tables sized for this one circuit, then a view into them (the view holds the only reference)
 int sp_nizk_gens_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, sp_nizk_gens** out) {
   SP_TRY(ctx)
-  (void)num_cons;
-  size_t num_vars_padded = next_pow2(std::max(num_vars, num_inputs + 1));  // lib.rs:475-481
+  const GenTables t(&ctx->c, num_cons, num_vars, num_inputs, 0);
   std::unique_ptr<sp_nizk_gens> g(new sp_nizk_gens);
-  g->g.reset(new R1CSGens(&ctx->c, "gens_r1cs_sat", num_vars_padded));
+  g->g.reset(new R1CSGens(&ctx->c, t, padded_num_vars(num_vars, num_inputs)));  // lib.rs:475-481
+  *out = g.release();
+  SP_CATCH(ctx)
+}
+int sp_nizk_gens_create_from(sp_ctx* ctx, const sp_gen_tables* tables, size_t num_cons, size_t num_vars, size_t num_inputs, sp_nizk_gens** out) {
+  SP_TRY(ctx)
+  (void)num_cons;
+  std::unique_ptr<sp_nizk_gens> g(new sp_nizk_gens);
+  g->g.reset(new R1CSGens(&ctx->c, *tables->t, padded_num_vars(num_vars, num_inputs)));
   *out = g.release();
   SP_CATCH(ctx)
 }
@@ -841,11 +850,48 @@ int sp_nizk_prove_resident(sp_ctx* ctx, const sp_instance* inst, const sp_poly* 
 // ---- SNARK
 int sp_snark_gens_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries, sp_snark_gens** out) {
   SP_TRY(ctx)
+  // next_pow2(0) = next_pow2(1): tables for one non-zero entry are the tables num_nz_entries = 0 has always had, and they include gens_r1cs_eval
+  const GenTables t(&ctx->c, num_cons, num_vars, num_inputs, std::max<size_t>(num_nz_entries, 1));
   std::unique_ptr<sp_snark_gens> g(new sp_snark_gens);
-  g->g.reset(new SnarkGens(&ctx->c, num_cons, num_vars, num_inputs, num_nz_entries));
+  g->g.reset(new SnarkGens(&ctx->c, t, num_cons, num_vars, num_inputs, num_nz_entries));
   *out = g.release();
   SP_CATCH(ctx)
 }
+int sp_snark_gens_create_from(sp_ctx* ctx, const sp_gen_tables* tables, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries,
+                              sp_snark_gens** out) {
+  SP_TRY(ctx)
+  std::unique_ptr<sp_snark_gens> g(new sp_snark_gens);
+  g->g.reset(new SnarkGens(&ctx->c, *tables->t, num_cons, num_vars, num_inputs, num_nz_entries));
+  *out = g.release();
+  SP_CATCH(ctx)
+}
+
+// ---- generator tables shared by gens views
+int sp_gen_tables_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries, sp_gen_tables** out) {
+  SP_TRY(ctx)
+  std::unique_ptr<sp_gen_tables> t(new sp_gen_tables);
+  t->t.reset(new GenTables(&ctx->c, num_cons, num_vars, num_inputs, num_nz_entries));
+  *out = t.release();
+  SP_CATCH(ctx)
+}
+void sp_gen_tables_free(sp_gen_tables* t) { delete t; }
+int sp_gen_tables_info(const sp_gen_tables* t, sp_gen_set_info* out, size_t cap, size_t* n) {
+  std::vector<const GenSet*> sets{t->t->r1cs_sat.get()};
+  if (t->t->r1cs_eval) sets.push_back(t->t->r1cs_eval.get());
+  *n = sets.size();
+  if (cap < sets.size()) return SP_ERR_INVALID_ARG;
+  for (size_t i = 0; i < sets.size(); i++) {
+    sp_gen_set_info& o = out[i];
+    memset(&o, 0, sizeof(o));
+    memcpy(o.label, sets[i]->label.data(), std::min(sets[i]->label.size(), sizeof(o.label) - 1));
+    o.nbases = sets[i]->nbases;
+    o.window_bits = sets[i]->wbits;
+    o.has_row_table = sets[i]->rows() != nullptr;
+    o.device_bytes = sets[i]->device_bytes();
+  }
+  return SP_OK;
+}
+unsigned long long sp_device_bytes_live(void) { return dev::pool_live_bytes(); }
 void sp_snark_gens_free(sp_snark_gens* g) { delete g; }
 int sp_snark_encode(sp_ctx* ctx, const sp_instance* inst, const sp_snark_gens* gens, sp_snark_encoding** out) {
   SP_TRY(ctx)

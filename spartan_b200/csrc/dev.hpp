@@ -27,6 +27,7 @@ void stream_sync(cudaStream_t s);
 void* pool_alloc(size_t bytes);
 void pool_free(void* p);
 size_t pool_release_cached();   // cudaFree every cached free block; returns their bytes
+size_t pool_live_bytes();       // rounded bytes of the blocks handed out and not yet freed, every device
 void* hmalloc_pinned(size_t bytes);
 void hfree_pinned(void* p);
 void h2d(void* d, const void* h, size_t bytes, cudaStream_t s);

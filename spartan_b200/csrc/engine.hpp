@@ -4,6 +4,7 @@
 #include <cstdlib>
 #include <map>
 #include <memory>
+#include <mutex>
 #include <string>
 #include <vector>
 #include "dev.hpp"
@@ -141,26 +142,47 @@ struct FineTimer {  // host wall-clock accumulator for latency hunting; a no-op 
   ~FineTimer() { stop(); }
 };
 
+// The device tables never change once built: views (GenTables) hand out raw pointers into them.  Only the host copies grow, when a view needs
+// the copy of a base no earlier view needed; they are added under `host_mu` and never removed, so a reference from tab() stays valid.
 struct GenSet {
   Ctx* ctx;
   std::string label;
   size_t nbases;
   DevBuf<ge> G;
   DevBuf<ge_niels> table;
-  int wbits = 8;               // window width of `table` (host_tab is always 8-bit)
+  int wbits = 8;               // window width of `table` (host copies are always 8-bit)
   DevBuf<ge_niels> row_table;  // d * G_j for the row MSM of large sets (dev::build_row_table); empty for small sets
   const ge_niels* rows() const { return row_table.n ? row_table.p : nullptr; }
-  std::map<size_t, HostBaseTable> host_tab;
   std::vector<Cp> compressed;  // lazily filled export
   GenSet(Ctx* c, const std::string& label, size_t nbases, const std::vector<size_t>& host_bases);
   GenSet(Ctx* c, const ge* d_points, size_t nbases, const std::vector<size_t>& host_bases);   // caller-supplied generators (device array)
   void finish(const std::vector<size_t>& host_bases);   // window tables + host copies, once G is filled
+  // host copies of the bases < nbases among `bases` that have none yet, built on ctx's stream through staging buffers that are freed on return
+  void add_host_tables(const std::vector<size_t>& bases);
   const HostBaseTable& tab(size_t base) const {
+    std::lock_guard<std::mutex> lk(host_mu);
     auto it = host_tab.find(base);
     if (it == host_tab.end()) throw std::runtime_error("spartan_b200: no host table for generator " + std::to_string(base));
     return it->second;
   }
+  bool has_tab(size_t base) const { std::lock_guard<std::mutex> lk(host_mu); return host_tab.count(base) != 0; }
   hge host_point(size_t base) const;  // 1 * G_base from the host table
+  size_t device_bytes() const { return G.n * sizeof(ge) + (table.n + row_table.n) * sizeof(ge_niels); }
+ private:
+  std::map<size_t, HostBaseTable> host_tab;
+  mutable std::mutex host_mu;
+};
+
+// Generator tables sized once for the largest circuit a caller proves (sp_gen_tables): the "gens_r1cs_sat" set and, when SPARK sizes are given, the
+// "gens_r1cs_eval" set.  MultiCommitGens::new(n, label) of any n is a prefix of the label's SHAKE stream (commitments.rs:15-33), so every
+// R1CSGens / SnarkGens for a circuit up to those sizes is a view into them, holding a reference to the sets it uses.
+struct GenTables {
+  Ctx* ctx;
+  std::shared_ptr<GenSet> r1cs_sat, r1cs_eval;   // r1cs_eval: null when num_nz_entries was 0
+  // set sizes (R1CSGens::bases, SparkDims::bases) and build order (R1CS first) as the private gens of one circuit have always used
+  GenTables(Ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries);
+  // SpError(SP_ERR_INVALID_ARG) unless a view on `c` fits: r1cs_bases of gens_r1cs_sat and (eval_bases > 0) eval_bases of gens_r1cs_eval
+  void require(const Ctx* c, size_t r1cs_bases, size_t eval_bases) const;
 };
 
 // A MultiCommitGens view (commitments.rs:8-12): G = set.G[off .. off+n), h = set.G[h]

@@ -107,6 +107,12 @@ size_t pool_release_cached() {
   std::lock_guard<std::mutex> lk(g_pool_mu);
   return drop_cached_locked();
 }
+size_t pool_live_bytes() {
+  std::lock_guard<std::mutex> lk(g_pool_mu);
+  size_t bytes = 0;
+  for (auto& kv : g_pool_live) bytes += kv.second.second;
+  return bytes;
+}
 void* pool_alloc(size_t bytes) {
   size_t r = pool_round(bytes);
   int dev = 0;

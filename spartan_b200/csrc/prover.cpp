@@ -181,25 +181,28 @@ void GenSet::finish(const std::vector<size_t>& host_bases) {
   if (wbits != 8 && wbits != 13 && wbits != 15) throw std::runtime_error("spartan_b200: SP_MSM_WINDOW must be 8, 13 or 15");
   table.alloc(dev::table_entries(nbases, wbits));
   dev::build_tables(table.p, G.p, nbases, wbits, ctx->stream);
+  add_host_tables(host_bases);
+  ctx->sync();
+}
+void GenSet::add_host_tables(const std::vector<size_t>& bases) {
   // host copies (8-bit windows) of the few generators the sigma protocols commit against
   std::vector<size_t> hb;
-  for (size_t b : host_bases) if (b < nbases && std::find(hb.begin(), hb.end(), b) == hb.end()) hb.push_back(b);
-  if (!hb.empty()) {
-    DevBuf<ge> sel(hb.size());
-    for (size_t i = 0; i < hb.size(); i++) dev::d2d(sel.p + i, G.p + hb[i], sizeof(ge), ctx->stream);
-    DevBuf<ge_niels> small(dev::table_entries(hb.size(), 8));
-    dev::build_tables(small.p, sel.p, hb.size(), 8, ctx->stream);
-    for (size_t i = 0; i < hb.size(); i++) {
-      std::vector<ge_niels> raw(32 * 128);
-      dev::d2h(raw.data(), small.p + i * 32 * 128, sizeof(ge_niels) * 32 * 128, ctx->stream);
-      ctx->sync();
-      HostBaseTable t;
-      t.e.resize(32 * 128);
-      for (size_t e = 0; e < raw.size(); e++) t.e[e] = to_hniels(raw[e]);
-      host_tab[hb[i]] = std::move(t);
-    }
+  for (size_t b : bases) if (b < nbases && !has_tab(b) && std::find(hb.begin(), hb.end(), b) == hb.end()) hb.push_back(b);
+  if (hb.empty()) return;
+  DevBuf<ge> sel(hb.size());
+  for (size_t i = 0; i < hb.size(); i++) dev::d2d(sel.p + i, G.p + hb[i], sizeof(ge), ctx->stream);
+  DevBuf<ge_niels> small(dev::table_entries(hb.size(), 8));
+  dev::build_tables(small.p, sel.p, hb.size(), 8, ctx->stream);
+  for (size_t i = 0; i < hb.size(); i++) {
+    std::vector<ge_niels> raw(32 * 128);
+    dev::d2h(raw.data(), small.p + i * 32 * 128, sizeof(ge_niels) * 32 * 128, ctx->stream);
+    ctx->sync();
+    HostBaseTable t;
+    t.e.resize(32 * 128);
+    for (size_t e = 0; e < raw.size(); e++) t.e[e] = to_hniels(raw[e]);
+    std::lock_guard<std::mutex> lk(host_mu);
+    host_tab.emplace(hb[i], std::move(t));   // a concurrent view may have added the same base: its copy is the same table
   }
-  ctx->sync();
 }
 hge GenSet::host_point(size_t base) const {
   hge acc = hge_identity();
@@ -211,12 +214,20 @@ hge host_commit(const GenSet& gs, const Term* terms, size_t nterms) {
   return acc;
 }
 
-R1CSGens::R1CSGens(Ctx* ctx, const std::string& label, size_t num_vars) {
+size_t R1CSGens::pc_n(size_t num_vars) {
   // R1CSGens::new (r1csproof.rs:68-73) -> PolyCommitmentGens::new(log2 num_vars) (dense_mlpoly.rs:31-35) ->
   // DotProductProofGens::new(2^ceil(ell/2)) = MultiCommitGens::new(n+1).split_at(n) (nizk/mod.rs:414-418)
   const size_t ell = log2_ceil(num_vars);
-  size_t n = (size_t)1 << (ell - ell / 2);
-  set.reset(new GenSet(ctx, label, std::max<size_t>(n + 2, 5), {0, 1, 2, 3, 4, n, n + 1}));  // gens_4 draws 5 points of the same stream
+  return (size_t)1 << (ell - ell / 2);
+}
+size_t R1CSGens::bases(size_t num_vars) { return std::max<size_t>(pc_n(num_vars) + 2, 5); }   // gens_4 draws 5 points of the same stream
+std::vector<size_t> R1CSGens::host_bases(size_t num_vars) { const size_t n = pc_n(num_vars); return {0, 1, 2, 3, 4, n, n + 1}; }
+
+R1CSGens::R1CSGens(const Ctx* ctx, const GenTables& tables, size_t num_vars) {
+  tables.require(ctx, bases(num_vars), 0);
+  set = tables.r1cs_sat;
+  set->add_host_tables(host_bases(num_vars));
+  const size_t n = pc_n(num_vars);
   gens_pc.n = n;
   gens_pc.gens_n = CommitKey{set.get(), 0, n, n + 1};
   gens_pc.gens_1 = CommitKey{set.get(), n, 1, n + 1};
@@ -547,7 +558,7 @@ Cp commit_rows_and_compress(Ctx& ctx, const CommitKey& key, const u256* d_scalar
   // blinds_late (instead of blinds): called AFTER the rows' MSM is in flight, so that the host draws the blinds from the random tape (0.8 us per
   // scalar of Keccak) while the device works; the blind terms blinds[i]*h are then a second, tiny launch added onto the rows.
   if (key.off != 0 || R > key.n) throw std::runtime_error("spartan_b200: commit_rows key mismatch");
-  const bool blind_on_host = !blinds || blinds[0].is_zero() || key.set->host_tab.count(key.h) != 0;   // the blind term needs the host copy of h's table
+  const bool blind_on_host = !blinds || blinds[0].is_zero() || key.set->has_tab(key.h);   // the blind term needs the host copy of h's table
   if (L == 1 && R >= 2 && R % 2 == 0 && !blinds_late && ctx.shard_world() == 1 && blind_on_host) {
     // one row (the Cx commitment of DotProductProofLog, nizk/mod.rs:466): a latency problem.  The row's sum reaches the host, which adds the
     // blind term and encodes, instead of a 265-product chain on one GPU thread; the blind term is computed while the kernel runs

@@ -14,11 +14,17 @@ struct PolyCommitmentGens {  // dense_mlpoly.rs:24-36 -> DotProductProofGens (ni
   CommitKey gens_n, gens_1;
 };
 struct R1CSGens {  // r1csproof.rs:39-74
-  std::unique_ptr<GenSet> set;
+  std::shared_ptr<GenSet> set;   // gens_r1cs_sat of the tables this is a view into
   PolyCommitmentGens gens_pc;
   CommitKey gens_1, gens_3, gens_4;
-  R1CSGens(Ctx* ctx, const std::string& label, size_t num_vars);
+  // a view into tables.r1cs_sat for a num_vars (padded) circuit; SpError(SP_ERR_INVALID_ARG) when the set is too short or of another context
+  R1CSGens(const Ctx* ctx, const GenTables& tables, size_t num_vars);
+  static size_t pc_n(size_t num_vars);                      // gens_pc.n
+  static size_t bases(size_t num_vars);                     // generators of gens_r1cs_sat the view uses
+  static std::vector<size_t> host_bases(size_t num_vars);   // the bases it needs host copies of
 };
+// num_vars as NIZKGens::new and SNARKGens::new pad it (lib.rs:288-294, :475-481)
+inline size_t padded_num_vars(size_t num_vars, size_t num_inputs) { return next_pow2(std::max(num_vars, num_inputs + 1)); }
 
 // ---- instance
 struct SparseMatDev {  // one of A, B, C: COO (reference order), CSR and CSC on the device; a host copy of the COO only when asked for

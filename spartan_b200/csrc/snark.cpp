@@ -17,18 +17,40 @@ static PolyCommitmentGens pc_view(const GenSet* set, size_t num_vars) {  // Poly
   return g;
 }
 
-SnarkGens::SnarkGens(Ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries) {
-  size_t nvp = next_pow2(std::max(num_vars, num_inputs + 1));  // lib.rs:288-294
-  gens_r1cs_sat.reset(new R1CSGens(ctx, "gens_r1cs_sat", nvp));
-  // R1CSCommitmentGens::new (r1cs.rs:34-47) -> SparseMatPolyCommitmentGens::new(label, x, y, nz, 3) (sparse_mlpoly.rs:292-317)
+SparkDims::SparkDims(size_t num_cons, size_t nvp, size_t num_nz_entries) {
   size_t x = log2_ceil(num_cons), y = log2_ceil(2 * nvp), lgnz = log2_ceil(next_pow2(num_nz_entries));
-  size_t v_ops = lgnz + log2_ceil(next_pow2(3 * 5)), v_mem = std::max(x, y) + 1, v_derefs = lgnz + log2_ceil(next_pow2(3 * 2));
-  size_t n_ops = (size_t)1 << (v_ops - v_ops / 2), n_mem = (size_t)1 << (v_mem - v_mem / 2), n_der = (size_t)1 << (v_derefs - v_derefs / 2);
-  size_t nmax = std::max(n_ops, std::max(n_mem, n_der));
-  eval_set.reset(new GenSet(ctx, "gens_r1cs_eval", nmax + 2, {n_ops, n_ops + 1, n_mem, n_mem + 1, n_der, n_der + 1}));
-  gens_ops = pc_view(eval_set.get(), v_ops);
-  gens_mem = pc_view(eval_set.get(), v_mem);
-  gens_derefs = pc_view(eval_set.get(), v_derefs);
+  v_ops = lgnz + log2_ceil(next_pow2(3 * 5)); v_mem = std::max(x, y) + 1; v_derefs = lgnz + log2_ceil(next_pow2(3 * 2));
+  n_ops = (size_t)1 << (v_ops - v_ops / 2); n_mem = (size_t)1 << (v_mem - v_mem / 2); n_der = (size_t)1 << (v_derefs - v_derefs / 2);
+}
+
+GenTables::GenTables(Ctx* c, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries) : ctx(c) {
+  const size_t nvp = padded_num_vars(num_vars, num_inputs);
+  r1cs_sat = std::make_shared<GenSet>(ctx, "gens_r1cs_sat", R1CSGens::bases(nvp), R1CSGens::host_bases(nvp));
+  if (num_nz_entries) {
+    const SparkDims d(num_cons, nvp, num_nz_entries);
+    r1cs_eval = std::make_shared<GenSet>(ctx, "gens_r1cs_eval", d.bases(), d.host_bases());
+  }
+}
+void GenTables::require(const Ctx* c, size_t r1cs_bases, size_t eval_bases) const {
+  if (c != ctx) throw SpError(SP_ERR_INVALID_ARG, "generator tables belong to another context: a view must be made on the context (device) that built them");
+  if (eval_bases && !r1cs_eval)
+    throw SpError(SP_ERR_INVALID_ARG, "generator tables were built without SNARK sizes (num_nz_entries = 0): a SNARKGens view needs their gens_r1cs_eval set");
+  if (r1cs_bases <= r1cs_sat->nbases && (!eval_bases || eval_bases <= r1cs_eval->nbases)) return;
+  std::string m = "generator tables too small for this circuit: gens_r1cs_sat needs " + std::to_string(r1cs_bases) + " generators, has " + std::to_string(r1cs_sat->nbases);
+  if (eval_bases) m += "; gens_r1cs_eval needs " + std::to_string(eval_bases) + ", has " + std::to_string(r1cs_eval->nbases);
+  throw SpError(SP_ERR_INVALID_ARG, m);
+}
+
+SnarkGens::SnarkGens(const Ctx* ctx, const GenTables& tables, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries) {
+  const size_t nvp = padded_num_vars(num_vars, num_inputs);  // lib.rs:288-294
+  const SparkDims d(num_cons, nvp, num_nz_entries);
+  tables.require(ctx, R1CSGens::bases(nvp), d.bases());     // both sets before either view: the message names both
+  gens_r1cs_sat.reset(new R1CSGens(ctx, tables, nvp));
+  eval_set = tables.r1cs_eval;
+  eval_set->add_host_tables(d.host_bases());
+  gens_ops = pc_view(eval_set.get(), d.v_ops);
+  gens_mem = pc_view(eval_set.get(), d.v_mem);
+  gens_derefs = pc_view(eval_set.get(), d.v_derefs);
 }
 
 static void commit_poly(Ctx& ctx, const u256* d_Z, size_t len, const PolyCommitmentGens& gens, PolyCommitment& out) {  // DensePolynomial::commit, no blinds

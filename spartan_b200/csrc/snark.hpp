@@ -5,11 +5,21 @@
 
 namespace sp {
 
+// R1CSCommitmentGens::new (r1cs.rs:34-47) -> SparseMatPolyCommitmentGens::new(label, x, y, nz, 3) (sparse_mlpoly.rs:292-317): the variable counts of
+// the ops, mem and derefs polynomials and their PolyCommitmentGens sizes
+struct SparkDims {
+  size_t v_ops, v_mem, v_derefs, n_ops, n_mem, n_der;
+  SparkDims(size_t num_cons, size_t num_vars_padded, size_t num_nz_entries);
+  size_t bases() const { return std::max(n_ops, std::max(n_mem, n_der)) + 2; }   // generators of gens_r1cs_eval the three views use
+  std::vector<size_t> host_bases() const { return {n_ops, n_ops + 1, n_mem, n_mem + 1, n_der, n_der + 1}; }
+};
+
 struct SnarkGens {  // lib.rs:277-309
   std::unique_ptr<R1CSGens> gens_r1cs_sat;
-  std::unique_ptr<GenSet> eval_set;  // label "gens_r1cs_eval": ops / mem / derefs generators share one SHAKE stream (sparse_mlpoly.rs:292-317)
+  std::shared_ptr<GenSet> eval_set;  // label "gens_r1cs_eval": ops / mem / derefs generators share one SHAKE stream (sparse_mlpoly.rs:292-317)
   PolyCommitmentGens gens_ops, gens_mem, gens_derefs;
-  SnarkGens(Ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries);
+  // a view into both sets of `tables`; SpError(SP_ERR_INVALID_ARG) when either is too short or missing, or the tables are of another context
+  SnarkGens(const Ctx* ctx, const GenTables& tables, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries);
 };
 
 struct AddrTimestampsDev {  // sparse_mlpoly.rs:213-272
