@@ -47,7 +47,7 @@ typedef struct sp_snark_encoding sp_snark_encoding; /* (ComputationCommitment, C
 int sp_device_count(void);
 int sp_ctx_create(int device, sp_ctx** out);
 void sp_ctx_destroy(sp_ctx* ctx);
-const char* sp_last_error(const sp_ctx* ctx);  /* ctx may be NULL: message of the last failed sp_ctx_create */
+const char* sp_last_error(const sp_ctx* ctx);  /* ctx may be NULL: message of the last failed sp_ctx_create or host-only call made without one */
 unsigned long long sp_kernel_launches(void);   /* kernels launched by this library since load */
 /* device blocks freed by the library are kept for reuse by later proofs of this process; this returns them to the driver (e.g. before another
  * process on the same GPU needs the memory) and gives their size in bytes.  Buffers still held by live objects are not touched. */
@@ -114,6 +114,35 @@ int sp_sumcheck_batched_eval(sp_ctx* ctx, int ninst, sp_poly* const* A, sp_poly*
 /* bound_poly_var_top(r) on every table (each shared C once) fused with the next round's evaluations */
 int sp_sumcheck_batched_fold_eval(sp_ctx* ctx, int ninst, sp_poly* const* A, sp_poly* const* B, sp_poly* const* C, const uint64_t r_mont[4],
                                   uint64_t* out /* ninst*3*4 */);
+/* ---- a whole sumcheck of a caller-defined polynomial (SumcheckInstanceProof::prove_cubic / prove_cubic_batched with any comb_func that is a
+ * sum of products of the tables, sumcheck.rs:183-424).  Inputs: k tables P_0 .. P_{k-1} of one length 2^m (the same handle may appear more
+ * than once), the composition g = sum_t coeff_t * prod_{j in factor_t} P_j (a factor may repeat: A*A*B), the claim and num_rounds (1 <= num_rounds
+ * <= m).  The degree is d = max_t nfactors_t.  Round j: s_j(t) = sum_x g(P(t, x)) at t = 0, 2, 3, .., d (bound points lo + t*(hi - lo));
+ * s_j(1) = e - s_j(0); the d+1 coefficients by interpolation over 0..d (UniPoly::from_evals for d = 2, 3, unipoly.rs:23-54); the transcript
+ * absorbs the polynomial (label "poly") and draws r_j ("challenge_nextround"); every distinct table is bound with r_j once, in place
+ * (bound_poly_var_top); e = s_j(r_j).  Outputs: *proof = bincode(SumcheckInstanceProof) (free with sp_free), r_out = the num_rounds challenges,
+ * finals_out = P_j[0] for every j < k after the last bind, e_out = the final e.  Every handle's sp_poly_len is then 2^(m - num_rounds).  Round
+ * polynomials always carry d+1 coefficients.  The claim is not checked (neither does the reference).
+ * SP_ERR_INVALID_ARG, with the tables untouched: unequal lengths or a length that is not a power of two >= 2, num_rounds out of range, a factor
+ * index >= k, a term without factors, d > SP_SC_MAX_DEGREE, k > SP_SC_MAX_TABLES, nterms outside 1..SP_SC_MAX_TERMS, a handle of another
+ * context.  SP_ERR_INVALID_SCALAR: a coefficient or the claim is not reduced.  One kernel launch per round plus a constant.  On a connected
+ * multi-GPU context the call runs on this rank's GPU alone. */
+#define SP_SC_MAX_DEGREE 6
+#define SP_SC_MAX_TABLES 8
+#define SP_SC_MAX_TERMS 32
+typedef struct { uint64_t coeff_mont[4]; uint32_t nfactors; uint32_t factor[SP_SC_MAX_DEGREE]; } sp_sc_term;
+int sp_sumcheck_prove_t(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim_mont[4], size_t num_rounds,
+                        uint8_t* strobe_state /* in, out */, uint8_t** proof, size_t* proof_len, uint64_t* r_out /* num_rounds x 4 */,
+                        uint64_t* finals_out /* k x 4 */, uint64_t e_out[4]);
+/* the same on Transcript::new(label) */
+int sp_sumcheck_prove(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim_mont[4], size_t num_rounds,
+                      const uint8_t* label, size_t label_len, uint8_t** proof, size_t* proof_len, uint64_t* r_out, uint64_t* finals_out, uint64_t e_out[4]);
+/* SumcheckInstanceProof::verify(claim, num_rounds, degree_bound, transcript) (sumcheck.rs:27-62), host only: ctx may be NULL (sp_last_error(NULL)
+ * then holds the message).  SP_ERR_VERIFY where the reference asserts (round count, degree of a round polynomial, s(0) + s(1) = e) or the bytes
+ * do not decode; the transcript is left as the reference's verify leaves it, accepted or not.  On success e_out = the final claim, r_out = the
+ * num_rounds challenges.  degree_bound must be >= 1. */
+int sp_sumcheck_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const uint64_t claim_mont[4], size_t num_rounds, size_t degree_bound,
+                         uint8_t* strobe_state /* in, out */, uint64_t e_out[4], uint64_t* r_out /* num_rounds x 4 */);
 int sp_eq_evals(sp_ctx* ctx, const uint64_t* r_mont, size_t ell, sp_poly** out);           /* EqPolynomial::evals   dense_mlpoly.rs:68-84 */
 int sp_poly_evaluate(sp_ctx* ctx, const sp_poly* p, const uint64_t* r_mont, size_t ell, uint64_t out[4]); /* DensePolynomial::evaluate :236 */
 int sp_poly_bound_rows(sp_ctx* ctx, const sp_poly* p, const uint64_t* L_mont, size_t L_size, sp_poly** out); /* DensePolynomial::bound :206 */

@@ -343,6 +343,73 @@ def fold_top(polys, r):
     ctx.check(lib.sp_fold_top(ctx.h, arr, C.c_int(len(polys)), _p(np.ascontiguousarray(r, dtype=np.uint64))))
 
 
+SP_SC_MAX_DEGREE, SP_SC_MAX_TABLES, SP_SC_MAX_TERMS = 6, 8, 32
+
+
+class _ScTerm(C.Structure):
+    _fields_ = [("coeff_mont", C.c_uint64 * 4), ("nfactors", C.c_uint32), ("factor", C.c_uint32 * SP_SC_MAX_DEGREE)]
+
+
+class Composition:
+    """g = sum_t coeff_t * prod_{j in factors_t} P_j, the comb_func of a sumcheck as data: `terms` is a list of (coeff_limbs, (i, j, ..)) with
+    coeff_limbs the coefficient's Montgomery limbs and (i, j, ..) table indices (a table may repeat: (0, 0, 1) is A*A*B)."""
+
+    def __init__(self, terms):
+        self.terms = [(np.ascontiguousarray(c, dtype=np.uint64).reshape(4), tuple(int(i) for i in f)) for c, f in terms]
+
+    @property
+    def degree(self):
+        return max((len(f) for _, f in self.terms), default=0)
+
+    def _c_terms(self):
+        arr = (_ScTerm * max(len(self.terms), 1))()
+        for t, (c, f) in enumerate(self.terms):
+            arr[t].coeff_mont[:] = [int(x) for x in c]
+            arr[t].nfactors = len(f)   # more than SP_SC_MAX_DEGREE factors: the count alone reaches the library, which refuses it
+            for i, j in enumerate(f[:SP_SC_MAX_DEGREE]):
+                arr[t].factor[i] = j
+        return arr
+
+
+def _transcript_state(transcript):
+    """a Transcript object (advanced in place) or a label (Transcript::new(label), discarded afterwards)"""
+    return transcript if isinstance(transcript, Transcript) else Transcript(bytes(transcript))
+
+
+def sumcheck_prove(polys, comp, claim, num_rounds, transcript):
+    """SumcheckInstanceProof::prove_cubic / prove_cubic_batched with comb_func = `comp` (a Composition) over the tables `polys`
+    (DensePolynomials of one length, bound in place).  Returns (proof_bytes = bincode(SumcheckInstanceProof), r as (num_rounds, 4) limbs,
+    finals = P_j[0] of every table as (k, 4) limbs, e = the final claim's limbs)."""
+    ctx = polys[0].ctx
+    t = _transcript_state(transcript)
+    terms = comp._c_terms()
+    out, n = C.POINTER(C.c_ubyte)(), _sz()
+    r = np.zeros((num_rounds, 4), dtype=np.uint64)
+    finals = np.zeros((len(polys), 4), dtype=np.uint64)
+    e = np.zeros(4, dtype=np.uint64)
+    ctx.check(lib.sp_sumcheck_prove_t(ctx.h, _handles(polys), C.c_int(len(polys)), terms, C.c_int(len(comp.terms)),
+                                      _p(np.ascontiguousarray(claim, dtype=np.uint64)), _sz(num_rounds), t.state, C.byref(out), C.byref(n), _p(r),
+                                      _p(finals), _p(e)))
+    return _take_bytes(out, n), r, finals, e
+
+
+def sumcheck_verify(proof, claim, num_rounds, degree_bound, transcript):
+    """SumcheckInstanceProof::verify (sumcheck.rs:27-62), on the host: returns (e, r) as Montgomery limbs, raises ProofVerifyError.  The
+    transcript (a Transcript object) is advanced as the reference's verify advances it, accepted or not."""
+    t = _transcript_state(transcript)
+    proof = bytes(proof)
+    e = np.zeros(4, dtype=np.uint64)
+    r = np.zeros((num_rounds, 4), dtype=np.uint64)
+    rc = lib.sp_sumcheck_verify_t(None, C.c_char_p(proof), _sz(len(proof)), _p(np.ascontiguousarray(claim, dtype=np.uint64)), _sz(num_rounds),
+                                  _sz(degree_bound), t.state, _p(e), _p(r))
+    if rc == SP_OK:
+        return e, r
+    msg = lib.sp_last_error(None).decode()
+    if rc == SP_ERR_VERIFY:
+        raise ProofVerifyError("InternalError: " + msg, rc)
+    raise SpartanB200Error("spartan_b200 error %d: %s" % (rc, msg))
+
+
 class MultiCommitGens:
     """commitments.rs:8-33"""
 

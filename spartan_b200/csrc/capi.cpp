@@ -996,6 +996,102 @@ int sp_snark_verify_t(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t
                       const uint8_t* proof, size_t proof_len) {
   return snark_verify_common(ctx, comm, inputs, ninputs, gens, TranscriptArg::caller(strobe_state), proof, proof_len);
 }
+// ---- a whole sumcheck of a caller-defined polynomial (prover.cpp: poly_sumcheck_prove).  Every argument is checked before the first launch, so a
+// refused call leaves the tables as they were.
+static int sumcheck_prove_common(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim[4],
+                                 size_t num_rounds, const TranscriptArg& ta, uint8_t** proof, size_t* proof_len, uint64_t* r_out, uint64_t* finals_out,
+                                 uint64_t e_out[4]) {
+  SP_TRY(ctx)
+  ta.check();
+  if (!tables || !terms || !claim || !proof || !proof_len || !r_out || !finals_out || !e_out) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: NULL argument");
+  if (k < 1 || k > SP_SC_MAX_TABLES)
+    throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: " + std::to_string(k) + " tables; 1 .. SP_SC_MAX_TABLES = " + std::to_string(SP_SC_MAX_TABLES) + " supported");
+  if (nterms < 1 || nterms > SP_SC_MAX_TERMS)
+    throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: " + std::to_string(nterms) + " terms; 1 .. SP_SC_MAX_TERMS = " + std::to_string(SP_SC_MAX_TERMS) + " supported");
+  for (int i = 0; i < k; i++) {
+    if (!tables[i]) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: table " + std::to_string(i) + " is NULL");
+    if (tables[i]->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: table " + std::to_string(i) + " belongs to another context");
+    if (tables[i]->len != tables[0]->len) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: tables differ in length");
+  }
+  const size_t len = tables[0]->len;
+  if (len < 2 || (len & (len - 1))) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: length must be a power of two >= 2");
+  const size_t m = log2_ceil(len);
+  if (num_rounds < 1 || num_rounds > m)
+    throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: num_rounds = " + std::to_string(num_rounds) + " outside 1 .. " + std::to_string(m) + " (the tables' variables)");
+  dev::ScPoly P;
+  memset(static_cast<void*>(&P), 0, sizeof P);
+  std::vector<sp_poly*> distinct;   // a handle passed twice is one table, bound once per round
+  std::vector<uint8_t> slot(k);
+  for (int i = 0; i < k; i++) {
+    const size_t at = std::find(distinct.begin(), distinct.end(), tables[i]) - distinct.begin();
+    if (at == distinct.size()) { distinct.push_back(tables[i]); P.t[at] = tables[i]->d.p; }
+    slot[i] = (uint8_t)at;
+  }
+  P.ntables = (int)distinct.size();
+  P.nterms = nterms;
+  const Fq one = Fq::one();
+  for (int t = 0; t < nterms; t++) {
+    const sp_sc_term& tm = terms[t];
+    const std::string at = "sumcheck_prove: term " + std::to_string(t);
+    if (tm.nfactors == 0) throw SpError(SP_ERR_INVALID_ARG, at + " has no factors");
+    if (tm.nfactors > SP_SC_MAX_DEGREE)
+      throw SpError(SP_ERR_INVALID_ARG, at + " has " + std::to_string(tm.nfactors) + " factors; degree <= SP_SC_MAX_DEGREE = " + std::to_string(SP_SC_MAX_DEGREE) + " supported");
+    for (uint32_t f = 0; f < tm.nfactors; f++) {
+      if (tm.factor[f] >= (uint32_t)k) throw SpError(SP_ERR_INVALID_ARG, at + ": table index " + std::to_string(tm.factor[f]) + " >= k = " + std::to_string(k));
+      P.fac[t][f] = slot[tm.factor[f]];
+    }
+    require_reduced(tm.coeff_mont, 1, "sumcheck_prove: coefficient");
+    const Fq c = fq_in(tm.coeff_mont);
+    P.coeff[t] = c.m;
+    P.unit[t] = c == one;
+    P.nfac[t] = (uint8_t)tm.nfactors;
+    P.degree = std::max(P.degree, (int)tm.nfactors);
+  }
+  require_reduced(claim, 1, "sumcheck_prove: claim");
+  Transcript T = ta.open();
+  SumcheckInstanceProof pr;
+  std::vector<Fq> r, finals;
+  Fq e;
+  poly_sumcheck_prove(ctx->c, P, len, fq_in(claim), num_rounds, T, pr, r, finals, e);
+  for (sp_poly* p : distinct) p->len >>= num_rounds;
+  ta.close(T);
+  const std::vector<uint8_t> bytes = to_bincode(pr);
+  *proof = dup_bytes(bytes); *proof_len = bytes.size();
+  for (size_t j = 0; j < num_rounds; j++) fq_out(r_out + 4 * j, r[j]);
+  for (int i = 0; i < k; i++) fq_out(finals_out + 4 * i, finals[slot[i]]);
+  fq_out(e_out, e);
+  SP_CATCH(ctx)
+}
+int sp_sumcheck_prove_t(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim[4], size_t num_rounds,
+                        uint8_t* strobe_state, uint8_t** proof, size_t* proof_len, uint64_t* r_out, uint64_t* finals_out, uint64_t e_out[4]) {
+  return sumcheck_prove_common(ctx, tables, k, terms, nterms, claim, num_rounds, TranscriptArg::caller(strobe_state), proof, proof_len, r_out, finals_out, e_out);
+}
+int sp_sumcheck_prove(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim[4], size_t num_rounds,
+                      const uint8_t* label, size_t label_len, uint8_t** proof, size_t* proof_len, uint64_t* r_out, uint64_t* finals_out, uint64_t e_out[4]) {
+  return sumcheck_prove_common(ctx, tables, k, terms, nterms, claim, num_rounds, TranscriptArg::fresh(label, label_len), proof, proof_len, r_out, finals_out,
+                               e_out);
+}
+// host only: no device work, so ctx may be NULL (the message then goes where sp_last_error(NULL) reads it)
+int sp_sumcheck_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const uint64_t claim[4], size_t num_rounds, size_t degree_bound,
+                         uint8_t* strobe_state, uint64_t e_out[4], uint64_t* r_out) {
+  std::string& err = ctx ? ctx->c.last_error : g_create_error;
+  try {
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if (!claim || !e_out || (!r_out && num_rounds) || (!proof && proof_len)) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_verify: NULL argument");
+    if (degree_bound < 1) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_verify: degree_bound must be >= 1");
+    require_reduced(claim, 1, "sumcheck_verify: claim");
+    Transcript T = ta.open();
+    TranscriptClose close{ta, T};
+    std::vector<Fq> r;
+    const Fq e = sumcheck_verify_bytes(proof, proof_len, fq_in(claim), num_rounds, degree_bound, T, r);
+    fq_out(e_out, e);
+    for (size_t j = 0; j < num_rounds; j++) fq_out(r_out + 4 * j, r[j]);
+    return SP_OK;
+  } catch (const SpError& e) { err = e.what(); return e.code; }
+  catch (const std::exception& e) { err = e.what(); return SP_ERR_INTERNAL; }
+}
+
 // ---- batch verifiers: proof i is checked as the single call would check it (statement i, inputs i, label i or caller transcript i); the group
 // equations of all of them are tested in one device pass (verifier.cpp, DESIGN.md "deferred checks")
 struct BatchArgs {

@@ -7,6 +7,7 @@
 #include <string>
 #include "field.cuh"
 #include "curve.cuh"
+#include "../../include/spartan_b200.h"
 
 struct CUstream_st;
 typedef CUstream_st* cudaStream_t;
@@ -101,6 +102,19 @@ void sc_fold_eval(ScKind kind, const ScInst* d_insts, int ninst, size_t len, con
 void sc_eval_g(const ScInst* d_insts, int ninst, size_t len, const u256* E, u256* out, void* scratch, cudaStream_t s, HostSig sig = HostSig(), const XRank& xr = XRank());
 void sc_fold_eval_g(const ScInst* d_insts, int ninst, size_t len, const u256& r, const u256* E, u256* out, void* scratch, cudaStream_t s, HostSig sig = HostSig(),
                     const XRank& xr = XRank());
+// ---- rounds of a sumcheck of a caller-defined polynomial g = sum_t coeff[t] * prod_f t[fac[t][f]] (kernels_sc.cu: k_scp_*).  The tables are
+// distinct (each is bound once per round); out = the `degree` evaluations at t = 0, 2, 3, .., degree (just t = 0 for degree 1)
+struct ScPoly {
+  u256* t[SP_SC_MAX_TABLES];
+  u256 coeff[SP_SC_MAX_TERMS];                          // Montgomery form
+  uint8_t fac[SP_SC_MAX_TERMS][SP_SC_MAX_DEGREE];       // table indices < ntables
+  uint8_t nfac[SP_SC_MAX_TERMS];                        // 1 .. degree
+  uint8_t unit[SP_SC_MAX_TERMS];                        // 1: coeff is one, the product is not multiplied by it
+  int ntables, nterms, degree;
+};
+void scp_eval(const ScPoly& p, size_t len, u256* out, void* scratch, cudaStream_t s, HostSig sig);
+// bind every table with r (len -> len/2, in place; len >= 4) and evaluate the next round on the result
+void scp_fold_eval(const ScPoly& p, size_t len, const u256& r, u256* out, void* scratch, cudaStream_t s, HostSig sig);
 // levels[k-1] (k = 1..K, back to back, n0 >> k entries each) = eq(tau[k+1..], .) from E0 = eq(tau[1..], .) of n0 entries
 void eq_suffix(u256* levels, const u256* E0, size_t n0, int K, cudaStream_t s);
 // fold only (bound_poly_var_top, dense_mlpoly.rs:215-223): tables[k][i] += r*(tables[k][i+len/2]-tables[k][i])

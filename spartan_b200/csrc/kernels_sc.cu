@@ -241,6 +241,127 @@ __global__ void __launch_bounds__(SC_SMALL_Q * 8) k_sc_fold_eval_small(ScBatch b
   }
 }
 
+// ---- sumcheck of a caller-defined polynomial (dev.hpp: ScPoly).  The factor indices are runtime values, and registers cannot be indexed at
+// run time without going to local memory, so a thread keeps the bound points of every table (x_k, advanced point by point) and their steps
+// d_k = hi - lo in its own column of dynamic shared memory, [x | d][ntables][SCP_THREADS]; the D accumulators (one per evaluation point) stay in
+// registers.  Columns are private to their thread: no barrier.
+#define SCP_THREADS 128
+__device__ __forceinline__ u256 scp_comb(const ScPoly& P, const u256* x) {
+  u256 sum = fq_zero();
+  for (int t = 0; t < P.nterms; t++) {
+    u256 prod = ld256(x + P.fac[t][0] * SCP_THREADS);
+    for (int f = 1; f < P.nfac[t]; f++) prod = fq_mul(prod, ld256(x + P.fac[t][f] * SCP_THREADS));
+    if (!P.unit[t]) prod = fq_mul(prod, P.coeff[t]);
+    sum = fq_add(sum, prod);
+  }
+  return sum;
+}
+// x holds the low halves (t = 0) on entry; the points t = 2, 3, .., D follow as x + t*d, built by additions like sumcheck.rs:209-221
+template <int D>
+__device__ __forceinline__ void scp_accumulate(u256 (&acc)[D], const ScPoly& P, u256* x, const u256* d) {
+  acc[0] = fq_add(acc[0], scp_comb(P, x));
+#pragma unroll
+  for (int p = 1; p < D; p++) {
+    for (int k = 0; k < P.ntables; k++) {
+      const u256 dk = ld256(d + k * SCP_THREADS);
+      u256 xk = fq_add(ld256(x + k * SCP_THREADS), dk);
+      if (p == 1) xk = fq_add(xk, dk);   // from t = 0 straight to t = 2
+      st256(x + k * SCP_THREADS, xk);
+    }
+    acc[p] = fq_add(acc[p], scp_comb(P, x));
+  }
+}
+template <int D>
+__global__ void __launch_bounds__(SCP_THREADS, 4) k_scp_eval(const __grid_constant__ ScPoly P, size_t len, u256* partials, unsigned int* counters,
+                                                            u256* out, HostSig sig) {
+  extern __shared__ uint4 scp_sh[];
+  u256* x = reinterpret_cast<u256*>(scp_sh) + threadIdx.x;
+  u256* d = x + P.ntables * SCP_THREADS;
+  const size_t half = len >> 1;
+  u256 acc[D];
+#pragma unroll
+  for (int p = 0; p < D; p++) acc[p] = fq_zero();
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < half; i += (size_t)gridDim.x * blockDim.x) {
+    for (int k = 0; k < P.ntables; k++) {
+      const u256 lo = ld256(P.t[k] + i), hi = ld256(P.t[k] + i + half);
+      st256(x + k * SCP_THREADS, lo);
+      st256(d + k * SCP_THREADS, fq_sub(hi, lo));
+    }
+    scp_accumulate<D>(acc, P, x, d);
+  }
+  block_reduce_finish<D>(acc, partials, counters, out, D, sig);
+}
+// fused: bind every table with r (len -> len/2, in place) and evaluate the next round, with k_sc_fold_eval's ownership of four elements per thread
+template <int D>
+__global__ void __launch_bounds__(SCP_THREADS, 4) k_scp_fold_eval(const __grid_constant__ ScPoly P, size_t len, const __grid_constant__ FqConst rc,
+                                                                 u256* partials, unsigned int* counters, u256* out, HostSig sig) {
+  extern __shared__ uint4 scp_sh[];
+  u256* x = reinterpret_cast<u256*>(scp_sh) + threadIdx.x;
+  u256* d = x + P.ntables * SCP_THREADS;
+  const size_t half = len >> 1, quarter = len >> 2;
+  u256 acc[D];
+#pragma unroll
+  for (int p = 0; p < D; p++) acc[p] = fq_zero();
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < quarter; i += (size_t)gridDim.x * blockDim.x) {
+    for (int k = 0; k < P.ntables; k++) {
+      u256* T = P.t[k];
+      const u256 lo = fq_fold_const(ld256(T + i), ld256(T + i + half), rc);   // dense_mlpoly.rs:218
+      const u256 hi = fq_fold_const(ld256(T + i + quarter), ld256(T + i + quarter + half), rc);
+      st256(T + i, lo); st256(T + i + quarter, hi);
+      st256(x + k * SCP_THREADS, lo);
+      st256(d + k * SCP_THREADS, fq_sub(hi, lo));
+    }
+    scp_accumulate<D>(acc, P, x, d);
+  }
+  block_reduce_finish<D>(acc, partials, counters, out, D, sig);
+}
+// Small tables (len/4 <= SC_SMALL_MAX), latency-bound as in k_sc_fold_eval_small: 32 indices per block; warp 2k + h binds half h of table k
+// (one fold per thread), then warp p evaluates point p (t = 0 for p = 0, else p + 1) from the bound values in shared memory.
+#define SCP_SMALL_Q 32
+__device__ __forceinline__ u256 scp_small_point(const u256 (&sh)[SP_SC_MAX_TABLES][2][SCP_SMALL_Q], int k, int e, int tp) {
+  const u256 lo = sh[k][0][e];
+  if (tp == 0) return lo;
+  const u256 hi = sh[k][1][e], dk = fq_sub(hi, lo);
+  u256 v = hi;
+  for (int s = 1; s < tp; s++) v = fq_add(v, dk);
+  return v;
+}
+template <int D>
+__global__ void __launch_bounds__(SCP_SMALL_Q * 2 * SP_SC_MAX_TABLES) k_scp_fold_eval_small(const __grid_constant__ ScPoly P, size_t len,
+                                                                                           const __grid_constant__ FqConst rc, u256* partials,
+                                                                                           unsigned int* counters, u256* out, HostSig sig) {
+  __shared__ u256 sh[SP_SC_MAX_TABLES][2][SCP_SMALL_Q];
+  const size_t half = len >> 1, quarter = len >> 2;
+  const int e = threadIdx.x % SCP_SMALL_Q, th = threadIdx.x / SCP_SMALL_Q;
+  const size_t i = (size_t)blockIdx.x * SCP_SMALL_Q + e;
+  const bool valid = i < quarter;
+  if (valid && th < 2 * P.ntables) {
+    const int k = th >> 1, h = th & 1;
+    const size_t idx = i + (h ? quarter : 0);
+    const u256 v = fq_fold_const(ld256(P.t[k] + idx), ld256(P.t[k] + idx + half), rc);   // dense_mlpoly.rs:218
+    st256(P.t[k] + idx, v);
+    sh[k][h][e] = v;
+  }
+  __syncthreads();
+  u256 acc[D];
+#pragma unroll
+  for (int p = 0; p < D; p++) acc[p] = fq_zero();
+  if (valid && th < D) {
+    const int tp = th == 0 ? 0 : th + 1;
+    u256 sum = fq_zero();
+    for (int t = 0; t < P.nterms; t++) {
+      u256 prod = scp_small_point(sh, P.fac[t][0], e, tp);
+      for (int f = 1; f < P.nfac[t]; f++) prod = fq_mul(prod, scp_small_point(sh, P.fac[t][f], e, tp));
+      if (!P.unit[t]) prod = fq_mul(prod, P.coeff[t]);
+      sum = fq_add(sum, prod);
+    }
+#pragma unroll
+    for (int p = 0; p < D; p++)
+      if (p == th) acc[p] = sum;
+  }
+  block_reduce_finish<D>(acc, partials, counters, out, D, sig);
+}
+
 struct FoldBatch {
   u256* t[64];
 };
@@ -343,6 +464,52 @@ void sc_fold_eval_g(const ScInst* insts, int ninst, size_t len, const u256& r, c
   if (grid.x > SC_MAX_BLOCKS) grid.x = SC_MAX_BLOCKS;
   k_sc_fold_eval_g<<<grid, 256, 0, s>>>(b, len, rc, E, partials, counters, out, sig, xr);
   SP_LAUNCHED(); check("sc_fold_eval_g");
+}
+// rc == null: the first round (k_scp_eval); else the fused bind + evaluate, in its small-table form for len/4 <= SC_SMALL_MAX
+template <int D>
+static void scp_launch(const ScPoly& P, size_t len, const FqConst* rc, u256* out, void* scratch, cudaStream_t s, HostSig sig) {
+  unsigned int* counters = (unsigned int*)scratch;
+  u256* partials = (u256*)((char*)scratch + 256);
+  if (rc && len / 4 <= SC_SMALL_MAX) {
+    const int nth = 2 * P.ntables > D ? 2 * P.ntables : D;
+    k_scp_fold_eval_small<D><<<(unsigned)((len / 4 + SCP_SMALL_Q - 1) / SCP_SMALL_Q), SCP_SMALL_Q * nth, 0, s>>>(P, len, *rc, partials, counters, out, sig);
+    return;
+  }
+  const size_t smem = 2 * (size_t)P.ntables * SCP_THREADS * sizeof(u256);   // up to 64 KB: above the default 48 KB opt-in
+  const void* fn = rc ? (const void*)k_scp_fold_eval<D> : (const void*)k_scp_eval<D>;
+  if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) check("scp shared memory");
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, SCP_THREADS, smem) != cudaSuccess) check("scp occupancy");
+  dim3 grid(grid_for(rc ? len / 4 : len / 2, SCP_THREADS, per_sm > 0 ? per_sm : 1));
+  if (grid.x > SC_MAX_BLOCKS) grid.x = SC_MAX_BLOCKS;
+  if (rc) k_scp_fold_eval<D><<<grid, SCP_THREADS, smem, s>>>(P, len, *rc, partials, counters, out, sig);
+  else k_scp_eval<D><<<grid, SCP_THREADS, smem, s>>>(P, len, partials, counters, out, sig);
+}
+static void scp_dispatch(const ScPoly& P, size_t len, const FqConst* rc, u256* out, void* scratch, cudaStream_t s, HostSig sig) {
+  if (P.ntables < 1 || P.ntables > SP_SC_MAX_TABLES || P.nterms < 1 || P.nterms > SP_SC_MAX_TERMS)
+    throw std::runtime_error("spartan_b200: sumcheck polynomial outside the kernel's limits");
+  switch (P.degree) {
+    case 1: scp_launch<1>(P, len, rc, out, scratch, s, sig); break;
+    case 2: scp_launch<2>(P, len, rc, out, scratch, s, sig); break;
+    case 3: scp_launch<3>(P, len, rc, out, scratch, s, sig); break;
+    case 4: scp_launch<4>(P, len, rc, out, scratch, s, sig); break;
+    case 5: scp_launch<5>(P, len, rc, out, scratch, s, sig); break;
+    case 6: scp_launch<6>(P, len, rc, out, scratch, s, sig); break;
+    default: throw std::runtime_error("spartan_b200: sumcheck polynomial degree outside 1.." + std::to_string(SP_SC_MAX_DEGREE));
+  }
+  SP_LAUNCHED();
+}
+void scp_eval(const ScPoly& p, size_t len, u256* out, void* scratch, cudaStream_t s, HostSig sig) {
+  ProfScope ps("scp_eval", (double)p.ntables * (double)len * 32.0, s);
+  scp_dispatch(p, len, nullptr, out, scratch, s, sig);
+  check("scp_eval");
+}
+void scp_fold_eval(const ScPoly& p, size_t len, const u256& r, u256* out, void* scratch, cudaStream_t s, HostSig sig) {
+  if (len < 4) throw std::runtime_error("spartan_b200: scp_fold_eval needs tables of at least four entries");
+  ProfScope ps(len / 4 <= SC_SMALL_MAX ? "scp_fold_eval_small" : "scp_fold_eval", (double)p.ntables * (double)len * 48.0, s);
+  const FqConst rc = fq_const_table(r);
+  scp_dispatch(p, len, &rc, out, scratch, s, sig);
+  check("scp_fold_eval");
 }
 static size_t eq_suffix_entries(size_t n0, int K) { size_t t = 0; for (int k = 1; k <= K; k++) t += n0 >> k; return t; }
 void eq_suffix(u256* levels, const u256* E0, size_t n0, int K, cudaStream_t s) {

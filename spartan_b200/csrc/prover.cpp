@@ -410,6 +410,42 @@ std::vector<Fq> ScRounds::wait() {
   return ev;
 }
 
+void poly_sumcheck_prove(Ctx& ctx, const dev::ScPoly& P, size_t len, const Fq& claim, size_t num_rounds, Transcript& T, SumcheckInstanceProof& proof,
+                         std::vector<Fq>& r, std::vector<Fq>& finals, Fq& e) {
+  const size_t d = (size_t)P.degree;
+  u256* d_out = ctx.small.p + 0;   // the d evaluations of a round
+  dev::HostSig sig = ctx.next_sig();
+  dev::scp_eval(P, len, d_out, ctx.red.p, ctx.stream, sig);
+  e = claim;
+  for (size_t j = 0; j < num_rounds; j++) {
+    ctx.wait_sig(sig);
+    std::vector<Fq> ev(d);
+    memcpy(static_cast<void*>(ev.data()), ctx.host_res, d * sizeof(u256));
+    std::vector<Fq> evals(d + 1);   // s_j(0), s_j(1) = e - s_j(0), s_j(2) .. s_j(d)
+    evals[0] = ev[0];
+    evals[1] = e - ev[0];
+    for (size_t t = 2; t <= d; t++) evals[t] = ev[t - 1];
+    UniPoly poly = UniPoly::from_evals(evals);
+    poly.append_to_transcript("poly", T);
+    const Fq r_j = T.challenge_scalar("challenge_nextround");
+    if (j + 1 < num_rounds) {   // bind and evaluate the next round while the host finishes this one
+      sig = ctx.next_sig();
+      dev::scp_fold_eval(P, len, r_j.m, d_out, ctx.red.p, ctx.stream, sig);
+    } else {
+      dev::fold_top(P.t, P.ntables, len, r_j.m, ctx.stream);
+    }
+    len >>= 1;
+    e = poly.evaluate(r_j);
+    proof.compressed_polys.push_back(poly.compress());
+    r.push_back(r_j);
+  }
+  sig = ctx.next_sig();
+  dev::heads(ctx.small.p + 8, P.t, P.ntables, ctx.stream, sig);
+  ctx.wait_sig(sig);
+  finals.resize(P.ntables);
+  memcpy(static_cast<void*>(finals.data()), ctx.host_res, P.ntables * sizeof(u256));
+}
+
 // ================================================================================================ ZK sumcheck on the device
 // prove_quad (sumcheck.rs:428-586) and prove_cubic_with_additive_term (sumcheck.rs:588-776).
 // tables: NT device arrays of length 2^num_rounds, folded in place (their first element holds the final evaluation).

@@ -74,14 +74,37 @@ struct UniPoly {  // unipoly.rs
       Fq a = two_inv * (e[2] - e[1] - e[1] + c);
       Fq b = e[1] - c - a;
       p.coeffs = {c, b, a};
-    } else {
+    } else if (e.size() == 4) {
       Fq d = e[0];
       Fq a = six_inv * (e[3] - e[2] - e[2] - e[2] + e[1] + e[1] + e[1] - e[0]);
       Fq b = two_inv * (e[0] + e[0] - e[1] - e[1] - e[1] - e[1] - e[1] + e[2] + e[2] + e[2] + e[2] - e[3]);
       Fq c = e[1] - d - a - b;
       p.coeffs = {d, c, b, a};
+    } else {
+      p.coeffs = lagrange(e);
     }
     return p;
+  }
+  // the coefficients of the polynomial of degree < n through (i, e[i]), i = 0 .. n-1: sum_i e[i] prod_{j != i} (x - j) / (i - j).  It is unique, so
+  // for n = 3, 4 it is what the closed forms above give
+  static std::vector<Fq> lagrange(const std::vector<Fq>& e) {
+    const size_t n = e.size();
+    std::vector<Fq> out(n, Fq::zero());
+    for (size_t i = 0; i < n; i++) {
+      std::vector<Fq> num{Fq::one()};   // prod_{j != i} (x - j), lowest coefficient first
+      Fq den = Fq::one();
+      for (size_t j = 0; j < n; j++) {
+        if (j == i) continue;
+        const Fq fj = Fq::from_u64(j);
+        std::vector<Fq> next(num.size() + 1, Fq::zero());
+        for (size_t k = 0; k < num.size(); k++) { next[k + 1] += num[k]; next[k] -= num[k] * fj; }
+        num.swap(next);
+        den *= i > j ? Fq::from_u64(i - j) : -Fq::from_u64(j - i);
+      }
+      const Fq w = e[i] * den.inv();
+      for (size_t k = 0; k < n; k++) out[k] += num[k] * w;
+    }
+    return out;
   }
   Fq evaluate(const Fq& r) const {  // unipoly.rs:72-80
     Fq ev = coeffs[0], power = r;
@@ -155,6 +178,15 @@ struct ScRounds {
   std::vector<Fq> wait();                                   // the 3 ninst evaluations of the last launch
   dev::XRank xr();                                          // the cross-rank exchange of the next launch (none once replicated)
 };
+
+// A sumcheck of a caller-defined polynomial (sp_sumcheck_prove_t): SumcheckInstanceProof::prove_cubic (sumcheck.rs:183-252) with comb_func the
+// sum of products P describes.  P.t: the distinct tables, `len` entries each, bound in place for num_rounds rounds.  Out: the proof, the challenges
+// r, finals[k] = P.t[k][0] after the last bind, and the final claim e.  One launch per round (k_scp_eval, then k_scp_fold_eval as soon as r_j is
+// drawn), then one bind and one gather of the first entries.  Single GPU.
+void poly_sumcheck_prove(Ctx& ctx, const dev::ScPoly& P, size_t len, const Fq& claim, size_t num_rounds, Transcript& T, SumcheckInstanceProof& proof,
+                         std::vector<Fq>& r, std::vector<Fq>& finals, Fq& e);
+// SumcheckInstanceProof::verify (sumcheck.rs:27-62) on bincode bytes; SpError(SP_ERR_VERIFY) where the reference asserts or the bytes do not decode
+Fq sumcheck_verify_bytes(const uint8_t* proof, size_t len, const Fq& claim, size_t num_rounds, size_t degree, Transcript& T, std::vector<Fq>& r);
 
 // <x, G[0..n)> of one row of n scalars against the per-window table of `gs`, for latency.  For n >= 2 (even) it is the inner-product round kernel
 // with a = (1, 1) and blocks of two generators: its "L" (odd j) and "R" (even j) reach the host through the kernel's own publication and are added

@@ -744,6 +744,11 @@ void verify_batch(Ctx& ctx, std::vector<VerifyJob>& jobs, const uint8_t seed[32]
 
 }  // namespace
 
+Fq sumcheck_verify_bytes(const uint8_t* proof, size_t len, const Fq& claim, size_t num_rounds, size_t degree, Transcript& T, std::vector<Fq>& r) {
+  const SumcheckInstanceProof p = from_bincode<SumcheckInstanceProof>(proof, len, SP_ERR_VERIFY, "sumcheck proof");
+  return sumcheck_verify(p, claim, num_rounds, degree, T, r);
+}
+
 // NIZK::verify (lib.rs:549-591)
 void nizk_verify(Ctx& ctx, const Instance& inst, const std::vector<Fq>& input, const R1CSGens& gens, Transcript& T, const uint8_t* proof, size_t len) {
   check_dims(inst.num_cons, inst.num_vars, inst.num_inputs);
