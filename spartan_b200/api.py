@@ -7,7 +7,7 @@ import zlib
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB_PATH = os.path.join(_HERE, "libspartan_b200%s.so" % os.environ.get("SP_LIB_TAG", ""))  # SP_LIB_TAG: tuning builds only
+_LIB_PATH = os.path.join(_HERE, "libspartan_b200.so")
 
 SP_OK, SP_ERR_NO_DEVICE, SP_ERR_CUDA, SP_ERR_INVALID_ARG, SP_ERR_INVALID_INDEX, SP_ERR_INVALID_SCALAR, SP_ERR_INVALID_INPUTS, SP_ERR_INTERNAL = range(8)
 SP_ERR_INVALID_POINT, SP_ERR_VERIFY, SP_ERR_DECOMPRESS = 8, 9, 10

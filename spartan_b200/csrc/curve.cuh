@@ -41,27 +41,17 @@ SP_HD ge ge_add(const ge& p, const ge& q) {
   return r;
 }
 // mixed addition with an affine niels point (7M); `neg` adds -q instead
-// SP_MADD_NI_MASK (tuning builds): bit k set = product k of the seven goes through the out-of-line fp_mul_ni (smaller loop body in k_msm_rows, whose top
-// stall is instruction fetch, against ~24 register moves per call); 0 = all inline (default)
-#ifndef SP_MADD_NI_MASK
-#define SP_MADD_NI_MASK 0
-#endif
-#if defined(__CUDA_ARCH__)
-#define SP_MADD_MUL(k, a, b) (((SP_MADD_NI_MASK >> (k)) & 1) ? fp_mul_ni(a, b) : fp_mul(a, b))
-#else
-#define SP_MADD_MUL(k, a, b) fp_mul(a, b)
-#endif
 SP_HD ge ge_madd(const ge& p, const ge_niels& q, bool neg) {
   u256 qa = neg ? q.ypx : q.ymx;  // (y-x) of +/-q
   u256 qb = neg ? q.ymx : q.ypx;
-  u256 A = SP_MADD_MUL(0, fp_sub(p.Y, p.X), qa);
-  u256 B = SP_MADD_MUL(1, fp_add(p.Y, p.X), qb);
-  u256 C = SP_MADD_MUL(2, p.T, q.t2d);
+  u256 A = fp_mul(fp_sub(p.Y, p.X), qa);
+  u256 B = fp_mul(fp_add(p.Y, p.X), qb);
+  u256 C = fp_mul(p.T, q.t2d);
   if (neg) C = fp_neg(C);
   u256 D = fp_add(p.Z, p.Z);
   u256 E = fp_sub(B, A), F = fp_sub(D, C), G = fp_add(D, C), H = fp_add(B, A);
   ge r;
-  r.X = SP_MADD_MUL(3, E, F); r.Y = SP_MADD_MUL(4, G, H); r.T = SP_MADD_MUL(5, E, H); r.Z = SP_MADD_MUL(6, F, G);
+  r.X = fp_mul(E, F); r.Y = fp_mul(G, H); r.T = fp_mul(E, H); r.Z = fp_mul(F, G);
   return r;
 }
 // dbl-2008-hwcd (4M + 4S)

@@ -202,18 +202,17 @@ void compress_batch(uint8_t* out32, const ge* in, size_t n, cudaStream_t s);
 // table[(j*NWIN + w)*2^(W-1) + (d-1)] = d * 2^(W*w) * G_j in affine-niels form; W (wbits) is 8 or 13, NWIN = ceil(253 / W)
 size_t table_entries(size_t nbases, int wbits);
 void build_tables(ge_niels* table, const ge* G, size_t nbases, int wbits, cudaStream_t s);
-// row table: rt[j*2^(W-1) + (d-1)] = d * G_j for every base; W is a build-time constant (-DSP_ROW_WBITS, 16 by default)
+// row table: rt[j*2^(W-1) + (d-1)] = d * G_j for every base; W = ROW_W = 16 (kernels.cu)
 size_t row_table_entries(size_t nbases);
 void build_row_table(ge_niels* rt, const ge* G, size_t nbases, cudaStream_t s);
 // out[row] = sum_{j<R} scalars[row*stride + j] * G_j  (+ blinds[row] * G_{blind_base} when blinds != null)
 // scalars are Montgomery-form; partial: scratch >= msm_scratch_bytes(L, R).  Many long rows run on `row_table` when the set has one (null: none),
 // every other shape on the per-window `table`.
 size_t msm_scratch_bytes(size_t L, size_t R);
-// launch shape overrides for an MSM that runs in the background of latency-bound work: cpt = column passes per CTA (0: automatic, 1 or 4: short- or
-// long-lived CTAs), smem_pad = bytes of unused dynamic shared memory per CTA (caps the resident CTAs per SM)
-struct MsmTune { int cpt = 0; size_t smem_pad = 0; };
+// smem_pad: bytes of unused dynamic shared memory per CTA, which cap the resident CTAs per SM (an MSM that runs in the background of
+// latency-bound work leaves them room)
 void msm_rows(ge* out, const ge_niels* table, int wbits, const ge_niels* row_table, const u256* scalars, size_t stride, size_t L, size_t R,
-              const u256* blinds, size_t blind_base, void* scratch, cudaStream_t s, const MsmTune& tune = MsmTune());
+              const u256* blinds, size_t blind_base, void* scratch, cudaStream_t s, size_t smem_pad = 0);
 
 void add_points(ge* a, const ge* b, size_t n, cudaStream_t s);   // a[i] += b[i]
 void sum_points(ge* out, const ge* in, int n, cudaStream_t s);   // out[0] = in[0] + ... + in[n-1], n <= 32

@@ -204,12 +204,12 @@ SP_HD bool fq_eq(const u256& a, const u256& b) {
 
 // Montgomery product a*b*2^-256 mod q, coarsely-integrated operand scanning on 32-bit limbs.
 // The three zero limbs of q (4,5,6) drop out of the reduction at compile time.
-#if defined(__CUDA_ARCH__) && defined(SP_NI_FQ)
+#ifdef __CUDA_ARCH__
 static __device__ __noinline__ u256 fq_mul_ni(u256 a, u256 b);
 #endif
 SP_HD u256 fq_mul_impl(const u256& a, const u256& b);
 SP_HD u256 fq_mul(const u256& a, const u256& b) {
-#if defined(__CUDA_ARCH__) && defined(SP_NI_FQ)
+#ifdef __CUDA_ARCH__
   return fq_mul_ni(a, b);   // keeps the instruction footprint of the big fused kernels inside the instruction cache
 #else
   return fq_mul_impl(a, b);
@@ -254,7 +254,7 @@ SP_HD u256 fq_mul_impl(const u256& a, const u256& b) {
   return fq_cond_sub_q(r);  // t < 2q and t[8] == 0
 #endif
 }
-#if defined(__CUDA_ARCH__) && defined(SP_NI_FQ)
+#ifdef __CUDA_ARCH__
 static __device__ __noinline__ u256 fq_mul_ni(u256 a, u256 b) { return fq_mul_impl(a, b); }
 #endif
 SP_HD u256 fq_sqr(const u256& a) { return fq_mul(a, a); }
@@ -459,17 +459,8 @@ SP_HD u256 fp_sub(const u256& a, const u256& b) {
 }
 SP_HD u256 fp_neg(const u256& a) { return fp_sub(fp_zero(), a); }
 
-#if defined(__CUDA_ARCH__)
-static __device__ __noinline__ u256 fp_mul_ni(u256 a, u256 b);
-#endif
 SP_HD u256 fp_mul_impl(const u256& a, const u256& b);
-SP_HD u256 fp_mul(const u256& a, const u256& b) {
-#if defined(__CUDA_ARCH__) && defined(SP_NI_FP)
-  return fp_mul_ni(a, b);
-#else
-  return fp_mul_impl(a, b);
-#endif
-}
+SP_HD u256 fp_mul(const u256& a, const u256& b) { return fp_mul_impl(a, b); }
 SP_HD u256 fp_mul_impl(const u256& a, const u256& b) {
 #if SP_HOST_FAST
   return host_fp_mul(a, b);

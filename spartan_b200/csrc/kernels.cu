@@ -503,11 +503,7 @@ void build_tables(ge_niels* table, const ge* G, size_t nbases, int wbits, cudaSt
 }
 // ---- row tables: entry (j, d-1) = d * G_j, d = 1 .. 2^(ROW_W-1), affine niels, no per-window copies (3.1 MB per generator at ROW_W = 16).  The row MSM
 // sums the entries of each window separately and pays the window shift once per row (k_msm_horner).  One thread per (generator, run of 64 entries).
-#ifndef SP_ROW_WBITS
-#define SP_ROW_WBITS 16
-#endif
-static_assert(SP_ROW_WBITS >= 14 && SP_ROW_WBITS <= 17, "row-table window width");
-constexpr int ROW_W = SP_ROW_WBITS, ROW_NWIN = (253 + ROW_W - 1) / ROW_W;
+constexpr int ROW_W = 16, ROW_NWIN = (253 + ROW_W - 1) / ROW_W;   // 17 bits measured level with 16 (DESIGN.md §7)
 constexpr size_t ROW_DEPTH = (size_t)1 << (ROW_W - 1);
 constexpr int ROW_BUILD_RUN = 64;
 size_t row_table_entries(size_t nbases) { return nbases * ROW_DEPTH; }
@@ -536,10 +532,7 @@ void build_row_table(ge_niels* rt, const ge* G, size_t nbases, cudaStream_t s) {
 // ---- multi-row fixed-base MSM
 // grid = (chunks, L); block = 128 threads = COLS columns x GROUPS window-groups of one row.  A thread owns one scalar and the windows
 // [g*WPT, (g+1)*WPT) of it; signed W-bit digits, zero digits are skipped (vartime, like the reference's vartime_multiscalar_mul).
-// Partial sums are tree-reduced through shared memory.
-#ifndef SP_MSM_LB
-#define SP_MSM_LB 1
-#endif
+// Partial sums are tree-reduced through shared memory.  At most 128 registers per thread (4 CTAs of 128 threads per SM).
 __device__ __forceinline__ ge shfl_down_ge(const ge& p, int delta) {
   ge r;
   r.X = shfl_down_256(p.X, delta); r.Y = shfl_down_256(p.Y, delta); r.Z = shfl_down_256(p.Z, delta); r.T = shfl_down_256(p.T, delta);
@@ -557,8 +550,8 @@ __device__ __forceinline__ ge block_sum_ge_128(ge acc) {
   return acc;
 }
 template <int WBITS, int GROUPS, int CPT>
-__global__ void __launch_bounds__(128, SP_MSM_LB) k_msm_rows(ge* partial, const ge_niels* __restrict__ table, const u256* __restrict__ scalars, size_t stride,
-                                                             size_t R, const u256* __restrict__ blinds, size_t blind_base) {
+__global__ void __launch_bounds__(128, 4) k_msm_rows(ge* partial, const ge_niels* __restrict__ table, const u256* __restrict__ scalars, size_t stride,
+                                                     size_t R, const u256* __restrict__ blinds, size_t blind_base) {
   constexpr int NWIN = (253 + WBITS - 1) / WBITS;
   constexpr int WPT = (NWIN + GROUPS - 1) / GROUPS;   // windows per thread
   constexpr int COLS = 128 / GROUPS;                  // columns per block per pass; CPT passes amortise the reduction tree
@@ -637,13 +630,8 @@ void sum_points(ge* out, const ge* in, int n, cudaStream_t s) {
 // points of both sides.  WPQ balances the two costs: a lone warp already keeps much of its
 // sub-partition's multiply pipe busy, so two windows per quad (4608 warps for 4096 generators) are throughput-bound; six or seven windows
 // per quad need a quarter of the warps and add only a few mixed additions to the dependent chain.
-#ifndef SP_IPAQ_THREADS
-#define SP_IPAQ_THREADS 256
-#endif
-#ifndef SP_IPAQ_SPLIT
-#define SP_IPAQ_SPLIT 4   // window groups per scalar (17 windows -> 5 per quad)
-#endif
-#define IPAQ_THREADS SP_IPAQ_THREADS
+constexpr int IPAQ_THREADS = 256;
+constexpr int IPAQ_SPLIT = 4;   // window groups per scalar (17 windows -> 5 per quad)
 template <int WBITS, int WPQ>
 __global__ void __launch_bounds__(IPAQ_THREADS, 2) k_ipa_msm_quad(ge* partial, const ge_niels* __restrict__ table, const u256* __restrict__ a, const u256* __restrict__ sv,
                                                                   size_t n_cur, size_t n_full, unsigned int* ticket, ge* out, HostSig sig,
@@ -770,7 +758,7 @@ __global__ void __launch_bounds__(IPAQ_THREADS, 2) k_ipa_msm_quad(ge* partial, c
   }
 }
 // windows per quad: the window count split into three groups (17 -> 6, 20 -> 7, 32 -> 11)
-template <int WBITS> struct IpaQ { static constexpr int NWIN = (253 + WBITS - 1) / WBITS, WPQ = (NWIN + SP_IPAQ_SPLIT - 1) / SP_IPAQ_SPLIT, QPS = (NWIN + WPQ - 1) / WPQ; };
+template <int WBITS> struct IpaQ { static constexpr int NWIN = (253 + WBITS - 1) / WBITS, WPQ = (NWIN + IPAQ_SPLIT - 1) / IPAQ_SPLIT, QPS = (NWIN + WPQ - 1) / WPQ; };
 template <int WBITS>
 static void ipa_msm_quad_launch(ge* out, const ge_niels* table, const u256* a, const u256* svec, size_t n_cur, size_t n_full, void* scratch, unsigned int* ticket,
                                 cudaStream_t s, HostSig sig, const u256* b, u256* c_out, HostSig sigc) {
@@ -780,7 +768,7 @@ static void ipa_msm_quad_launch(ge* out, const ge_niels* table, const u256* a, c
   k_ipa_msm_quad<WBITS, IpaQ<WBITS>::WPQ><<<grid, IPAQ_THREADS, 0, s>>>((ge*)scratch, table, a, svec, n_cur, n_full, ticket, out, sig, b, c_out, sigc);
 }
 size_t ipa_msm_scratch_points(size_t n_full, int wbits) {   // partial points of the quad-lane kernel (>= 2 blocks per side when the dots are fused)
-  const size_t nwin = (size_t)msm_nwin(wbits), total = n_full / 2, wpq = (nwin + SP_IPAQ_SPLIT - 1) / SP_IPAQ_SPLIT, qps = (nwin + wpq - 1) / wpq;
+  const size_t nwin = (size_t)msm_nwin(wbits), total = n_full / 2, wpq = (nwin + IPAQ_SPLIT - 1) / IPAQ_SPLIT, qps = (nwin + wpq - 1) / wpq;
   return 2 * std::max<size_t>((total * qps + IPAQ_THREADS / 4 - 1) / (IPAQ_THREADS / 4), 2);
 }
 void ipa_msm(ge* out, const ge_niels* table, int wbits, const u256* a, const u256* svec, size_t n_cur, size_t n_full, void* scratch, unsigned int* ticket,
@@ -820,13 +808,10 @@ __global__ void __launch_bounds__(128) k_msm_digits(int* digits, const u256* __r
     }
   }
 }
-#ifndef SP_ROW_CHUNK
-#define SP_ROW_CHUNK 256
-#endif
-constexpr size_t ROW_CHUNK = SP_ROW_CHUNK;
+constexpr size_t ROW_CHUNK = 256;
 // grid = (groups / 32, chunks): CTA (x, y) sums columns [y * ROW_CHUNK, (y + 1) * ROW_CHUNK) of the 32 (row, window) groups [32 x, 32 x + 32)
-__global__ void __launch_bounds__(128, SP_MSM_LB) k_msm_win(ge* part, const ge_niels* __restrict__ rt, const int* __restrict__ digits, size_t groups, size_t ncols,
-                                                            size_t R, size_t blind_base) {
+__global__ void __launch_bounds__(128, 4) k_msm_win(ge* part, const ge_niels* __restrict__ rt, const int* __restrict__ digits, size_t groups, size_t ncols,
+                                                    size_t R, size_t blind_base) {
   const size_t g = (size_t)blockIdx.x * 32 + threadIdx.x / 4;   // (row, window) = (g / ROW_NWIN, g % ROW_NWIN)
   const int lane = threadIdx.x % 4;
   const size_t c0 = (size_t)blockIdx.y * ROW_CHUNK, c1 = c0 + ROW_CHUNK < ncols ? c0 + ROW_CHUNK : ncols;
@@ -929,18 +914,16 @@ static void msm_launch(int groups, int cpt, dim3 grid, cudaStream_t s, ge* pp, c
   else msm_launch2<WBITS, 8>(cpt, grid, s, pp, table, sc, stride, R, bl, blind_base, smem_pad);
 }
 void msm_rows(ge* out, const ge_niels* table, int wbits, const ge_niels* row_table, const u256* scalars, size_t stride, size_t L, size_t R,
-              const u256* blinds, size_t blind_base, void* scratch, cudaStream_t s, const MsmTune& tune) {
+              const u256* blinds, size_t blind_base, void* scratch, cudaStream_t s, size_t smem_pad) {
   ProfScope ps("msm_rows", 32.0 * (double)L * (double)R + 32.0 * (double)R, s);
   if (row_table && msm_rows_use_row_table(L, R)) {
-    msm_rows_win(out, row_table, scalars, stride, L, R, blinds, blind_base, scratch, s, tune.smem_pad);
+    msm_rows_win(out, row_table, scalars, stride, L, R, blinds, blind_base, scratch, s, smem_pad);
     return;
   }
   const size_t ncols = R + (blinds ? 1 : 0);
   int groups = msm_pick_groups(L, R);
-  int cpt = tune.cpt ? tune.cpt : msm_pick_cpt(L, ncols, groups);
-  if (cpt != 4) cpt = 1;
+  int cpt = msm_pick_cpt(L, ncols, groups);
   size_t chunks = msm_chunks(ncols, groups, cpt);
-  const size_t smem_pad = tune.smem_pad;
   ge* partial = (ge*)scratch;
   for (size_t row0 = 0; row0 < L; row0 += 32768) {   // gridDim.y limit 65535
     size_t rows = L - row0 < 32768 ? L - row0 : 32768;

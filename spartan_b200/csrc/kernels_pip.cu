@@ -84,19 +84,15 @@ PipPlan pip_plan(size_t n, int c_override) {
   p.nwin = 253 / c + 1;
   p.nb = 1u << (c - 1);
   // tiles of 4*nb scalars (for c = 13..16: many blocks in flight beat amortising the nb-word flush further)
-  const char* tm = getenv("SP_PIP_TILE_MULT");
-  size_t tile = (size_t)p.nb * (tm ? (size_t)atoi(tm) : 4);
+  size_t tile = (size_t)p.nb * 4;
   if (tile < 8192) tile = 8192;
   p.tile = tile;
   p.ntiles = (n + tile - 1) / tile;
   if (!p.ntiles) p.ntiles = 1;
   // work items: at most S consecutive entries of one bucket, summed by G lanes.  G is sized so a lane gets ~64 additions from an average
   // bucket (n/nb entries), S so that an oversized bucket (skewed scalars) is split across items
-  const char* ge_ = getenv("SP_PIP_LANES");
   int G = 32;
   while (G > 1 && (n / p.nb) / (size_t)G < 64) G >>= 1;
-  if (ge_) G = atoi(ge_);
-  if (G < 1 || G > 32 || (G & (G - 1))) throw std::runtime_error("spartan_b200: SP_PIP_LANES must be a power of two <= 32");
   p.G = G;
   size_t S = 2 * (n / p.nb);
   if (S < (size_t)G * 64) S = (size_t)G * 64;
@@ -142,9 +138,7 @@ __global__ void __launch_bounds__(256) k_pip_prepare(uint32_t* __restrict__ kp, 
   }
 }
 
-#ifndef PIP_UNROLL
-#define PIP_UNROLL 8
-#endif
+constexpr int PIP_UNROLL = 8;
 // signed digit of window w: 0 = skip, else bucket |d|-1 and sign
 __device__ __forceinline__ int pip_digit(const uint32_t* __restrict__ kp, size_t n, size_t i, int w, int c, int nwin) {
   const int b = w * c, limb = b >> 5, sh = b & 31;
@@ -228,12 +222,9 @@ __global__ void __launch_bounds__(1024) k_pip_scatter(uint32_t* __restrict__ sor
   }
 }
 
-#ifndef SP_PIP_LB
-#define SP_PIP_LB 4
-#endif
 // G = lanes per work item (power of two <= 32): few lanes when buckets are small, so the shuffle tree (log2 G additions) stays a small
 // fraction of the item's mixed additions
-__global__ void __launch_bounds__(128, SP_PIP_LB) k_pip_accumulate(ge* __restrict__ partial, const ge_niels* __restrict__ pts, const uint32_t* __restrict__ sorted,
+__global__ void __launch_bounds__(128, 4) k_pip_accumulate(ge* __restrict__ partial, const ge_niels* __restrict__ pts, const uint32_t* __restrict__ sorted,
                                                                   const uint32_t* __restrict__ start, const uint32_t* __restrict__ counts,
                                                                   const uint32_t* __restrict__ istart, const uint32_t* __restrict__ nitems, size_t n, uint32_t nb,
                                                                   uint32_t S, size_t max_items, int G) {
@@ -263,11 +254,9 @@ __global__ void __launch_bounds__(128, SP_PIP_LB) k_pip_accumulate(ge* __restric
     const uint32_t v = vnext;
     if (e + G < last) {
       vnext = so[e + G];
-#ifndef SP_PIP_NO_PREFETCH
       const char* nq = reinterpret_cast<const char*>(pts + (vnext & 0x7fffffffu));
       asm volatile("prefetch.global.L2 [%0];" ::"l"(nq));
       asm volatile("prefetch.global.L2 [%0];" ::"l"(nq + 64));
-#endif
     }
     const ge_niels* q = pts + (v & 0x7fffffffu);
     ge_niels nl;

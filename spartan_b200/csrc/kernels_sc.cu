@@ -1,10 +1,6 @@
 // spartan_b200 — sumcheck-round kernels (K1/K2 of SURVEY.md §2b), their own translation unit so the two .cu files build in parallel.
 #include "kcommon.cuh"
 
-#ifndef SP_SC_LB
-#define SP_SC_LB 1
-#endif
-
 namespace sp {
 namespace dev {
 
@@ -42,7 +38,7 @@ __device__ __forceinline__ void sc_accumulate(u256 (&acc)[3], const u256 (&lo)[4
 }
 
 template <int KIND>
-__global__ void __launch_bounds__(256, SP_SC_LB) k_sc_eval(ScBatch batch, size_t len, u256* partials, unsigned int* counters, u256* out, HostSig sig,
+__global__ void __launch_bounds__(256, 2) k_sc_eval(ScBatch batch, size_t len, u256* partials, unsigned int* counters, u256* out, HostSig sig,
                                                                    const __grid_constant__ XRank xr) {
   constexpr int NT = KIND == SC_QUAD ? 2 : (KIND == SC_CUBIC3 ? 3 : 4);
   const ScInst& in = batch.inst[blockIdx.y];
@@ -64,7 +60,7 @@ __global__ void __launch_bounds__(256, SP_SC_LB) k_sc_eval(ScBatch batch, size_t
 // The bind is the constant-multiplier fold (fq_fold_const: table of r*2^(32j) mod q in uniform registers, 72 wide products and no separate
 // modular addition) instead of sub + Montgomery product + add; same canonical values.
 template <int KIND>
-__global__ void __launch_bounds__(256, SP_SC_LB) k_sc_fold_eval(ScBatch batch, size_t len, const __grid_constant__ FqConst rc, u256* partials,
+__global__ void __launch_bounds__(256, 2) k_sc_fold_eval(ScBatch batch, size_t len, const __grid_constant__ FqConst rc, u256* partials,
                                                        unsigned int* counters, u256* out, HostSig sig, const __grid_constant__ XRank xr) {
   constexpr int NT = KIND == SC_QUAD ? 2 : (KIND == SC_CUBIC3 ? 3 : 4);
   const ScInst& in = batch.inst[blockIdx.y];
@@ -99,7 +95,7 @@ __global__ void __launch_bounds__(256, SP_SC_LB) k_sc_fold_eval(ScBatch batch, s
 // cubic evaluations, no C table to bind, 2 values per instance to reduce.  The host rebuilds s_j(0), s_j(2), s_j(3) — the field elements the
 // reference computes (sumcheck.rs:296-355) — so the proof bytes do not change.  Streaming rounds only; the small-table tail runs the standard
 // kernels on C = prefix * eq(tau[j..], .).   out[3*inst + 0] = q(0), out[3*inst + 1] = q(inf).
-__global__ void __launch_bounds__(256, SP_SC_LB) k_sc_eval_g(ScBatch batch, size_t len, const u256* __restrict__ E, u256* partials, unsigned int* counters,
+__global__ void __launch_bounds__(256, 2) k_sc_eval_g(ScBatch batch, size_t len, const u256* __restrict__ E, u256* partials, unsigned int* counters,
                                                               u256* out, HostSig sig, const __grid_constant__ XRank xr) {
   const ScInst& in = batch.inst[blockIdx.y];
   const size_t half = len >> 1;
@@ -114,7 +110,7 @@ __global__ void __launch_bounds__(256, SP_SC_LB) k_sc_eval_g(ScBatch batch, size
 }
 // fused: bind A and B with r (len -> len/2, in place, constant-multiplier fold) and evaluate the next round's q(0), q(inf) with the weights
 // E = eq(tau[j+2..], .) of len/4 entries
-__global__ void __launch_bounds__(256, SP_SC_LB) k_sc_fold_eval_g(ScBatch batch, size_t len, const __grid_constant__ FqConst rc, const u256* __restrict__ E,
+__global__ void __launch_bounds__(256, 2) k_sc_fold_eval_g(ScBatch batch, size_t len, const __grid_constant__ FqConst rc, const u256* __restrict__ E,
                                                                    u256* partials, unsigned int* counters, u256* out, HostSig sig, const __grid_constant__ XRank xr) {
   const ScInst& in = batch.inst[blockIdx.y];
   const size_t half = len >> 1, quarter = len >> 2;
@@ -433,7 +429,7 @@ void sc_fold_eval(ScKind kind, const ScInst* insts, int ninst, size_t len, const
     SP_LAUNCHED(); check("sc_fold_eval_small");
     return;
   }
-  dim3 grid(grid_for(len / 4, 256, SP_SC_LB), ninst);
+  dim3 grid(grid_for(len / 4, 256, 2), ninst);
   if (grid.x > SC_MAX_BLOCKS) grid.x = SC_MAX_BLOCKS;
   switch (kind) {
     case SC_QUAD: k_sc_fold_eval<SC_QUAD><<<grid, 256, 0, s>>>(b, len, rc, partials, counters, out, sig, xr); break;
@@ -460,7 +456,7 @@ void sc_fold_eval_g(const ScInst* insts, int ninst, size_t len, const u256& r, c
   unsigned int* counters = (unsigned int*)scratch;
   u256* partials = (u256*)((char*)scratch + 256);
   const FqConst rc = fq_const_table(r);
-  dim3 grid(grid_for(len / 4, 256, SP_SC_LB), ninst);
+  dim3 grid(grid_for(len / 4, 256, 2), ninst);
   if (grid.x > SC_MAX_BLOCKS) grid.x = SC_MAX_BLOCKS;
   k_sc_fold_eval_g<<<grid, 256, 0, s>>>(b, len, rc, E, partials, counters, out, sig, xr);
   SP_LAUNCHED(); check("sc_fold_eval_g");

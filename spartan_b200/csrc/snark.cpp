@@ -509,8 +509,7 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
   for (int m = 0; m < 3; m++) { row_val[m] = derefs.p + (size_t)m * N; col_val[m] = derefs.p + (size_t)(3 + m) * N; }
   const size_t ell_d = log2_ceil(8 * N), L_d = (size_t)1 << (ell_d / 2), R_d = (size_t)1 << (ell_d - ell_d / 2);
   if (R_d != gens.gens_derefs.n) throw SpError(SP_ERR_INVALID_ARG, "polynomial size does not match the commitment generators (num_nz_entries too small?)");
-  static const bool early_ok = getenv("SP_NO_EARLY_DEREFS") == nullptr;
-  const bool early = early_ok && ctx.overlap && N % R_d == 0;                    // each of the two parts is a whole number of matrix rows
+  const bool early = ctx.overlap && N % R_d == 0;                 // each of the two parts is a whole number of matrix rows
   const size_t n_part = early ? 3 * N / R_d : 0;                  // rows per part; rows [2 n_part, L_d) are zero: the identity, 32 zero bytes
   const size_t Wd = (size_t)ctx.shard_world();
   const bool shard_rows = early && Wd > 1 && n_part % Wd == 0;    // rank r commits rows [r n_part/W, (r+1) n_part/W) of either part
@@ -523,16 +522,9 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
     Ctx& c; bool forked = false;
     ~ForkGuard() { if (forked) { try { dev::stream_sync(c.stream2); } catch (...) {} } }
   } fork_guard{ctx};
-  dev::MsmTune early_tune;
-  {
-    // three resident MSM CTAs per SM instead of four leave a quarter of every register file to the prover's stream (DESIGN.md's switch table
-    // has the H100 A/B)
-    static const char* e_cpt = getenv("SP_EARLY_MSM_CPT");
-    static const char* e_smem = getenv("SP_EARLY_MSM_SMEM");
-    early_tune.smem_pad = 60 << 10;
-    if (e_cpt) early_tune.cpt = atoi(e_cpt);
-    if (e_smem) early_tune.smem_pad = (size_t)atol(e_smem);
-  }
+  // a 60 KB shared-memory pad: three resident MSM CTAs per SM instead of four leave a quarter of every register file to the prover's stream
+  // (DESIGN.md §3 has the H100 A/B)
+  const size_t early_smem_pad = 60 << 10;
   if (early) {
     d_chal2.alloc(64); eq_small2.alloc(eq_small.n); early_rows.alloc(2 * cnt); early_comp.alloc(64 * cnt);
     const size_t need = dev::msm_scratch_bytes(cnt, R_d) + 64;
@@ -554,7 +546,7 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
     for (int m = 0; m < 3; m++) dev::gather(part ? col_val[m] : row_val[m], mem, (part ? enc.col : enc.row).ops_addr_idx[m].p, N, s2);
     const size_t first = (size_t)part * n_part + (shard_rows ? (size_t)ctx.rank() * cnt : 0);
     const CommitKey& key = gens.gens_derefs.gens_n;
-    dev::msm_rows(early_rows.p + (size_t)part * cnt, key.set->table.p, key.set->wbits, key.set->rows(), derefs.p + first * R_d, R_d, cnt, R_d, nullptr, key.h, ctx.scratch2.p, s2, early_tune);
+    dev::msm_rows(early_rows.p + (size_t)part * cnt, key.set->table.p, key.set->wbits, key.set->rows(), derefs.p + first * R_d, R_d, cnt, R_d, nullptr, key.h, ctx.scratch2.p, s2, early_smem_pad);
     dev::compress_batch(early_comp.p + 32 * (size_t)part * cnt, early_rows.p + (size_t)part * cnt, cnt, s2);
   };
   R1csHooks hooks;

@@ -193,16 +193,21 @@ def test_snark_caller_owned_transcript(sb):
         sb.SNARK.prove(inst, comm, vars_, inputs, gens, b"snark_example", sb.tape_seed(seed)).bytes
 
 
-def test_scheduling_switches_do_not_change_bytes():
-    """The background-stream commitment of the dereferenced values (snark.cpp) and its launch shape (column passes per CTA, shared-memory pad) only
-    change WHEN and HOW things are computed: the proof bytes with the commitment on the prover's stream, or with another launch shape, must equal
-    the default's (each variant is its own process: the switches are read once per process)."""
-    import json, subprocess, sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    shas = {}
-    for name, env in [("default", {}), ("no_early", {"SP_NO_EARLY_DEREFS": "1"}), ("cpt1_smem", {"SP_EARLY_MSM_CPT": "1", "SP_EARLY_MSM_SMEM": "61440"})]:
-        e = dict(os.environ); e.update(env)
-        out = subprocess.run([sys.executable, os.path.join(root, "tools", "ab_prove.py"), name, "12", "1"], env=e, capture_output=True, text=True, timeout=600)
-        assert out.returncode == 0, out.stderr[-2000:]
-        shas[name] = json.loads(out.stdout.strip().splitlines()[-1])["sha256"]
-    assert len(set(shas.values())) == 1, shas
+def test_overlap_does_not_change_bytes(sb):
+    """The background-stream commitment of the dereferenced values (snark.cpp) only changes WHEN things are computed: with the overlap off the
+    commitment runs on the prover's stream, and the proof bytes must equal the overlapped proof's."""
+    from test_instance_shapes import plan
+    n = 1 << 12
+    assert plan(n, n, 10, (n, n, n))["early"]   # a shape that takes the background path when the overlap is on
+    inst, vars_, inputs = sb.Instance.produce_synthetic_r1cs(n, n, 10, seed=0)
+    gens = sb.SNARKGens(n, n, 10, n)
+    comm = sb.SNARK.encode(inst, gens)
+    ctx = sb.default_context()
+    proofs = {}
+    try:
+        for overlap in (True, False):
+            ctx.set_overlap(overlap)
+            proofs[overlap] = sb.SNARK.prove(inst, comm, vars_, inputs, gens, b"example", sb.tape_seed(0)).bytes
+    finally:
+        ctx.set_overlap(True)
+    assert proofs[True] == proofs[False]

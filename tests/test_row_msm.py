@@ -11,7 +11,7 @@ from oracle.spartan_ref import core as oc
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 Q = oc.Q
-ROW_WIDTHS = (16, 17)   # row-table window widths a build may use (-DSP_ROW_WBITS, 16 by default): the GPU tests plant the edges of both
+ROW_WIDTHS = (16, 17)   # the row table's window width (16) and the 17-bit alternative measured in DESIGN.md §7: the GPU tests plant the edges of both
 
 
 def edge_scalars(W):

@@ -1,6 +1,6 @@
-"""A/B timing of SNARK::prove at 2^logn under the current environment (library tag / tuning switches are read from the environment by the
-library, so every variant is its own process): median and best of `reps` device-timed proofs, the phase timers of the last one and the sha256
-of the proof bytes (which no switch may change).  usage: ab_prove.py LABEL [logn=20] [reps=7]"""
+"""Timing of SNARK::prove at 2^logn under the current environment (the library reads SP_MSM_WINDOW and SP_FINE_TIMERS from it, so every
+variant is its own process): median and best of `reps` device-timed proofs, the phase timers of the last one and the sha256 of the proof bytes
+(which no window width may change).  usage: ab_prove.py LABEL [logn=20] [reps=7]"""
 import hashlib, json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import spartan_b200 as sb

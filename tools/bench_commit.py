@@ -13,7 +13,7 @@ def rand_table(n):
     return t
 
 
-res = {"tag": os.environ.get("SP_LIB_TAG", "")}
+res = {}
 for (L, R) in [(1024, 1024), (2048, 4096)]:
     g = sb.MultiCommitGens(R, b"bench-msm")
     p = sb.DensePolynomial(rand_table(L * R))

@@ -7,7 +7,6 @@ import spartan_b200 as sb
 from spartan_b200 import api
 
 logn = int(sys.argv[1]) if len(sys.argv) > 1 and sys.argv[1].isdigit() else 22
-tag = os.environ.get("SP_LIB_TAG", "")
 try:
     peak = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"]
 except Exception:
@@ -23,7 +22,7 @@ def rand_table(n):
     return t
 
 
-res = {"tag": tag, "logn": logn}
+res = {"logn": logn}
 for kind, nt, name in [(2, 4, "cubic4"), (0, 2, "quad"), (1, 3, "cubic3")]:
     polys = [sb.DensePolynomial(rand_table(n)) for _ in range(nt)]
     r = sb.prg_scalars("r", 1)[0]

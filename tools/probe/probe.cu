@@ -25,7 +25,7 @@ __global__ void k_lat(long long* cycles, u256* sink, int iters, const __grid_con
 #pragma unroll 1
   for (int i = 0; i < iters; i++) {
     if (OP == 0) a = fq_mul_impl(a, b);           // inline F_q Montgomery product
-    if (OP == 1) a = fq_mul(a, b);                // as the kernels call it (out of line with SP_NI_FQ)
+    if (OP == 1) a = fq_mul(a, b);                // as the kernels call it (out of line)
     if (OP == 2) a = fp_mul(a, b);
     if (OP == 3) P = ge_madd(P, N, false);
     if (OP == 4) P = ge_add(P, Q);
