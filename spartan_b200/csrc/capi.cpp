@@ -179,14 +179,14 @@ static int sumcheck_tables(Ctx& c, int kind, sp_poly* const* polys, bool sharded
   return nt;
 }
 // sharded: the kernel's cross-rank completion counter and the next exchange (every rank issues it in the same order)
-static dev::HostSig xr_sig(Ctx& c, bool sharded) { dev::HostSig s; if (sharded) s.done = c.sig_done.p; return s; }
+static dev::HostSig xr_sig(Ctx& c, bool sharded) { dev::HostSig s; if (sharded) s.done = c.sig_done.p + layout::SIG_DONE.off; return s; }
 static int sumcheck_eval(sp_ctx* ctx, int kind, sp_poly* const* polys, uint64_t out[3][4], bool sharded) {
   SP_TRY(ctx)
   Ctx& c = ctx->c;
   const int nt = sumcheck_tables(c, kind, polys, sharded);
   dev::ScInst in = make_inst(polys, nt);
-  dev::sc_eval((dev::ScKind)kind, &in, 1, polys[0]->len, c.small.p, c.red.p, c.stream, xr_sig(c, sharded), sharded ? c.comm->next_xr() : dev::XRank());
-  c.get_small(0, reinterpret_cast<Fq*>(out), 3);
+  dev::sc_eval((dev::ScKind)kind, &in, 1, polys[0]->len, c.small.p + layout::SMALL_ROUND.off, c.red.p, c.stream, xr_sig(c, sharded), sharded ? c.comm->next_xr() : dev::XRank());
+  c.get_small(layout::SMALL_ROUND.off, reinterpret_cast<Fq*>(out), 3);
   SP_CATCH(ctx)
 }
 static int sumcheck_fold_eval(sp_ctx* ctx, int kind, sp_poly* const* polys, const uint64_t r[4], uint64_t out[3][4], bool sharded) {
@@ -198,8 +198,8 @@ static int sumcheck_fold_eval(sp_ctx* ctx, int kind, sp_poly* const* polys, cons
                                               : "fold_eval needs length >= 4");
   Fq rr = fq_in(r);
   dev::ScInst in = make_inst(polys, nt);
-  dev::sc_fold_eval((dev::ScKind)kind, &in, 1, polys[0]->len, rr.m, c.small.p, c.red.p, c.stream, xr_sig(c, sharded), sharded ? c.comm->next_xr() : dev::XRank());
-  c.get_small(0, reinterpret_cast<Fq*>(out), 3);
+  dev::sc_fold_eval((dev::ScKind)kind, &in, 1, polys[0]->len, rr.m, c.small.p + layout::SMALL_ROUND.off, c.red.p, c.stream, xr_sig(c, sharded), sharded ? c.comm->next_xr() : dev::XRank());
+  c.get_small(layout::SMALL_ROUND.off, reinterpret_cast<Fq*>(out), 3);
   for (int i = 0; i < nt; i++) polys[i]->len /= 2;
   SP_CATCH(ctx)
 }
@@ -215,7 +215,7 @@ int sp_sumcheck_fold_eval_sharded(sp_ctx* ctx, int kind, sp_poly* const* polys, 
 // (the shared eq table poly_C_par) — it is then bound once, through a temporary, and copied back
 static void batched_insts(sp_ctx* ctx, int ninst, sp_poly* const* A, sp_poly* const* B, sp_poly* const* Cc, std::vector<dev::ScInst>& insts,
                           std::vector<std::pair<sp_poly*, std::unique_ptr<DevBuf<u256>>>>& shared, bool fold) {
-  if (ninst < 1 || ninst > 24) throw SpError(SP_ERR_INVALID_ARG, "batched sumcheck: 1..24 instances");
+  if (ninst < 1 || ninst > dev::SC_MAX_INST) throw SpError(SP_ERR_INVALID_ARG, "batched sumcheck: 1.." + std::to_string(dev::SC_MAX_INST) + " instances");
   const size_t len = A[0]->len;
   if (len < 2 || (len & (len - 1))) throw SpError(SP_ERR_INVALID_ARG, "length must be a power of two >= 2");
   for (int i = 0; i < ninst; i++) {
@@ -255,7 +255,7 @@ int sp_sumcheck_batched_eval(sp_ctx* ctx, int ninst, sp_poly* const* A, sp_poly*
 }
 int sp_sumcheck_batched_fold_eval(sp_ctx* ctx, int ninst, sp_poly* const* A, sp_poly* const* B, sp_poly* const* Cc, const uint64_t r[4], uint64_t* out) {
   SP_TRY(ctx)
-  if (ninst < 1 || ninst > 24) throw SpError(SP_ERR_INVALID_ARG, "batched sumcheck: 1..24 instances");
+  if (ninst < 1 || ninst > dev::SC_MAX_INST) throw SpError(SP_ERR_INVALID_ARG, "batched sumcheck: 1.." + std::to_string(dev::SC_MAX_INST) + " instances");
   if (A[0]->len < 4) throw SpError(SP_ERR_INVALID_ARG, "fold_eval needs length >= 4");
   std::vector<dev::ScInst> insts;
   std::vector<std::pair<sp_poly*, std::unique_ptr<DevBuf<u256>>>> shared;
@@ -290,9 +290,9 @@ int sp_poly_evaluate(sp_ctx* ctx, const sp_poly* p, const uint64_t* r, size_t el
   DevBuf<u256> d_r(ell + 1), small(dev::eq_evals_scratch(ell)), eq(p->len);
   dev::h2d(d_r.p, r, ell * 32, ctx->c.stream);
   dev::eq_evals(eq.p, d_r.p, (int)ell, small.p, ctx->c.stream);
-  dev::dot(ctx->c.small.p + 32, p->d.p, eq.p, p->len, ctx->c.red.p, ctx->c.stream);
+  dev::dot(ctx->c.small.p + layout::SMALL_DOT.off, p->d.p, eq.p, p->len, ctx->c.red.p, ctx->c.stream);
   Fq v;
-  ctx->c.get_small(32, &v, 1);
+  ctx->c.get_small(layout::SMALL_DOT.off, &v, 1);
   fq_out(out, v);
   SP_CATCH(ctx)
 }
@@ -311,9 +311,9 @@ int sp_poly_bound_rows(sp_ctx* ctx, const sp_poly* p, const uint64_t* Lm, size_t
 int sp_dot(sp_ctx* ctx, const sp_poly* a, const sp_poly* b, uint64_t out[4]) {
   SP_TRY(ctx)
   if (a->len != b->len) throw SpError(SP_ERR_INVALID_ARG, "dot: length mismatch");
-  dev::dot(ctx->c.small.p + 32, a->d.p, b->d.p, a->len, ctx->c.red.p, ctx->c.stream);
+  dev::dot(ctx->c.small.p + layout::SMALL_DOT.off, a->d.p, b->d.p, a->len, ctx->c.red.p, ctx->c.stream);
   Fq v;
-  ctx->c.get_small(32, &v, 1);
+  ctx->c.get_small(layout::SMALL_DOT.off, &v, 1);
   fq_out(out, v);
   SP_CATCH(ctx)
 }

@@ -54,6 +54,7 @@ struct ScInst {        // one sumcheck instance: up to four tables of the same c
   u256* c_out;         // where the folded C goes (== t[2] for private C; a ping-pong buffer when C is shared)
   int write_c;         // 1: this instance stores the folded C
 };
+constexpr int SC_MAX_INST = 24;   // instances of one batched launch: sc_eval and its siblings refuse more
 // Optional host notification of a reduction kernel: results are also stored to `host_out` (mapped pinned memory) and `seq` is then
 // published in `*flag`; `done` is a zero-initialised device counter (instances of a batched launch finish independently).
 struct HostSig {
@@ -69,9 +70,10 @@ struct HostSig {
 // All ranks execute the same sequence of collectives, so a sequence number identifies an operation on every rank.
 #define SP_MAX_RANKS 8
 #define SP_XR_SLOTS 4
-#define SP_XR_CAP 80                                   // u256 per (slot, source): 24 instances x 3 evaluations fit
+#define SP_XR_CAP 80                                   // u256 per (slot, source): a full batch's 3 evaluations per instance fit
 #define SP_WIN_CTRL_BYTES ((size_t)1 << 20)
 #define SP_WIN_HALF_BYTES ((size_t)96 << 20)
+static_assert(SP_XR_CAP >= 3 * SC_MAX_INST, "SP_XR_CAP: a mailbox must hold the 3 evaluations of each of SC_MAX_INST instances");
 struct WinCtrl {                                        // at offset 0 of every window
   unsigned int xflag[SP_MAX_RANKS];                     // [source]: sequence number of the last partial-sum message from `source`
   unsigned int bflag[SP_MAX_RANKS];                     // [source]: sequence number of the last bulk all-gather contribution from `source`

@@ -59,6 +59,64 @@ struct Comm {
   size_t next_half_off() { ++bseq; return SP_WIN_CTRL_BYTES + (size_t)(bseq & 1) * SP_WIN_HALF_BYTES; }
 };
 
+// Layout of the context's fixed scratch buffers: Ctx::small, Ctx::pinned (host_res and the flag words lie inside it) and Ctx::sig_done.  A region
+// is an offset and a capacity in its buffer's unit, and this is the one place to add one: the asserts keep the regions of a buffer apart and
+// inside it, and every capacity at the worst case its users reach.  Regions marked "shared" serve several users on purpose: those all run on the
+// prover's stream and each reads its result back before the next is enqueued, so no two of them are ever in flight together.
+namespace layout {
+struct Region { size_t off, cap; constexpr size_t end() const { return off + cap; } };
+// Ctx::small (device memory), in scalars
+constexpr size_t SMALL_SCALARS = 4096;
+constexpr Region SMALL_ROUND{0, 8};      // shared: a sumcheck round's evaluations, 3 of one instance (ZK sumcheck, sp_sumcheck_*) or one per degree (poly_sumcheck_prove)
+constexpr Region SMALL_HEADS{8, 8};      // the final table heads of poly_sumcheck_prove
+constexpr Region SMALL_IPA_C{16, 16};    // c_L, c_R of an inner-product round
+constexpr Region SMALL_DOT{32, 8};       // shared: one dot product (r1cs_prove, sp_dot, sp_poly_evaluate)
+constexpr Region SMALL_ABC{40, 8};       // A, B, C at (rx, ry) (instance_evaluate)
+constexpr Region SMALL_DOTP{48, 16};     // the two halves of a dot-product circuit's claim (snark_prove)
+constexpr Region SMALL_BATCH{64, 128};   // shared: batched_prove's 3 evaluations per instance; after it, snark_prove's 21 + 2 hash-layer evaluations
+constexpr Region SMALL_ONES{4000, 2};    // Ctx::ones()
+// Ctx::pinned (mapped host memory), in bytes
+constexpr size_t PINNED_BYTES = 1 << 20;
+constexpr size_t PIN_XY_PART = 4096;
+constexpr Region PIN_STAGE{0, 4096};                // shared: small copies to the host, each synchronised and read at once (get_small, a_hat | b_hat, the ZK sumcheck's
+                                                    // final table heads, the two last-layer entries of each of batched_prove's product circuits)
+constexpr Region PIN_ZKPRE{384 << 10, 96 << 10};    // ZkPre's encodings and points, read when its sumcheck starts
+constexpr Region PIN_RES{512 << 10, 256 << 10};     // Ctx::host_res: what kernels publish through dev::HostSig (the RES_ regions)
+constexpr Region PIN_FLAG{768 << 10, 64};           // Ctx::host_flag: the flag word of next_sig(), on a cache line of its own
+constexpr Region PIN_FLAG_C{PIN_FLAG.end(), 64};    // Ctx::host_flag_c: the second flag word of an inner-product round, likewise
+constexpr Region PIN_XY{960 << 10, 2 * PIN_XY_PART};   // snark_prove's equalized rx | ry, read by the background stream: PIN_XY_PART bytes each
+// Ctx::host_res, in scalars
+constexpr Region RES_OUT{0, 512};        // shared by the users of next_sig(): a sumcheck round's evaluations (3 per instance, batched_prove's 6 bound entries per
+                                         // instance behind them) and the values of dev::heads
+constexpr Region RES_IPA_C{0, 2};        // c_L, c_R of an inner-product round; inside RES_OUT, like RES_POINTS: no sumcheck runs during an inner-product argument
+constexpr Region RES_POINTS{8, 8};       // shared: L', R' of an inner-product round, in flight together with RES_IPA_C, and RowSum's one or two points
+// Ctx::sig_done (device memory), in words
+constexpr size_t SIG_WORDS = 4;
+constexpr Region SIG_DONE{0, 1};         // completion counter of next_sig()
+constexpr Region SIG_MSM_TICKET{1, 1};   // block ticket of dev::ipa_msm
+constexpr Region SIG_DONE_C{2, 1};       // completion counter of the second flag word
+
+#define SP_APART(a, b) static_assert(a.end() <= b.off, #a " runs into " #b)
+#define SP_HOLDS(a, n) static_assert(size_t(n) <= a.cap, #a " cannot hold " #n)
+SP_APART(SMALL_ROUND, SMALL_HEADS); SP_APART(SMALL_HEADS, SMALL_IPA_C); SP_APART(SMALL_IPA_C, SMALL_DOT); SP_APART(SMALL_DOT, SMALL_ABC);
+SP_APART(SMALL_ABC, SMALL_DOTP); SP_APART(SMALL_DOTP, SMALL_BATCH); SP_APART(SMALL_BATCH, SMALL_ONES);
+static_assert(SMALL_ONES.end() <= SMALL_SCALARS, "SMALL_ONES ends outside Ctx::small");
+SP_HOLDS(SMALL_ROUND, 3); SP_HOLDS(SMALL_ROUND, SP_SC_MAX_DEGREE); SP_HOLDS(SMALL_HEADS, SP_SC_MAX_TABLES); SP_HOLDS(SMALL_IPA_C, 2); SP_HOLDS(SMALL_DOT, 1);
+SP_HOLDS(SMALL_ABC, 3); SP_HOLDS(SMALL_DOTP, 2); SP_HOLDS(SMALL_BATCH, 3 * dev::SC_MAX_INST); SP_HOLDS(SMALL_BATCH, 21 + 2); SP_HOLDS(SMALL_ONES, 2);
+SP_APART(PIN_STAGE, PIN_ZKPRE); SP_APART(PIN_ZKPRE, PIN_RES); SP_APART(PIN_RES, PIN_FLAG); SP_APART(PIN_FLAG, PIN_FLAG_C); SP_APART(PIN_FLAG_C, PIN_XY);
+static_assert(PIN_XY.end() <= PINNED_BYTES, "PIN_XY ends outside Ctx::pinned");
+SP_HOLDS(PIN_STAGE, SMALL_BATCH.cap * sizeof(u256));   // get_small of any whole region of Ctx::small
+SP_HOLDS(PIN_STAGE, 2 * sizeof(u256) * dev::SC_MAX_INST); SP_HOLDS(PIN_STAGE, 4 * sizeof(u256));   // batched_prove's entries; a ZK sumcheck's 4 tables
+SP_HOLDS(PIN_RES, RES_OUT.end() * sizeof(u256));
+SP_APART(RES_IPA_C, RES_POINTS);
+static_assert(RES_POINTS.end() <= RES_OUT.end(), "RES_POINTS ends outside RES_OUT");
+SP_HOLDS(RES_OUT, (3 + 6) * dev::SC_MAX_INST); SP_HOLDS(RES_OUT, 64 /* dev::heads refuses more tables */); SP_HOLDS(RES_POINTS, 2 * sizeof(ge) / sizeof(u256));
+SP_APART(SIG_DONE, SIG_MSM_TICKET); SP_APART(SIG_MSM_TICKET, SIG_DONE_C);
+static_assert(SIG_DONE_C.end() <= SIG_WORDS, "SIG_DONE_C ends outside Ctx::sig_done");
+#undef SP_APART
+#undef SP_HOLDS
+}  // namespace layout
+
 struct Ctx {
   int device = 0;
   std::unique_ptr<Comm> comm;          // null: single-GPU context
@@ -85,12 +143,11 @@ struct Ctx {
   bool overlap = true;                 // sp_ctx_set_overlap: 0 keeps every kernel on the prover's stream (profiling: per-kernel event times free of concurrent work)
   void* ev_fork = nullptr; void* ev_join = nullptr;
   DevBuf<uint8_t> scratch2;        // MSM partial sums of the background stream
-  uint8_t* pinned = nullptr;       // staging for small host<->device exchanges
-  size_t pinned_bytes = 0;
+  uint8_t* pinned = nullptr;       // small host<->device exchanges (layout::PIN_*)
   DevBuf<uint8_t> scratch;         // MSM partial sums (growable)
   DevBuf<uint8_t> red;             // reduction tickets + per-block partials (fixed size, tickets zeroed once and self-resetting)
-  DevBuf<u256> small;              // challenges, results (device side); [4000, 4002) = two Montgomery ones
-  const u256* ones() const { return small.p + 4000; }
+  DevBuf<u256> small;              // challenges, results (device side: layout::SMALL_*)
+  const u256* ones() const { return small.p + layout::SMALL_ONES.off; }   // two Montgomery ones
   std::string last_error;
   // per-phase timers (profile feature of the reference, src/timer.rs): label -> milliseconds of the last prove
   std::vector<std::pair<std::string, double>> timings;
@@ -102,16 +159,17 @@ struct Ctx {
   // host-polled kernel results (mapped pinned memory): see dev::HostSig
   u256* host_res = nullptr;
   unsigned int* host_flag = nullptr;
+  unsigned int* host_flag_c = nullptr;   // second flag word: the dot products fused into the inner-product MSM launch
   DevBuf<unsigned int> sig_done;
   unsigned int sig_seq = 0;
-  unsigned int sigc_seq = 0;           // sequence of the second flag word (host_flag + 16)
-  dev::HostSig next_sig() { dev::HostSig s; s.host_out = host_res; s.flag = host_flag; s.done = sig_done.p; s.seq = ++sig_seq; return s; }
+  unsigned int sigc_seq = 0;           // sequence of the second flag word
+  dev::HostSig next_sig() {
+    dev::HostSig s; s.host_out = host_res + layout::RES_OUT.off; s.flag = host_flag; s.done = sig_done.p + layout::SIG_DONE.off; s.seq = ++sig_seq; return s;
+  }
   void wait_sig(const dev::HostSig& s);   // spins on the flag; falls back to a stream synchronise to surface CUDA errors
   void sync() { dev::stream_sync(stream); }
   void ensure_scratch(size_t bytes) { if (scratch.n < bytes) { sync(); scratch.alloc(bytes); } }
-  // upload k scalars to small[slot..]
-  void put_small(size_t slot, const Fq* v, size_t k);
-  void get_small(size_t slot, Fq* v, size_t k);  // synchronises
+  void get_small(size_t slot, Fq* v, size_t k);  // download k scalars from small[slot..]; synchronises
   void upload(u256* d, const Fq* h, size_t n);
   std::vector<Fq> download(const u256* d, size_t n);
 };
@@ -153,7 +211,6 @@ struct GenSet {
   int wbits = 8;               // window width of `table` (host copies are always 8-bit)
   DevBuf<ge_niels> row_table;  // d * G_j for the row MSM of large sets (dev::build_row_table); empty for small sets
   const ge_niels* rows() const { return row_table.n ? row_table.p : nullptr; }
-  std::vector<Cp> compressed;  // lazily filled export
   GenSet(Ctx* c, const std::string& label, size_t nbases, const std::vector<size_t>& host_bases);
   GenSet(Ctx* c, const ge* d_points, size_t nbases, const std::vector<size_t>& host_bases);   // caller-supplied generators (device array)
   void finish(const std::vector<size_t>& host_bases);   // window tables + host copies, once G is filled
@@ -166,7 +223,6 @@ struct GenSet {
     return it->second;
   }
   bool has_tab(size_t base) const { std::lock_guard<std::mutex> lk(host_mu); return host_tab.count(base) != 0; }
-  hge host_point(size_t base) const;  // 1 * G_base from the host table
   size_t device_bytes() const { return G.n * sizeof(ge) + (table.n + row_table.n) * sizeof(ge_niels); }
  private:
   std::map<size_t, HostBaseTable> host_tab;
@@ -194,6 +250,5 @@ struct CommitKey {
 struct Term { size_t base; Fq k; };
 // sum of k_i * G_{base_i} over host tables
 hge host_commit(const GenSet& gs, const Term* terms, size_t nterms);
-inline Cp host_commit_c(const GenSet& gs, const std::vector<Term>& t) { return compress(host_commit(gs, t.data(), t.size())); }
 
 }  // namespace sp

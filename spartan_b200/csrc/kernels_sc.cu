@@ -5,8 +5,7 @@ namespace sp {
 namespace dev {
 
 // =============================================================================================== sumcheck rounds
-#define SC_MAX_INST 24
-struct ScBatch {
+struct ScBatch {   // a kernel parameter: SC_MAX_INST (dev.hpp) instances
   ScInst inst[SC_MAX_INST];
 };
 

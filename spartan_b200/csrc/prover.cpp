@@ -35,18 +35,18 @@ Ctx::Ctx(int dev_) : device(dev_) {
   stream = dev::stream_create_prio(+1);
   stream2 = dev::stream_create_prio(-1);
   ev_fork = dev::event_create(); ev_join = dev::event_create();
-  pinned_bytes = 1 << 20;
-  pinned = (uint8_t*)dev::hmalloc_pinned(pinned_bytes);
-  host_res = reinterpret_cast<u256*>(pinned + (512 << 10));
-  host_flag = reinterpret_cast<unsigned int*>(pinned + (768 << 10));
+  pinned = (uint8_t*)dev::hmalloc_pinned(layout::PINNED_BYTES);
+  host_res = reinterpret_cast<u256*>(pinned + layout::PIN_RES.off);
+  host_flag = reinterpret_cast<unsigned int*>(pinned + layout::PIN_FLAG.off);
+  host_flag_c = reinterpret_cast<unsigned int*>(pinned + layout::PIN_FLAG_C.off);
   *host_flag = 0;
-  host_flag[16] = 0;   // second flag word (its own cache line): the dot products fused into the inner-product MSM launch
-  sig_done.alloc(4);
-  dev::dzero(sig_done.p, 16, stream);
-  small.alloc(4096);
-  dev::fill_one(small.p + 4000, 2, stream);   // ones(): two Montgomery ones
+  *host_flag_c = 0;
+  sig_done.alloc(layout::SIG_WORDS);
+  dev::dzero(sig_done.p, layout::SIG_WORDS * sizeof(unsigned int), stream);
+  small.alloc(layout::SMALL_SCALARS);
+  dev::fill_one(small.p + layout::SMALL_ONES.off, layout::SMALL_ONES.cap, stream);   // ones()
   scratch.alloc(1 << 20);
-  red.alloc(dev::sc_scratch_bytes(24));
+  red.alloc(dev::sc_scratch_bytes(dev::SC_MAX_INST));
   dev::dzero(red.p, red.n, stream);
   sync();
 }
@@ -117,14 +117,11 @@ u256* Ctx::allgather_cyclic(const u256* const* tables, int ntables, size_t n_loc
   return reinterpret_cast<u256*>(c.win[c.rank] + off);
 }
 
-void Ctx::put_small(size_t slot, const Fq* v, size_t k) {
-  // staged through pageable memory on purpose: cudaMemcpyAsync from pageable memory snapshots the source before returning
-  dev::h2d(small.p + slot, v, k * sizeof(u256), stream);
-}
 void Ctx::get_small(size_t slot, Fq* v, size_t k) {
-  dev::d2h(pinned, small.p + slot, k * sizeof(u256), stream);
+  uint8_t* stage = pinned + layout::PIN_STAGE.off;
+  dev::d2h(stage, small.p + slot, k * sizeof(u256), stream);
   sync();
-  memcpy(v, pinned, k * sizeof(u256));
+  memcpy(v, stage, k * sizeof(u256));
 }
 void Ctx::upload(u256* d, const Fq* h, size_t n) { dev::h2d(d, h, n * sizeof(u256), stream); sync(); }
 std::vector<Fq> Ctx::download(const u256* d, size_t n) {
@@ -203,10 +200,6 @@ void GenSet::add_host_tables(const std::vector<size_t>& bases) {
     std::lock_guard<std::mutex> lk(host_mu);
     host_tab.emplace(hb[i], std::move(t));   // a concurrent view may have added the same base: its copy is the same table
   }
-}
-hge GenSet::host_point(size_t base) const {
-  hge acc = hge_identity();
-  return hge_madd(acc, tab(base).e[0], false);
 }
 hge host_commit(const GenSet& gs, const Term* terms, size_t nterms) {
   hge acc = hge_identity();
@@ -406,21 +399,21 @@ void ScRounds::fold(const Fq& r) {
 std::vector<Fq> ScRounds::wait() {
   ctx.wait_sig(sig);
   std::vector<Fq> ev(3 * insts.size());
-  memcpy(static_cast<void*>(ev.data()), ctx.host_res, ev.size() * sizeof(u256));
+  memcpy(static_cast<void*>(ev.data()), ctx.host_res + layout::RES_OUT.off, ev.size() * sizeof(u256));
   return ev;
 }
 
 void poly_sumcheck_prove(Ctx& ctx, const dev::ScPoly& P, size_t len, const Fq& claim, size_t num_rounds, Transcript& T, SumcheckInstanceProof& proof,
                          std::vector<Fq>& r, std::vector<Fq>& finals, Fq& e) {
   const size_t d = (size_t)P.degree;
-  u256* d_out = ctx.small.p + 0;   // the d evaluations of a round
+  u256* d_out = ctx.small.p + layout::SMALL_ROUND.off;   // the d evaluations of a round
   dev::HostSig sig = ctx.next_sig();
   dev::scp_eval(P, len, d_out, ctx.red.p, ctx.stream, sig);
   e = claim;
   for (size_t j = 0; j < num_rounds; j++) {
     ctx.wait_sig(sig);
     std::vector<Fq> ev(d);
-    memcpy(static_cast<void*>(ev.data()), ctx.host_res, d * sizeof(u256));
+    memcpy(static_cast<void*>(ev.data()), ctx.host_res + layout::RES_OUT.off, d * sizeof(u256));
     std::vector<Fq> evals(d + 1);   // s_j(0), s_j(1) = e - s_j(0), s_j(2) .. s_j(d)
     evals[0] = ev[0];
     evals[1] = e - ev[0];
@@ -440,10 +433,10 @@ void poly_sumcheck_prove(Ctx& ctx, const dev::ScPoly& P, size_t len, const Fq& c
     r.push_back(r_j);
   }
   sig = ctx.next_sig();
-  dev::heads(ctx.small.p + 8, P.t, P.ntables, ctx.stream, sig);
+  dev::heads(ctx.small.p + layout::SMALL_HEADS.off, P.t, P.ntables, ctx.stream, sig);
   ctx.wait_sig(sig);
   finals.resize(P.ntables);
-  memcpy(static_cast<void*>(finals.data()), ctx.host_res, P.ntables * sizeof(u256));
+  memcpy(static_cast<void*>(finals.data()), ctx.host_res + layout::RES_OUT.off, P.ntables * sizeof(u256));
 }
 
 // ================================================================================================ ZK sumcheck on the device
@@ -478,8 +471,8 @@ struct ZkPre {
       rdel[j] = pre[j].r_delta; rbet[j] = pre[j].r_beta;
     }
     const size_t stage_bytes = num_rounds * (32 + 3 * sizeof(ge));
-    if (stage_bytes > (96u << 10)) throw std::runtime_error("spartan_b200: ZK sumcheck with too many rounds for the staging area");
-    stage = ctx.pinned + (384 << 10);
+    if (stage_bytes > layout::PIN_ZKPRE.cap) throw std::runtime_error("spartan_b200: ZK sumcheck with too many rounds for the staging area");
+    stage = ctx.pinned + layout::PIN_ZKPRE.off;
     d_s.alloc(num_rounds * nco); d_b.alloc(4 * num_rounds); d_pts.alloc(4 * num_rounds); d_c.alloc(32 * num_rounds);
     // pageable sources: the copies snapshot them before returning
     dev::h2d(d_s.p, dmat.data(), dmat.size() * sizeof(u256), ctx.stream);
@@ -541,7 +534,7 @@ static void zk_sumcheck_prove(Ctx& ctx, dev::ScKind kind, const Fq& claim, const
   for (int t = 0; t < 4; t++) inst.t[t] = t < nt ? tables[t] : nullptr;
   inst.c_out = inst.t[2];
   inst.write_c = 1;
-  ScRounds sc{ctx, kind, {inst}, ((size_t)1 << num_rounds) / W, sh, ctx.small.p + 0};
+  ScRounds sc{ctx, kind, {inst}, ((size_t)1 << num_rounds) / W, sh, ctx.small.p + layout::SMALL_ROUND.off};
   sc.eval();
   for (size_t j = 0; j < num_rounds; j++) {
     FineTimer fw(ctx, "zk wait evals");
@@ -581,9 +574,10 @@ static void zk_sumcheck_prove(Ctx& ctx, dev::ScKind kind, const Fq& claim, const
     proof.comm_evals.push_back(comm_claim_per_round);
   }
   finals.resize(nt);
-  for (int t = 0; t < nt; t++) dev::d2h(ctx.pinned + 32 * t, sc.insts[0].t[t], 32, ctx.stream);   // the replicated copies after a shard exit
+  uint8_t* stage = ctx.pinned + layout::PIN_STAGE.off;
+  for (int t = 0; t < nt; t++) dev::d2h(stage + 32 * t, sc.insts[0].t[t], 32, ctx.stream);   // the replicated copies after a shard exit
   ctx.sync();
-  memcpy(finals.data(), ctx.pinned, 32 * nt);
+  memcpy(finals.data(), stage, 32 * nt);
   blind_post = blinds_evals[num_rounds - 1];
 }
 
@@ -638,41 +632,44 @@ void append_poly_commitment(Transcript& T, const char* label, const PolyCommitme
 }
 
 void IpaRound::launch(size_t cur) {
-  // the dot products ride in the MSM's launch (two extra blocks with their own flag word, host_flag + 16, and completion counter)
-  sig_c.host_out = ctx.host_res; sig_c.flag = ctx.host_flag + 16; sig_c.done = ctx.sig_done.p + 2; sig_c.seq = ++ctx.sigc_seq;
+  // the dot products ride in the MSM's launch (two extra blocks with their own flag word, host_flag_c, and completion counter)
+  sig_c.host_out = ctx.host_res + layout::RES_IPA_C.off; sig_c.flag = ctx.host_flag_c; sig_c.done = ctx.sig_done.p + layout::SIG_DONE_C.off; sig_c.seq = ++ctx.sigc_seq;
   sig_lr = ctx.next_sig();
-  sig_lr.host_out = ctx.host_res + 8;
-  dev::ipa_msm(pts, gs.table.p, gs.wbits, a, svec, cur, n, ctx.scratch.p, ctx.sig_done.p + 1, ctx.stream, sig_lr, b, ctx.small.p + 16, sig_c);
+  sig_lr.host_out = ctx.host_res + layout::RES_POINTS.off;
+  dev::ipa_msm(pts, gs.table.p, gs.wbits, a, svec, cur, n, ctx.scratch.p, ctx.sig_done.p + layout::SIG_MSM_TICKET.off, ctx.stream, sig_lr, b,
+               ctx.small.p + layout::SMALL_IPA_C.off, sig_c);
 }
 void IpaRound::wait_c(Fq& c_L, Fq& c_R) {
   ctx.wait_sig(sig_c);
-  memcpy(&c_L, ctx.host_res, 32); memcpy(&c_R, ctx.host_res + 1, 32);
+  const u256* c = ctx.host_res + layout::RES_IPA_C.off;
+  memcpy(&c_L, c, 32); memcpy(&c_R, c + 1, 32);
 }
 void IpaRound::wait_LR(ge& L, ge& R) {
   ctx.wait_sig(sig_lr);
-  memcpy(&L, ctx.host_res + 8, sizeof(ge)); memcpy(&R, ctx.host_res + 12, sizeof(ge));
+  const ge* lr = reinterpret_cast<const ge*>(ctx.host_res + layout::RES_POINTS.off);
+  memcpy(&L, lr, sizeof(ge)); memcpy(&R, lr + 1, sizeof(ge));
 }
 void IpaRound::fold(size_t cur, const Fq& u, const Fq& u_inv) { dev::ipa_fold_update(a, b, svec, cur / 2, n, u.m, u_inv.m, ctx.stream); }
 
 RowSum::RowSum(Ctx& c, const GenSet& gs, const u256* d_x, size_t n_) : ctx(c), n(n_), pts(2) {
   if (n >= 2) {
     sig = ctx.next_sig();
-    sig.host_out = ctx.host_res + 8;
-    dev::ipa_msm(pts.p, gs.table.p, gs.wbits, ctx.ones(), d_x, 2, n, ctx.scratch.p, ctx.sig_done.p + 1, ctx.stream, sig);
+    sig.host_out = ctx.host_res + layout::RES_POINTS.off;
+    dev::ipa_msm(pts.p, gs.table.p, gs.wbits, ctx.ones(), d_x, 2, n, ctx.scratch.p, ctx.sig_done.p + layout::SIG_MSM_TICKET.off, ctx.stream, sig);
   } else {
     dev::msm_rows(pts.p, gs.table.p, gs.wbits, gs.rows(), d_x, n, 1, n, nullptr, 0, ctx.scratch.p, ctx.stream);
-    dev::d2h(ctx.host_res + 8, pts.p, sizeof(ge), ctx.stream);
+    dev::d2h(ctx.host_res + layout::RES_POINTS.off, pts.p, sizeof(ge), ctx.stream);
   }
 }
 hge RowSum::collect() {
   ge p[2];
   if (n < 2) {
     ctx.sync();
-    memcpy(&p[0], ctx.host_res + 8, sizeof(ge));
+    memcpy(&p[0], ctx.host_res + layout::RES_POINTS.off, sizeof(ge));
     return to_hge(p[0]);
   }
   ctx.wait_sig(sig);
-  memcpy(p, ctx.host_res + 8, 2 * sizeof(ge));
+  memcpy(p, ctx.host_res + layout::RES_POINTS.off, 2 * sizeof(ge));
   return hge_add(to_hge(p[0]), to_hge(p[1]));
 }
 
@@ -739,11 +736,12 @@ static void bullet_prove(Ctx& ctx, Transcript& T, const PolyCommitmentGens& gens
   if (k == 0) r_scale = get_r_scale();
   // g_hat = G_final[0] = <s, G>
   FineTimer f6(ctx, "ipa final");
-  dev::d2h(ctx.pinned, d_a, 32, ctx.stream);
-  dev::d2h(ctx.pinned + 32, d_b, 32, ctx.stream);
+  uint8_t* stage = ctx.pinned + layout::PIN_STAGE.off;
+  dev::d2h(stage, d_a, 32, ctx.stream);
+  dev::d2h(stage + 32, d_b, 32, ctx.stream);
   g_hat = RowSum(ctx, gs, svec.p, n).collect();
   ctx.sync();   // a_hat, b_hat
-  memcpy(&a_hat, ctx.pinned, 32); memcpy(&b_hat, ctx.pinned + 32, 32);
+  memcpy(&a_hat, stage, 32); memcpy(&b_hat, stage + 32, 32);
 }
 
 // DotProductProofLog::prove (nizk/mod.rs:440-525).  d_x: device x_vec (n, consumed); a_vec on the host (it is absorbed by the transcript).
@@ -988,9 +986,9 @@ void r1cs_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::v
     DevBuf<u256> d_eq(num_vars);
     dev::h2d(d_chal.p, ry1.data(), ry1.size() * sizeof(u256), ctx.stream);
     dev::eq_evals(d_eq.p, d_chal.p, (int)ry1.size(), eq_small.p, ctx.stream);
-    dev::dot(ctx.small.p + 32, d_vars, d_eq.p, num_vars, ctx.red.p, ctx.stream);
+    dev::dot(ctx.small.p + layout::SMALL_DOT.off, d_vars, d_eq.p, num_vars, ctx.red.p, ctx.stream);
     Fq eval_vars_at_ry;
-    ctx.get_small(32, &eval_vars_at_ry, 1);
+    ctx.get_small(layout::SMALL_DOT.off, &eval_vars_at_ry, 1);
     Fq blind_eval = tape.random_scalar("blind_eval");
     polyeval_prove(ctx, d_vars, &blinds_vars, ry1, eval_vars_at_ry, &blind_eval, gens.gens_pc, T, tape, proof.proof_eval_vars_at_ry, proof.comm_vars_at_ry);
     Fq blind_eval_Z_at_ry = (Fq::one() - ry[0]) * blind_eval;

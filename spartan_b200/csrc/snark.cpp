@@ -172,11 +172,14 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
                           std::vector<Fq>& rand_out) {
   const size_t np = prods.size(), nd = dotps.size();
   const size_t num_layers = prods[0]->num_layers;
+  // the limit of one launch, which the layout's capacities for the evaluations, the bound entries and the staged last-layer entries rest on
+  if (np + nd > (size_t)dev::SC_MAX_INST) throw SpError(SP_ERR_INTERNAL, "batched product proof of more than " + std::to_string(dev::SC_MAX_INST) + " instances");
   std::vector<Fq> claims_to_verify(np);
   {  // all evaluate()s with one sync
-    for (size_t i = 0; i < np; i++) dev::d2h(ctx.pinned + 64 * i, prods[i]->layer(num_layers - 1), 64, ctx.stream);
+    uint8_t* stage = ctx.pinned + layout::PIN_STAGE.off;
+    for (size_t i = 0; i < np; i++) dev::d2h(stage + 64 * i, prods[i]->layer(num_layers - 1), 64, ctx.stream);
     ctx.sync();
-    for (size_t i = 0; i < np; i++) { Fq v[2]; memcpy(v, ctx.pinned + 64 * i, 64); claims_to_verify[i] = v[0] * v[1]; }
+    for (size_t i = 0; i < np; i++) { Fq v[2]; memcpy(v, stage + 64 * i, 64); claims_to_verify[i] = v[0] * v[1]; }
   }
   const int W = prods[0]->W, rk = ctx.rank();
   const size_t Ks = prods[0]->Ks;
@@ -186,7 +189,8 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
   DevBuf<u256> cpar0(std::max<size_t>(max_half, 1));
   std::vector<Fq> rand;
   const size_t G_MIN = 2 * Ctx::SHARD_MIN_LOCAL;   // 16384 entries per table: the fused G kernel then always streams >= 32768
-  u256* d_out = ctx.small.p + 64;   // ninst * 3 scalars
+  u256* d_out = ctx.small.p + layout::SMALL_BATCH.off;   // ninst * 3 scalars
+  u256* const h_out = ctx.host_res + layout::RES_OUT.off;   // where they reach the host
   DevBuf<u256> d_heads(64);
   const int logW = (int)log2_ceil(W);
   // a layer's sumcheck runs on tables of half = len/2 entries (num_rounds variables), lhalf of them on this rank while the layer is sharded
@@ -269,7 +273,7 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
       else dev::sc_fold_eval_g(sc.insts.data(), (int)np, sc.len, r->m, Elev[j], d_out, ctx.red.p, ctx.stream, sc.sig, sc.xr());
       if (ndi) {
         sc.sig = ctx.next_sig();
-        sc.sig.host_out = ctx.host_res + 3 * np;
+        sc.sig.host_out = h_out + 3 * np;
         if (!r) dev::sc_eval(dev::SC_CUBIC3, sc.insts.data() + np, (int)ndi, sc.len, d_out + 3 * np, ctx.red.p, ctx.stream, sc.sig, sc.xr());
         else dev::sc_fold_eval(dev::SC_CUBIC3, sc.insts.data() + np, (int)ndi, sc.len, r->m, d_out + 3 * np, ctx.red.p, ctx.stream, sc.sig, sc.xr());
       }
@@ -341,7 +345,7 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
         sc.eval();
       } else if (j + 1 < num_rounds) {
         bound_on_host = j + 2 == num_rounds;
-        sc.fold_eval(r_j, bound_on_host ? ctx.host_res + 3 * ninst : nullptr);
+        sc.fold_eval(r_j, bound_on_host ? h_out + 3 * ninst : nullptr);
         // the product instances now read the shared C where instance 0 folded it, so the next fold writes it into the other ping-pong half;
         // after the shard exit they read its gathered copy instead and both halves are free
         for (size_t i = 0; i < np; i++)
@@ -364,7 +368,7 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
     std::vector<Fq> heads(3 * ninst);
     if (bound_on_host) {   // a0 + r (a1 - a0): what the fold computes (fq_fold_const), on the two entries the last launch published
       std::vector<Fq> bound(6 * ninst);
-      memcpy(bound.data(), ctx.host_res + 3 * ninst, 6 * ninst * sizeof(u256));
+      memcpy(bound.data(), h_out + 3 * ninst, 6 * ninst * sizeof(u256));
       const Fq& r = rand_prod.back();
       for (size_t k = 0; k < 3 * ninst; k++) heads[k] = bound[2 * k] + r * (bound[2 * k + 1] - bound[2 * k]);
       if (layer_id > 0) build_eq(shape_of(layer_id - 1), rand_prod);
@@ -375,7 +379,7 @@ static void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vecto
       dev::heads(d_heads.p, hp.data(), (int)hp.size(), ctx.stream, hs);
       if (layer_id > 0) build_eq(shape_of(layer_id - 1), rand_prod);
       ctx.wait_sig(hs);
-      memcpy(heads.data(), ctx.host_res, 3 * ninst * sizeof(u256));
+      memcpy(heads.data(), h_out, 3 * ninst * sizeof(u256));
     }
     lp.claims_prod_left.resize(np); lp.claims_prod_right.resize(np);
     for (size_t i = 0; i < np; i++) { lp.claims_prod_left[i] = heads[3 * i]; lp.claims_prod_right[i] = heads[3 * i + 1]; }
@@ -476,8 +480,8 @@ void instance_evaluate(Ctx& ctx, const Instance& inst, const std::vector<Fq>& rx
   dev::h2d(d_chal.p + rx.size(), ry.data(), ry.size() * sizeof(u256), ctx.stream);
   dev::eq_evals(try_.p, d_chal.p + rx.size(), (int)ry.size(), eq_small.p, ctx.stream);
   for (int m = 0; m < 3; m++)
-    dev::sparse_eval3(ctx.small.p + 40 + m, inst.M[m].coo_row.p, inst.M[m].coo_col.p, inst.M[m].coo_val.p, inst.M[m].nnz, trx.p, try_.p, ctx.red.p, ctx.stream);
-  ctx.get_small(40, out, 3);
+    dev::sparse_eval3(ctx.small.p + layout::SMALL_ABC.off + m, inst.M[m].coo_row.p, inst.M[m].coo_col.p, inst.M[m].coo_val.p, inst.M[m].nnz, trx.p, try_.p, ctx.red.p, ctx.stream);
+  ctx.get_small(layout::SMALL_ABC.off, out, 3);
 }
 
 // ================================================================================================ SNARK::prove
@@ -526,13 +530,14 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
   // (DESIGN.md §3 has the H100 A/B)
   const size_t early_smem_pad = 60 << 10;
   if (early) {
+    if (nxy * sizeof(u256) > layout::PIN_XY_PART) throw SpError(SP_ERR_INVALID_ARG, "instance with too many variables for the staged evaluation points");
     d_chal2.alloc(64); eq_small2.alloc(eq_small.n); early_rows.alloc(2 * cnt); early_comp.alloc(64 * cnt);
     const size_t need = dev::msm_scratch_bytes(cnt, R_d) + 64;
     if (ctx.scratch2.n < need) { dev::stream_sync(ctx.stream2); ctx.scratch2.alloc(need); }
   }
   auto early_part = [&](int part, const std::vector<Fq>& pt) {   // part 0: rows from rx, part 1: columns from ry
     // equalize (sparse_mlpoly.rs:1429-1445): left-pad the shorter point with zeros; staged in pinned memory so that the copy never waits for the stream
-    Fq* ext = reinterpret_cast<Fq*>(ctx.pinned + (960 << 10) + (size_t)part * 4096);
+    Fq* ext = reinterpret_cast<Fq*>(ctx.pinned + layout::PIN_XY.off + (size_t)part * layout::PIN_XY_PART);
     for (size_t i = 0; i < nxy - pt.size(); i++) ext[i] = Fq::zero();
     for (size_t i = 0; i < pt.size(); i++) ext[nxy - pt.size() + i] = pt[i];
     dev::event_record(ctx.ev_fork, ctx.stream);
@@ -654,7 +659,7 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
     dev::heads(d_roots.p, hp.data(), (int)hp.size(), ctx.stream, hs);
     ctx.wait_sig(hs);
     Fq v[32];
-    memcpy(v, ctx.host_res, sizeof v);
+    memcpy(v, ctx.host_res + layout::RES_OUT.off, sizeof v);
     for (int side = 0; side < 2; side++) for (int c = 0; c < 8; c++) roots[side][c] = v[16 * side + 2 * c] * v[16 * side + 2 * c + 1];
   }
   const Fq* rr = roots[0];
@@ -670,10 +675,11 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
   std::vector<DotpCircuit> dotps;
   for (int m = 0; m < 3; m++) {
     const u256* srcs[3] = {row_val[m], col_val[m], dv.val[m]};
-    dev::dot3(ctx.small.p + 48, srcs[0], srcs[1], srcs[2], hN, ctx.red.p, ctx.stream);
-    dev::dot3(ctx.small.p + 49, srcs[0] + hN, srcs[1] + hN, srcs[2] + hN, hN, ctx.red.p, ctx.stream);
+    u256* d_lr2 = ctx.small.p + layout::SMALL_DOTP.off;
+    dev::dot3(d_lr2, srcs[0], srcs[1], srcs[2], hN, ctx.red.p, ctx.stream);
+    dev::dot3(d_lr2 + 1, srcs[0] + hN, srcs[1] + hN, srcs[2] + hN, hN, ctx.red.p, ctx.stream);
     Fq lr2[2];
-    ctx.get_small(48, lr2, 2);
+    ctx.get_small(layout::SMALL_DOTP.off, lr2, 2);
     T.append_scalar("claim_eval_dotp_left", lr2[0]);
     T.append_scalar("claim_eval_dotp_right", lr2[1]);
     if (!(lr2[0] + lr2[1] == inst_evals[m])) throw SpError(SP_ERR_INTERNAL, "dot-product circuit does not evaluate to the claimed matrix evaluation");
@@ -720,11 +726,11 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
     for (int m = 0; m < 3; m++) tabs.push_back(dv.col_addr[m]);
     for (int m = 0; m < 3; m++) tabs.push_back(dv.col_ts[m]);
     for (int m = 0; m < 3; m++) tabs.push_back(dv.val[m]);
-    dev::dot_many(ctx.small.p + 64, tabs.data(), (int)tabs.size(), eq_ops.p, N, ctx.red.p, ctx.stream);
+    dev::dot_many(ctx.small.p + layout::SMALL_BATCH.off, tabs.data(), (int)tabs.size(), eq_ops.p, N, ctx.red.p, ctx.stream);
     const u256* mt[2] = {dv.row_audit, dv.col_audit};
-    dev::dot_many(ctx.small.p + 64 + 21, mt, 2, eq_mem.p, cells, ctx.red.p, ctx.stream);
+    dev::dot_many(ctx.small.p + layout::SMALL_BATCH.off + tabs.size(), mt, 2, eq_mem.p, cells, ctx.red.p, ctx.stream);
     std::vector<Fq> ev(23);
-    ctx.get_small(64, ev.data(), 23);
+    ctx.get_small(layout::SMALL_BATCH.off, ev.data(), 23);
     hl.derefs_row.assign(ev.begin(), ev.begin() + 3);
     hl.derefs_col.assign(ev.begin() + 3, ev.begin() + 6);
     hl.row_addr.assign(ev.begin() + 6, ev.begin() + 9);
