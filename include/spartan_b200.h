@@ -52,6 +52,24 @@ unsigned long long sp_kernel_launches(void);   /* kernels launched by this libra
 /* device blocks freed by the library are kept for reuse by later proofs of this process; this returns them to the driver (e.g. before another
  * process on the same GPU needs the memory) and gives their size in bytes.  Buffers still held by live objects are not touched. */
 unsigned long long sp_release_cached_memory(void);
+/* Memory-check mode, process-wide, single GPU (a debugging aid: slower, never for production).  While it is on, every device block the library
+ * hands out is filled first, fresh or reused: field elements and points with 0xFF bytes (above both moduli, not a point), everything else with
+ * zero; every block carries a zero guard band of at least 4 KiB past the requested size; and every entry point refills the context's persistent
+ * scratch (and a point set's sort workspace) before it starts.  So a read of memory the call did not write changes its result, and a write past a
+ * buffer's end lands in the guard, where the block's free or sp_debug_memcheck_scan reports it.  Switching the mode drops the cache of freed
+ * blocks; a block allocated before the switch is never reused under it.  Switch it on before the first context is created. */
+void sp_debug_memcheck(int on);
+typedef struct sp_memcheck_counts {
+  unsigned long long blocks_filled;        /* blocks handed out under the mode */
+  unsigned long long blocks_refilled;      /* ... of them, cached blocks reused */
+  unsigned long long context_refills;      /* entry points that refilled a context's persistent scratch */
+  unsigned long long guard_bytes_checked;
+  unsigned long long violations;           /* dirty guard bands found */
+} sp_memcheck_counts;
+/* the counters since load and, when there were violations, the first one's message, a newline and the latest one's ("" otherwise) */
+int sp_debug_memcheck_report(sp_memcheck_counts* out, char* violations, size_t buflen);
+/* synchronise the device and check the guard band of every live block; returns the violations found (~0 on a CUDA error) */
+unsigned long long sp_debug_memcheck_scan(void);
 
 /* ---- one proof over several GPUs (SURVEY.md 8(e); the reference is single-process, the loops being sharded are dense_mlpoly.rs:215-223,
  * sumcheck.rs:290-357 / :460-469 / :625-652, dense_mlpoly.rs:165-177, product_tree.rs:18-56).  One process per GPU, one context per process.

@@ -55,6 +55,39 @@ def release_cached_memory():
     return int(lib.sp_release_cached_memory())
 
 
+class _MemcheckCounts(C.Structure):
+    _fields_ = [(n, C.c_ulonglong) for n in ("blocks_filled", "blocks_refilled", "context_refills", "guard_bytes_checked", "violations")]
+
+
+lib.sp_debug_memcheck_scan.restype = C.c_ulonglong
+
+
+def debug_memcheck(on=True):
+    """process-wide memory-check mode (sp_debug_memcheck, single GPU): every device block filled when handed out and guarded past its end, the
+    contexts' persistent scratch refilled at every call.  Switch it on before the first Context is created"""
+    lib.sp_debug_memcheck(C.c_int(1 if on else 0))
+
+
+def debug_memcheck_scan():
+    """synchronise the device and check every live block's guard band; returns the violations found"""
+    n = int(lib.sp_debug_memcheck_scan())
+    if n == 2 ** 64 - 1:
+        raise SpartanB200Error("sp_debug_memcheck_scan: " + lib.sp_last_error(None).decode())
+    return n
+
+
+def debug_memcheck_report():
+    """the mode's counters since load, and the first and the latest violation's message ("" when there was none)"""
+    c = _MemcheckCounts()
+    buf = C.create_string_buffer(8192)
+    if lib.sp_debug_memcheck_report(C.byref(c), buf, _sz(len(buf))) != SP_OK:
+        raise SpartanB200Error("sp_debug_memcheck_report: message longer than the buffer")
+    out = {n: int(getattr(c, n)) for n, _ in _MemcheckCounts._fields_}
+    first, _, last = buf.value.decode().partition("\n")
+    out["first_violation"], out["last_violation"] = first, last
+    return out
+
+
 def _p(a):
     return a.ctypes.data_as(_vp) if isinstance(a, np.ndarray) else a
 

@@ -20,7 +20,8 @@ struct sp_gen_tables { std::unique_ptr<GenTables> t; };
 
 static std::string g_create_error;
 
-#define SP_TRY(ctxp) try {
+// every entry point with a context starts from refilled persistent scratch under the memory-check mode (Ctx::memcheck_refill)
+#define SP_TRY(ctxp) try { if (ctxp) (ctxp)->c.memcheck_refill();
 #define SP_CATCH(ctxp)                                                                           \
   }                                                                                              \
   catch (const SpError& e) { if (ctxp) (ctxp)->c.last_error = e.what(); return e.code; }        \
@@ -55,6 +56,20 @@ void sp_ctx_destroy(sp_ctx* ctx) { delete ctx; }
 const char* sp_last_error(const sp_ctx* ctx) { return ctx ? ctx->c.last_error.c_str() : g_create_error.c_str(); }
 unsigned long long sp_kernel_launches(void) { return dev::launch_count(); }
 unsigned long long sp_release_cached_memory(void) { return dev::pool_release_cached(); }
+void sp_debug_memcheck(int on) { dev::memcheck_enable(on != 0); }
+int sp_debug_memcheck_report(sp_memcheck_counts* out, char* violations, size_t buflen) {
+  std::string first, last;
+  const dev::MemcheckStats s = dev::memcheck_stats(&first, &last);
+  if (out) *out = sp_memcheck_counts{s.blocks_filled, s.blocks_refilled, s.context_refills, s.guard_bytes_checked, s.violations};
+  if (!violations) return SP_OK;
+  const std::string text = first.empty() ? "" : first + "\n" + last;
+  if (text.size() + 1 > buflen) return SP_ERR_INVALID_ARG;
+  memcpy(violations, text.c_str(), text.size() + 1);
+  return SP_OK;
+}
+unsigned long long sp_debug_memcheck_scan(void) {
+  try { return dev::memcheck_scan(); } catch (const std::exception& e) { g_create_error = e.what(); return ~0ull; }
+}
 int sp_timings(sp_ctx* ctx, char* buf, size_t buflen) {
   std::ostringstream os;
   for (auto& t : ctx->c.timings) os << t.first << "=" << t.second << ";";
@@ -544,6 +559,7 @@ static void msm_var_run(Ctx& c, const sp_points* p, size_t offset, const u256* d
     dev::PipPlan plan = dev::pip_plan(n, cenv ? atoi(cenv) : 0);
     const size_t need = dev::pip_scratch_bytes(plan);
     if (need > p->scratch_bytes) { p->scratch.alloc(need); p->scratch_bytes = need; }   // the sort workspace stays with the point set
+    else if (dev::memcheck_on()) dev::memcheck_fill(p->scratch.p, p->scratch.n, dev::FILL_ZERO);   // ... and is refilled like the context's
     dev::msm_var(out.p, p->pts.p + offset, d_scalars, plan, p->scratch.p, c.stream);
   }
   if (sharded) {

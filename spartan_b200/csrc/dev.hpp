@@ -5,6 +5,7 @@
 #include <stddef.h>
 #include <stdint.h>
 #include <string>
+#include <type_traits>
 #include "field.cuh"
 #include "curve.cuh"
 #include "../../include/spartan_b200.h"
@@ -25,10 +26,27 @@ void stream_destroy(cudaStream_t s);
 void stream_sync(cudaStream_t s);
 // size-bucketed caching allocator on top of cudaMalloc: a prove call allocates the same multi-hundred-MB buffers every time, and
 // cudaMalloc / cudaFree (which synchronises the device) would otherwise cost milliseconds per proof
-void* pool_alloc(size_t bytes);
+// `fill`: what a block holds when it is handed out under the memory-check mode (below); ignored otherwise
+enum PoolFill { FILL_ZERO = 0, FILL_FF = 1 };
+// field elements and points get 0xFF bytes: above both moduli and not a point, so a read of an entry nobody wrote shows in the result.  Every
+// other buffer (raw scratch, indices, counters, structs) gets zero, what fresh memory holds: an index read from it stays in range
+template <class T> constexpr int pool_fill_of() { return std::is_same<T, u256>::value || std::is_same<T, ge>::value || std::is_same<T, ge_niels>::value ? FILL_FF : FILL_ZERO; }
+void* pool_alloc(size_t bytes, int fill = FILL_ZERO);
 void pool_free(void* p);
 size_t pool_release_cached();   // cudaFree every cached free block; returns their bytes
 size_t pool_live_bytes();       // rounded bytes of the blocks handed out and not yet freed, every device
+// ---- memory-check mode (sp_debug_memcheck; single GPU: sharded windows are not pool memory).  While it is on, every block is filled when it is
+// handed out, fresh or reused (after a device synchronise, so the previous owner has finished), and carries a zero guard band of at least
+// MEMCHECK_GUARD bytes past the requested size; a non-zero guard byte found at pool_free or by memcheck_scan is a violation.  Switching it on or
+// off drops the free cache, and a block allocated before the switch is never cached under it.
+constexpr size_t MEMCHECK_GUARD = 4096;
+struct MemcheckStats { unsigned long long blocks_filled = 0, blocks_refilled = 0, context_refills = 0, guard_bytes_checked = 0, violations = 0; };
+void memcheck_enable(bool on);
+bool memcheck_on();
+MemcheckStats memcheck_stats(std::string* first_violation, std::string* last_violation);
+unsigned long long memcheck_scan();   // synchronises the device and checks the guard of every live block; returns the violations it found
+void memcheck_fill(void* d, size_t bytes, int fill);   // device memory, between two device synchronises
+void memcheck_count_refill();         // one context's persistent scratch refilled at an entry point
 void* hmalloc_pinned(size_t bytes);
 void hfree_pinned(void* p);
 void h2d(void* d, const void* h, size_t bytes, cudaStream_t s);

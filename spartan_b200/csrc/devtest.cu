@@ -13,6 +13,7 @@
 #include <cuda_runtime.h>
 #include <string.h>
 #include <exception>
+#include <stdexcept>
 #include <string>
 #include <vector>
 #include "kcommon.cuh"
@@ -27,14 +28,21 @@ namespace {
 constexpr int TPB = 128;
 unsigned blocks_for(size_t threads) { return (unsigned)((threads + TPB - 1) / TPB); }
 
-// device copies of one call's arrays, freed on return; the first failing CUDA call is kept and later steps are skipped
+// device copies of one call's arrays, freed on return; the first failing CUDA call is kept and later steps are skipped.  Under the memory-check
+// mode (spd_memcheck) the arrays come from the library's pool instead of cudaMalloc: filled by type and guarded, the guard checked on return.
 struct Call {
   std::vector<void*> bufs;
+  std::vector<bool> pooled;
   cudaError_t err = cudaSuccess;
   template <class T> T* alloc(size_t n) {
     void* d = nullptr;
-    if (err == cudaSuccess) err = cudaMalloc(&d, n * sizeof(T));
+    const bool mc = memcheck_on();
+    if (err == cudaSuccess) {
+      if (!mc) err = cudaMalloc(&d, n * sizeof(T));
+      else try { d = pool_alloc(n * sizeof(T), pool_fill_of<T>()); } catch (const std::exception&) { err = cudaErrorMemoryAllocation; }
+    }
     bufs.push_back(d);
+    pooled.push_back(mc);
     return (T*)d;
   }
   template <class T> T* in(const T* h, size_t n) {
@@ -47,11 +55,12 @@ struct Call {
   }
   bool ok() const { return err == cudaSuccess; }
   void launched() { if (err == cudaSuccess) err = cudaGetLastError(); }
-  ~Call() { for (void* p : bufs) if (p) cudaFree(p); }
+  ~Call() { for (size_t i = 0; i < bufs.size(); i++) if (bufs[i]) { if (pooled[i]) pool_free(bufs[i]); else cudaFree(bufs[i]); } }
 };
 
 // one call of a kernel hook: a Call whose wrappers run on a stream of its own (a blocking stream: ordered after the synchronous copies of in() and
-// before those of out()), drained before the buffers go, plus zeroed device and pinned host buffers for scratch and the HostSig words
+// before those of out()), drained before the buffers go, plus zeroed device and pinned host buffers for scratch and the HostSig words.  Scratch
+// counters and flag words start at zero by contract, also under the memory-check mode; pinned result arrays of field elements get 0xFF there.
 constexpr int SPD_REFUSED = -1;
 std::string g_last_error;
 struct KCall : Call {
@@ -70,7 +79,7 @@ struct KCall : Call {
   template <class T> T* host(size_t n) {
     void* p = nullptr;
     if (err == cudaSuccess) err = cudaMallocHost(&p, n * sizeof(T));
-    if (err == cudaSuccess) memset(p, 0, n * sizeof(T));
+    if (err == cudaSuccess) memset(p, memcheck_on() && pool_fill_of<T>() == FILL_FF ? 0xFF : 0, n * sizeof(T));
     pinned.push_back(p);
     return (T*)p;
   }
@@ -399,6 +408,92 @@ int spd_window_digits(size_t n, const u256* k, int wbits, int* out) {
 
 // ---------------------------------------------------------------------------------------------------- kernel hooks (the sp::dev wrappers)
 const char* spd_last_error() { return g_last_error.c_str(); }
+// ---- the memory-check mode of this library's own copy of the pool: the mirror of sp_debug_memcheck, sp_debug_memcheck_report and
+// sp_debug_memcheck_scan.  counters: blocks filled, reused blocks refilled, context refills, guard bytes checked, violations
+void spd_memcheck(int on) { memcheck_enable(on != 0); }
+int spd_memcheck_report(unsigned long long counters[5], char* violations, size_t cap) {
+  std::string first, last;
+  const MemcheckStats s = memcheck_stats(&first, &last);
+  const unsigned long long v[5] = {s.blocks_filled, s.blocks_refilled, s.context_refills, s.guard_bytes_checked, s.violations};
+  memcpy(counters, v, sizeof v);
+  const std::string text = first.empty() ? "" : first + "\n" + last;
+  if (text.size() + 1 > cap) return SPD_REFUSED;
+  memcpy(violations, text.c_str(), text.size() + 1);
+  return 0;
+}
+unsigned long long spd_memcheck_scan() {
+  try { return memcheck_scan(); } catch (const std::exception& e) { g_last_error = e.what(); return ~0ull; }
+}
+// The mode's mechanism on its own, through dev::pool_alloc: fresh and reused blocks read back as their fill class says, a block cached or live
+// before the switch is not handed out under it, a byte written past the requested size is reported by the scan and at free, and switching the
+// mode off restores the plain rounding.  0, or SPD_REFUSED with the failed check in spd_last_error(); `text` gets the messages of the two planted
+// overruns.  The mode is left as it was found.
+int spd_pool_selftest(char* text, size_t cap) {
+  const bool was = memcheck_on();
+  std::string notes;
+  const int rc = guarded([&]() -> int {
+    auto need = [](bool c, const char* what) { if (!c) throw std::runtime_error(std::string("pool self-test: ") + what); };
+    auto cu = [](cudaError_t e) { if (e != cudaSuccess) throw std::runtime_error(std::string("pool self-test: ") + cudaGetErrorString(e)); };
+    auto all = [&](const void* d, size_t n, uint8_t v) {
+      std::vector<uint8_t> h(n);
+      cu(cudaMemcpy(h.data(), d, n, cudaMemcpyDeviceToHost));
+      for (uint8_t x : h) if (x != v) return false;
+      return true;
+    };
+    auto stats = []() { return memcheck_stats(nullptr, nullptr); };
+    auto last = []() { std::string l; memcheck_stats(nullptr, &l); return l; };
+    const size_t B = 1000;   // far from a bucket edge: a 1 KiB block without the mode, 8 KiB with its 4 KiB guard
+    memcheck_enable(false);
+    void* before_cached = pool_alloc(B, FILL_FF);
+    cu(cudaMemset(before_cached, 0x5A, B));
+    pool_free(before_cached);
+    void* before_live = pool_alloc(B, FILL_FF);
+    cu(cudaMemset(before_live, 0x5A, B));
+    memcheck_enable(true);
+    const MemcheckStats s0 = stats();
+    const size_t live0 = pool_live_bytes();
+    uint8_t* a = (uint8_t*)pool_alloc(B, FILL_FF);
+    need(pool_live_bytes() - live0 == 8192, "a 1000-byte block under the mode is not 8 KiB");
+    need(stats().blocks_filled == s0.blocks_filled + 1 && stats().blocks_refilled == s0.blocks_refilled, "the block cached before the switch was handed out under it");
+    need(all(a, B, 0xFF), "a fresh u256 block does not read back all 0xFF");
+    need(all(a + B, 8192 - B, 0), "the guard band of a fresh block is not zero");
+    pool_free(before_live);   // allocated before the switch: freed, not cached
+    uint8_t* b = (uint8_t*)pool_alloc(B, FILL_FF);
+    need(stats().blocks_refilled == s0.blocks_refilled, "a block allocated before the switch was reused under it");
+    cu(cudaMemset(a, 0x11, B));
+    pool_free(a);
+    uint8_t* a2 = (uint8_t*)pool_alloc(B, FILL_FF);
+    need(a2 == a && stats().blocks_refilled == s0.blocks_refilled + 1, "a freed block was not reused");
+    need(all(a2, B, 0xFF), "a reused u256 block does not read back all 0xFF");
+    uint8_t* raw = (uint8_t*)pool_alloc(B, FILL_ZERO);
+    cu(cudaMemset(raw, 0x22, B));
+    pool_free(raw);
+    raw = (uint8_t*)pool_alloc(B, FILL_ZERO);
+    need(stats().blocks_refilled == s0.blocks_refilled + 2, "a freed raw block was not reused");
+    need(all(raw, B, 0), "a reused raw block does not read back zero");
+    const unsigned long long v0 = stats().violations;
+    cu(cudaMemset(a2 + B + 7, 1, 1));   // inside the guard, through the host API
+    need(memcheck_scan() == 1, "the scan missed a byte written past the end");
+    notes += last() + "\n";
+    need(memcheck_scan() == 0, "the scan reported one overrun twice");
+    cu(cudaMemset(raw + B, 1, 1));
+    pool_free(raw);
+    need(stats().violations == v0 + 2, "pool_free missed a byte written past the end");
+    notes += last();
+    pool_free(a2);
+    pool_free(b);
+    memcheck_enable(false);
+    const size_t live1 = pool_live_bytes();
+    void* c = pool_alloc(B, FILL_FF);
+    const size_t plain = pool_live_bytes() - live1;
+    pool_free(c);
+    need(plain == 1024, "switching the mode off did not restore the plain rounding");
+    return 0;
+  });
+  memcheck_enable(was);
+  if (cap) { const size_t n = notes.size() < cap - 1 ? notes.size() : cap - 1; memcpy(text, notes.data(), n); text[n] = 0; }
+  return rc;
+}
 unsigned long long spd_launch_count() { return launch_count(); }
 void spd_prof_enable(int on) { prof_enable(on != 0); }
 // "name:launches:total_ms:total_algorithmic_bytes;..." of the kernel families launched since spd_prof_enable(1), truncated to cap - 1 characters
@@ -527,7 +622,10 @@ int spd_sc_g_chain(int ninst, size_t len, u256* a, u256* b, const u256* E0, int 
       c.sync();
       c.out(out + (size_t)j * 3 * ninst, dout, 3 * (size_t)ninst);
       if (use_sig && c.ok()) {
-        memcpy(host_out + (size_t)j * 3 * ninst, sig.host_out, 3 * (size_t)ninst * sizeof(u256));
+        u256* h = host_out + (size_t)j * 3 * ninst;
+        memcpy(h, sig.host_out, 3 * (size_t)ninst * sizeof(u256));
+        // the eq-factored kernels publish q(0), q(inf) only: the third entry of their pinned slots is nobody's, and host_out says 0 there
+        if (j < jG) for (int i = 0; i < ninst; i++) memset(&h[3 * (size_t)i + 2], 0, sizeof(u256));
         flags[j] = *(volatile unsigned*)sig.flag;
         c.out(dones + j, sig.done, 1);
       }

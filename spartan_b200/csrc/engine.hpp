@@ -30,7 +30,7 @@ struct DevBuf {  // owning device allocation
   DevBuf(DevBuf&& o) noexcept : p(o.p), n(o.n) { o.p = nullptr; o.n = 0; }
   DevBuf& operator=(DevBuf&& o) noexcept { if (this != &o) { release(); p = o.p; n = o.n; o.p = nullptr; o.n = 0; } return *this; }
   ~DevBuf() { release(); }
-  void alloc(size_t count) { release(); p = (T*)dev::pool_alloc(count * sizeof(T)); n = count; }
+  void alloc(size_t count) { release(); p = (T*)dev::pool_alloc(count * sizeof(T), dev::pool_fill_of<T>()); n = count; }
   void release() { if (p) dev::pool_free(p); p = nullptr; n = 0; }
 };
 
@@ -169,6 +169,10 @@ struct Ctx {
   void wait_sig(const dev::HostSig& s);   // spins on the flag; falls back to a stream synchronise to surface CUDA errors
   void sync() { dev::stream_sync(stream); }
   void ensure_scratch(size_t bytes) { if (scratch.n < bytes) { sync(); scratch.alloc(bytes); } }
+  // memory-check mode (dev::memcheck_on): refill the scratch that persists between calls, at the start of every device entry point, as the
+  // allocator fills a block it hands out: scratch and scratch2 zero, small 0xFF (all but ones()), the pinned staging regions 0xFF.  The flag
+  // words, sig_done and the tickets in red keep their contract (zero or self-resetting) and are not touched.
+  void memcheck_refill();
   void get_small(size_t slot, Fq* v, size_t k);  // download k scalars from small[slot..]; synchronises
   void upload(u256* d, const Fq* h, size_t n);
   std::vector<Fq> download(const u256* d, size_t n);

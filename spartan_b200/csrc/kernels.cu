@@ -87,9 +87,21 @@ void stream_wait_event(cudaStream_t s, void* ev) { ck(cudaStreamWaitEvent(s, (cu
 void stream_destroy(cudaStream_t s) { cudaStreamDestroy(s); }
 void stream_sync(cudaStream_t s) { ck(cudaStreamSynchronize(s), "cudaStreamSynchronize"); }
 namespace {
+constexpr size_t UNGUARDED = ~(size_t)0;
+struct LiveBlock {
+  int dev; size_t size;           // device, rounded size
+  size_t req;                     // requested bytes of a block handed out under the memory-check mode (guard: [req, size)); UNGUARDED otherwise
+  int fill; unsigned long long seq;   // its fill class and allocation number under the mode
+};
 std::mutex g_pool_mu;
 std::multimap<std::pair<int, size_t>, void*> g_pool_free;  // (device, rounded size) -> cached block
-std::map<void*, std::pair<int, size_t>> g_pool_live;       // block -> (device, rounded size)
+std::map<void*, LiveBlock> g_pool_live;                    // block -> what pool_alloc handed out
+std::atomic<bool> g_memcheck{false};
+struct {   // memory-check counters and messages, under g_pool_mu
+  MemcheckStats st;
+  unsigned long long seq = 0;
+  std::string first, last;
+} g_mc;
 size_t pool_round(size_t b) {
   if (b < 256) b = 256;
   if (b <= (1u << 20)) { size_t r = 256; while (r < b) r <<= 1; return r; }
@@ -102,6 +114,28 @@ size_t drop_cached_locked() {   // caller holds g_pool_mu
   g_pool_free.clear();
   return bytes;
 }
+// the guard band [req, size) of a block handed out under the memory-check mode must still be zero.  Caller holds g_pool_mu and has synchronised
+// the device.  A dirty guard is reported once: it is zeroed again after the report.
+void guard_check_locked(void* p, const LiveBlock& b) {
+  const size_t n = b.size - b.req;
+  std::vector<uint8_t> h(n);
+  uint8_t* guard = (uint8_t*)p + b.req;
+  std::string msg;
+  if (cudaMemcpy(h.data(), guard, n, cudaMemcpyDeviceToHost) != cudaSuccess) {
+    msg = std::string("guard band unreadable (") + cudaGetErrorString(cudaGetLastError()) + ")";
+  } else {
+    g_mc.st.guard_bytes_checked += n;
+    size_t k = 0;
+    while (k < n && !h[k]) k++;
+    if (k == n) return;
+    msg = "first dirty guard byte at offset " + std::to_string(b.req + k) + " (" + std::to_string(k) + " bytes past the end)";
+    cudaMemset(guard, 0, n);
+  }
+  g_mc.st.violations++;
+  g_mc.last = "write past the end of device allocation #" + std::to_string(b.seq) + " (" + std::to_string(b.req) + " bytes requested, " +
+              (b.fill == FILL_FF ? "field elements / points" : "raw / integer") + "): " + msg;
+  if (g_mc.first.empty()) g_mc.first = g_mc.last;
+}
 }  // namespace
 size_t pool_release_cached() {
   std::lock_guard<std::mutex> lk(g_pool_mu);
@@ -110,17 +144,20 @@ size_t pool_release_cached() {
 size_t pool_live_bytes() {
   std::lock_guard<std::mutex> lk(g_pool_mu);
   size_t bytes = 0;
-  for (auto& kv : g_pool_live) bytes += kv.second.second;
+  for (auto& kv : g_pool_live) bytes += kv.second.size;
   return bytes;
 }
-void* pool_alloc(size_t bytes) {
-  size_t r = pool_round(bytes);
+void* pool_alloc(size_t bytes, int fill) {
+  const bool mc = g_memcheck.load(std::memory_order_relaxed);
+  size_t r = pool_round(mc ? bytes + MEMCHECK_GUARD : bytes);
+  if (mc) ck(cudaDeviceSynchronize(), "cudaDeviceSynchronize (memory check)");   // whoever used a cached block last has finished with it
   int dev = 0;
   cudaGetDevice(&dev);
   std::lock_guard<std::mutex> lk(g_pool_mu);
   auto it = g_pool_free.find({dev, r});
   void* p;
-  if (it != g_pool_free.end()) { p = it->second; g_pool_free.erase(it); }
+  const bool reused = it != g_pool_free.end();
+  if (reused) { p = it->second; g_pool_free.erase(it); }
   else {
     cudaError_t e = cudaMalloc(&p, r);
     if (e != cudaSuccess) {  // out of memory: drop the cache and retry once
@@ -129,7 +166,13 @@ void* pool_alloc(size_t bytes) {
       ck(cudaMalloc(&p, r), "cudaMalloc");
     }
   }
-  g_pool_live[p] = {dev, r};
+  if (!mc) { g_pool_live[p] = {dev, r, UNGUARDED, fill, 0}; return p; }
+  g_pool_live[p] = {dev, r, bytes, fill, ++g_mc.seq};
+  ck(cudaMemset(p, fill == FILL_FF ? 0xFF : 0, bytes), "cudaMemset (memory check)");
+  ck(cudaMemset((uint8_t*)p + bytes, 0, r - bytes), "cudaMemset (memory check guard)");
+  ck(cudaDeviceSynchronize(), "cudaDeviceSynchronize (memory check)");   // the legacy-stream fills are unordered with the library's streams
+  g_mc.st.blocks_filled++;
+  if (reused) g_mc.st.blocks_refilled++;
   return p;
 }
 void pool_free(void* p) {
@@ -137,13 +180,49 @@ void pool_free(void* p) {
   std::lock_guard<std::mutex> lk(g_pool_mu);
   auto it = g_pool_live.find(p);
   if (it == g_pool_live.end()) { cudaFree(p); return; }
+  const LiveBlock b = it->second;
+  g_pool_live.erase(it);
+  if (b.req != UNGUARDED) {   // no throw here: pool_free runs in destructors
+    if (cudaDeviceSynchronize() != cudaSuccess) cudaGetLastError();
+    guard_check_locked(p, b);
+  }
   // blocks of tens of GB (generator tables) are long-lived: do not hoard them.  Per-proof buffers stay cached even when they pass 1 GiB (2^22 constraints: the
   // 1.2 GB dot-product circuit buffer) — a cudaFree synchronises the device, i.e. waits for the background stream's MSM, and the cudaMalloc of the next proof
-  // would then make the proof time depend on whether that MSM had finished
-  if (it->second.second > ((size_t)8 << 30)) cudaFree(p);
-  else g_pool_free.insert({it->second, p});
-  g_pool_live.erase(it);
+  // would then make the proof time depend on whether that MSM had finished.  Under the memory-check mode, a block from before the switch is not cached.
+  if (b.size > ((size_t)8 << 30) || (g_memcheck.load(std::memory_order_relaxed) && b.req == UNGUARDED)) cudaFree(p);
+  else g_pool_free.insert({{b.dev, b.size}, p});
 }
+void memcheck_enable(bool on) {
+  std::lock_guard<std::mutex> lk(g_pool_mu);
+  if (g_memcheck.load() == on) return;
+  drop_cached_locked();   // a cached block is never handed out across the switch
+  g_memcheck.store(on);
+}
+bool memcheck_on() { return g_memcheck.load(std::memory_order_relaxed); }
+MemcheckStats memcheck_stats(std::string* first_violation, std::string* last_violation) {
+  std::lock_guard<std::mutex> lk(g_pool_mu);
+  if (first_violation) *first_violation = g_mc.first;
+  if (last_violation) *last_violation = g_mc.last;
+  return g_mc.st;
+}
+unsigned long long memcheck_scan() {
+  std::lock_guard<std::mutex> lk(g_pool_mu);
+  const unsigned long long before = g_mc.st.violations;
+  bool synced = false;
+  for (auto& kv : g_pool_live) {
+    if (kv.second.req == UNGUARDED) continue;
+    if (!synced) { ck(cudaDeviceSynchronize(), "cudaDeviceSynchronize (memory check scan)"); synced = true; }
+    guard_check_locked(kv.first, kv.second);
+  }
+  return g_mc.st.violations - before;
+}
+void memcheck_fill(void* d, size_t bytes, int fill) {
+  if (!bytes) return;
+  ck(cudaDeviceSynchronize(), "cudaDeviceSynchronize (memory check)");
+  ck(cudaMemset(d, fill == FILL_FF ? 0xFF : 0, bytes), "cudaMemset (memory check)");
+  ck(cudaDeviceSynchronize(), "cudaDeviceSynchronize (memory check)");
+}
+void memcheck_count_refill() { std::lock_guard<std::mutex> lk(g_pool_mu); g_mc.st.context_refills++; }
 void* hmalloc_pinned(size_t b) { void* p = nullptr; ck(cudaMallocHost(&p, b ? b : 16), "cudaMallocHost"); return p; }
 void hfree_pinned(void* p) { if (p) cudaFreeHost(p); }
 void h2d(void* d, const void* h, size_t b, cudaStream_t s) { g_h2d += b; if (b) ck(cudaMemcpyAsync(d, h, b, cudaMemcpyHostToDevice, s), "h2d"); }

@@ -36,6 +36,7 @@ Ctx::Ctx(int dev_) : device(dev_) {
   stream2 = dev::stream_create_prio(-1);
   ev_fork = dev::event_create(); ev_join = dev::event_create();
   pinned = (uint8_t*)dev::hmalloc_pinned(layout::PINNED_BYTES);
+  if (dev::memcheck_on()) memset(pinned, 0xFF, layout::PINNED_BYTES);   // before the flag words are zeroed
   host_res = reinterpret_cast<u256*>(pinned + layout::PIN_RES.off);
   host_flag = reinterpret_cast<unsigned int*>(pinned + layout::PIN_FLAG.off);
   host_flag_c = reinterpret_cast<unsigned int*>(pinned + layout::PIN_FLAG_C.off);
@@ -66,6 +67,19 @@ Ctx::~Ctx() {
   if (ev_a) { dev::event_destroy(ev_a); dev::event_destroy(ev_b); }
   dev::hfree_pinned(pinned);
   dev::stream_destroy(stream);
+}
+void Ctx::memcheck_refill() {
+  if (!dev::memcheck_on()) return;
+  sync();
+  dev::stream_sync(stream2);
+  dev::memcheck_fill(scratch.p, scratch.n, dev::FILL_ZERO);
+  dev::memcheck_fill(scratch2.p, scratch2.n, dev::FILL_ZERO);
+  // all of small but ones(), which nobody writes after Ctx::Ctx (a fill_one here would add a kernel launch to every call)
+  dev::memcheck_fill(small.p, layout::SMALL_ONES.off * sizeof(u256), dev::FILL_FF);
+  dev::memcheck_fill(small.p + layout::SMALL_ONES.end(), (small.n - layout::SMALL_ONES.end()) * sizeof(u256), dev::FILL_FF);
+  for (const layout::Region& r : {layout::PIN_STAGE, layout::PIN_ZKPRE, layout::PIN_RES, layout::PIN_XY}) memset(pinned + r.off, 0xFF, r.cap);
+  sync();
+  dev::memcheck_count_refill();
 }
 void Ctx::wait_sig(const dev::HostSig& s) {
   volatile unsigned int* f = s.flag;
