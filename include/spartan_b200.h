@@ -197,6 +197,64 @@ int sp_msm_var_resident(sp_ctx* ctx, const sp_points* p, size_t offset, const sp
  * returns the encoding of the whole sum (group.rs:98-117 on a vector split by index range) */
 int sp_msm_var_sharded(sp_ctx* ctx, const sp_points* p, size_t offset, const sp_poly* scalars, uint8_t out32[32]);
 
+/* ---- polynomial commitments and evaluation proofs for the caller's own tables: the Hyrax-style commitment of dense_mlpoly.rs (a table of 2^ell
+ * entries is an L x R matrix, L = 2^floor(ell/2) rows of R = 2^ceil(ell/2), each row committed with one Pedersen vector commitment) and its
+ * opening by PolyEvalProof (a bulletproofs inner-product argument), bytes identical to the reference's for the same transcript and tape.  Use:
+ * commit before a sumcheck, absorb the commitment, run sp_sumcheck_prove_t, then open every table at its r with sp_pc_eval_prove_joint_t on the
+ * same transcript.  Every entry below runs on this rank's GPU alone, also on a connected multi-GPU context.  Tables are read, never modified.
+ *
+ * PolyCommitmentGens::new(num_vars, label) (dense_mlpoly.rs:29-36) = DotProductProofGens::new(n, label), n = 2^(num_vars - num_vars/2)
+ * (nizk/mod.rs:414-418): n + 2 points of the label's SHAKE256 stream, gens_n = G[0..n) and gens_1 = G[n], both with h = G[n+1].  Device
+ * footprint (read it with sp_device_bytes_live): the n + 2 points and a fixed-base window table, of 8-bit windows (393 KB per generator) for
+ * n <= 256; for larger n a 16-bit row table (3.1 MB per generator) and 13-bit windows (7.9 MB per generator; 15-bit, 26.7 MB, from n = 2048),
+ * each only if it fits in 65% of the free device memory (else no row table, narrower windows: same bytes, slower).  num_vars = 20: n = 1024,
+ * about 11 GB; num_vars = 24: n = 4096, about 32 GB of window table plus 12.7 GB of row table. */
+typedef struct sp_pc_gens sp_pc_gens;
+#define SP_PC_MAX_TABLES 64
+int sp_pc_gens_create(sp_ctx* ctx, size_t num_vars, const uint8_t* label, size_t label_len, sp_pc_gens** out);
+/* PolyCommitmentGens::new(num_vars, label) for num_vars <= larger's, as a view of `larger`'s tables (MultiCommitGens::new of any size is a prefix of
+ * the label's stream): proves and verifies byte for byte as sp_pc_gens_create(num_vars, label) would, and holds no device memory of its own.  The
+ * tables live until the last of the handles that share them is freed.  SP_ERR_INVALID_ARG for a larger num_vars or a handle of another context. */
+int sp_pc_gens_create_from(sp_ctx* ctx, const sp_pc_gens* larger, size_t num_vars, sp_pc_gens** out);
+void sp_pc_gens_free(sp_pc_gens* g);
+/* RandomTape::new(b"proof") (random.rs:10-17) with its seed scalar, as a 203-byte STROBE state like a transcript's (SP_TRANSCRIPT_STATE_BYTES),
+ * so that one tape can be threaded through a commitment and later proofs.  The sp_transcript_* helpers work on it.  seed_mont must be FRESH OS
+ * RANDOMNESS (Scalar::from_bytes_wide of 64 random bytes, as RandomTape::new draws it): every blind is a function of it. */
+int sp_random_tape_new(const uint64_t seed_mont[4], uint8_t* tape_state /* out */);
+/* DensePolynomial::merge(polys).commit(gens, tape) (dense_mlpoly.rs:179-204, :259-272): with k = 1 DensePolynomial::commit of the table; with
+ * k > 1 the commitment to the k tables concatenated and zero-padded to the next power of two.  *comm = bincode(PolyCommitment) (free with
+ * sp_free).  tape_state NULL: no blinds, blinds_out (L scalars) gets zeros; else the tape draws random_vector("poly_blinds", L) and is advanced.
+ * blinds_out may be NULL.  SP_ERR_INVALID_ARG, nothing written: k outside 1 .. SP_PC_MAX_TABLES, lengths unequal or not a power of two, gens'
+ * n != R of the merged table (the reference asserts gens_n.n == R, commitments.rs:87-91), a handle of another context. */
+int sp_pc_commit(sp_ctx* ctx, const sp_pc_gens* gens, sp_poly* const* polys, int k, uint8_t* tape_state /* in, out; NULL = no blinds */, uint8_t** comm,
+                 size_t* comm_len, uint64_t* blinds_out /* L x 4 or NULL */);
+/* PolyEvalProof::prove(poly, blinds, r, Zr, blind_Zr, gens, transcript, tape) (dense_mlpoly.rs:312-365) on the caller's transcript and tape
+ * (both advanced).  ell = |r| = log2 of the table's length, 0 allowed.  blinds: the L blinds of the table's commitment or NULL (zero).  Zr NULL:
+ * computed on the device as Z(r); a given Zr is not checked (neither does the reference): the verifier rejects the proof.  blind_Zr NULL: zero.
+ * Out: *proof = bincode(PolyEvalProof) (free with sp_free), C_Zr32 = the commitment to Zr the proof is against, Zr_out = the Zr used.
+ * SP_ERR_INVALID_ARG: |r| != log2 length, gens' n != R; SP_ERR_INVALID_SCALAR: r, Zr, blind_Zr or a blind not reduced. */
+int sp_pc_eval_prove_t(sp_ctx* ctx, const sp_pc_gens* gens, const sp_poly* poly, const uint64_t* blinds_mont, const uint64_t* r_mont, size_t ell,
+                       const uint64_t* Zr_mont, const uint64_t* blind_Zr_mont, uint8_t* strobe_state /* in, out */, uint8_t* tape_state /* in, out */,
+                       uint8_t** proof, size_t* proof_len, uint8_t C_Zr32[32], uint64_t Zr_out[4]);
+/* PolyEvalProof::verify(gens, transcript, r, C_Zr, comm) (dense_mlpoly.rs:367-389) when C_Zr32 is given, verify_plain(.., Zr, ..) (:391-404) when
+ * Zr_mont is given (exactly one of them).  comm = bincode(PolyCommitment).  SP_OK = accepted; SP_ERR_VERIFY / SP_ERR_DECOMPRESS = rejected,
+ * sp_last_error names the failing check; the transcript is advanced as the reference's verify advances it, accepted or not (an argument
+ * refused with SP_ERR_INVALID_ARG / SP_ERR_INVALID_SCALAR leaves it untouched).  Needs the device (<s, G>). */
+int sp_pc_eval_verify_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t* comm, size_t comm_len, const uint64_t* r_mont, size_t ell,
+                        const uint8_t C_Zr32[32], const uint64_t Zr_mont[4], uint8_t* strobe_state /* in, out */, const uint8_t* proof, size_t proof_len);
+/* k tables of 2^m entries opened at one point r (m scalars) through one commitment to their merge (sp_pc_commit of the same k tables):
+ * DerefsEvalProof::prove_single (sparse_mlpoly.rs:80-123) without a protocol name (absorb b"Derefs evaluation proof" first to match
+ * DerefsEvalProof::prove).  evals_j = P_j(r) are computed on the device, padded with zeros to k' = next_pow2(k) and absorbed as "evals_ops_val";
+ * log2 k' challenges "challenge_combine_n_to_one" fold them (bound_poly_var_bot, last challenge first) into "joint_claim_eval"; the merge is proved
+ * at (challenges || r) by PolyEvalProof::prove without blind_Zr.  blinds: the joint commitment's L blinds or NULL.  Out: the proof, evals_out =
+ * the k evaluations.  After sp_sumcheck_prove_t over the same tables, r = its r_out and evals_out equals its finals_out.  Errors as sp_pc_commit. */
+int sp_pc_eval_prove_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, sp_poly* const* polys, int k, const uint64_t* blinds_mont, const uint64_t* r_mont,
+                             size_t m, uint8_t* strobe_state /* in, out */, uint8_t* tape_state /* in, out */, uint8_t** proof, size_t* proof_len,
+                             uint64_t* evals_out /* k x 4 */);
+/* DerefsEvalProof::verify_single (sparse_mlpoly.rs:149-176) for sp_pc_eval_prove_joint_t's proof: evals = the k claimed evaluations */
+int sp_pc_eval_verify_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t* comm, size_t comm_len, const uint64_t* r_mont, size_t m,
+                              const uint64_t* evals_mont, int k, uint8_t* strobe_state /* in, out */, const uint8_t* proof, size_t proof_len);
+
 /* ---- inner-product argument, operator level: BulletReductionProof::prove (src/nizk/bullet.rs:32-132) for a host that keeps the transcript and
  * the orchestration.  sp_ipa_begin copies a_vec / b_vec; the generator vector G is `gens` (G[0..n)).  Each round: sp_ipa_round_LR returns the
  * compressed L, R of bullet.rs:83-97 (c_L, c_R are formed inside; Q and H are the caller's points), the host appends them and derives u

@@ -606,6 +606,148 @@ class Transcript:
         return out.raw
 
 
+# ----------------------------------------------------------------------------- polynomial commitments of the caller's tables
+class PolyCommitmentGens:
+    """PolyCommitmentGens::new(num_vars, label) (dense_mlpoly.rs:29-36): the n = 2^(num_vars - num_vars/2) generators of gens_n, G_1 and h of the
+    label's stream, with their device tables (footprint: include/spartan_b200.h, sp_pc_gens_create).  view(num_vars) gives the gens of a smaller
+    num_vars of the same label as a view of these tables."""
+
+    def __init__(self, num_vars, label, ctx=None):
+        self.ctx = ctx or default_context()
+        self.num_vars, self.n = num_vars, 1 << (num_vars - num_vars // 2)
+        h = _vp()
+        self.ctx.check(lib.sp_pc_gens_create(self.ctx.h, _sz(num_vars), C.c_char_p(bytes(label)), _sz(len(label)), C.byref(h)))
+        self.h = h
+
+    def view(self, num_vars):
+        o = PolyCommitmentGens.__new__(PolyCommitmentGens)
+        o.ctx, o.num_vars, o.n = self.ctx, num_vars, 1 << (num_vars - num_vars // 2)
+        h = _vp()
+        self.ctx.check(lib.sp_pc_gens_create_from(self.ctx.h, self.h, _sz(num_vars), C.byref(h)))
+        o.h = h
+        return o
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None):
+                lib.sp_pc_gens_free(self.h)
+                self.h = None
+        except Exception:
+            pass
+
+
+class RandomTape(Transcript):
+    """RandomTape::new(b"proof") (random.rs:10-17) as caller state (a merlin transcript, advanced in place by the calls that draw from it).
+    seed=None draws the seed scalar from the OS, as the reference does; a given seed (Montgomery limbs, e.g. tape_seed(i)) makes every blind a
+    public function of it: byte-parity tests only."""
+
+    def __init__(self, seed=None):
+        s = random_tape_seed() if seed is None else np.ascontiguousarray(seed, dtype=np.uint64).reshape(4)
+        self.state = C.create_string_buffer(203)
+        rc = lib.sp_random_tape_new(_p(s), self.state)
+        if rc != SP_OK:
+            raise SpartanB200Error("spartan_b200 error %d: %s" % (rc, lib.sp_last_error(None).decode()))
+
+
+class PolyCommitment:
+    """dense_mlpoly.rs:38-41: the L compressed row commitments"""
+
+    def __init__(self, C_rows):
+        self.C = list(C_rows)
+
+    def to_bytes(self):
+        """bincode(PolyCommitment)"""
+        return len(self.C).to_bytes(8, "little") + b"".join(self.C)
+
+    @classmethod
+    def from_bytes(cls, data):
+        data = bytes(data)
+        n = int.from_bytes(data[:8], "little")
+        if len(data) != 8 + 32 * n:
+            raise SpartanB200Error("PolyCommitment: %d bytes do not hold %d points" % (len(data), n))
+        return cls([data[8 + 32 * i:40 + 32 * i] for i in range(n)])
+
+    def append_to_transcript(self, label, transcript):
+        """dense_mlpoly.rs:292-300, on a Transcript"""
+        transcript.append_message(label, b"poly_commitment_begin")
+        for c in self.C:
+            transcript.append_message(b"poly_commitment_share", c)
+        transcript.append_message(label, b"poly_commitment_end")
+
+
+def _poly_list(polys):
+    return [polys] if isinstance(polys, DensePolynomial) else list(polys)
+
+
+def _opt_limbs(x):
+    return None if x is None else _p(np.ascontiguousarray(x, dtype=np.uint64))
+
+
+def poly_commit(polys, gens, tape=None):
+    """DensePolynomial::commit(gens, tape) (dense_mlpoly.rs:179-204) of one DensePolynomial, or of DensePolynomial::merge of a list of them
+    (concatenated, zero-padded to a power of two; dense_mlpoly.rs:259-272).  tape: a RandomTape (advanced) or None (no blinds).
+    Returns (PolyCommitment, blinds as (L, 4) Montgomery limbs)."""
+    polys = _poly_list(polys)
+    ctx = gens.ctx
+    k = len(polys)
+    ell = (max(polys[0].len(), 1).bit_length() - 1 + (k - 1).bit_length()) if k else 0   # log2 of the merge's length
+    blinds = np.zeros((1 << (ell // 2), 4), dtype=np.uint64)
+    out, n = C.POINTER(C.c_ubyte)(), _sz()
+    ctx.check(lib.sp_pc_commit(ctx.h, gens.h, _handles(polys), C.c_int(k), tape.state if tape is not None else None, C.byref(out), C.byref(n),
+                               _p(blinds)))
+    return PolyCommitment.from_bytes(_take_bytes(out, n)), blinds
+
+
+class PolyEvalProof:
+    """dense_mlpoly.rs:307-404, plus DerefsEvalProof::prove_single / verify_single (sparse_mlpoly.rs:80-176) as prove_joint / verify_joint.
+    `data` = bincode(PolyEvalProof).  Transcripts: a Transcript (advanced in place) or a label (a fresh Transcript::new(label))."""
+
+    def __init__(self, data):
+        self.data = bytes(data)
+
+    @staticmethod
+    def prove(poly, blinds, r, Zr, blind_Zr, gens, transcript, tape):
+        """PolyEvalProof::prove: returns (proof, C_Zr compressed, Zr limbs).  Zr=None: Z(r), computed on the device; blinds / blind_Zr None: zero"""
+        ctx = poly.ctx
+        t, r = _transcript_state(transcript), _limbs(r)
+        out, n = C.POINTER(C.c_ubyte)(), _sz()
+        c_zr, zr = C.create_string_buffer(32), np.zeros(4, dtype=np.uint64)
+        ctx.check(lib.sp_pc_eval_prove_t(ctx.h, gens.h, poly.h, _opt_limbs(blinds), _p(r), _sz(len(r)), _opt_limbs(Zr), _opt_limbs(blind_Zr), t.state,
+                                         tape.state, C.byref(out), C.byref(n), c_zr, _p(zr)))
+        return PolyEvalProof(_take_bytes(out, n)), c_zr.raw, zr
+
+    def verify(self, gens, transcript, r, C_Zr, comm):
+        """PolyEvalProof::verify against the commitment C_Zr (32 bytes); raises ProofVerifyError"""
+        self._verify(gens, transcript, r, C.c_char_p(bytes(C_Zr)), None, comm)
+
+    def verify_plain(self, gens, transcript, r, Zr, comm):
+        """PolyEvalProof::verify_plain against the evaluation Zr (limbs); raises ProofVerifyError"""
+        self._verify(gens, transcript, r, None, _p(np.ascontiguousarray(Zr, dtype=np.uint64)), comm)
+
+    def _verify(self, gens, transcript, r, c_zr, zr, comm):
+        t, r, cb = _transcript_state(transcript), _limbs(r), comm.to_bytes()
+        gens.ctx.check(lib.sp_pc_eval_verify_t(gens.ctx.h, gens.h, C.c_char_p(cb), _sz(len(cb)), _p(r), _sz(len(r)), c_zr, zr, t.state,
+                                               C.c_char_p(self.data), _sz(len(self.data))))
+
+    @staticmethod
+    def prove_joint(polys, blinds, r, gens, transcript, tape):
+        """k tables opened at one point r through their joint commitment (poly_commit of the same list): returns (proof, evals as (k, 4) limbs)"""
+        polys = _poly_list(polys)
+        ctx = polys[0].ctx
+        t, r = _transcript_state(transcript), _limbs(r)
+        out, n = C.POINTER(C.c_ubyte)(), _sz()
+        evals = np.zeros((len(polys), 4), dtype=np.uint64)
+        ctx.check(lib.sp_pc_eval_prove_joint_t(ctx.h, gens.h, _handles(polys), C.c_int(len(polys)), _opt_limbs(blinds), _p(r), _sz(len(r)), t.state,
+                                               tape.state, C.byref(out), C.byref(n), _p(evals)))
+        return PolyEvalProof(_take_bytes(out, n)), evals
+
+    def verify_joint(self, gens, transcript, r, evals, comm):
+        """DerefsEvalProof::verify_single for prove_joint's proof; raises ProofVerifyError"""
+        t, r, ev, cb = _transcript_state(transcript), _limbs(r), _limbs(evals), comm.to_bytes()
+        gens.ctx.check(lib.sp_pc_eval_verify_joint_t(gens.ctx.h, gens.h, C.c_char_p(cb), _sz(len(cb)), _p(r), _sz(len(r)), _p(ev), C.c_int(len(ev)),
+                                                     t.state, C.c_char_p(self.data), _sz(len(self.data))))
+
+
 # ----------------------------------------------------------------------------- public API of lib.rs
 class Assignment:
     """lib.rs:57-104: a vector of scalars given as canonical 32-byte strings"""

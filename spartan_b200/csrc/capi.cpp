@@ -1108,6 +1108,206 @@ int sp_sumcheck_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, co
   catch (const std::exception& e) { err = e.what(); return SP_ERR_INTERNAL; }
 }
 
+// ---- polynomial commitments and evaluation proofs for the caller's tables (prover.cpp: pc_*).  Every argument is checked before the first
+// launch and before the transcript or the tape is touched, so a refused call leaves the tables, the transcript and the tape as they were.
+}  // extern "C"
+struct sp_pc_gens {
+  Ctx* ctx;
+  std::shared_ptr<GenSet> set;   // shared by the views made from it
+  size_t num_vars;
+  PolyCommitmentGens g;
+};
+// the k tables of one call: non-null handles of this context, of one power-of-two length; returns log2 of it
+static size_t pc_tables(sp_ctx* ctx, sp_poly* const* polys, int k, const std::string& what, std::vector<const u256*>& out) {
+  if (!polys) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL table array");
+  if (k < 1 || k > SP_PC_MAX_TABLES)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": " + std::to_string(k) + " tables; 1 .. SP_PC_MAX_TABLES = " + std::to_string(SP_PC_MAX_TABLES) + " supported");
+  for (int i = 0; i < k; i++) {
+    if (!polys[i]) throw SpError(SP_ERR_INVALID_ARG, what + ": table " + std::to_string(i) + " is NULL");
+    if (polys[i]->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, what + ": table " + std::to_string(i) + " belongs to another context");
+    if (polys[i]->len != polys[0]->len) throw SpError(SP_ERR_INVALID_ARG, what + ": tables differ in length");
+  }
+  const size_t len = polys[0]->len;
+  if (!len || (len & (len - 1))) throw SpError(SP_ERR_INVALID_ARG, what + ": the table length must be a power of two");
+  out.assign(k, nullptr);
+  for (int i = 0; i < k; i++) out[i] = polys[i]->d.p;
+  return log2_ceil(len);
+}
+// gens of this context whose n is the row length R = 2^ceil(ell/2) of a table of 2^ell entries (commitments.rs:87-91 asserts gens_n.n == R)
+static void pc_check_gens(sp_ctx* ctx, const sp_pc_gens* g, size_t ell, const std::string& what) {
+  if (!g) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL gens");
+  if (g->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, what + ": the gens belong to another context");
+  if (g->g.n != pc_gens_n(ell))
+    throw SpError(SP_ERR_INVALID_ARG, what + ": gens for num_vars = " + std::to_string(g->num_vars) + " have n = " + std::to_string(g->g.n) +
+                                          ", a table of 2^" + std::to_string(ell) + " entries needs n = R = " + std::to_string(pc_gens_n(ell)));
+}
+static const size_t PC_MAX_VARS = 60;
+static Transcript pc_tape_open(const uint8_t* tape_state, const std::string& what) {
+  if (!tape_state) throw SpError(SP_ERR_INVALID_ARG, what + ": tape state is NULL");
+  return Transcript(Transcript::FromState(), tape_state);
+}
+extern "C" {
+
+int sp_pc_gens_create(sp_ctx* ctx, size_t num_vars, const uint8_t* label, size_t label_len, sp_pc_gens** out) {
+  SP_TRY(ctx)
+  if (!out || (!label && label_len)) throw SpError(SP_ERR_INVALID_ARG, "pc_gens_create: NULL argument");
+  if (num_vars > PC_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, "pc_gens_create: num_vars = " + std::to_string(num_vars) + " > " + std::to_string(PC_MAX_VARS));
+  const size_t n = pc_gens_n(num_vars);
+  std::unique_ptr<sp_pc_gens> g(new sp_pc_gens{&ctx->c, nullptr, num_vars, {}});
+  g->set = std::make_shared<GenSet>(&ctx->c, std::string((const char*)label, label_len), n + 2, std::vector<size_t>{n, n + 1});
+  g->g = pc_gens_view(*g->set, num_vars);
+  *out = g.release();
+  SP_CATCH(ctx)
+}
+int sp_pc_gens_create_from(sp_ctx* ctx, const sp_pc_gens* larger, size_t num_vars, sp_pc_gens** out) {
+  SP_TRY(ctx)
+  if (!larger || !out) throw SpError(SP_ERR_INVALID_ARG, "pc_gens_create_from: NULL argument");
+  if (larger->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, "pc_gens_create_from: the gens belong to another context");
+  if (num_vars > larger->num_vars)
+    throw SpError(SP_ERR_INVALID_ARG, "pc_gens_create_from: num_vars = " + std::to_string(num_vars) + " > the larger gens' " + std::to_string(larger->num_vars));
+  std::unique_ptr<sp_pc_gens> g(new sp_pc_gens{&ctx->c, larger->set, num_vars, {}});
+  g->g = pc_gens_view(*g->set, num_vars);
+  *out = g.release();
+  SP_CATCH(ctx)
+}
+void sp_pc_gens_free(sp_pc_gens* g) { delete g; }
+
+// host only: no context
+int sp_random_tape_new(const uint64_t seed[4], uint8_t* tape_state) {
+  try {
+    if (!seed || !tape_state) throw SpError(SP_ERR_INVALID_ARG, "random_tape_new: NULL argument");
+    require_reduced(seed, 1, "random_tape_new: seed");
+    RandomTape(std::string("proof"), fq_in(seed)).state().export_state(tape_state);   // random.rs:10-17
+    return SP_OK;
+  } catch (const SpError& e) { g_create_error = e.what(); return e.code; }
+}
+
+int sp_pc_commit(sp_ctx* ctx, const sp_pc_gens* gens, sp_poly* const* polys, int k, uint8_t* tape_state, uint8_t** comm, size_t* comm_len, uint64_t* blinds_out) {
+  SP_TRY(ctx)
+  const std::string what = "pc_commit";
+  if (!comm || !comm_len) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  std::vector<const u256*> t;
+  const size_t m = pc_tables(ctx, polys, k, what, t), ell = m + log2_ceil(next_pow2((size_t)k));
+  pc_check_gens(ctx, gens, ell, what);
+  const size_t L = (size_t)1 << (ell / 2);
+  std::vector<Fq> blinds(L, Fq::zero());
+  std::unique_ptr<RandomTape> tape;
+  if (tape_state) {
+    tape.reset(new RandomTape(pc_tape_open(tape_state, what)));
+    blinds = tape->random_vector("poly_blinds", L);   // dense_mlpoly.rs:185-189
+  }
+  const std::vector<uint8_t> bytes = to_bincode(pc_commit(ctx->c, gens->g, t.data(), k, m, tape ? blinds.data() : nullptr));
+  if (tape) tape->state().export_state(tape_state);
+  *comm = dup_bytes(bytes); *comm_len = bytes.size();
+  if (blinds_out) for (size_t i = 0; i < L; i++) fq_out(blinds_out + 4 * i, blinds[i]);
+  SP_CATCH(ctx)
+}
+
+int sp_pc_eval_prove_t(sp_ctx* ctx, const sp_pc_gens* gens, const sp_poly* poly, const uint64_t* blinds, const uint64_t* r, size_t ell, const uint64_t* Zr,
+                       const uint64_t* blind_Zr, uint8_t* strobe_state, uint8_t* tape_state, uint8_t** proof, size_t* proof_len, uint8_t C_Zr32[32],
+                       uint64_t Zr_out[4]) {
+  SP_TRY(ctx)
+  const std::string what = "pc_eval_prove";
+  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+  ta.check();
+  if (!poly || !proof || !proof_len || !C_Zr32 || !Zr_out || (!r && ell)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  sp_poly* const p = const_cast<sp_poly*>(poly);
+  std::vector<const u256*> t;
+  if (pc_tables(ctx, &p, 1, what, t) != ell || ell > PC_MAX_VARS)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(ell) + " but the table has " + std::to_string(poly->len) + " entries");
+  pc_check_gens(ctx, gens, ell, what);
+  const size_t L = (size_t)1 << (ell / 2);
+  require_reduced(r, ell, "pc_eval_prove: r");
+  if (Zr) require_reduced(Zr, 1, "pc_eval_prove: Zr");
+  if (blind_Zr) require_reduced(blind_Zr, 1, "pc_eval_prove: blind_Zr");
+  if (blinds) require_reduced(blinds, L, "pc_eval_prove: blinds");
+  RandomTape tape(pc_tape_open(tape_state, what));
+  Transcript T = ta.open();
+  const std::vector<Fq> bl = blinds ? fq_vec(blinds, L) : std::vector<Fq>();
+  const Fq Zr_in = Zr ? fq_in(Zr) : Fq::zero(), bZr = blind_Zr ? fq_in(blind_Zr) : Fq::zero();
+  PolyEvalProof P;
+  Cp C;
+  Fq zr;
+  polyeval_prove(ctx->c, poly->d.p, blinds ? &bl : nullptr, fq_vec(r, ell), Zr ? &Zr_in : nullptr, blind_Zr ? &bZr : nullptr, gens->g, T, tape, P, C, &zr);
+  ta.close(T);
+  tape.state().export_state(tape_state);
+  const std::vector<uint8_t> bytes = to_bincode(P);
+  *proof = dup_bytes(bytes); *proof_len = bytes.size();
+  memcpy(C_Zr32, C.b, 32);
+  fq_out(Zr_out, zr);
+  SP_CATCH(ctx)
+}
+
+int sp_pc_eval_verify_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t* comm, size_t comm_len, const uint64_t* r, size_t ell, const uint8_t C_Zr32[32],
+                        const uint64_t Zr[4], uint8_t* strobe_state, const uint8_t* proof, size_t proof_len) {
+  SP_TRY(ctx)
+  const std::string what = "pc_eval_verify";
+  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+  ta.check();
+  if ((!comm && comm_len) || (!proof && proof_len) || (!r && ell)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  if (!C_Zr32 == !Zr) throw SpError(SP_ERR_INVALID_ARG, what + ": give exactly one of C_Zr and Zr");
+  if (ell > PC_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(ell) + " > " + std::to_string(PC_MAX_VARS));
+  pc_check_gens(ctx, gens, ell, what);
+  require_reduced(r, ell, "pc_eval_verify: r");
+  if (Zr) require_reduced(Zr, 1, "pc_eval_verify: Zr");
+  const PolyCommitment pc = from_bincode<PolyCommitment>(comm, comm_len, SP_ERR_INVALID_ARG, "polynomial commitment");
+  Cp c;
+  if (C_Zr32) memcpy(c.b, C_Zr32, 32);
+  const Fq zr = Zr ? fq_in(Zr) : Fq::zero();
+  Transcript T = ta.open();
+  TranscriptClose close{ta, T};
+  pc_eval_verify(ctx->c, gens->g, pc, fq_vec(r, ell), C_Zr32 ? &c : nullptr, Zr ? &zr : nullptr, T, proof, proof_len);
+  SP_CATCH(ctx)
+}
+
+int sp_pc_eval_prove_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, sp_poly* const* polys, int k, const uint64_t* blinds, const uint64_t* r, size_t m,
+                             uint8_t* strobe_state, uint8_t* tape_state, uint8_t** proof, size_t* proof_len, uint64_t* evals_out) {
+  SP_TRY(ctx)
+  const std::string what = "pc_eval_prove_joint";
+  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+  ta.check();
+  if (!proof || !proof_len || !evals_out || (!r && m)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  std::vector<const u256*> t;
+  if (pc_tables(ctx, polys, k, what, t) != m || m > PC_MAX_VARS)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(m) + " but the tables have " + std::to_string(polys[0]->len) + " entries");
+  const size_t ell = m + log2_ceil(next_pow2((size_t)k)), L = (size_t)1 << (ell / 2);
+  pc_check_gens(ctx, gens, ell, what);
+  require_reduced(r, m, "pc_eval_prove_joint: r");
+  if (blinds) require_reduced(blinds, L, "pc_eval_prove_joint: blinds");
+  RandomTape tape(pc_tape_open(tape_state, what));
+  Transcript T = ta.open();
+  const std::vector<Fq> bl = blinds ? fq_vec(blinds, L) : std::vector<Fq>();
+  PolyEvalProof P;
+  std::vector<Fq> evals;
+  pc_eval_prove_joint(ctx->c, gens->g, t.data(), k, fq_vec(r, m), blinds ? &bl : nullptr, T, tape, P, evals);
+  ta.close(T);
+  tape.state().export_state(tape_state);
+  const std::vector<uint8_t> bytes = to_bincode(P);
+  *proof = dup_bytes(bytes); *proof_len = bytes.size();
+  for (int j = 0; j < k; j++) fq_out(evals_out + 4 * j, evals[j]);
+  SP_CATCH(ctx)
+}
+
+int sp_pc_eval_verify_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t* comm, size_t comm_len, const uint64_t* r, size_t m, const uint64_t* evals,
+                              int k, uint8_t* strobe_state, const uint8_t* proof, size_t proof_len) {
+  SP_TRY(ctx)
+  const std::string what = "pc_eval_verify_joint";
+  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+  ta.check();
+  if ((!comm && comm_len) || (!proof && proof_len) || (!r && m) || !evals) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  if (k < 1 || k > SP_PC_MAX_TABLES)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": " + std::to_string(k) + " evaluations; 1 .. SP_PC_MAX_TABLES = " + std::to_string(SP_PC_MAX_TABLES) + " supported");
+  if (m > PC_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(m) + " > " + std::to_string(PC_MAX_VARS));
+  pc_check_gens(ctx, gens, m + log2_ceil(next_pow2((size_t)k)), what);
+  require_reduced(r, m, "pc_eval_verify_joint: r");
+  require_reduced(evals, (size_t)k, "pc_eval_verify_joint: evals");
+  const PolyCommitment pc = from_bincode<PolyCommitment>(comm, comm_len, SP_ERR_INVALID_ARG, "polynomial commitment");
+  Transcript T = ta.open();
+  TranscriptClose close{ta, T};
+  pc_eval_verify_joint(ctx->c, gens->g, pc, fq_vec(r, m), fq_vec(evals, (size_t)k), T, proof, proof_len);
+  SP_CATCH(ctx)
+}
+
 // ---- batch verifiers: proof i is checked as the single call would check it (statement i, inputs i, label i or caller transcript i); the group
 // equations of all of them are tested in one device pass (verifier.cpp, DESIGN.md "deferred checks")
 struct BatchArgs {

@@ -149,6 +149,10 @@ void dot(u256* out, const u256* a, const u256* b, size_t n, void* scratch, cudaS
 void dot_many(u256* out, const u256* const* a_list, int count, const u256* b, size_t n, void* scratch, cudaStream_t s);
 void dot3(u256* out, const u256* a, const u256* b, const u256* c, size_t n, void* scratch, cudaStream_t s);
 void bound_rows(u256* out, const u256* Z, const u256* L, size_t L_size, size_t R_size, u256* scratch /* >= 64*R_size */, cudaStream_t s);
+// out[j * R_size + i] = sum_r L[r] * tables[j][r * R_size + i] for k <= SP_PC_MAX_TABLES tables of L_size x R_size entries: bound_rows of every
+// table, each table read once, in one launch (plus a sum of the slabs when the rows are split)
+size_t bound_rows_many_scratch(int k, size_t L_size, size_t R_size);   // scalars
+void bound_rows_many(u256* out, const u256* const* tables, int k, const u256* L, size_t L_size, size_t R_size, u256* scratch, cudaStream_t s);
 void lincomb3(u256* out, const u256* A, const u256* B, const u256* C, const u256* d_rabc /*3*/, size_t n, cudaStream_t s);
 void hadamard_many(u256* const* outs, const u256* const* as, const u256* const* bs, int count, size_t n, cudaStream_t s);
 void to_canonical(u256* out, const u256* in, size_t n, cudaStream_t s);   // Montgomery -> canonical little-endian integers (transcript bytes)
@@ -233,6 +237,16 @@ size_t msm_scratch_bytes(size_t L, size_t R);
 // latency-bound work leaves them room)
 void msm_rows(ge* out, const ge_niels* table, int wbits, const ge_niels* row_table, const u256* scalars, size_t stride, size_t L, size_t R,
               const u256* blinds, size_t blind_base, void* scratch, cudaStream_t s, size_t smem_pad = 0);
+// The table-list form: row i of the L rows is row i % rows_per_table of table t[i / rows_per_table] (row_len = R scalars per row, rows back to
+// back); the rows of tables at or past ntables are zero and are not read, so they give the identity, or blinds[i] * G_blind_base alone.  The
+// rows of k tables concatenated and zero-padded (DensePolynomial::merge) without a copy.  Same kernels, scratch and launch shapes as msm_rows.
+struct TableRows {
+  const u256* t[SP_PC_MAX_TABLES];
+  int ntables;
+  size_t rows_per_table, row_len;
+};
+void msm_rows_tables(ge* out, const ge_niels* table, int wbits, const ge_niels* row_table, const TableRows& tr, size_t L, size_t R, const u256* blinds,
+                     size_t blind_base, void* scratch, cudaStream_t s);
 
 void add_points(ge* a, const ge* b, size_t n, cudaStream_t s);   // a[i] += b[i]
 void sum_points(ge* out, const ge* in, int n, cudaStream_t s);   // out[0] = in[0] + ... + in[n-1], n <= 32

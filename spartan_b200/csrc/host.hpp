@@ -241,6 +241,9 @@ class Transcript {  // merlin::Transcript + ProofTranscript (transcript.rs:5-37)
 class RandomTape {  // random.rs:6-28; the OsRng seed scalar is an explicit input here (SURVEY.md §8d)
  public:
   RandomTape(const std::string& name, const Fq& seed) : tape_(name) { tape_.append_scalar("init_randomness", seed); }
+  // a tape is a merlin transcript: the caller's tape crosses the C ABI as its STROBE state, like a transcript
+  explicit RandomTape(const Transcript& state) : tape_(state) {}
+  const Transcript& state() const { return tape_; }
   Fq random_scalar(const char* label) { return tape_.challenge_scalar(label); }
   std::vector<Fq> random_vector(const char* label, size_t n) { return tape_.challenge_vector(label, n); }
 

@@ -393,6 +393,47 @@ void bound_rows(u256* out, const u256* Z, const u256* L, size_t L_size, size_t R
   k_sum_slabs<<<(unsigned)((R_size + 127) / 128), 128, 0, s>>>(out, scratch, R_size, nslabs);
   SP_LAUNCHED(); SP_LAUNCHED(); check("bound_rows");
 }
+// bound_rows of k tables against one L in one pass over the tables: blockIdx.z is the table, and table j's partial sums of slab y land at
+// part[(y * k + j) * R_size + i], so that k_sum_slabs over k * R_size entries leaves table j's result at out[j * R_size ..]
+struct TablePtrs { const u256* t[SP_PC_MAX_TABLES]; };
+__global__ void __launch_bounds__(128) k_bound_rows_many(u256* part, TablePtrs tp, const u256* __restrict__ L, size_t L_size, size_t R_size,
+                                                        size_t rows_per_slab) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= R_size) return;
+  const u256* __restrict__ Z = tp.t[blockIdx.z];
+  const size_t j0 = (size_t)blockIdx.y * rows_per_slab, j1 = j0 + rows_per_slab < L_size ? j0 + rows_per_slab : L_size;
+  u256 acc = fq_zero();
+  for (size_t j = j0; j < j1; j++) acc = fq_add(acc, fq_mul(ld256_ro(L + j), ld256_ro(Z + j * R_size + i)));
+  st256(part + ((size_t)blockIdx.y * gridDim.z + blockIdx.z) * R_size + i, acc);
+}
+// enough slabs for about 16 CTAs per SM over all tables, at most 64 and at most one per row
+static size_t bound_rows_many_slabs(int k, size_t L_size, size_t R_size) {
+  const size_t blocks = ((R_size + 127) / 128) * (size_t)k, want = (size_t)sm_count() * 16;
+  size_t nslabs = std::min<size_t>(std::min<size_t>((want + blocks - 1) / blocks, 64), L_size);
+  nslabs = std::max<size_t>(nslabs, 1);
+  const size_t rows_per_slab = (L_size + nslabs - 1) / nslabs;
+  return (L_size + rows_per_slab - 1) / rows_per_slab;
+}
+size_t bound_rows_many_scratch(int k, size_t L_size, size_t R_size) {
+  const size_t nslabs = bound_rows_many_slabs(k, L_size, R_size);
+  return nslabs > 1 ? nslabs * (size_t)k * R_size : 1;
+}
+void bound_rows_many(u256* out, const u256* const* tables, int k, const u256* L, size_t L_size, size_t R_size, u256* scratch, cudaStream_t s) {
+  ProfScope ps("bound_rows_many", 32.0 * (double)k * (double)L_size * (double)R_size, s);
+  if (k < 1 || k > SP_PC_MAX_TABLES) throw std::runtime_error("spartan_b200: bound_rows_many supports 1 .. SP_PC_MAX_TABLES tables");
+  TablePtrs tp;
+  for (int j = 0; j < k; j++) tp.t[j] = tables[j];
+  const size_t nslabs = bound_rows_many_slabs(k, L_size, R_size), rows_per_slab = (L_size + nslabs - 1) / nslabs;
+  const unsigned bx = (unsigned)((R_size + 127) / 128);
+  k_bound_rows_many<<<dim3(bx, (unsigned)nslabs, (unsigned)k), 128, 0, s>>>(nslabs > 1 ? scratch : out, tp, L, L_size, R_size, rows_per_slab);
+  SP_LAUNCHED();
+  if (nslabs > 1) {
+    const size_t n = (size_t)k * R_size;
+    k_sum_slabs<<<(unsigned)((n + 127) / 128), 128, 0, s>>>(out, scratch, n, (int)nslabs);
+    SP_LAUNCHED();
+  }
+  check("bound_rows_many");
+}
 
 __global__ void k_lincomb3(u256* out, const u256* __restrict__ A, const u256* __restrict__ B, const u256* __restrict__ C,
                            const u256* __restrict__ rabc, size_t n) {
@@ -628,9 +669,30 @@ __device__ __forceinline__ ge block_sum_ge_128(ge acc) {
   if (threadIdx.x == 0) { acc = ge_add(acc, sm[1]); acc = ge_add(acc, ge_add(sm[2], sm[3])); }
   return acc;
 }
-template <int WBITS, int GROUPS, int CPT>
-__global__ void __launch_bounds__(128, 4) k_msm_rows(ge* partial, const ge_niels* __restrict__ table, const u256* __restrict__ scalars, size_t stride,
-                                                     size_t R, const u256* __restrict__ blinds, size_t blind_base) {
+// Where the MSM's rows come from.  RowStride: row r at scalars + r * stride.  RowTables (dev::TableRows): row r is row r % rows_per_table of
+// table r / rows_per_table; the rows of tables at or past ntables are zero and are never read (PADDED: row() may return null for them).
+struct RowStride {
+  const u256* scalars;
+  size_t stride;
+  static constexpr bool PADDED = false;
+  __device__ __forceinline__ const u256* row(size_t r) const { return scalars + r * stride; }
+  RowStride skip(size_t rows) const { return RowStride{scalars + rows * stride, stride}; }
+};
+struct RowTables {
+  const u256* t[SP_PC_MAX_TABLES];
+  int ntables, rpt_log, len_log;   // rows per table and scalars per row are powers of two: shifts, no division in the kernels
+  size_t first;                    // rows skipped by the launch's grid (gridDim.y limit)
+  static constexpr bool PADDED = true;
+  __device__ __forceinline__ const u256* row(size_t r) const {
+    r += first;
+    const size_t j = r >> rpt_log;
+    return j < (size_t)ntables ? t[j] + ((r - (j << rpt_log)) << len_log) : nullptr;
+  }
+  RowTables skip(size_t rows) const { RowTables o = *this; o.first += rows; return o; }
+};
+template <int WBITS, int GROUPS, int CPT, class Src>
+__global__ void __launch_bounds__(128, 4) k_msm_rows(ge* partial, const ge_niels* __restrict__ table, const Src src, size_t R,
+                                                     const u256* __restrict__ blinds, size_t blind_base) {
   constexpr int NWIN = (253 + WBITS - 1) / WBITS;
   constexpr int WPT = (NWIN + GROUPS - 1) / GROUPS;   // windows per thread
   constexpr int COLS = 128 / GROUPS;                  // columns per block per pass; CPT passes amortise the reduction tree
@@ -646,8 +708,11 @@ __global__ void __launch_bounds__(128, 4) k_msm_rows(ge* partial, const ge_niels
     if (col >= ncols) break;
     u256 k;
     size_t base;
-    if (col < R) { k = ld256_ro(scalars + row * stride + col); base = col; }
-    else { k = ld256_ro(blinds + row); base = blind_base; }
+    if (col < R) {
+      const u256* rp = src.row(row);
+      if (Src::PADDED && !rp) continue;
+      k = ld256_ro(rp + col); base = col;
+    } else { k = ld256_ro(blinds + row); base = blind_base; }
     if (fq_is_zero(k)) continue;
     k = fq_from_mont(k);  // group.rs:110-113: scalars leave Montgomery form before the MSM
     // carry into this thread's first window from the signed recoding of the lower windows
@@ -871,11 +936,16 @@ void ipa_msm(ge* out, const ge_niels* table, int wbits, const u256* a, const u25
 // MSM runs on the background stream: a kernel of the prover's stream that does not fit beside the resident MSM CTAs starts only when some of them
 // retire, and one lane owning a whole 4096-column row (256 additions) delayed the inner-product rounds running beside it by 2 ms per proof.
 // The doubling tail runs quad_dbl (quad.cuh).
-__global__ void __launch_bounds__(128) k_msm_digits(int* digits, const u256* __restrict__ scalars, size_t stride, size_t L, size_t R, const u256* __restrict__ blinds) {
+template <class Src>
+__global__ void __launch_bounds__(128) k_msm_digits(int* digits, const Src src, size_t L, size_t R, const u256* __restrict__ blinds) {
   const size_t ncols = R + (blinds ? 1 : 0);
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < L * ncols; i += (size_t)gridDim.x * blockDim.x) {
     const size_t row = i / ncols, col = i - row * ncols;
-    u256 k = col < R ? ld256_ro(scalars + row * stride + col) : ld256_ro(blinds + row);
+    u256 k;
+    if (col < R) {
+      const u256* rp = src.row(row);
+      k = Src::PADDED && !rp ? fq_zero() : ld256_ro(rp + col);
+    } else k = ld256_ro(blinds + row);
     int* dst = digits + row * ROW_NWIN * ncols + col;
     const bool zero = fq_is_zero(k);
     if (!zero) k = fq_from_mont(k);  // group.rs:110-113: scalars leave Montgomery form before the MSM
@@ -936,13 +1006,14 @@ __global__ void __launch_bounds__(32) k_msm_horner(ge* out, const ge* __restrict
 static size_t row_msm_chunks(size_t ncols) { return (ncols + ROW_CHUNK - 1) / ROW_CHUNK; }
 static size_t row_msm_points_bytes(size_t L, size_t ncols) { return (L * ROW_NWIN * (row_msm_chunks(ncols) + 1) * sizeof(ge) + 255) / 256 * 256; }
 static size_t row_msm_scratch_bytes(size_t L, size_t ncols) { return row_msm_points_bytes(L, ncols) + L * ROW_NWIN * ncols * sizeof(int); }
-static void msm_rows_win(ge* out, const ge_niels* rt, const u256* scalars, size_t stride, size_t L, size_t R, const u256* blinds, size_t blind_base,
-                         void* scratch, cudaStream_t s, size_t smem_pad) {
+template <class Src>
+static void msm_rows_win(ge* out, const ge_niels* rt, const Src& src, size_t L, size_t R, const u256* blinds, size_t blind_base, void* scratch,
+                         cudaStream_t s, size_t smem_pad) {
   const size_t ncols = R + (blinds ? 1 : 0), groups = L * ROW_NWIN, chunks = row_msm_chunks(ncols);
   ge* sums = (ge*)scratch;
   ge* part = sums + groups;
   int* digits = (int*)((char*)scratch + row_msm_points_bytes(L, ncols));
-  k_msm_digits<<<grid_for(L * ncols, 128, 16), 128, 0, s>>>(digits, scalars, stride, L, R, blinds);
+  k_msm_digits<<<grid_for(L * ncols, 128, 16), 128, 0, s>>>(digits, src, L, R, blinds);
   if (smem_pad > (48u << 10)) cudaFuncSetAttribute(k_msm_win, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pad);
   k_msm_win<<<dim3((unsigned)((groups + 31) / 32), (unsigned)chunks), 128, smem_pad, s>>>(part, rt, digits, groups, ncols, R, blind_base);
   k_msm_chunks<<<(unsigned)((groups + 127) / 128), 128, 0, s>>>(sums, part, groups, (int)chunks);
@@ -972,31 +1043,31 @@ size_t msm_scratch_bytes(size_t L, size_t R) {
   const size_t per_window = L * msm_chunks(R + 1, 8, 1) * sizeof(ge);
   return msm_rows_use_row_table(L, R) ? std::max(per_window, row_msm_scratch_bytes(L, R + 1)) : per_window;
 }
-template <int WBITS, int GROUPS>
-static void msm_launch2(int cpt, dim3 grid, cudaStream_t s, ge* pp, const ge_niels* table, const u256* sc, size_t stride, size_t R, const u256* bl,
-                        size_t blind_base, size_t smem_pad) {
+template <int WBITS, int GROUPS, class Src>
+static void msm_launch2(int cpt, dim3 grid, cudaStream_t s, ge* pp, const ge_niels* table, const Src& src, size_t R, const u256* bl, size_t blind_base,
+                        size_t smem_pad) {
   // smem_pad: unused dynamic shared memory that only lowers the number of resident CTAs per SM (a background MSM leaves room for the
   // latency-bound kernels of the main stream)
   if (cpt == 4) {
-    if (smem_pad > (48u << 10)) cudaFuncSetAttribute(k_msm_rows<WBITS, GROUPS, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pad);
-    k_msm_rows<WBITS, GROUPS, 4><<<grid, 128, smem_pad, s>>>(pp, table, sc, stride, R, bl, blind_base);
+    if (smem_pad > (48u << 10)) cudaFuncSetAttribute(k_msm_rows<WBITS, GROUPS, 4, Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pad);
+    k_msm_rows<WBITS, GROUPS, 4, Src><<<grid, 128, smem_pad, s>>>(pp, table, src, R, bl, blind_base);
   } else {
-    if (smem_pad > (48u << 10)) cudaFuncSetAttribute(k_msm_rows<WBITS, GROUPS, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pad);
-    k_msm_rows<WBITS, GROUPS, 1><<<grid, 128, smem_pad, s>>>(pp, table, sc, stride, R, bl, blind_base);
+    if (smem_pad > (48u << 10)) cudaFuncSetAttribute(k_msm_rows<WBITS, GROUPS, 1, Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pad);
+    k_msm_rows<WBITS, GROUPS, 1, Src><<<grid, 128, smem_pad, s>>>(pp, table, src, R, bl, blind_base);
   }
 }
-template <int WBITS>
-static void msm_launch(int groups, int cpt, dim3 grid, cudaStream_t s, ge* pp, const ge_niels* table, const u256* sc, size_t stride, size_t R, const u256* bl,
+template <int WBITS, class Src>
+static void msm_launch(int groups, int cpt, dim3 grid, cudaStream_t s, ge* pp, const ge_niels* table, const Src& src, size_t R, const u256* bl,
                        size_t blind_base, size_t smem_pad) {
-  if (groups == 1) msm_launch2<WBITS, 1>(cpt, grid, s, pp, table, sc, stride, R, bl, blind_base, smem_pad);
-  else if (groups == 4) msm_launch2<WBITS, 4>(cpt, grid, s, pp, table, sc, stride, R, bl, blind_base, smem_pad);
-  else msm_launch2<WBITS, 8>(cpt, grid, s, pp, table, sc, stride, R, bl, blind_base, smem_pad);
+  if (groups == 1) msm_launch2<WBITS, 1>(cpt, grid, s, pp, table, src, R, bl, blind_base, smem_pad);
+  else if (groups == 4) msm_launch2<WBITS, 4>(cpt, grid, s, pp, table, src, R, bl, blind_base, smem_pad);
+  else msm_launch2<WBITS, 8>(cpt, grid, s, pp, table, src, R, bl, blind_base, smem_pad);
 }
-void msm_rows(ge* out, const ge_niels* table, int wbits, const ge_niels* row_table, const u256* scalars, size_t stride, size_t L, size_t R,
-              const u256* blinds, size_t blind_base, void* scratch, cudaStream_t s, size_t smem_pad) {
-  ProfScope ps("msm_rows", 32.0 * (double)L * (double)R + 32.0 * (double)R, s);
+template <class Src>
+static void msm_rows_src(ge* out, const ge_niels* table, int wbits, const ge_niels* row_table, const Src& src, size_t L, size_t R, const u256* blinds,
+                         size_t blind_base, void* scratch, cudaStream_t s, size_t smem_pad) {
   if (row_table && msm_rows_use_row_table(L, R)) {
-    msm_rows_win(out, row_table, scalars, stride, L, R, blinds, blind_base, scratch, s, smem_pad);
+    msm_rows_win(out, row_table, src, L, R, blinds, blind_base, scratch, s, smem_pad);
     return;
   }
   const size_t ncols = R + (blinds ? 1 : 0);
@@ -1007,18 +1078,37 @@ void msm_rows(ge* out, const ge_niels* table, int wbits, const ge_niels* row_tab
   for (size_t row0 = 0; row0 < L; row0 += 32768) {   // gridDim.y limit 65535
     size_t rows = L - row0 < 32768 ? L - row0 : 32768;
     dim3 grid((unsigned)chunks, (unsigned)rows);
-    const u256* sc = scalars + row0 * stride;
+    const Src sc = src.skip(row0);
     const u256* bl = blinds ? blinds + row0 : nullptr;
     ge* pp = partial + row0 * chunks;
-    if (wbits == 8) msm_launch<8>(groups, cpt, grid, s, pp, table, sc, stride, R, bl, blind_base, smem_pad);
-    else if (wbits == 13) msm_launch<13>(groups, cpt, grid, s, pp, table, sc, stride, R, bl, blind_base, smem_pad);
-    else if (wbits == 15) msm_launch<15>(groups, cpt, grid, s, pp, table, sc, stride, R, bl, blind_base, smem_pad);
+    if (wbits == 8) msm_launch<8>(groups, cpt, grid, s, pp, table, sc, R, bl, blind_base, smem_pad);
+    else if (wbits == 13) msm_launch<13>(groups, cpt, grid, s, pp, table, sc, R, bl, blind_base, smem_pad);
+    else if (wbits == 15) msm_launch<15>(groups, cpt, grid, s, pp, table, sc, R, bl, blind_base, smem_pad);
     else throw std::runtime_error("spartan_b200: unsupported MSM window width");
     SP_LAUNCHED();
   }
   if (chunks <= 32) k_msm_reduce_small<<<(unsigned)L, 32, 0, s>>>(out, partial, (int)chunks);
   else k_msm_reduce<<<(unsigned)L, 128, 0, s>>>(out, partial, (int)chunks);
   SP_LAUNCHED(); check("msm_rows");
+}
+void msm_rows(ge* out, const ge_niels* table, int wbits, const ge_niels* row_table, const u256* scalars, size_t stride, size_t L, size_t R,
+              const u256* blinds, size_t blind_base, void* scratch, cudaStream_t s, size_t smem_pad) {
+  ProfScope ps("msm_rows", 32.0 * (double)L * (double)R + 32.0 * (double)R, s);
+  msm_rows_src(out, table, wbits, row_table, RowStride{scalars, stride}, L, R, blinds, blind_base, scratch, s, smem_pad);
+}
+void msm_rows_tables(ge* out, const ge_niels* table, int wbits, const ge_niels* row_table, const TableRows& tr, size_t L, size_t R, const u256* blinds,
+                     size_t blind_base, void* scratch, cudaStream_t s) {
+  // only the rows of the tables are read: 32 bytes per scalar of ntables * rows_per_table rows, plus the generators' R
+  ProfScope ps("msm_rows_tables", 32.0 * (double)std::min<size_t>(L, (size_t)tr.ntables * tr.rows_per_table) * (double)R + 32.0 * (double)R, s);
+  const bool pow2 = tr.rows_per_table && !(tr.rows_per_table & (tr.rows_per_table - 1)) && R && !(R & (R - 1));
+  if (tr.row_len != R || tr.ntables < 1 || tr.ntables > SP_PC_MAX_TABLES || !pow2) throw std::runtime_error("spartan_b200: msm_rows_tables: inconsistent table list");
+  RowTables src;
+  for (int j = 0; j < tr.ntables; j++) src.t[j] = tr.t[j];
+  src.ntables = tr.ntables;
+  src.rpt_log = __builtin_ctzll(tr.rows_per_table);
+  src.len_log = __builtin_ctzll(R);
+  src.first = 0;
+  msm_rows_src(out, table, wbits, row_table, src, L, R, blinds, blind_base, scratch, s, 0);
 }
 
 }  // namespace dev

@@ -806,8 +806,8 @@ static void dotproduct_log_prove(Ctx& ctx, const PolyCommitmentGens& gens, Trans
 }
 
 // PolyEvalProof::prove (dense_mlpoly.rs:312-365).  d_Z: device table of 2^|r| scalars (read-only).
-void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt, const std::vector<Fq>& r, const Fq& Zr, const Fq* blind_Zr_opt,
-                           const PolyCommitmentGens& gens, Transcript& T, RandomTape& tape, PolyEvalProof& proof, Cp& C_Zr) {
+void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt, const std::vector<Fq>& r, const Fq* Zr, const Fq* blind_Zr_opt,
+                    const PolyCommitmentGens& gens, Transcript& T, RandomTape& tape, PolyEvalProof& proof, Cp& C_Zr, Fq* Zr_out) {
   T.append_protocol_name("polynomial evaluation proof");
   FineTimer fp(ctx, "polyeval pre (eq, bound_rows)");
   size_t ell = r.size(), lv = ell / 2;
@@ -821,6 +821,13 @@ void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt
   std::vector<uint8_t> a_canon(32 * R_size);
   dev::d2h(a_canon.data(), d_Rc.p, 32 * R_size, ctx.stream);
   dev::bound_rows(d_LZ.p, d_Z, d_L.p, L_size, R_size, tmp.p, ctx.stream);  // DensePolynomial::bound (dense_mlpoly.rs:206-213)
+  Fq Zr_dev;
+  if (!Zr) {   // Z(r) = <bound(Z, L), R>: the bound rows already hold everything Z contributes
+    dev::dot(ctx.small.p + layout::SMALL_DOT.off, d_LZ.p, d_R.p, R_size, ctx.red.p, ctx.stream);
+    ctx.get_small(layout::SMALL_DOT.off, &Zr_dev, 1);
+  }
+  const Fq& Zr_used = Zr ? *Zr : Zr_dev;
+  if (Zr_out) *Zr_out = Zr_used;
   Fq LZ_blind = Fq::zero();
   if (blinds_opt) {
     std::vector<Fq> Lev = ctx.download(d_L.p, L_size);
@@ -829,7 +836,112 @@ void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt
   ctx.sync();
   Fq blind_Zr = blind_Zr_opt ? *blind_Zr_opt : Fq::zero();
   fp.stop();
-  dotproduct_log_prove(ctx, gens, T, tape, d_LZ.p, LZ_blind, d_R.p, a_canon, Zr, blind_Zr, proof.proof, C_Zr);
+  dotproduct_log_prove(ctx, gens, T, tape, d_LZ.p, LZ_blind, d_R.p, a_canon, Zr_used, blind_Zr, proof.proof, C_Zr);
+}
+
+// ================================================================================================ the caller's tables (sp_pc_*)
+PolyCommitmentGens pc_gens_view(GenSet& set, size_t num_vars) {
+  const size_t n = pc_gens_n(num_vars);
+  if (set.nbases < n + 2)
+    throw SpError(SP_ERR_INVALID_ARG, "PolyCommitmentGens for num_vars = " + std::to_string(num_vars) + " needs " + std::to_string(n + 2) + " generators, the set has " +
+                                          std::to_string(set.nbases));
+  set.add_host_tables({n, n + 1});
+  PolyCommitmentGens g;   // DotProductProofGens::new (nizk/mod.rs:414-418): MultiCommitGens::new(n + 1, label).split_at(n)
+  g.n = n;
+  g.gens_n = CommitKey{&set, 0, n, n + 1};
+  g.gens_1 = CommitKey{&set, n, 1, n + 1};
+  return g;
+}
+
+// the merge of k tables of 2^m entries gathered into one zero-padded buffer (the shapes whose rows straddle tables: at most 2^12 entries)
+static DevBuf<u256> pc_gather(Ctx& ctx, const u256* const* tables, int k, size_t m) {
+  const size_t len = (size_t)1 << m, used = (size_t)k * len, total = next_pow2((size_t)k) * len;
+  DevBuf<u256> z(total);
+  for (int j = 0; j < k; j++) dev::d2d(z.p + j * len, tables[j], len * sizeof(u256), ctx.stream);
+  if (total > used) dev::dzero(z.p + used, (total - used) * sizeof(u256), ctx.stream);
+  return z;
+}
+
+PolyCommitment pc_commit(Ctx& ctx, const PolyCommitmentGens& gens, const u256* const* tables, int k, size_t m, const Fq* blinds) {
+  const size_t c = log2_ceil(next_pow2((size_t)k)), ell = m + c, L = (size_t)1 << (ell / 2), R = (size_t)1 << (ell - ell / 2);
+  if (gens.n != R) throw SpError(SP_ERR_INVALID_ARG, "poly commit: gens.n != R");
+  PolyCommitment comm;
+  if (!pc_rows_in_tables(m, c)) {
+    DevBuf<u256> merged = pc_gather(ctx, tables, k, m);
+    commit_rows_and_compress(ctx, gens.gens_n, merged.p, R, L, R, blinds, comm.C);
+    return comm;
+  }
+  // every row of every table (and the blind-only padding rows) in one launch, reading the tables where they are
+  const CommitKey& key = gens.gens_n;
+  ctx.ensure_scratch(dev::msm_scratch_bytes(L, R) + 64);
+  DevBuf<ge> rows(L);
+  DevBuf<u256> d_bl;
+  if (blinds) { d_bl.alloc(L); dev::h2d(d_bl.p, blinds, L * sizeof(u256), ctx.stream); }
+  dev::TableRows tr;
+  for (int j = 0; j < k; j++) tr.t[j] = tables[j];
+  tr.ntables = k;
+  tr.rows_per_table = ((size_t)1 << m) / R;
+  tr.row_len = R;
+  dev::msm_rows_tables(rows.p, key.set->table.p, key.set->wbits, key.set->rows(), tr, L, R, blinds ? d_bl.p : nullptr, key.h, ctx.scratch.p, ctx.stream);
+  DevBuf<uint8_t> comp(32 * L);
+  dev::compress_batch(comp.p, rows.p, L, ctx.stream);
+  comm.C.resize(L);
+  dev::d2h(comm.C.data(), comp.p, 32 * L, ctx.stream);
+  ctx.sync();
+  return comm;
+}
+
+void pc_eval_prove_joint(Ctx& ctx, const PolyCommitmentGens& gens, const u256* const* tables, int k, const std::vector<Fq>& r, const std::vector<Fq>* blinds_opt,
+                         Transcript& T, RandomTape& tape, PolyEvalProof& proof, std::vector<Fq>& evals) {
+  const size_t m = r.size(), c = log2_ceil(next_pow2((size_t)k)), ell = m + c, lv = ell / 2;
+  DevBuf<u256> d_r(m + 1), d_ev(k);
+  dev::h2d(d_r.p, r.data(), m * sizeof(u256), ctx.stream);
+  // evals[j] = <rows[j], eq> (dot_many takes 32 tables a launch)
+  auto evaluate = [&](const u256* const* rows, const u256* d_eq, size_t n) {
+    for (int j0 = 0; j0 < k; j0 += 32) dev::dot_many(d_ev.p + j0, rows + j0, std::min(32, k - j0), d_eq, n, ctx.red.p, ctx.stream);
+    evals = ctx.download(d_ev.p, k);
+  };
+  Fq joint;
+  if (!pc_rows_in_tables(m, c)) {
+    const size_t len = (size_t)1 << m;
+    DevBuf<u256> merged = pc_gather(ctx, tables, k, m), d_eq(len), eqs(dev::eq_evals_scratch(m));
+    dev::eq_evals(d_eq.p, d_r.p, (int)m, eqs.p, ctx.stream);
+    evaluate(tables, d_eq.p, len);
+    const std::vector<Fq> r_joint = combine_to_one(T, evals, r, "evals_ops_val", "challenge_combine_n_to_one", "joint_claim_eval", joint);
+    Cp C_Zr;
+    polyeval_prove(ctx, merged.p, blinds_opt, r_joint, &joint, nullptr, gens, T, tape, proof, C_Zr);
+    return;
+  }
+  // The merge's row split puts the table index in the top c of its lv row bits, so its left eq factor is eq(ch) (x) eq(r[..lv - c]) and its bound
+  // rows are sum_j eq(ch)_j LZ_j with LZ_j = bound(Z_j, eq(r[..lv - c])) (tables past k are zero).  The LZ_j need only r: one pass over the tables
+  // gives them, the evaluations <LZ_j, eq(r[lv - c..])> follow, and the challenges only combine k rows of R_J entries.
+  const size_t lt = lv - c, Lt = (size_t)1 << lt, RJ = (size_t)1 << (ell - lv);
+  DevBuf<u256> d_Lt(Lt), d_R(RJ), eqs(dev::eq_evals_scratch(std::max(lt, ell - lv))), LZs((size_t)k * RJ),
+      tmp(std::max(dev::bound_rows_many_scratch(k, Lt, RJ), (size_t)k * RJ));
+  dev::eq_evals(d_Lt.p, d_r.p, (int)lt, eqs.p, ctx.stream);
+  dev::eq_evals(d_R.p, d_r.p + lt, (int)(ell - lv), eqs.p, ctx.stream);
+  dev::bound_rows_many(LZs.p, tables, k, d_Lt.p, Lt, RJ, tmp.p, ctx.stream);
+  std::vector<const u256*> lz(k);
+  for (int j = 0; j < k; j++) lz[j] = LZs.p + (size_t)j * RJ;
+  evaluate(lz.data(), d_R.p, RJ);
+  const std::vector<Fq> r_joint = combine_to_one(T, evals, r, "evals_ops_val", "challenge_combine_n_to_one", "joint_claim_eval", joint);
+  const std::vector<Fq> eq_ch = host_eq_evals(std::vector<Fq>(r_joint.begin(), r_joint.begin() + c));
+  DevBuf<u256> d_eqch(k), d_LZ(RJ), d_Rc(RJ);
+  dev::h2d(d_eqch.p, eq_ch.data(), (size_t)k * sizeof(u256), ctx.stream);
+  dev::bound_rows(d_LZ.p, LZs.p, d_eqch.p, (size_t)k, RJ, tmp.p, ctx.stream);
+  Fq LZ_blind = Fq::zero();
+  if (blinds_opt) {
+    const std::vector<Fq> Lv = host_eq_evals(std::vector<Fq>(r_joint.begin(), r_joint.begin() + lv));
+    for (size_t i = 0; i < Lv.size(); i++) LZ_blind += (*blinds_opt)[i] * Lv[i];
+  }
+  // the rest of PolyEvalProof::prove (dense_mlpoly.rs:312-365), as polyeval_prove runs it
+  T.append_protocol_name("polynomial evaluation proof");
+  dev::to_canonical(d_Rc.p, d_R.p, RJ, ctx.stream);
+  std::vector<uint8_t> a_canon(32 * RJ);
+  dev::d2h(a_canon.data(), d_Rc.p, 32 * RJ, ctx.stream);
+  ctx.sync();
+  Cp C_Zr;
+  dotproduct_log_prove(ctx, gens, T, tape, d_LZ.p, LZ_blind, d_R.p, a_canon, joint, Fq::zero(), proof.proof, C_Zr);
 }
 
 // ================================================================================================ instance
@@ -1004,7 +1116,7 @@ void r1cs_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::v
     Fq eval_vars_at_ry;
     ctx.get_small(layout::SMALL_DOT.off, &eval_vars_at_ry, 1);
     Fq blind_eval = tape.random_scalar("blind_eval");
-    polyeval_prove(ctx, d_vars, &blinds_vars, ry1, eval_vars_at_ry, &blind_eval, gens.gens_pc, T, tape, proof.proof_eval_vars_at_ry, proof.comm_vars_at_ry);
+    polyeval_prove(ctx, d_vars, &blinds_vars, ry1, &eval_vars_at_ry, &blind_eval, gens.gens_pc, T, tape, proof.proof_eval_vars_at_ry, proof.comm_vars_at_ry);
     Fq blind_eval_Z_at_ry = (Fq::one() - ry[0]) * blind_eval;
     Fq blind_expected_claim_postsc2 = claims2[1] * blind_eval_Z_at_ry;
     Fq claim_post_phase2 = claims2[0] * claims2[1];

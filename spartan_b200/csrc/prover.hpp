@@ -134,9 +134,36 @@ std::vector<Fq> zk_round_weights(const std::vector<Fq>& w, const Fq& r_j, size_t
 void append_claims_phase2(Transcript& T, const std::array<Cp, 4>& c);
 // NIZK::prove / verify before the R1CS proof: protocol name and R1CSShapeDigest (lib.rs:513-514, :558-559)
 void append_nizk_head(Transcript& T, const Instance& inst);
-// PolyEvalProof::prove (dense_mlpoly.rs:312-365) on a device-resident table
-void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt, const std::vector<Fq>& r, const Fq& Zr, const Fq* blind_Zr_opt,
-                    const PolyCommitmentGens& gens, Transcript& T, RandomTape& tape, PolyEvalProof& proof, Cp& C_Zr);
+// PolyEvalProof::prove (dense_mlpoly.rs:312-365) on a device-resident table.  Zr null: Zr = Z(r) = <LZ, eq(r[ell/2..])>, computed on the device
+// from the bound rows (Z is not read again), and returned through Zr_out when that is set
+void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt, const std::vector<Fq>& r, const Fq* Zr, const Fq* blind_Zr_opt,
+                    const PolyCommitmentGens& gens, Transcript& T, RandomTape& tape, PolyEvalProof& proof, Cp& C_Zr, Fq* Zr_out = nullptr);
+
+// ---- the caller's own tables (sp_pc_*): k tables of 2^m entries each, committed and opened as DensePolynomial::merge of them (dense_mlpoly.rs:259-272),
+// on this rank's GPU alone
+// PolyCommitmentGens::new(num_vars, label) (dense_mlpoly.rs:29-36): gens_n.n = 2^(num_vars - num_vars/2), n + 2 points of the label's stream
+inline size_t pc_gens_n(size_t num_vars) { return (size_t)1 << (num_vars - num_vars / 2); }
+PolyCommitmentGens pc_gens_view(GenSet& set, size_t num_vars);   // adds the host tables of bases n, n + 1 when missing
+// The merge of k tables is 2^(m+c) entries, c = log2 next_pow2(k), split as a matrix of 2^floor((m+c)/2) rows of R = 2^ceil((m+c)/2).  A row lies
+// inside one table when R <= 2^m: the device then reads the tables where they are.  Otherwise the merge has at most 2^12 entries (c <= 6) and is
+// gathered into one buffer.
+inline bool pc_rows_in_tables(size_t m, size_t c) { return (m + c + 1) / 2 <= m; }
+// DensePolynomial::merge(tables).commit (dense_mlpoly.rs:179-204) with the row blinds `blinds` (L of them) or none (null)
+PolyCommitment pc_commit(Ctx& ctx, const PolyCommitmentGens& gens, const u256* const* tables, int k, size_t m, const Fq* blinds);
+// DerefsEvalProof::prove_single (sparse_mlpoly.rs:80-123), no protocol name: the k evaluations at r (out: evals) combined to one claim on the merge
+// at (challenges || r), proved by PolyEvalProof::prove without blind_Zr.  blinds_opt: the merge's commitment blinds
+void pc_eval_prove_joint(Ctx& ctx, const PolyCommitmentGens& gens, const u256* const* tables, int k, const std::vector<Fq>& r, const std::vector<Fq>* blinds_opt,
+                         Transcript& T, RandomTape& tape, PolyEvalProof& proof, std::vector<Fq>& evals);
+// the n-to-1 reduction of DerefsEvalProof / HashLayerProof (sparse_mlpoly.rs:80-123): evals padded to a power of two and absorbed, log2 of that many
+// challenges, the evaluations folded by bound_poly_var_bot (last challenge first) into `joint`, which is absorbed; returns challenges || rand
+std::vector<Fq> combine_to_one(Transcript& T, std::vector<Fq> evals, const std::vector<Fq>& rand, const char* label_evals, const char* label_challenge,
+                               const char* label_joint, Fq& joint);
+// PolyEvalProof::verify (C_Zr given) / verify_plain (Zr given) on bincode bytes, and DerefsEvalProof::verify_single (sparse_mlpoly.rs:149-176), with
+// the Immediate checker (verifier.cpp): SpError(SP_ERR_VERIFY / SP_ERR_DECOMPRESS) naming the failing check
+void pc_eval_verify(Ctx& ctx, const PolyCommitmentGens& gens, const PolyCommitment& comm, const std::vector<Fq>& r, const Cp* C_Zr, const Fq* Zr, Transcript& T,
+                    const uint8_t* proof, size_t len);
+void pc_eval_verify_joint(Ctx& ctx, const PolyCommitmentGens& gens, const PolyCommitment& comm, const std::vector<Fq>& r, const std::vector<Fq>& evals,
+                          Transcript& T, const uint8_t* proof, size_t len);
 
 // exposed pieces (C-ABI operator level and tests)
 Cp commit_rows_and_compress(Ctx& ctx, const CommitKey& key, const u256* d_scalars, size_t stride, size_t L, size_t R, const Fq* blinds,

@@ -442,8 +442,8 @@ void equalize(std::vector<Fq>& rx, std::vector<Fq>& ry) {
   if (rx.size() < ry.size()) rx.insert(rx.begin(), ry.size() - rx.size(), Fq::zero());
   if (ry.size() < rx.size()) ry.insert(ry.begin(), rx.size() - ry.size(), Fq::zero());
 }
-static std::vector<Fq> combine_to_one(Transcript& T, std::vector<Fq> evals, const std::vector<Fq>& rand, const char* label_evals,
-                                      const char* label_challenge, const char* label_joint, Fq& joint) {
+std::vector<Fq> combine_to_one(Transcript& T, std::vector<Fq> evals, const std::vector<Fq>& rand, const char* label_evals,
+                               const char* label_challenge, const char* label_joint, Fq& joint) {
   evals.resize(next_pow2(evals.size()), Fq::zero());
   T.append_scalars(label_evals, evals);
   std::vector<Fq> r_joint = T.challenge_vector(label_challenge, log2_ceil(evals.size()));
@@ -747,19 +747,19 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
   {  // DerefsEvalProof::prove (sparse_mlpoly.rs:125-149, prove_single :80-123)
     T.append_protocol_name("Derefs evaluation proof");
     const std::vector<Fq> r_joint = combine_to_one(T, hl, HashOpening::derefs, rand_ops, joint);
-    polyeval_prove(ctx, derefs.p, nullptr, r_joint, joint, nullptr, gens.gens_derefs, T, tape, hl.proof_derefs, dummy);
+    polyeval_prove(ctx, derefs.p, nullptr, r_joint, &joint, nullptr, gens.gens_derefs, T, tape, hl.proof_derefs, dummy);
   }
   mark("  polyeval_derefs(2^23)", th);
   th = std::chrono::steady_clock::now();
   {  // ops decommitment (sparse_mlpoly.rs:766-797)
     const std::vector<Fq> r_joint = combine_to_one(T, hl, HashOpening::ops, rand_ops, joint);
-    polyeval_prove(ctx, enc.comb_ops.p, nullptr, r_joint, joint, nullptr, gens.gens_ops, T, tape, hl.proof_ops, dummy);
+    polyeval_prove(ctx, enc.comb_ops.p, nullptr, r_joint, &joint, nullptr, gens.gens_ops, T, tape, hl.proof_ops, dummy);
   }
   mark("  polyeval_ops(2^24)", th);
   th = std::chrono::steady_clock::now();
   {  // mem decommitment (sparse_mlpoly.rs:799-824)
     const std::vector<Fq> r_joint = combine_to_one(T, hl, HashOpening::mem, rand_mem, joint);
-    polyeval_prove(ctx, enc.comb_mem.p, nullptr, r_joint, joint, nullptr, gens.gens_mem, T, tape, hl.proof_mem, dummy);
+    polyeval_prove(ctx, enc.comb_mem.p, nullptr, r_joint, &joint, nullptr, gens.gens_mem, T, tape, hl.proof_mem, dummy);
   }
   mark("  polyeval_mem(2^22)", th);
   mark("evalproof_layered_network", tn);

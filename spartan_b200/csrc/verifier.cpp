@@ -765,6 +765,24 @@ void snark_verify(Ctx& ctx, const SnarkEncoding& enc, const std::vector<Fq>& inp
   snark_replay(chk, enc.comm, input, gens, T, p);
 }
 
+// PolyEvalProof::verify (dense_mlpoly.rs:367-389) against the caller's C_Zr, or verify_plain (:391-404) against Zr
+void pc_eval_verify(Ctx& ctx, const PolyCommitmentGens& gens, const PolyCommitment& comm, const std::vector<Fq>& r, const Cp* C_Zr, const Fq* Zr, Transcript& T,
+                    const uint8_t* proof, size_t len) {
+  const PolyEvalProof p = from_bincode<PolyEvalProof>(proof, len, SP_ERR_VERIFY, "polynomial evaluation proof");
+  Immediate chk(ctx);
+  if (Zr) polyeval_verify_plain(chk, p, gens, T, r, *Zr, comm);
+  else polyeval_verify(chk, p, gens, T, r, P(Fq::one(), *C_Zr, "C_Zr"), *C_Zr, comm);
+}
+// DerefsEvalProof::verify_single (sparse_mlpoly.rs:149-176)
+void pc_eval_verify_joint(Ctx& ctx, const PolyCommitmentGens& gens, const PolyCommitment& comm, const std::vector<Fq>& r, const std::vector<Fq>& evals,
+                          Transcript& T, const uint8_t* proof, size_t len) {
+  const PolyEvalProof p = from_bincode<PolyEvalProof>(proof, len, SP_ERR_VERIFY, "polynomial evaluation proof");
+  Fq joint;
+  const std::vector<Fq> r_joint = combine_to_one(T, evals, r, "evals_ops_val", "challenge_combine_n_to_one", "joint_claim_eval", joint);
+  Immediate chk(ctx);
+  polyeval_verify_plain(chk, p, gens, T, r_joint, joint, comm);
+}
+
 void nizk_verify_batch(Ctx& ctx, const R1CSGens& gens, std::vector<VerifyJob>& jobs, const uint8_t seed[32]) {
   for (auto& j : jobs) check_dims(j.inst->num_cons, j.inst->num_vars, j.inst->num_inputs);
   verify_batch<NizkProof>(
