@@ -255,6 +255,65 @@ int sp_pc_eval_prove_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, sp_poly* const
 int sp_pc_eval_verify_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t* comm, size_t comm_len, const uint64_t* r_mont, size_t m,
                               const uint64_t* evals_mont, int k, uint8_t* strobe_state /* in, out */, const uint8_t* proof, size_t proof_len);
 
+/* ---- product circuits over the caller's tables and the batched proof of their products: the grand-product argument of the reference's memory
+ * check (ProductCircuit, ProductCircuitEvalProofBatched, product_tree.rs), bytes identical to the reference's for the same transcript.  Use, e.g.
+ * for an offline memory check, multiset equality or a lookup argument: commit to the tuple tables (sp_pc_commit), draw the fingerprint
+ * challenges, build one circuit per fingerprinted multiset (sp_prod_build), absorb the products, prove them (sp_prod_prove_t), and open the
+ * tables at the point the proof ends on (sp_pc_eval_prove_joint_t); the verifier checks the leaf claims with sp_prod_leaf_eval.  Every entry runs
+ * on this rank's GPU alone, also on a connected multi-GPU context.  No dot-product circuits: the proof's claims_dotp are three empty vectors
+ * (the reference's prove with dotp_circuit_vec empty).
+ *
+ * Circuit c's leaf at index x < 2^m is an affine form of up to SP_PROD_MAX_SOURCES of the tables and of x itself:
+ *   leaf_c[x] = const_c + index_coeff_c * x + sum_{s < nsources_c} coeff_{c,s} * tables[source_{c,s}][x]
+ * A plain table is one source with coefficient one.  The memory check's hash(addr, val, ts) - r_multiset = ts*r^2 + val*r + addr - gamma
+ * (sparse_mlpoly.rs:542-591) is sources (ts, r^2), (val, r), (addr, 1) and const -gamma; for init / audit addr is the index (index_coeff = 1), and
+ * the write set's ts + 1 moves r^2 into the constant.  All scalars are Montgomery limbs and must be reduced (< q).
+ *
+ * Device footprint (32 bytes per scalar): 2^(m+1) scalars per circuit, every layer kept, from sp_prod_build until sp_prod_prove_t or sp_prod_free;
+ * sp_prod_prove_t adds 2^m scalars of eq tables (poly_C_par and its two ping-pong halves) plus O(2^(m/2)) scalars, released on return.  At
+ * m = 20: 64 MiB per circuit and 32 MiB for the proof. */
+#define SP_PROD_MAX_CIRCUITS 24   /* = the instances of one batched sumcheck launch: one launch per round */
+#define SP_PROD_MAX_SOURCES 3
+typedef struct {
+  uint32_t nsources;                          /* 0 .. SP_PROD_MAX_SOURCES */
+  uint32_t source[SP_PROD_MAX_SOURCES];       /* indices into the tables array */
+  uint64_t coeff_mont[SP_PROD_MAX_SOURCES][4];
+  uint64_t index_coeff_mont[4];               /* times x: IdentityPolynomial (dense_mlpoly.rs:101-117) */
+  uint64_t const_mont[4];
+} sp_prod_leaves;
+typedef struct sp_prod_circuits sp_prod_circuits;
+/* ProductCircuit::new of each of k circuits of 2^m leaves, then ProductCircuit::evaluate (product_tree.rs:36-63).  tables: ntables handles of one
+ * length 2^m, m >= 1 (the reference panics without a product layer); the same handle may appear twice.  leaves NULL: k = ntables and circuit i's
+ * leaves are table i.  Out: *out, and products_out = the k products.  The tables are read, never modified.  One launch builds the leaves and the
+ * first product layer of every circuit; each further layer is one launch per group of at most 16 circuits: 1 + ceil(k/16) (m - 2) launches for
+ * m >= 2, one for m = 1.
+ * SP_ERR_INVALID_ARG: k outside 1 .. SP_PROD_MAX_CIRCUITS, ntables < 1, a NULL table or one of another context, unequal lengths or a length that
+ * is not a power of two >= 2, nsources > SP_PROD_MAX_SOURCES or a source >= ntables, leaves NULL with k != ntables.  SP_ERR_INVALID_SCALAR: a
+ * coefficient or constant not reduced.  A refused call allocates and launches nothing. */
+int sp_prod_build(sp_ctx* ctx, sp_poly* const* tables, int ntables, const sp_prod_leaves* leaves, int k, sp_prod_circuits** out,
+                  uint64_t* products_out /* k x 4 */);
+/* ProductCircuitEvalProofBatched::prove(circuits, [], transcript) (product_tree.rs:259-383) on the caller's transcript.  The proof does not absorb
+ * the products: absorb them first, as ProductLayerProof::prove does (sparse_mlpoly.rs:1061-1064).  Out: *proof = bincode(ProductCircuitEvalProofBatched)
+ * (free with sp_free), rand_out = the m scalars of the point the proof ends on, leaf_evals_out = each circuit's leaf polynomial at rand (the
+ * last claims_to_verify: the values sp_prod_verify_t returns as leaf claims).  Consumes the circuits: their layers are bound in place and released,
+ * and a second call on the handle is refused (SP_ERR_INVALID_ARG), as are a NULL handle and one of another context; a refused call leaves the
+ * transcript untouched.  Launches, independent of k: one per sumcheck round plus a few per layer (tests/test_gpu_product.py states the count). */
+int sp_prod_prove_t(sp_ctx* ctx, sp_prod_circuits* c, uint8_t* strobe_state /* in, out */, uint8_t** proof, size_t* proof_len,
+                    uint64_t* rand_out /* m x 4 */, uint64_t* leaf_evals_out /* k x 4 */);
+void sp_prod_free(sp_prod_circuits* c);
+/* ProductCircuitEvalProofBatched::verify(products, [], 2^m, transcript) (product_tree.rs:385-485), host only: ctx may be NULL (sp_last_error(NULL)
+ * then holds the message).  SP_OK: accepted, rand_out = the m scalars, leaf_claims_out = the k claims about the leaf polynomials at rand.
+ * SP_ERR_VERIFY: rejected (wrong depth, claim shapes, a layer check, non-empty dotp claims, bytes that do not decode), the transcript left as the
+ * reference's verify leaves it.  SP_ERR_INVALID_ARG: k outside 1 .. SP_PROD_MAX_CIRCUITS or m outside 1 .. 60; SP_ERR_INVALID_SCALAR: a product
+ * not reduced; either leaves the transcript untouched. */
+int sp_prod_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const uint64_t* products_mont, int k, size_t m,
+                     uint8_t* strobe_state /* in, out */, uint64_t* rand_out /* m x 4 */, uint64_t* leaf_claims_out /* k x 4 */);
+/* host only: each circuit's leaf polynomial at rand (m scalars) from the tables' values there (e.g. sp_pc_eval_prove_joint_t's evals_out):
+ * const + index_coeff * sum_i 2^(m-1-i) rand_i + sum_s coeff_s * table_evals[source_s].  The verifier compares it with sp_prod_verify_t's leaf
+ * claims.  leaves NULL: circuit i is table i (k = ntables).  Refusals as sp_prod_build's. */
+int sp_prod_leaf_eval(const sp_prod_leaves* leaves, int k, const uint64_t* table_evals_mont, int ntables, const uint64_t* rand_mont, size_t m,
+                      uint64_t* out /* k x 4 */);
+
 /* ---- inner-product argument, operator level: BulletReductionProof::prove (src/nizk/bullet.rs:32-132) for a host that keeps the transcript and
  * the orchestration.  sp_ipa_begin copies a_vec / b_vec; the generator vector G is `gens` (G[0..n)).  Each round: sp_ipa_round_LR returns the
  * compressed L, R of bullet.rs:83-97 (c_L, c_R are formed inside; Q and H are the caller's points), the host appends them and derives u

@@ -748,6 +748,124 @@ class PolyEvalProof:
                                                      t.state, C.c_char_p(self.data), _sz(len(self.data))))
 
 
+# ----------------------------------------------------------------------------- product circuits of the caller's tables
+SP_PROD_MAX_CIRCUITS, SP_PROD_MAX_SOURCES = 24, 3
+
+
+class _ProdLeaves(C.Structure):
+    _fields_ = [("nsources", C.c_uint32), ("source", C.c_uint32 * SP_PROD_MAX_SOURCES), ("coeff_mont", (C.c_uint64 * 4) * SP_PROD_MAX_SOURCES),
+                ("index_coeff_mont", C.c_uint64 * 4), ("const_mont", C.c_uint64 * 4)]
+
+
+def _scalar_arg(x):
+    """a Python int (< q) or Montgomery limbs -> limbs"""
+    if isinstance(x, (int, np.integer)):
+        return scalar_from_bytes(int(x).to_bytes(32, "little"))
+    return np.ascontiguousarray(x, dtype=np.uint64).reshape(4)
+
+
+class ProductLeaves:
+    """One product circuit's leaves as an affine form of the tables and of the index x (sp_prod_leaves):
+    leaf[x] = const + index_coeff * x + sum over sources (i, coeff) of coeff * tables[i][x].  Scalars: Python ints (< q) or Montgomery limbs.
+    The memory check's hash(addr, val, ts) - gamma = ts*r^2 + val*r + addr - gamma (sparse_mlpoly.rs:542-591) is
+    ProductLeaves([(ts, r^2), (val, r), (addr, 1)], const=-gamma), with index_coeff=1 instead of an addr table for init and audit."""
+
+    def __init__(self, sources=(), index_coeff=0, const=0):
+        self.sources = [(int(i), _scalar_arg(c)) for i, c in sources]
+        self.index_coeff, self.const = _scalar_arg(index_coeff), _scalar_arg(const)
+
+    def _fill(self, out):
+        out.nsources = len(self.sources)   # more than SP_PROD_MAX_SOURCES: the count alone reaches the library, which refuses it
+        for s, (i, c) in enumerate(self.sources[:SP_PROD_MAX_SOURCES]):
+            out.source[s] = i
+            out.coeff_mont[s][:] = [int(v) for v in c]
+        out.index_coeff_mont[:] = [int(v) for v in self.index_coeff]
+        out.const_mont[:] = [int(v) for v in self.const]
+
+
+def _c_leaves(leaves):
+    if leaves is None:
+        return None
+    arr = (_ProdLeaves * max(len(leaves), 1))()
+    for l, a in zip(leaves, arr):
+        l._fill(a)
+    return arr
+
+
+class ProductCircuits:
+    """ProductCircuit::new of k circuits, then ProductCircuit::evaluate (product_tree.rs:36-63), on the GPU: `tables` are DensePolynomials of
+    one length 2^m (m >= 1), read and never modified; `leaves` a list of ProductLeaves (at most SP_PROD_MAX_CIRCUITS), or None for one circuit
+    per table.  .products: the k products as (k, 4) limbs; .num_vars = m.  ProductCircuitEvalProofBatched.prove consumes the circuits."""
+
+    def __init__(self, tables, leaves=None):
+        tables = _poly_list(tables)
+        self.ctx = tables[0].ctx if tables else default_context()
+        self.k = len(tables) if leaves is None else len(leaves)
+        products = np.zeros((max(self.k, 1), 4), dtype=np.uint64)
+        h = _vp()
+        self.ctx.check(lib.sp_prod_build(self.ctx.h, _handles(tables), C.c_int(len(tables)), _c_leaves(leaves), C.c_int(self.k), C.byref(h),
+                                         _p(products)))
+        self.h = h
+        self.products = products[:self.k]
+        self.num_vars = tables[0].len().bit_length() - 1
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None):
+                lib.sp_prod_free(self.h)
+                self.h = None
+        except Exception:
+            pass
+
+
+class ProductCircuitEvalProofBatched:
+    """product_tree.rs:250-485 without dot-product circuits.  Transcripts: a Transcript (advanced in place) or a label."""
+
+    @staticmethod
+    def prove(circuits, transcript):
+        """ProductCircuitEvalProofBatched::prove(circuits, [], transcript) (product_tree.rs:259-383).  Absorb the products first: the proof does
+        not.  Returns (proof bytes = bincode, rand as (m, 4) limbs, leaf_evals = each circuit's leaf polynomial at rand as (k, 4) limbs)."""
+        ctx, t = circuits.ctx, _transcript_state(transcript)
+        out, n = C.POINTER(C.c_ubyte)(), _sz()
+        rand = np.zeros((circuits.num_vars, 4), dtype=np.uint64)
+        evals = np.zeros((max(circuits.k, 1), 4), dtype=np.uint64)
+        ctx.check(lib.sp_prod_prove_t(ctx.h, circuits.h, t.state, C.byref(out), C.byref(n), _p(rand), _p(evals)))
+        return _take_bytes(out, n), rand, evals[:circuits.k]
+
+    @staticmethod
+    def verify(proof, products, num_vars, transcript):
+        """ProductCircuitEvalProofBatched::verify(products, [], 2^num_vars, transcript) (product_tree.rs:385-485), on the host: returns (rand,
+        leaf_claims) as limbs, raises ProofVerifyError.  The transcript is advanced as the reference's verify advances it, accepted or not."""
+        t, proof, prods = _transcript_state(transcript), bytes(proof), _limbs(products)
+        rand = np.zeros((max(num_vars, 1), 4), dtype=np.uint64)
+        claims = np.zeros((max(len(prods), 1), 4), dtype=np.uint64)
+        rc = lib.sp_prod_verify_t(None, C.c_char_p(proof), _sz(len(proof)), _p(prods), C.c_int(len(prods)), _sz(num_vars), t.state, _p(rand),
+                                  _p(claims))
+        if rc == SP_OK:
+            return rand[:num_vars], claims[:len(prods)]
+        msg = lib.sp_last_error(None).decode()
+        if rc == SP_ERR_VERIFY:
+            raise ProofVerifyError("InternalError: " + msg, rc)
+        if rc == SP_ERR_INVALID_SCALAR:
+            raise R1CSError("InvalidScalar: " + msg)
+        raise SpartanB200Error("spartan_b200 error %d: %s" % (rc, msg))
+
+
+def product_leaf_eval(leaves, table_evals, rand):
+    """the leaf polynomials at rand from the tables' values there (sp_prod_leaf_eval), on the host: (k, 4) limbs.  leaves None: one circuit per
+    table.  A verifier compares these with ProductCircuitEvalProofBatched.verify's leaf claims."""
+    ev, r = _limbs(table_evals), _limbs(rand)
+    k = len(ev) if leaves is None else len(leaves)
+    out = np.zeros((max(k, 1), 4), dtype=np.uint64)
+    rc = lib.sp_prod_leaf_eval(_c_leaves(leaves), C.c_int(k), _p(ev), C.c_int(len(ev)), _p(r), _sz(len(r)), _p(out))
+    if rc != SP_OK:
+        msg = lib.sp_last_error(None).decode()
+        if rc == SP_ERR_INVALID_SCALAR:
+            raise R1CSError("InvalidScalar: " + msg)
+        raise SpartanB200Error("spartan_b200 error %d: %s" % (rc, msg))
+    return out[:k]
+
+
 # ----------------------------------------------------------------------------- public API of lib.rs
 class Assignment:
     """lib.rs:57-104: a vector of scalars given as canonical 32-byte strings"""

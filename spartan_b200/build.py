@@ -11,7 +11,7 @@ NVCC = os.environ.get("SP_NVCC", "/usr/local/cuda/bin/nvcc")
 CXX = "/usr/bin/g++"
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CU = ["kernels.cu", "kernels_sc.cu", "kernels_pip.cu", "kernels_inst.cu", "comm.cu"]
-CPP = ["prover.cpp", "snark.cpp", "verifier.cpp", "capi.cpp", "deflate.cpp"]
+CPP = ["prover.cpp", "product.cpp", "snark.cpp", "verifier.cpp", "capi.cpp", "deflate.cpp"]
 HDR = ["field.cuh", "mul_ptx.cuh", "curve.cuh", "kcommon.cuh", "quad.cuh","dev.hpp", "host.hpp", "host_fe51.hpp", "engine.hpp", "prover.hpp", "snark.hpp", "wire.hpp", os.path.join("..", "..", "include", "spartan_b200.h")]
 
 

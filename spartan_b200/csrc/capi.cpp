@@ -1308,6 +1308,167 @@ int sp_pc_eval_verify_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t
   SP_CATCH(ctx)
 }
 
+// ---- product circuits of the caller's tables (product.cpp: prod_*).  Every argument is checked before the first launch or allocation and before
+// the transcript is touched, so a refused call leaves the tables, the transcript and the device memory as they were.
+}  // extern "C"
+struct sp_prod_circuits {
+  Ctx* ctx;
+  size_t m;
+  std::vector<std::unique_ptr<ProdCircuit>> cs;   // released by the proof
+  bool spent;
+};
+static const size_t PROD_MAX_VARS = 60;
+// one circuit's leaf form, checked: leaf[x] = cst + idx * x + sum_s coeff[s] * table[src[s]][x]
+struct LeafForm { uint32_t nsrc = 0; uint32_t src[SP_PROD_MAX_SOURCES] = {}; Fq coeff[SP_PROD_MAX_SOURCES], idx = Fq::zero(), cst = Fq::zero(); };
+static void prod_counts(const sp_prod_leaves* leaves, int k, int ntables, const std::string& what) {
+  if (k < 1 || k > SP_PROD_MAX_CIRCUITS)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": " + std::to_string(k) + " circuits; 1 .. SP_PROD_MAX_CIRCUITS = " + std::to_string(SP_PROD_MAX_CIRCUITS) + " supported");
+  if (ntables < 1) throw SpError(SP_ERR_INVALID_ARG, what + ": " + std::to_string(ntables) + " tables; at least one needed");
+  if (!leaves && k != ntables)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": leaves NULL (circuit i = table i) needs k = ntables, got k = " + std::to_string(k) + ", ntables = " + std::to_string(ntables));
+}
+static std::vector<LeafForm> prod_forms(const sp_prod_leaves* leaves, int k, int ntables, const std::string& what) {
+  prod_counts(leaves, k, ntables, what);
+  std::vector<LeafForm> f(k);
+  for (int c = 0; c < k; c++) {
+    if (!leaves) { f[c].nsrc = 1; f[c].src[0] = (uint32_t)c; f[c].coeff[0] = Fq::one(); continue; }
+    const sp_prod_leaves& l = leaves[c];
+    const std::string at = what + ": circuit " + std::to_string(c);
+    if (l.nsources > SP_PROD_MAX_SOURCES)
+      throw SpError(SP_ERR_INVALID_ARG, at + " has " + std::to_string(l.nsources) + " sources; at most SP_PROD_MAX_SOURCES = " + std::to_string(SP_PROD_MAX_SOURCES));
+    for (uint32_t s = 0; s < l.nsources; s++)
+      if (l.source[s] >= (uint32_t)ntables)
+        throw SpError(SP_ERR_INVALID_ARG, at + ": source " + std::to_string(s) + " is table " + std::to_string(l.source[s]) + " >= ntables = " + std::to_string(ntables));
+  }
+  if (leaves)
+    for (int c = 0; c < k; c++) {
+      const sp_prod_leaves& l = leaves[c];
+      const std::string at = what + ": circuit " + std::to_string(c);
+      require_reduced(&l.coeff_mont[0][0], l.nsources, (at + ": coefficient").c_str());
+      require_reduced(l.index_coeff_mont, 1, (at + ": index coefficient").c_str());
+      require_reduced(l.const_mont, 1, (at + ": constant").c_str());
+      f[c].nsrc = l.nsources;
+      for (uint32_t s = 0; s < l.nsources; s++) { f[c].src[s] = l.source[s]; f[c].coeff[s] = fq_in(l.coeff_mont[s]); }
+      f[c].idx = fq_in(l.index_coeff_mont);
+      f[c].cst = fq_in(l.const_mont);
+    }
+  return f;
+}
+// the tables of a build: non-null handles of this context, of one power-of-two length >= 2; returns log2 of it
+static size_t prod_tables(sp_ctx* ctx, sp_poly* const* tables, int ntables, const std::string& what) {
+  if (!tables) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL table array");
+  for (int i = 0; i < ntables; i++) {
+    if (!tables[i]) throw SpError(SP_ERR_INVALID_ARG, what + ": table " + std::to_string(i) + " is NULL");
+    if (tables[i]->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, what + ": table " + std::to_string(i) + " belongs to another context");
+    if (tables[i]->len != tables[0]->len) throw SpError(SP_ERR_INVALID_ARG, what + ": tables differ in length");
+  }
+  const size_t len = tables[0]->len;
+  if (len < 2 || (len & (len - 1)) || log2_ceil(len) > PROD_MAX_VARS)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": the table length must be a power of two >= 2 (a circuit needs a product layer), got " + std::to_string(len));
+  return log2_ceil(len);
+}
+extern "C" {
+
+int sp_prod_build(sp_ctx* ctx, sp_poly* const* tables, int ntables, const sp_prod_leaves* leaves, int k, sp_prod_circuits** out, uint64_t* products_out) {
+  SP_TRY(ctx)
+  const std::string what = "prod_build";
+  if (!out || !products_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  prod_counts(leaves, k, ntables, what);   // before any table is looked at
+  const size_t m = prod_tables(ctx, tables, ntables, what);
+  const std::vector<LeafForm> f = prod_forms(leaves, k, ntables, what);
+  const Fq one = Fq::one();
+  std::vector<dev::ProdLeaves> d(k);
+  for (int c = 0; c < k; c++) {
+    dev::ProdLeaves& p = d[c];
+    memset(static_cast<void*>(&p), 0, sizeof p);
+    p.nsrc = f[c].nsrc;
+    for (uint32_t s = 0; s < f[c].nsrc; s++) {
+      p.src[s] = tables[f[c].src[s]]->d.p;
+      p.coeff[s] = f[c].coeff[s].m;
+      if (f[c].coeff[s] == one) p.flags |= dev::PROD_UNIT0 << s;
+    }
+    p.idx = f[c].idx.m; p.cst = f[c].cst.m;
+    if (!f[c].idx.is_zero()) p.flags |= dev::PROD_IDX;
+    if (!f[c].cst.is_zero()) p.flags |= dev::PROD_CST;
+  }
+  std::unique_ptr<sp_prod_circuits> h(new sp_prod_circuits{&ctx->c, m, {}, false});
+  const std::vector<Fq> products = prod_build(ctx->c, d, (size_t)1 << m, h->cs);
+  for (int c = 0; c < k; c++) fq_out(products_out + 4 * c, products[c]);
+  *out = h.release();
+  SP_CATCH(ctx)
+}
+
+int sp_prod_prove_t(sp_ctx* ctx, sp_prod_circuits* c, uint8_t* strobe_state, uint8_t** proof, size_t* proof_len, uint64_t* rand_out, uint64_t* leaf_evals_out) {
+  SP_TRY(ctx)
+  const std::string what = "prod_prove";
+  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+  ta.check();
+  if (!proof || !proof_len || !rand_out || !leaf_evals_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  if (!c) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL circuits handle");
+  if (c->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, what + ": the circuits belong to another context");
+  if (c->spent) throw SpError(SP_ERR_INVALID_ARG, what + ": the circuits were consumed by an earlier proof (their layers are bound in place)");
+  std::vector<ProdCircuit*> cs;
+  for (auto& p : c->cs) cs.push_back(p.get());
+  Transcript T = ta.open();
+  c->spent = true;
+  ProductCircuitEvalProofBatched P;
+  std::vector<Fq> rand, evals;
+  prod_prove(ctx->c, cs, T, P, rand, evals);
+  c->cs.clear();
+  ta.close(T);
+  const std::vector<uint8_t> bytes = to_bincode(P);
+  *proof = dup_bytes(bytes); *proof_len = bytes.size();
+  for (size_t j = 0; j < rand.size(); j++) fq_out(rand_out + 4 * j, rand[j]);
+  for (size_t i = 0; i < evals.size(); i++) fq_out(leaf_evals_out + 4 * i, evals[i]);
+  SP_CATCH(ctx)
+}
+
+void sp_prod_free(sp_prod_circuits* c) { delete c; }
+
+// host only: no device work, so ctx may be NULL (the message then goes where sp_last_error(NULL) reads it)
+int sp_prod_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const uint64_t* products, int k, size_t m, uint8_t* strobe_state, uint64_t* rand_out,
+                     uint64_t* leaf_claims_out) {
+  std::string& err = ctx ? ctx->c.last_error : g_create_error;
+  try {
+    const std::string what = "prod_verify";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if ((!proof && proof_len) || !products || !rand_out || !leaf_claims_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    if (k < 1 || k > SP_PROD_MAX_CIRCUITS)
+      throw SpError(SP_ERR_INVALID_ARG, what + ": " + std::to_string(k) + " products; 1 .. SP_PROD_MAX_CIRCUITS = " + std::to_string(SP_PROD_MAX_CIRCUITS) + " supported");
+    if (m < 1 || m > PROD_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": m = " + std::to_string(m) + "; 1 .. " + std::to_string(PROD_MAX_VARS) + " supported");
+    require_reduced(products, (size_t)k, "prod_verify: product");
+    Transcript T = ta.open();
+    TranscriptClose close{ta, T};
+    const BatchedOut o = prod_verify(proof, proof_len, fq_vec(products, (size_t)k), m, T);
+    for (size_t j = 0; j < m; j++) fq_out(rand_out + 4 * j, o.rand[j]);
+    for (int i = 0; i < k; i++) fq_out(leaf_claims_out + 4 * i, o.claims[i]);
+    return SP_OK;
+  } catch (const SpError& e) { err = e.what(); return e.code; }
+  catch (const std::exception& e) { err = e.what(); return SP_ERR_INTERNAL; }
+}
+
+// host only
+int sp_prod_leaf_eval(const sp_prod_leaves* leaves, int k, const uint64_t* table_evals, int ntables, const uint64_t* rand, size_t m, uint64_t* out) {
+  try {
+    const std::string what = "prod_leaf_eval";
+    if (!table_evals || !out || (!rand && m)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    if (m > PROD_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": m = " + std::to_string(m) + " > " + std::to_string(PROD_MAX_VARS));
+    const std::vector<LeafForm> f = prod_forms(leaves, k, ntables, what);
+    require_reduced(table_evals, (size_t)ntables, "prod_leaf_eval: table evaluation");
+    require_reduced(rand, m, "prod_leaf_eval: rand");
+    Fq id = Fq::zero();   // IdentityPolynomial::evaluate (dense_mlpoly.rs:105-115): sum_i 2^(m-1-i) rand_i
+    for (size_t i = 0; i < m; i++) id += Fq::from_u64((uint64_t)1 << (m - 1 - i)) * fq_in(rand + 4 * i);
+    for (int c = 0; c < k; c++) {
+      Fq v = f[c].cst + f[c].idx * id;
+      for (uint32_t s = 0; s < f[c].nsrc; s++) v += f[c].coeff[s] * fq_in(table_evals + 4 * f[c].src[s]);
+      fq_out(out + 4 * c, v);
+    }
+    return SP_OK;
+  } catch (const SpError& e) { g_create_error = e.what(); return e.code; }
+  catch (const std::exception& e) { g_create_error = e.what(); return SP_ERR_INTERNAL; }
+}
+
 // ---- batch verifiers: proof i is checked as the single call would check it (statement i, inputs i, label i or caller transcript i); the group
 // equations of all of them are tested in one device pass (verifier.cpp, DESIGN.md "deferred checks")
 struct BatchArgs {

@@ -155,6 +155,18 @@ size_t bound_rows_many_scratch(int k, size_t L_size, size_t R_size);   // scalar
 void bound_rows_many(u256* out, const u256* const* tables, int k, const u256* L, size_t L_size, size_t R_size, u256* scratch, cudaStream_t s);
 void lincomb3(u256* out, const u256* A, const u256* B, const u256* C, const u256* d_rabc /*3*/, size_t n, cudaStream_t s);
 void hadamard_many(u256* const* outs, const u256* const* as, const u256* const* bs, int count, size_t n, cudaStream_t s);
+// ---- the leaves of the caller's product circuits (sp_prod_build): leaf[x] = cst + idx * x + sum_{s < nsrc} coeff[s] * src[s][x] for x < n, written
+// to layer0 (n entries), and layer1[x] = leaf[x] * leaf[x + n/2] for x < n/2 (the first product layer) when layer1 is set.  The sources are only read.
+enum { PROD_UNIT0 = 1 /* bit s: coeff[s] is one */, PROD_IDX = 8 /* idx != 0 */, PROD_CST = 16 /* cst != 0 */ };
+struct ProdLeaves {
+  const u256* src[SP_PROD_MAX_SOURCES];
+  u256 coeff[SP_PROD_MAX_SOURCES], idx, cst;   // Montgomery form
+  u256* layer0;
+  u256* layer1;
+  uint32_t nsrc, flags;
+};
+// k <= SP_PROD_MAX_CIRCUITS circuits of n >= 2 leaves each, in one launch (blockIdx.y = circuit)
+void prod_leaves(const ProdLeaves* circuits, int k, size_t n, cudaStream_t s);
 void to_canonical(u256* out, const u256* in, size_t n, cudaStream_t s);   // Montgomery -> canonical little-endian integers (transcript bytes)
 void gather(u256* out, const u256* mem, const uint32_t* idx, size_t n, cudaStream_t s);
 // hash layer of the SPARK memory check: out = ts*r^2 + val*r + addr - g  (sparse_mlpoly.rs:545-600)

@@ -462,6 +462,46 @@ void hadamard_many(u256* const* outs, const u256* const* as, const u256* const* 
   k_hadamard_many<<<grid, 256, 0, s>>>(hb, n);
   SP_LAUNCHED(); check("hadamard_many");
 }
+// The descriptors of SP_PROD_MAX_CIRCUITS circuits (about 5 KB) travel as one kernel parameter: the large parameter space of sm_70+ with
+// CUDA >= 12.1 (up to 32764 bytes), so the launch needs no descriptor upload, no device allocation and no copy ahead of it.
+struct ProdBatch { ProdLeaves c[SP_PROD_MAX_CIRCUITS]; };
+static_assert(sizeof(ProdBatch) + sizeof(size_t) <= 32764, "k_prod_leaves: the descriptors exceed the kernel parameter space");
+__device__ __forceinline__ u256 prod_leaf(const ProdLeaves& d, const u256& idx_r2, size_t x) {
+  u256 v = d.flags & PROD_CST ? d.cst : fq_zero();
+  if (d.flags & PROD_IDX) {   // idx * x in Montgomery form: idx * R^2 times the plain integer x, one product
+    u256 xi = fq_zero();
+    xi.v[0] = (uint32_t)x; xi.v[1] = (uint32_t)(x >> 32);
+    v = fq_add(v, fq_mul(idx_r2, xi));
+  }
+#pragma unroll
+  for (int s = 0; s < SP_PROD_MAX_SOURCES; s++) {
+    if ((uint32_t)s >= d.nsrc) break;
+    const u256 t = ld256_ro(d.src[s] + x);
+    v = fq_add(v, (d.flags >> s) & PROD_UNIT0 ? t : fq_mul(d.coeff[s], t));
+  }
+  return v;
+}
+// a thread owns the pair (x, x + n/2): both leaves, and their product, the entry x of the first product layer
+__global__ void __launch_bounds__(256) k_prod_leaves(const ProdBatch b, size_t half) {
+  const ProdLeaves& d = b.c[blockIdx.y];
+  const u256 idx_r2 = d.flags & PROD_IDX ? fq_mul(d.idx, fq_R2()) : fq_zero();
+  for (size_t x = (size_t)blockIdx.x * blockDim.x + threadIdx.x; x < half; x += (size_t)gridDim.x * blockDim.x) {
+    const u256 lo = prod_leaf(d, idx_r2, x), hi = prod_leaf(d, idx_r2, x + half);
+    st256(d.layer0 + x, lo);
+    st256(d.layer0 + x + half, hi);
+    if (d.layer1) st256(d.layer1 + x, fq_mul(lo, hi));
+  }
+}
+void prod_leaves(const ProdLeaves* circuits, int k, size_t n, cudaStream_t s) {
+  if (k < 1 || k > SP_PROD_MAX_CIRCUITS || n < 2) throw std::runtime_error("spartan_b200: prod_leaves takes 1 .. SP_PROD_MAX_CIRCUITS circuits of >= 2 leaves");
+  double bytes = 0;
+  ProdBatch b;
+  for (int i = 0; i < k; i++) { b.c[i] = circuits[i]; bytes += (double)n * (32.0 * (circuits[i].nsrc + 1) + (circuits[i].layer1 ? 16.0 : 0.0)); }
+  ProfScope ps("prod_leaves", bytes, s);
+  dim3 grid(grid_for(n / 2, 256, 4), k);
+  k_prod_leaves<<<grid, 256, 0, s>>>(b, n / 2);
+  SP_LAUNCHED(); check("prod_leaves");
+}
 __global__ void k_to_canonical(u256* out, const u256* __restrict__ in, size_t n) {   // Scalar::to_bytes (ristretto255.rs:419) for a whole vector
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) st256(out + i, fq_from_mont(ld256_ro(in + i)));
 }

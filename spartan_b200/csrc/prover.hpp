@@ -215,6 +215,55 @@ void poly_sumcheck_prove(Ctx& ctx, const dev::ScPoly& P, size_t len, const Fq& c
 // SumcheckInstanceProof::verify (sumcheck.rs:27-62) on bincode bytes; SpError(SP_ERR_VERIFY) where the reference asserts or the bytes do not decode
 Fq sumcheck_verify_bytes(const uint8_t* proof, size_t len, const Fq& claim, size_t num_rounds, size_t degree, Transcript& T, std::vector<Fq>& r);
 
+// ---- product circuits (product.cpp): SPARK's memory check (snark_prove) and the caller's own (sp_prod_*)
+// ProductCircuit (product_tree.rs:11-63): every layer kept; layer k has n/2^k entries (left half | right half).
+// Single GPU: one 2n-scalar buffer, layer k at offset 2n - 2n/2^k.  Sharded over W ranks (cyclic partition: entry i of a layer on rank i mod W):
+// the big layers [0, Ks) hold only this rank's n/(2^k W) entries (`loc`, same offset rule on the local sizes) — the Hadamard product that builds
+// layer k+1 pairs i with i + len/2, which stay on one rank — and the layers from Ks on are replicated in `rep` (a circuit over n/2^Ks inputs).
+struct ProdCircuit {
+  DevBuf<u256> loc, rep;
+  size_t n = 0, num_layers = 0, Ks = 0;
+  int W = 1;
+  void alloc(Ctx& ctx, size_t n_) {
+    n = n_; num_layers = log2_ceil(n_); W = ctx.shard_world(); Ks = 0;
+    // layer k's sumcheck runs on tables of n/2^(k+1) entries: shard it while those are worth sharding
+    while (Ks + 1 < num_layers && ctx.shard_table((n >> Ks) / 2)) Ks++;
+    if (Ks) loc.alloc(2 * (n / W));
+    rep.alloc(2 * (n >> Ks));
+  }
+  bool sharded(size_t k) const { return k < Ks; }
+  size_t layer_len(size_t k) const { return n >> k; }                                  // global entries
+  size_t local_len(size_t k) const { return k < Ks ? (n >> k) / W : n >> k; }          // entries this rank holds
+  u256* layer(size_t k) {
+    if (k < Ks) { const size_t nl = n / W; return loc.p + (2 * nl - 2 * (nl >> k)); }
+    const size_t nr = n >> Ks, kk = k - Ks;
+    return rep.p + (2 * nr - 2 * (nr >> kk));
+  }
+};
+// every layer after layer `from` of a group of at most 16 equally sized circuits whose layers up to `from` are built: one launch per layer
+// (compute_layer, product_tree.rs:18-34); at the boundary between the sharded and the replicated layers the local products are all-gathered into
+// every rank's copy
+void build_circuits(Ctx& ctx, std::vector<ProdCircuit*> cs, size_t from = 0);
+// DotProductCircuit (product_tree.rs:66-108) of `len` entries; the tables the sumcheck binds are this rank's cyclic shards when `sharded`
+struct DotpCircuit { u256 *left, *right, *weight; size_t len; bool sharded; Fq claim; };
+// ProductCircuitEvalProofBatched::prove (product_tree.rs:259-383) with SumcheckInstanceProof::prove_cubic_batched (sumcheck.rs:254-424) inlined.
+// The product circuits' layers are bound in place.  rand_out: the point the proof ends on
+void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vector<DotpCircuit>& dotps, Transcript& T, ProductCircuitEvalProofBatched& out,
+                   std::vector<Fq>& rand_out);
+// what ProductCircuitEvalProofBatched::verify (product_tree.rs:385-485; verifier.cpp: batched_verify) returns: the product circuits' claims about
+// their leaf polynomials at rand, three claims per pair of dot-product circuits, and rand
+struct BatchedOut { std::vector<Fq> claims, claims_dotp, rand; };
+// ProductCircuitEvalProofBatched::verify(products, [], 2^m, T) on bincode bytes (sp_prod_verify_t): SpError(SP_ERR_VERIFY) where the reference
+// asserts or the bytes do not decode
+BatchedOut prod_verify(const uint8_t* proof, size_t len, const std::vector<Fq>& products, size_t m, Transcript& T);
+// The caller's circuits (sp_prod_build): `leaves` without their layer pointers, k <= SP_PROD_MAX_CIRCUITS of them over tables of n = 2^m >= 2
+// entries, on this rank's GPU alone.  Allocates every circuit, writes the leaves and the first product layer in one launch (dev::prod_leaves),
+// the other layers with build_circuits in groups of at most 16, and returns the k products (ProductCircuit::evaluate)
+std::vector<Fq> prod_build(Ctx& ctx, std::vector<dev::ProdLeaves> leaves, size_t n, std::vector<std::unique_ptr<ProdCircuit>>& out);
+// ProductCircuitEvalProofBatched::prove(circuits, [], T) of the caller's circuits (no dot-product circuits), on this rank's GPU alone; leaf_evals:
+// each circuit's leaf polynomial at rand, the claims the verifier is left with
+void prod_prove(Ctx& ctx, std::vector<ProdCircuit*>& cs, Transcript& T, ProductCircuitEvalProofBatched& out, std::vector<Fq>& rand, std::vector<Fq>& leaf_evals);
+
 // <x, G[0..n)> of one row of n scalars against the per-window table of `gs`, for latency.  For n >= 2 (even) it is the inner-product round kernel
 // with a = (1, 1) and blocks of two generators: its "L" (odd j) and "R" (even j) reach the host through the kernel's own publication and are added
 // there, one launch instead of msm_rows + reduce + compress + copy.  n = 1 runs msm_rows.  The constructor launches, collect() waits.

@@ -465,7 +465,6 @@ void r1cs_verify(Checker& chk, const R1CSProof& p, size_t num_vars, size_t num_c
 }
 
 // ---- SPARK
-struct BatchedOut { std::vector<Fq> claims, claims_dotp, rand; };
 // ProductCircuitEvalProofBatched::verify (product_tree.rs:385-485)
 BatchedOut batched_verify(const ProductCircuitEvalProofBatched& p, const std::vector<Fq>& claims_prod, const std::vector<Fq>& claims_dotp, size_t len, Transcript& T) {
   const size_t num_layers = log2_ceil(len), np = claims_prod.size();
@@ -743,6 +742,11 @@ void verify_batch(Ctx& ctx, std::vector<VerifyJob>& jobs, const uint8_t seed[32]
 }
 
 }  // namespace
+
+BatchedOut prod_verify(const uint8_t* proof, size_t len, const std::vector<Fq>& products, size_t m, Transcript& T) {
+  const ProductCircuitEvalProofBatched p = from_bincode<ProductCircuitEvalProofBatched>(proof, len, SP_ERR_VERIFY, "product circuit proof");
+  return batched_verify(p, products, {}, (size_t)1 << m, T);
+}
 
 Fq sumcheck_verify_bytes(const uint8_t* proof, size_t len, const Fq& claim, size_t num_rounds, size_t degree, Transcript& T, std::vector<Fq>& r) {
   const SumcheckInstanceProof p = from_bincode<SumcheckInstanceProof>(proof, len, SP_ERR_VERIFY, "sumcheck proof");
