@@ -224,6 +224,25 @@ def test_single_open_large_oracle_verifies(sb, ell):
 
 
 # ---------------------------------------------------------------------------------------------------- joint openings
+def oracle_joint_prove(Z, r, blinds, ell, ot, otape):
+    """(proof, evaluations) of the oracle's DerefsEvalProof.prove; with the joint commitment's blinds (DerefsEvalProof.prove has none) the same
+    steps with PolyEvalProof.prove given those blinds"""
+    k = len(Z)
+    c = shape(len(r), k)[0]
+    evals = [oc.evaluate(z, r) for z in Z]
+    merged = type("Merged", (), {"comb": sk.merge(Z)})
+    if blinds is None:
+        return sk.DerefsEvalProof.prove(merged, evals, [], r, ogens(ell), ot, otape).proof_derefs, evals
+    ot.append_protocol_name(b"Derefs evaluation proof")
+    ev = evals + [0] * (oc.next_pow2(k) - k)
+    ot.append_scalars(b"evals_ops_val", ev)
+    ch = ot.challenge_vector(b"challenge_combine_n_to_one", c)
+    for i in reversed(range(c)):
+        ev = oc.bound_bot_ints(ev, ch[i])
+    ot.append_scalar(b"joint_claim_eval", ev[0])
+    return pr.PolyEvalProof.prove(merged.comb, blinds, ch + r, ev[0], None, ogens(ell), ot, otape)[0], evals
+
+
 @pytest.mark.parametrize("m,k", JOINT)
 def test_joint_open_parity(sb, big, m, k):
     """parity with DerefsEvalProof.prove (the CPU model of test_pc_model.py is pinned to it), blinds of the joint commitment when k is odd"""
@@ -244,19 +263,7 @@ def test_joint_open_parity(sb, big, m, k):
     proof, evals = sb.PolyEvalProof.prove_joint(polys, blinds, oc.to_arr(r), g, st, stape)
     n = launches(sb)
     sb.api.prof_enable(False)
-    want_evals = [oc.evaluate(z, r) for z in Z]
-    merged = type("Merged", (), {"comb": sk.merge(Z)})
-    if k % 2:   # DerefsEvalProof.prove has no blinds: the same steps with PolyEvalProof.prove given the commitment's blinds
-        ot.append_protocol_name(b"Derefs evaluation proof")
-        ev = want_evals + [0] * (oc.next_pow2(k) - k)
-        ot.append_scalars(b"evals_ops_val", ev)
-        ch = ot.challenge_vector(b"challenge_combine_n_to_one", c)
-        for i in reversed(range(c)):
-            ev = oc.bound_bot_ints(ev, ch[i])
-        ot.append_scalar(b"joint_claim_eval", ev[0])
-        want, _ = pr.PolyEvalProof.prove(merged.comb, ints(blinds), ch + r, ev[0], None, ogens(ell), ot, otape)
-    else:
-        want = sk.DerefsEvalProof.prove(merged, want_evals, [], r, ogens(ell), ot, otape).proof_derefs
+    want, want_evals = oracle_joint_prove(Z, r, ints(blinds) if k % 2 else None, ell, ot, otape)
     assert ints(evals) == want_evals
     assert proof.data == pr.ser(want)
     assert same_transcript(ot, st) and same_tape(otape, stape)

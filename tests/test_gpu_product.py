@@ -2,7 +2,10 @@
 ProductCircuitEvalProofBatched): products, proof bytes, rand, leaf evaluations and transcript states against the oracle's ProductCircuit and
 ProductCircuitEvalProofBatched for plain and fingerprinted leaves on both sides of hadamard_many's 16-circuit group and of batched_prove's
 eq-factored threshold, the tables left as they were, a 2^22 batch checked by the library's verifier, a read-only memory check on one transcript
-with the oracle replaying it, the refusals, the launch counts, and the parity cases again under the memory-check mode."""
+with the oracle replaying it, the refusals, the launch counts, and the parity cases again under the memory-check mode.  The edge kind runs every
+affine form k_prod_leaves distinguishes (no source, a coefficient of 0 or q - 1, a unit coefficient before or after non-unit ones, one table as
+every source, index coefficients other than 0 and 1) on tables with zeros and runs of ones; 2^19 leaves take the kernel's grid-stride loop past
+its first pass on 132 SMs."""
 import json
 import os
 import subprocess
@@ -87,6 +90,36 @@ def fingerprint_descs(k, r, g):
     return out, 3 * ((k + 3) // 4)
 
 
+def edge_descs(k, r, g):
+    """the forms k_prod_leaves tells apart, cycled over k circuits of three tables: no source (index only, with index coefficients 2, r and
+    q - 1, or index and constant), a coefficient of 0 or q - 1, a unit coefficient at source 0 ahead of non-unit ones and the reverse, one table
+    as all three sources, a constant of q - 1, and a table alone (its zeros make the product 0; so do the index-only forms at x = 0)"""
+    forms = [([], 2, 0), ([], r, 0), ([], Q - 1, 0), ([], g, r),
+             ([(0, 0), (1, r)], 0, g),
+             ([(1, Q - 1), (2, r)], 1, 0),
+             ([(0, 1), (1, r), (2, Q - 1)], 0, 0),
+             ([(2, r), (1, Q - 1), (0, 1)], 2, g),
+             ([(0, r), (0, 1), (0, g)], 0, 0),
+             ([(1, r)], 0, Q - 1),
+             ([(0, 1)], 0, 0)]
+    return [forms[c % len(forms)] for c in range(k)], 3
+
+
+def edge_tables(n, tag):
+    """three tables with zeros, runs of ones and q - 1 planted at both ends and in the middle"""
+    T = [oc.prg_scalars("prod-gpu-%s-%d" % (tag, j), n) for j in range(3)]
+    zero, one, top = oc.to_arr([0, 1, Q - 1])
+    run = max(1, min(8, n // 4))
+    T[0][0] = T[0][n - 1] = T[0][n // 2] = zero
+    T[0][n // 4:n // 4 + run] = one
+    T[1][:run] = one
+    T[1][n - 1] = top
+    T[1][n // 2] = zero
+    T[2][n - run:] = one
+    T[2][0] = top
+    return T
+
+
 def case(sb, m, k, kind, tag):
     """tables, descriptors and the library's leaves argument (None for plain leaves: circuit i = table i)"""
     n = 1 << m
@@ -94,8 +127,11 @@ def case(sb, m, k, kind, tag):
         descs, nt = [([(c, 1)], 0, 0) for c in range(k)], k
     else:
         r, g = oc.to_ints(oc.prg_scalars("prod-gpu-rg-%s-%d-%d" % (tag, m, k), 2))
-        descs, nt = fingerprint_descs(k, r, g)
-    T = [oc.prg_scalars("prod-gpu-%s-%d-%d-%d" % (tag, m, k, j), n) for j in range(nt)]
+        descs, nt = (fingerprint_descs if kind == "fingerprint" else edge_descs)(k, r, g)
+    if kind == "edge":
+        T = edge_tables(n, "%s-%d-%d" % (tag, m, k))
+    else:
+        T = [oc.prg_scalars("prod-gpu-%s-%d-%d-%d" % (tag, m, k, j), n) for j in range(nt)]
     leaves = None if kind == "plain" else [sb.ProductLeaves(s, index_coeff=i, const=c) for s, i, c in descs]
     return T, descs, leaves
 
@@ -121,10 +157,22 @@ def prove_launches(m):
 
 
 # ---------------------------------------------------------------------------------------------------- parity with the oracle
-@pytest.mark.parametrize("kind", ["plain", "fingerprint"])
+@pytest.mark.parametrize("kind", ["plain", "fingerprint", "edge"])
 @pytest.mark.parametrize("k", KS)
 @pytest.mark.parametrize("m", MS)
 def test_build_prove_parity(sb, m, k, kind):
+    build_prove_parity(sb, m, k, kind)
+
+
+@pytest.mark.parametrize("kind", ["plain", "edge"])
+@pytest.mark.parametrize("k", [1, 2, 17])
+def test_build_prove_parity_second_grid_pass(sb, k, kind):
+    """2^19 leaves: 2^18 leaf pairs are more threads than k_prod_leaves' grid holds on 132 SMs (4 CTAs of 256 per SM), so each thread takes a
+    second pair"""
+    build_prove_parity(sb, 19, k, kind)
+
+
+def build_prove_parity(sb, m, k, kind):
     n = 1 << m
     T, descs, leaves = case(sb, m, k, kind, "par")
     polys = [sb.DensePolynomial(t) for t in T]
@@ -142,6 +190,12 @@ def test_build_prove_parity(sb, m, k, kind):
     assert same_transcript(ot, st)
     for p, t in zip(polys, T):   # read, never modified
         assert np.array_equal(p.to_numpy(), t)
+    if kind == "edge":   # the verifier's side of every form: sp_prod_leaf_eval on the host from the tables' values at rand
+        tev = [oc.evaluate(t, orand) for t in T]
+        want = [leaf_eval(d, tev, orand) for d in descs]
+        assert ints(sb.product_leaf_eval(leaves, oc.to_arr(tev), rand)) == want
+        assert ints(evals) == want
+        assert 0 in products
 
 
 def test_launch_counts(sb):

@@ -137,3 +137,34 @@ def test_table_list_rows_reproduce_commit_rows(m, k, blinded):
     assert got == want
     if not blinded:   # a padding row without a blind is the identity
         assert all(c == bytes(32) for c in want[k * ((1 << m) // R):])
+
+
+@pytest.mark.parametrize("sms,no_instance", [(114, ("window", 8, 4)), (132, None)])
+def test_limit_shapes_reach_every_branch(sms, no_instance):
+    """the chooser of test_gpu_poly_commit_limits.py finds a shape for every launch path of the joint commitment and every slab split of the
+    joint opening on 114 and 132 SMs, and each chosen shape takes the path it was chosen for.  Two paths no power-of-two table list reaches
+    while the set has its row table (the set skips it only when device memory is short, which a shared GPU cannot be made to be):
+    GROUPS = 1 of the table-list per-window MSM, since the per-window form runs only up to 2^16 merged entries, where L (R + 1) stays below
+    1024 per SM; and the per-window MSM's batches of 32768 rows, which need L > 32768, so ell >= 32.  On 114 SMs GROUPS = 8 with CPT = 4 is
+    not reached either: the shapes with 8 groups have too few blocks for four column passes."""
+    from test_gpu_poly_commit_limits import COMMIT_INSTANCES, OPEN_BRANCHES, choose_shapes, commit_branch, commit_shapes, open_branch
+    from test_gpu_poly_commit_limits import dims
+    commit, opening = choose_shapes(sms)
+    instances = COMMIT_INSTANCES - {no_instance}
+    assert {b[0] for b in commit} == instances
+    for inst in instances:
+        assert {b[1] for b in commit if b[0] == inst} == {"k = 1", "k = 2^c", "padded k"}, inst
+    assert {b[2] for b in commit if b[0] == "row table"} == {False, True}
+    for b, (m, k, bl) in commit.items():
+        assert commit_branch(m, k, bl, sms) == b
+    assert any(k == MAX_TABLES and commit_branch(m, k, bl, sms)[0] == "row table" for m, k, bl in commit_shapes(sms))
+    assert set(opening) == OPEN_BRANCHES
+    for b, (m, k) in opening.items():
+        assert open_branch(m, k, sms) == b or (b == "k > 32" and k > 32), b
+    # what stays unreached: no GROUPS = 1 on the per-window form of a table list, which a table list takes only up to 2^16 merged entries
+    for m in range(0, 31):
+        for k in range(1, MAX_TABLES + 1):
+            for bl in (False, True):
+                b = commit_branch(m, k, bl, sms)
+                if b is not None and b[0] != "row table":
+                    assert dims(m, k)[1] <= 16 and b[0][1] != 1, (m, k, bl, b)
