@@ -190,7 +190,8 @@ int sp_points_derive(sp_ctx* ctx, const uint8_t* label, size_t label_len, size_t
 size_t sp_points_len(const sp_points* p);
 void sp_points_free(sp_points* p);
 int sp_points_export(sp_ctx* ctx, const sp_points* p, size_t offset, size_t n, uint8_t* out32);
-/* GroupElement::vartime_multiscalar_mul(scalars[0..n), points[offset..offset+n)).compress() */
+/* GroupElement::vartime_multiscalar_mul(scalars[0..n), points[offset..offset+n)).compress(); SP_ERR_INVALID_ARG, before any launch, when
+ * [offset, offset + n) is not inside the set (an offset + n that wraps past 2^64 included), here and in sp_points_export */
 int sp_msm_var(sp_ctx* ctx, const sp_points* p, size_t offset, const uint64_t* scalars_mont, size_t n, uint8_t out32[32]);
 int sp_msm_var_resident(sp_ctx* ctx, const sp_points* p, size_t offset, const sp_poly* scalars, uint8_t out32[32]);
 /* every rank of a connected context passes its slice of the points and of the scalars; point-add all-reduce of the W partial sums; every rank

@@ -531,16 +531,21 @@ int sp_points_derive(sp_ctx* ctx, const uint8_t* label, size_t label_len, size_t
 }
 size_t sp_points_len(const sp_points* p) { return p->n; }
 void sp_points_free(sp_points* p) { delete p; }
+// [offset, offset + n) inside the point set, without forming offset + n (a caller's offset of 2^64 - 1 wraps it)
+static void points_range(const sp_points* p, size_t offset, size_t n, const char* what) {
+  if (offset > p->n || n > p->n - offset) throw SpError(SP_ERR_INVALID_ARG, std::string(what) + ": range outside the point set");
+}
 int sp_points_export(sp_ctx* ctx, const sp_points* p, size_t offset, size_t n, uint8_t* out32) {
   SP_TRY(ctx)
-  if (offset + n > p->n) throw SpError(SP_ERR_INVALID_ARG, "points_export: range outside the point set");
-  // 1 * P_i through the MSM path's own mixed addition, then compress
-  DevBuf<ge> g(n + 1);
-  DevBuf<uint8_t> comp(32 * n + 1);
-  dev::niels_to_ge(g.p, p->pts.p + offset, n, ctx->c.stream);
-  dev::compress_batch(comp.p, g.p, n, ctx->c.stream);
-  dev::d2h(out32, comp.p, 32 * n, ctx->c.stream);
-  ctx->c.sync();
+  points_range(p, offset, n, "points_export");
+  if (n) {   // 1 * P_i through the MSM path's own mixed addition, then compress (no empty launch for n = 0)
+    DevBuf<ge> g(n);
+    DevBuf<uint8_t> comp(32 * n);
+    dev::niels_to_ge(g.p, p->pts.p + offset, n, ctx->c.stream);
+    dev::compress_batch(comp.p, g.p, n, ctx->c.stream);
+    dev::d2h(out32, comp.p, 32 * n, ctx->c.stream);
+    ctx->c.sync();
+  }
   SP_CATCH(ctx)
 }
 // sharded: the MSM split over the ranks of a connected context.  Every rank passes ITS slice of the points (offset, scalars->len) and of the
@@ -548,7 +553,7 @@ int sp_points_export(sp_ctx* ctx, const sp_points* p, size_t offset, size_t n, u
 // returns the same encoding of the sum over all ranks.
 static void msm_var_run(Ctx& c, const sp_points* p, size_t offset, const u256* d_scalars, size_t n, uint8_t out32[32], bool sharded) {
   if (sharded && c.world() < 2) throw SpError(SP_ERR_INVALID_ARG, "not a connected multi-GPU context");
-  if (offset + n > p->n) throw SpError(SP_ERR_INVALID_ARG, "msm_var: range outside the point set");
+  points_range(p, offset, n, "msm_var");
   DevBuf<ge> out(1), total;
   DevBuf<uint8_t> comp(32);
   if (n == 0) {
@@ -577,6 +582,7 @@ int sp_msm_var_sharded(sp_ctx* ctx, const sp_points* p, size_t offset, const sp_
 }
 int sp_msm_var(sp_ctx* ctx, const sp_points* p, size_t offset, const uint64_t* scalars, size_t n, uint8_t out32[32]) {
   SP_TRY(ctx)
+  points_range(p, offset, n, "msm_var");   // before the scalars' upload
   DevBuf<u256> d(n ? n : 1);
   dev::h2d(d.p, scalars, n * 32, ctx->c.stream);
   msm_var_run(ctx->c, p, offset, d.p, n, out32, false);

@@ -728,6 +728,16 @@ int spd_msm_var_segmented(size_t K, size_t n, const ge* pts, const u256* scalars
     return (int)c.err;
   });
 }
+// the launch plan msm_var runs for n points (pip_plan, c_override = 0: the default window width):
+// out = {c, nwin, nb, tile, ntiles, G, S, max_items, pip_scratch_bytes}
+int spd_pip_plan(size_t n, int c_override, uint64_t out[9]) {
+  return guarded([&] {
+    const PipPlan p = pip_plan(n, c_override);
+    const uint64_t v[9] = {(uint64_t)p.c, (uint64_t)p.nwin, p.nb, p.tile, p.ntiles, (uint64_t)p.G, p.S, p.max_items, pip_scratch_bytes(p)};
+    memcpy(out, v, sizeof(v));
+    return 0;
+  });
+}
 // ipa_srow over `nitems` rows packed back to back in rows[0 .. total) (in, out): item i writes or adds 2^lg_n[i] entries at row_off[i];
 // u_sq: 32 scalars per item
 int spd_ipa_srow(size_t nitems, const uint32_t* lg_n, const uint32_t* add, const u256* allinv, const u256* scale, const u256* u_sq, const uint64_t* row_off,

@@ -85,8 +85,8 @@ def test_context_scratch_refilled_every_call(memcheck):
 
 # ---------------------------------------------------------------------------------------------------- b. the suite under the mode
 SUITE = ["test_gpu_kernels.py", "test_gpu_arith.py", "test_gpu_golden.py", "test_gpu_sumcheck_poly.py", "test_gpu_sumcheck_poly_limits.py",
-         "test_gpu_msm_var.py", "test_row_msm.py", "test_gpu_msm_instances.py", "test_gpu_verify_batch.py", "test_gpu_instance_device.py",
-         "test_gpu_snark.py", "test_gpu_gen_tables.py", "test_gpu_instance_shapes.py"]
+         "test_gpu_msm_var.py", "test_gpu_msm_var_limits.py", "test_row_msm.py", "test_gpu_msm_instances.py", "test_gpu_verify_batch.py",
+         "test_gpu_instance_device.py", "test_gpu_snark.py", "test_gpu_gen_tables.py", "test_gpu_instance_shapes.py"]
 DESELECT = {
     # starts one process per MSM window width; those processes run without the mode (the window widths' kernels are each checked in-process by
     # test_msm_rows_every_instance)
