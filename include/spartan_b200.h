@@ -6,6 +6,7 @@
  * replaces (paths relative to /root/reference).  Conventions:
  *   - every function returns an int status: SP_OK or an SP_ERR_* code; sp_last_error() gives the message.  No exception or
  *     panic crosses the boundary (the reference panics on misuse, e.g. src/r1csproof.rs:156).
+ *   - a transcript or tape state whose position bytes are out of range is refused with SP_ERR_INVALID_ARG.
  *   - scalars cross as `uint64_t[4]` little-endian limbs in MONTGOMERY form = the in-memory layout of `Scalar`
  *     (src/scalar/ristretto255.rs:195-199), so a Rust `&[Scalar]` is passed as-is (`as_ptr() as *const u64`).
  *     Where the reference API takes canonical bytes (`[u8;32]`, src/lib.rs:64,121) so does this ABI.

@@ -98,8 +98,43 @@ def _limbs(a):
     return a.reshape(-1, 4)
 
 
-class Context:
+def _status_error(rc, msg):
+    """the exception for a failed call's status and message"""
+    if rc == SP_ERR_INVALID_INDEX:
+        return R1CSError("InvalidIndex: " + msg)
+    if rc == SP_ERR_INVALID_SCALAR:
+        return R1CSError("InvalidScalar: " + msg)
+    if rc == SP_ERR_INVALID_INPUTS:
+        return R1CSError("InvalidNumberOfInputs: " + msg)
+    if rc == SP_ERR_VERIFY:
+        return ProofVerifyError("InternalError: " + msg, rc)
+    if rc == SP_ERR_DECOMPRESS:
+        return ProofVerifyError("DecompressionError: " + msg, rc)
+    return SpartanB200Error("spartan_b200 error %d: %s" % (rc, msg))
+
+
+def _check_host(rc):
+    """raises for a failed host-only call, whose message sp_last_error(NULL) holds"""
+    if rc != SP_OK:
+        raise _status_error(rc, lib.sp_last_error(None).decode())
+
+
+class _Handle:
+    """owner of one library object `h`, released by the class's `_free` when the Python object goes"""
+    _free = None
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None):
+                self._free(self.h)
+                self.h = None
+        except Exception:
+            pass
+
+
+class Context(_Handle):
     """One per GPU / host thread.  Fails loudly when no CUDA device is present."""
+    _free = lib.sp_ctx_destroy
 
     def __init__(self, device=0):
         h = _vp()
@@ -110,20 +145,8 @@ class Context:
         self.device = device
 
     def check(self, rc):
-        if rc == SP_OK:
-            return
-        msg = lib.sp_last_error(self.h).decode()
-        if rc == SP_ERR_INVALID_INDEX:
-            raise R1CSError("InvalidIndex: " + msg)
-        if rc == SP_ERR_INVALID_SCALAR:
-            raise R1CSError("InvalidScalar: " + msg)
-        if rc == SP_ERR_INVALID_INPUTS:
-            raise R1CSError("InvalidNumberOfInputs: " + msg)
-        if rc == SP_ERR_VERIFY:
-            raise ProofVerifyError("InternalError: " + msg, rc)
-        if rc == SP_ERR_DECOMPRESS:
-            raise ProofVerifyError("DecompressionError: " + msg, rc)
-        raise SpartanB200Error("spartan_b200 error %d: %s" % (rc, msg))
+        if rc != SP_OK:
+            raise _status_error(rc, lib.sp_last_error(self.h).decode())
 
     def connect_peers(self, rank, world, allgather):
         """Join `world` single-GPU processes into one sharded prover (sp_comm_export / sp_comm_connect).  `allgather(b: bytes) -> list[bytes]`
@@ -155,14 +178,6 @@ class Context:
                 k, v = item.split("=")
                 out[k] = float(v)
         return out
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.sp_ctx_destroy(self.h)
-                self.h = None
-        except Exception:
-            pass
 
 
 _default_ctx = None
@@ -239,8 +254,9 @@ def _sync_torch(ctx):
 
 
 # ----------------------------------------------------------------------------- operator level
-class DensePolynomial:
+class DensePolynomial(_Handle):
     """dense_mlpoly.rs:18-22 with Z resident on the device"""
+    _free = lib.sp_poly_free
 
     def __init__(self, Z, ctx=None):
         self.ctx = ctx or default_context()
@@ -309,14 +325,6 @@ class DensePolynomial:
         h = _vp()
         ctx.check(lib.sp_eq_evals(ctx.h, _p(r), _sz(len(r)), C.byref(h)))
         return DensePolynomial._wrap(ctx, h)
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.sp_poly_free(self.h)
-                self.h = None
-        except Exception:
-            pass
 
 
 def sumcheck_eval(kind, polys):
@@ -433,18 +441,14 @@ def sumcheck_verify(proof, claim, num_rounds, degree_bound, transcript):
     proof = bytes(proof)
     e = np.zeros(4, dtype=np.uint64)
     r = np.zeros((num_rounds, 4), dtype=np.uint64)
-    rc = lib.sp_sumcheck_verify_t(None, C.c_char_p(proof), _sz(len(proof)), _p(np.ascontiguousarray(claim, dtype=np.uint64)), _sz(num_rounds),
-                                  _sz(degree_bound), t.state, _p(e), _p(r))
-    if rc == SP_OK:
-        return e, r
-    msg = lib.sp_last_error(None).decode()
-    if rc == SP_ERR_VERIFY:
-        raise ProofVerifyError("InternalError: " + msg, rc)
-    raise SpartanB200Error("spartan_b200 error %d: %s" % (rc, msg))
+    _check_host(lib.sp_sumcheck_verify_t(None, C.c_char_p(proof), _sz(len(proof)), _p(np.ascontiguousarray(claim, dtype=np.uint64)), _sz(num_rounds),
+                                         _sz(degree_bound), t.state, _p(e), _p(r)))
+    return e, r
 
 
-class MultiCommitGens:
+class MultiCommitGens(_Handle):
     """commitments.rs:8-33"""
+    _free = lib.sp_gens_free
 
     def __init__(self, n, label, ctx=None):
         self.ctx = ctx or default_context()
@@ -476,18 +480,11 @@ class MultiCommitGens:
         self.ctx.check(lib.sp_msm(self.ctx.h, self.h, _p(s), _sz(len(s)), out))
         return out.raw
 
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.sp_gens_free(self.h)
-                self.h = None
-        except Exception:
-            pass
 
-
-class BulletReduction:
+class BulletReduction(_Handle):
     """operator-level BulletReductionProof::prove (nizk/bullet.rs:32-132): the device keeps a, b and the (implicitly folded) generators, the
     caller keeps the transcript.  round_LR() -> (L, R) compressed; fold(u, u_inv); finish() -> (a_hat, b_hat, G_hat compressed)."""
+    _free = lib.sp_ipa_free
 
     def __init__(self, gens, a_vec, b_vec):
         self.ctx = gens.ctx
@@ -509,17 +506,10 @@ class BulletReduction:
         self.ctx.check(lib.sp_ipa_finish(self.ctx.h, self.h, _p(a), _p(b), g))
         return a, b, g.raw
 
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.sp_ipa_free(self.h)
-                self.h = None
-        except Exception:
-            pass
 
-
-class Points:
+class Points(_Handle):
     """A caller-supplied `&[GroupElement]` (group.rs:8-9) resident on the device, for the variable-base MSM (bucket method, no tables)."""
+    _free = lib.sp_points_free
 
     def __init__(self, compressed, ctx=None):
         """compressed: list of 32-byte ristretto255 encodings; raises if any does not decompress"""
@@ -563,14 +553,6 @@ class Points:
         self.ctx.check(lib.sp_msm_var_sharded(self.ctx.h, self.h, _sz(offset), scalars.h, out))
         return out.raw
 
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.sp_points_free(self.h)
-                self.h = None
-        except Exception:
-            pass
-
 
 def point_roundtrip(points, ctx=None):
     ctx = ctx or default_context()
@@ -598,19 +580,20 @@ class Transcript:
 
     def append_message(self, label, msg):
         msg = bytes(msg)
-        lib.sp_transcript_append_message(self.state, C.c_char_p(label), _sz(len(label)), C.c_char_p(msg), _sz(len(msg)))
+        _check_host(lib.sp_transcript_append_message(self.state, C.c_char_p(label), _sz(len(label)), C.c_char_p(msg), _sz(len(msg))))
 
     def challenge_bytes(self, label, n):
         out = C.create_string_buffer(n)
-        lib.sp_transcript_challenge_bytes(self.state, C.c_char_p(label), _sz(len(label)), out, _sz(n))
+        _check_host(lib.sp_transcript_challenge_bytes(self.state, C.c_char_p(label), _sz(len(label)), out, _sz(n)))
         return out.raw
 
 
 # ----------------------------------------------------------------------------- polynomial commitments of the caller's tables
-class PolyCommitmentGens:
+class PolyCommitmentGens(_Handle):
     """PolyCommitmentGens::new(num_vars, label) (dense_mlpoly.rs:29-36): the n = 2^(num_vars - num_vars/2) generators of gens_n, G_1 and h of the
     label's stream, with their device tables (footprint: include/spartan_b200.h, sp_pc_gens_create).  view(num_vars) gives the gens of a smaller
     num_vars of the same label as a view of these tables."""
+    _free = lib.sp_pc_gens_free
 
     def __init__(self, num_vars, label, ctx=None):
         self.ctx = ctx or default_context()
@@ -627,14 +610,6 @@ class PolyCommitmentGens:
         o.h = h
         return o
 
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.sp_pc_gens_free(self.h)
-                self.h = None
-        except Exception:
-            pass
-
 
 class RandomTape(Transcript):
     """RandomTape::new(b"proof") (random.rs:10-17) as caller state (a merlin transcript, advanced in place by the calls that draw from it).
@@ -644,9 +619,7 @@ class RandomTape(Transcript):
     def __init__(self, seed=None):
         s = random_tape_seed() if seed is None else np.ascontiguousarray(seed, dtype=np.uint64).reshape(4)
         self.state = C.create_string_buffer(203)
-        rc = lib.sp_random_tape_new(_p(s), self.state)
-        if rc != SP_OK:
-            raise SpartanB200Error("spartan_b200 error %d: %s" % (rc, lib.sp_last_error(None).decode()))
+        _check_host(lib.sp_random_tape_new(_p(s), self.state))
 
 
 class PolyCommitment:
@@ -792,10 +765,11 @@ def _c_leaves(leaves):
     return arr
 
 
-class ProductCircuits:
+class ProductCircuits(_Handle):
     """ProductCircuit::new of k circuits, then ProductCircuit::evaluate (product_tree.rs:36-63), on the GPU: `tables` are DensePolynomials of
     one length 2^m (m >= 1), read and never modified; `leaves` a list of ProductLeaves (at most SP_PROD_MAX_CIRCUITS), or None for one circuit
     per table.  .products: the k products as (k, 4) limbs; .num_vars = m.  ProductCircuitEvalProofBatched.prove consumes the circuits."""
+    _free = lib.sp_prod_free
 
     def __init__(self, tables, leaves=None):
         tables = _poly_list(tables)
@@ -808,14 +782,6 @@ class ProductCircuits:
         self.h = h
         self.products = products[:self.k]
         self.num_vars = tables[0].len().bit_length() - 1
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.sp_prod_free(self.h)
-                self.h = None
-        except Exception:
-            pass
 
 
 class ProductCircuitEvalProofBatched:
@@ -839,16 +805,9 @@ class ProductCircuitEvalProofBatched:
         t, proof, prods = _transcript_state(transcript), bytes(proof), _limbs(products)
         rand = np.zeros((max(num_vars, 1), 4), dtype=np.uint64)
         claims = np.zeros((max(len(prods), 1), 4), dtype=np.uint64)
-        rc = lib.sp_prod_verify_t(None, C.c_char_p(proof), _sz(len(proof)), _p(prods), C.c_int(len(prods)), _sz(num_vars), t.state, _p(rand),
-                                  _p(claims))
-        if rc == SP_OK:
-            return rand[:num_vars], claims[:len(prods)]
-        msg = lib.sp_last_error(None).decode()
-        if rc == SP_ERR_VERIFY:
-            raise ProofVerifyError("InternalError: " + msg, rc)
-        if rc == SP_ERR_INVALID_SCALAR:
-            raise R1CSError("InvalidScalar: " + msg)
-        raise SpartanB200Error("spartan_b200 error %d: %s" % (rc, msg))
+        _check_host(lib.sp_prod_verify_t(None, C.c_char_p(proof), _sz(len(proof)), _p(prods), C.c_int(len(prods)), _sz(num_vars), t.state, _p(rand),
+                                         _p(claims)))
+        return rand[:num_vars], claims[:len(prods)]
 
 
 def product_leaf_eval(leaves, table_evals, rand):
@@ -857,12 +816,7 @@ def product_leaf_eval(leaves, table_evals, rand):
     ev, r = _limbs(table_evals), _limbs(rand)
     k = len(ev) if leaves is None else len(leaves)
     out = np.zeros((max(k, 1), 4), dtype=np.uint64)
-    rc = lib.sp_prod_leaf_eval(_c_leaves(leaves), C.c_int(k), _p(ev), C.c_int(len(ev)), _p(r), _sz(len(r)), _p(out))
-    if rc != SP_OK:
-        msg = lib.sp_last_error(None).decode()
-        if rc == SP_ERR_INVALID_SCALAR:
-            raise R1CSError("InvalidScalar: " + msg)
-        raise SpartanB200Error("spartan_b200 error %d: %s" % (rc, msg))
+    _check_host(lib.sp_prod_leaf_eval(_c_leaves(leaves), C.c_int(k), _p(ev), C.c_int(len(ev)), _p(r), _sz(len(r)), _p(out)))
     return out[:k]
 
 
@@ -890,8 +844,9 @@ VarsAssignment = Assignment
 InputsAssignment = Assignment
 
 
-class Instance:
+class Instance(_Handle):
     """lib.rs:111-274"""
+    _free = lib.sp_instance_free
 
     def __init__(self, ctx, h):
         self.ctx, self.h = ctx, h
@@ -986,14 +941,6 @@ class Instance:
         self.ctx.check(lib.sp_instance_is_sat(self.ctx.h, self.h, _p(vars.limbs), _sz(len(vars)), _p(inputs.limbs), _sz(len(inputs)), C.byref(sat)))
         return bool(sat.value)
 
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.sp_instance_free(self.h)
-                self.h = None
-        except Exception:
-            pass
-
 
 def _take_bytes(out, n):
     b = C.string_at(out, n.value)
@@ -1005,11 +952,12 @@ class _GenSetInfo(C.Structure):
     _fields_ = [("label", C.c_char * 32), ("nbases", C.c_size_t), ("window_bits", C.c_int), ("has_row_table", C.c_int), ("device_bytes", C.c_size_t)]
 
 
-class GeneratorTables:
+class GeneratorTables(_Handle):
     """Generator tables sized once for the largest circuit a caller proves (sp_gen_tables): the gens_r1cs_sat set for circuits up to
     (num_cons, num_vars, num_inputs) and, if num_nz_entries > 0, the gens_r1cs_eval set up to that many non-zeros.  NIZKGens(..., tables=t)
     and SNARKGens(..., tables=t) for any circuit whose every dimension is <= these are views that share the tables' device memory and prove
     the same bytes as gens of their own.  Views keep the tables alive: `del` this object whenever convenient."""
+    _free = lib.sp_gen_tables_free
 
     def __init__(self, num_cons, num_vars, num_inputs, num_nz_entries=0, ctx=None):
         self.ctx = ctx or default_context()
@@ -1024,14 +972,6 @@ class GeneratorTables:
         return [{"label": s.label.decode(), "nbases": int(s.nbases), "window_bits": int(s.window_bits), "has_row_table": bool(s.has_row_table),
                  "device_bytes": int(s.device_bytes)} for s in out[:n.value]]
 
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.sp_gen_tables_free(self.h)
-                self.h = None
-        except Exception:
-            pass
-
 
 def device_bytes_live():
     """device bytes in blocks the library holds for live objects (its cache of freed blocks excluded): unlike the driver's free-memory
@@ -1039,8 +979,9 @@ def device_bytes_live():
     return int(lib.sp_device_bytes_live())
 
 
-class NIZKGens:
+class NIZKGens(_Handle):
     """lib.rs:468-486.  tables=GeneratorTables: a view into them instead of generator tables of its own"""
+    _free = lib.sp_nizk_gens_free
 
     def __init__(self, num_cons, num_vars, num_inputs, ctx=None, tables=None):
         self.ctx = ctx or (tables.ctx if tables is not None else default_context())
@@ -1054,14 +995,6 @@ class NIZKGens:
     @staticmethod
     def new(num_cons, num_vars, num_inputs, ctx=None):
         return NIZKGens(num_cons, num_vars, num_inputs, ctx)
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.sp_nizk_gens_free(self.h)
-                self.h = None
-        except Exception:
-            pass
 
 
 class NIZK:
@@ -1108,8 +1041,9 @@ class NIZK:
         return _verify_batch(gens.ctx, lib.sp_nizk_verify_batch, lib.sp_nizk_verify_batch_t, inst, proofs, inputs, transcript_label, gens, seed)
 
 
-class SNARKGens:
+class SNARKGens(_Handle):
     """lib.rs:277-309.  tables=GeneratorTables (built with num_nz_entries > 0): a view into them instead of generator tables of its own"""
+    _free = lib.sp_snark_gens_free
 
     def __init__(self, num_cons, num_vars, num_inputs, num_nz_entries, ctx=None, tables=None):
         self.ctx = ctx or (tables.ctx if tables is not None else default_context())
@@ -1125,17 +1059,10 @@ class SNARKGens:
     def new(num_cons, num_vars, num_inputs, num_nz_entries, ctx=None):
         return SNARKGens(num_cons, num_vars, num_inputs, num_nz_entries, ctx)
 
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.sp_snark_gens_free(self.h)
-                self.h = None
-        except Exception:
-            pass
 
-
-class ComputationCommitment:
+class ComputationCommitment(_Handle):
     """(ComputationCommitment, ComputationDecommitment) pair of SNARK::encode (lib.rs:44-55): the decommitment stays on the device"""
+    _free = lib.sp_snark_encoding_free
 
     def __init__(self, ctx, h):
         self.ctx, self.h = ctx, h
@@ -1152,14 +1079,6 @@ class ComputationCommitment:
         out, n = C.POINTER(C.c_ubyte)(), _sz()
         lib.sp_snark_commitment_bytes(self.h, C.byref(out), C.byref(n))
         return _take_bytes(out, n)
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.sp_snark_encoding_free(self.h)
-                self.h = None
-        except Exception:
-            pass
 
 
 class SNARK:

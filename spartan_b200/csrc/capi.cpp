@@ -1,4 +1,5 @@
-// spartan_b200 — extern "C" boundary (include/spartan_b200.h).  Catches every exception and maps it to a status code.
+// spartan_b200 — extern "C" boundary (include/spartan_b200.h).  Every entry that can fail runs its body through guarded() or host_guarded(),
+// which catch every exception and map it to a status code.
 #include "../../include/spartan_b200.h"
 #include <stdlib.h>
 #include <algorithm>
@@ -17,21 +18,44 @@ struct sp_nizk_gens { std::unique_ptr<R1CSGens> g; };
 struct sp_snark_gens { std::unique_ptr<SnarkGens> g; };
 struct sp_snark_encoding { std::unique_ptr<SnarkEncoding> e; };
 struct sp_gen_tables { std::unique_ptr<GenTables> t; };
+struct sp_pc_gens {
+  Ctx* ctx;
+  std::shared_ptr<GenSet> set;   // shared by the views made from it
+  size_t num_vars;
+  PolyCommitmentGens g;
+};
+struct sp_prod_circuits {
+  Ctx* ctx;
+  size_t m;
+  std::vector<std::unique_ptr<ProdCircuit>> cs;   // released by the proof
+  bool spent;
+};
 
-static std::string g_create_error;
+// the message sp_last_error(NULL) reads: of the last failed sp_ctx_create, or of the last failed host-only call made without a context
+static std::string g_last_error;
 
-// every entry point with a context starts from refilled persistent scratch under the memory-check mode (Ctx::memcheck_refill)
-#define SP_TRY(ctxp) try { if (ctxp) (ctxp)->c.memcheck_refill();
-#define SP_CATCH(ctxp)                                                                           \
-  }                                                                                              \
-  catch (const SpError& e) { if (ctxp) (ctxp)->c.last_error = e.what(); return e.code; }        \
-  catch (const std::exception& e) {                                                              \
-    if (ctxp) (ctxp)->c.last_error = e.what();                                                   \
-    return std::string(e.what()).find("CUDA") != std::string::npos ? SP_ERR_CUDA : SP_ERR_INTERNAL; \
-  }                                                                                              \
-  catch (...) { if (ctxp) (ctxp)->c.last_error = "unknown error"; return SP_ERR_INTERNAL; }      \
-  return SP_OK;
+// ---- the catch ladder.  host_guarded: entries without device work; the message goes to the context when one is given, else to g_last_error.
+template <class F>
+static int host_guarded(sp_ctx* ctx, const F& body) {
+  std::string& err = ctx ? ctx->c.last_error : g_last_error;
+  try {
+    body();
+    return SP_OK;
+  } catch (const SpError& e) { err = e.what(); return e.code; }
+  catch (const dev::CudaError& e) { err = e.what(); return SP_ERR_CUDA; }
+  catch (const std::exception& e) { err = e.what(); return SP_ERR_INTERNAL; }
+  catch (...) { err = "unknown error"; return SP_ERR_INTERNAL; }
+}
+// guarded: entries with a context, which start from refilled persistent scratch under the memory-check mode (Ctx::memcheck_refill)
+template <class F>
+static int guarded(sp_ctx* ctx, const F& body) {
+  return host_guarded(ctx, [&] {
+    if (ctx) ctx->c.memcheck_refill();
+    body();
+  });
+}
 
+// ---- scalars and results
 static Fq fq_in(const uint64_t l[4]) { Fq f; memcpy(&f.m, l, 32); return f; }
 static void fq_out(uint64_t l[4], const Fq& f) { memcpy(l, &f.m, 32); }
 static std::vector<Fq> fq_vec(const uint64_t* l, size_t n) { std::vector<Fq> v(n); if (n) memcpy(v.data(), l, 32 * n); return v; }
@@ -40,20 +64,219 @@ static void require_reduced(const uint64_t* l, size_t n, const char* what) {
   for (size_t i = 0; i < n; i++)
     if (!fq_bytes_canonical(reinterpret_cast<const uint8_t*>(l + 4 * i))) throw SpError(SP_ERR_INVALID_SCALAR, std::string(what) + ": scalar limbs are not reduced modulo q");
 }
-static uint8_t* dup_bytes(const std::vector<uint8_t>& v) { uint8_t* p = (uint8_t*)malloc(v.size() ? v.size() : 1); memcpy(p, v.data(), v.size()); return p; }
+// bytes handed to the caller, who releases them with sp_free
+static void put_bytes(uint8_t** out, size_t* out_len, const std::vector<uint8_t>& v) {
+  uint8_t* p = (uint8_t*)malloc(v.size() ? v.size() : 1);
+  memcpy(p, v.data(), v.size());
+  *out = p;
+  *out_len = v.size();
+}
+static void put_scalars(uint64_t* out, const std::vector<Fq>& v) { if (!v.empty()) memcpy(out, v.data(), 32 * v.size()); }
+
+// ---- argument checks shared by the caller-facing entries
+static void require_count(const std::string& what, int k, const char* noun, const char* max_name, int max) {
+  if (k < 1 || k > max)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": " + std::to_string(k) + " " + noun + "; 1 .. " + max_name + " = " + std::to_string(max) + " supported");
+}
+// a handle the call reads: not NULL, and made on this context
+template <class H>
+static void require_owned(const sp_ctx* ctx, const H* h, const std::string& what, const std::string& name) {
+  if (!h) throw SpError(SP_ERR_INVALID_ARG, what + ": " + name + " is NULL");
+  if (h->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, what + ": " + name + " belongs to another context");
+}
+// the k >= 1 tables of one call: handles of this context, of one power-of-two length >= min_len
+struct Tables { size_t len; std::vector<const u256*> d; };
+static Tables caller_tables(const sp_ctx* ctx, sp_poly* const* polys, int k, const std::string& what, size_t min_len) {
+  if (!polys) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL table array");
+  Tables t{0, std::vector<const u256*>(k)};
+  for (int i = 0; i < k; i++) {
+    require_owned(ctx, polys[i], what, "table " + std::to_string(i));
+    if (polys[i]->len != polys[0]->len) throw SpError(SP_ERR_INVALID_ARG, what + ": tables differ in length");
+    t.d[i] = polys[i]->d.p;
+  }
+  t.len = polys[0]->len;
+  if (t.len < min_len || (t.len & (t.len - 1)))
+    throw SpError(SP_ERR_INVALID_ARG, what + ": the table length must be a power of two >= " + std::to_string(min_len) + ", got " + std::to_string(t.len));
+  return t;
+}
+
+// ---- transcripts and witnesses of the proof entries
+// the caller's transcript: either a fresh Transcript::new(label) or (the _t entry points) the caller-owned STROBE state, updated in place
+struct TranscriptArg {
+  const uint8_t* label; size_t label_len; uint8_t* state; bool from_state;
+  static TranscriptArg fresh(const uint8_t* label, size_t label_len) { return {label, label_len, nullptr, false}; }
+  static TranscriptArg caller(uint8_t* state) { return {nullptr, 0, state, true}; }
+  void check() const { if (from_state && !state) throw SpError(SP_ERR_INVALID_ARG, "transcript state is NULL"); }
+  Transcript open() const { return from_state ? Transcript(Transcript::FromState(), state) : Transcript(std::string((const char*)label, label_len)); }
+  void close(const Transcript& T) const { if (from_state) T.export_state(state); }
+};
+// the verifiers' _t forms update the caller's transcript state whether or not the proof is accepted (a _t prove writes it back only on success)
+struct TranscriptClose { const TranscriptArg& ta; const Transcript& T; ~TranscriptClose() { ta.close(T); } };
+static DevBuf<u256> upload_padded_vars(Ctx& c, const Instance& I, const uint64_t* vars, size_t nvars) {
+  if (nvars > I.num_vars) throw SpError(SP_ERR_INVALID_INPUTS, "R1CSError::InvalidNumberOfInputs (vars)");
+  DevBuf<u256> d(I.num_vars);
+  dev::h2d(d.p, vars, nvars * 32, c.stream);
+  if (nvars < I.num_vars) dev::dzero(d.p + nvars, (I.num_vars - nvars) * 32, c.stream);  // Assignment::pad (lib.rs:91-104)
+  return d;
+}
+// the witness of a prove call: the caller's host limbs, padded on upload (Assignment::pad), or a resident poly already padded to num_vars
+struct VarsArg { const uint64_t* host; size_t nvars; const sp_poly* resident; };
+static const u256* vars_on_device(Ctx& c, const Instance& I, const VarsArg& v, DevBuf<u256>& upload) {
+  if (!v.resident) { upload = upload_padded_vars(c, I, v.host, v.nvars); return upload.p; }
+  if (v.resident->len != I.num_vars) throw SpError(SP_ERR_INVALID_INPUTS, "resident vars must already be padded to num_vars");
+  return v.resident->d.p;
+}
+// The body NIZK and SNARK proofs share.  `prove(d_vars, inputs, T, seed)` runs the statement's own prover and returns the proof's bincode.
+template <class Prove>
+static void prove_statement(Ctx& c, const Instance& I, const VarsArg& vars, const uint64_t* inputs, size_t ninputs, const TranscriptArg& ta,
+                            const uint64_t seed[4], uint8_t** proof, size_t* proof_len, const Prove& prove) {
+  ta.check();
+  DevBuf<u256> upload;
+  const u256* d_vars = vars_on_device(c, I, vars, upload);
+  if (ninputs != I.num_inputs) throw SpError(SP_ERR_INVALID_INPUTS, "R1CSError::InvalidNumberOfInputs");
+  if (!seed) throw SpError(SP_ERR_INVALID_ARG, "tape seed is NULL: draw it from the OS RNG (random.rs:13-15); a fixed seed makes every blind public");
+  require_reduced(inputs, ninputs, "inputs"); require_reduced(seed, 1, "tape seed");
+  Transcript T = ta.open();
+  const std::vector<uint8_t> bytes = prove(d_vars, fq_vec(inputs, ninputs), T, fq_in(seed));
+  ta.close(T);
+  put_bytes(proof, proof_len, bytes);
+}
+// SP_FINE_TIMERS=1: the sub-phase timers of the last verify call (single or batch) replace sp_timings, as a prove call's do
+static void flush_fine(Ctx& c) {
+  if (!FineTimer::enabled()) return;
+  c.timings.clear();
+  for (auto& f : c.fine) c.timings.push_back({"fine:" + f.first, f.second});
+  c.fine.clear();
+}
+// The body NIZK and SNARK verification share.  `verify(inputs, T)` runs the statement's own verifier.
+template <class Verify>
+static int verify_statement(sp_ctx* ctx, const uint64_t* inputs, size_t ninputs, const TranscriptArg& ta, const Verify& verify) {
+  return guarded(ctx, [&] {
+    ta.check();
+    require_reduced(inputs, ninputs, "inputs");
+    Transcript T = ta.open();
+    TranscriptClose close{ta, T};
+    verify(fq_vec(inputs, ninputs), T);
+    flush_fine(ctx->c);
+  });
+}
+
+// ---- batch verifiers: proof i is checked as the single call would check it (statement i, inputs i, label i or caller transcript i); the group
+// equations of all of them are tested in one device pass (verifier.cpp, DESIGN.md "deferred checks")
+struct BatchArgs {
+  size_t k;
+  const uint64_t* const* inputs; const size_t* ninputs;
+  const uint8_t* const* labels; const size_t* label_lens;   // fresh transcripts, or
+  uint8_t* const* states;                                    // the callers' transcripts (the _t forms)
+  const uint8_t* const* proofs; const size_t* proof_lens;
+  const uint8_t* seed; int* status;
+};
+static std::vector<VerifyJob> batch_jobs(const BatchArgs& a, const void* const* stmts) {
+  const bool bad_transcripts = a.states ? false : (!a.labels || !a.label_lens);
+  if (!stmts || !a.inputs || !a.ninputs || !a.proofs || !a.proof_lens || !a.status || bad_transcripts)
+    throw SpError(SP_ERR_INVALID_ARG, "verify_batch: NULL array");
+  std::vector<VerifyJob> jobs;
+  jobs.reserve(a.k);
+  for (size_t i = 0; i < a.k; i++) {
+    const std::string at = "verify_batch: proof " + std::to_string(i) + ": ";
+    if (!stmts[i]) throw SpError(SP_ERR_INVALID_ARG, at + "NULL statement handle");
+    if (!a.proofs[i] && a.proof_lens[i]) throw SpError(SP_ERR_INVALID_ARG, at + "NULL proof");
+    if (!a.inputs[i] && a.ninputs[i]) throw SpError(SP_ERR_INVALID_ARG, at + "NULL inputs");
+    require_reduced(a.inputs[i], a.ninputs[i], "inputs");
+    if (a.states && !a.states[i]) throw SpError(SP_ERR_INVALID_ARG, at + "transcript state is NULL");
+    Transcript T = a.states ? Transcript(Transcript::FromState(), a.states[i]) : Transcript(std::string((const char*)a.labels[i], a.label_lens[i]));
+    jobs.push_back(VerifyJob{nullptr, nullptr, fq_vec(a.inputs[i], a.ninputs[i]), T, a.proofs[i], a.proof_lens[i]});
+  }
+  return jobs;
+}
+// statuses and transcripts out; SP_ERR_VERIFY with the first rejection's message when any proof is rejected
+static void batch_finish(Ctx& c, const BatchArgs& a, const std::vector<VerifyJob>& jobs) {
+  size_t first = a.k;
+  for (size_t i = 0; i < a.k; i++) {
+    a.status[i] = jobs[i].status;
+    if (a.states) jobs[i].T.export_state(a.states[i]);
+    if (jobs[i].status != SP_OK && first == a.k) first = i;
+  }
+  flush_fine(c);
+  if (first < a.k) throw SpError(SP_ERR_VERIFY, "proof " + std::to_string(first) + ": " + jobs[first].msg);
+}
+// The body NIZK and SNARK batch verification share.  `verify(jobs)` points the jobs at their statements and verifies them.
+template <class Verify>
+static int verify_batch(sp_ctx* ctx, const void* const* stmts, const void* gens, const BatchArgs& a, const Verify& verify) {
+  return guarded(ctx, [&] {
+    if (!a.seed) throw SpError(SP_ERR_INVALID_ARG, "verify_batch: weight seed is NULL: draw 32 bytes from the OS RNG on every call");
+    if (!a.k) return;
+    if (!gens) throw SpError(SP_ERR_INVALID_ARG, "verify_batch: NULL gens");
+    std::vector<VerifyJob> jobs = batch_jobs(a, stmts);
+    verify(jobs);
+    batch_finish(ctx->c, a, jobs);
+  });
+}
+
+// ---- polynomial commitments of the caller's tables
+// gens of this context whose n is the row length R = 2^ceil(ell/2) of a table of 2^ell entries (commitments.rs:87-91 asserts gens_n.n == R)
+static void pc_check_gens(const sp_ctx* ctx, const sp_pc_gens* g, size_t ell, const std::string& what) {
+  require_owned(ctx, g, what, "gens handle");
+  if (g->g.n != pc_gens_n(ell))
+    throw SpError(SP_ERR_INVALID_ARG, what + ": gens for num_vars = " + std::to_string(g->num_vars) + " have n = " + std::to_string(g->g.n) +
+                                          ", a table of 2^" + std::to_string(ell) + " entries needs n = R = " + std::to_string(pc_gens_n(ell)));
+}
+static const size_t PC_MAX_VARS = 60;
+static Transcript pc_tape_open(const uint8_t* tape_state, const std::string& what) {
+  if (!tape_state) throw SpError(SP_ERR_INVALID_ARG, what + ": tape state is NULL");
+  return Transcript(Transcript::FromState(), tape_state);
+}
+
+// ---- product circuits of the caller's tables
+static const size_t PROD_MAX_VARS = 60;
+// one circuit's leaf form, checked: leaf[x] = cst + idx * x + sum_s coeff[s] * table[src[s]][x]
+struct LeafForm { uint32_t nsrc = 0; uint32_t src[SP_PROD_MAX_SOURCES] = {}; Fq coeff[SP_PROD_MAX_SOURCES], idx = Fq::zero(), cst = Fq::zero(); };
+static void prod_counts(const sp_prod_leaves* leaves, int k, int ntables, const std::string& what) {
+  require_count(what, k, "circuits", "SP_PROD_MAX_CIRCUITS", SP_PROD_MAX_CIRCUITS);
+  if (ntables < 1) throw SpError(SP_ERR_INVALID_ARG, what + ": " + std::to_string(ntables) + " tables; at least one needed");
+  if (!leaves && k != ntables)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": leaves NULL (circuit i = table i) needs k = ntables, got k = " + std::to_string(k) + ", ntables = " + std::to_string(ntables));
+}
+static std::vector<LeafForm> prod_forms(const sp_prod_leaves* leaves, int k, int ntables, const std::string& what) {
+  prod_counts(leaves, k, ntables, what);
+  std::vector<LeafForm> f(k);
+  for (int c = 0; c < k; c++) {
+    if (!leaves) { f[c].nsrc = 1; f[c].src[0] = (uint32_t)c; f[c].coeff[0] = Fq::one(); continue; }
+    const sp_prod_leaves& l = leaves[c];
+    const std::string at = what + ": circuit " + std::to_string(c);
+    if (l.nsources > SP_PROD_MAX_SOURCES)
+      throw SpError(SP_ERR_INVALID_ARG, at + " has " + std::to_string(l.nsources) + " sources; at most SP_PROD_MAX_SOURCES = " + std::to_string(SP_PROD_MAX_SOURCES));
+    for (uint32_t s = 0; s < l.nsources; s++)
+      if (l.source[s] >= (uint32_t)ntables)
+        throw SpError(SP_ERR_INVALID_ARG, at + ": source " + std::to_string(s) + " is table " + std::to_string(l.source[s]) + " >= ntables = " + std::to_string(ntables));
+  }
+  if (leaves)
+    for (int c = 0; c < k; c++) {
+      const sp_prod_leaves& l = leaves[c];
+      const std::string at = what + ": circuit " + std::to_string(c);
+      require_reduced(&l.coeff_mont[0][0], l.nsources, (at + ": coefficient").c_str());
+      require_reduced(l.index_coeff_mont, 1, (at + ": index coefficient").c_str());
+      require_reduced(l.const_mont, 1, (at + ": constant").c_str());
+      f[c].nsrc = l.nsources;
+      for (uint32_t s = 0; s < l.nsources; s++) { f[c].src[s] = l.source[s]; f[c].coeff[s] = fq_in(l.coeff_mont[s]); }
+      f[c].idx = fq_in(l.index_coeff_mont);
+      f[c].cst = fq_in(l.const_mont);
+    }
+  return f;
+}
 
 extern "C" {
 
 int sp_device_count(void) { return dev::device_count(); }
 int sp_ctx_create(int device, sp_ctx** out) {
   try {
-    if (dev::device_count() <= device) { g_create_error = "no CUDA device (spartan_b200 has no CPU fallback)"; return SP_ERR_NO_DEVICE; }
+    if (dev::device_count() <= device) { g_last_error = "no CUDA device (spartan_b200 has no CPU fallback)"; return SP_ERR_NO_DEVICE; }
     *out = new sp_ctx(device);
     return SP_OK;
-  } catch (const std::exception& e) { g_create_error = e.what(); return SP_ERR_CUDA; }
+  } catch (const std::exception& e) { g_last_error = e.what(); return SP_ERR_CUDA; }
 }
 void sp_ctx_destroy(sp_ctx* ctx) { delete ctx; }
-const char* sp_last_error(const sp_ctx* ctx) { return ctx ? ctx->c.last_error.c_str() : g_create_error.c_str(); }
+const char* sp_last_error(const sp_ctx* ctx) { return ctx ? ctx->c.last_error.c_str() : g_last_error.c_str(); }
 unsigned long long sp_kernel_launches(void) { return dev::launch_count(); }
 unsigned long long sp_release_cached_memory(void) { return dev::pool_release_cached(); }
 void sp_debug_memcheck(int on) { dev::memcheck_enable(on != 0); }
@@ -68,7 +291,7 @@ int sp_debug_memcheck_report(sp_memcheck_counts* out, char* violations, size_t b
   return SP_OK;
 }
 unsigned long long sp_debug_memcheck_scan(void) {
-  try { return dev::memcheck_scan(); } catch (const std::exception& e) { g_create_error = e.what(); return ~0ull; }
+  try { return dev::memcheck_scan(); } catch (const std::exception& e) { g_last_error = e.what(); return ~0ull; }
 }
 int sp_timings(sp_ctx* ctx, char* buf, size_t buflen) {
   std::ostringstream os;
@@ -82,17 +305,17 @@ int sp_timings(sp_ctx* ctx, char* buf, size_t buflen) {
 // ---- intra-proof sharding: one process per GPU, windows exchanged as CUDA IPC handles by whatever transport the host has
 size_t sp_comm_handle_bytes(void) { return dev::ipc_handle_bytes(); }
 int sp_comm_export(sp_ctx* ctx, uint8_t* handle_out) {
-  SP_TRY(ctx)
-  ctx->c.comm_create();
-  if (ctx->c.comm->connected) throw SpError(SP_ERR_INVALID_ARG, "communicator already connected");
-  ctx->c.comm->export_handle(handle_out);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    ctx->c.comm_create();
+    if (ctx->c.comm->connected) throw SpError(SP_ERR_INVALID_ARG, "communicator already connected");
+    ctx->c.comm->export_handle(handle_out);
+  });
 }
 int sp_comm_connect(sp_ctx* ctx, int rank, int world, const uint8_t* handles) {
-  SP_TRY(ctx)
-  if (!ctx->c.comm) throw SpError(SP_ERR_INVALID_ARG, "sp_comm_export must be called first (it creates the window whose handle the peers map)");
-  ctx->c.comm->connect(rank, world, handles);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (!ctx->c.comm) throw SpError(SP_ERR_INVALID_ARG, "sp_comm_export must be called first (it creates the window whose handle the peers map)");
+    ctx->c.comm->connect(rank, world, handles);
+  });
 }
 int sp_comm_set_enabled(sp_ctx* ctx, int enabled) { ctx->c.shard_enabled = enabled != 0; return SP_OK; }
 int sp_ctx_set_overlap(sp_ctx* ctx, int enabled) { ctx->c.overlap = enabled != 0; return SP_OK; }
@@ -107,19 +330,19 @@ int sp_prof_report(char* buf, size_t buflen) {
   return SP_OK;
 }
 int sp_timer_start(sp_ctx* ctx) {
-  SP_TRY(ctx)
-  if (!ctx->c.ev_a) { ctx->c.ev_a = dev::event_create(); ctx->c.ev_b = dev::event_create(); }   // events belong to the context (device)
-  dev::event_record(ctx->c.ev_a, ctx->c.stream);
-  ctx->c.timer_running = true;
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (!ctx->c.ev_a) { ctx->c.ev_a = dev::event_create(); ctx->c.ev_b = dev::event_create(); }   // events belong to the context (device)
+    dev::event_record(ctx->c.ev_a, ctx->c.stream);
+    ctx->c.timer_running = true;
+  });
 }
 int sp_timer_stop_ms(sp_ctx* ctx, float* ms) {
-  SP_TRY(ctx)
-  if (!ctx->c.timer_running) throw SpError(SP_ERR_INVALID_ARG, "sp_timer_stop_ms without sp_timer_start");
-  dev::event_record(ctx->c.ev_b, ctx->c.stream);
-  *ms = dev::event_elapsed_ms(ctx->c.ev_a, ctx->c.ev_b);
-  ctx->c.timer_running = false;
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (!ctx->c.timer_running) throw SpError(SP_ERR_INVALID_ARG, "sp_timer_stop_ms without sp_timer_start");
+    dev::event_record(ctx->c.ev_b, ctx->c.stream);
+    *ms = dev::event_elapsed_ms(ctx->c.ev_a, ctx->c.ev_b);
+    ctx->c.timer_running = false;
+  });
 }
 
 // ---- scalars
@@ -141,19 +364,19 @@ int sp_scalar_invert(const uint64_t a[4], uint64_t out[4]) {
 
 // ---- polys
 int sp_poly_upload(sp_ctx* ctx, const uint64_t* limbs, size_t len, sp_poly** out) {
-  SP_TRY(ctx)
-  std::unique_ptr<sp_poly> p(new sp_poly{&ctx->c, DevBuf<u256>(len), len});
-  dev::h2d(p->d.p, limbs, len * 32, ctx->c.stream);
-  ctx->c.sync();
-  *out = p.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    std::unique_ptr<sp_poly> p(new sp_poly{&ctx->c, DevBuf<u256>(len), len});
+    dev::h2d(p->d.p, limbs, len * 32, ctx->c.stream);
+    ctx->c.sync();
+    *out = p.release();
+  });
 }
 int sp_poly_download(sp_ctx* ctx, const sp_poly* p, uint64_t* limbs, size_t len) {
-  SP_TRY(ctx)
-  if (len > p->d.n) throw SpError(SP_ERR_INVALID_ARG, "download length exceeds allocation");
-  dev::d2h(limbs, p->d.p, len * 32, ctx->c.stream);
-  ctx->c.sync();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (len > p->d.n) throw SpError(SP_ERR_INVALID_ARG, "download length exceeds allocation");
+    dev::d2h(limbs, p->d.p, len * 32, ctx->c.stream);
+    ctx->c.sync();
+  });
 }
 size_t sp_poly_len(const sp_poly* p) { return p->len; }
 void sp_poly_free(sp_poly* p) { delete p; }
@@ -163,17 +386,17 @@ static void check_same_len(sp_poly* const* polys, int k) {
   if (polys[0]->len < 2 || (polys[0]->len & (polys[0]->len - 1))) throw SpError(SP_ERR_INVALID_ARG, "length must be a power of two >= 2");
 }
 int sp_fold_top(sp_ctx* ctx, sp_poly* const* polys, int k, const uint64_t r[4]) {
-  SP_TRY(ctx)
-  if (k < 1) throw SpError(SP_ERR_INVALID_ARG, "fold_top: no polynomials");
-  check_same_len(polys, k);
-  for (int i = 0; i < k; i++) for (int j = 0; j < i; j++) if (polys[i] == polys[j]) throw SpError(SP_ERR_INVALID_ARG, "fold_top: the same polynomial passed twice");
-  Fq rr = fq_in(r);
-  std::vector<u256*> t(k);
-  for (int i = 0; i < k; i++) t[i] = polys[i]->d.p;
-  dev::fold_top(t.data(), k, polys[0]->len, rr.m, ctx->c.stream);
-  ctx->c.sync();
-  for (int i = 0; i < k; i++) polys[i]->len /= 2;
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (k < 1) throw SpError(SP_ERR_INVALID_ARG, "fold_top: no polynomials");
+    check_same_len(polys, k);
+    for (int i = 0; i < k; i++) for (int j = 0; j < i; j++) if (polys[i] == polys[j]) throw SpError(SP_ERR_INVALID_ARG, "fold_top: the same polynomial passed twice");
+    Fq rr = fq_in(r);
+    std::vector<u256*> t(k);
+    for (int i = 0; i < k; i++) t[i] = polys[i]->d.p;
+    dev::fold_top(t.data(), k, polys[0]->len, rr.m, ctx->c.stream);
+    ctx->c.sync();
+    for (int i = 0; i < k; i++) polys[i]->len /= 2;
+  });
 }
 static int kind_tables(int kind) { return kind == 0 ? 2 : kind == 1 ? 3 : 4; }
 static dev::ScInst make_inst(sp_poly* const* polys, int nt) {
@@ -196,27 +419,27 @@ static int sumcheck_tables(Ctx& c, int kind, sp_poly* const* polys, bool sharded
 // sharded: the kernel's cross-rank completion counter and the next exchange (every rank issues it in the same order)
 static dev::HostSig xr_sig(Ctx& c, bool sharded) { dev::HostSig s; if (sharded) s.done = c.sig_done.p + layout::SIG_DONE.off; return s; }
 static int sumcheck_eval(sp_ctx* ctx, int kind, sp_poly* const* polys, uint64_t out[3][4], bool sharded) {
-  SP_TRY(ctx)
-  Ctx& c = ctx->c;
-  const int nt = sumcheck_tables(c, kind, polys, sharded);
-  dev::ScInst in = make_inst(polys, nt);
-  dev::sc_eval((dev::ScKind)kind, &in, 1, polys[0]->len, c.small.p + layout::SMALL_ROUND.off, c.red.p, c.stream, xr_sig(c, sharded), sharded ? c.comm->next_xr() : dev::XRank());
-  c.get_small(layout::SMALL_ROUND.off, reinterpret_cast<Fq*>(out), 3);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    Ctx& c = ctx->c;
+    const int nt = sumcheck_tables(c, kind, polys, sharded);
+    dev::ScInst in = make_inst(polys, nt);
+    dev::sc_eval((dev::ScKind)kind, &in, 1, polys[0]->len, c.small.p + layout::SMALL_ROUND.off, c.red.p, c.stream, xr_sig(c, sharded), sharded ? c.comm->next_xr() : dev::XRank());
+    c.get_small(layout::SMALL_ROUND.off, reinterpret_cast<Fq*>(out), 3);
+  });
 }
 static int sumcheck_fold_eval(sp_ctx* ctx, int kind, sp_poly* const* polys, const uint64_t r[4], uint64_t out[3][4], bool sharded) {
-  SP_TRY(ctx)
-  Ctx& c = ctx->c;
-  const int nt = sumcheck_tables(c, kind, polys, sharded);
-  if (polys[0]->len < (sharded ? Ctx::SHARD_MIN_LOCAL : 4))
-    throw SpError(SP_ERR_INVALID_ARG, sharded ? "sharded fold_eval needs shards of at least 8192 entries (gather the shards and finish on one GPU)"
-                                              : "fold_eval needs length >= 4");
-  Fq rr = fq_in(r);
-  dev::ScInst in = make_inst(polys, nt);
-  dev::sc_fold_eval((dev::ScKind)kind, &in, 1, polys[0]->len, rr.m, c.small.p + layout::SMALL_ROUND.off, c.red.p, c.stream, xr_sig(c, sharded), sharded ? c.comm->next_xr() : dev::XRank());
-  c.get_small(layout::SMALL_ROUND.off, reinterpret_cast<Fq*>(out), 3);
-  for (int i = 0; i < nt; i++) polys[i]->len /= 2;
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    Ctx& c = ctx->c;
+    const int nt = sumcheck_tables(c, kind, polys, sharded);
+    if (polys[0]->len < (sharded ? Ctx::SHARD_MIN_LOCAL : 4))
+      throw SpError(SP_ERR_INVALID_ARG, sharded ? "sharded fold_eval needs shards of at least 8192 entries (gather the shards and finish on one GPU)"
+                                                : "fold_eval needs length >= 4");
+    Fq rr = fq_in(r);
+    dev::ScInst in = make_inst(polys, nt);
+    dev::sc_fold_eval((dev::ScKind)kind, &in, 1, polys[0]->len, rr.m, c.small.p + layout::SMALL_ROUND.off, c.red.p, c.stream, xr_sig(c, sharded), sharded ? c.comm->next_xr() : dev::XRank());
+    c.get_small(layout::SMALL_ROUND.off, reinterpret_cast<Fq*>(out), 3);
+    for (int i = 0; i < nt; i++) polys[i]->len /= 2;
+  });
 }
 int sp_sumcheck_eval(sp_ctx* ctx, int kind, sp_poly* const* polys, uint64_t out[3][4]) { return sumcheck_eval(ctx, kind, polys, out, false); }
 int sp_sumcheck_fold_eval(sp_ctx* ctx, int kind, sp_poly* const* polys, const uint64_t r[4], uint64_t out[3][4]) {
@@ -258,89 +481,89 @@ static void batched_insts(sp_ctx* ctx, int ninst, sp_poly* const* A, sp_poly* co
   (void)ctx;
 }
 int sp_sumcheck_batched_eval(sp_ctx* ctx, int ninst, sp_poly* const* A, sp_poly* const* B, sp_poly* const* Cc, uint64_t* out) {
-  SP_TRY(ctx)
-  std::vector<dev::ScInst> insts;
-  std::vector<std::pair<sp_poly*, std::unique_ptr<DevBuf<u256>>>> shared;
-  batched_insts(ctx, ninst, A, B, Cc, insts, shared, false);
-  DevBuf<u256> d_out(3 * ninst);
-  dev::sc_eval(dev::SC_CUBIC3, insts.data(), ninst, A[0]->len, d_out.p, ctx->c.red.p, ctx->c.stream);
-  dev::d2h(out, d_out.p, 96 * (size_t)ninst, ctx->c.stream);
-  ctx->c.sync();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    std::vector<dev::ScInst> insts;
+    std::vector<std::pair<sp_poly*, std::unique_ptr<DevBuf<u256>>>> shared;
+    batched_insts(ctx, ninst, A, B, Cc, insts, shared, false);
+    DevBuf<u256> d_out(3 * ninst);
+    dev::sc_eval(dev::SC_CUBIC3, insts.data(), ninst, A[0]->len, d_out.p, ctx->c.red.p, ctx->c.stream);
+    dev::d2h(out, d_out.p, 96 * (size_t)ninst, ctx->c.stream);
+    ctx->c.sync();
+  });
 }
 int sp_sumcheck_batched_fold_eval(sp_ctx* ctx, int ninst, sp_poly* const* A, sp_poly* const* B, sp_poly* const* Cc, const uint64_t r[4], uint64_t* out) {
-  SP_TRY(ctx)
-  if (ninst < 1 || ninst > dev::SC_MAX_INST) throw SpError(SP_ERR_INVALID_ARG, "batched sumcheck: 1.." + std::to_string(dev::SC_MAX_INST) + " instances");
-  if (A[0]->len < 4) throw SpError(SP_ERR_INVALID_ARG, "fold_eval needs length >= 4");
-  std::vector<dev::ScInst> insts;
-  std::vector<std::pair<sp_poly*, std::unique_ptr<DevBuf<u256>>>> shared;
-  batched_insts(ctx, ninst, A, B, Cc, insts, shared, true);
-  Fq rr = fq_in(r);
-  DevBuf<u256> d_out(3 * ninst);
-  const size_t len = A[0]->len;
-  dev::sc_fold_eval(dev::SC_CUBIC3, insts.data(), ninst, len, rr.m, d_out.p, ctx->c.red.p, ctx->c.stream);
-  for (auto& sh : shared) dev::d2d(sh.first->d.p, sh.second->p, (len / 2) * sizeof(u256), ctx->c.stream);
-  dev::d2h(out, d_out.p, 96 * (size_t)ninst, ctx->c.stream);
-  ctx->c.sync();
-  std::vector<sp_poly*> seen;
-  for (int i = 0; i < ninst; i++)
-    for (sp_poly* p : {A[i], B[i], Cc[i]})
-      if (std::find(seen.begin(), seen.end(), p) == seen.end()) { seen.push_back(p); p->len /= 2; }
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (ninst < 1 || ninst > dev::SC_MAX_INST) throw SpError(SP_ERR_INVALID_ARG, "batched sumcheck: 1.." + std::to_string(dev::SC_MAX_INST) + " instances");
+    if (A[0]->len < 4) throw SpError(SP_ERR_INVALID_ARG, "fold_eval needs length >= 4");
+    std::vector<dev::ScInst> insts;
+    std::vector<std::pair<sp_poly*, std::unique_ptr<DevBuf<u256>>>> shared;
+    batched_insts(ctx, ninst, A, B, Cc, insts, shared, true);
+    Fq rr = fq_in(r);
+    DevBuf<u256> d_out(3 * ninst);
+    const size_t len = A[0]->len;
+    dev::sc_fold_eval(dev::SC_CUBIC3, insts.data(), ninst, len, rr.m, d_out.p, ctx->c.red.p, ctx->c.stream);
+    for (auto& sh : shared) dev::d2d(sh.first->d.p, sh.second->p, (len / 2) * sizeof(u256), ctx->c.stream);
+    dev::d2h(out, d_out.p, 96 * (size_t)ninst, ctx->c.stream);
+    ctx->c.sync();
+    std::vector<sp_poly*> seen;
+    for (int i = 0; i < ninst; i++)
+      for (sp_poly* p : {A[i], B[i], Cc[i]})
+        if (std::find(seen.begin(), seen.end(), p) == seen.end()) { seen.push_back(p); p->len /= 2; }
+  });
 }
 int sp_eq_evals(sp_ctx* ctx, const uint64_t* r, size_t ell, sp_poly** out) {
-  SP_TRY(ctx)
-  size_t n = (size_t)1 << ell;
-  std::unique_ptr<sp_poly> p(new sp_poly{&ctx->c, DevBuf<u256>(n), n});
-  DevBuf<u256> d_r(ell + 1), small(dev::eq_evals_scratch(ell));
-  dev::h2d(d_r.p, r, ell * 32, ctx->c.stream);
-  dev::eq_evals(p->d.p, d_r.p, (int)ell, small.p, ctx->c.stream);
-  ctx->c.sync();
-  *out = p.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    size_t n = (size_t)1 << ell;
+    std::unique_ptr<sp_poly> p(new sp_poly{&ctx->c, DevBuf<u256>(n), n});
+    DevBuf<u256> d_r(ell + 1), small(dev::eq_evals_scratch(ell));
+    dev::h2d(d_r.p, r, ell * 32, ctx->c.stream);
+    dev::eq_evals(p->d.p, d_r.p, (int)ell, small.p, ctx->c.stream);
+    ctx->c.sync();
+    *out = p.release();
+  });
 }
 int sp_poly_evaluate(sp_ctx* ctx, const sp_poly* p, const uint64_t* r, size_t ell, uint64_t out[4]) {
-  SP_TRY(ctx)
-  if (p->len != (size_t)1 << ell) throw SpError(SP_ERR_INVALID_ARG, "evaluate: |r| != num_vars");
-  DevBuf<u256> d_r(ell + 1), small(dev::eq_evals_scratch(ell)), eq(p->len);
-  dev::h2d(d_r.p, r, ell * 32, ctx->c.stream);
-  dev::eq_evals(eq.p, d_r.p, (int)ell, small.p, ctx->c.stream);
-  dev::dot(ctx->c.small.p + layout::SMALL_DOT.off, p->d.p, eq.p, p->len, ctx->c.red.p, ctx->c.stream);
-  Fq v;
-  ctx->c.get_small(layout::SMALL_DOT.off, &v, 1);
-  fq_out(out, v);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (p->len != (size_t)1 << ell) throw SpError(SP_ERR_INVALID_ARG, "evaluate: |r| != num_vars");
+    DevBuf<u256> d_r(ell + 1), small(dev::eq_evals_scratch(ell)), eq(p->len);
+    dev::h2d(d_r.p, r, ell * 32, ctx->c.stream);
+    dev::eq_evals(eq.p, d_r.p, (int)ell, small.p, ctx->c.stream);
+    dev::dot(ctx->c.small.p + layout::SMALL_DOT.off, p->d.p, eq.p, p->len, ctx->c.red.p, ctx->c.stream);
+    Fq v;
+    ctx->c.get_small(layout::SMALL_DOT.off, &v, 1);
+    fq_out(out, v);
+  });
 }
 int sp_poly_bound_rows(sp_ctx* ctx, const sp_poly* p, const uint64_t* Lm, size_t L_size, sp_poly** out) {
-  SP_TRY(ctx)
-  if (L_size == 0 || p->len % L_size) throw SpError(SP_ERR_INVALID_ARG, "bound: L does not divide the length");
-  size_t R_size = p->len / L_size;
-  std::unique_ptr<sp_poly> o(new sp_poly{&ctx->c, DevBuf<u256>(R_size), R_size});
-  DevBuf<u256> d_L(L_size), tmp(64 * R_size);
-  dev::h2d(d_L.p, Lm, L_size * 32, ctx->c.stream);
-  dev::bound_rows(o->d.p, p->d.p, d_L.p, L_size, R_size, tmp.p, ctx->c.stream);
-  ctx->c.sync();
-  *out = o.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (L_size == 0 || p->len % L_size) throw SpError(SP_ERR_INVALID_ARG, "bound: L does not divide the length");
+    size_t R_size = p->len / L_size;
+    std::unique_ptr<sp_poly> o(new sp_poly{&ctx->c, DevBuf<u256>(R_size), R_size});
+    DevBuf<u256> d_L(L_size), tmp(64 * R_size);
+    dev::h2d(d_L.p, Lm, L_size * 32, ctx->c.stream);
+    dev::bound_rows(o->d.p, p->d.p, d_L.p, L_size, R_size, tmp.p, ctx->c.stream);
+    ctx->c.sync();
+    *out = o.release();
+  });
 }
 int sp_dot(sp_ctx* ctx, const sp_poly* a, const sp_poly* b, uint64_t out[4]) {
-  SP_TRY(ctx)
-  if (a->len != b->len) throw SpError(SP_ERR_INVALID_ARG, "dot: length mismatch");
-  dev::dot(ctx->c.small.p + layout::SMALL_DOT.off, a->d.p, b->d.p, a->len, ctx->c.red.p, ctx->c.stream);
-  Fq v;
-  ctx->c.get_small(layout::SMALL_DOT.off, &v, 1);
-  fq_out(out, v);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (a->len != b->len) throw SpError(SP_ERR_INVALID_ARG, "dot: length mismatch");
+    dev::dot(ctx->c.small.p + layout::SMALL_DOT.off, a->d.p, b->d.p, a->len, ctx->c.red.p, ctx->c.stream);
+    Fq v;
+    ctx->c.get_small(layout::SMALL_DOT.off, &v, 1);
+    fq_out(out, v);
+  });
 }
 
 // ---- gens / commitments
 int sp_gens_create(sp_ctx* ctx, const uint8_t* label, size_t label_len, size_t n, sp_gens** out) {
-  SP_TRY(ctx)
-  std::unique_ptr<sp_gens> g(new sp_gens);
-  g->n = n;
-  g->set.reset(new GenSet(&ctx->c, std::string((const char*)label, label_len), n + 1, {}));
-  *out = g.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    std::unique_ptr<sp_gens> g(new sp_gens);
+    g->n = n;
+    g->set.reset(new GenSet(&ctx->c, std::string((const char*)label, label_len), n + 1, {}));
+    *out = g.release();
+  });
 }
 // n ristretto255 encodings -> device points.  ok == null: an encoding that is not a point is an SP_ERR_INVALID_POINT naming its index
 // (`what`); otherwise ok[i] tells whether encoding i is a point.
@@ -358,60 +581,58 @@ static DevBuf<ge> decode_points(Ctx& c, const uint8_t* in32, size_t n, const cha
   return pts;
 }
 int sp_gens_upload(sp_ctx* ctx, const uint8_t* compressed32, size_t n, sp_gens** out) {
-  SP_TRY(ctx)
-  DevBuf<ge> g = decode_points(ctx->c, compressed32, n + 1, "gens_upload");
-  std::unique_ptr<sp_gens> G(new sp_gens);
-  G->n = n;
-  G->set.reset(new GenSet(&ctx->c, g.p, n + 1, {}));
-  *out = G.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    DevBuf<ge> g = decode_points(ctx->c, compressed32, n + 1, "gens_upload");
+    std::unique_ptr<sp_gens> G(new sp_gens);
+    G->n = n;
+    G->set.reset(new GenSet(&ctx->c, g.p, n + 1, {}));
+    *out = G.release();
+  });
 }
 void sp_gens_free(sp_gens* g) { delete g; }
 int sp_gens_export(sp_ctx* ctx, const sp_gens* g, uint8_t* out32) {
-  SP_TRY(ctx)
-  DevBuf<uint8_t> comp(32 * (g->n + 1));
-  dev::compress_batch(comp.p, g->set->G.p, g->n + 1, ctx->c.stream);
-  dev::d2h(out32, comp.p, 32 * (g->n + 1), ctx->c.stream);
-  ctx->c.sync();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    DevBuf<uint8_t> comp(32 * (g->n + 1));
+    dev::compress_batch(comp.p, g->set->G.p, g->n + 1, ctx->c.stream);
+    dev::d2h(out32, comp.p, 32 * (g->n + 1), ctx->c.stream);
+    ctx->c.sync();
+  });
 }
 int sp_msm(sp_ctx* ctx, const sp_gens* g, const uint64_t* scalars, size_t n, uint8_t out32[32]) {
-  SP_TRY(ctx)
-  if (n > g->n) throw SpError(SP_ERR_INVALID_ARG, "msm: more scalars than generators");
-  DevBuf<u256> d(n ? n : 1);
-  dev::h2d(d.p, scalars, n * 32, ctx->c.stream);
-  CommitKey key{g->set.get(), 0, g->n, g->n};
-  std::vector<Cp> out;
-  commit_rows_and_compress(ctx->c, key, d.p, n, 1, n, nullptr, out);
-  memcpy(out32, out[0].b, 32);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (n > g->n) throw SpError(SP_ERR_INVALID_ARG, "msm: more scalars than generators");
+    DevBuf<u256> d(n ? n : 1);
+    dev::h2d(d.p, scalars, n * 32, ctx->c.stream);
+    CommitKey key{g->set.get(), 0, g->n, g->n};
+    std::vector<Cp> out;
+    commit_rows_and_compress(ctx->c, key, d.p, n, 1, n, nullptr, out);
+    memcpy(out32, out[0].b, 32);
+  });
 }
 int sp_commit_rows(sp_ctx* ctx, const sp_gens* g, const sp_poly* p, size_t L, size_t R, const uint64_t* blinds, uint8_t* out32) {
-  SP_TRY(ctx)
-  if (L * R != p->len || R > g->n) throw SpError(SP_ERR_INVALID_ARG, "commit_rows: shape mismatch");
-  CommitKey key{g->set.get(), 0, g->n, g->n};
-  std::vector<Fq> bl;
-  if (blinds) bl = fq_vec(blinds, L);
-  std::vector<Cp> out;
-  commit_rows_and_compress(ctx->c, key, p->d.p, R, L, R, blinds ? bl.data() : nullptr, out);
-  memcpy(out32, out.data(), 32 * L);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (L * R != p->len || R > g->n) throw SpError(SP_ERR_INVALID_ARG, "commit_rows: shape mismatch");
+    CommitKey key{g->set.get(), 0, g->n, g->n};
+    std::vector<Fq> bl;
+    if (blinds) bl = fq_vec(blinds, L);
+    std::vector<Cp> out;
+    commit_rows_and_compress(ctx->c, key, p->d.p, R, L, R, blinds ? bl.data() : nullptr, out);
+    memcpy(out32, out.data(), 32 * L);
+  });
 }
 int sp_point_decompress_check(sp_ctx* ctx, const uint8_t* in32, size_t n, int* ok) {
-  SP_TRY(ctx)
-  decode_points(ctx->c, in32, n, nullptr, ok);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] { decode_points(ctx->c, in32, n, nullptr, ok); });
 }
 int sp_point_roundtrip(sp_ctx* ctx, const uint8_t* in32, size_t n, uint8_t* out32) {
-  SP_TRY(ctx)
-  DevBuf<uint8_t> d_in(32 * n), d_out(32 * n);
-  DevBuf<ge> pts(n);
-  dev::h2d(d_in.p, in32, 32 * n, ctx->c.stream);
-  dev::decompress_batch(pts.p, nullptr, d_in.p, n, ctx->c.stream);
-  dev::compress_batch(d_out.p, pts.p, n, ctx->c.stream);
-  dev::d2h(out32, d_out.p, 32 * n, ctx->c.stream);
-  ctx->c.sync();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    DevBuf<uint8_t> d_in(32 * n), d_out(32 * n);
+    DevBuf<ge> pts(n);
+    dev::h2d(d_in.p, in32, 32 * n, ctx->c.stream);
+    dev::decompress_batch(pts.p, nullptr, d_in.p, n, ctx->c.stream);
+    dev::compress_batch(d_out.p, pts.p, n, ctx->c.stream);
+    dev::d2h(out32, d_out.p, 32 * n, ctx->c.stream);
+    ctx->c.sync();
+  });
 }
 
 // ---- inner-product argument, operator level: BulletReductionProof::prove (nizk/bullet.rs:32-132) with the host keeping the transcript.
@@ -428,64 +649,64 @@ static hge point_in(const uint8_t p32[32], const char* what) {
   return to_hge(g);
 }
 int sp_ipa_begin(sp_ctx* ctx, const sp_gens* gens, const sp_poly* a_vec, const sp_poly* b_vec, sp_ipa** out) {
-  SP_TRY(ctx)
-  const size_t n = a_vec->len;
-  if (n < 1 || (n & (n - 1)) || b_vec->len != n || n > gens->n) throw SpError(SP_ERR_INVALID_ARG, "ipa: |a| = |b| = a power of two, at most the generator count");
-  std::unique_ptr<sp_ipa> h(new sp_ipa);
-  h->ctx = &ctx->c; h->gs = gens->set.get(); h->n = n; h->cur = n;
-  h->a.alloc(n); h->b.alloc(n); h->svec.alloc(n); h->pts.alloc(2);
-  dev::d2d(h->a.p, a_vec->d.p, n * sizeof(u256), ctx->c.stream);
-  dev::d2d(h->b.p, b_vec->d.p, n * sizeof(u256), ctx->c.stream);
-  dev::fill_one(h->svec.p, n, ctx->c.stream);
-  // the fused round launch and, for n >= 2, the one-row sum of sp_ipa_finish run on ipa_msm scratch; n = 1 runs msm_rows
-  ctx->c.ensure_scratch(std::max(dev::msm_scratch_bytes(1, n), dev::ipa_msm_scratch_points(n, gens->set->wbits) * sizeof(sp::ge)) + 64);
-  ctx->c.sync();
-  *out = h.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    const size_t n = a_vec->len;
+    if (n < 1 || (n & (n - 1)) || b_vec->len != n || n > gens->n) throw SpError(SP_ERR_INVALID_ARG, "ipa: |a| = |b| = a power of two, at most the generator count");
+    std::unique_ptr<sp_ipa> h(new sp_ipa);
+    h->ctx = &ctx->c; h->gs = gens->set.get(); h->n = n; h->cur = n;
+    h->a.alloc(n); h->b.alloc(n); h->svec.alloc(n); h->pts.alloc(2);
+    dev::d2d(h->a.p, a_vec->d.p, n * sizeof(u256), ctx->c.stream);
+    dev::d2d(h->b.p, b_vec->d.p, n * sizeof(u256), ctx->c.stream);
+    dev::fill_one(h->svec.p, n, ctx->c.stream);
+    // the fused round launch and, for n >= 2, the one-row sum of sp_ipa_finish run on ipa_msm scratch; n = 1 runs msm_rows
+    ctx->c.ensure_scratch(std::max(dev::msm_scratch_bytes(1, n), dev::ipa_msm_scratch_points(n, gens->set->wbits) * sizeof(sp::ge)) + 64);
+    ctx->c.sync();
+    *out = h.release();
+  });
 }
 void sp_ipa_free(sp_ipa* h) { delete h; }
 static IpaRound ipa_round(sp_ipa* h) { return IpaRound{*h->ctx, *h->gs, h->a.p, h->b.p, h->svec.p, h->n, h->pts.p}; }
 // L = <a_L, G_R> + c_L*Q + blind_L*H,  R = <a_R, G_L> + c_R*Q + blind_R*H  with c_L = <a_L, b_R>, c_R = <a_R, b_L>   (bullet.rs:74-97)
 int sp_ipa_round_LR(sp_ctx* ctx, sp_ipa* h, const uint8_t Q32[32], const uint8_t H32[32], const uint64_t blind_L[4], const uint64_t blind_R[4], uint8_t L32[32],
                     uint8_t R32[32]) {
-  SP_TRY(ctx)
-  if (h->cur < 2) throw SpError(SP_ERR_INVALID_ARG, "ipa: the reduction is complete");
-  const hge Q = point_in(Q32, "Q"), H = point_in(H32, "H");
-  IpaRound rd = ipa_round(h);
-  rd.launch(h->cur);
-  Fq cc[2];
-  rd.wait_c(cc[0], cc[1]);
-  ge lr[2];
-  rd.wait_LR(lr[0], lr[1]);
-  const Fq bl[2] = {fq_in(blind_L), fq_in(blind_R)};
-  Cp outp[2];
-  hge full[2];
-  for (int k = 0; k < 2; k++) full[k] = hge_add(to_hge(lr[k]), hge_add(hge_scalarmul(cc[k].canonical(), Q), hge_scalarmul(bl[k].canonical(), H)));
-  compress2(full[0], full[1], outp[0], outp[1]);
-  memcpy(L32, outp[0].b, 32); memcpy(R32, outp[1].b, 32);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (h->cur < 2) throw SpError(SP_ERR_INVALID_ARG, "ipa: the reduction is complete");
+    const hge Q = point_in(Q32, "Q"), H = point_in(H32, "H");
+    IpaRound rd = ipa_round(h);
+    rd.launch(h->cur);
+    Fq cc[2];
+    rd.wait_c(cc[0], cc[1]);
+    ge lr[2];
+    rd.wait_LR(lr[0], lr[1]);
+    const Fq bl[2] = {fq_in(blind_L), fq_in(blind_R)};
+    Cp outp[2];
+    hge full[2];
+    for (int k = 0; k < 2; k++) full[k] = hge_add(to_hge(lr[k]), hge_add(hge_scalarmul(cc[k].canonical(), Q), hge_scalarmul(bl[k].canonical(), H)));
+    compress2(full[0], full[1], outp[0], outp[1]);
+    memcpy(L32, outp[0].b, 32); memcpy(R32, outp[1].b, 32);
+  });
 }
 // a_L <- a_L*u + u^-1*a_R,  b_L <- b_L*u^-1 + u*b_R,  G_L <- u^-1*G_L + u*G_R (kept implicit in s)      (bullet.rs:105-108)
 int sp_ipa_fold(sp_ctx* ctx, sp_ipa* h, const uint64_t u[4], const uint64_t u_inv[4]) {
-  SP_TRY(ctx)
-  if (h->cur < 2) throw SpError(SP_ERR_INVALID_ARG, "ipa: the reduction is complete");
-  const Fq uu = fq_in(u), ui = fq_in(u_inv);
-  if (!(uu * ui == Fq::one())) throw SpError(SP_ERR_INVALID_SCALAR, "ipa: u_inv is not the inverse of u");
-  ipa_round(h).fold(h->cur, uu, ui);
-  h->cur /= 2;
-  ctx->c.sync();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (h->cur < 2) throw SpError(SP_ERR_INVALID_ARG, "ipa: the reduction is complete");
+    const Fq uu = fq_in(u), ui = fq_in(u_inv);
+    if (!(uu * ui == Fq::one())) throw SpError(SP_ERR_INVALID_SCALAR, "ipa: u_inv is not the inverse of u");
+    ipa_round(h).fold(h->cur, uu, ui);
+    h->cur /= 2;
+    ctx->c.sync();
+  });
 }
 // a[0], b[0] and G[0] of the fully folded vectors (bullet.rs:113-122: the caller forms Gamma_hat from them)
 int sp_ipa_finish(sp_ctx* ctx, sp_ipa* h, uint64_t a_hat[4], uint64_t b_hat[4], uint8_t G_hat32[32]) {
-  SP_TRY(ctx)
-  Ctx& c = ctx->c;
-  if (h->cur != 1) throw SpError(SP_ERR_INVALID_ARG, "ipa: rounds remain");
-  dev::d2h(a_hat, h->a.p, 32, c.stream);
-  dev::d2h(b_hat, h->b.p, 32, c.stream);
-  const Cp G = compress(RowSum(c, *h->gs, h->svec.p, h->n).collect());
-  memcpy(G_hat32, G.b, 32);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    Ctx& c = ctx->c;
+    if (h->cur != 1) throw SpError(SP_ERR_INVALID_ARG, "ipa: rounds remain");
+    dev::d2h(a_hat, h->a.p, 32, c.stream);
+    dev::d2h(b_hat, h->b.p, 32, c.stream);
+    const Cp G = compress(RowSum(c, *h->gs, h->svec.p, h->n).collect());
+    memcpy(G_hat32, G.b, 32);
+  });
 }
 
 // ---- variable-base MSM (kernels_pip.cu)
@@ -495,39 +716,39 @@ static void points_from_ge(sp_ctx* ctx, sp_points* P, const ge* d_ge, size_t n) 
   dev::points_to_niels(P->pts.p, d_ge, n, ctx->c.stream);
 }
 int sp_points_upload(sp_ctx* ctx, const uint8_t* in32, size_t n, sp_points** out) {
-  SP_TRY(ctx)
-  DevBuf<ge> g = decode_points(ctx->c, in32, n, "points_upload");
-  std::unique_ptr<sp_points> P(new sp_points);
-  points_from_ge(ctx, P.get(), g.p, n);
-  ctx->c.sync();
-  *out = P.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    DevBuf<ge> g = decode_points(ctx->c, in32, n, "points_upload");
+    std::unique_ptr<sp_points> P(new sp_points);
+    points_from_ge(ctx, P.get(), g.p, n);
+    ctx->c.sync();
+    *out = P.release();
+  });
 }
 int sp_points_derive(sp_ctx* ctx, const uint8_t* label, size_t label_len, size_t n, sp_points** out) {
-  SP_TRY(ctx)
-  // the same SHAKE256(label || basepoint) stream as MultiCommitGens::new, squeezed and mapped in slabs so 2^24 points need no 1 GiB staging buffer
-  static const uint8_t basepoint[32] = {0xe2, 0xf2, 0xae, 0x0a, 0x6a, 0xbc, 0x4e, 0x71, 0xa8, 0x84, 0xa9, 0x61, 0xc5, 0x00, 0x51, 0x5f,
-                                        0x58, 0xe3, 0x0b, 0x6a, 0xa5, 0x82, 0xdd, 0x8d, 0xb6, 0xa6, 0x59, 0x45, 0xe0, 0x8d, 0x2d, 0x76};
-  std::vector<uint8_t> seed(label, label + label_len);
-  seed.insert(seed.end(), basepoint, basepoint + 32);
-  Shake256 xof(seed.data(), seed.size());
-  std::unique_ptr<sp_points> P(new sp_points);
-  P->ctx = &ctx->c; P->n = n;
-  P->pts.alloc(n ? n : 1);
-  const size_t slab = (size_t)1 << 18;
-  std::vector<uint8_t> uni(64 * std::min(slab, n ? n : 1));
-  DevBuf<uint8_t> d_uni(uni.size());
-  DevBuf<ge> g(std::min(slab, n ? n : 1));
-  for (size_t i0 = 0; i0 < n; i0 += slab) {
-    size_t m = std::min(slab, n - i0);
-    xof.squeeze(uni.data(), 64 * m);
-    dev::h2d(d_uni.p, uni.data(), 64 * m, ctx->c.stream);
-    dev::gens_from_uniform(g.p, d_uni.p, m, ctx->c.stream);
-    dev::points_to_niels(P->pts.p + i0, g.p, m, ctx->c.stream);
-    ctx->c.sync();
-  }
-  *out = P.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    // the same SHAKE256(label || basepoint) stream as MultiCommitGens::new, squeezed and mapped in slabs so 2^24 points need no 1 GiB staging buffer
+    static const uint8_t basepoint[32] = {0xe2, 0xf2, 0xae, 0x0a, 0x6a, 0xbc, 0x4e, 0x71, 0xa8, 0x84, 0xa9, 0x61, 0xc5, 0x00, 0x51, 0x5f,
+                                          0x58, 0xe3, 0x0b, 0x6a, 0xa5, 0x82, 0xdd, 0x8d, 0xb6, 0xa6, 0x59, 0x45, 0xe0, 0x8d, 0x2d, 0x76};
+    std::vector<uint8_t> seed(label, label + label_len);
+    seed.insert(seed.end(), basepoint, basepoint + 32);
+    Shake256 xof(seed.data(), seed.size());
+    std::unique_ptr<sp_points> P(new sp_points);
+    P->ctx = &ctx->c; P->n = n;
+    P->pts.alloc(n ? n : 1);
+    const size_t slab = (size_t)1 << 18;
+    std::vector<uint8_t> uni(64 * std::min(slab, n ? n : 1));
+    DevBuf<uint8_t> d_uni(uni.size());
+    DevBuf<ge> g(std::min(slab, n ? n : 1));
+    for (size_t i0 = 0; i0 < n; i0 += slab) {
+      size_t m = std::min(slab, n - i0);
+      xof.squeeze(uni.data(), 64 * m);
+      dev::h2d(d_uni.p, uni.data(), 64 * m, ctx->c.stream);
+      dev::gens_from_uniform(g.p, d_uni.p, m, ctx->c.stream);
+      dev::points_to_niels(P->pts.p + i0, g.p, m, ctx->c.stream);
+      ctx->c.sync();
+    }
+    *out = P.release();
+  });
 }
 size_t sp_points_len(const sp_points* p) { return p->n; }
 void sp_points_free(sp_points* p) { delete p; }
@@ -536,17 +757,17 @@ static void points_range(const sp_points* p, size_t offset, size_t n, const char
   if (offset > p->n || n > p->n - offset) throw SpError(SP_ERR_INVALID_ARG, std::string(what) + ": range outside the point set");
 }
 int sp_points_export(sp_ctx* ctx, const sp_points* p, size_t offset, size_t n, uint8_t* out32) {
-  SP_TRY(ctx)
-  points_range(p, offset, n, "points_export");
-  if (n) {   // 1 * P_i through the MSM path's own mixed addition, then compress (no empty launch for n = 0)
-    DevBuf<ge> g(n);
-    DevBuf<uint8_t> comp(32 * n);
-    dev::niels_to_ge(g.p, p->pts.p + offset, n, ctx->c.stream);
-    dev::compress_batch(comp.p, g.p, n, ctx->c.stream);
-    dev::d2h(out32, comp.p, 32 * n, ctx->c.stream);
-    ctx->c.sync();
-  }
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    points_range(p, offset, n, "points_export");
+    if (n) {   // 1 * P_i through the MSM path's own mixed addition, then compress (no empty launch for n = 0)
+      DevBuf<ge> g(n);
+      DevBuf<uint8_t> comp(32 * n);
+      dev::niels_to_ge(g.p, p->pts.p + offset, n, ctx->c.stream);
+      dev::compress_batch(comp.p, g.p, n, ctx->c.stream);
+      dev::d2h(out32, comp.p, 32 * n, ctx->c.stream);
+      ctx->c.sync();
+    }
+  });
 }
 // sharded: the MSM split over the ranks of a connected context.  Every rank passes ITS slice of the points (offset, scalars->len) and of the
 // scalars; the partial sums meet in a point-add all-reduce (all-gather of the W extended points into every window, W-term sum) and every rank
@@ -576,22 +797,18 @@ static void msm_var_run(Ctx& c, const sp_points* p, size_t offset, const u256* d
   c.sync();
 }
 int sp_msm_var_sharded(sp_ctx* ctx, const sp_points* p, size_t offset, const sp_poly* scalars, uint8_t out32[32]) {
-  SP_TRY(ctx)
-  msm_var_run(ctx->c, p, offset, scalars->d.p, scalars->len, out32, true);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] { msm_var_run(ctx->c, p, offset, scalars->d.p, scalars->len, out32, true); });
 }
 int sp_msm_var(sp_ctx* ctx, const sp_points* p, size_t offset, const uint64_t* scalars, size_t n, uint8_t out32[32]) {
-  SP_TRY(ctx)
-  points_range(p, offset, n, "msm_var");   // before the scalars' upload
-  DevBuf<u256> d(n ? n : 1);
-  dev::h2d(d.p, scalars, n * 32, ctx->c.stream);
-  msm_var_run(ctx->c, p, offset, d.p, n, out32, false);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    points_range(p, offset, n, "msm_var");   // before the scalars' upload
+    DevBuf<u256> d(n ? n : 1);
+    dev::h2d(d.p, scalars, n * 32, ctx->c.stream);
+    msm_var_run(ctx->c, p, offset, d.p, n, out32, false);
+  });
 }
 int sp_msm_var_resident(sp_ctx* ctx, const sp_points* p, size_t offset, const sp_poly* scalars, uint8_t out32[32]) {
-  SP_TRY(ctx)
-  msm_var_run(ctx->c, p, offset, scalars->d.p, scalars->len, out32, false);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] { msm_var_run(ctx->c, p, offset, scalars->d.p, scalars->len, out32, false); });
 }
 
 // ---- instances
@@ -633,24 +850,24 @@ static sp_instance* instance_from_device(Ctx& c, size_t num_cons, size_t num_var
 int sp_instance_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, const uint64_t* A_row, const uint64_t* A_col, const uint8_t* A_val,
                        size_t nA, const uint64_t* B_row, const uint64_t* B_col, const uint8_t* B_val, size_t nB, const uint64_t* C_row, const uint64_t* C_col,
                        const uint8_t* C_val, size_t nC, sp_instance** out) {
-  SP_TRY(ctx)
-  // the host arrays go to the device as they are and meet the same checks as sp_instance_create_device's
-  const uint64_t* rows[3] = {A_row, B_row, C_row};
-  const uint64_t* cols[3] = {A_col, B_col, C_col};
-  const uint8_t* vals[3] = {A_val, B_val, C_val};
-  const size_t nn[3] = {nA, nB, nC};
-  DevBuf<uint64_t> d_row[3], d_col[3];
-  DevBuf<uint8_t> d_val[3];
-  dev::CooIn in;
-  for (int m = 0; m < 3; m++) {
-    d_row[m].alloc(nn[m]); d_col[m].alloc(nn[m]); d_val[m].alloc(32 * nn[m]);
-    dev::h2d(d_row[m].p, rows[m], nn[m] * sizeof(uint64_t), ctx->c.stream);
-    dev::h2d(d_col[m].p, cols[m], nn[m] * sizeof(uint64_t), ctx->c.stream);
-    dev::h2d(d_val[m].p, vals[m], 32 * nn[m], ctx->c.stream);
-    in.row[m] = d_row[m].p; in.col[m] = d_col[m].p; in.val[m] = d_val[m].p; in.n[m] = nn[m];
-  }
-  *out = instance_from_device(ctx->c, num_cons, num_vars, num_inputs, in);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    // the host arrays go to the device as they are and meet the same checks as sp_instance_create_device's
+    const uint64_t* rows[3] = {A_row, B_row, C_row};
+    const uint64_t* cols[3] = {A_col, B_col, C_col};
+    const uint8_t* vals[3] = {A_val, B_val, C_val};
+    const size_t nn[3] = {nA, nB, nC};
+    DevBuf<uint64_t> d_row[3], d_col[3];
+    DevBuf<uint8_t> d_val[3];
+    dev::CooIn in;
+    for (int m = 0; m < 3; m++) {
+      d_row[m].alloc(nn[m]); d_col[m].alloc(nn[m]); d_val[m].alloc(32 * nn[m]);
+      dev::h2d(d_row[m].p, rows[m], nn[m] * sizeof(uint64_t), ctx->c.stream);
+      dev::h2d(d_col[m].p, cols[m], nn[m] * sizeof(uint64_t), ctx->c.stream);
+      dev::h2d(d_val[m].p, vals[m], 32 * nn[m], ctx->c.stream);
+      in.row[m] = d_row[m].p; in.col[m] = d_col[m].p; in.val[m] = d_val[m].p; in.n[m] = nn[m];
+    }
+    *out = instance_from_device(ctx->c, num_cons, num_vars, num_inputs, in);
+  });
 }
 
 static void require_device(const Ctx& c, const void* p, size_t n, const char* what) {
@@ -660,32 +877,32 @@ static void require_device(const Ctx& c, const void* p, size_t n, const char* wh
 int sp_instance_create_device(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, const uint64_t* A_row, const uint64_t* A_col,
                               const uint8_t* A_val, size_t nA, const uint64_t* B_row, const uint64_t* B_col, const uint8_t* B_val, size_t nB,
                               const uint64_t* C_row, const uint64_t* C_col, const uint8_t* C_val, size_t nC, sp_instance** out) {
-  SP_TRY(ctx)
-  const dev::CooIn in = {{A_row, B_row, C_row}, {A_col, B_col, C_col}, {A_val, B_val, C_val}, {nA, nB, nC}};
-  static const char* names[3][3] = {{"A_row", "A_col", "A_val"}, {"B_row", "B_col", "B_val"}, {"C_row", "C_col", "C_val"}};
-  for (int m = 0; m < 3; m++) {
-    require_device(ctx->c, in.row[m], in.n[m], names[m][0]);
-    require_device(ctx->c, in.col[m], in.n[m], names[m][1]);
-    require_device(ctx->c, in.val[m], in.n[m], names[m][2]);
-  }
-  *out = instance_from_device(ctx->c, num_cons, num_vars, num_inputs, in);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    const dev::CooIn in = {{A_row, B_row, C_row}, {A_col, B_col, C_col}, {A_val, B_val, C_val}, {nA, nB, nC}};
+    static const char* names[3][3] = {{"A_row", "A_col", "A_val"}, {"B_row", "B_col", "B_val"}, {"C_row", "C_col", "C_val"}};
+    for (int m = 0; m < 3; m++) {
+      require_device(ctx->c, in.row[m], in.n[m], names[m][0]);
+      require_device(ctx->c, in.col[m], in.n[m], names[m][1]);
+      require_device(ctx->c, in.val[m], in.n[m], names[m][2]);
+    }
+    *out = instance_from_device(ctx->c, num_cons, num_vars, num_inputs, in);
+  });
 }
 
 int sp_poly_from_canonical_device(sp_ctx* ctx, const uint8_t* d_canonical32, size_t n, sp_poly** out) {
-  SP_TRY(ctx)
-  Ctx& c = ctx->c;
-  require_device(c, d_canonical32, n, "poly_from_canonical_device");
-  std::unique_ptr<sp_poly> p(new sp_poly{&c, DevBuf<u256>(n), n});
-  DevBuf<unsigned long long> err(1);
-  dev::set_max_u64(err.p, c.stream);
-  dev::canonical_to_mont(p->d.p, d_canonical32, n, err.p, c.stream);
-  unsigned long long first = 0;
-  dev::d2h(&first, err.p, sizeof(first), c.stream);
-  c.sync();
-  if (first != ~0ull) throw SpError(SP_ERR_INVALID_SCALAR, "R1CSError::InvalidScalar (entry " + std::to_string(first) + ")");
-  *out = p.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    Ctx& c = ctx->c;
+    require_device(c, d_canonical32, n, "poly_from_canonical_device");
+    std::unique_ptr<sp_poly> p(new sp_poly{&c, DevBuf<u256>(n), n});
+    DevBuf<unsigned long long> err(1);
+    dev::set_max_u64(err.p, c.stream);
+    dev::canonical_to_mont(p->d.p, d_canonical32, n, err.p, c.stream);
+    unsigned long long first = 0;
+    dev::d2h(&first, err.p, sizeof(first), c.stream);
+    c.sync();
+    if (first != ~0ull) throw SpError(SP_ERR_INVALID_SCALAR, "R1CSError::InvalidScalar (entry " + std::to_string(first) + ")");
+    *out = p.release();
+  });
 }
 
 static std::vector<Fq> prg_scalars(const std::string& tag, size_t n, uint64_t seed) {
@@ -702,38 +919,38 @@ static std::vector<Fq> prg_scalars(const std::string& tag, size_t n, uint64_t se
 
 int sp_instance_synthetic(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, uint64_t seed, sp_instance** out, uint64_t* vars_out,
                           uint64_t* inputs_out) {
-  SP_TRY(ctx)
-  // R1CSShape::produce_synthetic_r1cs (r1cs.rs:160-238)
-  if (next_pow2(num_cons) != num_cons || next_pow2(num_vars) != num_vars || !(num_inputs < num_vars)) throw SpError(SP_ERR_INVALID_ARG, "synthetic: sizes");
-  size_t size_z = num_vars + num_inputs + 1;
-  std::vector<Fq> Z = prg_scalars("Z", size_z, seed);
-  Z[num_vars] = Fq::one();
-  std::unique_ptr<sp_instance> I(new sp_instance);
-  I->inst.num_cons = num_cons; I->inst.num_vars = num_vars; I->inst.num_inputs = num_inputs;
-  SparseMatDev &A = I->inst.M[0], &B = I->inst.M[1], &Cm = I->inst.M[2];
-  // batch inversion of the Z values used as C_val denominators
-  std::vector<Fq> zinv(size_z), pref(size_z);
-  Fq acc = Fq::one();
-  for (size_t i = 0; i < size_z; i++) { pref[i] = acc; if (!Z[i].is_zero()) acc *= Z[i]; }
-  Fq ainv = acc.inv();
-  for (size_t i = size_z; i-- > 0;) { if (Z[i].is_zero()) { zinv[i] = Fq::zero(); continue; } zinv[i] = ainv * pref[i]; ainv *= Z[i]; }
-  for (size_t i = 0; i < num_cons; i++) {
-    size_t a = i % size_z, b = (i + 2) % size_z, c = (i + 3) % size_z;
-    A.row.push_back((uint32_t)i); A.col.push_back((uint32_t)a); A.val.push_back(Fq::one());
-    B.row.push_back((uint32_t)i); B.col.push_back((uint32_t)b); B.val.push_back(Fq::one());
-    Fq ab = Z[a] * Z[b];
-    Cm.row.push_back((uint32_t)i);
-    if (Z[c].is_zero()) { Cm.col.push_back((uint32_t)num_vars); Cm.val.push_back(ab); }
-    else { Cm.col.push_back((uint32_t)c); Cm.val.push_back(ab * zinv[c]); }
-  }
-  // the COO column index space is [vars | 1 | inputs] padded to 2*num_vars: columns >= num_vars need no shift here because
-  // produce_synthetic_r1cs requires num_vars to be a power of two already (r1cs.rs:172-176)
-  I->inst.upload_coo(&ctx->c);
-  I->inst.finalize(&ctx->c);
-  memcpy(vars_out, Z.data(), 32 * num_vars);
-  memcpy(inputs_out, Z.data() + num_vars + 1, 32 * num_inputs);
-  *out = I.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    // R1CSShape::produce_synthetic_r1cs (r1cs.rs:160-238)
+    if (next_pow2(num_cons) != num_cons || next_pow2(num_vars) != num_vars || !(num_inputs < num_vars)) throw SpError(SP_ERR_INVALID_ARG, "synthetic: sizes");
+    size_t size_z = num_vars + num_inputs + 1;
+    std::vector<Fq> Z = prg_scalars("Z", size_z, seed);
+    Z[num_vars] = Fq::one();
+    std::unique_ptr<sp_instance> I(new sp_instance);
+    I->inst.num_cons = num_cons; I->inst.num_vars = num_vars; I->inst.num_inputs = num_inputs;
+    SparseMatDev &A = I->inst.M[0], &B = I->inst.M[1], &Cm = I->inst.M[2];
+    // batch inversion of the Z values used as C_val denominators
+    std::vector<Fq> zinv(size_z), pref(size_z);
+    Fq acc = Fq::one();
+    for (size_t i = 0; i < size_z; i++) { pref[i] = acc; if (!Z[i].is_zero()) acc *= Z[i]; }
+    Fq ainv = acc.inv();
+    for (size_t i = size_z; i-- > 0;) { if (Z[i].is_zero()) { zinv[i] = Fq::zero(); continue; } zinv[i] = ainv * pref[i]; ainv *= Z[i]; }
+    for (size_t i = 0; i < num_cons; i++) {
+      size_t a = i % size_z, b = (i + 2) % size_z, c = (i + 3) % size_z;
+      A.row.push_back((uint32_t)i); A.col.push_back((uint32_t)a); A.val.push_back(Fq::one());
+      B.row.push_back((uint32_t)i); B.col.push_back((uint32_t)b); B.val.push_back(Fq::one());
+      Fq ab = Z[a] * Z[b];
+      Cm.row.push_back((uint32_t)i);
+      if (Z[c].is_zero()) { Cm.col.push_back((uint32_t)num_vars); Cm.val.push_back(ab); }
+      else { Cm.col.push_back((uint32_t)c); Cm.val.push_back(ab * zinv[c]); }
+    }
+    // the COO column index space is [vars | 1 | inputs] padded to 2*num_vars: columns >= num_vars need no shift here because
+    // produce_synthetic_r1cs requires num_vars to be a power of two already (r1cs.rs:172-176)
+    I->inst.upload_coo(&ctx->c);
+    I->inst.finalize(&ctx->c);
+    memcpy(vars_out, Z.data(), 32 * num_vars);
+    memcpy(inputs_out, Z.data() + num_vars + 1, 32 * num_inputs);
+    *out = I.release();
+  });
 }
 void sp_instance_free(sp_instance* inst) { delete inst; }
 int sp_instance_dims(const sp_instance* inst, size_t* nc, size_t* nv, size_t* ni) {
@@ -742,118 +959,78 @@ int sp_instance_dims(const sp_instance* inst, size_t* nc, size_t* nv, size_t* ni
 }
 int sp_instance_set_digest(sp_instance* inst, const uint8_t* digest, size_t len) { inst->inst.digest.assign(digest, digest + len); return SP_OK; }
 int sp_instance_bincode(const sp_instance* inst, uint8_t** out, size_t* len) {
-  try {
-    std::vector<uint8_t> raw = inst->inst.shape_bincode();
-    *out = dup_bytes(raw); *len = raw.size();
-    return SP_OK;
-  } catch (...) { return SP_ERR_INTERNAL; }
+  return host_guarded(nullptr, [&] { put_bytes(out, len, inst->inst.shape_bincode()); });
 }
 // R1CSShape::get_digest (r1cs.rs:154-158): the bytes NIZK::prove / verify absorb (lib.rs:514) — the caller's (sp_instance_set_digest) or, by
 // default, this library's miniz-level-6 zlib stream of bincode(shape), computed on first use
 int sp_instance_digest(const sp_instance* inst, uint8_t** out, size_t* len) {
-  try {
-    const std::vector<uint8_t>& d = inst->inst.shape_digest();
-    *out = dup_bytes(d); *len = d.size();
-    return SP_OK;
-  } catch (...) { return SP_ERR_INTERNAL; }
+  return host_guarded(nullptr, [&] { put_bytes(out, len, inst->inst.shape_digest()); });
 }
 int sp_instance_nnz(const sp_instance* inst, int m, size_t* nnz) { if (m < 0 || m > 2) return SP_ERR_INVALID_ARG; *nnz = inst->inst.M[m].nnz; return SP_OK; }
 int sp_instance_export(const sp_instance* inst, int m, uint64_t* row, uint64_t* col, uint64_t* val) {
   if (m < 0 || m > 2) return SP_ERR_INVALID_ARG;
-  try {
+  return host_guarded(nullptr, [&] {
     inst->inst.host_coo();
     const SparseMatDev& M = inst->inst.M[m];
     for (size_t k = 0; k < M.nnz; k++) { row[k] = M.row[k]; col[k] = M.col[k]; }
     if (M.nnz) memcpy(val, M.val.data(), 32 * M.nnz);
-    return SP_OK;
-  } catch (...) { return SP_ERR_INTERNAL; }
-}
-
-static DevBuf<u256> upload_padded_vars(Ctx& c, const Instance& I, const uint64_t* vars, size_t nvars) {
-  if (nvars > I.num_vars) throw SpError(SP_ERR_INVALID_INPUTS, "R1CSError::InvalidNumberOfInputs (vars)");
-  DevBuf<u256> d(I.num_vars);
-  dev::h2d(d.p, vars, nvars * 32, c.stream);
-  if (nvars < I.num_vars) dev::dzero(d.p + nvars, (I.num_vars - nvars) * 32, c.stream);  // Assignment::pad (lib.rs:91-104)
-  return d;
+  });
 }
 
 int sp_instance_is_sat(sp_ctx* ctx, const sp_instance* inst, const uint64_t* vars, size_t nvars, const uint64_t* inputs, size_t ninputs, int* sat) {
-  SP_TRY(ctx)
-  const Instance& I = inst->inst;
-  if (ninputs != I.num_inputs) throw SpError(SP_ERR_INVALID_INPUTS, "R1CSError::InvalidNumberOfInputs");
-  Ctx& c = ctx->c;
-  DevBuf<u256> d_vars = upload_padded_vars(c, I, vars, nvars);
-  DevBuf<u256> z(2 * I.num_vars), Az(I.num_cons), Bz(I.num_cons), Cz(I.num_cons);
-  dev::d2d(z.p, d_vars.p, I.num_vars * 32, c.stream);
-  std::vector<Fq> tail(1 + ninputs);
-  tail[0] = Fq::one();
-  if (ninputs) memcpy(&tail[1], inputs, 32 * ninputs);
-  dev::h2d(z.p + I.num_vars, tail.data(), tail.size() * 32, c.stream);
-  dev::dzero(z.p + I.num_vars + tail.size(), (I.num_vars - tail.size()) * 32, c.stream);
-  u256* outs[3] = {Az.p, Bz.p, Cz.p};
-  for (int m = 0; m < 3; m++) dev::spmv(outs[m], I.num_cons, I.M[m].csr_ptr.p, I.M[m].csr_idx.p, I.M[m].csr_val.p, z.p, c.stream);
-  DevBuf<u256> prod(I.num_cons);
-  u256* prods[1] = {prod.p};
-  const u256 *as[1] = {Az.p}, *bs[1] = {Bz.p};
-  dev::hadamard_many(prods, as, bs, 1, I.num_cons, c.stream);
-  std::vector<Fq> p = c.download(prod.p, I.num_cons), cz = c.download(Cz.p, I.num_cons);
-  *sat = 1;
-  for (size_t i = 0; i < I.num_cons; i++) if (!(p[i] == cz[i])) { *sat = 0; break; }   // r1cs.rs:265
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    const Instance& I = inst->inst;
+    if (ninputs != I.num_inputs) throw SpError(SP_ERR_INVALID_INPUTS, "R1CSError::InvalidNumberOfInputs");
+    Ctx& c = ctx->c;
+    DevBuf<u256> d_vars = upload_padded_vars(c, I, vars, nvars);
+    DevBuf<u256> z(2 * I.num_vars), Az(I.num_cons), Bz(I.num_cons), Cz(I.num_cons);
+    dev::d2d(z.p, d_vars.p, I.num_vars * 32, c.stream);
+    std::vector<Fq> tail(1 + ninputs);
+    tail[0] = Fq::one();
+    if (ninputs) memcpy(&tail[1], inputs, 32 * ninputs);
+    dev::h2d(z.p + I.num_vars, tail.data(), tail.size() * 32, c.stream);
+    dev::dzero(z.p + I.num_vars + tail.size(), (I.num_vars - tail.size()) * 32, c.stream);
+    u256* outs[3] = {Az.p, Bz.p, Cz.p};
+    for (int m = 0; m < 3; m++) dev::spmv(outs[m], I.num_cons, I.M[m].csr_ptr.p, I.M[m].csr_idx.p, I.M[m].csr_val.p, z.p, c.stream);
+    DevBuf<u256> prod(I.num_cons);
+    u256* prods[1] = {prod.p};
+    const u256 *as[1] = {Az.p}, *bs[1] = {Bz.p};
+    dev::hadamard_many(prods, as, bs, 1, I.num_cons, c.stream);
+    std::vector<Fq> p = c.download(prod.p, I.num_cons), cz = c.download(Cz.p, I.num_cons);
+    *sat = 1;
+    for (size_t i = 0; i < I.num_cons; i++) if (!(p[i] == cz[i])) { *sat = 0; break; }   // r1cs.rs:265
+  });
 }
 
 // ---- NIZK
 // private gens: tables sized for this one circuit, then a view into them (the view holds the only reference)
 int sp_nizk_gens_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, sp_nizk_gens** out) {
-  SP_TRY(ctx)
-  const GenTables t(&ctx->c, num_cons, num_vars, num_inputs, 0);
-  std::unique_ptr<sp_nizk_gens> g(new sp_nizk_gens);
-  g->g.reset(new R1CSGens(&ctx->c, t, padded_num_vars(num_vars, num_inputs)));  // lib.rs:475-481
-  *out = g.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    const GenTables t(&ctx->c, num_cons, num_vars, num_inputs, 0);
+    std::unique_ptr<sp_nizk_gens> g(new sp_nizk_gens);
+    g->g.reset(new R1CSGens(&ctx->c, t, padded_num_vars(num_vars, num_inputs)));  // lib.rs:475-481
+    *out = g.release();
+  });
 }
 int sp_nizk_gens_create_from(sp_ctx* ctx, const sp_gen_tables* tables, size_t num_cons, size_t num_vars, size_t num_inputs, sp_nizk_gens** out) {
-  SP_TRY(ctx)
-  (void)num_cons;
-  std::unique_ptr<sp_nizk_gens> g(new sp_nizk_gens);
-  g->g.reset(new R1CSGens(&ctx->c, *tables->t, padded_num_vars(num_vars, num_inputs)));
-  *out = g.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    (void)num_cons;
+    std::unique_ptr<sp_nizk_gens> g(new sp_nizk_gens);
+    g->g.reset(new R1CSGens(&ctx->c, *tables->t, padded_num_vars(num_vars, num_inputs)));
+    *out = g.release();
+  });
 }
 void sp_nizk_gens_free(sp_nizk_gens* g) { delete g; }
 
-// the caller's transcript: either a fresh Transcript::new(label) or (the _t entry points) the caller-owned STROBE state, updated in place
-struct TranscriptArg {
-  const uint8_t* label; size_t label_len; uint8_t* state; bool from_state;
-  static TranscriptArg fresh(const uint8_t* label, size_t label_len) { return {label, label_len, nullptr, false}; }
-  static TranscriptArg caller(uint8_t* state) { return {nullptr, 0, state, true}; }
-  void check() const { if (from_state && !state) throw SpError(SP_ERR_INVALID_ARG, "transcript state is NULL"); }
-  Transcript open() const { return from_state ? Transcript(Transcript::FromState(), state) : Transcript(std::string((const char*)label, label_len)); }
-  void close(const Transcript& T) const { if (from_state) T.export_state(state); }
-};
-// the witness of a prove call: the caller's host limbs, padded on upload (Assignment::pad), or a resident poly already padded to num_vars
-struct VarsArg { const uint64_t* host; size_t nvars; const sp_poly* resident; };
-static const u256* vars_on_device(Ctx& c, const Instance& I, const VarsArg& v, DevBuf<u256>& upload) {
-  if (!v.resident) { upload = upload_padded_vars(c, I, v.host, v.nvars); return upload.p; }
-  if (v.resident->len != I.num_vars) throw SpError(SP_ERR_INVALID_INPUTS, "resident vars must already be padded to num_vars");
-  return v.resident->d.p;
-}
 static int nizk_prove_common(sp_ctx* ctx, const sp_instance* inst, const VarsArg& vars, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens,
                              const TranscriptArg& ta, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  SP_TRY(ctx)
-  ta.check();
-  DevBuf<u256> upload;
-  const u256* d_vars = vars_on_device(ctx->c, inst->inst, vars, upload);
-  if (ninputs != inst->inst.num_inputs) throw SpError(SP_ERR_INVALID_INPUTS, "R1CSError::InvalidNumberOfInputs");
-  if (!seed) throw SpError(SP_ERR_INVALID_ARG, "tape seed is NULL: draw it from the OS RNG (random.rs:13-15); a fixed seed makes every blind public");
-  require_reduced(inputs, ninputs, "inputs"); require_reduced(seed, 1, "tape seed");
-  Transcript T = ta.open();
-  NizkProof P;
-  nizk_prove(ctx->c, inst->inst, d_vars, fq_vec(inputs, ninputs), *gens->g, T, fq_in(seed), P);
-  ta.close(T);
-  const std::vector<uint8_t> bytes = to_bincode(P);
-  *proof = dup_bytes(bytes); *proof_len = bytes.size();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    prove_statement(ctx->c, inst->inst, vars, inputs, ninputs, ta, seed, proof, proof_len, [&](const u256* d_vars, const std::vector<Fq>& in, Transcript& T, const Fq& s) {
+      NizkProof P;
+      nizk_prove(ctx->c, inst->inst, d_vars, in, *gens->g, T, s, P);
+      return to_bincode(P);
+    });
+  });
 }
 int sp_nizk_prove(sp_ctx* ctx, const sp_instance* inst, const uint64_t* vars, size_t nvars, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens,
                   const uint8_t* label, size_t label_len, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
@@ -871,30 +1048,30 @@ int sp_nizk_prove_resident(sp_ctx* ctx, const sp_instance* inst, const sp_poly* 
 
 // ---- SNARK
 int sp_snark_gens_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries, sp_snark_gens** out) {
-  SP_TRY(ctx)
-  // next_pow2(0) = next_pow2(1): tables for one non-zero entry are the tables num_nz_entries = 0 has always had, and they include gens_r1cs_eval
-  const GenTables t(&ctx->c, num_cons, num_vars, num_inputs, std::max<size_t>(num_nz_entries, 1));
-  std::unique_ptr<sp_snark_gens> g(new sp_snark_gens);
-  g->g.reset(new SnarkGens(&ctx->c, t, num_cons, num_vars, num_inputs, num_nz_entries));
-  *out = g.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    // next_pow2(0) = next_pow2(1): tables for one non-zero entry are the tables num_nz_entries = 0 has always had, and they include gens_r1cs_eval
+    const GenTables t(&ctx->c, num_cons, num_vars, num_inputs, std::max<size_t>(num_nz_entries, 1));
+    std::unique_ptr<sp_snark_gens> g(new sp_snark_gens);
+    g->g.reset(new SnarkGens(&ctx->c, t, num_cons, num_vars, num_inputs, num_nz_entries));
+    *out = g.release();
+  });
 }
 int sp_snark_gens_create_from(sp_ctx* ctx, const sp_gen_tables* tables, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries,
                               sp_snark_gens** out) {
-  SP_TRY(ctx)
-  std::unique_ptr<sp_snark_gens> g(new sp_snark_gens);
-  g->g.reset(new SnarkGens(&ctx->c, *tables->t, num_cons, num_vars, num_inputs, num_nz_entries));
-  *out = g.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    std::unique_ptr<sp_snark_gens> g(new sp_snark_gens);
+    g->g.reset(new SnarkGens(&ctx->c, *tables->t, num_cons, num_vars, num_inputs, num_nz_entries));
+    *out = g.release();
+  });
 }
 
 // ---- generator tables shared by gens views
 int sp_gen_tables_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_nz_entries, sp_gen_tables** out) {
-  SP_TRY(ctx)
-  std::unique_ptr<sp_gen_tables> t(new sp_gen_tables);
-  t->t.reset(new GenTables(&ctx->c, num_cons, num_vars, num_inputs, num_nz_entries));
-  *out = t.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    std::unique_ptr<sp_gen_tables> t(new sp_gen_tables);
+    t->t.reset(new GenTables(&ctx->c, num_cons, num_vars, num_inputs, num_nz_entries));
+    *out = t.release();
+  });
 }
 void sp_gen_tables_free(sp_gen_tables* t) { delete t; }
 int sp_gen_tables_info(const sp_gen_tables* t, sp_gen_set_info* out, size_t cap, size_t* n) {
@@ -916,45 +1093,36 @@ int sp_gen_tables_info(const sp_gen_tables* t, sp_gen_set_info* out, size_t cap,
 unsigned long long sp_device_bytes_live(void) { return dev::pool_live_bytes(); }
 void sp_snark_gens_free(sp_snark_gens* g) { delete g; }
 int sp_snark_encode(sp_ctx* ctx, const sp_instance* inst, const sp_snark_gens* gens, sp_snark_encoding** out) {
-  SP_TRY(ctx)
-  std::unique_ptr<sp_snark_encoding> e(new sp_snark_encoding);
-  e->e.reset(new SnarkEncoding());
-  snark_encode(ctx->c, inst->inst, *gens->g, *e->e);
-  *out = e.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    std::unique_ptr<sp_snark_encoding> e(new sp_snark_encoding);
+    e->e.reset(new SnarkEncoding());
+    snark_encode(ctx->c, inst->inst, *gens->g, *e->e);
+    *out = e.release();
+  });
 }
 void sp_snark_encoding_free(sp_snark_encoding* e) { delete e; }
 int sp_snark_commitment_bytes(const sp_snark_encoding* e, uint8_t** out, size_t* len) {
-  const std::vector<uint8_t> bytes = to_bincode(e->e->comm);
-  *out = dup_bytes(bytes); *len = bytes.size();
-  return SP_OK;
+  return host_guarded(nullptr, [&] { put_bytes(out, len, to_bincode(e->e->comm)); });
 }
 // a verifier holds only the ComputationCommitment: bincode(ComputationCommitment) -> a handle usable with sp_snark_verify (not with sp_snark_prove)
 int sp_snark_commitment_load(sp_ctx* ctx, const uint8_t* bytes, size_t len, sp_snark_encoding** out) {
-  SP_TRY(ctx)
-  std::unique_ptr<sp_snark_encoding> E(new sp_snark_encoding);
-  E->e.reset(new SnarkEncoding);
-  E->e->comm = from_bincode<ComputationCommitment>(bytes, len, SP_ERR_INVALID_ARG, "computation commitment");
-  *out = E.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    std::unique_ptr<sp_snark_encoding> E(new sp_snark_encoding);
+    E->e.reset(new SnarkEncoding);
+    E->e->comm = from_bincode<ComputationCommitment>(bytes, len, SP_ERR_INVALID_ARG, "computation commitment");
+    *out = E.release();
+  });
 }
 static int snark_prove_common(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const VarsArg& vars, const uint64_t* inputs, size_t ninputs,
                               const sp_snark_gens* gens, const TranscriptArg& ta, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  SP_TRY(ctx)
-  ta.check();
-  DevBuf<u256> upload;
-  const u256* d_vars = vars_on_device(ctx->c, inst->inst, vars, upload);
-  if (ninputs != inst->inst.num_inputs) throw SpError(SP_ERR_INVALID_INPUTS, "R1CSError::InvalidNumberOfInputs");
-  if (!enc->e->comb_ops.p) throw SpError(SP_ERR_INVALID_ARG, "this handle holds a commitment only (sp_snark_commitment_load): proving needs sp_snark_encode");
-  if (!seed) throw SpError(SP_ERR_INVALID_ARG, "tape seed is NULL: draw it from the OS RNG (random.rs:13-15); a fixed seed makes every blind public");
-  require_reduced(inputs, ninputs, "inputs"); require_reduced(seed, 1, "tape seed");
-  Transcript T = ta.open();
-  SnarkProof P;
-  snark_prove(ctx->c, inst->inst, *enc->e, d_vars, fq_vec(inputs, ninputs), *gens->g, T, fq_in(seed), P);
-  ta.close(T);
-  const std::vector<uint8_t> bytes = to_bincode(P);
-  *proof = dup_bytes(bytes); *proof_len = bytes.size();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (!enc->e->comb_ops.p) throw SpError(SP_ERR_INVALID_ARG, "this handle holds a commitment only (sp_snark_commitment_load): proving needs sp_snark_encode");
+    prove_statement(ctx->c, inst->inst, vars, inputs, ninputs, ta, seed, proof, proof_len, [&](const u256* d_vars, const std::vector<Fq>& in, Transcript& T, const Fq& s) {
+      SnarkProof P;
+      snark_prove(ctx->c, inst->inst, *enc->e, d_vars, in, *gens->g, T, s, P);
+      return to_bincode(P);
+    });
+  });
 }
 int sp_snark_prove(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const uint64_t* vars, size_t nvars, const uint64_t* inputs, size_t ninputs,
                    const sp_snark_gens* gens, const uint8_t* label, size_t label_len, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
@@ -970,37 +1138,14 @@ int sp_snark_prove_resident(sp_ctx* ctx, const sp_instance* inst, const sp_snark
   return snark_prove_common(ctx, inst, enc, {nullptr, 0, vars}, inputs, ninputs, gens, TranscriptArg::fresh(label, label_len), seed, proof, proof_len);
 }
 
-// ---- verifiers.  The _t forms verify on the caller's transcript state (lib.rs:423-429, :549-555), which is updated in place whether or not the
-// proof is accepted (a _t prove writes it back only on success).
-struct TranscriptClose { const TranscriptArg& ta; const Transcript& T; ~TranscriptClose() { ta.close(T); } };
-// SP_FINE_TIMERS=1: the sub-phase timers of the last verify call (single or batch) replace sp_timings, as a prove call's do
-static void flush_fine(Ctx& c) {
-  if (!FineTimer::enabled()) return;
-  c.timings.clear();
-  for (auto& f : c.fine) c.timings.push_back({"fine:" + f.first, f.second});
-  c.fine.clear();
-}
+// ---- verifiers.  The _t forms verify on the caller's transcript state (lib.rs:423-429, :549-555).
 static int nizk_verify_common(sp_ctx* ctx, const sp_instance* inst, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens, const TranscriptArg& ta,
                               const uint8_t* proof, size_t proof_len) {
-  SP_TRY(ctx)
-  ta.check();
-  require_reduced(inputs, ninputs, "inputs");
-  Transcript T = ta.open();
-  TranscriptClose close{ta, T};
-  nizk_verify(ctx->c, inst->inst, fq_vec(inputs, ninputs), *gens->g, T, proof, proof_len);
-  flush_fine(ctx->c);
-  SP_CATCH(ctx)
+  return verify_statement(ctx, inputs, ninputs, ta, [&](const std::vector<Fq>& in, Transcript& T) { nizk_verify(ctx->c, inst->inst, in, *gens->g, T, proof, proof_len); });
 }
 static int snark_verify_common(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t* inputs, size_t ninputs, const sp_snark_gens* gens,
                                const TranscriptArg& ta, const uint8_t* proof, size_t proof_len) {
-  SP_TRY(ctx)
-  ta.check();
-  require_reduced(inputs, ninputs, "inputs");
-  Transcript T = ta.open();
-  TranscriptClose close{ta, T};
-  snark_verify(ctx->c, *comm->e, fq_vec(inputs, ninputs), *gens->g, T, proof, proof_len);
-  flush_fine(ctx->c);
-  SP_CATCH(ctx)
+  return verify_statement(ctx, inputs, ninputs, ta, [&](const std::vector<Fq>& in, Transcript& T) { snark_verify(ctx->c, *comm->e, in, *gens->g, T, proof, proof_len); });
 }
 int sp_nizk_verify(sp_ctx* ctx, const sp_instance* inst, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens, const uint8_t* label, size_t label_len,
                    const uint8_t* proof, size_t proof_len) {
@@ -1023,66 +1168,57 @@ int sp_snark_verify_t(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t
 static int sumcheck_prove_common(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim[4],
                                  size_t num_rounds, const TranscriptArg& ta, uint8_t** proof, size_t* proof_len, uint64_t* r_out, uint64_t* finals_out,
                                  uint64_t e_out[4]) {
-  SP_TRY(ctx)
-  ta.check();
-  if (!tables || !terms || !claim || !proof || !proof_len || !r_out || !finals_out || !e_out) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: NULL argument");
-  if (k < 1 || k > SP_SC_MAX_TABLES)
-    throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: " + std::to_string(k) + " tables; 1 .. SP_SC_MAX_TABLES = " + std::to_string(SP_SC_MAX_TABLES) + " supported");
-  if (nterms < 1 || nterms > SP_SC_MAX_TERMS)
-    throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: " + std::to_string(nterms) + " terms; 1 .. SP_SC_MAX_TERMS = " + std::to_string(SP_SC_MAX_TERMS) + " supported");
-  for (int i = 0; i < k; i++) {
-    if (!tables[i]) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: table " + std::to_string(i) + " is NULL");
-    if (tables[i]->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: table " + std::to_string(i) + " belongs to another context");
-    if (tables[i]->len != tables[0]->len) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: tables differ in length");
-  }
-  const size_t len = tables[0]->len;
-  if (len < 2 || (len & (len - 1))) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: length must be a power of two >= 2");
-  const size_t m = log2_ceil(len);
-  if (num_rounds < 1 || num_rounds > m)
-    throw SpError(SP_ERR_INVALID_ARG, "sumcheck_prove: num_rounds = " + std::to_string(num_rounds) + " outside 1 .. " + std::to_string(m) + " (the tables' variables)");
-  dev::ScPoly P;
-  memset(static_cast<void*>(&P), 0, sizeof P);
-  std::vector<sp_poly*> distinct;   // a handle passed twice is one table, bound once per round
-  std::vector<uint8_t> slot(k);
-  for (int i = 0; i < k; i++) {
-    const size_t at = std::find(distinct.begin(), distinct.end(), tables[i]) - distinct.begin();
-    if (at == distinct.size()) { distinct.push_back(tables[i]); P.t[at] = tables[i]->d.p; }
-    slot[i] = (uint8_t)at;
-  }
-  P.ntables = (int)distinct.size();
-  P.nterms = nterms;
-  const Fq one = Fq::one();
-  for (int t = 0; t < nterms; t++) {
-    const sp_sc_term& tm = terms[t];
-    const std::string at = "sumcheck_prove: term " + std::to_string(t);
-    if (tm.nfactors == 0) throw SpError(SP_ERR_INVALID_ARG, at + " has no factors");
-    if (tm.nfactors > SP_SC_MAX_DEGREE)
-      throw SpError(SP_ERR_INVALID_ARG, at + " has " + std::to_string(tm.nfactors) + " factors; degree <= SP_SC_MAX_DEGREE = " + std::to_string(SP_SC_MAX_DEGREE) + " supported");
-    for (uint32_t f = 0; f < tm.nfactors; f++) {
-      if (tm.factor[f] >= (uint32_t)k) throw SpError(SP_ERR_INVALID_ARG, at + ": table index " + std::to_string(tm.factor[f]) + " >= k = " + std::to_string(k));
-      P.fac[t][f] = slot[tm.factor[f]];
+  return guarded(ctx, [&] {
+    const std::string what = "sumcheck_prove";
+    ta.check();
+    if (!tables || !terms || !claim || !proof || !proof_len || !r_out || !finals_out || !e_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    require_count(what, k, "tables", "SP_SC_MAX_TABLES", SP_SC_MAX_TABLES);
+    require_count(what, nterms, "terms", "SP_SC_MAX_TERMS", SP_SC_MAX_TERMS);
+    const size_t len = caller_tables(ctx, tables, k, what, 2).len, m = log2_ceil(len);
+    if (num_rounds < 1 || num_rounds > m)
+      throw SpError(SP_ERR_INVALID_ARG, what + ": num_rounds = " + std::to_string(num_rounds) + " outside 1 .. " + std::to_string(m) + " (the tables' variables)");
+    dev::ScPoly P;
+    memset(static_cast<void*>(&P), 0, sizeof P);
+    std::vector<sp_poly*> distinct;   // a handle passed twice is one table, bound once per round
+    std::vector<uint8_t> slot(k);
+    for (int i = 0; i < k; i++) {
+      const size_t at = std::find(distinct.begin(), distinct.end(), tables[i]) - distinct.begin();
+      if (at == distinct.size()) { distinct.push_back(tables[i]); P.t[at] = tables[i]->d.p; }
+      slot[i] = (uint8_t)at;
     }
-    require_reduced(tm.coeff_mont, 1, "sumcheck_prove: coefficient");
-    const Fq c = fq_in(tm.coeff_mont);
-    P.coeff[t] = c.m;
-    P.unit[t] = c == one;
-    P.nfac[t] = (uint8_t)tm.nfactors;
-    P.degree = std::max(P.degree, (int)tm.nfactors);
-  }
-  require_reduced(claim, 1, "sumcheck_prove: claim");
-  Transcript T = ta.open();
-  SumcheckInstanceProof pr;
-  std::vector<Fq> r, finals;
-  Fq e;
-  poly_sumcheck_prove(ctx->c, P, len, fq_in(claim), num_rounds, T, pr, r, finals, e);
-  for (sp_poly* p : distinct) p->len >>= num_rounds;
-  ta.close(T);
-  const std::vector<uint8_t> bytes = to_bincode(pr);
-  *proof = dup_bytes(bytes); *proof_len = bytes.size();
-  for (size_t j = 0; j < num_rounds; j++) fq_out(r_out + 4 * j, r[j]);
-  for (int i = 0; i < k; i++) fq_out(finals_out + 4 * i, finals[slot[i]]);
-  fq_out(e_out, e);
-  SP_CATCH(ctx)
+    P.ntables = (int)distinct.size();
+    P.nterms = nterms;
+    const Fq one = Fq::one();
+    for (int t = 0; t < nterms; t++) {
+      const sp_sc_term& tm = terms[t];
+      const std::string at = what + ": term " + std::to_string(t);
+      if (tm.nfactors == 0) throw SpError(SP_ERR_INVALID_ARG, at + " has no factors");
+      if (tm.nfactors > SP_SC_MAX_DEGREE)
+        throw SpError(SP_ERR_INVALID_ARG, at + " has " + std::to_string(tm.nfactors) + " factors; degree <= SP_SC_MAX_DEGREE = " + std::to_string(SP_SC_MAX_DEGREE) + " supported");
+      for (uint32_t f = 0; f < tm.nfactors; f++) {
+        if (tm.factor[f] >= (uint32_t)k) throw SpError(SP_ERR_INVALID_ARG, at + ": table index " + std::to_string(tm.factor[f]) + " >= k = " + std::to_string(k));
+        P.fac[t][f] = slot[tm.factor[f]];
+      }
+      require_reduced(tm.coeff_mont, 1, "sumcheck_prove: coefficient");
+      const Fq c = fq_in(tm.coeff_mont);
+      P.coeff[t] = c.m;
+      P.unit[t] = c == one;
+      P.nfac[t] = (uint8_t)tm.nfactors;
+      P.degree = std::max(P.degree, (int)tm.nfactors);
+    }
+    require_reduced(claim, 1, "sumcheck_prove: claim");
+    Transcript T = ta.open();
+    SumcheckInstanceProof pr;
+    std::vector<Fq> r, finals;
+    Fq e;
+    poly_sumcheck_prove(ctx->c, P, len, fq_in(claim), num_rounds, T, pr, r, finals, e);
+    for (sp_poly* p : distinct) p->len >>= num_rounds;
+    ta.close(T);
+    put_bytes(proof, proof_len, to_bincode(pr));
+    put_scalars(r_out, r);
+    for (int i = 0; i < k; i++) fq_out(finals_out + 4 * i, finals[slot[i]]);
+    fq_out(e_out, e);
+  });
 }
 int sp_sumcheck_prove_t(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim[4], size_t num_rounds,
                         uint8_t* strobe_state, uint8_t** proof, size_t* proof_len, uint64_t* r_out, uint64_t* finals_out, uint64_t e_out[4]) {
@@ -1096,8 +1232,7 @@ int sp_sumcheck_prove(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_te
 // host only: no device work, so ctx may be NULL (the message then goes where sp_last_error(NULL) reads it)
 int sp_sumcheck_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const uint64_t claim[4], size_t num_rounds, size_t degree_bound,
                          uint8_t* strobe_state, uint64_t e_out[4], uint64_t* r_out) {
-  std::string& err = ctx ? ctx->c.last_error : g_create_error;
-  try {
+  return host_guarded(ctx, [&] {
     const TranscriptArg ta = TranscriptArg::caller(strobe_state);
     ta.check();
     if (!claim || !e_out || (!r_out && num_rounds) || (!proof && proof_len)) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_verify: NULL argument");
@@ -1106,327 +1241,222 @@ int sp_sumcheck_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, co
     Transcript T = ta.open();
     TranscriptClose close{ta, T};
     std::vector<Fq> r;
-    const Fq e = sumcheck_verify_bytes(proof, proof_len, fq_in(claim), num_rounds, degree_bound, T, r);
-    fq_out(e_out, e);
-    for (size_t j = 0; j < num_rounds; j++) fq_out(r_out + 4 * j, r[j]);
-    return SP_OK;
-  } catch (const SpError& e) { err = e.what(); return e.code; }
-  catch (const std::exception& e) { err = e.what(); return SP_ERR_INTERNAL; }
+    fq_out(e_out, sumcheck_verify_bytes(proof, proof_len, fq_in(claim), num_rounds, degree_bound, T, r));
+    put_scalars(r_out, r);
+  });
 }
 
 // ---- polynomial commitments and evaluation proofs for the caller's tables (prover.cpp: pc_*).  Every argument is checked before the first
 // launch and before the transcript or the tape is touched, so a refused call leaves the tables, the transcript and the tape as they were.
-}  // extern "C"
-struct sp_pc_gens {
-  Ctx* ctx;
-  std::shared_ptr<GenSet> set;   // shared by the views made from it
-  size_t num_vars;
-  PolyCommitmentGens g;
-};
-// the k tables of one call: non-null handles of this context, of one power-of-two length; returns log2 of it
-static size_t pc_tables(sp_ctx* ctx, sp_poly* const* polys, int k, const std::string& what, std::vector<const u256*>& out) {
-  if (!polys) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL table array");
-  if (k < 1 || k > SP_PC_MAX_TABLES)
-    throw SpError(SP_ERR_INVALID_ARG, what + ": " + std::to_string(k) + " tables; 1 .. SP_PC_MAX_TABLES = " + std::to_string(SP_PC_MAX_TABLES) + " supported");
-  for (int i = 0; i < k; i++) {
-    if (!polys[i]) throw SpError(SP_ERR_INVALID_ARG, what + ": table " + std::to_string(i) + " is NULL");
-    if (polys[i]->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, what + ": table " + std::to_string(i) + " belongs to another context");
-    if (polys[i]->len != polys[0]->len) throw SpError(SP_ERR_INVALID_ARG, what + ": tables differ in length");
-  }
-  const size_t len = polys[0]->len;
-  if (!len || (len & (len - 1))) throw SpError(SP_ERR_INVALID_ARG, what + ": the table length must be a power of two");
-  out.assign(k, nullptr);
-  for (int i = 0; i < k; i++) out[i] = polys[i]->d.p;
-  return log2_ceil(len);
-}
-// gens of this context whose n is the row length R = 2^ceil(ell/2) of a table of 2^ell entries (commitments.rs:87-91 asserts gens_n.n == R)
-static void pc_check_gens(sp_ctx* ctx, const sp_pc_gens* g, size_t ell, const std::string& what) {
-  if (!g) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL gens");
-  if (g->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, what + ": the gens belong to another context");
-  if (g->g.n != pc_gens_n(ell))
-    throw SpError(SP_ERR_INVALID_ARG, what + ": gens for num_vars = " + std::to_string(g->num_vars) + " have n = " + std::to_string(g->g.n) +
-                                          ", a table of 2^" + std::to_string(ell) + " entries needs n = R = " + std::to_string(pc_gens_n(ell)));
-}
-static const size_t PC_MAX_VARS = 60;
-static Transcript pc_tape_open(const uint8_t* tape_state, const std::string& what) {
-  if (!tape_state) throw SpError(SP_ERR_INVALID_ARG, what + ": tape state is NULL");
-  return Transcript(Transcript::FromState(), tape_state);
-}
-extern "C" {
-
 int sp_pc_gens_create(sp_ctx* ctx, size_t num_vars, const uint8_t* label, size_t label_len, sp_pc_gens** out) {
-  SP_TRY(ctx)
-  if (!out || (!label && label_len)) throw SpError(SP_ERR_INVALID_ARG, "pc_gens_create: NULL argument");
-  if (num_vars > PC_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, "pc_gens_create: num_vars = " + std::to_string(num_vars) + " > " + std::to_string(PC_MAX_VARS));
-  const size_t n = pc_gens_n(num_vars);
-  std::unique_ptr<sp_pc_gens> g(new sp_pc_gens{&ctx->c, nullptr, num_vars, {}});
-  g->set = std::make_shared<GenSet>(&ctx->c, std::string((const char*)label, label_len), n + 2, std::vector<size_t>{n, n + 1});
-  g->g = pc_gens_view(*g->set, num_vars);
-  *out = g.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    if (!out || (!label && label_len)) throw SpError(SP_ERR_INVALID_ARG, "pc_gens_create: NULL argument");
+    if (num_vars > PC_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, "pc_gens_create: num_vars = " + std::to_string(num_vars) + " > " + std::to_string(PC_MAX_VARS));
+    const size_t n = pc_gens_n(num_vars);
+    std::unique_ptr<sp_pc_gens> g(new sp_pc_gens{&ctx->c, nullptr, num_vars, {}});
+    g->set = std::make_shared<GenSet>(&ctx->c, std::string((const char*)label, label_len), n + 2, std::vector<size_t>{n, n + 1});
+    g->g = pc_gens_view(*g->set, num_vars);
+    *out = g.release();
+  });
 }
 int sp_pc_gens_create_from(sp_ctx* ctx, const sp_pc_gens* larger, size_t num_vars, sp_pc_gens** out) {
-  SP_TRY(ctx)
-  if (!larger || !out) throw SpError(SP_ERR_INVALID_ARG, "pc_gens_create_from: NULL argument");
-  if (larger->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, "pc_gens_create_from: the gens belong to another context");
-  if (num_vars > larger->num_vars)
-    throw SpError(SP_ERR_INVALID_ARG, "pc_gens_create_from: num_vars = " + std::to_string(num_vars) + " > the larger gens' " + std::to_string(larger->num_vars));
-  std::unique_ptr<sp_pc_gens> g(new sp_pc_gens{&ctx->c, larger->set, num_vars, {}});
-  g->g = pc_gens_view(*g->set, num_vars);
-  *out = g.release();
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    const std::string what = "pc_gens_create_from";
+    if (!out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    require_owned(ctx, larger, what, "gens handle");
+    if (num_vars > larger->num_vars)
+      throw SpError(SP_ERR_INVALID_ARG, what + ": num_vars = " + std::to_string(num_vars) + " > the larger gens' " + std::to_string(larger->num_vars));
+    std::unique_ptr<sp_pc_gens> g(new sp_pc_gens{&ctx->c, larger->set, num_vars, {}});
+    g->g = pc_gens_view(*g->set, num_vars);
+    *out = g.release();
+  });
 }
 void sp_pc_gens_free(sp_pc_gens* g) { delete g; }
 
 // host only: no context
 int sp_random_tape_new(const uint64_t seed[4], uint8_t* tape_state) {
-  try {
+  return host_guarded(nullptr, [&] {
     if (!seed || !tape_state) throw SpError(SP_ERR_INVALID_ARG, "random_tape_new: NULL argument");
     require_reduced(seed, 1, "random_tape_new: seed");
     RandomTape(std::string("proof"), fq_in(seed)).state().export_state(tape_state);   // random.rs:10-17
-    return SP_OK;
-  } catch (const SpError& e) { g_create_error = e.what(); return e.code; }
+  });
 }
 
 int sp_pc_commit(sp_ctx* ctx, const sp_pc_gens* gens, sp_poly* const* polys, int k, uint8_t* tape_state, uint8_t** comm, size_t* comm_len, uint64_t* blinds_out) {
-  SP_TRY(ctx)
-  const std::string what = "pc_commit";
-  if (!comm || !comm_len) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
-  std::vector<const u256*> t;
-  const size_t m = pc_tables(ctx, polys, k, what, t), ell = m + log2_ceil(next_pow2((size_t)k));
-  pc_check_gens(ctx, gens, ell, what);
-  const size_t L = (size_t)1 << (ell / 2);
-  std::vector<Fq> blinds(L, Fq::zero());
-  std::unique_ptr<RandomTape> tape;
-  if (tape_state) {
-    tape.reset(new RandomTape(pc_tape_open(tape_state, what)));
-    blinds = tape->random_vector("poly_blinds", L);   // dense_mlpoly.rs:185-189
-  }
-  const std::vector<uint8_t> bytes = to_bincode(pc_commit(ctx->c, gens->g, t.data(), k, m, tape ? blinds.data() : nullptr));
-  if (tape) tape->state().export_state(tape_state);
-  *comm = dup_bytes(bytes); *comm_len = bytes.size();
-  if (blinds_out) for (size_t i = 0; i < L; i++) fq_out(blinds_out + 4 * i, blinds[i]);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    const std::string what = "pc_commit";
+    if (!comm || !comm_len) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    require_count(what, k, "tables", "SP_PC_MAX_TABLES", SP_PC_MAX_TABLES);
+    const Tables t = caller_tables(ctx, polys, k, what, 1);
+    const size_t m = log2_ceil(t.len), ell = m + log2_ceil(next_pow2((size_t)k));
+    pc_check_gens(ctx, gens, ell, what);
+    const size_t L = (size_t)1 << (ell / 2);
+    std::vector<Fq> blinds(L, Fq::zero());
+    std::unique_ptr<RandomTape> tape;
+    if (tape_state) {
+      tape.reset(new RandomTape(pc_tape_open(tape_state, what)));
+      blinds = tape->random_vector("poly_blinds", L);   // dense_mlpoly.rs:185-189
+    }
+    const std::vector<uint8_t> bytes = to_bincode(pc_commit(ctx->c, gens->g, t.d.data(), k, m, tape ? blinds.data() : nullptr));
+    if (tape) tape->state().export_state(tape_state);
+    put_bytes(comm, comm_len, bytes);
+    if (blinds_out) put_scalars(blinds_out, blinds);
+  });
 }
 
 int sp_pc_eval_prove_t(sp_ctx* ctx, const sp_pc_gens* gens, const sp_poly* poly, const uint64_t* blinds, const uint64_t* r, size_t ell, const uint64_t* Zr,
                        const uint64_t* blind_Zr, uint8_t* strobe_state, uint8_t* tape_state, uint8_t** proof, size_t* proof_len, uint8_t C_Zr32[32],
                        uint64_t Zr_out[4]) {
-  SP_TRY(ctx)
-  const std::string what = "pc_eval_prove";
-  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-  ta.check();
-  if (!poly || !proof || !proof_len || !C_Zr32 || !Zr_out || (!r && ell)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
-  sp_poly* const p = const_cast<sp_poly*>(poly);
-  std::vector<const u256*> t;
-  if (pc_tables(ctx, &p, 1, what, t) != ell || ell > PC_MAX_VARS)
-    throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(ell) + " but the table has " + std::to_string(poly->len) + " entries");
-  pc_check_gens(ctx, gens, ell, what);
-  const size_t L = (size_t)1 << (ell / 2);
-  require_reduced(r, ell, "pc_eval_prove: r");
-  if (Zr) require_reduced(Zr, 1, "pc_eval_prove: Zr");
-  if (blind_Zr) require_reduced(blind_Zr, 1, "pc_eval_prove: blind_Zr");
-  if (blinds) require_reduced(blinds, L, "pc_eval_prove: blinds");
-  RandomTape tape(pc_tape_open(tape_state, what));
-  Transcript T = ta.open();
-  const std::vector<Fq> bl = blinds ? fq_vec(blinds, L) : std::vector<Fq>();
-  const Fq Zr_in = Zr ? fq_in(Zr) : Fq::zero(), bZr = blind_Zr ? fq_in(blind_Zr) : Fq::zero();
-  PolyEvalProof P;
-  Cp C;
-  Fq zr;
-  polyeval_prove(ctx->c, poly->d.p, blinds ? &bl : nullptr, fq_vec(r, ell), Zr ? &Zr_in : nullptr, blind_Zr ? &bZr : nullptr, gens->g, T, tape, P, C, &zr);
-  ta.close(T);
-  tape.state().export_state(tape_state);
-  const std::vector<uint8_t> bytes = to_bincode(P);
-  *proof = dup_bytes(bytes); *proof_len = bytes.size();
-  memcpy(C_Zr32, C.b, 32);
-  fq_out(Zr_out, zr);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    const std::string what = "pc_eval_prove";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if (!poly || !proof || !proof_len || !C_Zr32 || !Zr_out || (!r && ell)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    sp_poly* const p = const_cast<sp_poly*>(poly);
+    if (log2_ceil(caller_tables(ctx, &p, 1, what, 1).len) != ell || ell > PC_MAX_VARS)
+      throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(ell) + " but the table has " + std::to_string(poly->len) + " entries");
+    pc_check_gens(ctx, gens, ell, what);
+    const size_t L = (size_t)1 << (ell / 2);
+    require_reduced(r, ell, "pc_eval_prove: r");
+    if (Zr) require_reduced(Zr, 1, "pc_eval_prove: Zr");
+    if (blind_Zr) require_reduced(blind_Zr, 1, "pc_eval_prove: blind_Zr");
+    if (blinds) require_reduced(blinds, L, "pc_eval_prove: blinds");
+    RandomTape tape(pc_tape_open(tape_state, what));
+    Transcript T = ta.open();
+    const std::vector<Fq> bl = blinds ? fq_vec(blinds, L) : std::vector<Fq>();
+    const Fq Zr_in = Zr ? fq_in(Zr) : Fq::zero(), bZr = blind_Zr ? fq_in(blind_Zr) : Fq::zero();
+    PolyEvalProof P;
+    Cp C;
+    Fq zr;
+    polyeval_prove(ctx->c, poly->d.p, blinds ? &bl : nullptr, fq_vec(r, ell), Zr ? &Zr_in : nullptr, blind_Zr ? &bZr : nullptr, gens->g, T, tape, P, C, &zr);
+    ta.close(T);
+    tape.state().export_state(tape_state);
+    put_bytes(proof, proof_len, to_bincode(P));
+    memcpy(C_Zr32, C.b, 32);
+    fq_out(Zr_out, zr);
+  });
 }
 
 int sp_pc_eval_verify_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t* comm, size_t comm_len, const uint64_t* r, size_t ell, const uint8_t C_Zr32[32],
                         const uint64_t Zr[4], uint8_t* strobe_state, const uint8_t* proof, size_t proof_len) {
-  SP_TRY(ctx)
-  const std::string what = "pc_eval_verify";
-  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-  ta.check();
-  if ((!comm && comm_len) || (!proof && proof_len) || (!r && ell)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
-  if (!C_Zr32 == !Zr) throw SpError(SP_ERR_INVALID_ARG, what + ": give exactly one of C_Zr and Zr");
-  if (ell > PC_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(ell) + " > " + std::to_string(PC_MAX_VARS));
-  pc_check_gens(ctx, gens, ell, what);
-  require_reduced(r, ell, "pc_eval_verify: r");
-  if (Zr) require_reduced(Zr, 1, "pc_eval_verify: Zr");
-  const PolyCommitment pc = from_bincode<PolyCommitment>(comm, comm_len, SP_ERR_INVALID_ARG, "polynomial commitment");
-  Cp c;
-  if (C_Zr32) memcpy(c.b, C_Zr32, 32);
-  const Fq zr = Zr ? fq_in(Zr) : Fq::zero();
-  Transcript T = ta.open();
-  TranscriptClose close{ta, T};
-  pc_eval_verify(ctx->c, gens->g, pc, fq_vec(r, ell), C_Zr32 ? &c : nullptr, Zr ? &zr : nullptr, T, proof, proof_len);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    const std::string what = "pc_eval_verify";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if ((!comm && comm_len) || (!proof && proof_len) || (!r && ell)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    if (!C_Zr32 == !Zr) throw SpError(SP_ERR_INVALID_ARG, what + ": give exactly one of C_Zr and Zr");
+    if (ell > PC_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(ell) + " > " + std::to_string(PC_MAX_VARS));
+    pc_check_gens(ctx, gens, ell, what);
+    require_reduced(r, ell, "pc_eval_verify: r");
+    if (Zr) require_reduced(Zr, 1, "pc_eval_verify: Zr");
+    const PolyCommitment pc = from_bincode<PolyCommitment>(comm, comm_len, SP_ERR_INVALID_ARG, "polynomial commitment");
+    Cp c;
+    if (C_Zr32) memcpy(c.b, C_Zr32, 32);
+    const Fq zr = Zr ? fq_in(Zr) : Fq::zero();
+    Transcript T = ta.open();
+    TranscriptClose close{ta, T};
+    pc_eval_verify(ctx->c, gens->g, pc, fq_vec(r, ell), C_Zr32 ? &c : nullptr, Zr ? &zr : nullptr, T, proof, proof_len);
+  });
 }
 
 int sp_pc_eval_prove_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, sp_poly* const* polys, int k, const uint64_t* blinds, const uint64_t* r, size_t m,
                              uint8_t* strobe_state, uint8_t* tape_state, uint8_t** proof, size_t* proof_len, uint64_t* evals_out) {
-  SP_TRY(ctx)
-  const std::string what = "pc_eval_prove_joint";
-  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-  ta.check();
-  if (!proof || !proof_len || !evals_out || (!r && m)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
-  std::vector<const u256*> t;
-  if (pc_tables(ctx, polys, k, what, t) != m || m > PC_MAX_VARS)
-    throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(m) + " but the tables have " + std::to_string(polys[0]->len) + " entries");
-  const size_t ell = m + log2_ceil(next_pow2((size_t)k)), L = (size_t)1 << (ell / 2);
-  pc_check_gens(ctx, gens, ell, what);
-  require_reduced(r, m, "pc_eval_prove_joint: r");
-  if (blinds) require_reduced(blinds, L, "pc_eval_prove_joint: blinds");
-  RandomTape tape(pc_tape_open(tape_state, what));
-  Transcript T = ta.open();
-  const std::vector<Fq> bl = blinds ? fq_vec(blinds, L) : std::vector<Fq>();
-  PolyEvalProof P;
-  std::vector<Fq> evals;
-  pc_eval_prove_joint(ctx->c, gens->g, t.data(), k, fq_vec(r, m), blinds ? &bl : nullptr, T, tape, P, evals);
-  ta.close(T);
-  tape.state().export_state(tape_state);
-  const std::vector<uint8_t> bytes = to_bincode(P);
-  *proof = dup_bytes(bytes); *proof_len = bytes.size();
-  for (int j = 0; j < k; j++) fq_out(evals_out + 4 * j, evals[j]);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    const std::string what = "pc_eval_prove_joint";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if (!proof || !proof_len || !evals_out || (!r && m)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    require_count(what, k, "tables", "SP_PC_MAX_TABLES", SP_PC_MAX_TABLES);
+    const Tables t = caller_tables(ctx, polys, k, what, 1);
+    if (log2_ceil(t.len) != m || m > PC_MAX_VARS)
+      throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(m) + " but the tables have " + std::to_string(t.len) + " entries");
+    const size_t ell = m + log2_ceil(next_pow2((size_t)k)), L = (size_t)1 << (ell / 2);
+    pc_check_gens(ctx, gens, ell, what);
+    require_reduced(r, m, "pc_eval_prove_joint: r");
+    if (blinds) require_reduced(blinds, L, "pc_eval_prove_joint: blinds");
+    RandomTape tape(pc_tape_open(tape_state, what));
+    Transcript T = ta.open();
+    const std::vector<Fq> bl = blinds ? fq_vec(blinds, L) : std::vector<Fq>();
+    PolyEvalProof P;
+    std::vector<Fq> evals;
+    pc_eval_prove_joint(ctx->c, gens->g, t.d.data(), k, fq_vec(r, m), blinds ? &bl : nullptr, T, tape, P, evals);
+    ta.close(T);
+    tape.state().export_state(tape_state);
+    put_bytes(proof, proof_len, to_bincode(P));
+    put_scalars(evals_out, evals);
+  });
 }
 
 int sp_pc_eval_verify_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t* comm, size_t comm_len, const uint64_t* r, size_t m, const uint64_t* evals,
                               int k, uint8_t* strobe_state, const uint8_t* proof, size_t proof_len) {
-  SP_TRY(ctx)
-  const std::string what = "pc_eval_verify_joint";
-  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-  ta.check();
-  if ((!comm && comm_len) || (!proof && proof_len) || (!r && m) || !evals) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
-  if (k < 1 || k > SP_PC_MAX_TABLES)
-    throw SpError(SP_ERR_INVALID_ARG, what + ": " + std::to_string(k) + " evaluations; 1 .. SP_PC_MAX_TABLES = " + std::to_string(SP_PC_MAX_TABLES) + " supported");
-  if (m > PC_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(m) + " > " + std::to_string(PC_MAX_VARS));
-  pc_check_gens(ctx, gens, m + log2_ceil(next_pow2((size_t)k)), what);
-  require_reduced(r, m, "pc_eval_verify_joint: r");
-  require_reduced(evals, (size_t)k, "pc_eval_verify_joint: evals");
-  const PolyCommitment pc = from_bincode<PolyCommitment>(comm, comm_len, SP_ERR_INVALID_ARG, "polynomial commitment");
-  Transcript T = ta.open();
-  TranscriptClose close{ta, T};
-  pc_eval_verify_joint(ctx->c, gens->g, pc, fq_vec(r, m), fq_vec(evals, (size_t)k), T, proof, proof_len);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    const std::string what = "pc_eval_verify_joint";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if ((!comm && comm_len) || (!proof && proof_len) || (!r && m) || !evals) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    require_count(what, k, "evaluations", "SP_PC_MAX_TABLES", SP_PC_MAX_TABLES);
+    if (m > PC_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(m) + " > " + std::to_string(PC_MAX_VARS));
+    pc_check_gens(ctx, gens, m + log2_ceil(next_pow2((size_t)k)), what);
+    require_reduced(r, m, "pc_eval_verify_joint: r");
+    require_reduced(evals, (size_t)k, "pc_eval_verify_joint: evals");
+    const PolyCommitment pc = from_bincode<PolyCommitment>(comm, comm_len, SP_ERR_INVALID_ARG, "polynomial commitment");
+    Transcript T = ta.open();
+    TranscriptClose close{ta, T};
+    pc_eval_verify_joint(ctx->c, gens->g, pc, fq_vec(r, m), fq_vec(evals, (size_t)k), T, proof, proof_len);
+  });
 }
 
 // ---- product circuits of the caller's tables (product.cpp: prod_*).  Every argument is checked before the first launch or allocation and before
 // the transcript is touched, so a refused call leaves the tables, the transcript and the device memory as they were.
-}  // extern "C"
-struct sp_prod_circuits {
-  Ctx* ctx;
-  size_t m;
-  std::vector<std::unique_ptr<ProdCircuit>> cs;   // released by the proof
-  bool spent;
-};
-static const size_t PROD_MAX_VARS = 60;
-// one circuit's leaf form, checked: leaf[x] = cst + idx * x + sum_s coeff[s] * table[src[s]][x]
-struct LeafForm { uint32_t nsrc = 0; uint32_t src[SP_PROD_MAX_SOURCES] = {}; Fq coeff[SP_PROD_MAX_SOURCES], idx = Fq::zero(), cst = Fq::zero(); };
-static void prod_counts(const sp_prod_leaves* leaves, int k, int ntables, const std::string& what) {
-  if (k < 1 || k > SP_PROD_MAX_CIRCUITS)
-    throw SpError(SP_ERR_INVALID_ARG, what + ": " + std::to_string(k) + " circuits; 1 .. SP_PROD_MAX_CIRCUITS = " + std::to_string(SP_PROD_MAX_CIRCUITS) + " supported");
-  if (ntables < 1) throw SpError(SP_ERR_INVALID_ARG, what + ": " + std::to_string(ntables) + " tables; at least one needed");
-  if (!leaves && k != ntables)
-    throw SpError(SP_ERR_INVALID_ARG, what + ": leaves NULL (circuit i = table i) needs k = ntables, got k = " + std::to_string(k) + ", ntables = " + std::to_string(ntables));
-}
-static std::vector<LeafForm> prod_forms(const sp_prod_leaves* leaves, int k, int ntables, const std::string& what) {
-  prod_counts(leaves, k, ntables, what);
-  std::vector<LeafForm> f(k);
-  for (int c = 0; c < k; c++) {
-    if (!leaves) { f[c].nsrc = 1; f[c].src[0] = (uint32_t)c; f[c].coeff[0] = Fq::one(); continue; }
-    const sp_prod_leaves& l = leaves[c];
-    const std::string at = what + ": circuit " + std::to_string(c);
-    if (l.nsources > SP_PROD_MAX_SOURCES)
-      throw SpError(SP_ERR_INVALID_ARG, at + " has " + std::to_string(l.nsources) + " sources; at most SP_PROD_MAX_SOURCES = " + std::to_string(SP_PROD_MAX_SOURCES));
-    for (uint32_t s = 0; s < l.nsources; s++)
-      if (l.source[s] >= (uint32_t)ntables)
-        throw SpError(SP_ERR_INVALID_ARG, at + ": source " + std::to_string(s) + " is table " + std::to_string(l.source[s]) + " >= ntables = " + std::to_string(ntables));
-  }
-  if (leaves)
-    for (int c = 0; c < k; c++) {
-      const sp_prod_leaves& l = leaves[c];
-      const std::string at = what + ": circuit " + std::to_string(c);
-      require_reduced(&l.coeff_mont[0][0], l.nsources, (at + ": coefficient").c_str());
-      require_reduced(l.index_coeff_mont, 1, (at + ": index coefficient").c_str());
-      require_reduced(l.const_mont, 1, (at + ": constant").c_str());
-      f[c].nsrc = l.nsources;
-      for (uint32_t s = 0; s < l.nsources; s++) { f[c].src[s] = l.source[s]; f[c].coeff[s] = fq_in(l.coeff_mont[s]); }
-      f[c].idx = fq_in(l.index_coeff_mont);
-      f[c].cst = fq_in(l.const_mont);
-    }
-  return f;
-}
-// the tables of a build: non-null handles of this context, of one power-of-two length >= 2; returns log2 of it
-static size_t prod_tables(sp_ctx* ctx, sp_poly* const* tables, int ntables, const std::string& what) {
-  if (!tables) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL table array");
-  for (int i = 0; i < ntables; i++) {
-    if (!tables[i]) throw SpError(SP_ERR_INVALID_ARG, what + ": table " + std::to_string(i) + " is NULL");
-    if (tables[i]->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, what + ": table " + std::to_string(i) + " belongs to another context");
-    if (tables[i]->len != tables[0]->len) throw SpError(SP_ERR_INVALID_ARG, what + ": tables differ in length");
-  }
-  const size_t len = tables[0]->len;
-  if (len < 2 || (len & (len - 1)) || log2_ceil(len) > PROD_MAX_VARS)
-    throw SpError(SP_ERR_INVALID_ARG, what + ": the table length must be a power of two >= 2 (a circuit needs a product layer), got " + std::to_string(len));
-  return log2_ceil(len);
-}
-extern "C" {
-
 int sp_prod_build(sp_ctx* ctx, sp_poly* const* tables, int ntables, const sp_prod_leaves* leaves, int k, sp_prod_circuits** out, uint64_t* products_out) {
-  SP_TRY(ctx)
-  const std::string what = "prod_build";
-  if (!out || !products_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
-  prod_counts(leaves, k, ntables, what);   // before any table is looked at
-  const size_t m = prod_tables(ctx, tables, ntables, what);
-  const std::vector<LeafForm> f = prod_forms(leaves, k, ntables, what);
-  const Fq one = Fq::one();
-  std::vector<dev::ProdLeaves> d(k);
-  for (int c = 0; c < k; c++) {
-    dev::ProdLeaves& p = d[c];
-    memset(static_cast<void*>(&p), 0, sizeof p);
-    p.nsrc = f[c].nsrc;
-    for (uint32_t s = 0; s < f[c].nsrc; s++) {
-      p.src[s] = tables[f[c].src[s]]->d.p;
-      p.coeff[s] = f[c].coeff[s].m;
-      if (f[c].coeff[s] == one) p.flags |= dev::PROD_UNIT0 << s;
+  return guarded(ctx, [&] {
+    const std::string what = "prod_build";
+    if (!out || !products_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    prod_counts(leaves, k, ntables, what);   // before any table is looked at
+    const size_t m = log2_ceil(caller_tables(ctx, tables, ntables, what, 2).len);
+    const std::vector<LeafForm> f = prod_forms(leaves, k, ntables, what);
+    const Fq one = Fq::one();
+    std::vector<dev::ProdLeaves> d(k);
+    for (int c = 0; c < k; c++) {
+      dev::ProdLeaves& p = d[c];
+      memset(static_cast<void*>(&p), 0, sizeof p);
+      p.nsrc = f[c].nsrc;
+      for (uint32_t s = 0; s < f[c].nsrc; s++) {
+        p.src[s] = tables[f[c].src[s]]->d.p;
+        p.coeff[s] = f[c].coeff[s].m;
+        if (f[c].coeff[s] == one) p.flags |= dev::PROD_UNIT0 << s;
+      }
+      p.idx = f[c].idx.m; p.cst = f[c].cst.m;
+      if (!f[c].idx.is_zero()) p.flags |= dev::PROD_IDX;
+      if (!f[c].cst.is_zero()) p.flags |= dev::PROD_CST;
     }
-    p.idx = f[c].idx.m; p.cst = f[c].cst.m;
-    if (!f[c].idx.is_zero()) p.flags |= dev::PROD_IDX;
-    if (!f[c].cst.is_zero()) p.flags |= dev::PROD_CST;
-  }
-  std::unique_ptr<sp_prod_circuits> h(new sp_prod_circuits{&ctx->c, m, {}, false});
-  const std::vector<Fq> products = prod_build(ctx->c, d, (size_t)1 << m, h->cs);
-  for (int c = 0; c < k; c++) fq_out(products_out + 4 * c, products[c]);
-  *out = h.release();
-  SP_CATCH(ctx)
+    std::unique_ptr<sp_prod_circuits> h(new sp_prod_circuits{&ctx->c, m, {}, false});
+    put_scalars(products_out, prod_build(ctx->c, d, (size_t)1 << m, h->cs));
+    *out = h.release();
+  });
 }
 
 int sp_prod_prove_t(sp_ctx* ctx, sp_prod_circuits* c, uint8_t* strobe_state, uint8_t** proof, size_t* proof_len, uint64_t* rand_out, uint64_t* leaf_evals_out) {
-  SP_TRY(ctx)
-  const std::string what = "prod_prove";
-  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-  ta.check();
-  if (!proof || !proof_len || !rand_out || !leaf_evals_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
-  if (!c) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL circuits handle");
-  if (c->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, what + ": the circuits belong to another context");
-  if (c->spent) throw SpError(SP_ERR_INVALID_ARG, what + ": the circuits were consumed by an earlier proof (their layers are bound in place)");
-  std::vector<ProdCircuit*> cs;
-  for (auto& p : c->cs) cs.push_back(p.get());
-  Transcript T = ta.open();
-  c->spent = true;
-  ProductCircuitEvalProofBatched P;
-  std::vector<Fq> rand, evals;
-  prod_prove(ctx->c, cs, T, P, rand, evals);
-  c->cs.clear();
-  ta.close(T);
-  const std::vector<uint8_t> bytes = to_bincode(P);
-  *proof = dup_bytes(bytes); *proof_len = bytes.size();
-  for (size_t j = 0; j < rand.size(); j++) fq_out(rand_out + 4 * j, rand[j]);
-  for (size_t i = 0; i < evals.size(); i++) fq_out(leaf_evals_out + 4 * i, evals[i]);
-  SP_CATCH(ctx)
+  return guarded(ctx, [&] {
+    const std::string what = "prod_prove";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if (!proof || !proof_len || !rand_out || !leaf_evals_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    require_owned(ctx, c, what, "circuits handle");
+    if (c->spent) throw SpError(SP_ERR_INVALID_ARG, what + ": the circuits were consumed by an earlier proof (their layers are bound in place)");
+    std::vector<ProdCircuit*> cs;
+    for (auto& p : c->cs) cs.push_back(p.get());
+    Transcript T = ta.open();
+    c->spent = true;
+    ProductCircuitEvalProofBatched P;
+    std::vector<Fq> rand, evals;
+    prod_prove(ctx->c, cs, T, P, rand, evals);
+    c->cs.clear();
+    ta.close(T);
+    put_bytes(proof, proof_len, to_bincode(P));
+    put_scalars(rand_out, rand);
+    put_scalars(leaf_evals_out, evals);
+  });
 }
 
 void sp_prod_free(sp_prod_circuits* c) { delete c; }
@@ -1434,29 +1464,25 @@ void sp_prod_free(sp_prod_circuits* c) { delete c; }
 // host only: no device work, so ctx may be NULL (the message then goes where sp_last_error(NULL) reads it)
 int sp_prod_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const uint64_t* products, int k, size_t m, uint8_t* strobe_state, uint64_t* rand_out,
                      uint64_t* leaf_claims_out) {
-  std::string& err = ctx ? ctx->c.last_error : g_create_error;
-  try {
+  return host_guarded(ctx, [&] {
     const std::string what = "prod_verify";
     const TranscriptArg ta = TranscriptArg::caller(strobe_state);
     ta.check();
     if ((!proof && proof_len) || !products || !rand_out || !leaf_claims_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
-    if (k < 1 || k > SP_PROD_MAX_CIRCUITS)
-      throw SpError(SP_ERR_INVALID_ARG, what + ": " + std::to_string(k) + " products; 1 .. SP_PROD_MAX_CIRCUITS = " + std::to_string(SP_PROD_MAX_CIRCUITS) + " supported");
+    require_count(what, k, "products", "SP_PROD_MAX_CIRCUITS", SP_PROD_MAX_CIRCUITS);
     if (m < 1 || m > PROD_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": m = " + std::to_string(m) + "; 1 .. " + std::to_string(PROD_MAX_VARS) + " supported");
     require_reduced(products, (size_t)k, "prod_verify: product");
     Transcript T = ta.open();
     TranscriptClose close{ta, T};
     const BatchedOut o = prod_verify(proof, proof_len, fq_vec(products, (size_t)k), m, T);
-    for (size_t j = 0; j < m; j++) fq_out(rand_out + 4 * j, o.rand[j]);
-    for (int i = 0; i < k; i++) fq_out(leaf_claims_out + 4 * i, o.claims[i]);
-    return SP_OK;
-  } catch (const SpError& e) { err = e.what(); return e.code; }
-  catch (const std::exception& e) { err = e.what(); return SP_ERR_INTERNAL; }
+    put_scalars(rand_out, o.rand);
+    put_scalars(leaf_claims_out, o.claims);
+  });
 }
 
 // host only
 int sp_prod_leaf_eval(const sp_prod_leaves* leaves, int k, const uint64_t* table_evals, int ntables, const uint64_t* rand, size_t m, uint64_t* out) {
-  try {
+  return host_guarded(nullptr, [&] {
     const std::string what = "prod_leaf_eval";
     if (!table_evals || !out || (!rand && m)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     if (m > PROD_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": m = " + std::to_string(m) + " > " + std::to_string(PROD_MAX_VARS));
@@ -1470,75 +1496,21 @@ int sp_prod_leaf_eval(const sp_prod_leaves* leaves, int k, const uint64_t* table
       for (uint32_t s = 0; s < f[c].nsrc; s++) v += f[c].coeff[s] * fq_in(table_evals + 4 * f[c].src[s]);
       fq_out(out + 4 * c, v);
     }
-    return SP_OK;
-  } catch (const SpError& e) { g_create_error = e.what(); return e.code; }
-  catch (const std::exception& e) { g_create_error = e.what(); return SP_ERR_INTERNAL; }
+  });
 }
 
-// ---- batch verifiers: proof i is checked as the single call would check it (statement i, inputs i, label i or caller transcript i); the group
-// equations of all of them are tested in one device pass (verifier.cpp, DESIGN.md "deferred checks")
-struct BatchArgs {
-  size_t k;
-  const uint64_t* const* inputs; const size_t* ninputs;
-  const uint8_t* const* labels; const size_t* label_lens;   // fresh transcripts, or
-  uint8_t* const* states;                                    // the callers' transcripts (the _t forms)
-  const uint8_t* const* proofs; const size_t* proof_lens;
-  const uint8_t* seed; int* status;
-};
-static std::vector<VerifyJob> batch_jobs(const BatchArgs& a, const void* const* stmts) {
-  const bool bad_transcripts = a.states ? false : (!a.labels || !a.label_lens);
-  if (!stmts || !a.inputs || !a.ninputs || !a.proofs || !a.proof_lens || !a.status || bad_transcripts)
-    throw SpError(SP_ERR_INVALID_ARG, "verify_batch: NULL array");
-  std::vector<VerifyJob> jobs;
-  jobs.reserve(a.k);
-  for (size_t i = 0; i < a.k; i++) {
-    const std::string at = "verify_batch: proof " + std::to_string(i) + ": ";
-    if (!stmts[i]) throw SpError(SP_ERR_INVALID_ARG, at + "NULL statement handle");
-    if (!a.proofs[i] && a.proof_lens[i]) throw SpError(SP_ERR_INVALID_ARG, at + "NULL proof");
-    if (!a.inputs[i] && a.ninputs[i]) throw SpError(SP_ERR_INVALID_ARG, at + "NULL inputs");
-    require_reduced(a.inputs[i], a.ninputs[i], "inputs");
-    if (a.states && !a.states[i]) throw SpError(SP_ERR_INVALID_ARG, at + "transcript state is NULL");
-    Transcript T = a.states ? Transcript(Transcript::FromState(), a.states[i]) : Transcript(std::string((const char*)a.labels[i], a.label_lens[i]));
-    jobs.push_back(VerifyJob{nullptr, nullptr, fq_vec(a.inputs[i], a.ninputs[i]), T, a.proofs[i], a.proof_lens[i]});
-  }
-  return jobs;
-}
-// statuses, transcripts and the first rejection's message out; SP_ERR_VERIFY when any proof is rejected
-static int batch_finish(sp_ctx* ctx, const BatchArgs& a, const std::vector<VerifyJob>& jobs) {
-  int rc = SP_OK;
-  for (size_t i = 0; i < a.k; i++) {
-    a.status[i] = jobs[i].status;
-    if (a.states) jobs[i].T.export_state(a.states[i]);
-    if (jobs[i].status != SP_OK && rc == SP_OK) { rc = SP_ERR_VERIFY; ctx->c.last_error = "proof " + std::to_string(i) + ": " + jobs[i].msg; }
-  }
-  flush_fine(ctx->c);
-  return rc;
-}
+// ---- batch verifiers
 static int nizk_verify_batch_common(sp_ctx* ctx, const sp_instance* const* insts, const sp_nizk_gens* gens, const BatchArgs& a) {
-  int rc = SP_OK;
-  SP_TRY(ctx)
-  if (!a.seed) throw SpError(SP_ERR_INVALID_ARG, "verify_batch: weight seed is NULL: draw 32 bytes from the OS RNG on every call");
-  if (!a.k) return SP_OK;
-  if (!gens) throw SpError(SP_ERR_INVALID_ARG, "verify_batch: NULL gens");
-  std::vector<VerifyJob> jobs = batch_jobs(a, reinterpret_cast<const void* const*>(insts));
-  for (size_t i = 0; i < a.k; i++) jobs[i].inst = &insts[i]->inst;
-  nizk_verify_batch(ctx->c, *gens->g, jobs, a.seed);
-  rc = batch_finish(ctx, a, jobs);
-  if (rc != SP_OK) return rc;
-  SP_CATCH(ctx)
+  return verify_batch(ctx, reinterpret_cast<const void* const*>(insts), gens, a, [&](std::vector<VerifyJob>& jobs) {
+    for (size_t i = 0; i < a.k; i++) jobs[i].inst = &insts[i]->inst;
+    nizk_verify_batch(ctx->c, *gens->g, jobs, a.seed);
+  });
 }
 static int snark_verify_batch_common(sp_ctx* ctx, const sp_snark_encoding* const* comms, const sp_snark_gens* gens, const BatchArgs& a) {
-  int rc = SP_OK;
-  SP_TRY(ctx)
-  if (!a.seed) throw SpError(SP_ERR_INVALID_ARG, "verify_batch: weight seed is NULL: draw 32 bytes from the OS RNG on every call");
-  if (!a.k) return SP_OK;
-  if (!gens) throw SpError(SP_ERR_INVALID_ARG, "verify_batch: NULL gens");
-  std::vector<VerifyJob> jobs = batch_jobs(a, reinterpret_cast<const void* const*>(comms));
-  for (size_t i = 0; i < a.k; i++) jobs[i].enc = comms[i]->e.get();
-  snark_verify_batch(ctx->c, *gens->g, jobs, a.seed);
-  rc = batch_finish(ctx, a, jobs);
-  if (rc != SP_OK) return rc;
-  SP_CATCH(ctx)
+  return verify_batch(ctx, reinterpret_cast<const void* const*>(comms), gens, a, [&](std::vector<VerifyJob>& jobs) {
+    for (size_t i = 0; i < a.k; i++) jobs[i].enc = comms[i]->e.get();
+    snark_verify_batch(ctx->c, *gens->g, jobs, a.seed);
+  });
 }
 int sp_nizk_verify_batch(sp_ctx* ctx, size_t k, const sp_instance* const* insts, const uint64_t* const* inputs_mont, const size_t* ninputs,
                          const sp_nizk_gens* gens, const uint8_t* const* labels, const size_t* label_lens, const uint8_t* const* proofs,
@@ -1553,37 +1525,31 @@ int sp_snark_verify_batch(sp_ctx* ctx, size_t k, const sp_snark_encoding* const*
 int sp_nizk_verify_batch_t(sp_ctx* ctx, size_t k, const sp_instance* const* insts, const uint64_t* const* inputs_mont, const size_t* ninputs,
                            const sp_nizk_gens* gens, uint8_t* const* strobe_states, const uint8_t* const* proofs, const size_t* proof_lens,
                            const uint8_t weight_seed[32], int* status) {
-  if (!strobe_states && k) { if (ctx) ctx->c.last_error = "verify_batch: NULL array"; return SP_ERR_INVALID_ARG; }
   return nizk_verify_batch_common(ctx, insts, gens, {k, inputs_mont, ninputs, nullptr, nullptr, strobe_states, proofs, proof_lens, weight_seed, status});
 }
 int sp_snark_verify_batch_t(sp_ctx* ctx, size_t k, const sp_snark_encoding* const* comms, const uint64_t* const* inputs_mont, const size_t* ninputs,
                             const sp_snark_gens* gens, uint8_t* const* strobe_states, const uint8_t* const* proofs, const size_t* proof_lens,
                             const uint8_t weight_seed[32], int* status) {
-  if (!strobe_states && k) { if (ctx) ctx->c.last_error = "verify_batch: NULL array"; return SP_ERR_INVALID_ARG; }
   return snark_verify_batch_common(ctx, comms, gens, {k, inputs_mont, ninputs, nullptr, nullptr, strobe_states, proofs, proof_lens, weight_seed, status});
 }
 
 // merlin::Transcript for hosts without merlin (tests, C callers): the state buffer is the whole object
 int sp_transcript_new(const uint8_t* label, size_t label_len, uint8_t* strobe_state) {
-  Transcript T(std::string((const char*)label, label_len));
-  T.export_state(strobe_state);
-  return SP_OK;
+  return host_guarded(nullptr, [&] { Transcript(std::string((const char*)label, label_len)).export_state(strobe_state); });
 }
 int sp_transcript_append_message(uint8_t* strobe_state, const uint8_t* label, size_t label_len, const uint8_t* msg, size_t msg_len) {
-  try {
+  return host_guarded(nullptr, [&] {
     Transcript T(Transcript::FromState(), strobe_state);
     T.append_message(std::string((const char*)label, label_len).c_str(), msg, msg_len);
     T.export_state(strobe_state);
-    return SP_OK;
-  } catch (...) { return SP_ERR_INVALID_ARG; }
+  });
 }
 int sp_transcript_challenge_bytes(uint8_t* strobe_state, const uint8_t* label, size_t label_len, uint8_t* out, size_t n) {
-  try {
+  return host_guarded(nullptr, [&] {
     Transcript T(Transcript::FromState(), strobe_state);
     T.challenge_bytes(std::string((const char*)label, label_len).c_str(), out, n);
     T.export_state(strobe_state);
-    return SP_OK;
-  } catch (...) { return SP_ERR_INVALID_ARG; }
+  });
 }
 
 void sp_free(void* p) { free(p); }

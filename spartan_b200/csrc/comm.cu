@@ -13,10 +13,6 @@
 namespace sp {
 namespace dev {
 
-static void ck(cudaError_t e, const char* what) {
-  if (e != cudaSuccess) throw std::runtime_error(std::string("spartan_b200 CUDA error in ") + what + ": " + cudaGetErrorString(e));
-}
-
 // ---- windows
 void* win_alloc(size_t bytes) {   // plain cudaMalloc (IPC-exportable), zero-filled
   void* p = nullptr;

@@ -4,6 +4,7 @@
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
+#include <stdexcept>
 #include <string>
 #include <type_traits>
 #include "field.cuh"
@@ -17,7 +18,13 @@ namespace sp {
 namespace dev {
 
 // ---- runtime plumbing
-void check(const char* what);  // throws std::runtime_error on a pending CUDA error
+struct CudaError : std::runtime_error {  // a failed CUDA call; the C ABI returns SP_ERR_CUDA for it
+  using std::runtime_error::runtime_error;
+};
+void check(const char* what);  // throws CudaError on a pending CUDA error
+#ifdef __CUDACC__
+void ck(cudaError_t e, const char* what);  // throws CudaError unless e is cudaSuccess
+#endif
 int device_count();
 void set_device(int dev);
 cudaStream_t stream_create_prio(int level);   // > 0: greatest priority of the device, < 0: least

@@ -14,11 +14,6 @@ namespace sp {
 
 void shake256(uint8_t* out, size_t outlen, const uint8_t* in, size_t inlen);
 
-struct SpError : std::runtime_error {  // carries a C-ABI status code (include/spartan_b200.h)
-  int code;
-  SpError(int c, const std::string& m) : std::runtime_error(m), code(c) {}
-};
-
 template <class T>
 struct DevBuf {  // owning device allocation
   T* p = nullptr;

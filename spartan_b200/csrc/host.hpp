@@ -13,8 +13,14 @@
 #include "curve.cuh"
 #include "field.cuh"
 #include "host_fe51.hpp"
+#include "../../include/spartan_b200.h"
 
 namespace sp {
+
+struct SpError : std::runtime_error {  // carries a C-ABI status code (include/spartan_b200.h)
+  int code;
+  SpError(int c, const std::string& m) : std::runtime_error(m), code(c) {}
+};
 
 inline size_t log2_ceil(size_t x) { size_t l = 0; while (((size_t)1 << l) < x) l++; return l; }   // 0 for x <= 1
 inline size_t next_pow2(size_t x) { return (size_t)1 << log2_ceil(x); }
@@ -156,7 +162,7 @@ class Transcript {  // merlin::Transcript + ProofTranscript (transcript.rs:5-37)
   Transcript(FromState, const uint8_t* in) {
     memcpy(st_, in, 200);
     pos_ = in[200]; pos_begin_ = in[201]; cur_flags_ = in[202];
-    if (pos_ >= R || pos_begin_ > R) throw std::runtime_error("spartan_b200: not a STROBE-128 transcript state (position out of range)");
+    if (pos_ >= R || pos_begin_ > R) throw SpError(SP_ERR_INVALID_ARG, "spartan_b200: not a STROBE-128 transcript state (position out of range)");
   }
   void export_state(uint8_t* out) const { memcpy(out, st_, 200); out[200] = pos_; out[201] = pos_begin_; out[202] = cur_flags_; }
   void append_message(const char* label, const uint8_t* msg, size_t len) {

@@ -66,13 +66,10 @@ std::string prof_report() {
   return out;
 }
 
-void check(const char* what) {
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("spartan_b200 CUDA error in ") + what + ": " + cudaGetErrorString(e));
+void ck(cudaError_t e, const char* what) {
+  if (e != cudaSuccess) throw CudaError(std::string("spartan_b200 CUDA error in ") + what + ": " + cudaGetErrorString(e));
 }
-static void ck(cudaError_t e, const char* what) {
-  if (e != cudaSuccess) throw std::runtime_error(std::string("spartan_b200 CUDA error in ") + what + ": " + cudaGetErrorString(e));
-}
+void check(const char* what) { ck(cudaGetLastError(), what); }
 int device_count() { int n = 0; if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; } return n; }
 void set_device(int d) { ck(cudaSetDevice(d), "cudaSetDevice"); }
 // level > 0: the device's greatest priority (the transcript-serialised stream of small kernels), level < 0: its least (background MSMs)

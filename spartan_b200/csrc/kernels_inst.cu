@@ -13,9 +13,6 @@
 namespace sp {
 namespace dev {
 
-static void ck(cudaError_t e, const char* what) {
-  if (e != cudaSuccess) throw std::runtime_error(std::string("spartan_b200 CUDA error in ") + what + ": " + cudaGetErrorString(e));
-}
 static int key_bits(size_t nkeys) {   // radix bits that cover the keys 0 .. nkeys-1 (at least one: CUB wants a non-empty bit range)
   int b = 1;
   while (b < 32 && ((size_t)1 << b) < nkeys) b++;
