@@ -12,7 +12,10 @@
 // and pinned buffers on return and returns 0, a CUDA status, or SPD_REFUSED when a wrapper threw (spd_last_error() then holds its message).
 #include <cuda_runtime.h>
 #include <string.h>
+#include <algorithm>
+#include <chrono>
 #include <exception>
+#include <memory>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -227,6 +230,102 @@ __global__ void k_window_digits(size_t n, const u256* k, int* out) {
     const uint32_t v = msm_window<WBITS>(x, w0) + carry;
     out[i * NWIN + w0] = v > HALF ? (int)v - (int)(2 * HALF) : (int)v;
   }
+}
+
+// ---- generator-table checker.  An affine-niels table of nslots generators, entry (j, w, d) at (j nwin + w) depth + d - 1, must hold
+// d 2^(W w) G_{base(j)}: per-window tables (W = 8, 13, 15: nwin = ceil(253 / W), depth = 2^(W-1)), row tables (nwin = 1, depth = 2^15), host copies
+// (the 8-bit layout over a list of bases).  One thread per run of CHECK_RUN entries of one window computes B = 2^(W w) G by W w doublings and
+// d0 B by double-and-add from G itself, never from the table, then walks the run with one mixed addition per entry and compares each stored entry
+// with the extended point by cross-multiplication (ypx Z = Y + X, ymx Z = Y - X, t2d Z = 2d T mod p, both sides canonical) and requires every
+// stored coordinate to be canonical (< p), as ge_to_niels leaves it.  A wrong entry is therefore reported at its own index and nowhere else.
+constexpr size_t CHECK_RUN = 256;
+constexpr unsigned CHECK_LIST = 1u << 16;   // bad indices kept for the report; past this the list is no longer the first ones in index order
+enum { CK_SEEN, CK_BAD, CK_YPX, CK_YMX, CK_T2D, CK_NONCANON, CK_LISTED, CK_COUNTERS };
+__global__ void __launch_bounds__(64) k_niels_check(const ge_niels* __restrict__ table, size_t nslots, int wbits, int nwin, size_t depth, const ge* __restrict__ G,
+                                                    const int64_t* __restrict__ bases, unsigned long long* counters, unsigned long long* list) {
+  const size_t runs = (depth + CHECK_RUN - 1) / CHECK_RUN;
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nslots * (size_t)nwin * runs) return;
+  const size_t j = t / ((size_t)nwin * runs), r = t % runs;
+  const int w = (int)((t / runs) % nwin);
+  const ge* g = G + (bases ? (size_t)bases[j] : j);
+  ge B;
+  B.X = ld256_ro(&g->X); B.Y = ld256_ro(&g->Y); B.Z = ld256_ro(&g->Z); B.T = ld256_ro(&g->T);
+  for (int k = 0; k < wbits * w; k++) B = ge_dbl(B);
+  const ge_niels Bn = ge_to_niels(B);
+  const size_t d0 = r * CHECK_RUN + 1, d1 = d0 + CHECK_RUN - 1 < depth ? d0 + CHECK_RUN - 1 : depth;
+  u256 k0 = fq_zero();
+  k0.v[0] = (uint32_t)d0;
+  ge acc = ge_scalarmul(k0, B);
+  const ge_niels* e = table + ((size_t)j * nwin + w) * depth;
+  atomicAdd(&counters[CK_SEEN], (unsigned long long)(d1 - d0 + 1));
+  for (size_t d = d0; d <= d1; d++) {
+    if (d > d0) acc = ge_madd(acc, Bn, false);
+    const u256 ypx = ld256_ro(&e[d - 1].ypx), ymx = ld256_ro(&e[d - 1].ymx), t2d = ld256_ro(&e[d - 1].t2d);
+    const bool b_ypx = !fp_eq(fp_mul(ypx, acc.Z), fp_add(acc.Y, acc.X));
+    const bool b_ymx = !fp_eq(fp_mul(ymx, acc.Z), fp_sub(acc.Y, acc.X));
+    const bool b_t2d = !fp_eq(fp_mul(t2d, acc.Z), fp_mul(acc.T, fp_2D()));
+    const bool b_canon = !fq_eq(fp_canon(ypx), ypx) || !fq_eq(fp_canon(ymx), ymx) || !fq_eq(fp_canon(t2d), t2d);
+    if (!(b_ypx || b_ymx || b_t2d || b_canon)) continue;
+    atomicAdd(&counters[CK_BAD], 1ull);
+    if (b_ypx) atomicAdd(&counters[CK_YPX], 1ull);
+    if (b_ymx) atomicAdd(&counters[CK_YMX], 1ull);
+    if (b_t2d) atomicAdd(&counters[CK_T2D], 1ull);
+    if (b_canon) atomicAdd(&counters[CK_NONCANON], 1ull);
+    const unsigned long long slot = atomicAdd(&counters[CK_LISTED], 1ull);
+    if (slot < CHECK_LIST) list[slot] = ((size_t)j * nwin + w) * depth + d - 1;
+  }
+}
+
+// one check on c's stream.  out (24 words): entries the kernel compared, bad entries, ypx / ymx / t2d mismatches, entries with a non-canonical coordinate, the
+// number of indices listed (<= 16), 1 when they are exactly the first bad entries in index order, then the listed entry indices, ascending
+constexpr int CHECK_OUT = 24;
+void niels_check(KCall& c, const ge_niels* table, size_t nslots, int wbits, const ge* G, const int64_t* d_bases, uint64_t* out) {
+  memset(out, 0, CHECK_OUT * sizeof(uint64_t));
+  const int nwin = wbits ? (253 + wbits - 1) / wbits : 1;
+  const size_t depth = (size_t)1 << (wbits ? wbits - 1 : 15);
+  unsigned long long* counters = c.zeros<unsigned long long>(CK_COUNTERS);
+  unsigned long long* list = c.alloc<unsigned long long>(CHECK_LIST);
+  const size_t threads = nslots * (size_t)nwin * ((depth + CHECK_RUN - 1) / CHECK_RUN);
+  if (c.ok() && threads) k_niels_check<<<(unsigned)((threads + 63) / 64), 64, 0, c.s>>>(table, nslots, wbits, nwin, depth, G, d_bases, counters, list);
+  c.launched();
+  c.sync();
+  unsigned long long h[CK_COUNTERS];
+  c.out(h, counters, CK_COUNTERS);
+  if (!c.ok()) return;
+  const size_t kept = h[CK_LISTED] < CHECK_LIST ? h[CK_LISTED] : CHECK_LIST;
+  std::vector<unsigned long long> idx(kept);
+  c.out(idx.data(), list, kept);
+  std::sort(idx.begin(), idx.end());
+  for (int k = 0; k < 6; k++) out[k] = h[CK_SEEN + k];
+  out[6] = kept < 16 ? kept : 16;
+  out[7] = h[CK_LISTED] <= CHECK_LIST ? 1 : 0;
+  for (size_t k = 0; k < out[6]; k++) out[8 + k] = idx[k];
+}
+// radix-2^51 host limbs -> the 256-bit value they stand for; limbs past 51 bits (never written by to_hniels) give all ones, which no canonical
+// coordinate equals
+u256 fe51_value(const fe51& a) {
+  u256 r;
+  for (int i = 0; i < 5; i++)
+    if (a.v[i] >> 51) { for (int k = 0; k < 8; k++) r.v[k] = 0xffffffffu; return r; }
+  const uint64_t w[4] = {a.v[0] | (a.v[1] << 51), (a.v[1] >> 13) | (a.v[2] << 38), (a.v[2] >> 26) | (a.v[3] << 25), (a.v[3] >> 39) | (a.v[4] << 12)};
+  for (int k = 0; k < 4; k++) { r.v[2 * k] = (uint32_t)w[k]; r.v[2 * k + 1] = (uint32_t)(w[k] >> 32); }
+  return r;
+}
+struct ReleaseCached { ~ReleaseCached() { pool_release_cached(); } };   // a set's freed tables go back to the device, not to this library's pool
+// a generator set built as the library builds one: by label, or (enc non-null) from nbases encodings decoded on the device as sp_gens_upload does
+std::unique_ptr<GenSet> make_set(Ctx& ctx, const uint8_t* label, size_t label_len, size_t nbases, const uint8_t* enc, const std::vector<size_t>& hb) {
+  if (!enc) return std::unique_ptr<GenSet>(new GenSet(&ctx, std::string((const char*)label, label_len), nbases, hb));
+  DevBuf<uint8_t> d_in(32 * nbases);
+  DevBuf<ge> pts(nbases);
+  DevBuf<int> d_ok(nbases);
+  std::vector<int> ok(nbases);
+  h2d(d_in.p, enc, 32 * nbases, ctx.stream);
+  decompress_batch(pts.p, d_ok.p, d_in.p, nbases, ctx.stream);
+  d2h(ok.data(), d_ok.p, sizeof(int) * nbases, ctx.stream);
+  ctx.sync();
+  for (size_t i = 0; i < nbases; i++) if (!ok[i]) throw std::runtime_error("encoding " + std::to_string(i) + " is not a ristretto255 point");
+  return std::unique_ptr<GenSet>(new GenSet(&ctx, pts.p, nbases, hb));
 }
 
 }  // namespace
@@ -785,6 +884,105 @@ int spd_deferred_check(size_t nproofs, const uint32_t* eq_start, const uint32_t*
       }
     const std::vector<bool> r = deferred_check(ctx, gs, proofs, seed32);
     for (size_t i = 0; i < nproofs; i++) ok[i] = r[i] ? 1 : 0;
+    return 0;
+  });
+}
+
+// ---- generator tables
+// Checks the affine-niels table in device memory d_table (k_niels_check): nslots generators in the per-window layout of wbits = 8, 13 or 15, or in
+// the row layout (wbits = 0); slot j holds the multiples of d_G[bases[j]] (bases: nslots host entries, or null for slot j = generator j).  out: the
+// 24-word report of niels_check.  d_table and d_G are only read.
+int spd_niels_table_check(const void* d_table, size_t nslots, int wbits, const void* d_G, const int64_t* bases, uint64_t* out) {
+  if ((wbits != 0 && wbits != 8 && wbits != 13 && wbits != 15) || nslots < 1) return (int)cudaErrorInvalidValue;
+  return guarded([&] {
+    KCall c;
+    const int64_t* db = bases ? c.in(bases, nslots) : nullptr;
+    niels_check(c, (const ge_niels*)d_table, nslots, wbits, (const ge*)d_G, db, out);
+    return (int)c.err;
+  });
+}
+
+// Builds one generator set through GenSet's production constructors (nbases generators of the SHAKE256 stream of `label`, or with enc non-null the
+// nbases caller encodings) with the host copies of host_bases, adds those of extra_bases afterwards as a view does, and checks every entry the set
+// holds: the per-window table at the width the set chose, the row table when it built one, and the host copies of every requested base below
+// nbases (radix 2^51, taken back to 256-bit values) in the 8-bit layout against their generators.  out: three 24-word reports (niels_check) for the
+// per-window table, the row table (all zero without one) and the host copies, whose slot j is base host_checked[j] (n_host + n_extra entries of
+// room).  info: the window width, 1 when a row table was built, the free and total device bytes just before the build, the set's device bytes and
+// the number of host copies checked.  G_enc: the nbases generators' encodings (k_compress).  ms: build and check wall times.  The set is freed and
+// this library's cached blocks released before the call returns.
+int spd_gen_set_check(const uint8_t* label, size_t label_len, size_t nbases, const uint8_t* enc, const int64_t* host_bases, size_t n_host,
+                      const int64_t* extra_bases, size_t n_extra, uint8_t* G_enc, int64_t* info, int64_t* host_checked, uint64_t* out, double* ms) {
+  if (nbases < 1) return (int)cudaErrorInvalidValue;
+  return guarded([&] {
+    ReleaseCached rel;
+    pool_release_cached();
+    Ctx ctx(0);
+    const std::vector<size_t> hb(host_bases, host_bases + n_host), xb(extra_bases, extra_bases + n_extra);
+    size_t free0 = 0, total0 = 0;
+    mem_info(&free0, &total0);
+    const auto t0 = std::chrono::steady_clock::now();
+    std::unique_ptr<GenSet> gs = make_set(ctx, label, label_len, nbases, enc, hb);
+    gs->add_host_tables(xb);
+    ctx.sync();
+    const auto t1 = std::chrono::steady_clock::now();
+    std::vector<size_t> want;
+    for (const std::vector<size_t>* v : {&hb, &xb})
+      for (size_t b : *v)
+        if (b < nbases && std::find(want.begin(), want.end(), b) == want.end()) want.push_back(b);
+    for (size_t b : want) if (!gs->has_tab(b)) throw std::runtime_error("the set holds no host copy of base " + std::to_string(b));
+    {
+      KCall c;
+      niels_check(c, gs->table.p, nbases, gs->wbits, gs->G.p, nullptr, out);
+      if (gs->rows()) niels_check(c, gs->rows(), nbases, 0, gs->G.p, nullptr, out + CHECK_OUT);
+      else memset(out + CHECK_OUT, 0, CHECK_OUT * sizeof(uint64_t));
+      memset(out + 2 * CHECK_OUT, 0, CHECK_OUT * sizeof(uint64_t));
+      if (!want.empty()) {
+        const size_t per = 32 * 128;
+        std::vector<ge_niels> h(want.size() * per);
+        for (size_t i = 0; i < want.size(); i++) {
+          const HostBaseTable& tb = gs->tab(want[i]);
+          if (tb.e.size() != per) throw std::runtime_error("host copy of base " + std::to_string(want[i]) + " has " + std::to_string(tb.e.size()) + " entries");
+          for (size_t e = 0; e < per; e++) h[i * per + e] = ge_niels{fe51_value(tb.e[e].ypx), fe51_value(tb.e[e].ymx), fe51_value(tb.e[e].t2d)};
+        }
+        const std::vector<int64_t> wb(want.begin(), want.end());
+        const ge_niels* dh = c.in(h.data(), h.size());
+        const int64_t* dwb = c.in(wb.data(), wb.size());
+        niels_check(c, dh, want.size(), 8, gs->G.p, dwb, out + 2 * CHECK_OUT);
+      }
+      if (!c.ok()) return (int)c.err;
+    }
+    const auto t2 = std::chrono::steady_clock::now();
+    DevBuf<uint8_t> comp(32 * nbases);
+    compress_batch(comp.p, gs->G.p, nbases, ctx.stream);
+    d2h(G_enc, comp.p, 32 * nbases, ctx.stream);
+    ctx.sync();
+    const int64_t v[6] = {gs->wbits, gs->rows() ? 1 : 0, (int64_t)free0, (int64_t)total0, (int64_t)gs->device_bytes(), (int64_t)want.size()};
+    memcpy(info, v, sizeof v);
+    for (size_t i = 0; i < want.size(); i++) host_checked[i] = (int64_t)want[i];
+    ms[0] = std::chrono::duration<double, std::milli>(t1 - t0).count();
+    ms[1] = std::chrono::duration<double, std::milli>(t2 - t1).count();
+    return 0;
+  });
+}
+
+// Builds the set of spd_gen_set_check by label (no host copies) and copies its per-window table (row = 0) or its row table (row = 1) into the
+// caller's device buffer d_table (room for cap entries of 96 bytes), and its nbases generators into d_G (128 bytes each), so that a check can run
+// on a copy the caller alters; the set's own tables are only read.  info: the window width and the entries copied.  SPD_REFUSED when the set has
+// no row table or the table needs more than cap entries.
+int spd_gen_table_copy(const uint8_t* label, size_t label_len, size_t nbases, int row, void* d_table, size_t cap, void* d_G, int64_t* info) {
+  if (nbases < 1) return (int)cudaErrorInvalidValue;
+  return guarded([&] {
+    ReleaseCached rel;
+    Ctx ctx(0);
+    std::unique_ptr<GenSet> gs = make_set(ctx, label, label_len, nbases, nullptr, {});
+    const DevBuf<ge_niels>& t = row ? gs->row_table : gs->table;
+    if (!t.n) throw std::runtime_error("the set has no row table");
+    if (t.n > cap) throw std::runtime_error("the table has " + std::to_string(t.n) + " entries, the buffer room for " + std::to_string(cap));
+    d2d(d_table, t.p, t.n * sizeof(ge_niels), ctx.stream);
+    d2d(d_G, gs->G.p, nbases * sizeof(ge), ctx.stream);
+    ctx.sync();
+    info[0] = gs->wbits;
+    info[1] = (int64_t)t.n;
     return 0;
   });
 }
