@@ -316,6 +316,63 @@ int sp_prod_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const 
 int sp_prod_leaf_eval(const sp_prod_leaves* leaves, int k, const uint64_t* table_evals_mont, int ntables, const uint64_t* rand_mont, size_t m,
                       uint64_t* out /* k x 4 */);
 
+/* ---- SPARK: commitments to the caller's sparse matrices and proofs of their evaluations (SparseMatPolyCommitmentGens, SparseMatPolynomial::
+ * multi_commit / multi_evaluate, SparseMatPolyEvalProof::{prove, verify}, src/sparse_mlpoly.rs), for b = 1 .. SP_SPARK_MAX_BATCH matrices of
+ * 2^num_vars_x rows and 2^num_vars_y columns each (x != y allowed; the memory has 2^max(x, y) cells).  SNARK::encode / prove / verify run
+ * through the same code with the three R1CS matrices.  Every entry runs on this rank's GPU alone, also on a connected multi-GPU context.
+ *
+ * b = 3: commitment and proof bytes are the reference's.  Other b: the reference's ProductLayerProof::prove asserts b = 3 (sparse_mlpoly.rs:
+ * 1121-1122, a TODO); its verifier is general in b.  The proof is the generalisation the TODO implies: the ops product proof batches the circuits
+ * row.read[0..b), row.write[0..b), col.read[0..b), col.write[0..b) with the dot-product circuits left_0, right_0, left_1, right_1, .. (the order
+ * the verifier's claims_dotp_circuit assumes, :1264-1270), and the reference's verify accepts it.  b <= 4 because those 6b circuits go in one
+ * batched sumcheck launch per round (24 instances). */
+#define SP_SPARK_MAX_BATCH 4
+typedef struct sp_spark_gens sp_spark_gens;
+typedef struct sp_spark_dense sp_spark_dense;   /* MultiSparseMatPolynomialAsDense on the device (sparse_mlpoly.rs:274-282) */
+/* SparseMatPolyCommitmentGens::new(label, num_vars_x, num_vars_y, num_nz_entries, batch_size) (sparse_mlpoly.rs:292-317): gens_ops, gens_mem and
+ * gens_derefs as views of one set of the label's SHAKE stream, of num_vars_ops = log2 next_pow2(nz) + log2 next_pow2(5b), num_vars_mem =
+ * max(x, y) + 1, num_vars_derefs = log2 next_pow2(nz) + log2 next_pow2(2b).  Device footprint as sp_pc_gens_create's for the largest of the three
+ * n = 2^(v - v/2): nz = 2^20 with b = 4 gives n_ops = 8192, whose full-width tables do not fit beside a prover, so the set falls back to narrower
+ * windows (same bytes, speed not measured).  SP_ERR_INVALID_ARG: batch_size outside 1 .. SP_SPARK_MAX_BATCH, max(x, y) = 0 or > 30. */
+int sp_spark_gens_create(sp_ctx* ctx, const uint8_t* label, size_t label_len, size_t num_vars_x, size_t num_vars_y, size_t num_nz_entries, size_t batch_size,
+                         sp_spark_gens** out);
+void sp_spark_gens_free(sp_spark_gens* g);
+/* one matrix's entries: nnz (row, col, canonical 32-byte value) */
+typedef struct { const uint64_t* row; const uint64_t* col; const uint8_t* val32; size_t nnz; } sp_spark_entries;
+/* SparseMatPolynomial::multi_commit(polys, gens) (sparse_mlpoly.rs:483-503) of b matrices.  *dense: the decommitment, on the device (free with
+ * sp_spark_dense_free): comb_ops (next_pow2(5b) N scalars), comb_mem (2 * 2^max(x, y)) and 2b N address indices, N = max_i next_pow2(nnz_i);
+ * 32 bytes per scalar, so nz = 2^20, b = 3 holds 512 MiB of comb_ops.  *comm = bincode(SparseMatPolyCommitment) (free with sp_free).
+ * SP_ERR_INVALID_INDEX: a row >= 2^x ("row") or col >= 2^y ("col"); SP_ERR_INVALID_SCALAR: a value >= q; the first bad entry in (matrix, entry,
+ * row/col/scalar) order is reported.  SP_ERR_INVALID_ARG, before anything is allocated: b outside 1 .. SP_SPARK_MAX_BATCH, N < 2 (every matrix
+ * has at most one entry: the product circuits would have no layer), max(x, y) = 0 or > 30 (32-bit addresses), gens of other sizes (their three
+ * views' n against those of (x, y, N, b)), a handle of another context, NULL arrays with nnz > 0. */
+int sp_spark_commit(sp_ctx* ctx, const sp_spark_gens* gens, const sp_spark_entries* matrices, int b, size_t num_vars_x, size_t num_vars_y,
+                    sp_spark_dense** dense, uint8_t** comm, size_t* comm_len);
+/* the same with every array in DEVICE memory of the context's GPU: the synchronisation rules and pointer checks of sp_instance_create_device */
+int sp_spark_commit_device(sp_ctx* ctx, const sp_spark_gens* gens, const sp_spark_entries* matrices, int b, size_t num_vars_x, size_t num_vars_y,
+                           sp_spark_dense** dense, uint8_t** comm, size_t* comm_len);
+void sp_spark_dense_free(sp_spark_dense* d);
+/* SparseMatPolynomial::multi_evaluate (sparse_mlpoly.rs:440-452) on the device: out[i] = M_i(rx, ry), |rx| = x, |ry| = y */
+int sp_spark_evaluate(sp_ctx* ctx, const sp_spark_dense* dense, const uint64_t* rx_mont, size_t x, const uint64_t* ry_mont, size_t y,
+                      uint64_t* out /* b x 4 */);
+/* SparseMatPolyEvalProof::prove(dense, rx, ry, evals, gens, transcript, tape) (sparse_mlpoly.rs:1447-1514) on the caller's transcript and tape
+ * (both advanced).  Like the reference's, the proof absorbs neither the commitment nor the evaluations: the caller absorbs them first, as
+ * SNARK::prove absorbs Ar/Br/Cr_claim.  evals NULL: computed on the device; given evals that differ from M_i(rx, ry) are refused.  Out: *proof =
+ * bincode(SparseMatPolyEvalProof) (free with sp_free), evals_out = the b evaluations.  SP_ERR_INVALID_ARG: |rx| != x or |ry| != y of the dense,
+ * gens that do not fit it, a wrong evaluation, a handle of another context; SP_ERR_INVALID_SCALAR: rx, ry or evals not reduced.  A refused call
+ * leaves the transcript and the tape untouched. */
+int sp_spark_eval_prove_t(sp_ctx* ctx, const sp_spark_dense* dense, const sp_spark_gens* gens, const uint64_t* rx_mont, size_t x, const uint64_t* ry_mont,
+                          size_t y, const uint64_t* evals_mont /* b x 4 or NULL */, uint8_t* strobe_state /* in, out */, uint8_t* tape_state /* in, out */,
+                          uint8_t** proof, size_t* proof_len, uint64_t* evals_out /* b x 4 */);
+/* SparseMatPolyEvalProof::verify(comm, rx, ry, evals, gens, transcript) (sparse_mlpoly.rs:1516-1557).  comm = bincode(SparseMatPolyCommitment).
+ * SP_OK: accepted.  SP_ERR_VERIFY / SP_ERR_DECOMPRESS: rejected, sp_last_error names the check, the transcript advanced as the reference's verify
+ * advances it.  A commitment that does not decode or does not fit the call (batch_size != b, num_ops not a power of two >= 2, num_mem_cells !=
+ * 2^max(x, y), gens whose views do not fit) is SP_ERR_VERIFY with the transcript untouched.  SP_ERR_INVALID_ARG: b outside 1 ..
+ * SP_SPARK_MAX_BATCH, NULL arguments; SP_ERR_INVALID_SCALAR: rx, ry or evals not reduced; both leave the transcript untouched. */
+int sp_spark_eval_verify_t(sp_ctx* ctx, const sp_spark_gens* gens, const uint8_t* comm, size_t comm_len, const uint64_t* rx_mont, size_t x,
+                           const uint64_t* ry_mont, size_t y, const uint64_t* evals_mont, int b, uint8_t* strobe_state /* in, out */, const uint8_t* proof,
+                           size_t proof_len);
+
 /* ---- inner-product argument, operator level: BulletReductionProof::prove (src/nizk/bullet.rs:32-132) for a host that keeps the transcript and
  * the orchestration.  sp_ipa_begin copies a_vec / b_vec; the generator vector G is `gens` (G[0..n)).  Each round: sp_ipa_round_LR returns the
  * compressed L, R of bullet.rs:83-97 (c_L, c_R are formed inside; Q and H are the caller's points), the host appends them and derives u

@@ -11,4 +11,5 @@ from .api import (  # noqa: F401
     sumcheck_prove, sumcheck_verify, debug_memcheck, debug_memcheck_report, debug_memcheck_scan,
     PolyCommitmentGens, PolyCommitment, PolyEvalProof, RandomTape, poly_commit,
     ProductLeaves, ProductCircuits, ProductCircuitEvalProofBatched, product_leaf_eval,
+    SparseMatPolyCommitmentGens, SparseMatPolyCommitment, SparseMatPolyDense, SparseMatPolynomial, SparseMatPolyEvalProof,
 )

@@ -820,6 +820,167 @@ def product_leaf_eval(leaves, table_evals, rand):
     return out[:k]
 
 
+# ----------------------------------------------------------------------------- SPARK: the caller's sparse matrices
+SP_SPARK_MAX_BATCH = 4
+
+
+class _SparkEntries(C.Structure):
+    _fields_ = [("row", _vp), ("col", _vp), ("val32", _vp), ("nnz", C.c_size_t)]
+
+
+class SparseMatPolyCommitmentGens(_Handle):
+    """SparseMatPolyCommitmentGens::new(label, num_vars_x, num_vars_y, num_nz_entries, batch_size) (sparse_mlpoly.rs:292-317): gens_ops, gens_mem
+    and gens_derefs as views of one generator set of the label (footprint: include/spartan_b200.h, sp_spark_gens_create)."""
+    _free = lib.sp_spark_gens_free
+
+    def __init__(self, label, num_vars_x, num_vars_y, num_nz_entries, batch_size, ctx=None):
+        self.ctx = ctx or default_context()
+        self.num_vars_x, self.num_vars_y, self.batch_size = num_vars_x, num_vars_y, batch_size
+        label = bytes(label)
+        h = _vp()
+        self.ctx.check(lib.sp_spark_gens_create(self.ctx.h, C.c_char_p(label), _sz(len(label)), _sz(num_vars_x), _sz(num_vars_y), _sz(num_nz_entries),
+                                                _sz(batch_size), C.byref(h)))
+        self.h = h
+
+
+class SparseMatPolyCommitment:
+    """sparse_mlpoly.rs:319-341: batch_size, num_ops, num_mem_cells and the commitments to comb_ops and comb_mem"""
+
+    def __init__(self, batch_size, num_ops, num_mem_cells, comm_comb_ops, comm_comb_mem):
+        self.batch_size, self.num_ops, self.num_mem_cells = batch_size, num_ops, num_mem_cells
+        self.comm_comb_ops, self.comm_comb_mem = comm_comb_ops, comm_comb_mem
+
+    def to_bytes(self):
+        """bincode(SparseMatPolyCommitment)"""
+        return (self.batch_size.to_bytes(8, "little") + self.num_ops.to_bytes(8, "little") + self.num_mem_cells.to_bytes(8, "little")
+                + self.comm_comb_ops.to_bytes() + self.comm_comb_mem.to_bytes())
+
+    @classmethod
+    def from_bytes(cls, data):
+        data = bytes(data)
+        if len(data) < 32:
+            raise SpartanB200Error("SparseMatPolyCommitment: %d bytes are too few" % len(data))
+        u = [int.from_bytes(data[8 * i:8 * i + 8], "little") for i in range(4)]
+        n_ops = 32 + 32 * u[3]
+        ops = PolyCommitment.from_bytes(data[24:n_ops])
+        return cls(u[0], u[1], u[2], ops, PolyCommitment.from_bytes(data[n_ops:]))
+
+    def append_to_transcript(self, label, transcript):
+        """sparse_mlpoly.rs:329-341 on a Transcript (the reference ignores the label)"""
+        for name, v in ((b"batch_size", self.batch_size), (b"num_ops", self.num_ops), (b"num_mem_cells", self.num_mem_cells)):
+            transcript.append_message(name, int(v).to_bytes(8, "little"))
+        self.comm_comb_ops.append_to_transcript(b"comm_comb_ops", transcript)
+        self.comm_comb_mem.append_to_transcript(b"comm_comb_mem", transcript)
+
+
+class SparseMatPolyDense(_Handle):
+    """MultiSparseMatPolynomialAsDense (sparse_mlpoly.rs:274-282) on the device: what multi_commit returns beside the commitment"""
+    _free = lib.sp_spark_dense_free
+
+    def __init__(self, ctx, h, batch_size, num_vars_x, num_vars_y):
+        self.ctx, self.h = ctx, h
+        self.batch_size, self.num_vars_x, self.num_vars_y = batch_size, num_vars_x, num_vars_y
+
+
+class SparseMatPolynomial:
+    """SparseMatPolynomial (sparse_mlpoly.rs:31-37): 2^num_vars_x rows, 2^num_vars_y columns, entries (row, col, val).  vals: canonical 32-byte
+    scalars as an (nnz, 32) uint8 array, a list of 32-byte strings or of ints (< q)."""
+
+    def __init__(self, num_vars_x, num_vars_y, rows, cols, vals):
+        self.num_vars_x, self.num_vars_y = num_vars_x, num_vars_y
+        self.rows = np.ascontiguousarray(rows, dtype=np.uint64).reshape(-1)
+        self.cols = np.ascontiguousarray(cols, dtype=np.uint64).reshape(-1)
+        if isinstance(vals, np.ndarray):
+            self.vals = np.ascontiguousarray(vals, dtype=np.uint8).reshape(-1, 32)
+        else:
+            self.vals = np.frombuffer(b"".join(int(v).to_bytes(32, "little") if isinstance(v, (int, np.integer)) else bytes(v) for v in vals),
+                                      dtype=np.uint8).reshape(-1, 32)
+        if not len(self.rows) == len(self.cols) == len(self.vals):
+            raise SpartanB200Error("SparseMatPolynomial: rows, cols and vals differ in length")
+        self.device = False
+
+    @classmethod
+    def from_tensors(cls, num_vars_x, num_vars_y, rows, cols, vals, ctx=None):
+        """the entries as CUDA tensors on ctx.device: rows and cols int64 of length nnz, vals uint8 of shape (nnz, 32); multi_commit reads them there"""
+        ctx = ctx or default_context()
+        torch = _torch()
+        o = cls.__new__(cls)
+        o.num_vars_x, o.num_vars_y, o.ctx, o.device = num_vars_x, num_vars_y, ctx, True
+        o.rows = _device_tensor(rows, ctx, "rows", torch.int64)
+        o.cols = _device_tensor(cols, ctx, "cols", torch.int64)
+        o.vals = _device_tensor(vals, ctx, "vals", torch.uint8, 32)
+        if not o.rows.shape[0] == o.cols.shape[0] == o.vals.shape[0]:
+            raise SpartanB200Error("rows, cols and vals differ in length (%d, %d, %d)" % (o.rows.shape[0], o.cols.shape[0], o.vals.shape[0]))
+        return o
+
+    def _entries(self):
+        if self.device:
+            return _SparkEntries(self.rows.data_ptr(), self.cols.data_ptr(), self.vals.data_ptr(), self.rows.shape[0])
+        return _SparkEntries(self.rows.ctypes.data, self.cols.ctypes.data, self.vals.ctypes.data, len(self.rows))
+
+    @staticmethod
+    def multi_commit(polys, gens):
+        """SparseMatPolynomial::multi_commit (sparse_mlpoly.rs:483-503) of 1 .. SP_SPARK_MAX_BATCH matrices of one shape, all host or all device
+        entries: returns (SparseMatPolyCommitment, SparseMatPolyDense)"""
+        polys = list(polys)
+        ctx = gens.ctx
+        device = bool(polys) and polys[0].device
+        if any(p.device != device for p in polys):
+            raise SpartanB200Error("multi_commit: mix of host and device matrices")
+        if any((p.num_vars_x, p.num_vars_y) != (polys[0].num_vars_x, polys[0].num_vars_y) for p in polys):
+            raise SpartanB200Error("multi_commit: matrices of different shapes")
+        x, y = (polys[0].num_vars_x, polys[0].num_vars_y) if polys else (0, 0)
+        arr = (_SparkEntries * max(len(polys), 1))(*[p._entries() for p in polys])
+        if device:
+            _sync_torch(ctx)
+        h, out, n = _vp(), C.POINTER(C.c_ubyte)(), _sz()
+        entry = lib.sp_spark_commit_device if device else lib.sp_spark_commit
+        ctx.check(entry(ctx.h, gens.h, arr, C.c_int(len(polys)), _sz(x), _sz(y), C.byref(h), C.byref(out), C.byref(n)))
+        dense = SparseMatPolyDense(ctx, h, len(polys), x, y)
+        return SparseMatPolyCommitment.from_bytes(_take_bytes(out, n)), dense
+
+    @staticmethod
+    def multi_evaluate(dense_or_polys, rx, ry, gens=None):
+        """SparseMatPolynomial::multi_evaluate (sparse_mlpoly.rs:440-452) on the device: the b evaluations M_i(rx, ry) as (b, 4) limbs.  Takes a
+        SparseMatPolyDense, or a list of SparseMatPolynomial together with gens that fit them (they are committed first)."""
+        dense = dense_or_polys
+        if not isinstance(dense, SparseMatPolyDense):
+            if gens is None:
+                raise SpartanB200Error("multi_evaluate of SparseMatPolynomials needs their gens")
+            dense = SparseMatPolynomial.multi_commit(dense_or_polys, gens)[1]
+        rx, ry = _limbs(rx), _limbs(ry)
+        out = np.zeros((dense.batch_size, 4), dtype=np.uint64)
+        dense.ctx.check(lib.sp_spark_evaluate(dense.ctx.h, dense.h, _p(rx), _sz(len(rx)), _p(ry), _sz(len(ry)), _p(out)))
+        return out
+
+
+class SparseMatPolyEvalProof:
+    """sparse_mlpoly.rs:1418-1557.  `data` = bincode(SparseMatPolyEvalProof).  Transcripts: a Transcript (advanced in place) or a label.  Neither
+    prove nor verify absorbs the commitment or the evaluations: the caller does, before the call."""
+
+    def __init__(self, data):
+        self.data = bytes(data)
+
+    @staticmethod
+    def prove(dense, rx, ry, evals, gens, transcript, tape):
+        """SparseMatPolyEvalProof::prove: returns (proof, evals as (b, 4) limbs).  evals=None: computed on the device; given evals must be
+        M_i(rx, ry)."""
+        ctx, t = dense.ctx, _transcript_state(transcript)
+        rx, ry = _limbs(rx), _limbs(ry)
+        out, n = C.POINTER(C.c_ubyte)(), _sz()
+        ev = np.zeros((dense.batch_size, 4), dtype=np.uint64)
+        ctx.check(lib.sp_spark_eval_prove_t(ctx.h, dense.h, gens.h, _p(rx), _sz(len(rx)), _p(ry), _sz(len(ry)),
+                                            None if evals is None else _p(_limbs(evals)), t.state, tape.state, C.byref(out), C.byref(n), _p(ev)))
+        return SparseMatPolyEvalProof(_take_bytes(out, n)), ev
+
+    def verify(self, comm, rx, ry, evals, gens, transcript):
+        """SparseMatPolyEvalProof::verify: raises ProofVerifyError; the transcript is advanced as the reference's verify advances it"""
+        t, rx, ry, ev = _transcript_state(transcript), _limbs(rx), _limbs(ry), _limbs(evals)
+        cb = comm.to_bytes() if isinstance(comm, SparseMatPolyCommitment) else bytes(comm)
+        gens.ctx.check(lib.sp_spark_eval_verify_t(gens.ctx.h, gens.h, C.c_char_p(cb), _sz(len(cb)), _p(rx), _sz(len(rx)), _p(ry), _sz(len(ry)), _p(ev),
+                                                  C.c_int(len(ev)), t.state, C.c_char_p(self.data), _sz(len(self.data))))
+
+
 # ----------------------------------------------------------------------------- public API of lib.rs
 class Assignment:
     """lib.rs:57-104: a vector of scalars given as canonical 32-byte strings"""

@@ -24,6 +24,8 @@ struct sp_pc_gens {
   size_t num_vars;
   PolyCommitmentGens g;
 };
+struct sp_spark_gens { Ctx* ctx; size_t x, y, nz, b; SparkGens g; };
+struct sp_spark_dense { Ctx* ctx; SparkDense d; };
 struct sp_prod_circuits {
   Ctx* ctx;
   size_t m;
@@ -831,7 +833,7 @@ static sp_instance* instance_from_device(Ctx& c, size_t num_cons, size_t num_var
   }
   DevBuf<unsigned long long> err(1);
   dev::set_max_u64(err.p, c.stream);
-  dev::inst_ingest(in, co, num_cons, num_vars, num_inputs, num_vars_padded, err.p, c.stream);
+  dev::inst_ingest(in, 3, co, num_cons, num_vars + 1 + num_inputs, num_vars, num_vars_padded - num_vars, err.p, c.stream);
   unsigned long long first = 0;
   dev::d2h(&first, err.p, sizeof(first), c.stream);
   c.sync();
@@ -878,7 +880,7 @@ int sp_instance_create_device(sp_ctx* ctx, size_t num_cons, size_t num_vars, siz
                               const uint8_t* A_val, size_t nA, const uint64_t* B_row, const uint64_t* B_col, const uint8_t* B_val, size_t nB,
                               const uint64_t* C_row, const uint64_t* C_col, const uint8_t* C_val, size_t nC, sp_instance** out) {
   return guarded(ctx, [&] {
-    const dev::CooIn in = {{A_row, B_row, C_row}, {A_col, B_col, C_col}, {A_val, B_val, C_val}, {nA, nB, nC}};
+    const dev::CooIn in = {{A_row, B_row, C_row}, {A_col, B_col, C_col}, {A_val, B_val, C_val}, {nA, nB, nC}};   // matrices past C: empty
     static const char* names[3][3] = {{"A_row", "A_col", "A_val"}, {"B_row", "B_col", "B_val"}, {"C_row", "C_col", "C_val"}};
     for (int m = 0; m < 3; m++) {
       require_device(ctx->c, in.row[m], in.n[m], names[m][0]);
@@ -1116,7 +1118,7 @@ int sp_snark_commitment_load(sp_ctx* ctx, const uint8_t* bytes, size_t len, sp_s
 static int snark_prove_common(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const VarsArg& vars, const uint64_t* inputs, size_t ninputs,
                               const sp_snark_gens* gens, const TranscriptArg& ta, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
   return guarded(ctx, [&] {
-    if (!enc->e->comb_ops.p) throw SpError(SP_ERR_INVALID_ARG, "this handle holds a commitment only (sp_snark_commitment_load): proving needs sp_snark_encode");
+    if (!enc->e->dense.comb_ops.p) throw SpError(SP_ERR_INVALID_ARG, "this handle holds a commitment only (sp_snark_commitment_load): proving needs sp_snark_encode");
     prove_statement(ctx->c, inst->inst, vars, inputs, ninputs, ta, seed, proof, proof_len, [&](const u256* d_vars, const std::vector<Fq>& in, Transcript& T, const Fq& s) {
       SnarkProof P;
       snark_prove(ctx->c, inst->inst, *enc->e, d_vars, in, *gens->g, T, s, P);
@@ -1496,6 +1498,181 @@ int sp_prod_leaf_eval(const sp_prod_leaves* leaves, int k, const uint64_t* table
       for (uint32_t s = 0; s < f[c].nsrc; s++) v += f[c].coeff[s] * fq_in(table_evals + 4 * f[c].src[s]);
       fq_out(out + 4 * c, v);
     }
+  });
+}
+
+// ---- SPARK of the caller's matrices (snark.cpp: spark_*).  Every argument is checked before the first allocation and before the transcript or
+// the tape is touched, so a refused call leaves them as they were.
+static const size_t SPARK_MAX_VARS = 30;   // 32-bit addresses, and fewer than 2^31 cells to sort
+static void spark_shape(size_t x, size_t y, const std::string& what) {
+  if (std::max(x, y) == 0) throw SpError(SP_ERR_INVALID_ARG, what + ": num_vars_x = num_vars_y = 0 (one memory cell) is not supported");
+  if (std::max(x, y) > SPARK_MAX_VARS)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": max(num_vars_x, num_vars_y) = " + std::to_string(std::max(x, y)) + " > " + std::to_string(SPARK_MAX_VARS) +
+                                          " (addresses are 32-bit)");
+}
+static void spark_check_gens(const sp_ctx* ctx, const sp_spark_gens* g, size_t x, size_t y, size_t N, size_t b, const std::string& what) {
+  require_owned(ctx, g, what, "gens handle");
+  if (!SparkDims(x, y, N, b).fits(g->g))
+    throw SpError(SP_ERR_INVALID_ARG, what + ": gens for (x, y, nz, b) = (" + std::to_string(g->x) + ", " + std::to_string(g->y) + ", " + std::to_string(g->nz) +
+                                          ", " + std::to_string(g->b) + ") do not fit (" + std::to_string(x) + ", " + std::to_string(y) + ", " + std::to_string(N) +
+                                          ", " + std::to_string(b) + ")");
+}
+static void spark_commit_common(sp_ctx* ctx, const sp_spark_gens* gens, const sp_spark_entries* mats, int b, size_t x, size_t y, sp_spark_dense** dense,
+                                uint8_t** comm, size_t* comm_len, bool device) {
+  const std::string what = device ? "spark_commit_device" : "spark_commit";
+  Ctx& c = ctx->c;
+  if (!dense || !comm || !comm_len || !mats) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  require_count(what, b, "matrices", "SP_SPARK_MAX_BATCH", SP_SPARK_MAX_BATCH);
+  spark_shape(x, y, what);
+  size_t N = 1;
+  for (int m = 0; m < b; m++) {
+    const sp_spark_entries& e = mats[m];
+    if (e.nnz && (!e.row || !e.col || !e.val32)) throw SpError(SP_ERR_INVALID_ARG, what + ": matrix " + std::to_string(m) + ": NULL array");
+    if (e.nnz >= ((size_t)1 << 31)) throw SpError(SP_ERR_INVALID_ARG, what + ": matrix " + std::to_string(m) + ": 2^31 or more entries");
+    if (device) {
+      const std::string at = "matrix " + std::to_string(m);
+      require_device(c, e.row, e.nnz, (at + " row").c_str());
+      require_device(c, e.col, e.nnz, (at + " col").c_str());
+      require_device(c, e.val32, e.nnz, (at + " val").c_str());
+    }
+    N = std::max(N, next_pow2(e.nnz));
+  }
+  if (N < 2) throw SpError(SP_ERR_INVALID_ARG, what + ": every matrix has at most one entry (num_ops = 1 leaves the product circuits without layers)");
+  spark_check_gens(ctx, gens, x, y, N, (size_t)b, what);
+  // the caller's entries on the device (host arrays are copied as they are) meet the checks of sp_instance_create: row < 2^x, col < 2^y, val < q
+  DevBuf<uint64_t> d_row[SP_SPARK_MAX_BATCH], d_col[SP_SPARK_MAX_BATCH];
+  DevBuf<uint8_t> d_val[SP_SPARK_MAX_BATCH];
+  DevBuf<uint32_t> row[SP_SPARK_MAX_BATCH], col[SP_SPARK_MAX_BATCH];
+  DevBuf<u256> val[SP_SPARK_MAX_BATCH];
+  dev::CooIn in{};
+  dev::CooOut co{};
+  SparkMatrix sm[SP_SPARK_MAX_BATCH];
+  for (int m = 0; m < b; m++) {
+    const sp_spark_entries& e = mats[m];
+    in.row[m] = e.row; in.col[m] = e.col; in.val[m] = e.val32; in.n[m] = e.nnz;
+    if (!device) {
+      d_row[m].alloc(e.nnz); d_col[m].alloc(e.nnz); d_val[m].alloc(32 * e.nnz);
+      dev::h2d(d_row[m].p, e.row, e.nnz * sizeof(uint64_t), c.stream);
+      dev::h2d(d_col[m].p, e.col, e.nnz * sizeof(uint64_t), c.stream);
+      dev::h2d(d_val[m].p, e.val32, 32 * e.nnz, c.stream);
+      in.row[m] = d_row[m].p; in.col[m] = d_col[m].p; in.val[m] = d_val[m].p;
+    }
+    row[m].alloc(e.nnz); col[m].alloc(e.nnz); val[m].alloc(e.nnz);
+    co.row[m] = row[m].p; co.col[m] = col[m].p; co.val[m] = val[m].p;
+    sm[m] = SparkMatrix{row[m].p, col[m].p, val[m].p, e.nnz};
+  }
+  DevBuf<unsigned long long> err(1);
+  dev::set_max_u64(err.p, c.stream);
+  const size_t ncols = (size_t)1 << y;
+  dev::inst_ingest(in, b, co, (size_t)1 << x, ncols, ncols, 0, err.p, c.stream);
+  unsigned long long first = 0;
+  dev::d2h(&first, err.p, sizeof(first), c.stream);
+  c.sync();
+  if (first != ~0ull) {   // the first bad entry in (matrix, entry) order; within it row, then column, then scalar
+    const unsigned code = (unsigned)(first & 3);
+    const std::string at = " (matrix " + std::to_string(first >> 42) + ", entry " + std::to_string((first >> 2) & (((unsigned long long)1 << 40) - 1)) + ")";
+    if (code == dev::INGEST_ROW) throw SpError(SP_ERR_INVALID_INDEX, what + ": row out of range" + at);
+    if (code == dev::INGEST_COL) throw SpError(SP_ERR_INVALID_INDEX, what + ": col out of range" + at);
+    throw SpError(SP_ERR_INVALID_SCALAR, what + ": value not a canonical scalar" + at);
+  }
+  std::unique_ptr<sp_spark_dense> d(new sp_spark_dense{&c, {}});
+  SparseMatPolyCommitment cm;
+  spark_commit(c, sm, (size_t)b, x, y, gens->g, d->d, cm);
+  put_bytes(comm, comm_len, to_bincode(cm));
+  *dense = d.release();
+}
+// rx, ry of a dense's shape
+static void spark_point(const sp_spark_dense* d, const uint64_t* rx, size_t x, const uint64_t* ry, size_t y, const std::string& what) {
+  if ((!rx && x) || (!ry && y)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  if (x != d->d.x || y != d->d.y)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": |rx| = " + std::to_string(x) + ", |ry| = " + std::to_string(y) + " but the matrices have 2^" + std::to_string(d->d.x) +
+                                          " rows and 2^" + std::to_string(d->d.y) + " columns");
+  require_reduced(rx, x, (what + ": rx").c_str());
+  require_reduced(ry, y, (what + ": ry").c_str());
+}
+
+int sp_spark_gens_create(sp_ctx* ctx, const uint8_t* label, size_t label_len, size_t x, size_t y, size_t nz, size_t b, sp_spark_gens** out) {
+  return guarded(ctx, [&] {
+    const std::string what = "spark_gens_create";
+    if (!out || (!label && label_len)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    if (b < 1 || b > SP_SPARK_MAX_BATCH)
+      throw SpError(SP_ERR_INVALID_ARG, what + ": batch_size = " + std::to_string(b) + "; 1 .. SP_SPARK_MAX_BATCH = " + std::to_string(SP_SPARK_MAX_BATCH) + " supported");
+    spark_shape(x, y, what);
+    if (nz > ((size_t)1 << 31)) throw SpError(SP_ERR_INVALID_ARG, what + ": num_nz_entries > 2^31");
+    const SparkDims d(x, y, nz, b);
+    auto set = std::make_shared<GenSet>(&ctx->c, std::string((const char*)label, label_len), d.bases(), d.host_bases());
+    std::unique_ptr<sp_spark_gens> g(new sp_spark_gens{&ctx->c, x, y, nz, b, SparkGens(set, d)});
+    *out = g.release();
+  });
+}
+void sp_spark_gens_free(sp_spark_gens* g) { delete g; }
+int sp_spark_commit(sp_ctx* ctx, const sp_spark_gens* gens, const sp_spark_entries* matrices, int b, size_t x, size_t y, sp_spark_dense** dense, uint8_t** comm,
+                    size_t* comm_len) {
+  return guarded(ctx, [&] { spark_commit_common(ctx, gens, matrices, b, x, y, dense, comm, comm_len, false); });
+}
+int sp_spark_commit_device(sp_ctx* ctx, const sp_spark_gens* gens, const sp_spark_entries* matrices, int b, size_t x, size_t y, sp_spark_dense** dense,
+                           uint8_t** comm, size_t* comm_len) {
+  return guarded(ctx, [&] { spark_commit_common(ctx, gens, matrices, b, x, y, dense, comm, comm_len, true); });
+}
+void sp_spark_dense_free(sp_spark_dense* d) { delete d; }
+int sp_spark_evaluate(sp_ctx* ctx, const sp_spark_dense* dense, const uint64_t* rx, size_t x, const uint64_t* ry, size_t y, uint64_t* out) {
+  return guarded(ctx, [&] {
+    const std::string what = "spark_evaluate";
+    if (!out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    require_owned(ctx, dense, what, "dense handle");
+    spark_point(dense, rx, x, ry, y, what);
+    std::vector<Fq> ev(dense->d.b);
+    spark_evaluate(ctx->c, dense->d, fq_vec(rx, x), fq_vec(ry, y), ev.data());
+    put_scalars(out, ev);
+  });
+}
+int sp_spark_eval_prove_t(sp_ctx* ctx, const sp_spark_dense* dense, const sp_spark_gens* gens, const uint64_t* rx, size_t x, const uint64_t* ry, size_t y,
+                          const uint64_t* evals, uint8_t* strobe_state, uint8_t* tape_state, uint8_t** proof, size_t* proof_len, uint64_t* evals_out) {
+  return guarded(ctx, [&] {
+    const std::string what = "spark_eval_prove";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if (!proof || !proof_len || !evals_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    require_owned(ctx, dense, what, "dense handle");
+    const SparkDense& d = dense->d;
+    spark_check_gens(ctx, gens, d.x, d.y, d.N, d.b, what);
+    spark_point(dense, rx, x, ry, y, what);
+    if (evals) require_reduced(evals, d.b, (what + ": evals").c_str());
+    RandomTape tape(pc_tape_open(tape_state, what));
+    const std::vector<Fq> vx = fq_vec(rx, x), vy = fq_vec(ry, y);
+    std::vector<Fq> ev(d.b);
+    spark_evaluate(ctx->c, d, vx, vy, ev.data());
+    if (evals)
+      for (size_t m = 0; m < d.b; m++)
+        if (!(fq_in(evals + 4 * m) == ev[m])) throw SpError(SP_ERR_INVALID_ARG, what + ": evals[" + std::to_string(m) + "] is not M_" + std::to_string(m) + "(rx, ry)");
+    Transcript T = ta.open();
+    ctx->c.timings.clear();
+    SparseMatPolyEvalProof P;
+    spark_eval_prove(ctx->c, d, vx, vy, ev, gens->g, T, tape, P);
+    ta.close(T);
+    tape.state().export_state(tape_state);
+    put_bytes(proof, proof_len, to_bincode(P));
+    put_scalars(evals_out, ev);
+  });
+}
+int sp_spark_eval_verify_t(sp_ctx* ctx, const sp_spark_gens* gens, const uint8_t* comm, size_t comm_len, const uint64_t* rx, size_t x, const uint64_t* ry,
+                           size_t y, const uint64_t* evals, int b, uint8_t* strobe_state, const uint8_t* proof, size_t proof_len) {
+  return guarded(ctx, [&] {
+    const std::string what = "spark_eval_verify";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if ((!comm && comm_len) || (!proof && proof_len) || (!rx && x) || (!ry && y) || !evals) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    require_count(what, b, "evaluations", "SP_SPARK_MAX_BATCH", SP_SPARK_MAX_BATCH);
+    require_owned(ctx, gens, what, "gens handle");
+    if (std::max(x, y) > SPARK_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": max(|rx|, |ry|) > " + std::to_string(SPARK_MAX_VARS));
+    require_reduced(rx, x, (what + ": rx").c_str());
+    require_reduced(ry, y, (what + ": ry").c_str());
+    require_reduced(evals, (size_t)b, (what + ": evals").c_str());
+    const SparseMatPolyCommitment cm = from_bincode<SparseMatPolyCommitment>(comm, comm_len, SP_ERR_VERIFY, "sparse polynomial commitment");
+    check_spark_commitment(cm, (size_t)b, x, y, gens->g);
+    Transcript T = ta.open();
+    TranscriptClose close{ta, T};
+    spark_eval_verify(ctx->c, cm, fq_vec(rx, x), fq_vec(ry, y), fq_vec(evals, (size_t)b), gens->g, T, proof, proof_len);
   });
 }
 

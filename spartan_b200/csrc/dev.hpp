@@ -216,13 +216,15 @@ void sparse_eval3(u256* out, const uint32_t* row, const uint32_t* col, const u25
 bool is_device_pointer(const void* p, int device);   // memory allocated on `device` (cudaMemoryTypeDevice)
 void set_max_u64(unsigned long long* w, cudaStream_t s);
 void d2h_sync(void* h, const void* d, size_t bytes);  // blocking copy outside any stream's order (data no pending work writes)
-// Instance::new (lib.rs:129-198) entries of A, B, C from caller arrays: row < num_cons, col < num_vars + 1 + num_inputs, value < q; columns from
-// num_vars on move up by num_vars_padded - num_vars; values to Montgomery form.  The first bad entry in (matrix, entry, row/col/scalar) order
-// wins: *err = min over bad entries of ((m << 40 | k) << 2) | code (*err = ~0 beforehand: none)
+// Instance::new (lib.rs:129-198) entries of A, B, C, or of a caller's SPARK matrices, from caller arrays: `nmat` matrices, row < num_rows,
+// col < num_cols, value < q; columns from num_vars on move up by `shift` (the R1CS input columns; num_vars = num_cols: none); values to
+// Montgomery form.  The first bad entry in (matrix, entry, row/col/scalar) order wins: *err = min over bad entries of ((m << 40 | k) << 2) | code
+// (*err = ~0 beforehand: none)
 enum { INGEST_ROW = 0, INGEST_COL = 1, INGEST_SCALAR = 2 };
-struct CooIn { const uint64_t* row[3]; const uint64_t* col[3]; const uint8_t* val[3]; size_t n[3]; };
-struct CooOut { uint32_t* row[3]; uint32_t* col[3]; u256* val[3]; };
-void inst_ingest(const CooIn& in, const CooOut& out, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_vars_padded, unsigned long long* err,
+constexpr int INGEST_MAX_MATRICES = SP_SPARK_MAX_BATCH;   // >= 3, the R1CS matrices
+struct CooIn { const uint64_t* row[INGEST_MAX_MATRICES]; const uint64_t* col[INGEST_MAX_MATRICES]; const uint8_t* val[INGEST_MAX_MATRICES]; size_t n[INGEST_MAX_MATRICES]; };
+struct CooOut { uint32_t* row[INGEST_MAX_MATRICES]; uint32_t* col[INGEST_MAX_MATRICES]; u256* val[INGEST_MAX_MATRICES]; };
+void inst_ingest(const CooIn& in, int nmat, const CooOut& out, size_t num_rows, size_t num_cols, size_t num_vars, size_t shift, unsigned long long* err,
                  cudaStream_t s);
 // entries [from, to) = (row i, column pad_col, value 0): the padding of an instance with fewer than two constraints
 void inst_pad_rows(uint32_t* row, uint32_t* col, u256* val, size_t from, size_t to, uint32_t pad_col, cudaStream_t s);
@@ -232,10 +234,11 @@ void canonical_to_mont(u256* out, const uint8_t* in32, size_t n, unsigned long l
 size_t compress_scratch_bytes(size_t nmajor, size_t nnz);
 void build_compressed(uint32_t* ptr, uint32_t* idx, u256* v, size_t nmajor, const uint32_t* major, const uint32_t* minor, const u256* val, size_t nnz,
                       void* scratch, cudaStream_t s);
-// AddrTimestamps::new (sparse_mlpoly.rs:220-254), one side: the addresses src[m][0..nnz[m]) zero-padded to N -> idx[m] (N each) and, as field
-// elements over the 3N positions (matrix-major), addr_f, ts_f (read_ts) and audit_f (cells); *bad |= 1 when an address is >= cells
-struct SparkAddrs { const uint32_t* src[3]; size_t nnz[3]; uint32_t* idx[3]; };
-size_t spark_ts_scratch_bytes(size_t N, size_t cells);
+// AddrTimestamps::new (sparse_mlpoly.rs:220-254), one side of b <= SP_SPARK_MAX_BATCH matrices: the addresses src[m][0..nnz[m]) zero-padded to N
+// -> idx[m] (N each) and, as field elements over the b N positions (matrix-major, the reference loop's order), addr_f, ts_f (read_ts) and audit_f
+// (cells, counts over all b matrices); *bad |= 1 when an address is >= cells
+struct SparkAddrs { const uint32_t* src[SP_SPARK_MAX_BATCH]; size_t nnz[SP_SPARK_MAX_BATCH]; uint32_t* idx[SP_SPARK_MAX_BATCH]; int b; };
+size_t spark_ts_scratch_bytes(size_t b, size_t N, size_t cells);
 void spark_timestamps(const SparkAddrs& sa, u256* addr_f, u256* ts_f, u256* audit_f, size_t N, size_t cells, void* scratch, unsigned int* bad, cudaStream_t s);
 
 // ---- group: generators, fixed-base window tables, multi-row MSM, compression (K3/K4/K6)

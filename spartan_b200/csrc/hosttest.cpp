@@ -4,6 +4,7 @@
 #include "host.hpp"
 #include "engine.hpp"
 #include "wire.hpp"
+#include "snark.hpp"
 using namespace sp;
 
 namespace sp { void shake256(uint8_t* out, size_t outlen, const uint8_t* in, size_t inlen); }
@@ -14,6 +15,13 @@ static void out256(uint8_t* b, const u256& x) { memcpy(b, &x, 32); }
 #include "deflate.cpp"   // host-only translation unit, pulled in here so the CPU tests can call it without the CUDA library
 
 extern "C" {
+
+// SparkDims of SparseMatPolyCommitmentGens::new(x, y, nz, b): out = v_ops, v_mem, v_derefs, n_ops, n_mem, n_der
+void sph_spark_dims(size_t x, size_t y, size_t nz, size_t b, size_t out[6]) {
+  const sp::SparkDims d(x, y, nz, b);
+  const size_t v[6] = {d.v_ops, d.v_mem, d.v_derefs, d.n_ops, d.n_mem, d.n_der};
+  for (int i = 0; i < 6; i++) out[i] = v[i];
+}
 // R1CSShape digest compressor: zlib stream of miniz level 6 (deflate.cpp); returns the length (out must hold len + len/8 + 128 bytes)
 size_t spt_zlib6(const uint8_t* in, size_t len, uint8_t* out) {
   std::vector<uint8_t> z = sp::miniz_zlib_level6(in, len);

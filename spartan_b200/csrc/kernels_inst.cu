@@ -45,30 +45,37 @@ __device__ __forceinline__ u256 ld_bytes32(const uint8_t* p, bool aligned) {
   return r;
 }
 
-// ---- Instance::new entries: one pass over A, B and C
-__global__ void k_inst_ingest(CooIn in, CooOut out, size_t total, uint64_t num_cons, uint64_t num_vars, uint64_t ncols, uint64_t shift, int aligned,
+// ---- Instance::new entries (or a caller's SPARK matrices): one pass over every matrix
+__global__ void k_inst_ingest(CooIn in, CooOut out, size_t total, uint64_t num_rows, uint64_t num_cols, uint64_t num_vars, uint64_t shift, int aligned,
                               unsigned long long* err) {
   for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
     int m = 0;
     size_t k = t;
-    if (k >= in.n[0]) { k -= in.n[0]; m = 1; if (k >= in.n[1]) { k -= in.n[1]; m = 2; } }
+#pragma unroll
+    for (int j = 0; j < INGEST_MAX_MATRICES - 1; j++)
+      if (m == j && k >= in.n[j]) { k -= in.n[j]; m = j + 1; }
     const uint64_t r = in.row[m][k], c = in.col[m][k];
     const u256 x = ld_bytes32(in.val[m] + 32 * k, aligned);
     // the host path's order within one entry: row, column, scalar
-    const unsigned code = r >= num_cons ? INGEST_ROW : c >= ncols ? INGEST_COL : !fq_canonical(x) ? INGEST_SCALAR : 3u;
+    const unsigned code = r >= num_rows ? INGEST_ROW : c >= num_cols ? INGEST_COL : !fq_canonical(x) ? INGEST_SCALAR : 3u;
     if (code != 3u) { atomicMin(err, ((((unsigned long long)m << 40) | k) << 2) | code); continue; }
     out.row[m][k] = (uint32_t)r;
     out.col[m][k] = (uint32_t)(c >= num_vars ? c + shift : c);
     st256(out.val[m] + k, fq_to_mont(x));
   }
 }
-void inst_ingest(const CooIn& in, const CooOut& out, size_t num_cons, size_t num_vars, size_t num_inputs, size_t num_vars_padded, unsigned long long* err,
+void inst_ingest(const CooIn& in, int nmat, const CooOut& out, size_t num_rows, size_t num_cols, size_t num_vars, size_t shift, unsigned long long* err,
                  cudaStream_t s) {
-  const size_t total = in.n[0] + in.n[1] + in.n[2];
-  if (!total) return;
+  CooIn a = in;   // the matrices past nmat are empty: the kernel's matrix search never reaches them
+  size_t total = 0;
   bool aligned = true;
-  for (int m = 0; m < 3; m++) aligned = aligned && (in.n[m] == 0 || ((uintptr_t)in.val[m] & 15) == 0);
-  k_inst_ingest<<<grid_for(total, 256, 8), 256, 0, s>>>(in, out, total, num_cons, num_vars, num_vars + 1 + num_inputs, num_vars_padded - num_vars, aligned ? 1 : 0, err);
+  for (int m = 0; m < INGEST_MAX_MATRICES; m++) {
+    if (m >= nmat) a.n[m] = 0;
+    total += a.n[m];
+    aligned = aligned && (a.n[m] == 0 || ((uintptr_t)a.val[m] & 15) == 0);
+  }
+  if (!total) return;
+  k_inst_ingest<<<grid_for(total, 256, 8), 256, 0, s>>>(a, out, total, num_rows, num_cols, num_vars, shift, aligned ? 1 : 0, err);
   SP_LAUNCHED(); check("inst_ingest");
 }
 __global__ void k_inst_pad_rows(uint32_t* row, uint32_t* col, u256* val, size_t from, size_t to, uint32_t pad_col) {
@@ -161,11 +168,14 @@ void build_compressed(uint32_t* ptr, uint32_t* idx, u256* v, size_t nmajor, cons
   ck(cub::DeviceScan::ExclusiveSum(w.temp, tb, w.cnt, ptr, (int)(nmajor + 1), s), "scan");   // cnt[nmajor] = 0, so ptr[nmajor] = nnz
 }
 
-// ---- AddrTimestamps::new (sparse_mlpoly.rs:220-254) for one side: 3N positions in the reference loop's order (matrix-major, zero-padded to N);
+// ---- AddrTimestamps::new (sparse_mlpoly.rs:220-254) for one side: b N positions in the reference loop's order (matrix-major, zero-padded to N);
 // read_ts of a position = earlier positions with its address = its rank within its run after a stable sort by address; audit = run lengths
-size_t spark_ts_scratch_bytes(size_t N, size_t cells) { check_items(3 * N); check_items(cells); return align256(4 * 3 * N) + align256(4 * cells) + SortScratch::bytes(cells, 3 * N); }
+size_t spark_ts_scratch_bytes(size_t b, size_t N, size_t cells) {
+  check_items(b * N); check_items(cells);
+  return align256(4 * b * N) + align256(4 * cells) + SortScratch::bytes(cells, b * N);
+}
 __global__ void k_ts_addrs(SparkAddrs sa, size_t N, uint32_t* keys, u256* addr_f) {
-  for (size_t pos = (size_t)blockIdx.x * blockDim.x + threadIdx.x; pos < 3 * N; pos += (size_t)gridDim.x * blockDim.x) {
+  for (size_t pos = (size_t)blockIdx.x * blockDim.x + threadIdx.x; pos < (size_t)sa.b * N; pos += (size_t)gridDim.x * blockDim.x) {
     const int m = (int)(pos / N);
     const size_t i = pos - (size_t)m * N;
     const uint32_t a = i < sa.nnz[m] ? sa.src[m][i] : 0u;
@@ -185,8 +195,8 @@ __global__ void k_u32_to_fq(u256* out, const uint32_t* __restrict__ v, size_t n)
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) st256(out + i, fq_from_u64(v[i]));
 }
 void spark_timestamps(const SparkAddrs& sa, u256* addr_f, u256* ts_f, u256* audit_f, size_t N, size_t cells, void* scratch, unsigned int* bad, cudaStream_t s) {
-  ProfScope ps("spark_timestamps", 3.0 * N * (32 + 32 + 32) + 40.0 * cells, s);
-  const size_t n = 3 * N;
+  const size_t n = (size_t)sa.b * N;
+  ProfScope ps("spark_timestamps", (double)n * (32 + 32 + 32) + 40.0 * cells, s);
   uint32_t* keys = (uint32_t*)scratch;
   uint32_t* off = (uint32_t*)((char*)scratch + align256(4 * n));
   SortScratch w((char*)scratch + align256(4 * n) + align256(4 * cells), cells, n);

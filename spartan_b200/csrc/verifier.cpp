@@ -532,8 +532,8 @@ void hash_helper(const std::vector<Fq>& rand_mem, const Fq& claim_init, const st
   if (!(h(init_addr, init_val, audit_ts) == claim_audit)) throw Reject("hash layer: audit");
 }
 // SparseMatPolyEvalProof::verify (sparse_mlpoly.rs:1516-1557) -> PolyEvalNetworkProof::verify (:1356-1416)
-void spark_verify(Checker& chk, const SparseMatPolyEvalProof& p, const ComputationCommitment& comm, std::vector<Fq> rx, std::vector<Fq> ry,
-                  const Fq evals[3], const SnarkGens& gens, Transcript& T) {
+void spark_verify(Checker& chk, const SparseMatPolyEvalProof& p, const SparseMatPolyCommitment& comm, std::vector<Fq> rx, std::vector<Fq> ry,
+                  const std::vector<Fq>& evals, const SparkGens& gens, Transcript& T) {
   T.append_protocol_name("Sparse polynomial evaluation proof");
   equalize(rx, ry);
   if (((size_t)1 << rx.size()) != comm.num_mem_cells) throw Reject("memory size");
@@ -541,7 +541,7 @@ void spark_verify(Checker& chk, const SparseMatPolyEvalProof& p, const Computati
   std::vector<Fq> r_mem = T.challenge_vector("challenge_r_hash", 2);
   const Fq &r_hash = r_mem[0], &r_multiset = r_mem[1];
   T.append_protocol_name("Sparse polynomial evaluation proof");      // PolyEvalNetworkProof::protocol_name is the same string
-  const size_t ni = 3, num_ops = next_pow2(comm.num_ops), num_cells = (size_t)1 << rx.size();
+  const size_t ni = evals.size(), num_ops = next_pow2(comm.num_ops), num_cells = (size_t)1 << rx.size();
   // ---- ProductLayerProof::verify (sparse_mlpoly.rs:1228-1305)
   const ProductLayerProof& pl = p.proof_prod_layer;
   T.append_protocol_name("Sparse polynomial product layer proof");
@@ -601,7 +601,7 @@ void check_commitment(const ComputationCommitment& comm) {
   // SparseMatPolyCommitment consistency (sparse_mlpoly.rs:366-420): 3 matrices, power-of-two op count of at least 2 (what snark_encode
   // produces: one op leaves the product circuits without layers), cells = max(num_cons, 2*num_vars)
   const size_t cells = std::max(comm.num_cons, 2 * comm.num_vars);
-  if (comm.batch_size != 3 || !pow2(comm.num_ops) || comm.num_ops < 2 || comm.num_mem_cells != cells)
+  if (comm.comm.batch_size != 3 || !pow2(comm.comm.num_ops) || comm.comm.num_ops < 2 || comm.comm.num_mem_cells != cells)
     throw SpError(SP_ERR_INVALID_ARG, "verifier: inconsistent computation commitment");
 }
 
@@ -633,7 +633,7 @@ void snark_replay(Checker& chk, const ComputationCommitment& comm, const std::ve
   T.append_scalar("Ar_claim", evals[0]);
   T.append_scalar("Br_claim", evals[1]);
   T.append_scalar("Cr_claim", evals[2]);
-  spark_verify(chk, p.r1cs_eval_proof, comm, rx, ry, evals, gens, T);
+  spark_verify(chk, p.r1cs_eval_proof, comm.comm, rx, ry, std::vector<Fq>(evals, evals + 3), gens.gens_r1cs_eval, T);
 }
 
 // every point a proof carries, in wire order (the fields io() lists)
@@ -769,6 +769,21 @@ void snark_verify(Ctx& ctx, const SnarkEncoding& enc, const std::vector<Fq>& inp
   snark_replay(chk, enc.comm, input, gens, T, p);
 }
 
+void check_spark_commitment(const SparseMatPolyCommitment& c, size_t nevals, size_t x, size_t y, const SparkGens& gens) {
+  if (c.batch_size != nevals) throw Reject("commitment batch size " + std::to_string(c.batch_size) + " != " + std::to_string(nevals) + " evaluations");
+  if (nevals < 1 || nevals > SP_SPARK_MAX_BATCH) throw Reject("batch size outside 1 .. SP_SPARK_MAX_BATCH");
+  if (!pow2(c.num_ops) || c.num_ops < 2) throw Reject("commitment num_ops is not a power of two >= 2");
+  if (std::max(x, y) >= 63 || c.num_mem_cells != ((size_t)1 << std::max(x, y))) throw Reject("commitment num_mem_cells != 2^max(|rx|, |ry|)");
+  if (!SparkDims(x, y, c.num_ops, c.batch_size).fits(gens)) throw Reject("generators do not fit the commitment's sizes");
+}
+// SparseMatPolyEvalProof::verify (sparse_mlpoly.rs:1516-1557) of a caller's proof
+void spark_eval_verify(Ctx& ctx, const SparseMatPolyCommitment& comm, const std::vector<Fq>& rx, const std::vector<Fq>& ry, const std::vector<Fq>& evals,
+                       const SparkGens& gens, Transcript& T, const uint8_t* proof, size_t len) {
+  const SparseMatPolyEvalProof p = from_bincode<SparseMatPolyEvalProof>(proof, len, SP_ERR_VERIFY, "proof");
+  Immediate chk(ctx);
+  spark_verify(chk, p, comm, rx, ry, evals, gens, T);
+}
+
 // PolyEvalProof::verify (dense_mlpoly.rs:367-389) against the caller's C_Zr, or verify_plain (:391-404) against Zr
 void pc_eval_verify(Ctx& ctx, const PolyCommitmentGens& gens, const PolyCommitment& comm, const std::vector<Fq>& r, const Cp* C_Zr, const Fq* Zr, Transcript& T,
                     const uint8_t* proof, size_t len) {
@@ -800,7 +815,7 @@ void snark_verify_batch(Ctx& ctx, const SnarkGens& gens, std::vector<VerifyJob>&
       ctx, jobs, seed, [&](Checker& chk, const VerifyJob& j, Transcript& T, const SnarkProof& p) { snark_replay(chk, j.enc->comm, j.input, gens, T, p); },
       [&](const VerifyJob& j, Transcript& T) { snark_verify(ctx, *j.enc, j.input, gens, T, j.proof, j.len); },
       [](const VerifyJob& j, std::vector<Cp>& out) {
-        for (const PolyCommitment* c : {&j.enc->comm.comm_comb_ops, &j.enc->comm.comm_comb_mem})
+        for (const PolyCommitment* c : {&j.enc->comm.comm.comm_comb_ops, &j.enc->comm.comm.comm_comb_mem})
           if (c->C.size() <= 8) out.insert(out.end(), c->C.begin(), c->C.end());
       });
 }

@@ -118,7 +118,7 @@ struct R1CSProof {
       proof_eq_sc_phase2);
   }
 };
-// ---- product_tree.rs / sparse_mlpoly.rs (SNARK only)
+// ---- product_tree.rs / sparse_mlpoly.rs
 struct LayerProofBatched {
   static constexpr size_t MIN_BYTES = 8;
   SumcheckInstanceProof proof; std::vector<Fq> claims_prod_left, claims_prod_right;
@@ -161,12 +161,17 @@ struct SnarkProof {  // lib.rs:313-317
   SparseMatPolyEvalProof r1cs_eval_proof;
   template <class A> void io(A& a) { a(r1cs_sat_proof, inst_evals, r1cs_eval_proof); }
 };
-// ComputationCommitment { R1CSCommitment { .., SparseMatPolyCommitment } } (r1cs.rs:49-55, sparse_mlpoly.rs:319-327)
-struct ComputationCommitment {
-  size_t num_cons = 0, num_vars = 0, num_inputs = 0;
+// SparseMatPolyCommitment (sparse_mlpoly.rs:319-327)
+struct SparseMatPolyCommitment {
   size_t batch_size = 0, num_ops = 0, num_mem_cells = 0;
   PolyCommitment comm_comb_ops, comm_comb_mem;
-  template <class A> void io(A& a) { a(num_cons, num_vars, num_inputs, batch_size, num_ops, num_mem_cells, comm_comb_ops, comm_comb_mem); }
+  template <class A> void io(A& a) { a(batch_size, num_ops, num_mem_cells, comm_comb_ops, comm_comb_mem); }
+};
+// ComputationCommitment { R1CSCommitment { .., SparseMatPolyCommitment } } (r1cs.rs:49-55): bincode has no framing, so the nesting adds no bytes
+struct ComputationCommitment {
+  size_t num_cons = 0, num_vars = 0, num_inputs = 0;
+  SparseMatPolyCommitment comm;
+  template <class A> void io(A& a) { a(num_cons, num_vars, num_inputs, comm); }
 };
 
 }  // namespace sp
