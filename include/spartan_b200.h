@@ -257,6 +257,62 @@ int sp_pc_eval_prove_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, sp_poly* const
 int sp_pc_eval_verify_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t* comm, size_t comm_len, const uint64_t* r_mont, size_t m,
                               const uint64_t* evals_mont, int k, uint8_t* strobe_state /* in, out */, const uint8_t* proof, size_t proof_len);
 
+/* ---- zero-knowledge sumchecks of a caller-defined polynomial and the sigma protocols that tie committed claims together (sumcheck.rs:64-776,
+ * nizk/mod.rs:16-406), on the caller's transcript and tape (both advanced, and written back only when a prove succeeds) and the caller's
+ * MultiCommitGens: gens_1 has n = 1, gens_n the n the proof needs; the two may be different sets (sp_gens_create, or sp_gens_upload of the
+ * split_at views the reference uses, e.g. gens_pc.gens.gens_1 = [G_n, h]).  Commitments cross as 32-byte ristretto255 encodings.  Bytes equal
+ * the reference's for the same transcript, tape and generators.  Every argument is checked before the first launch, tape draw or transcript
+ * write, so a refused call leaves the tables, the transcript and the tape byte-identical.  SP_ERR_INVALID_ARG: gens_1.n != 1, a gens_n.n other
+ * than the proof's length, a handle of another context, a NULL argument; SP_ERR_INVALID_SCALAR: an unreduced scalar; SP_ERR_INVALID_POINT: a
+ * commitment given to a verify that does not decompress.  The verifies return SP_OK when they accept, SP_ERR_VERIFY / SP_ERR_DECOMPRESS when they
+ * reject (sp_last_error names the check), and leave the transcript where the reference's verify leaves it.  The sigma protocols commit on the
+ * host; each set's host tables are built at its first such use.  On a connected multi-GPU context every entry runs on this rank's GPU alone. */
+/* DotProductProof is linear in n: n <= SP_DOTPROD_MAX_N (a ZK sumcheck's rounds need d + 1 <= 7); longer vectors belong to PolyEvalProof */
+#define SP_DOTPROD_MAX_N 64
+/* ZKSumcheckInstanceProof::prove_quad / prove_cubic_with_additive_term (sumcheck.rs:428-776) generalised to the composition of
+ * sp_sumcheck_prove_t (same tables, terms, num_rounds and refusals; degree d = max nfactors, 1 <= d <= SP_SC_MAX_DEGREE).  The tape draws
+ * blinds_poly and blinds_evals (num_rounds each), then per round d_vec, r_delta, r_beta.  Round j: s_j(0), s_j(2) .. s_j(d) on the device, s_j(1) =
+ * claim_j - s_j(0), coefficients as sp_sumcheck_prove_t's; comm_poly = commit(coeffs; blinds_poly[j]; gens_n) absorbed, r_j drawn, then
+ * comm_claim_per_round, comm_eval = commit(s_j(r_j); blinds_evals[j]; gens_1), the weights w ("combine_two_claims_to_one") and
+ * DotProductProof::prove with a = w0 (2, 1, .., 1) + w1 (1, r_j, .., r_j^d).  At d = 2 with A*B, and at d = 3 with A*B*C - A*D, the bytes are the
+ * reference's two provers'.  gens_n.n must be d + 1.  Out: *proof = bincode(ZKSumcheckInstanceProof) (free with sp_free), r_out, finals_out as
+ * sp_sumcheck_prove_t's, blind_post_out = blinds_evals[num_rounds - 1] (the blind of the last comm_eval).  One kernel launch per round plus a
+ * constant, once gens_1 and gens_n have their host tables (the first call on a set builds them, with launches of their own); no table data
+ * reaches the host.  num_rounds is also capped by the pinned area that stages the rounds' tape-only commitments (SP_ERR_INVALID_ARG names the
+ * limit, over 200 rounds). */
+int sp_zk_sumcheck_prove_t(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim_mont[4],
+                           const uint64_t blind_claim_mont[4], size_t num_rounds, const sp_gens* gens_1, const sp_gens* gens_n,
+                           uint8_t* strobe_state /* in, out */, uint8_t* tape_state /* in, out */, uint8_t** proof, size_t* proof_len,
+                           uint64_t* r_out /* num_rounds x 4 */, uint64_t* finals_out /* k x 4 */, uint64_t blind_post_out[4]);
+/* ZKSumcheckInstanceProof::verify(comm_claim, num_rounds, degree_bound, gens_1, gens_n, transcript) (sumcheck.rs:84-179): num_rounds >= 1,
+ * gens_n.n = degree_bound + 1 <= SP_DOTPROD_MAX_N.  On success comm_eval_out32 = the last comm_eval, r_out = the num_rounds challenges. */
+int sp_zk_sumcheck_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const uint8_t comm_claim32[32], size_t num_rounds, size_t degree_bound,
+                            const sp_gens* gens_1, const sp_gens* gens_n, uint8_t* strobe_state /* in, out */, uint8_t comm_eval_out32[32],
+                            uint64_t* r_out /* num_rounds x 4 */);
+/* KnowledgeProof::prove(gens_n, transcript, tape, x, r) -> (proof, C)  /  ::verify(gens_n, transcript, C)        nizk/mod.rs:27-75; gens_n.n = 1 */
+int sp_knowledge_prove_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state, uint8_t* tape_state, const uint64_t x_mont[4], const uint64_t r_mont[4],
+                         uint8_t** proof, size_t* proof_len, uint8_t C_out32[32]);
+int sp_knowledge_verify_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state, const uint8_t C32[32], const uint8_t* proof, size_t proof_len);
+/* EqualityProof::prove(gens_n, transcript, tape, v1, s1, v2, s2) -> (proof, C1, C2)  /  ::verify(gens_n, transcript, C1, C2)   :88-143; n = 1 */
+int sp_equality_prove_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state, uint8_t* tape_state, const uint64_t v1_mont[4], const uint64_t s1_mont[4],
+                        const uint64_t v2_mont[4], const uint64_t s2_mont[4], uint8_t** proof, size_t* proof_len, uint8_t C1_out32[32], uint8_t C2_out32[32]);
+int sp_equality_verify_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state, const uint8_t C1_32[32], const uint8_t C2_32[32], const uint8_t* proof,
+                         size_t proof_len);
+/* ProductProof::prove(gens_n, transcript, tape, x, rX, y, rY, z, rZ) -> (proof, X, Y, Z)  /  ::verify(gens_n, transcript, X, Y, Z)
+ *                                                                                                                     :159-290; n = 1 */
+int sp_product_prove_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state, uint8_t* tape_state, const uint64_t x_mont[4], const uint64_t rX_mont[4],
+                       const uint64_t y_mont[4], const uint64_t rY_mont[4], const uint64_t z_mont[4], const uint64_t rZ_mont[4], uint8_t** proof,
+                       size_t* proof_len, uint8_t X_out32[32], uint8_t Y_out32[32], uint8_t Z_out32[32]);
+int sp_product_verify_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state, const uint8_t X32[32], const uint8_t Y32[32], const uint8_t Z32[32],
+                        const uint8_t* proof, size_t proof_len);
+/* DotProductProof::prove(gens_1, gens_n, transcript, tape, x_vec, blind_x, a_vec, y, blind_y) -> (proof, Cx, Cy)  /
+ * ::verify(gens_1, gens_n, transcript, a_vec, Cx, Cy)                              :311-405; vectors of n = gens_n.n <= SP_DOTPROD_MAX_N entries */
+int sp_dotproduct_prove_t(sp_ctx* ctx, const sp_gens* gens_1, const sp_gens* gens_n, uint8_t* strobe_state, uint8_t* tape_state, const uint64_t* x_vec_mont,
+                          const uint64_t blind_x_mont[4], const uint64_t* a_vec_mont, size_t n, const uint64_t y_mont[4], const uint64_t blind_y_mont[4],
+                          uint8_t** proof, size_t* proof_len, uint8_t Cx_out32[32], uint8_t Cy_out32[32]);
+int sp_dotproduct_verify_t(sp_ctx* ctx, const sp_gens* gens_1, const sp_gens* gens_n, uint8_t* strobe_state, const uint64_t* a_vec_mont, size_t n,
+                           const uint8_t Cx32[32], const uint8_t Cy32[32], const uint8_t* proof, size_t proof_len);
+
 /* ---- product circuits over the caller's tables and the batched proof of their products: the grand-product argument of the reference's memory
  * check (ProductCircuit, ProductCircuitEvalProofBatched, product_tree.rs), bytes identical to the reference's for the same transcript.  Use, e.g.
  * for an offline memory check, multiset equality or a lookup argument: commit to the tuple tables (sp_pc_commit), draw the fingerprint

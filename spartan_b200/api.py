@@ -721,6 +721,134 @@ class PolyEvalProof:
                                                      t.state, C.c_char_p(self.data), _sz(len(self.data))))
 
 
+# ----------------------------------------------------------------------------- zero-knowledge sumchecks and sigma protocols
+SP_DOTPROD_MAX_N = 64
+
+
+def _scalar(x):
+    return _p(np.ascontiguousarray(x, dtype=np.uint64).reshape(4))
+
+
+def _point(c):
+    c = bytes(c)
+    if len(c) != 32:
+        raise SpartanB200Error("a commitment is 32 bytes, got %d" % len(c))
+    return C.c_char_p(c)
+
+
+class ZKSumcheckInstanceProof:
+    """sumcheck.rs:64-776: the zero-knowledge sumcheck of a Composition over DensePolynomials (bound in place), every round polynomial and
+    evaluation hidden in a Pedersen commitment and tied together by a DotProductProof.  `data` = bincode(ZKSumcheckInstanceProof).  Scalars are
+    Montgomery limbs, commitments 32-byte encodings; gens_1 / gens_n are MultiCommitGens with n = 1 and n = degree + 1."""
+
+    def __init__(self, data):
+        self.data = bytes(data)
+
+    @staticmethod
+    def prove(polys, comp, claim, blind_claim, num_rounds, gens_1, gens_n, transcript, tape):
+        """prove_quad / prove_cubic_with_additive_term for any composition: returns (proof, r as (num_rounds, 4) limbs, finals as (k, 4) limbs,
+        blind_post = the blind of the last comm_eval)"""
+        ctx = polys[0].ctx
+        terms = comp._c_terms()
+        out, n = C.POINTER(C.c_ubyte)(), _sz()
+        r = np.zeros((num_rounds, 4), dtype=np.uint64)
+        finals = np.zeros((len(polys), 4), dtype=np.uint64)
+        blind_post = np.zeros(4, dtype=np.uint64)
+        ctx.check(lib.sp_zk_sumcheck_prove_t(ctx.h, _handles(polys), C.c_int(len(polys)), terms, C.c_int(len(comp.terms)), _scalar(claim),
+                                             _scalar(blind_claim), _sz(num_rounds), gens_1.h, gens_n.h, transcript.state, tape.state, C.byref(out),
+                                             C.byref(n), _p(r), _p(finals), _p(blind_post)))
+        return ZKSumcheckInstanceProof(_take_bytes(out, n)), r, finals, blind_post
+
+    def verify(self, comm_claim, num_rounds, degree_bound, gens_1, gens_n, transcript):
+        """sumcheck.rs:84-179: returns (comm_eval = the last round's commitment, r); raises ProofVerifyError"""
+        ctx = gens_1.ctx
+        comm_eval = C.create_string_buffer(32)
+        r = np.zeros((max(num_rounds, 1), 4), dtype=np.uint64)
+        ctx.check(lib.sp_zk_sumcheck_verify_t(ctx.h, C.c_char_p(self.data), _sz(len(self.data)), _point(comm_claim), _sz(num_rounds), _sz(degree_bound),
+                                              gens_1.h, gens_n.h, transcript.state, comm_eval, _p(r)))
+        return comm_eval.raw, r[:num_rounds]
+
+
+class KnowledgeProof:
+    """nizk/mod.rs:16-75: knowledge of the opening (x, r) of C = x*G + r*h"""
+
+    def __init__(self, data):
+        self.data = bytes(data)
+
+    @staticmethod
+    def prove(gens_n, transcript, tape, x, r):
+        """returns (proof, C)"""
+        out, n, Cc = C.POINTER(C.c_ubyte)(), _sz(), C.create_string_buffer(32)
+        gens_n.ctx.check(lib.sp_knowledge_prove_t(gens_n.ctx.h, gens_n.h, transcript.state, tape.state, _scalar(x), _scalar(r), C.byref(out), C.byref(n),
+                                                  Cc))
+        return KnowledgeProof(_take_bytes(out, n)), Cc.raw
+
+    def verify(self, gens_n, transcript, C_):
+        gens_n.ctx.check(lib.sp_knowledge_verify_t(gens_n.ctx.h, gens_n.h, transcript.state, _point(C_), C.c_char_p(self.data), _sz(len(self.data))))
+
+
+class EqualityProof:
+    """nizk/mod.rs:78-143: C1 = v*G + s1*h and C2 = v*G + s2*h open to the same v"""
+
+    def __init__(self, data):
+        self.data = bytes(data)
+
+    @staticmethod
+    def prove(gens_n, transcript, tape, v1, s1, v2, s2):
+        """returns (proof, C1, C2)"""
+        out, n, c1, c2 = C.POINTER(C.c_ubyte)(), _sz(), C.create_string_buffer(32), C.create_string_buffer(32)
+        gens_n.ctx.check(lib.sp_equality_prove_t(gens_n.ctx.h, gens_n.h, transcript.state, tape.state, _scalar(v1), _scalar(s1), _scalar(v2), _scalar(s2),
+                                                 C.byref(out), C.byref(n), c1, c2))
+        return EqualityProof(_take_bytes(out, n)), c1.raw, c2.raw
+
+    def verify(self, gens_n, transcript, C1, C2):
+        gens_n.ctx.check(lib.sp_equality_verify_t(gens_n.ctx.h, gens_n.h, transcript.state, _point(C1), _point(C2), C.c_char_p(self.data),
+                                                  _sz(len(self.data))))
+
+
+class ProductProof:
+    """nizk/mod.rs:147-290: X, Y, Z commit to x, y and z = x*y"""
+
+    def __init__(self, data):
+        self.data = bytes(data)
+
+    @staticmethod
+    def prove(gens_n, transcript, tape, x, rX, y, rY, z, rZ):
+        """returns (proof, X, Y, Z)"""
+        out, n = C.POINTER(C.c_ubyte)(), _sz()
+        X, Y, Z = C.create_string_buffer(32), C.create_string_buffer(32), C.create_string_buffer(32)
+        gens_n.ctx.check(lib.sp_product_prove_t(gens_n.ctx.h, gens_n.h, transcript.state, tape.state, _scalar(x), _scalar(rX), _scalar(y), _scalar(rY),
+                                                _scalar(z), _scalar(rZ), C.byref(out), C.byref(n), X, Y, Z))
+        return ProductProof(_take_bytes(out, n)), X.raw, Y.raw, Z.raw
+
+    def verify(self, gens_n, transcript, X, Y, Z):
+        gens_n.ctx.check(lib.sp_product_verify_t(gens_n.ctx.h, gens_n.h, transcript.state, _point(X), _point(Y), _point(Z), C.c_char_p(self.data),
+                                                 _sz(len(self.data))))
+
+
+class DotProductProof:
+    """nizk/mod.rs:293-406: Cx commits to x_vec, Cy to y = <a_vec, x_vec>; vectors of gens_n.n <= SP_DOTPROD_MAX_N entries"""
+
+    def __init__(self, data):
+        self.data = bytes(data)
+
+    @staticmethod
+    def prove(gens_1, gens_n, transcript, tape, x_vec, blind_x, a_vec, y, blind_y):
+        """returns (proof, Cx, Cy)"""
+        x, a = _limbs(x_vec), _limbs(a_vec)
+        if len(x) != len(a):
+            raise SpartanB200Error("DotProductProof: x_vec has %d entries, a_vec %d" % (len(x), len(a)))
+        out, n, cx, cy = C.POINTER(C.c_ubyte)(), _sz(), C.create_string_buffer(32), C.create_string_buffer(32)
+        gens_1.ctx.check(lib.sp_dotproduct_prove_t(gens_1.ctx.h, gens_1.h, gens_n.h, transcript.state, tape.state, _p(x), _scalar(blind_x), _p(a),
+                                                   _sz(len(x)), _scalar(y), _scalar(blind_y), C.byref(out), C.byref(n), cx, cy))
+        return DotProductProof(_take_bytes(out, n)), cx.raw, cy.raw
+
+    def verify(self, gens_1, gens_n, transcript, a, Cx, Cy):
+        a = _limbs(a)
+        gens_1.ctx.check(lib.sp_dotproduct_verify_t(gens_1.ctx.h, gens_1.h, gens_n.h, transcript.state, _p(a), _sz(len(a)), _point(Cx), _point(Cy),
+                                                    C.c_char_p(self.data), _sz(len(self.data))))
+
+
 # ----------------------------------------------------------------------------- product circuits of the caller's tables
 SP_PROD_MAX_CIRCUITS, SP_PROD_MAX_SOURCES = 24, 3
 

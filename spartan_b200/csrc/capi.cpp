@@ -1167,6 +1167,48 @@ int sp_snark_verify_t(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t
 }
 // ---- a whole sumcheck of a caller-defined polynomial (prover.cpp: poly_sumcheck_prove).  Every argument is checked before the first launch, so a
 // refused call leaves the tables as they were.
+// The checked polynomial of the caller's tables and terms: P.t holds the distinct tables (a handle passed twice is one table, bound once per round),
+// slot[i] the distinct table of index i
+struct CallerPoly { dev::ScPoly P; size_t len; std::vector<sp_poly*> distinct; std::vector<uint8_t> slot; };
+static CallerPoly caller_poly(const sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, size_t num_rounds, const std::string& what) {
+  require_count(what, k, "tables", "SP_SC_MAX_TABLES", SP_SC_MAX_TABLES);
+  require_count(what, nterms, "terms", "SP_SC_MAX_TERMS", SP_SC_MAX_TERMS);
+  CallerPoly cp;
+  cp.len = caller_tables(ctx, tables, k, what, 2).len;
+  const size_t m = log2_ceil(cp.len);
+  if (num_rounds < 1 || num_rounds > m)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": num_rounds = " + std::to_string(num_rounds) + " outside 1 .. " + std::to_string(m) + " (the tables' variables)");
+  dev::ScPoly& P = cp.P;
+  memset(static_cast<void*>(&P), 0, sizeof P);
+  cp.slot.resize(k);
+  for (int i = 0; i < k; i++) {
+    const size_t at = std::find(cp.distinct.begin(), cp.distinct.end(), tables[i]) - cp.distinct.begin();
+    if (at == cp.distinct.size()) { cp.distinct.push_back(tables[i]); P.t[at] = tables[i]->d.p; }
+    cp.slot[i] = (uint8_t)at;
+  }
+  P.ntables = (int)cp.distinct.size();
+  P.nterms = nterms;
+  const Fq one = Fq::one();
+  const std::string coeff_what = what + ": coefficient";
+  for (int t = 0; t < nterms; t++) {
+    const sp_sc_term& tm = terms[t];
+    const std::string at = what + ": term " + std::to_string(t);
+    if (tm.nfactors == 0) throw SpError(SP_ERR_INVALID_ARG, at + " has no factors");
+    if (tm.nfactors > SP_SC_MAX_DEGREE)
+      throw SpError(SP_ERR_INVALID_ARG, at + " has " + std::to_string(tm.nfactors) + " factors; degree <= SP_SC_MAX_DEGREE = " + std::to_string(SP_SC_MAX_DEGREE) + " supported");
+    for (uint32_t f = 0; f < tm.nfactors; f++) {
+      if (tm.factor[f] >= (uint32_t)k) throw SpError(SP_ERR_INVALID_ARG, at + ": table index " + std::to_string(tm.factor[f]) + " >= k = " + std::to_string(k));
+      P.fac[t][f] = cp.slot[tm.factor[f]];
+    }
+    require_reduced(tm.coeff_mont, 1, coeff_what.c_str());
+    const Fq c = fq_in(tm.coeff_mont);
+    P.coeff[t] = c.m;
+    P.unit[t] = c == one;
+    P.nfac[t] = (uint8_t)tm.nfactors;
+    P.degree = std::max(P.degree, (int)tm.nfactors);
+  }
+  return cp;
+}
 static int sumcheck_prove_common(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim[4],
                                  size_t num_rounds, const TranscriptArg& ta, uint8_t** proof, size_t* proof_len, uint64_t* r_out, uint64_t* finals_out,
                                  uint64_t e_out[4]) {
@@ -1174,51 +1216,18 @@ static int sumcheck_prove_common(sp_ctx* ctx, sp_poly* const* tables, int k, con
     const std::string what = "sumcheck_prove";
     ta.check();
     if (!tables || !terms || !claim || !proof || !proof_len || !r_out || !finals_out || !e_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
-    require_count(what, k, "tables", "SP_SC_MAX_TABLES", SP_SC_MAX_TABLES);
-    require_count(what, nterms, "terms", "SP_SC_MAX_TERMS", SP_SC_MAX_TERMS);
-    const size_t len = caller_tables(ctx, tables, k, what, 2).len, m = log2_ceil(len);
-    if (num_rounds < 1 || num_rounds > m)
-      throw SpError(SP_ERR_INVALID_ARG, what + ": num_rounds = " + std::to_string(num_rounds) + " outside 1 .. " + std::to_string(m) + " (the tables' variables)");
-    dev::ScPoly P;
-    memset(static_cast<void*>(&P), 0, sizeof P);
-    std::vector<sp_poly*> distinct;   // a handle passed twice is one table, bound once per round
-    std::vector<uint8_t> slot(k);
-    for (int i = 0; i < k; i++) {
-      const size_t at = std::find(distinct.begin(), distinct.end(), tables[i]) - distinct.begin();
-      if (at == distinct.size()) { distinct.push_back(tables[i]); P.t[at] = tables[i]->d.p; }
-      slot[i] = (uint8_t)at;
-    }
-    P.ntables = (int)distinct.size();
-    P.nterms = nterms;
-    const Fq one = Fq::one();
-    for (int t = 0; t < nterms; t++) {
-      const sp_sc_term& tm = terms[t];
-      const std::string at = what + ": term " + std::to_string(t);
-      if (tm.nfactors == 0) throw SpError(SP_ERR_INVALID_ARG, at + " has no factors");
-      if (tm.nfactors > SP_SC_MAX_DEGREE)
-        throw SpError(SP_ERR_INVALID_ARG, at + " has " + std::to_string(tm.nfactors) + " factors; degree <= SP_SC_MAX_DEGREE = " + std::to_string(SP_SC_MAX_DEGREE) + " supported");
-      for (uint32_t f = 0; f < tm.nfactors; f++) {
-        if (tm.factor[f] >= (uint32_t)k) throw SpError(SP_ERR_INVALID_ARG, at + ": table index " + std::to_string(tm.factor[f]) + " >= k = " + std::to_string(k));
-        P.fac[t][f] = slot[tm.factor[f]];
-      }
-      require_reduced(tm.coeff_mont, 1, "sumcheck_prove: coefficient");
-      const Fq c = fq_in(tm.coeff_mont);
-      P.coeff[t] = c.m;
-      P.unit[t] = c == one;
-      P.nfac[t] = (uint8_t)tm.nfactors;
-      P.degree = std::max(P.degree, (int)tm.nfactors);
-    }
+    const CallerPoly cp = caller_poly(ctx, tables, k, terms, nterms, num_rounds, what);
     require_reduced(claim, 1, "sumcheck_prove: claim");
     Transcript T = ta.open();
     SumcheckInstanceProof pr;
     std::vector<Fq> r, finals;
     Fq e;
-    poly_sumcheck_prove(ctx->c, P, len, fq_in(claim), num_rounds, T, pr, r, finals, e);
-    for (sp_poly* p : distinct) p->len >>= num_rounds;
+    poly_sumcheck_prove(ctx->c, cp.P, cp.len, fq_in(claim), num_rounds, T, pr, r, finals, e);
+    for (sp_poly* p : cp.distinct) p->len >>= num_rounds;
     ta.close(T);
     put_bytes(proof, proof_len, to_bincode(pr));
     put_scalars(r_out, r);
-    for (int i = 0; i < k; i++) fq_out(finals_out + 4 * i, finals[slot[i]]);
+    for (int i = 0; i < k; i++) fq_out(finals_out + 4 * i, finals[cp.slot[i]]);
     fq_out(e_out, e);
   });
 }
@@ -1245,6 +1254,269 @@ int sp_sumcheck_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, co
     std::vector<Fq> r;
     fq_out(e_out, sumcheck_verify_bytes(proof, proof_len, fq_in(claim), num_rounds, degree_bound, T, r));
     put_scalars(r_out, r);
+  });
+}
+
+// ---- ZK sumchecks of a caller-defined polynomial and the sigma protocols (nizk/mod.rs), on the caller's transcript and tape and the caller's
+// MultiCommitGens (sp_gens: G[0..n), h = G[n]).  Every argument is checked before the first launch, tape draw or transcript write, so a refused
+// call leaves the tables, the transcript and the tape as they were.
+static CommitKey gens_key(const sp_ctx* ctx, const sp_gens* g, const std::string& what, const char* name) {
+  if (!g) throw SpError(SP_ERR_INVALID_ARG, what + ": " + name + " is NULL");
+  if (g->set->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, what + ": " + name + " belongs to another context");
+  return CommitKey{g->set.get(), 0, g->n, g->n};
+}
+static void require_gens_n(const CommitKey& k, size_t n, const std::string& what, const char* name, const std::string& why) {
+  if (k.n != n) throw SpError(SP_ERR_INVALID_ARG, what + ": " + name + ".n = " + std::to_string(k.n) + " but " + why + " needs " + std::to_string(n));
+}
+// the host copies of every generator and h of the sets the call commits against, built once per set (after the checks)
+static void gens_host_tables(const sp_gens* g) {
+  std::vector<size_t> b(g->n + 1);
+  for (size_t i = 0; i <= g->n; i++) b[i] = i;
+  g->set->add_host_tables(b);
+}
+static Cp cp_in(const uint8_t* p32, const std::string& what) {
+  if (!p32) throw SpError(SP_ERR_INVALID_ARG, what + " is NULL");
+  point_in(p32, what.c_str());   // SP_ERR_INVALID_POINT unless it decompresses
+  Cp c;
+  memcpy(c.b, p32, 32);
+  return c;
+}
+static Fq scalar_in(const uint64_t* l, const std::string& what) {
+  if (!l) throw SpError(SP_ERR_INVALID_ARG, what + " is NULL");
+  require_reduced(l, 1, what.c_str());
+  return fq_in(l);
+}
+static void cp_out(uint8_t* out32, const Cp& c) { if (out32) memcpy(out32, c.b, 32); }
+// a prove entry's transcript and tape: both opened after the checks, both written back on success only
+struct ProveStates {
+  const TranscriptArg ta;
+  uint8_t* tape_state;
+  ProveStates(uint8_t* strobe_state, uint8_t* tape, const std::string& what) : ta(TranscriptArg::caller(strobe_state)), tape_state(tape) {
+    ta.check();
+    if (!tape_state) throw SpError(SP_ERR_INVALID_ARG, what + ": tape state is NULL");
+  }
+};
+
+int sp_zk_sumcheck_prove_t(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim[4],
+                           const uint64_t blind_claim[4], size_t num_rounds, const sp_gens* gens_1, const sp_gens* gens_n, uint8_t* strobe_state,
+                           uint8_t* tape_state, uint8_t** proof, size_t* proof_len, uint64_t* r_out, uint64_t* finals_out, uint64_t blind_post_out[4]) {
+  return guarded(ctx, [&] {
+    const std::string what = "zk_sumcheck_prove";
+    const ProveStates st(strobe_state, tape_state, what);
+    if (!tables || !terms || !proof || !proof_len || !r_out || !finals_out || !blind_post_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    const CallerPoly cp = caller_poly(ctx, tables, k, terms, nterms, num_rounds, what);
+    if (num_rounds > zk_sumcheck_max_rounds())
+      throw SpError(SP_ERR_INVALID_ARG, what + ": num_rounds = " + std::to_string(num_rounds) + " > " + std::to_string(zk_sumcheck_max_rounds()) +
+                                            ", the rounds a ZK sumcheck stages");
+    const CommitKey g1 = gens_key(ctx, gens_1, what, "gens_1"), gn = gens_key(ctx, gens_n, what, "gens_n");
+    require_gens_n(g1, 1, what, "gens_1", "a claim's commitment");
+    require_gens_n(gn, (size_t)cp.P.degree + 1, what, "gens_n", "a round polynomial of degree " + std::to_string(cp.P.degree));
+    const Fq c = scalar_in(claim, what + ": claim"), bc = scalar_in(blind_claim, what + ": blind_claim");
+    gens_host_tables(gens_1);
+    gens_host_tables(gens_n);
+    Transcript T = st.ta.open();
+    RandomTape tape(pc_tape_open(tape_state, what));
+    ZKSumcheckInstanceProof pr;
+    std::vector<Fq> r, finals;
+    Fq blind_post;
+    zk_poly_sumcheck_prove(ctx->c, cp.P, cp.len, c, bc, num_rounds, g1, gn, T, tape, pr, r, finals, blind_post);
+    for (sp_poly* p : cp.distinct) p->len >>= num_rounds;
+    st.ta.close(T);
+    tape.state().export_state(tape_state);
+    put_bytes(proof, proof_len, to_bincode(pr));
+    put_scalars(r_out, r);
+    for (int i = 0; i < k; i++) fq_out(finals_out + 4 * i, finals[cp.slot[i]]);
+    fq_out(blind_post_out, blind_post);
+  });
+}
+int sp_zk_sumcheck_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const uint8_t comm_claim32[32], size_t num_rounds, size_t degree_bound,
+                            const sp_gens* gens_1, const sp_gens* gens_n, uint8_t* strobe_state, uint8_t comm_eval_out32[32], uint64_t* r_out) {
+  return guarded(ctx, [&] {
+    const std::string what = "zk_sumcheck_verify";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if ((!proof && proof_len) || !comm_eval_out32 || !r_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    if (num_rounds < 1) throw SpError(SP_ERR_INVALID_ARG, what + ": num_rounds must be >= 1");
+    if (degree_bound < 1 || degree_bound + 1 > SP_DOTPROD_MAX_N)
+      throw SpError(SP_ERR_INVALID_ARG, what + ": degree_bound = " + std::to_string(degree_bound) + " outside 1 .. SP_DOTPROD_MAX_N - 1 = " + std::to_string(SP_DOTPROD_MAX_N - 1));
+    const CommitKey g1 = gens_key(ctx, gens_1, what, "gens_1"), gn = gens_key(ctx, gens_n, what, "gens_n");
+    require_gens_n(g1, 1, what, "gens_1", "a claim's commitment");
+    require_gens_n(gn, degree_bound + 1, what, "gens_n", "degree_bound = " + std::to_string(degree_bound));
+    const Cp cc = cp_in(comm_claim32, what + ": comm_claim");
+    gens_host_tables(gens_1);
+    gens_host_tables(gens_n);
+    Transcript T = ta.open();
+    TranscriptClose close{ta, T};
+    std::vector<Fq> r;
+    cp_out(comm_eval_out32, zk_sumcheck_verify_bytes(ctx->c, proof, proof_len, cc, num_rounds, degree_bound, g1, gn, T, r));
+    put_scalars(r_out, r);
+  });
+}
+
+int sp_knowledge_prove_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state, uint8_t* tape_state, const uint64_t x[4], const uint64_t r[4],
+                         uint8_t** proof, size_t* proof_len, uint8_t C_out32[32]) {
+  return guarded(ctx, [&] {
+    const std::string what = "knowledge_prove";
+    const ProveStates st(strobe_state, tape_state, what);
+    if (!proof || !proof_len || !C_out32) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    const CommitKey g = gens_key(ctx, gens_n, what, "gens_n");
+    require_gens_n(g, 1, what, "gens_n", "a scalar's commitment");
+    const Fq fx = scalar_in(x, what + ": x"), fr = scalar_in(r, what + ": r");
+    gens_host_tables(gens_n);
+    Transcript T = st.ta.open();
+    RandomTape tape(pc_tape_open(tape_state, what));
+    Cp C;
+    const KnowledgeProof p = knowledge_prove(g, T, tape, fx, fr, C);
+    st.ta.close(T);
+    tape.state().export_state(tape_state);
+    put_bytes(proof, proof_len, to_bincode(p));
+    cp_out(C_out32, C);
+  });
+}
+int sp_knowledge_verify_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state, const uint8_t C32[32], const uint8_t* proof, size_t proof_len) {
+  return guarded(ctx, [&] {
+    const std::string what = "knowledge_verify";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if (!proof && proof_len) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    const CommitKey g = gens_key(ctx, gens_n, what, "gens_n");
+    require_gens_n(g, 1, what, "gens_n", "a scalar's commitment");
+    const Cp C = cp_in(C32, what + ": C");
+    gens_host_tables(gens_n);
+    Transcript T = ta.open();
+    TranscriptClose close{ta, T};
+    knowledge_verify_bytes(ctx->c, g, T, C, proof, proof_len);
+  });
+}
+
+int sp_equality_prove_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state, uint8_t* tape_state, const uint64_t v1[4], const uint64_t s1[4],
+                        const uint64_t v2[4], const uint64_t s2[4], uint8_t** proof, size_t* proof_len, uint8_t C1_out32[32], uint8_t C2_out32[32]) {
+  return guarded(ctx, [&] {
+    const std::string what = "equality_prove";
+    const ProveStates st(strobe_state, tape_state, what);
+    if (!proof || !proof_len || !C1_out32 || !C2_out32) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    const CommitKey g = gens_key(ctx, gens_n, what, "gens_n");
+    require_gens_n(g, 1, what, "gens_n", "a scalar's commitment");
+    const Fq a1 = scalar_in(v1, what + ": v1"), b1 = scalar_in(s1, what + ": s1"), a2 = scalar_in(v2, what + ": v2"), b2 = scalar_in(s2, what + ": s2");
+    gens_host_tables(gens_n);
+    Transcript T = st.ta.open();
+    RandomTape tape(pc_tape_open(tape_state, what));
+    Cp C1, C2;
+    const EqualityProof p = equality_prove(g, T, tape, a1, b1, a2, b2, &C1, &C2);
+    st.ta.close(T);
+    tape.state().export_state(tape_state);
+    put_bytes(proof, proof_len, to_bincode(p));
+    cp_out(C1_out32, C1);
+    cp_out(C2_out32, C2);
+  });
+}
+int sp_equality_verify_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state, const uint8_t C1_32[32], const uint8_t C2_32[32], const uint8_t* proof,
+                         size_t proof_len) {
+  return guarded(ctx, [&] {
+    const std::string what = "equality_verify";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if (!proof && proof_len) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    const CommitKey g = gens_key(ctx, gens_n, what, "gens_n");
+    require_gens_n(g, 1, what, "gens_n", "a scalar's commitment");
+    const Cp C1 = cp_in(C1_32, what + ": C1"), C2 = cp_in(C2_32, what + ": C2");
+    gens_host_tables(gens_n);
+    Transcript T = ta.open();
+    TranscriptClose close{ta, T};
+    equality_verify_bytes(ctx->c, g, T, C1, C2, proof, proof_len);
+  });
+}
+
+int sp_product_prove_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state, uint8_t* tape_state, const uint64_t x[4], const uint64_t rX[4],
+                       const uint64_t y[4], const uint64_t rY[4], const uint64_t z[4], const uint64_t rZ[4], uint8_t** proof, size_t* proof_len,
+                       uint8_t X_out32[32], uint8_t Y_out32[32], uint8_t Z_out32[32]) {
+  return guarded(ctx, [&] {
+    const std::string what = "product_prove";
+    const ProveStates st(strobe_state, tape_state, what);
+    if (!proof || !proof_len || !X_out32 || !Y_out32 || !Z_out32) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    const CommitKey g = gens_key(ctx, gens_n, what, "gens_n");
+    require_gens_n(g, 1, what, "gens_n", "a scalar's commitment");
+    const Fq fx = scalar_in(x, what + ": x"), frX = scalar_in(rX, what + ": rX"), fy = scalar_in(y, what + ": y"), frY = scalar_in(rY, what + ": rY"),
+             fz = scalar_in(z, what + ": z"), frZ = scalar_in(rZ, what + ": rZ");
+    gens_host_tables(gens_n);
+    Transcript T = st.ta.open();
+    RandomTape tape(pc_tape_open(tape_state, what));
+    Cp X, Y, Z;
+    const ProductProof p = product_prove(g, T, tape, fx, frX, fy, frY, fz, frZ, X, Y, Z);
+    st.ta.close(T);
+    tape.state().export_state(tape_state);
+    put_bytes(proof, proof_len, to_bincode(p));
+    cp_out(X_out32, X);
+    cp_out(Y_out32, Y);
+    cp_out(Z_out32, Z);
+  });
+}
+int sp_product_verify_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state, const uint8_t X32[32], const uint8_t Y32[32], const uint8_t Z32[32],
+                        const uint8_t* proof, size_t proof_len) {
+  return guarded(ctx, [&] {
+    const std::string what = "product_verify";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if (!proof && proof_len) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    const CommitKey g = gens_key(ctx, gens_n, what, "gens_n");
+    require_gens_n(g, 1, what, "gens_n", "a scalar's commitment");
+    const Cp X = cp_in(X32, what + ": X"), Y = cp_in(Y32, what + ": Y"), Z = cp_in(Z32, what + ": Z");
+    gens_host_tables(gens_n);
+    Transcript T = ta.open();
+    TranscriptClose close{ta, T};
+    product_verify_bytes(ctx->c, g, T, X, Y, Z, proof, proof_len);
+  });
+}
+
+// the vectors of a DotProductProof: n = gens_n.n entries, 1 <= n <= SP_DOTPROD_MAX_N
+static void dotproduct_len(const CommitKey& g1, const CommitKey& gn, size_t n, const std::string& what) {
+  require_gens_n(g1, 1, what, "gens_1", "a scalar's commitment");
+  if (n < 1 || n > SP_DOTPROD_MAX_N)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": n = " + std::to_string(n) + " outside 1 .. SP_DOTPROD_MAX_N = " + std::to_string(SP_DOTPROD_MAX_N) +
+                                          " (longer vectors: PolyEvalProof)");
+  require_gens_n(gn, n, what, "gens_n", "vectors of length n = " + std::to_string(n));
+}
+int sp_dotproduct_prove_t(sp_ctx* ctx, const sp_gens* gens_1, const sp_gens* gens_n, uint8_t* strobe_state, uint8_t* tape_state, const uint64_t* x_vec,
+                          const uint64_t blind_x[4], const uint64_t* a_vec, size_t n, const uint64_t y[4], const uint64_t blind_y[4], uint8_t** proof,
+                          size_t* proof_len, uint8_t Cx_out32[32], uint8_t Cy_out32[32]) {
+  return guarded(ctx, [&] {
+    const std::string what = "dotproduct_prove";
+    const ProveStates st(strobe_state, tape_state, what);
+    if (!proof || !proof_len || !Cx_out32 || !Cy_out32 || !x_vec || !a_vec) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    const CommitKey g1 = gens_key(ctx, gens_1, what, "gens_1"), gn = gens_key(ctx, gens_n, what, "gens_n");
+    dotproduct_len(g1, gn, n, what);
+    require_reduced(x_vec, n, (what + ": x_vec").c_str());
+    require_reduced(a_vec, n, (what + ": a_vec").c_str());
+    const Fq bx = scalar_in(blind_x, what + ": blind_x"), fy = scalar_in(y, what + ": y"), by = scalar_in(blind_y, what + ": blind_y");
+    gens_host_tables(gens_1);
+    gens_host_tables(gens_n);
+    Transcript T = st.ta.open();
+    RandomTape tape(pc_tape_open(tape_state, what));
+    Cp Cx, Cy;
+    const DotProductProof p = dotproduct_prove(g1, gn, T, tape, fq_vec(x_vec, n), bx, fq_vec(a_vec, n), fy, by, nullptr, nullptr, &Cx, &Cy);
+    st.ta.close(T);
+    tape.state().export_state(tape_state);
+    put_bytes(proof, proof_len, to_bincode(p));
+    cp_out(Cx_out32, Cx);
+    cp_out(Cy_out32, Cy);
+  });
+}
+int sp_dotproduct_verify_t(sp_ctx* ctx, const sp_gens* gens_1, const sp_gens* gens_n, uint8_t* strobe_state, const uint64_t* a_vec, size_t n,
+                           const uint8_t Cx32[32], const uint8_t Cy32[32], const uint8_t* proof, size_t proof_len) {
+  return guarded(ctx, [&] {
+    const std::string what = "dotproduct_verify";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if ((!proof && proof_len) || !a_vec) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    const CommitKey g1 = gens_key(ctx, gens_1, what, "gens_1"), gn = gens_key(ctx, gens_n, what, "gens_n");
+    dotproduct_len(g1, gn, n, what);
+    require_reduced(a_vec, n, (what + ": a_vec").c_str());
+    const Cp Cx = cp_in(Cx32, what + ": Cx"), Cy = cp_in(Cy32, what + ": Cy");
+    gens_host_tables(gens_1);
+    gens_host_tables(gens_n);
+    Transcript T = ta.open();
+    TranscriptClose close{ta, T};
+    dotproduct_verify_bytes(ctx->c, g1, gn, T, fq_vec(a_vec, n), Cx, Cy, proof, proof_len);
   });
 }
 

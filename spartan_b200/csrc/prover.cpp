@@ -275,7 +275,7 @@ void append_nizk_head(Transcript& T, const Instance& inst) {
   T.append_message("R1CSShapeDigest", digest.data(), digest.size());
 }
 
-static KnowledgeProof knowledge_prove(const CommitKey& g, Transcript& T, RandomTape& tape, const Fq& x, const Fq& r, Cp& C_out) {  // nizk/mod.rs:27-52
+KnowledgeProof knowledge_prove(const CommitKey& g, Transcript& T, RandomTape& tape, const Fq& x, const Fq& r, Cp& C_out) {  // nizk/mod.rs:27-52
   T.append_protocol_name("knowledge proof");
   Fq t1 = tape.random_scalar("t1"), t2 = tape.random_scalar("t2");
   C_out = compress(commit1(g, x, r));
@@ -288,11 +288,14 @@ static KnowledgeProof knowledge_prove(const CommitKey& g, Transcript& T, RandomT
   p.z2 = r * c + t2;
   return p;
 }
-static EqualityProof equality_prove(const CommitKey& g, Transcript& T, RandomTape& tape, const Fq& v1, const Fq& s1, const Fq& v2, const Fq& s2) {  // :88-116
+EqualityProof equality_prove(const CommitKey& g, Transcript& T, RandomTape& tape, const Fq& v1, const Fq& s1, const Fq& v2, const Fq& s2, Cp* C1_out,
+                             Cp* C2_out) {  // :88-116
   T.append_protocol_name("equality proof");
   Fq r = tape.random_scalar("r");
   Cp C1 = compress(commit1(g, v1, s1)); T.append_point("C1", C1.b);
   Cp C2 = compress(commit1(g, v2, s2)); T.append_point("C2", C2.b);
+  if (C1_out) *C1_out = C1;
+  if (C2_out) *C2_out = C2;
   EqualityProof p;
   Term t[1] = {{g.h, r}};
   p.alpha = compress(host_commit(*g.set, t, 1));  // r * h
@@ -301,8 +304,8 @@ static EqualityProof equality_prove(const CommitKey& g, Transcript& T, RandomTap
   p.z = c * (s1 - s2) + r;
   return p;
 }
-static ProductProof product_prove(const CommitKey& g, Transcript& T, RandomTape& tape, const Fq& x, const Fq& rX, const Fq& y, const Fq& rY, const Fq& z,
-                                  const Fq& rZ, Cp& X, Cp& Y, Cp& Z) {  // nizk/mod.rs:159-229
+ProductProof product_prove(const CommitKey& g, Transcript& T, RandomTape& tape, const Fq& x, const Fq& rX, const Fq& y, const Fq& rY, const Fq& z,
+                           const Fq& rZ, Cp& X, Cp& Y, Cp& Z) {  // nizk/mod.rs:159-229
   T.append_protocol_name("product proof");
   Fq b1 = tape.random_scalar("b1"), b2 = tape.random_scalar("b2"), b3 = tape.random_scalar("b3"), b4 = tape.random_scalar("b4"), b5 = tape.random_scalar("b5");
   X = compress(commit1(g, x, rX)); T.append_point("X", X.b);
@@ -318,12 +321,9 @@ static ProductProof product_prove(const CommitKey& g, Transcript& T, RandomTape&
   p.z = {b1 + c * x, b2 + c * rX, b3 + c * y, b4 + c * rY, b5 + c * (rZ - rX * y)};
   return p;
 }
-// DotProductProof::prove (nizk/mod.rs:311-370); Cx is passed in when the caller already holds commit(x_vec; blind_x)
-// `pre` (optional): tape draws made ahead of time in the reference's order, with the commitments that depend on the tape only
-struct DotPre { std::vector<Fq> d_vec; Fq r_delta, r_beta; Cp delta; hge r_beta_h; };
-static DotProductProof dotproduct_prove(const CommitKey& g1, const CommitKey& gn, Transcript& T, RandomTape& tape, const std::vector<Fq>& x_vec,
-                                        const Fq& blind_x, const std::vector<Fq>& a_vec, const Fq& y, const Fq& blind_y, const Cp* Cx_known,
-                                        const DotPre* pre = nullptr) {
+DotProductProof dotproduct_prove(const CommitKey& g1, const CommitKey& gn, Transcript& T, RandomTape& tape, const std::vector<Fq>& x_vec,
+                                 const Fq& blind_x, const std::vector<Fq>& a_vec, const Fq& y, const Fq& blind_y, const Cp* Cx_known, const DotPre* pre,
+                                 Cp* Cx_out, Cp* Cy_out) {
   T.append_protocol_name("dot product proof");
   size_t n = x_vec.size();
   std::vector<Fq> d_vec = pre ? pre->d_vec : tape.random_vector("d_vec", n);
@@ -332,6 +332,8 @@ static DotProductProof dotproduct_prove(const CommitKey& g1, const CommitKey& gn
   T.append_point("Cx", Cx.b);
   Cp Cy = compress(commit1(g1, y, blind_y));
   T.append_point("Cy", Cy.b);
+  if (Cx_out) *Cx_out = Cx;
+  if (Cy_out) *Cy_out = Cy;
   T.append_scalars("a", a_vec);
   DotProductProof p;
   p.delta = pre ? pre->delta : compress(commitv(gn, d_vec, r_delta));
@@ -461,6 +463,8 @@ void poly_sumcheck_prove(Ctx& ctx, const dev::ScPoly& P, size_t len, const Fq& c
 //   delta_j = commit(d_vec_j; r_delta_j) and the blind halves blinds_poly[j]*h, blinds_evals[j]*h, r_beta_j*h — in four batched device MSMs.
 // enqueue() draws and launches (no synchronisation: the results travel to pinned host memory), finish() converts them once the stream has been synchronised;
 // r1cs_prove enqueues phase one's behind the witness commitment's MSM, so that neither the draws nor the launches sit on the critical path.
+// the staging area holds, per round, delta_j's encoding and three points
+size_t zk_sumcheck_max_rounds() { return layout::PIN_ZKPRE.cap / (32 + 3 * sizeof(ge)); }
 struct ZkPre {
   size_t num_rounds = 0, nco = 0;
   std::vector<Fq> blinds_poly, blinds_evals;
@@ -472,6 +476,7 @@ struct ZkPre {
   uint8_t* stage = nullptr;   // pinned: 32*num_rounds encodings, then 3*num_rounds points
   bool enqueued = false, finished = false;
   void enqueue(Ctx& ctx, int degree, size_t rounds, const CommitKey& g1, const CommitKey& gn, RandomTape& tape) {
+    if (rounds > zk_sumcheck_max_rounds()) throw std::runtime_error("spartan_b200: ZK sumcheck with too many rounds for the staging area");
     num_rounds = rounds; nco = (size_t)degree + 1;
     blinds_poly = tape.random_vector("blinds_poly", num_rounds);
     blinds_evals = tape.random_vector("blinds_evals", num_rounds);
@@ -484,8 +489,6 @@ struct ZkPre {
       for (size_t i = 0; i < nco; i++) dmat[j * nco + i] = pre[j].d_vec[i];
       rdel[j] = pre[j].r_delta; rbet[j] = pre[j].r_beta;
     }
-    const size_t stage_bytes = num_rounds * (32 + 3 * sizeof(ge));
-    if (stage_bytes > layout::PIN_ZKPRE.cap) throw std::runtime_error("spartan_b200: ZK sumcheck with too many rounds for the staging area");
     stage = ctx.pinned + layout::PIN_ZKPRE.off;
     d_s.alloc(num_rounds * nco); d_b.alloc(4 * num_rounds); d_pts.alloc(4 * num_rounds); d_c.alloc(32 * num_rounds);
     // pageable sources: the copies snapshot them before returning
@@ -495,12 +498,13 @@ struct ZkPre {
     dev::h2d(d_b.p + 2 * num_rounds, blinds_poly.data(), num_rounds * sizeof(u256), ctx.stream);
     dev::h2d(d_b.p + 3 * num_rounds, blinds_evals.data(), num_rounds * sizeof(u256), ctx.stream);
     if (ctx.scratch.n < dev::msm_scratch_bytes(num_rounds, nco) + 64) ctx.ensure_scratch(dev::msm_scratch_bytes(num_rounds, nco) + 64);
-    const GenSet& gs = *gn.set;
-    dev::msm_rows(d_pts.p, gs.table.p, gs.wbits, gs.rows(), d_s.p, nco, num_rounds, nco, d_b.p, gn.h, ctx.scratch.p, ctx.stream);                    // delta_j
+    // each blind term against the h of its own key: gens_1 and gens_n may be different generator sets (the caller's)
+    const GenSet &s1 = *g1.set, &sn = *gn.set;
+    dev::msm_rows(d_pts.p, sn.table.p, sn.wbits, sn.rows(), d_s.p, nco, num_rounds, nco, d_b.p, gn.h, ctx.scratch.p, ctx.stream);                    // delta_j
     dev::compress_batch(d_c.p, d_pts.p, num_rounds, ctx.stream);
-    dev::msm_rows(d_pts.p + num_rounds, gs.table.p, gs.wbits, gs.rows(), d_s.p, 0, num_rounds, 0, d_b.p + num_rounds, g1.h, ctx.scratch.p, ctx.stream);      // r_beta_j * h
-    dev::msm_rows(d_pts.p + 2 * num_rounds, gs.table.p, gs.wbits, gs.rows(), d_s.p, 0, num_rounds, 0, d_b.p + 2 * num_rounds, gn.h, ctx.scratch.p, ctx.stream);  // blinds_poly[j] * h
-    dev::msm_rows(d_pts.p + 3 * num_rounds, gs.table.p, gs.wbits, gs.rows(), d_s.p, 0, num_rounds, 0, d_b.p + 3 * num_rounds, g1.h, ctx.scratch.p, ctx.stream);  // blinds_evals[j] * h
+    dev::msm_rows(d_pts.p + num_rounds, s1.table.p, s1.wbits, s1.rows(), d_s.p, 0, num_rounds, 0, d_b.p + num_rounds, g1.h, ctx.scratch.p, ctx.stream);      // r_beta_j * h
+    dev::msm_rows(d_pts.p + 2 * num_rounds, sn.table.p, sn.wbits, sn.rows(), d_s.p, 0, num_rounds, 0, d_b.p + 2 * num_rounds, gn.h, ctx.scratch.p, ctx.stream);  // blinds_poly[j] * h
+    dev::msm_rows(d_pts.p + 3 * num_rounds, s1.table.p, s1.wbits, s1.rows(), d_s.p, 0, num_rounds, 0, d_b.p + 3 * num_rounds, g1.h, ctx.scratch.p, ctx.stream);  // blinds_evals[j] * h
     dev::d2h(stage, d_c.p, 32 * num_rounds, ctx.stream);
     dev::d2h(stage + 32 * num_rounds, d_pts.p + num_rounds, 3 * num_rounds * sizeof(ge), ctx.stream);
     enqueued = true;
@@ -518,6 +522,57 @@ struct ZkPre {
   }
 };
 
+// The host side of a ZK sumcheck's rounds, shared by both drivers below.  commit(): round j's polynomial from the device's evaluations, comm_poly,
+// r_j.  The driver then launches the bind with r_j (fused with the next round's evaluation), and prove() runs the rest of the round — comm_eval, the
+// two weights and the DotProductProof — while that kernel runs.
+struct ZkRounds {
+  const CommitKey &g1, &gn;
+  Transcript& T;
+  RandomTape& tape;
+  const ZkPre& zp;
+  ZKSumcheckInstanceProof& proof;
+  size_t degree;
+  Fq claim_per_round;
+  const Fq blind_claim;
+  Cp comm_claim_per_round;
+  UniPoly poly;
+  Cp comm_poly;
+  ZkRounds(const CommitKey& g1_, const CommitKey& gn_, Transcript& T_, RandomTape& tape_, const ZkPre& zp_, ZKSumcheckInstanceProof& proof_,
+           size_t degree_, const Fq& claim, const Fq& blind_claim_)
+      : g1(g1_), gn(gn_), T(T_), tape(tape_), zp(zp_), proof(proof_), degree(degree_), claim_per_round(claim), blind_claim(blind_claim_),
+        comm_claim_per_round(compress(commit1(g1_, claim, blind_claim_))) {}
+  // ev: s_j(0), s_j(2) .. s_j(degree); s_j(1) = claim - s_j(0)
+  Fq commit(size_t j, const Fq* ev) {
+    std::vector<Fq> evals = {ev[0], claim_per_round - ev[0]};
+    for (size_t t = 2; t <= degree; t++) evals.push_back(ev[t - 1]);
+    poly = UniPoly::from_evals(evals);
+    std::vector<Term> t;   // commit(coeffs; blinds_poly[j]; gens_n) = sum coeff_i*G_i + (blinds_poly[j]*h)
+    for (size_t i = 0; i < poly.coeffs.size(); i++) t.push_back({gn.off + i, poly.coeffs[i]});
+    comm_poly = compress(hge_add(host_commit(*gn.set, t.data(), t.size()), zp.bp_h[j]));
+    T.append_point("comm_poly", comm_poly.b);
+    proof.comm_polys.push_back(comm_poly);
+    return T.challenge_scalar("challenge_nextround");
+  }
+  void prove(size_t j, const Fq& r_j) {
+    Fq eval = poly.evaluate(r_j);
+    Term te[1] = {{g1.off, eval}};
+    Cp comm_eval = compress(hge_add(host_commit(*g1.set, te, 1), zp.be_h[j]));   // eval*G + blinds_evals[j]*h
+    T.append_point("comm_claim_per_round", comm_claim_per_round.b);
+    T.append_point("comm_eval", comm_eval.b);
+    std::vector<Fq> w = T.challenge_vector("combine_two_claims_to_one", 2);
+    Fq target = w[0] * claim_per_round + w[1] * eval;
+    const Fq& blind_sc = j == 0 ? blind_claim : zp.blinds_evals[j - 1];
+    Fq blind = w[0] * blind_sc + w[1] * zp.blinds_evals[j];
+    // (the reference also recomputes comm_target from the two decompressed commitments and asserts equality, sumcheck.rs:531/:722;
+    //  it is a self-check with no effect on the transcript)
+    const std::vector<Fq> a = zk_round_weights(w, r_j, degree);
+    proof.proofs.push_back(dotproduct_prove(g1, gn, T, tape, poly.coeffs, zp.blinds_poly[j], a, target, blind, &comm_poly, &zp.pre[j]));
+    claim_per_round = eval;
+    comm_claim_per_round = comm_eval;
+    proof.comm_evals.push_back(comm_claim_per_round);
+  }
+};
+
 // sharded: `tables` are this rank's cyclic shards (length 2^num_rounds / world).  The first rounds then run on the shards — the fused
 // kernels exchange their partial sums over NVLink before handing the round's evaluations to the host — until the local tables drop below
 // streaming size; the shards are then all-gathered into replicated tables (in the window) and the latency-bound tail runs on every rank alike.
@@ -532,18 +587,7 @@ static void zk_sumcheck_prove(Ctx& ctx, dev::ScKind kind, const Fq& claim, const
   if (!zp.enqueued) zp.enqueue(ctx, degree, num_rounds, g1, gn, tape);
   if (zp.num_rounds != num_rounds || zp.nco != (size_t)degree + 1) throw std::runtime_error("spartan_b200: ZK sumcheck pre-computation of the wrong shape");
   if (!zp.finished) { ctx.sync(); zp.finish(ctx); }
-  const std::vector<Fq>& blinds_poly = zp.blinds_poly;
-  const std::vector<Fq>& blinds_evals = zp.blinds_evals;
-  const std::vector<DotPre>& pre = zp.pre;
-  const std::vector<hge>& bp_h = zp.bp_h;
-  const std::vector<hge>& be_h = zp.be_h;
-  Fq claim_per_round = claim;
-  Cp comm_claim_per_round = compress(commit1(g1, claim_per_round, blind_claim));
-  auto commit_poly_pre = [&](const std::vector<Fq>& coeffs, size_t j) {   // commit(coeffs; blinds_poly[j]; gens_n) = sum coeff_i*G_i + (blinds_poly[j]*h)
-    std::vector<Term> t;
-    for (size_t i = 0; i < coeffs.size(); i++) t.push_back({gn.off + i, coeffs[i]});
-    return compress(hge_add(host_commit(*gn.set, t.data(), t.size()), bp_h[j]));
-  };
+  ZkRounds zr(g1, gn, T, tape, zp, proof, (size_t)degree, claim, blind_claim);
   dev::ScInst inst;
   for (int t = 0; t < 4; t++) inst.t[t] = t < nt ? tables[t] : nullptr;
   inst.c_out = inst.t[2];
@@ -555,44 +599,57 @@ static void zk_sumcheck_prove(Ctx& ctx, dev::ScKind kind, const Fq& claim, const
     const std::vector<Fq> e = sc.wait();
     fw.stop();
     FineTimer fh(ctx, "zk host commit_poly+challenge");
-    std::vector<Fq> evals = {e[0], claim_per_round - e[0], e[1]};
-    if (degree == 3) evals.push_back(e[2]);
-    UniPoly poly = UniPoly::from_evals(evals);
-    Cp comm_poly = commit_poly_pre(poly.coeffs, j);
-    T.append_point("comm_poly", comm_poly.b);
-    proof.comm_polys.push_back(comm_poly);
-    Fq r_j = T.challenge_scalar("challenge_nextround");
+    const Fq r_j = zr.commit(j, e.data());
     // bind the tables to r_j on the device right away (fused with the next round's evaluation); the host continues with the
     // sigma protocol of this round while the kernel runs
     if (j + 1 < num_rounds) sc.fold_eval(r_j);
     else sc.fold(r_j);
     fh.stop();
     FineTimer fs(ctx, "zk host sigma (overlaps kernel)");
-
-    Fq eval = poly.evaluate(r_j);
-    Term te[1] = {{g1.off, eval}};
-    Cp comm_eval = compress(hge_add(host_commit(*g1.set, te, 1), be_h[j]));   // eval*G + blinds_evals[j]*h
-    T.append_point("comm_claim_per_round", comm_claim_per_round.b);
-    T.append_point("comm_eval", comm_eval.b);
-    std::vector<Fq> w = T.challenge_vector("combine_two_claims_to_one", 2);
-    Fq target = w[0] * claim_per_round + w[1] * eval;
-    const Fq& blind_sc = j == 0 ? blind_claim : blinds_evals[j - 1];
-    Fq blind = w[0] * blind_sc + w[1] * blinds_evals[j];
-    // (the reference also recomputes comm_target from the two decompressed commitments and asserts equality, sumcheck.rs:531/:722;
-    //  it is a self-check with no effect on the transcript)
-    const std::vector<Fq> a = zk_round_weights(w, r_j, degree);
-    proof.proofs.push_back(dotproduct_prove(g1, gn, T, tape, poly.coeffs, blinds_poly[j], a, target, blind, &comm_poly, &pre[j]));
-    claim_per_round = eval;
-    comm_claim_per_round = comm_eval;
+    zr.prove(j, r_j);
     r.push_back(r_j);
-    proof.comm_evals.push_back(comm_claim_per_round);
   }
   finals.resize(nt);
   uint8_t* stage = ctx.pinned + layout::PIN_STAGE.off;
   for (int t = 0; t < nt; t++) dev::d2h(stage + 32 * t, sc.insts[0].t[t], 32, ctx.stream);   // the replicated copies after a shard exit
   ctx.sync();
   memcpy(finals.data(), stage, 32 * nt);
-  blind_post = blinds_evals[num_rounds - 1];
+  blind_post = zp.blinds_evals[num_rounds - 1];
+}
+
+void zk_poly_sumcheck_prove(Ctx& ctx, const dev::ScPoly& P, size_t len, const Fq& claim, const Fq& blind_claim, size_t num_rounds, const CommitKey& g1,
+                            const CommitKey& gn, Transcript& T, RandomTape& tape, ZKSumcheckInstanceProof& proof, std::vector<Fq>& r,
+                            std::vector<Fq>& finals, Fq& blind_post) {
+  const size_t d = (size_t)P.degree;
+  ZkPre zp;
+  zp.enqueue(ctx, P.degree, num_rounds, g1, gn, tape);
+  u256* d_out = ctx.small.p + layout::SMALL_ROUND.off;   // the d evaluations of a round
+  dev::HostSig sig = ctx.next_sig();
+  dev::scp_eval(P, len, d_out, ctx.red.p, ctx.stream, sig);
+  ctx.sync();
+  zp.finish(ctx);
+  ZkRounds zr(g1, gn, T, tape, zp, proof, d, claim, blind_claim);
+  std::vector<Fq> ev(d);
+  for (size_t j = 0; j < num_rounds; j++) {
+    ctx.wait_sig(sig);
+    memcpy(static_cast<void*>(ev.data()), ctx.host_res + layout::RES_OUT.off, d * sizeof(u256));
+    const Fq r_j = zr.commit(j, ev.data());
+    if (j + 1 < num_rounds) {   // bind and evaluate the next round while the host runs this round's sigma protocol
+      sig = ctx.next_sig();
+      dev::scp_fold_eval(P, len, r_j.m, d_out, ctx.red.p, ctx.stream, sig);
+    } else {
+      dev::fold_top(P.t, P.ntables, len, r_j.m, ctx.stream);
+    }
+    len >>= 1;
+    zr.prove(j, r_j);
+    r.push_back(r_j);
+  }
+  sig = ctx.next_sig();
+  dev::heads(ctx.small.p + layout::SMALL_HEADS.off, P.t, P.ntables, ctx.stream, sig);
+  ctx.wait_sig(sig);
+  finals.resize(P.ntables);
+  memcpy(static_cast<void*>(finals.data()), ctx.host_res + layout::RES_OUT.off, P.ntables * sizeof(u256));
+  blind_post = zp.blinds_evals[num_rounds - 1];
 }
 
 // ================================================================================================ polynomial commitment / evaluation proof

@@ -134,6 +134,30 @@ std::vector<Fq> zk_round_weights(const std::vector<Fq>& w, const Fq& r_j, size_t
 void append_claims_phase2(Transcript& T, const std::array<Cp, 4>& c);
 // NIZK::prove / verify before the R1CS proof: protocol name and R1CSShapeDigest (lib.rs:513-514, :558-559)
 void append_nizk_head(Transcript& T, const Instance& inst);
+// ---- sigma protocols (nizk/mod.rs), on the host over the host tables of the bases they commit against: g.off and g.h; DotProductProof also
+// gn.off .. gn.off + n - 1.  Each returns the proof and, through the out-parameters, the commitments the reference returns alongside it.
+KnowledgeProof knowledge_prove(const CommitKey& g, Transcript& T, RandomTape& tape, const Fq& x, const Fq& r, Cp& C_out);   // :27-52
+EqualityProof equality_prove(const CommitKey& g, Transcript& T, RandomTape& tape, const Fq& v1, const Fq& s1, const Fq& v2, const Fq& s2,
+                             Cp* C1_out = nullptr, Cp* C2_out = nullptr);   // :88-116
+ProductProof product_prove(const CommitKey& g, Transcript& T, RandomTape& tape, const Fq& x, const Fq& rX, const Fq& y, const Fq& rY, const Fq& z,
+                           const Fq& rZ, Cp& X, Cp& Y, Cp& Z);   // :159-229
+// DotProductProof::prove (:311-370).  Cx_known: commit(x_vec; blind_x) when the caller already holds it.  pre: the tape draws made ahead of time
+// in the reference's order, with the commitments that depend on the tape only (a ZK sumcheck's rounds)
+struct DotPre { std::vector<Fq> d_vec; Fq r_delta, r_beta; Cp delta; hge r_beta_h; };
+DotProductProof dotproduct_prove(const CommitKey& g1, const CommitKey& gn, Transcript& T, RandomTape& tape, const std::vector<Fq>& x_vec,
+                                 const Fq& blind_x, const std::vector<Fq>& a_vec, const Fq& y, const Fq& blind_y, const Cp* Cx_known,
+                                 const DotPre* pre = nullptr, Cp* Cx_out = nullptr, Cp* Cy_out = nullptr);
+// their verifiers (verifier.cpp, the Immediate checker) on bincode bytes: SpError(SP_ERR_VERIFY / SP_ERR_DECOMPRESS) naming the failing check, the
+// transcript advanced as the reference's verify advances it.  The caller's commitments (C, C1, .., Cy) must decompress.
+void knowledge_verify_bytes(Ctx& ctx, const CommitKey& g, Transcript& T, const Cp& C, const uint8_t* proof, size_t len);
+void equality_verify_bytes(Ctx& ctx, const CommitKey& g, Transcript& T, const Cp& C1, const Cp& C2, const uint8_t* proof, size_t len);
+void product_verify_bytes(Ctx& ctx, const CommitKey& g, Transcript& T, const Cp& X, const Cp& Y, const Cp& Z, const uint8_t* proof, size_t len);
+void dotproduct_verify_bytes(Ctx& ctx, const CommitKey& g1, const CommitKey& gn, Transcript& T, const std::vector<Fq>& a, const Cp& Cx, const Cp& Cy,
+                             const uint8_t* proof, size_t len);
+// ZKSumcheckInstanceProof::verify (sumcheck.rs:84-179): returns the last comm_eval, r the num_rounds (>= 1) challenges
+Cp zk_sumcheck_verify_bytes(Ctx& ctx, const uint8_t* proof, size_t len, const Cp& comm_claim, size_t num_rounds, size_t degree, const CommitKey& g1,
+                            const CommitKey& gn, Transcript& T, std::vector<Fq>& r);
+
 // PolyEvalProof::prove (dense_mlpoly.rs:312-365) on a device-resident table.  Zr null: Zr = Z(r) = <LZ, eq(r[ell/2..])>, computed on the device
 // from the bound rows (Z is not read again), and returned through Zr_out when that is set
 void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt, const std::vector<Fq>& r, const Fq* Zr, const Fq* blind_Zr_opt,
@@ -212,6 +236,16 @@ struct ScRounds {
 // drawn), then one bind and one gather of the first entries.  Single GPU.
 void poly_sumcheck_prove(Ctx& ctx, const dev::ScPoly& P, size_t len, const Fq& claim, size_t num_rounds, Transcript& T, SumcheckInstanceProof& proof,
                          std::vector<Fq>& r, std::vector<Fq>& finals, Fq& e);
+// The ZK sumcheck of the same polynomial (sp_zk_sumcheck_prove_t): ZKSumcheckInstanceProof::prove_quad / prove_cubic_with_additive_term
+// (sumcheck.rs:428-776) with comb_func P, of degree d = P.degree, on the caller's transcript and tape.  g1: n = 1, gn: n = d + 1 (they may come from
+// different generator sets); both need the host tables of the bases the rounds commit against (g1.off, g1.h, gn.off .. gn.off + d).  The rounds run
+// on the device as poly_sumcheck_prove's do, one launch per round, with the host's sigma work of round j overlapping the launch of round j + 1.
+// Out: the proof, r, finals as poly_sumcheck_prove's, blind_post = blinds_evals[num_rounds - 1].  Single GPU.
+// the most rounds one ZK sumcheck stages its tape-only commitments for (a fixed pinned region of the context)
+size_t zk_sumcheck_max_rounds();
+void zk_poly_sumcheck_prove(Ctx& ctx, const dev::ScPoly& P, size_t len, const Fq& claim, const Fq& blind_claim, size_t num_rounds, const CommitKey& g1,
+                            const CommitKey& gn, Transcript& T, RandomTape& tape, ZKSumcheckInstanceProof& proof, std::vector<Fq>& r,
+                            std::vector<Fq>& finals, Fq& blind_post);
 // SumcheckInstanceProof::verify (sumcheck.rs:27-62) on bincode bytes; SpError(SP_ERR_VERIFY) where the reference asserts or the bytes do not decode
 Fq sumcheck_verify_bytes(const uint8_t* proof, size_t len, const Fq& claim, size_t num_rounds, size_t degree, Transcript& T, std::vector<Fq>& r);
 

@@ -753,6 +753,35 @@ Fq sumcheck_verify_bytes(const uint8_t* proof, size_t len, const Fq& claim, size
   return sumcheck_verify(p, claim, num_rounds, degree, T, r);
 }
 
+// the caller's sigma proofs and ZK sumchecks (sp_knowledge_verify_t .. sp_zk_sumcheck_verify_t)
+void knowledge_verify_bytes(Ctx& ctx, const CommitKey& g, Transcript& T, const Cp& C, const uint8_t* proof, size_t len) {
+  const KnowledgeProof p = from_bincode<KnowledgeProof>(proof, len, SP_ERR_VERIFY, "knowledge proof");
+  Immediate chk(ctx);
+  knowledge_verify(chk, p, g, T, C);
+}
+void equality_verify_bytes(Ctx& ctx, const CommitKey& g, Transcript& T, const Cp& C1, const Cp& C2, const uint8_t* proof, size_t len) {
+  const EqualityProof p = from_bincode<EqualityProof>(proof, len, SP_ERR_VERIFY, "equality proof");
+  Immediate chk(ctx);
+  equality_verify(chk, p, g, T, unpack(C1, "C1"), C1, C2);
+}
+void product_verify_bytes(Ctx& ctx, const CommitKey& g, Transcript& T, const Cp& X, const Cp& Y, const Cp& Z, const uint8_t* proof, size_t len) {
+  const ProductProof p = from_bincode<ProductProof>(proof, len, SP_ERR_VERIFY, "product proof");
+  Immediate chk(ctx);
+  product_verify(chk, p, g, T, X, Y, Z);
+}
+void dotproduct_verify_bytes(Ctx& ctx, const CommitKey& g1, const CommitKey& gn, Transcript& T, const std::vector<Fq>& a, const Cp& Cx, const Cp& Cy,
+                             const uint8_t* proof, size_t len) {
+  const DotProductProof p = from_bincode<DotProductProof>(proof, len, SP_ERR_VERIFY, "dot product proof");
+  Immediate chk(ctx);
+  dotproduct_verify(chk, p, g1, gn, T, a, Cx, unpack(Cy, "Cy"), Cy);
+}
+Cp zk_sumcheck_verify_bytes(Ctx& ctx, const uint8_t* proof, size_t len, const Cp& comm_claim, size_t num_rounds, size_t degree, const CommitKey& g1,
+                            const CommitKey& gn, Transcript& T, std::vector<Fq>& r) {
+  const ZKSumcheckInstanceProof p = from_bincode<ZKSumcheckInstanceProof>(proof, len, SP_ERR_VERIFY, "ZK sumcheck proof");
+  Immediate chk(ctx);
+  return zk_sumcheck_verify(chk, p, unpack(comm_claim, "comm_claim"), comm_claim, num_rounds, degree, g1, gn, T, r);
+}
+
 // NIZK::verify (lib.rs:549-591)
 void nizk_verify(Ctx& ctx, const Instance& inst, const std::vector<Fq>& input, const R1CSGens& gens, Transcript& T, const uint8_t* proof, size_t len) {
   check_dims(inst.num_cons, inst.num_vars, inst.num_inputs);
