@@ -429,6 +429,43 @@ int sp_spark_eval_verify_t(sp_ctx* ctx, const sp_spark_gens* gens, const uint8_t
                            const uint64_t* ry_mont, size_t y, const uint64_t* evals_mont, int b, uint8_t* strobe_state /* in, out */, const uint8_t* proof,
                            size_t proof_len);
 
+/* ---- products of the caller's sparse matrices with vectors on the device: SparseMatPolynomial::multiply_vec (src/sparse_mlpoly.rs:454-464) and
+ * compute_eval_table_sparse (:466-481), for b = 1 .. SP_SPMAT_MAX_BATCH matrices of one shape (2^num_vars_x rows, 2^num_vars_y columns, x, y
+ * <= 30, fewer than 2^32 entries in all, nnz = 0 allowed).  b <= 8 = SP_SC_MAX_TABLES: the outputs are the tables of one caller sumcheck.
+ *
+ * sp_spmat holds every matrix twice on the device, sorted by row and sorted by column (stable: equal keys keep the caller's order), each entry as
+ * a 32-bit key, a 32-bit source index and a 32-byte Montgomery value: 80 bytes per entry, so 2^22 entries hold 320 MiB.  Building it also needs
+ * about 56 bytes per entry of the largest matrix, released on return: 40 for the ingested copy (row, column, value) and 16 for the sort (positions,
+ * permutation, and CUB's alternate key and value buffers); host arrays are staged on the device first, 48 bytes per entry more.  It records the
+ * largest row and column of all its entries, so a product call checks its bounds without reading the device.
+ *
+ * Every product runs on tiles of 1024 entries of the whole batch, whatever the rows' lengths: one row or column holding most entries costs what
+ * the same number of entries spread over many rows costs.  One call launches SP_SPMAT_PRODUCT_LAUNCHES kernels for every shape and skew (the
+ * weighted eval table one more), plus one memset per output; no table crosses PCIe.  Field addition is exact, so the outputs are the reference's
+ * bytes. */
+#define SP_SPMAT_MAX_BATCH 8
+#define SP_SPMAT_PRODUCT_LAUNCHES 3
+typedef struct sp_spmat sp_spmat;
+/* the b matrices' entries (sp_spark_entries of host arrays).  SP_ERR_INVALID_INDEX: a row >= 2^x ("row") or col >= 2^y ("col");
+ * SP_ERR_INVALID_SCALAR: a value >= q; the first bad entry in (matrix, entry, row/col/scalar) order is reported.  SP_ERR_INVALID_ARG, before
+ * anything is allocated: b outside 1 .. SP_SPMAT_MAX_BATCH, x or y > 30, 2^32 or more entries in all, NULL arrays with nnz > 0. */
+int sp_spmat_create(sp_ctx* ctx, const sp_spark_entries* matrices, int b, size_t num_vars_x, size_t num_vars_y, sp_spmat** out);
+/* the same with every array in DEVICE memory of the context's GPU: the synchronisation rules and pointer checks of sp_instance_create_device */
+int sp_spmat_create_device(sp_ctx* ctx, const sp_spark_entries* matrices, int b, size_t num_vars_x, size_t num_vars_y, sp_spmat** out);
+void sp_spmat_free(sp_spmat* m);
+/* multiply_vec of every matrix: outs[m] = M_m z, a new polynomial of num_rows entries (free each with sp_poly_free).  As in the reference,
+ * len(z) = num_cols, and num_rows, num_cols >= 1 may be any sizes (not only 2^x, 2^y, nor powers of two) that hold every entry: rows past the
+ * last entry read zero.  SP_ERR_INVALID_ARG where the reference panics (len(z) != num_cols, a row >= num_rows, a col >= num_cols), and for
+ * num_rows or num_cols of 0 or above 2^32, NULL arguments, handles of another context.  A refused call launches nothing, allocates no output
+ * and leaves z and outs untouched. */
+int sp_spmat_multiply_vec(sp_ctx* ctx, const sp_spmat* mats, size_t num_rows, size_t num_cols, const sp_poly* z, sp_poly** outs /* b */);
+/* compute_eval_table_sparse of every matrix: outs[m] = M_m^T e, num_cols entries, with e the eq table of len(e) = num_rows entries (not the
+ * point).  weights != NULL: the one table outs[0] = sum_m w_m M_m^T e (the R1CS prover's r_A, r_B, r_C combination), from the b tables in
+ * scratch and one more launch.  Refusals as sp_spmat_multiply_vec's (len(e) != num_rows instead of len(z)), and SP_ERR_INVALID_SCALAR for a
+ * weight that is not reduced; e, the weights and outs are left untouched. */
+int sp_spmat_eval_table(sp_ctx* ctx, const sp_spmat* mats, const sp_poly* e, size_t num_rows, size_t num_cols, const uint64_t* weights_mont /* b x 4 or NULL */,
+                        sp_poly** outs /* b, or 1 with weights */);
+
 /* ---- inner-product argument, operator level: BulletReductionProof::prove (src/nizk/bullet.rs:32-132) for a host that keeps the transcript and
  * the orchestration.  sp_ipa_begin copies a_vec / b_vec; the generator vector G is `gens` (G[0..n)).  Each round: sp_ipa_round_LR returns the
  * compressed L, R of bullet.rs:83-97 (c_L, c_R are formed inside; Q and H are the caller's points), the host appends them and derives u

@@ -13,4 +13,5 @@ from .api import (  # noqa: F401
     ZKSumcheckInstanceProof, KnowledgeProof, EqualityProof, ProductProof, DotProductProof,
     ProductLeaves, ProductCircuits, ProductCircuitEvalProofBatched, product_leaf_eval,
     SparseMatPolyCommitmentGens, SparseMatPolyCommitment, SparseMatPolyDense, SparseMatPolynomial, SparseMatPolyEvalProof,
+    SparseMatProducts,
 )

@@ -950,6 +950,8 @@ def product_leaf_eval(leaves, table_evals, rand):
 
 # ----------------------------------------------------------------------------- SPARK: the caller's sparse matrices
 SP_SPARK_MAX_BATCH = 4
+SP_SPMAT_MAX_BATCH = 8
+SP_SPMAT_PRODUCT_LAUNCHES = 3
 
 
 class _SparkEntries(C.Structure):
@@ -1080,6 +1082,79 @@ class SparseMatPolynomial:
         out = np.zeros((dense.batch_size, 4), dtype=np.uint64)
         dense.ctx.check(lib.sp_spark_evaluate(dense.ctx.h, dense.h, _p(rx), _sz(len(rx)), _p(ry), _sz(len(ry)), _p(out)))
         return out
+
+    @staticmethod
+    def multi_products(polys, ctx=None):
+        """the device form of 1 .. SP_SPMAT_MAX_BATCH matrices of one shape, all host or all device entries, for their products with vectors
+        (sp_spmat_create): a SparseMatProducts.  Host matrices go to ctx (default: the default context), device ones stay on theirs."""
+        polys = list(polys)
+        device = bool(polys) and polys[0].device
+        if any(p.device != device for p in polys):
+            raise SpartanB200Error("multi_products: mix of host and device matrices")
+        if any((p.num_vars_x, p.num_vars_y) != (polys[0].num_vars_x, polys[0].num_vars_y) for p in polys):
+            raise SpartanB200Error("multi_products: matrices of different shapes")
+        if device:
+            ctx = polys[0].ctx
+            if any(p.ctx is not ctx for p in polys):
+                raise SpartanB200Error("multi_products: device matrices of different contexts")
+            _sync_torch(ctx)
+        ctx = ctx or default_context()
+        x, y = (polys[0].num_vars_x, polys[0].num_vars_y) if polys else (0, 0)
+        arr = (_SparkEntries * max(len(polys), 1))(*[p._entries() for p in polys])
+        h = _vp()
+        entry = lib.sp_spmat_create_device if device else lib.sp_spmat_create
+        ctx.check(entry(ctx.h, arr, C.c_int(len(polys)), _sz(x), _sz(y), C.byref(h)))
+        return SparseMatProducts(ctx, h, len(polys))
+
+    def _products(self):
+        if getattr(self, "_spmat", None) is None:
+            self._spmat = SparseMatPolynomial.multi_products([self], self.ctx if self.device else None)
+        return self._spmat
+
+    def multiply_vec(self, num_rows, num_cols, z):
+        """SparseMatPolynomial::multiply_vec (sparse_mlpoly.rs:454-464) on the device: M z as a DensePolynomial of num_rows entries.  z: a
+        DensePolynomial or host Montgomery limbs of num_cols entries.  The device form is built on first use and kept on the object."""
+        return self._products().multiply_vec(num_rows, num_cols, z)[0]
+
+    def compute_eval_table_sparse(self, rx, num_rows, num_cols):
+        """SparseMatPolynomial::compute_eval_table_sparse (sparse_mlpoly.rs:466-481) on the device: M^T rx as a DensePolynomial of num_cols
+        entries.  rx is the eq table of num_rows entries (eq(r_x, .) as the reference passes it), not the point r_x; a DensePolynomial or host
+        Montgomery limbs."""
+        return self._products().compute_eval_table_sparse(rx, num_rows, num_cols)[0]
+
+
+class SparseMatProducts(_Handle):
+    """b matrices on the device, each sorted by row and by column (80 bytes per entry; include/spartan_b200.h, sp_spmat), for multiply_vec and
+    compute_eval_table_sparse of all of them in one call"""
+    _free = lib.sp_spmat_free
+
+    def __init__(self, ctx, h, batch_size):
+        self.ctx, self.h, self.batch_size = ctx, h, batch_size
+
+    def _vector(self, v):
+        if isinstance(v, DensePolynomial):
+            return v
+        return DensePolynomial(v, self.ctx)
+
+    def multiply_vec(self, num_rows, num_cols, z):
+        """[M_m z for every matrix m]: b DensePolynomials of num_rows entries; len(z) must be num_cols"""
+        z = self._vector(z)
+        outs = (_vp * self.batch_size)()
+        self.ctx.check(lib.sp_spmat_multiply_vec(self.ctx.h, self.h, _sz(num_rows), _sz(num_cols), z.h, outs))
+        return [DensePolynomial._wrap(self.ctx, _vp(outs[i])) for i in range(self.batch_size)]
+
+    def compute_eval_table_sparse(self, rx, num_rows, num_cols, weights=None):
+        """[M_m^T rx for every matrix m], b DensePolynomials of num_cols entries, with rx the eq table of num_rows entries (not the point).  With
+        weights (b scalars as Montgomery limbs): the one DensePolynomial sum_m weights[m] M_m^T rx."""
+        rx = self._vector(rx)
+        w = None if weights is None else _limbs(weights)
+        if w is not None and len(w) != self.batch_size:
+            raise SpartanB200Error("compute_eval_table_sparse: %d weights for %d matrices" % (len(w), self.batch_size))
+        n = 1 if w is not None else self.batch_size
+        outs = (_vp * n)()
+        self.ctx.check(lib.sp_spmat_eval_table(self.ctx.h, self.h, rx.h, _sz(num_rows), _sz(num_cols), None if w is None else _p(w), outs))
+        res = [DensePolynomial._wrap(self.ctx, _vp(outs[i])) for i in range(n)]
+        return res[0] if w is not None else res
 
 
 class SparseMatPolyEvalProof:

@@ -1949,6 +1949,151 @@ int sp_spark_eval_verify_t(sp_ctx* ctx, const sp_spark_gens* gens, const uint8_t
 }
 
 // ---- batch verifiers
+// ---- products of the caller's matrices (kernels_inst.cu: spmat_products).  Every argument is checked before the first allocation or launch.
+static_assert(SP_SPMAT_MAX_BATCH == SP_SC_MAX_TABLES, "the b products of one call are the tables of one caller sumcheck");
+static_assert(SP_SPMAT_MAX_BATCH >= SP_SPARK_MAX_BATCH, "a SPARK batch's matrices fit one product call");
+struct SpmatOrder {   // one matrix sorted by key: row order (key = row, src = col) or column order (key = col, src = row)
+  DevBuf<uint32_t> key, src;
+  DevBuf<u256> val;
+};
+struct sp_spmat {
+  Ctx* ctx;
+  int b;
+  size_t x, y, total;
+  size_t nnz[SP_SPMAT_MAX_BATCH];
+  SpmatOrder by_row[SP_SPMAT_MAX_BATCH], by_col[SP_SPMAT_MAX_BATCH];
+  uint64_t max_row, max_col;   // over every entry; meaningful when total > 0
+};
+static const size_t SPMAT_MAX_VARS = 30;
+static void spmat_create_common(sp_ctx* ctx, const sp_spark_entries* mats, int b, size_t x, size_t y, sp_spmat** out, bool device) {
+  const std::string what = device ? "spmat_create_device" : "spmat_create";
+  Ctx& c = ctx->c;
+  if (!out || !mats) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  require_count(what, b, "matrices", "SP_SPMAT_MAX_BATCH", SP_SPMAT_MAX_BATCH);
+  if (std::max(x, y) > SPMAT_MAX_VARS)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": max(num_vars_x, num_vars_y) = " + std::to_string(std::max(x, y)) + " > " + std::to_string(SPMAT_MAX_VARS));
+  size_t total = 0;
+  for (int m = 0; m < b; m++) {
+    const sp_spark_entries& e = mats[m];
+    const std::string at = what + ": matrix " + std::to_string(m);
+    if (e.nnz && (!e.row || !e.col || !e.val32)) throw SpError(SP_ERR_INVALID_ARG, at + ": NULL array");
+    if (device) {
+      require_device(c, e.row, e.nnz, (at + " row").c_str());
+      require_device(c, e.col, e.nnz, (at + " col").c_str());
+      require_device(c, e.val32, e.nnz, (at + " val").c_str());
+    }
+    total += e.nnz;
+    if (e.nnz >= ((size_t)1 << 32) || total >= ((size_t)1 << 32)) throw SpError(SP_ERR_INVALID_ARG, what + ": 2^32 or more entries in all");
+  }
+  std::unique_ptr<sp_spmat> S(new sp_spmat{&c, b, x, y, total, {}, {}, {}, 0, 0});
+  // matrix by matrix: the entries meet the checks of sp_instance_create (row < 2^x, col < 2^y, val < q) on the device, then both sorts
+  for (int m = 0; m < b; m++) {
+    const sp_spark_entries& e = mats[m];
+    const size_t n = e.nnz;
+    S->nnz[m] = n;
+    if (!n) continue;
+    dev::CooIn in{};
+    in.row[0] = e.row; in.col[0] = e.col; in.val[0] = e.val32; in.n[0] = n;
+    DevBuf<uint64_t> d_row, d_col;
+    DevBuf<uint8_t> d_val;
+    if (!device) {
+      d_row.alloc(n); d_col.alloc(n); d_val.alloc(32 * n);
+      dev::h2d(d_row.p, e.row, n * sizeof(uint64_t), c.stream);
+      dev::h2d(d_col.p, e.col, n * sizeof(uint64_t), c.stream);
+      dev::h2d(d_val.p, e.val32, 32 * n, c.stream);
+      in.row[0] = d_row.p; in.col[0] = d_col.p; in.val[0] = d_val.p;
+    }
+    DevBuf<uint32_t> row(n), col(n);
+    DevBuf<u256> val(n);
+    dev::CooOut co{};
+    co.row[0] = row.p; co.col[0] = col.p; co.val[0] = val.p;
+    DevBuf<unsigned long long> err(1);
+    dev::set_max_u64(err.p, c.stream);
+    dev::inst_ingest(in, 1, co, (size_t)1 << x, (size_t)1 << y, (size_t)1 << y, 0, err.p, c.stream);
+    unsigned long long first = 0;
+    dev::d2h(&first, err.p, sizeof(first), c.stream);
+    c.sync();
+    if (first != ~0ull) {   // the matrices are checked in order, so this is the first bad entry in (matrix, entry) order
+      const unsigned code = (unsigned)(first & 3);
+      const std::string at = " (matrix " + std::to_string(m) + ", entry " + std::to_string((first >> 2) & (((unsigned long long)1 << 40) - 1)) + ")";
+      if (code == dev::INGEST_ROW) throw SpError(SP_ERR_INVALID_INDEX, what + ": row out of range" + at);
+      if (code == dev::INGEST_COL) throw SpError(SP_ERR_INVALID_INDEX, what + ": col out of range" + at);
+      throw SpError(SP_ERR_INVALID_SCALAR, what + ": value not a canonical scalar" + at);
+    }
+    DevBuf<uint8_t> scratch(dev::spmat_sort_scratch_bytes(n));
+    SpmatOrder& R = S->by_row[m];
+    SpmatOrder& C = S->by_col[m];
+    R.key.alloc(n); R.src.alloc(n); R.val.alloc(n);
+    C.key.alloc(n); C.src.alloc(n); C.val.alloc(n);
+    dev::spmat_sort(R.key.p, R.src.p, R.val.p, row.p, col.p, val.p, (size_t)1 << x, n, scratch.p, c.stream);
+    dev::spmat_sort(C.key.p, C.src.p, C.val.p, col.p, row.p, val.p, (size_t)1 << y, n, scratch.p, c.stream);
+    uint32_t last[2] = {0, 0};   // the largest row and column: the last keys of the two orders
+    dev::d2h(&last[0], R.key.p + n - 1, 4, c.stream);
+    dev::d2h(&last[1], C.key.p + n - 1, 4, c.stream);
+    c.sync();
+    S->max_row = std::max<uint64_t>(S->max_row, last[0]);
+    S->max_col = std::max<uint64_t>(S->max_col, last[1]);
+  }
+  *out = S.release();
+}
+// M_m z (transpose = false: row order, z of num_cols entries, outputs of num_rows) or M_m^T e (column order, e of num_rows, outputs of num_cols)
+static void spmat_product(sp_ctx* ctx, const sp_spmat* S, const sp_poly* x, size_t num_rows, size_t num_cols, const uint64_t* weights, sp_poly** outs,
+                          bool transpose) {
+  const std::string what = transpose ? "spmat_eval_table" : "spmat_multiply_vec";
+  const char* xname = transpose ? "e" : "z";
+  Ctx& c = ctx->c;
+  if (!outs) throw SpError(SP_ERR_INVALID_ARG, what + ": outs is NULL");
+  require_owned(ctx, S, what, "matrices");
+  require_owned(ctx, x, what, xname);
+  const size_t lim = (size_t)1 << 32;
+  if (num_rows < 1 || num_rows > lim) throw SpError(SP_ERR_INVALID_ARG, what + ": num_rows = " + std::to_string(num_rows) + "; 1 .. 2^32 supported");
+  if (num_cols < 1 || num_cols > lim) throw SpError(SP_ERR_INVALID_ARG, what + ": num_cols = " + std::to_string(num_cols) + "; 1 .. 2^32 supported");
+  const size_t want = transpose ? num_rows : num_cols;
+  if (x->len != want)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": len(" + xname + ") = " + std::to_string(x->len) + " but " + (transpose ? "num_rows" : "num_cols") + " = " +
+                                          std::to_string(want));
+  if (S->total && S->max_row >= num_rows)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": num_rows = " + std::to_string(num_rows) + " but an entry has row " + std::to_string(S->max_row));
+  if (S->total && S->max_col >= num_cols)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": num_cols = " + std::to_string(num_cols) + " but an entry has col " + std::to_string(S->max_col));
+  if (weights) require_reduced(weights, (size_t)S->b, (what + ": weights").c_str());
+  const size_t nout = transpose ? num_cols : num_rows;
+  dev::SpmatBatch B{};
+  B.b = S->b;
+  const int nres = weights ? 1 : S->b;
+  std::vector<std::unique_ptr<sp_poly>> res(nres);
+  for (int i = 0; i < nres; i++) res[i].reset(new sp_poly{&c, DevBuf<u256>(nout), nout});
+  DevBuf<u256> tables(weights ? nout * S->b : 0);   // the per-matrix tables of the weighted sum
+  for (int m = 0; m < S->b; m++) {
+    const SpmatOrder& o = transpose ? S->by_col[m] : S->by_row[m];
+    B.key[m] = o.key.p; B.src[m] = o.src.p; B.val[m] = o.val.p; B.nnz[m] = S->nnz[m];
+    B.out[m] = weights ? tables.p + nout * m : res[m]->d.p;
+  }
+  DevBuf<uint8_t> scratch(dev::spmat_products_scratch_bytes(S->total));
+  dev::spmat_products(B, x->d.p, nout, scratch.p, c.stream);
+  if (weights) {
+    dev::LincombTables lt{};
+    lt.b = S->b;
+    for (int m = 0; m < S->b; m++) { lt.t[m] = B.out[m]; memcpy(&lt.w[m], weights + 4 * m, 32); }
+    dev::lincomb_many(res[0]->d.p, lt, nout, c.stream);
+  }
+  for (int i = 0; i < nres; i++) outs[i] = res[i].release();
+}
+
+int sp_spmat_create(sp_ctx* ctx, const sp_spark_entries* matrices, int b, size_t num_vars_x, size_t num_vars_y, sp_spmat** out) {
+  return guarded(ctx, [&] { spmat_create_common(ctx, matrices, b, num_vars_x, num_vars_y, out, false); });
+}
+int sp_spmat_create_device(sp_ctx* ctx, const sp_spark_entries* matrices, int b, size_t num_vars_x, size_t num_vars_y, sp_spmat** out) {
+  return guarded(ctx, [&] { spmat_create_common(ctx, matrices, b, num_vars_x, num_vars_y, out, true); });
+}
+void sp_spmat_free(sp_spmat* m) { delete m; }
+int sp_spmat_multiply_vec(sp_ctx* ctx, const sp_spmat* mats, size_t num_rows, size_t num_cols, const sp_poly* z, sp_poly** outs) {
+  return guarded(ctx, [&] { spmat_product(ctx, mats, z, num_rows, num_cols, nullptr, outs, false); });
+}
+int sp_spmat_eval_table(sp_ctx* ctx, const sp_spmat* mats, const sp_poly* e, size_t num_rows, size_t num_cols, const uint64_t* weights_mont, sp_poly** outs) {
+  return guarded(ctx, [&] { spmat_product(ctx, mats, e, num_rows, num_cols, weights_mont, outs, true); });
+}
+
 static int nizk_verify_batch_common(sp_ctx* ctx, const sp_instance* const* insts, const sp_nizk_gens* gens, const BatchArgs& a) {
   return verify_batch(ctx, reinterpret_cast<const void* const*>(insts), gens, a, [&](std::vector<VerifyJob>& jobs) {
     for (size_t i = 0; i < a.k; i++) jobs[i].inst = &insts[i]->inst;

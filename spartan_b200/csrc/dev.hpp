@@ -234,6 +234,42 @@ void canonical_to_mont(u256* out, const uint8_t* in32, size_t n, unsigned long l
 size_t compress_scratch_bytes(size_t nmajor, size_t nnz);
 void build_compressed(uint32_t* ptr, uint32_t* idx, u256* v, size_t nmajor, const uint32_t* major, const uint32_t* minor, const u256* val, size_t nnz,
                       void* scratch, cudaStream_t s);
+// ---- the caller's matrices as products (sp_spmat): every matrix in row order (key = row, src = col) and in column order (key = col, src = row)
+// sorted copy of nnz entries by key < nkeys, stable (equal keys keep their input order); scratch >= spmat_sort_scratch_bytes(nnz)
+size_t spmat_sort_scratch_bytes(size_t nnz);
+void spmat_sort(uint32_t* key_out, uint32_t* src_out, u256* val_out, const uint32_t* key, const uint32_t* src, const u256* val, size_t nkeys, size_t nnz,
+                void* scratch, cudaStream_t s);
+// out[m][key] = sum over the entries of matrix m with that key of val * x[src], for m < b; every out[m] has nout entries (zero where no entry has the
+// key; every key < nout).  Tiles of SPMAT_TILE entries of the batch whatever the rows' lengths, and three launches for every shape
+// (kernels_inst.cu); scratch >= spmat_products_scratch_bytes(sum of nnz)
+constexpr int SPMAT_THREADS = 256, SPMAT_ITEMS = 4, SPMAT_TILE = SPMAT_THREADS * SPMAT_ITEMS;
+struct SpmatBatch {
+  const uint32_t* key[SP_SPMAT_MAX_BATCH];
+  const uint32_t* src[SP_SPMAT_MAX_BATCH];
+  const u256* val[SP_SPMAT_MAX_BATCH];
+  size_t nnz[SP_SPMAT_MAX_BATCH];
+  u256* out[SP_SPMAT_MAX_BATCH];
+  int b;
+};
+// the carries of spmat_products in its scratch: n1 = 2 per tile of the entries (level 1), n2 = 2 per tile of those (level 2); values (32 B) and
+// keys (8 B) of each level, every region at a 256-byte boundary.  The one layout both the size and the carving read
+struct SpmatCarries {
+  size_t n1, n2, cv1, cv2, ck1, ck2, bytes;   // carry counts, byte offsets of the four regions, total bytes
+  static size_t carries(size_t n) { return 2 * ((n + SPMAT_TILE - 1) / SPMAT_TILE); }
+  static size_t up256(size_t b) { return (b + 255) & ~(size_t)255; }
+  explicit SpmatCarries(size_t total) : n1(carries(total)), n2(carries(n1)) {
+    cv1 = 0;
+    cv2 = cv1 + up256(32 * n1);
+    ck1 = cv2 + up256(32 * n2);
+    ck2 = ck1 + up256(8 * n1);
+    bytes = ck2 + 8 * n2;
+  }
+};
+size_t spmat_products_scratch_bytes(size_t total);   // SpmatCarries(total).bytes
+void spmat_products(const SpmatBatch& B, const u256* x, size_t nout, void* scratch, cudaStream_t s);
+// out[i] = sum_{m < b} w[m] * t[m][i] (w: Montgomery form)
+struct LincombTables { const u256* t[SP_SPMAT_MAX_BATCH]; u256 w[SP_SPMAT_MAX_BATCH]; int b; };
+void lincomb_many(u256* out, const LincombTables& lt, size_t n, cudaStream_t s);
 // AddrTimestamps::new (sparse_mlpoly.rs:220-254), one side of b <= SP_SPARK_MAX_BATCH matrices: the addresses src[m][0..nnz[m]) zero-padded to N
 // -> idx[m] (N each) and, as field elements over the b N positions (matrix-major, the reference loop's order), addr_f, ts_f (read_ts) and audit_f
 // (cells, counts over all b matrices); *bad |= 1 when an address is >= cells

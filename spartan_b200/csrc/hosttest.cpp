@@ -22,6 +22,14 @@ void sph_spark_dims(size_t x, size_t y, size_t nz, size_t b, size_t out[6]) {
   const size_t v[6] = {d.v_ops, d.v_mem, d.v_derefs, d.n_ops, d.n_mem, d.n_der};
   for (int i = 0; i < 6; i++) out[i] = v[i];
 }
+// entries per tile of the segmented matrix products (kernels_inst.cu: spmat_products)
+size_t sph_spmat_tile(void) { return sp::dev::SPMAT_TILE; }
+// the carry layout of spmat_products for `total` entries: out = n1, n2, offsets of cv1, cv2, ck1, ck2, scratch bytes
+void sph_spmat_carries(size_t total, size_t out[7]) {
+  const sp::dev::SpmatCarries L(total);
+  const size_t v[7] = {L.n1, L.n2, L.cv1, L.cv2, L.ck1, L.ck2, L.bytes};
+  for (int i = 0; i < 7; i++) out[i] = v[i];
+}
 // R1CSShape digest compressor: zlib stream of miniz level 6 (deflate.cpp); returns the length (out must hold len + len/8 + 128 bytes)
 size_t spt_zlib6(const uint8_t* in, size_t len, uint8_t* out) {
   std::vector<uint8_t> z = sp::miniz_zlib_level6(in, len);

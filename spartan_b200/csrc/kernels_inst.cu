@@ -168,6 +168,204 @@ void build_compressed(uint32_t* ptr, uint32_t* idx, u256* v, size_t nmajor, cons
   ck(cub::DeviceScan::ExclusiveSum(w.temp, tb, w.cnt, ptr, (int)(nmajor + 1), s), "scan");   // cnt[nmajor] = 0, so ptr[nmajor] = nnz
 }
 
+// ---- the caller's matrices in one sorted order: keys sorted stably (CUB radix sort), src and val gathered along
+size_t spmat_sort_scratch_bytes(size_t nnz) { check_items(nnz); return 2 * align256(4 * nnz) + align256(sort_temp_bytes(nnz)); }
+void spmat_sort(uint32_t* key_out, uint32_t* src_out, u256* val_out, const uint32_t* key, const uint32_t* src, const u256* val, size_t nkeys, size_t nnz,
+                void* scratch, cudaStream_t s) {
+  if (!nnz) return;
+  ProfScope ps("spmat_sort", 80.0 * (double)nnz, s);
+  char* p = (char*)scratch;
+  uint32_t* iota = (uint32_t*)p; p += align256(4 * nnz);
+  uint32_t* perm = (uint32_t*)p; p += align256(4 * nnz);
+  k_hist_iota<<<grid_for(nnz, 256, 8), 256, 0, s>>>(key, nnz, 0, nullptr, iota, nullptr);   // nkeys = 0: the positions only, no histogram
+  SP_LAUNCHED(); check("hist_iota");
+  size_t tb = sort_temp_bytes(nnz);
+  ck(cub::DeviceRadixSort::SortPairs(p, tb, key, key_out, iota, perm, (int)nnz, 0, key_bits(nkeys), s), "sort");
+  k_gather_compressed<<<grid_for(nnz, 256, 8), 256, 0, s>>>(perm, src, val, nnz, src_out, val_out);
+  SP_LAUNCHED(); check("gather_compressed");
+}
+
+// ---- segmented products out_m[key] = sum val * x[src] over the entries of b matrices, each sorted by key (merge-based SpMV, Merrill & Garland):
+// every CTA takes SPMAT_TILE consecutive entries of the concatenated batch whatever the rows' lengths.  An entry's segment key is (m << 32 | key),
+// so a segment never crosses a matrix boundary.  Inside a tile, runs of equal key are summed in registers and joined across threads by a
+// segmented scan (warp shuffles, then the warps' carries through shared memory).  A segment that starts and ends inside the tile is stored
+// directly: the entries are sorted, so no other tile holds its key.  The tile's first and last segments go to a carry array of (key, partial)
+// pairs (two per tile; a tile of one segment pairs it with a zero of the same key), which is again sorted by key and reduced the same way: one
+// more tiled pass leaves 2 ceil(2 ceil(n / TILE) / TILE) carries, at most 2^14 for n < 2^32, which one CTA finishes.  Every output key is
+// stored exactly once; the keys no entry has keep the zero the outputs start from.
+struct SegOut { u256* out[SP_SPMAT_MAX_BATCH]; };
+struct SegEnds { unsigned long long kf, kl; u256 vf, vl; int single; };
+__device__ __forceinline__ void seg_store(const SegOut& o, unsigned long long k, const u256& v) { st256(o.out[k >> 32] + (uint32_t)k, v); }
+__device__ __forceinline__ u256 shfl_up_256(const u256& x, int delta) {
+  u256 r;
+#pragma unroll
+  for (int i = 0; i < 8; i++) r.v[i] = __shfl_up_sync(0xffffffffu, x.v[i], delta);
+  return r;
+}
+// level 0: the matrices' entries; an entry's value is val * x[src]
+struct SegEntries {
+  const uint32_t* key[SP_SPMAT_MAX_BATCH];
+  const uint32_t* src[SP_SPMAT_MAX_BATCH];
+  const u256* val[SP_SPMAT_MAX_BATCH];
+  unsigned long long start[SP_SPMAT_MAX_BATCH + 1];   // matrix m holds the global entries start[m] .. start[m + 1]
+  const u256* x;
+  int b;
+  __device__ __forceinline__ void load(size_t t, unsigned long long& k, u256& v) const {
+    int m = 0;
+#pragma unroll
+    for (int j = 1; j < SP_SPMAT_MAX_BATCH; j++) m += (j < b && t >= start[j]) ? 1 : 0;
+    const size_t i = t - start[m];
+    k = ((unsigned long long)m << 32) | key[m][i];
+    v = fq_mul(ld256_ro(val[m] + i), ld256_ro(x + src[m][i]));
+  }
+};
+// levels 1 and 2: the carries of the level below
+struct SegCarries {
+  const unsigned long long* k;
+  const u256* v;
+  __device__ __forceinline__ void load(size_t t, unsigned long long& key, u256& val) const { key = k[t]; val = ld256(v + t); }
+};
+
+// one tile of nt <= SPMAT_TILE items from `base`: stores the segments inside it, returns its first and last segments in `ends` (all threads)
+template <class Src>
+__device__ __forceinline__ void seg_tile(const Src& src, size_t base, int nt, const SegOut& o, SegEnds& ends) {
+  __shared__ unsigned long long skey[SPMAT_TILE];
+  __shared__ u256 wv[SPMAT_THREADS / 32];
+  __shared__ int wf[SPMAT_THREADS / 32];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, j0 = tid * SPMAT_ITEMS;
+  const int nitems = max(0, min(SPMAT_ITEMS, nt - j0));
+  unsigned long long k[SPMAT_ITEMS];
+  u256 p[SPMAT_ITEMS];
+#pragma unroll
+  for (int j = 0; j < SPMAT_ITEMS; j++) {
+    k[j] = 0; p[j] = fq_zero();
+    if (j < nitems) { src.load(base + j0 + j, k[j], p[j]); skey[j0 + j] = k[j]; }
+  }
+  __syncthreads();
+  // head: an item, not the tile's first, whose key differs from its predecessor's.  Scan value: the sum since the thread's last head (all of it
+  // without one), flagged when the thread has a head
+  bool head[SPMAT_ITEMS];
+  int f = 0;
+  u256 v = fq_zero();
+#pragma unroll
+  for (int j = 0; j < SPMAT_ITEMS; j++) {
+    head[j] = j < nitems && j0 + j > 0 && k[j] != (j ? k[j - 1] : skey[j0 - 1]);
+    if (head[j]) { f = 1; v = fq_zero(); }
+    if (j < nitems) v = fq_add(v, p[j]);
+  }
+  // inclusive segmented scan over the warp: (fa, va) + (fb, vb) = (fa | fb, fb ? vb : va + vb)
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const u256 vo = shfl_up_256(v, d);
+    const int fo = __shfl_up_sync(0xffffffffu, f, d);
+    if (lane >= d) {
+      if (!f) v = fq_add(vo, v);
+      f |= fo;
+    }
+  }
+  if (lane == 31) { wv[warp] = v; wf[warp] = f; }
+  // exclusive within the warp
+  u256 ce = shfl_up_256(v, 1);
+  int fe = __shfl_up_sync(0xffffffffu, f, 1);
+  if (lane == 0) { ce = fq_zero(); fe = 0; }
+  __syncthreads();
+  // the earlier warps' carry: their aggregates back to the nearest flagged one
+  u256 cw = fq_zero();
+  int fw = 0;
+  for (int w = warp - 1; w >= 0; w--) {
+    cw = fq_add(wv[w], cw);
+    if (wf[w]) { fw = 1; break; }
+  }
+  u256 run = fe ? ce : fq_add(cw, ce);   // the open segment's sum at the thread's first item
+  int seen = fw | fe;                    // a head earlier in the tile: the open segment is not the tile's first
+#pragma unroll
+  for (int j = 0; j < SPMAT_ITEMS; j++) {
+    if (head[j]) {
+      const unsigned long long kp = j ? k[j - 1] : skey[j0 - 1];
+      if (seen) seg_store(o, kp, run);
+      else { ends.kf = kp; ends.vf = run; }
+      run = fq_zero();
+      seen = 1;
+    }
+    if (j < nitems) run = fq_add(run, p[j]);
+  }
+  if (nitems > 0 && j0 + nitems == nt) {   // the tile's last item
+    ends.kl = k[nitems - 1]; ends.vl = run; ends.single = !seen;
+    if (!seen) { ends.kf = ends.kl; ends.vf = run; }
+  }
+  __syncthreads();
+}
+template <class Src>
+__global__ void __launch_bounds__(SPMAT_THREADS) k_seg_tiles(Src src, size_t n, SegOut o, unsigned long long* ck, u256* cv) {
+  __shared__ SegEnds ends;
+  const size_t base = (size_t)blockIdx.x * SPMAT_TILE;
+  if (base >= n) return;
+  seg_tile(src, base, (int)min((size_t)SPMAT_TILE, n - base), o, ends);
+  if (threadIdx.x == 0) {
+    ck[2 * blockIdx.x] = ends.kf; st256(cv + 2 * blockIdx.x, ends.vf);
+    ck[2 * blockIdx.x + 1] = ends.kl; st256(cv + 2 * blockIdx.x + 1, ends.single ? fq_zero() : ends.vl);
+  }
+}
+// the last level in one CTA: the tiles in order, the segment open at a tile's end carried into the next
+__global__ void __launch_bounds__(SPMAT_THREADS) k_seg_final(SegCarries src, size_t n, SegOut o) {
+  __shared__ SegEnds ends;
+  unsigned long long rk = 0;
+  u256 rv = fq_zero();
+  bool open = false;
+  for (size_t base = 0; base < n; base += SPMAT_TILE) {
+    seg_tile(src, base, (int)min((size_t)SPMAT_TILE, n - base), o, ends);
+    if (threadIdx.x == 0) {
+      u256 first = ends.vf;
+      if (open && rk == ends.kf) first = fq_add(rv, first);
+      else if (open) seg_store(o, rk, rv);
+      if (ends.single) { rk = ends.kf; rv = first; }
+      else { seg_store(o, ends.kf, first); rk = ends.kl; rv = ends.vl; }
+      open = true;
+    }
+  }
+  if (threadIdx.x == 0 && open) seg_store(o, rk, rv);
+}
+size_t spmat_products_scratch_bytes(size_t total) { return SpmatCarries(total).bytes; }
+void spmat_products(const SpmatBatch& B, const u256* x, size_t nout, void* scratch, cudaStream_t s) {
+  SegEntries e{};
+  SegOut o{};
+  size_t total = 0;
+  for (int m = 0; m < B.b; m++) {
+    e.key[m] = B.key[m]; e.src[m] = B.src[m]; e.val[m] = B.val[m]; e.start[m] = total;
+    o.out[m] = B.out[m];
+    total += B.nnz[m];
+    dzero(B.out[m], 32 * nout, s);
+  }
+  for (int m = B.b; m <= SP_SPMAT_MAX_BATCH; m++) e.start[m] = total;
+  e.x = x; e.b = B.b;
+  const SpmatCarries L(total);
+  const size_t n1 = L.n1, n2 = L.n2;
+  ProfScope ps("spmat_products", 72.0 * (double)total + 32.0 * (double)nout * B.b, s);
+  char* p = (char*)scratch;
+  u256* cv1 = (u256*)(p + L.cv1);
+  u256* cv2 = (u256*)(p + L.cv2);
+  unsigned long long* ck1 = (unsigned long long*)(p + L.ck1);
+  unsigned long long* ck2 = (unsigned long long*)(p + L.ck2);
+  // a fixed three launches (SP_SPMAT_PRODUCT_LAUNCHES) for every shape; the grids of empty levels run one CTA that returns at once
+  k_seg_tiles<<<(unsigned)std::max<size_t>(1, n1 / 2), SPMAT_THREADS, 0, s>>>(e, total, o, ck1, cv1);
+  k_seg_tiles<<<(unsigned)std::max<size_t>(1, n2 / 2), SPMAT_THREADS, 0, s>>>(SegCarries{ck1, cv1}, n1, o, ck2, cv2);
+  k_seg_final<<<1, SPMAT_THREADS, 0, s>>>(SegCarries{ck2, cv2}, n2, o);
+  SP_LAUNCHED(); SP_LAUNCHED(); SP_LAUNCHED(); check("spmat_products");
+}
+// out = sum_m w[m] * t[m] (the weighted eval table: k_lincomb3 for b tables)
+__global__ void k_lincomb_many(u256* out, LincombTables lt, size_t n) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    u256 acc = fq_mul(lt.w[0], ld256_ro(lt.t[0] + i));
+    for (int m = 1; m < lt.b; m++) acc = fq_add(acc, fq_mul(lt.w[m], ld256_ro(lt.t[m] + i)));
+    st256(out + i, acc);
+  }
+}
+void lincomb_many(u256* out, const LincombTables& lt, size_t n, cudaStream_t s) {
+  ProfScope ps("lincomb_many", 32.0 * (double)n * (lt.b + 1), s);
+  k_lincomb_many<<<grid_for(n, 256, 4), 256, 0, s>>>(out, lt, n);
+  SP_LAUNCHED(); check("lincomb_many");
+}
+
 // ---- AddrTimestamps::new (sparse_mlpoly.rs:220-254) for one side: b N positions in the reference loop's order (matrix-major, zero-padded to N);
 // read_ts of a position = earlier positions with its address = its rank within its run after a stable sort by address; audit = run lengths
 size_t spark_ts_scratch_bytes(size_t b, size_t N, size_t cells) {
