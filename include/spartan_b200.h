@@ -318,8 +318,9 @@ int sp_dotproduct_verify_t(sp_ctx* ctx, const sp_gens* gens_1, const sp_gens* ge
  * for an offline memory check, multiset equality or a lookup argument: commit to the tuple tables (sp_pc_commit), draw the fingerprint
  * challenges, build one circuit per fingerprinted multiset (sp_prod_build), absorb the products, prove them (sp_prod_prove_t), and open the
  * tables at the point the proof ends on (sp_pc_eval_prove_joint_t); the verifier checks the leaf claims with sp_prod_leaf_eval.  Every entry runs
- * on this rank's GPU alone, also on a connected multi-GPU context.  No dot-product circuits: the proof's claims_dotp are three empty vectors
- * (the reference's prove with dotp_circuit_vec empty).
+ * on this rank's GPU alone, also on a connected multi-GPU context.  sp_prod_build / sp_prod_prove_t / sp_prod_verify_t prove products alone
+ * (the reference's prove with dotp_circuit_vec empty: the proof's claims_dotp are three empty vectors); the _dotp entries below also prove dot
+ * products batched into the last layer's sumcheck.
  *
  * Circuit c's leaf at index x < 2^m is an affine form of up to SP_PROD_MAX_SOURCES of the tables and of x itself:
  *   leaf_c[x] = const_c + index_coeff_c * x + sum_{s < nsources_c} coeff_{c,s} * tables[source_{c,s}][x]
@@ -354,7 +355,8 @@ int sp_prod_build(sp_ctx* ctx, sp_poly* const* tables, int ntables, const sp_pro
  * the products: absorb them first, as ProductLayerProof::prove does (sparse_mlpoly.rs:1061-1064).  Out: *proof = bincode(ProductCircuitEvalProofBatched)
  * (free with sp_free), rand_out = the m scalars of the point the proof ends on, leaf_evals_out = each circuit's leaf polynomial at rand (the
  * last claims_to_verify: the values sp_prod_verify_t returns as leaf claims).  Consumes the circuits: their layers are bound in place and released,
- * and a second call on the handle is refused (SP_ERR_INVALID_ARG), as are a NULL handle and one of another context; a refused call leaves the
+ * and a second call on the handle is refused (SP_ERR_INVALID_ARG), as are a NULL handle, one of another context and one made by
+ * sp_prod_build_dotp with dot products (prove it with sp_prod_prove_dotp_t; the handle is then not consumed); a refused call leaves the
  * transcript untouched.  Launches, independent of k: one per sumcheck round plus a few per layer (tests/test_gpu_product.py states the count). */
 int sp_prod_prove_t(sp_ctx* ctx, sp_prod_circuits* c, uint8_t* strobe_state /* in, out */, uint8_t** proof, size_t* proof_len,
                     uint64_t* rand_out /* m x 4 */, uint64_t* leaf_evals_out /* k x 4 */);
@@ -371,6 +373,40 @@ int sp_prod_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const 
  * claims.  leaves NULL: circuit i is table i (k = ntables).  Refusals as sp_prod_build's. */
 int sp_prod_leaf_eval(const sp_prod_leaves* leaves, int k, const uint64_t* table_evals_mont, int ntables, const uint64_t* rand_mont, size_t m,
                       uint64_t* out /* k x 4 */);
+
+/* ---- dot products beside the product circuits: ProductCircuitEvalProofBatched::prove(prod_circuit_vec, dotp_circuit_vec, transcript) with the
+ * caller's dot products sum_x left[x] * right[x] * weight[x] over x < 2^m, batched into the sumcheck of the circuits' last layer (product_tree.rs:
+ * 259-485).  SPARK proves a sparse evaluation this way from its dereferenced values (sparse_mlpoly.rs:1090-1117); a caller's own memory check
+ * proves the value its reads add up to.  Each operand is an affine form of the tables, exactly as a circuit's leaves (sp_prod_leaves): a plain
+ * table, a fingerprint, the index or a constant (weight = 1 is const = one).  The library splits each dot product into its halves
+ * [0, 2^(m-1)) and [2^(m-1), 2^m) (DotProductCircuit::split) and batches them as the reference's verifier pairs them: dotp_circuit_vec =
+ * half 0 of dot product 0, half 1 of dot product 0, half 0 of dot product 1, ..  So `let (l, r) = d.split(); dotp_vec.push(l); dotp_vec.push(r)`
+ * is one dot product here, and claims_dotp_vec is the 2 kd half sums sp_prod_build_dotp returns.
+ * Limits: 1 <= k, 1 <= kd and k + 2 kd <= SP_PROD_MAX_CIRCUITS (the circuits and both halves of every dot product are instances of one batched
+ * sumcheck launch).  Device footprint: 3 * 2^m scalars per dot product (its operands, bound in place by the proof), from sp_prod_build_dotp until
+ * sp_prod_prove_dotp_t or sp_prod_free; at m = 20, 96 MiB per dot product. */
+/* sp_prod_build with kd dot products: dotp_forms holds 3 kd forms, (left, right, weight) of each dot product.  One more launch than sp_prod_build
+ * writes every dot product's operands and sums each half.  Out: as sp_prod_build's, and dotp_claims_out = the two half sums of each dot product
+ * (claims_dotp_vec, DotProductCircuit::evaluate of each half).  Refusals as sp_prod_build's, also for the dot products' counts, sources, reduced
+ * coefficients and constants, and NULL dotp_forms or dotp_claims_out; a refused call allocates and launches nothing. */
+int sp_prod_build_dotp(sp_ctx* ctx, sp_poly* const* tables, int ntables, const sp_prod_leaves* leaves, int k, const sp_prod_leaves* dotp_forms /* 3 kd */,
+                       int kd, sp_prod_circuits** out, uint64_t* products_out /* k x 4 */, uint64_t* dotp_claims_out /* 2 kd x 4 */);
+/* sp_prod_prove_t for a handle of either build: the proof carries the dot products' final claims, and dotp_evals_out = (left, right, weight) at
+ * rand of each dot product (the values sp_prod_verify_dotp_t returns as dotp claims).  dotp_evals_out may be NULL for a handle without dot
+ * products.  Consumes the circuits, and refuses as sp_prod_prove_t.  Launches: sp_prod_prove_t's, plus one per eq-factored round of the last
+ * layer (rounds whose tables hold >= 2^14 entries: the dot-product instances take a second launch there), plus, when the last layer's tables
+ * (two per circuit, six per dot product) exceed 64, one at m = 1 and m >= 15 and two at m = 2 (the gather of its final claims at m <= 2 and
+ * the bind of its one round at m = 2 or of the switch out of its eq-factored rounds at m >= 15 take 64 tables per launch;
+ * tests/test_gpu_product_dotp.py states the count). */
+int sp_prod_prove_dotp_t(sp_ctx* ctx, sp_prod_circuits* c, uint8_t* strobe_state /* in, out */, uint8_t** proof, size_t* proof_len,
+                         uint64_t* rand_out /* m x 4 */, uint64_t* leaf_evals_out /* k x 4 */, uint64_t* dotp_evals_out /* 3 kd x 4 */);
+/* ProductCircuitEvalProofBatched::verify(products, dotp_claims, 2^m, transcript), host only (ctx may be NULL): dotp_claims = the 2 kd half sums.
+ * SP_OK: accepted, rand_out and leaf_claims_out as sp_prod_verify_t's, and dotp_claims_out = (left, right, weight) at rand of each dot product: the
+ * verifier checks them with sp_prod_leaf_eval on the operand forms.  SP_ERR_VERIFY, SP_ERR_INVALID_ARG and SP_ERR_INVALID_SCALAR as
+ * sp_prod_verify_t's, also for kd (the limits above), NULL dotp_claims or dotp_claims_out and half sums not reduced. */
+int sp_prod_verify_dotp_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const uint64_t* products_mont, int k, const uint64_t* dotp_claims_mont /* 2 kd x 4 */,
+                          int kd, size_t m, uint8_t* strobe_state /* in, out */, uint64_t* rand_out /* m x 4 */, uint64_t* leaf_claims_out /* k x 4 */,
+                          uint64_t* dotp_claims_out /* 3 kd x 4 */);
 
 /* ---- SPARK: commitments to the caller's sparse matrices and proofs of their evaluations (SparseMatPolyCommitmentGens, SparseMatPolynomial::
  * multi_commit / multi_evaluate, SparseMatPolyEvalProof::{prove, verify}, src/sparse_mlpoly.rs), for b = 1 .. SP_SPARK_MAX_BATCH matrices of

@@ -896,24 +896,36 @@ def _c_leaves(leaves):
 class ProductCircuits(_Handle):
     """ProductCircuit::new of k circuits, then ProductCircuit::evaluate (product_tree.rs:36-63), on the GPU: `tables` are DensePolynomials of
     one length 2^m (m >= 1), read and never modified; `leaves` a list of ProductLeaves (at most SP_PROD_MAX_CIRCUITS), or None for one circuit
-    per table.  .products: the k products as (k, 4) limbs; .num_vars = m.  ProductCircuitEvalProofBatched.prove consumes the circuits."""
+    per table.  .products: the k products as (k, 4) limbs; .num_vars = m.  ProductCircuitEvalProofBatched.prove consumes the circuits.
+    `dotps`: a list of kd (left, right, weight) triples of ProductLeaves, the dot products sum_x left[x] right[x] weight[x] to prove beside the
+    circuits (k + 2 kd <= SP_PROD_MAX_CIRCUITS); .dotp_claims: the two half sums of each as (kd, 2, 4) limbs (claims_dotp_vec), and
+    ProductCircuitEvalProofBatched.prove_dotp proves them."""
     _free = lib.sp_prod_free
 
-    def __init__(self, tables, leaves=None):
+    def __init__(self, tables, leaves=None, dotps=None):
         tables = _poly_list(tables)
         self.ctx = tables[0].ctx if tables else default_context()
         self.k = len(tables) if leaves is None else len(leaves)
+        self.kd = 0 if dotps is None else len(dotps)
         products = np.zeros((max(self.k, 1), 4), dtype=np.uint64)
+        claims = np.zeros((max(self.kd, 1), 2, 4), dtype=np.uint64)
         h = _vp()
-        self.ctx.check(lib.sp_prod_build(self.ctx.h, _handles(tables), C.c_int(len(tables)), _c_leaves(leaves), C.c_int(self.k), C.byref(h),
-                                         _p(products)))
+        if dotps is None:
+            self.ctx.check(lib.sp_prod_build(self.ctx.h, _handles(tables), C.c_int(len(tables)), _c_leaves(leaves), C.c_int(self.k), C.byref(h),
+                                             _p(products)))
+        else:
+            forms = _c_leaves([f for d in dotps for f in d])
+            self.ctx.check(lib.sp_prod_build_dotp(self.ctx.h, _handles(tables), C.c_int(len(tables)), _c_leaves(leaves), C.c_int(self.k), forms,
+                                                  C.c_int(self.kd), C.byref(h), _p(products), _p(claims)))
         self.h = h
         self.products = products[:self.k]
+        self.dotp_claims = claims[:self.kd]
         self.num_vars = tables[0].len().bit_length() - 1
 
 
 class ProductCircuitEvalProofBatched:
-    """product_tree.rs:250-485 without dot-product circuits.  Transcripts: a Transcript (advanced in place) or a label."""
+    """product_tree.rs:250-485: prove / verify for product circuits alone, prove_dotp / verify_dotp with the caller's dot products.  Transcripts:
+    a Transcript (advanced in place) or a label."""
 
     @staticmethod
     def prove(circuits, transcript):
@@ -936,6 +948,34 @@ class ProductCircuitEvalProofBatched:
         _check_host(lib.sp_prod_verify_t(None, C.c_char_p(proof), _sz(len(proof)), _p(prods), C.c_int(len(prods)), _sz(num_vars), t.state, _p(rand),
                                          _p(claims)))
         return rand[:num_vars], claims[:len(prods)]
+
+    @staticmethod
+    def prove_dotp(circuits, transcript):
+        """ProductCircuitEvalProofBatched::prove(circuits, dotp halves, transcript) of ProductCircuits built with or without dotps.  Absorb the
+        products (and what the caller's protocol absorbs of the half sums) first.  Returns (proof bytes, rand (m, 4), leaf_evals (k, 4),
+        dotp_evals = (left, right, weight) of each dot product at rand as (kd, 3, 4) limbs)."""
+        ctx, t = circuits.ctx, _transcript_state(transcript)
+        out, n = C.POINTER(C.c_ubyte)(), _sz()
+        rand = np.zeros((circuits.num_vars, 4), dtype=np.uint64)
+        evals = np.zeros((max(circuits.k, 1), 4), dtype=np.uint64)
+        dotp = np.zeros((max(circuits.kd, 1), 3, 4), dtype=np.uint64)
+        ctx.check(lib.sp_prod_prove_dotp_t(ctx.h, circuits.h, t.state, C.byref(out), C.byref(n), _p(rand), _p(evals), _p(dotp)))
+        return _take_bytes(out, n), rand, evals[:circuits.k], dotp[:circuits.kd]
+
+    @staticmethod
+    def verify_dotp(proof, products, dotp_claims, num_vars, transcript):
+        """ProductCircuitEvalProofBatched::verify(products, dotp_claims, 2^num_vars, transcript) on the host, dotp_claims the (kd, 2, 4) half sums:
+        returns (rand, leaf_claims, dotp_claims = (left, right, weight) of each dot product at rand as (kd, 3, 4) limbs), raises ProofVerifyError.
+        The transcript is advanced as the reference's verify advances it, accepted or not."""
+        t, proof, prods = _transcript_state(transcript), bytes(proof), _limbs(products)
+        halves = _limbs(np.asarray(dotp_claims, dtype=np.uint64).reshape(-1, 4))
+        kd = len(halves) // 2
+        rand = np.zeros((max(num_vars, 1), 4), dtype=np.uint64)
+        claims = np.zeros((max(len(prods), 1), 4), dtype=np.uint64)
+        dotp = np.zeros((max(kd, 1), 3, 4), dtype=np.uint64)
+        _check_host(lib.sp_prod_verify_dotp_t(None, C.c_char_p(proof), _sz(len(proof)), _p(prods), C.c_int(len(prods)), _p(halves), C.c_int(kd),
+                                              _sz(num_vars), t.state, _p(rand), _p(claims), _p(dotp)))
+        return rand[:num_vars], claims[:len(prods)], dotp[:kd]
 
 
 def product_leaf_eval(leaves, table_evals, rand):

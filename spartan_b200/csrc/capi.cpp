@@ -31,6 +31,7 @@ struct sp_prod_circuits {
   size_t m;
   std::vector<std::unique_ptr<ProdCircuit>> cs;   // released by the proof
   bool spent;
+  ProdDotps dotps;                                 // sp_prod_build_dotp's dot products, likewise
 };
 
 // the message sp_last_error(NULL) reads: of the last failed sp_ctx_create, or of the last failed host-only call made without a context
@@ -239,13 +240,15 @@ static void prod_counts(const sp_prod_leaves* leaves, int k, int ntables, const 
   if (!leaves && k != ntables)
     throw SpError(SP_ERR_INVALID_ARG, what + ": leaves NULL (circuit i = table i) needs k = ntables, got k = " + std::to_string(k) + ", ntables = " + std::to_string(ntables));
 }
-static std::vector<LeafForm> prod_forms(const sp_prod_leaves* leaves, int k, int ntables, const std::string& what) {
-  prod_counts(leaves, k, ntables, what);
+// the k forms of `leaves` checked: every count and source first (SP_ERR_INVALID_ARG), then every scalar (SP_ERR_INVALID_SCALAR).  name(c): what a
+// message calls form c.  leaves NULL: form c is table c
+template <class Name>
+static std::vector<LeafForm> checked_forms(const sp_prod_leaves* leaves, int k, int ntables, const Name& name) {
   std::vector<LeafForm> f(k);
   for (int c = 0; c < k; c++) {
     if (!leaves) { f[c].nsrc = 1; f[c].src[0] = (uint32_t)c; f[c].coeff[0] = Fq::one(); continue; }
     const sp_prod_leaves& l = leaves[c];
-    const std::string at = what + ": circuit " + std::to_string(c);
+    const std::string at = name(c);
     if (l.nsources > SP_PROD_MAX_SOURCES)
       throw SpError(SP_ERR_INVALID_ARG, at + " has " + std::to_string(l.nsources) + " sources; at most SP_PROD_MAX_SOURCES = " + std::to_string(SP_PROD_MAX_SOURCES));
     for (uint32_t s = 0; s < l.nsources; s++)
@@ -255,7 +258,7 @@ static std::vector<LeafForm> prod_forms(const sp_prod_leaves* leaves, int k, int
   if (leaves)
     for (int c = 0; c < k; c++) {
       const sp_prod_leaves& l = leaves[c];
-      const std::string at = what + ": circuit " + std::to_string(c);
+      const std::string at = name(c);
       require_reduced(&l.coeff_mont[0][0], l.nsources, (at + ": coefficient").c_str());
       require_reduced(l.index_coeff_mont, 1, (at + ": index coefficient").c_str());
       require_reduced(l.const_mont, 1, (at + ": constant").c_str());
@@ -265,6 +268,34 @@ static std::vector<LeafForm> prod_forms(const sp_prod_leaves* leaves, int k, int
       f[c].cst = fq_in(l.const_mont);
     }
   return f;
+}
+static std::vector<LeafForm> prod_forms(const sp_prod_leaves* leaves, int k, int ntables, const std::string& what) {
+  prod_counts(leaves, k, ntables, what);
+  return checked_forms(leaves, k, ntables, [&](int c) { return what + ": circuit " + std::to_string(c); });
+}
+// the caller's dot products next to k circuits: 1 <= kd and k + 2 kd <= SP_PROD_MAX_CIRCUITS (the circuits and both halves of every dot product
+// are instances of one batched sumcheck launch)
+static void dotp_counts(int k, int kd, const std::string& what) {
+  if (kd < 1 || k + 2 * (int64_t)kd > SP_PROD_MAX_CIRCUITS)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": " + std::to_string(kd) + " dot products next to " + std::to_string(k) + " circuits; 1 <= kd and k + 2 kd <= SP_PROD_MAX_CIRCUITS = " +
+                                          std::to_string(SP_PROD_MAX_CIRCUITS) + " supported");
+}
+static const char* const DOTP_OPERAND[3] = {"left", "right", "weight"};
+// a checked form on the device: its sources resolved to the tables' device pointers
+static dev::AffineForm device_form(const LeafForm& f, sp_poly* const* tables) {
+  dev::AffineForm p;
+  memset(static_cast<void*>(&p), 0, sizeof p);
+  const Fq one = Fq::one();
+  p.nsrc = f.nsrc;
+  for (uint32_t s = 0; s < f.nsrc; s++) {
+    p.src[s] = tables[f.src[s]]->d.p;
+    p.coeff[s] = f.coeff[s].m;
+    if (f.coeff[s] == one) p.flags |= dev::PROD_UNIT0 << s;
+  }
+  p.idx = f.idx.m; p.cst = f.cst.m;
+  if (!f.idx.is_zero()) p.flags |= dev::PROD_IDX;
+  if (!f.cst.is_zero()) p.flags |= dev::PROD_CST;
+  return p;
 }
 
 extern "C" {
@@ -1682,75 +1713,111 @@ int sp_pc_eval_verify_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t
 
 // ---- product circuits of the caller's tables (product.cpp: prod_*).  Every argument is checked before the first launch or allocation and before
 // the transcript is touched, so a refused call leaves the tables, the transcript and the device memory as they were.
-int sp_prod_build(sp_ctx* ctx, sp_poly* const* tables, int ntables, const sp_prod_leaves* leaves, int k, sp_prod_circuits** out, uint64_t* products_out) {
-  return guarded(ctx, [&] {
-    const std::string what = "prod_build";
-    if (!out || !products_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
-    prod_counts(leaves, k, ntables, what);   // before any table is looked at
-    const size_t m = log2_ceil(caller_tables(ctx, tables, ntables, what, 2).len);
-    const std::vector<LeafForm> f = prod_forms(leaves, k, ntables, what);
-    const Fq one = Fq::one();
-    std::vector<dev::ProdLeaves> d(k);
-    for (int c = 0; c < k; c++) {
-      dev::ProdLeaves& p = d[c];
-      memset(static_cast<void*>(&p), 0, sizeof p);
-      p.nsrc = f[c].nsrc;
-      for (uint32_t s = 0; s < f[c].nsrc; s++) {
-        p.src[s] = tables[f[c].src[s]]->d.p;
-        p.coeff[s] = f[c].coeff[s].m;
-        if (f[c].coeff[s] == one) p.flags |= dev::PROD_UNIT0 << s;
-      }
-      p.idx = f[c].idx.m; p.cst = f[c].cst.m;
-      if (!f[c].idx.is_zero()) p.flags |= dev::PROD_IDX;
-      if (!f[c].cst.is_zero()) p.flags |= dev::PROD_CST;
-    }
-    std::unique_ptr<sp_prod_circuits> h(new sp_prod_circuits{&ctx->c, m, {}, false});
-    put_scalars(products_out, prod_build(ctx->c, d, (size_t)1 << m, h->cs));
-    *out = h.release();
+// the body of sp_prod_build (dotp_forms NULL, kd = 0) and sp_prod_build_dotp
+static void prod_build_entry(sp_ctx* ctx, sp_poly* const* tables, int ntables, const sp_prod_leaves* leaves, int k, const sp_prod_leaves* dotp_forms, int kd,
+                             sp_prod_circuits** out, uint64_t* products_out, uint64_t* dotp_claims_out, const std::string& what) {
+  if (!out || !products_out || (kd && (!dotp_forms || !dotp_claims_out))) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  prod_counts(leaves, k, ntables, what);   // before any table is looked at
+  if (dotp_forms) dotp_counts(k, kd, what);
+  const size_t m = log2_ceil(caller_tables(ctx, tables, ntables, what, 2).len);
+  const std::vector<LeafForm> f = prod_forms(leaves, k, ntables, what);
+  const std::vector<LeafForm> g = checked_forms(dotp_forms, 3 * kd, ntables, [&](int c) {
+    return what + ": dot product " + std::to_string(c / 3) + " " + DOTP_OPERAND[c % 3];
   });
+  std::vector<dev::ProdLeaves> d(k);
+  for (int c = 0; c < k; c++) d[c] = dev::ProdLeaves{device_form(f[c], tables), nullptr, nullptr};
+  std::vector<dev::DotpOperands> dd(kd);
+  for (int i = 0; i < kd; i++) dd[i] = dev::DotpOperands{{device_form(g[3 * i], tables), device_form(g[3 * i + 1], tables), device_form(g[3 * i + 2], tables)}, nullptr};
+  std::unique_ptr<sp_prod_circuits> h(new sp_prod_circuits{&ctx->c, m, {}, false, {}});
+  put_scalars(products_out, prod_build(ctx->c, d, dd, (size_t)1 << m, h->cs, h->dotps));
+  for (size_t j = 0; j < h->dotps.d.size(); j++) fq_out(dotp_claims_out + 4 * j, h->dotps.d[j].claim);
+  *out = h.release();
+}
+
+int sp_prod_build(sp_ctx* ctx, sp_poly* const* tables, int ntables, const sp_prod_leaves* leaves, int k, sp_prod_circuits** out, uint64_t* products_out) {
+  return guarded(ctx, [&] { prod_build_entry(ctx, tables, ntables, leaves, k, nullptr, 0, out, products_out, nullptr, "prod_build"); });
+}
+
+int sp_prod_build_dotp(sp_ctx* ctx, sp_poly* const* tables, int ntables, const sp_prod_leaves* leaves, int k, const sp_prod_leaves* dotp_forms, int kd,
+                       sp_prod_circuits** out, uint64_t* products_out, uint64_t* dotp_claims_out) {
+  return guarded(ctx, [&] {
+    const std::string what = "prod_build_dotp";
+    if (!dotp_forms || !dotp_claims_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    prod_build_entry(ctx, tables, ntables, leaves, k, dotp_forms, kd, out, products_out, dotp_claims_out, what);
+  });
+}
+
+// the body of sp_prod_prove_t (dotp_evals_out NULL: refuses a handle with dot products) and sp_prod_prove_dotp_t
+static void prod_prove_entry(sp_ctx* ctx, sp_prod_circuits* c, uint8_t* strobe_state, uint8_t** proof, size_t* proof_len, uint64_t* rand_out,
+                             uint64_t* leaf_evals_out, uint64_t* dotp_evals_out, bool with_dotp, const std::string& what) {
+  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+  ta.check();
+  if (!proof || !proof_len || !rand_out || !leaf_evals_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  require_owned(ctx, c, what, "circuits handle");
+  if (c->spent) throw SpError(SP_ERR_INVALID_ARG, what + ": the circuits were consumed by an earlier proof (their layers are bound in place)");
+  if (!c->dotps.d.empty() && !with_dotp)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": the circuits hold dot products, whose evaluations only sp_prod_prove_dotp_t returns");
+  if (!c->dotps.d.empty() && !dotp_evals_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  std::vector<ProdCircuit*> cs;
+  for (auto& p : c->cs) cs.push_back(p.get());
+  Transcript T = ta.open();
+  c->spent = true;
+  ProductCircuitEvalProofBatched P;
+  std::vector<Fq> rand, evals, dotp_evals;
+  prod_prove(ctx->c, cs, c->dotps.d, T, P, rand, evals, dotp_evals);
+  c->cs.clear();
+  c->dotps = ProdDotps();
+  ta.close(T);
+  put_bytes(proof, proof_len, to_bincode(P));
+  put_scalars(rand_out, rand);
+  put_scalars(leaf_evals_out, evals);
+  if (dotp_evals_out) put_scalars(dotp_evals_out, dotp_evals);
 }
 
 int sp_prod_prove_t(sp_ctx* ctx, sp_prod_circuits* c, uint8_t* strobe_state, uint8_t** proof, size_t* proof_len, uint64_t* rand_out, uint64_t* leaf_evals_out) {
-  return guarded(ctx, [&] {
-    const std::string what = "prod_prove";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
-    if (!proof || !proof_len || !rand_out || !leaf_evals_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
-    require_owned(ctx, c, what, "circuits handle");
-    if (c->spent) throw SpError(SP_ERR_INVALID_ARG, what + ": the circuits were consumed by an earlier proof (their layers are bound in place)");
-    std::vector<ProdCircuit*> cs;
-    for (auto& p : c->cs) cs.push_back(p.get());
-    Transcript T = ta.open();
-    c->spent = true;
-    ProductCircuitEvalProofBatched P;
-    std::vector<Fq> rand, evals;
-    prod_prove(ctx->c, cs, T, P, rand, evals);
-    c->cs.clear();
-    ta.close(T);
-    put_bytes(proof, proof_len, to_bincode(P));
-    put_scalars(rand_out, rand);
-    put_scalars(leaf_evals_out, evals);
-  });
+  return guarded(ctx, [&] { prod_prove_entry(ctx, c, strobe_state, proof, proof_len, rand_out, leaf_evals_out, nullptr, false, "prod_prove"); });
+}
+
+int sp_prod_prove_dotp_t(sp_ctx* ctx, sp_prod_circuits* c, uint8_t* strobe_state, uint8_t** proof, size_t* proof_len, uint64_t* rand_out,
+                         uint64_t* leaf_evals_out, uint64_t* dotp_evals_out) {
+  return guarded(ctx, [&] { prod_prove_entry(ctx, c, strobe_state, proof, proof_len, rand_out, leaf_evals_out, dotp_evals_out, true, "prod_prove_dotp"); });
 }
 
 void sp_prod_free(sp_prod_circuits* c) { delete c; }
+
+// the body of sp_prod_verify_t (kd = 0) and sp_prod_verify_dotp_t; host only
+static void prod_verify_entry(const uint8_t* proof, size_t proof_len, const uint64_t* products, int k, const uint64_t* dotp_claims, int kd, size_t m,
+                              uint8_t* strobe_state, uint64_t* rand_out, uint64_t* leaf_claims_out, uint64_t* dotp_claims_out, const std::string& what) {
+  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+  ta.check();
+  if ((!proof && proof_len) || !products || !rand_out || !leaf_claims_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  require_count(what, k, "products", "SP_PROD_MAX_CIRCUITS", SP_PROD_MAX_CIRCUITS);
+  if (dotp_claims) dotp_counts(k, kd, what);
+  if (m < 1 || m > PROD_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": m = " + std::to_string(m) + "; 1 .. " + std::to_string(PROD_MAX_VARS) + " supported");
+  require_reduced(products, (size_t)k, (what + ": product").c_str());
+  require_reduced(dotp_claims, 2 * (size_t)kd, (what + ": dotp claim").c_str());
+  Transcript T = ta.open();
+  TranscriptClose close{ta, T};
+  const BatchedOut o = prod_verify(proof, proof_len, fq_vec(products, (size_t)k), fq_vec(dotp_claims, 2 * (size_t)kd), m, T);
+  put_scalars(rand_out, o.rand);
+  put_scalars(leaf_claims_out, o.claims);
+  if (dotp_claims_out) put_scalars(dotp_claims_out, o.claims_dotp);
+}
 
 // host only: no device work, so ctx may be NULL (the message then goes where sp_last_error(NULL) reads it)
 int sp_prod_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const uint64_t* products, int k, size_t m, uint8_t* strobe_state, uint64_t* rand_out,
                      uint64_t* leaf_claims_out) {
   return host_guarded(ctx, [&] {
-    const std::string what = "prod_verify";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
-    if ((!proof && proof_len) || !products || !rand_out || !leaf_claims_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
-    require_count(what, k, "products", "SP_PROD_MAX_CIRCUITS", SP_PROD_MAX_CIRCUITS);
-    if (m < 1 || m > PROD_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": m = " + std::to_string(m) + "; 1 .. " + std::to_string(PROD_MAX_VARS) + " supported");
-    require_reduced(products, (size_t)k, "prod_verify: product");
-    Transcript T = ta.open();
-    TranscriptClose close{ta, T};
-    const BatchedOut o = prod_verify(proof, proof_len, fq_vec(products, (size_t)k), m, T);
-    put_scalars(rand_out, o.rand);
-    put_scalars(leaf_claims_out, o.claims);
+    prod_verify_entry(proof, proof_len, products, k, nullptr, 0, m, strobe_state, rand_out, leaf_claims_out, nullptr, "prod_verify");
+  });
+}
+
+int sp_prod_verify_dotp_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const uint64_t* products, int k, const uint64_t* dotp_claims, int kd, size_t m,
+                          uint8_t* strobe_state, uint64_t* rand_out, uint64_t* leaf_claims_out, uint64_t* dotp_claims_out) {
+  return host_guarded(ctx, [&] {
+    const std::string what = "prod_verify_dotp";
+    if (!dotp_claims || !dotp_claims_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    prod_verify_entry(proof, proof_len, products, k, dotp_claims, kd, m, strobe_state, rand_out, leaf_claims_out, dotp_claims_out, what);
   });
 }
 

@@ -117,6 +117,8 @@ struct XRank {
 
 // scratch: >= sc_scratch_bytes(); out: ninst*3 scalars [e0,e2,e3] (e3 = 0 for SC_QUAD), device memory
 size_t sc_scratch_bytes(int ninst);
+// out[i] = tables[i][0] for count <= HEADS_PER_LAUNCH tables (the kernel parameter holds that many pointers)
+constexpr int HEADS_PER_LAUNCH = 64;
 void heads(u256* out, const u256* const* tables, int count, cudaStream_t s, HostSig sig = HostSig());
 void sc_eval(ScKind kind, const ScInst* d_insts, int ninst, size_t len, u256* out, void* scratch, cudaStream_t s, HostSig sig = HostSig(), const XRank& xr = XRank());
 // fold every table of every instance by r (len -> len/2, in place) and evaluate the next round on the result; r travels as a kernel argument.
@@ -162,18 +164,32 @@ size_t bound_rows_many_scratch(int k, size_t L_size, size_t R_size);   // scalar
 void bound_rows_many(u256* out, const u256* const* tables, int k, const u256* L, size_t L_size, size_t R_size, u256* scratch, cudaStream_t s);
 void lincomb3(u256* out, const u256* A, const u256* B, const u256* C, const u256* d_rabc /*3*/, size_t n, cudaStream_t s);
 void hadamard_many(u256* const* outs, const u256* const* as, const u256* const* bs, int count, size_t n, cudaStream_t s);
-// ---- the leaves of the caller's product circuits (sp_prod_build): leaf[x] = cst + idx * x + sum_{s < nsrc} coeff[s] * src[s][x] for x < n, written
-// to layer0 (n entries), and layer1[x] = leaf[x] * leaf[x + n/2] for x < n/2 (the first product layer) when layer1 is set.  The sources are only read.
+// ---- the leaves of the caller's product circuits (sp_prod_build) and the operands of their dot products (sp_prod_build_dotp): affine forms
+// form[x] = cst + idx * x + sum_{s < nsrc} coeff[s] * src[s][x] of the caller's tables, which are only read
 enum { PROD_UNIT0 = 1 /* bit s: coeff[s] is one */, PROD_IDX = 8 /* idx != 0 */, PROD_CST = 16 /* cst != 0 */ };
-struct ProdLeaves {
+struct AffineForm {
   const u256* src[SP_PROD_MAX_SOURCES];
   u256 coeff[SP_PROD_MAX_SOURCES], idx, cst;   // Montgomery form
+  uint32_t nsrc, flags;
+};
+// a circuit's leaves: the form for x < n written to layer0 (n entries), and layer1[x] = leaf[x] * leaf[x + n/2] for x < n/2 (the first product
+// layer) when layer1 is set
+struct ProdLeaves {
+  AffineForm f;
   u256* layer0;
   u256* layer1;
-  uint32_t nsrc, flags;
 };
 // k <= SP_PROD_MAX_CIRCUITS circuits of n >= 2 leaves each, in one launch (blockIdx.y = circuit)
 void prod_leaves(const ProdLeaves* circuits, int k, size_t n, cudaStream_t s);
+// a dot product sum_x left[x] right[x] weight[x]: its three operand forms, written for x < n to out = [left | right | weight] (3n entries)
+constexpr int PROD_MAX_DOTP = (SP_PROD_MAX_CIRCUITS - 1) / 2;   // one circuit and the two halves of each dot product in one batched sumcheck
+struct DotpOperands {
+  AffineForm f[3];   // left, right, weight
+  u256* out;
+};
+// kd <= PROD_MAX_DOTP dot products of n >= 2 entries each in one launch (blockIdx.y = dot product): the operands, and half_sums[2d + h] = the sum
+// of left * right * weight over half h (entries [h n/2, (h + 1) n/2)) of dot product d.  scratch: Ctx::red (>= sc_scratch_bytes(SC_MAX_INST))
+void dotp_operands(const DotpOperands* dotps, int kd, size_t n, u256* half_sums, void* scratch, cudaStream_t s);
 void to_canonical(u256* out, const u256* in, size_t n, cudaStream_t s);   // Montgomery -> canonical little-endian integers (transcript bytes)
 void gather(u256* out, const u256* mem, const uint32_t* idx, size_t n, cudaStream_t s);
 // hash layer of the SPARK memory check: out = ts*r^2 + val*r + addr - g  (sparse_mlpoly.rs:545-600)

@@ -68,7 +68,8 @@ constexpr Region SMALL_IPA_C{16, 16};    // c_L, c_R of an inner-product round
 constexpr Region SMALL_DOT{32, 8};       // shared: one dot product (r1cs_prove, sp_dot, sp_poly_evaluate)
 constexpr Region SMALL_ABC{40, 8};       // the matrices at (rx, ry) (sparse_evaluate)
 constexpr Region SMALL_DOTP{48, 16};     // the two halves of a dot-product circuit's claim (snark_prove)
-constexpr Region SMALL_BATCH{64, 128};   // shared: batched_prove's 3 evaluations per instance; after it, spark_eval_prove's 7b + 2 hash-layer evaluations
+constexpr Region SMALL_BATCH{64, 128};   // shared: batched_prove's 3 evaluations per instance; after it, spark_eval_prove's 7b + 2 hash-layer evaluations;
+                                         // before it, prod_build's two half sums per dot product
 constexpr Region SMALL_ONES{4000, 2};    // Ctx::ones()
 // Ctx::pinned (mapped host memory), in bytes
 constexpr size_t PINNED_BYTES = 1 << 20;
@@ -97,15 +98,16 @@ SP_APART(SMALL_ROUND, SMALL_HEADS); SP_APART(SMALL_HEADS, SMALL_IPA_C); SP_APART
 SP_APART(SMALL_ABC, SMALL_DOTP); SP_APART(SMALL_DOTP, SMALL_BATCH); SP_APART(SMALL_BATCH, SMALL_ONES);
 static_assert(SMALL_ONES.end() <= SMALL_SCALARS, "SMALL_ONES ends outside Ctx::small");
 SP_HOLDS(SMALL_ROUND, 3); SP_HOLDS(SMALL_ROUND, SP_SC_MAX_DEGREE); SP_HOLDS(SMALL_HEADS, SP_SC_MAX_TABLES); SP_HOLDS(SMALL_IPA_C, 2); SP_HOLDS(SMALL_DOT, 1);
-SP_HOLDS(SMALL_ABC, SP_SPARK_MAX_BATCH); SP_HOLDS(SMALL_DOTP, 2); SP_HOLDS(SMALL_BATCH, 3 * dev::SC_MAX_INST); SP_HOLDS(SMALL_BATCH, 7 * SP_SPARK_MAX_BATCH + 2); SP_HOLDS(SMALL_ONES, 2);
+SP_HOLDS(SMALL_ABC, SP_SPARK_MAX_BATCH); SP_HOLDS(SMALL_DOTP, 2); SP_HOLDS(SMALL_BATCH, 3 * dev::SC_MAX_INST); SP_HOLDS(SMALL_BATCH, 7 * SP_SPARK_MAX_BATCH + 2); SP_HOLDS(SMALL_BATCH, 2 * dev::PROD_MAX_DOTP); SP_HOLDS(SMALL_ONES, 2);
 SP_APART(PIN_STAGE, PIN_ZKPRE); SP_APART(PIN_ZKPRE, PIN_RES); SP_APART(PIN_RES, PIN_FLAG); SP_APART(PIN_FLAG, PIN_FLAG_C); SP_APART(PIN_FLAG_C, PIN_XY);
 static_assert(PIN_XY.end() <= PINNED_BYTES, "PIN_XY ends outside Ctx::pinned");
 SP_HOLDS(PIN_STAGE, SMALL_BATCH.cap * sizeof(u256));   // get_small of any whole region of Ctx::small
 SP_HOLDS(PIN_STAGE, 2 * sizeof(u256) * dev::SC_MAX_INST); SP_HOLDS(PIN_STAGE, 4 * sizeof(u256));   // batched_prove's entries; a ZK sumcheck's 4 tables
+SP_HOLDS(PIN_STAGE, 2 * sizeof(u256) * SP_PROD_MAX_CIRCUITS);   // prod_build's two last-layer entries per circuit and two half sums per dot product
 SP_HOLDS(PIN_RES, RES_OUT.end() * sizeof(u256));
 SP_APART(RES_IPA_C, RES_POINTS);
 static_assert(RES_POINTS.end() <= RES_OUT.end(), "RES_POINTS ends outside RES_OUT");
-SP_HOLDS(RES_OUT, (3 + 6) * dev::SC_MAX_INST); SP_HOLDS(RES_OUT, 64 /* dev::heads refuses more tables */); SP_HOLDS(RES_OUT, 2 * 2 * (2 + 2 * SP_SPARK_MAX_BATCH) /* spark_eval_prove heads */); SP_HOLDS(RES_POINTS, 2 * sizeof(ge) / sizeof(u256));
+SP_HOLDS(RES_OUT, (3 + 6) * dev::SC_MAX_INST); SP_HOLDS(RES_OUT, 3 * dev::SC_MAX_INST /* batched_prove's heads: two per product instance, three per dot-product instance */); SP_HOLDS(RES_OUT, 2 * 2 * (2 + 2 * SP_SPARK_MAX_BATCH) /* spark_eval_prove heads */); SP_HOLDS(RES_POINTS, 2 * sizeof(ge) / sizeof(u256));
 SP_APART(SIG_DONE, SIG_MSM_TICKET); SP_APART(SIG_MSM_TICKET, SIG_DONE_C);
 static_assert(SIG_DONE_C.end() <= SIG_WORDS, "SIG_DONE_C ends outside Ctx::sig_done");
 #undef SP_APART

@@ -14,6 +14,7 @@
 //   K7     eq_evals, dot, bound_rows, lincomb3, hadamard, spmv, SPARK hash layer, IPA helpers.
 // All arithmetic is exact 256-bit integer work on the INT32 pipe; no tensor-core formulation exists (DESIGN.md).
 #include <cuda_runtime.h>
+#include <algorithm>
 #include <stdexcept>
 #include <string>
 #include <map>
@@ -340,8 +341,8 @@ void dot_many(u256* out, const u256* const* a_list, int count, const u256* b, si
 }
 
 // first elements of up to 64 tables -> one contiguous array (+ the host, through HostSig): the layer claims of the batched product proofs
-struct HeadBatch { const u256* p[64]; };
-__global__ void __launch_bounds__(64) k_heads(HeadBatch hb, int count, u256* out, HostSig sig) {
+struct HeadBatch { const u256* p[HEADS_PER_LAUNCH]; };
+__global__ void __launch_bounds__(HEADS_PER_LAUNCH) k_heads(HeadBatch hb, int count, u256* out, HostSig sig) {
   if ((int)threadIdx.x < count) {
     u256 v = ld256(hb.p[threadIdx.x]);
     st256(out + threadIdx.x, v);
@@ -354,10 +355,10 @@ __global__ void __launch_bounds__(64) k_heads(HeadBatch hb, int count, u256* out
   }
 }
 void heads(u256* out, const u256* const* tables, int count, cudaStream_t s, HostSig sig) {
-  if (count > 64) throw std::runtime_error("spartan_b200: heads supports at most 64 tables");
+  if (count > HEADS_PER_LAUNCH) throw std::runtime_error("spartan_b200: heads supports at most " + std::to_string(HEADS_PER_LAUNCH) + " tables");
   HeadBatch hb;
   for (int i = 0; i < count; i++) hb.p[i] = tables[i];
-  k_heads<<<1, 64, 0, s>>>(hb, count, out, sig);
+  k_heads<<<1, HEADS_PER_LAUNCH, 0, s>>>(hb, count, out, sig);
   SP_LAUNCHED(); check("heads");
 }
 
@@ -463,27 +464,30 @@ void hadamard_many(u256* const* outs, const u256* const* as, const u256* const* 
 // CUDA >= 12.1 (up to 32764 bytes), so the launch needs no descriptor upload, no device allocation and no copy ahead of it.
 struct ProdBatch { ProdLeaves c[SP_PROD_MAX_CIRCUITS]; };
 static_assert(sizeof(ProdBatch) + sizeof(size_t) <= 32764, "k_prod_leaves: the descriptors exceed the kernel parameter space");
-__device__ __forceinline__ u256 prod_leaf(const ProdLeaves& d, const u256& idx_r2, size_t x) {
-  u256 v = d.flags & PROD_CST ? d.cst : fq_zero();
-  if (d.flags & PROD_IDX) {   // idx * x in Montgomery form: idx * R^2 times the plain integer x, one product
+// idx * R^2, so that idx * x in Montgomery form is one product with the plain integer x
+__device__ __forceinline__ u256 form_idx_r2(const AffineForm& f) { return f.flags & PROD_IDX ? fq_mul(f.idx, fq_R2()) : fq_zero(); }
+// the form at entry x: cst + idx * x + sum_s coeff[s] * src[s][x]
+__device__ __forceinline__ u256 form_at(const AffineForm& f, const u256& idx_r2, size_t x) {
+  u256 v = f.flags & PROD_CST ? f.cst : fq_zero();
+  if (f.flags & PROD_IDX) {
     u256 xi = fq_zero();
     xi.v[0] = (uint32_t)x; xi.v[1] = (uint32_t)(x >> 32);
     v = fq_add(v, fq_mul(idx_r2, xi));
   }
 #pragma unroll
   for (int s = 0; s < SP_PROD_MAX_SOURCES; s++) {
-    if ((uint32_t)s >= d.nsrc) break;
-    const u256 t = ld256_ro(d.src[s] + x);
-    v = fq_add(v, (d.flags >> s) & PROD_UNIT0 ? t : fq_mul(d.coeff[s], t));
+    if ((uint32_t)s >= f.nsrc) break;
+    const u256 t = ld256_ro(f.src[s] + x);
+    v = fq_add(v, (f.flags >> s) & PROD_UNIT0 ? t : fq_mul(f.coeff[s], t));
   }
   return v;
 }
 // a thread owns the pair (x, x + n/2): both leaves, and their product, the entry x of the first product layer
 __global__ void __launch_bounds__(256) k_prod_leaves(const ProdBatch b, size_t half) {
   const ProdLeaves& d = b.c[blockIdx.y];
-  const u256 idx_r2 = d.flags & PROD_IDX ? fq_mul(d.idx, fq_R2()) : fq_zero();
+  const u256 idx_r2 = form_idx_r2(d.f);
   for (size_t x = (size_t)blockIdx.x * blockDim.x + threadIdx.x; x < half; x += (size_t)gridDim.x * blockDim.x) {
-    const u256 lo = prod_leaf(d, idx_r2, x), hi = prod_leaf(d, idx_r2, x + half);
+    const u256 lo = form_at(d.f, idx_r2, x), hi = form_at(d.f, idx_r2, x + half);
     st256(d.layer0 + x, lo);
     st256(d.layer0 + x + half, hi);
     if (d.layer1) st256(d.layer1 + x, fq_mul(lo, hi));
@@ -493,11 +497,60 @@ void prod_leaves(const ProdLeaves* circuits, int k, size_t n, cudaStream_t s) {
   if (k < 1 || k > SP_PROD_MAX_CIRCUITS || n < 2) throw std::runtime_error("spartan_b200: prod_leaves takes 1 .. SP_PROD_MAX_CIRCUITS circuits of >= 2 leaves");
   double bytes = 0;
   ProdBatch b;
-  for (int i = 0; i < k; i++) { b.c[i] = circuits[i]; bytes += (double)n * (32.0 * (circuits[i].nsrc + 1) + (circuits[i].layer1 ? 16.0 : 0.0)); }
+  for (int i = 0; i < k; i++) { b.c[i] = circuits[i]; bytes += (double)n * (32.0 * (circuits[i].f.nsrc + 1) + (circuits[i].layer1 ? 16.0 : 0.0)); }
   ProfScope ps("prod_leaves", bytes, s);
   dim3 grid(grid_for(n / 2, 256, 4), k);
   k_prod_leaves<<<grid, 256, 0, s>>>(b, n / 2);
   SP_LAUNCHED(); check("prod_leaves");
+}
+struct DotpBatch { DotpOperands d[PROD_MAX_DOTP]; };
+static_assert(sizeof(DotpBatch) + 2 * sizeof(void*) + 2 * sizeof(size_t) <= 32764, "k_dotp_operands: the descriptors exceed the kernel parameter space");
+// a thread owns the pair (x, x + n/2): the three operands at both entries, and left * right * weight added to the sum of its half
+__global__ void __launch_bounds__(256) k_dotp_operands(const DotpBatch b, size_t half, u256* partials, unsigned int* counters, u256* out) {
+  const DotpOperands& d = b.d[blockIdx.y];
+  const size_t n = 2 * half;
+  u256 idx_r2[3];
+#pragma unroll
+  for (int o = 0; o < 3; o++) idx_r2[o] = form_idx_r2(d.f[o]);
+  u256 acc[2] = {fq_zero(), fq_zero()};
+  for (size_t x = (size_t)blockIdx.x * blockDim.x + threadIdx.x; x < half; x += (size_t)gridDim.x * blockDim.x) {
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const size_t at = x + h * half;
+      u256 prod = fq_one();
+#pragma unroll
+      for (int o = 0; o < 3; o++) {
+        const u256 v = form_at(d.f[o], idx_r2[o], at);
+        st256(d.out + o * n + at, v);
+        prod = o ? fq_mul(prod, v) : v;
+      }
+      acc[h] = fq_add(acc[h], prod);
+    }
+  }
+  block_reduce_finish<2>(acc, partials, counters, out, 2);
+}
+void dotp_operands(const DotpOperands* dotps, int kd, size_t n, u256* half_sums, void* scratch, cudaStream_t s) {
+  if (kd < 1 || kd > PROD_MAX_DOTP || n < 2) throw std::runtime_error("spartan_b200: dotp_operands takes 1 .. PROD_MAX_DOTP dot products of >= 2 entries");
+  double bytes = 96.0 * (double)n * kd;   // the operands written; each distinct source table read once
+  const u256* seen[3 * PROD_MAX_DOTP * SP_PROD_MAX_SOURCES];
+  int ns = 0;
+  DotpBatch b;
+  for (int i = 0; i < kd; i++) {
+    b.d[i] = dotps[i];
+    for (int o = 0; o < 3; o++)
+      for (uint32_t t = 0; t < dotps[i].f[o].nsrc; t++) {
+        const u256* p = dotps[i].f[o].src[t];
+        if (std::find(seen, seen + ns, p) == seen + ns) { seen[ns++] = p; bytes += 32.0 * (double)n; }
+      }
+  }
+  ProfScope ps("dotp_operands", bytes, s);
+  // the partial sums of every block, two per block and dot product, in the reduction scratch the sumcheck rounds use
+  const size_t cap = (sc_scratch_bytes(SC_MAX_INST) - 256) / (2 * sizeof(u256) * (size_t)kd);
+  dim3 grid(std::min<size_t>(grid_for(n / 2, 256, 4), cap), kd);
+  unsigned int* counters = (unsigned int*)scratch;
+  u256* partials = (u256*)((char*)scratch + 256);
+  k_dotp_operands<<<grid, 256, 0, s>>>(b, n / 2, partials, counters, half_sums);
+  SP_LAUNCHED(); check("dotp_operands");
 }
 __global__ void k_to_canonical(u256* out, const u256* __restrict__ in, size_t n) {   // Scalar::to_bytes (ristretto255.rs:419) for a whole vector
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) st256(out + i, fq_from_mont(ld256_ro(in + i)));

@@ -50,7 +50,7 @@ void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vector<DotpC
   const size_t G_MIN = 2 * Ctx::SHARD_MIN_LOCAL;   // 16384 entries per table: the fused G kernel then always streams >= 32768
   u256* d_out = ctx.small.p + layout::SMALL_BATCH.off;   // ninst * 3 scalars
   u256* const h_out = ctx.host_res + layout::RES_OUT.off;   // where they reach the host
-  DevBuf<u256> d_heads(64);
+  DevBuf<u256> d_heads(3 * dev::SC_MAX_INST);
   const int logW = (int)log2_ceil(W);
   // a layer's sumcheck runs on tables of half = len/2 entries (num_rounds variables), lhalf of them on this rank while the layer is sharded
   struct Shape { size_t half, num_rounds, lhalf; bool sh; int logW; };
@@ -231,8 +231,9 @@ void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vector<DotpC
       const Fq& r = rand_prod.back();
       for (size_t k = 0; k < 3 * ninst; k++) heads[k] = bound[2 * k] + r * (bound[2 * k + 1] - bound[2 * k]);
       if (layer_id > 0) build_eq(shape_of(layer_id - 1), rand_prod);
-    } else {  // layers of fewer than two rounds: one gather kernel that also publishes the values to the host.  It takes A and B of a product
-              // instance and A, B and C of a dot-product circuit: 2 * SC_MAX_INST heads for a batch of product circuits alone, within its 64
+    } else {  // layers of fewer than two rounds: a gather kernel that also publishes the values to the host.  It takes A and B of a product
+              // instance and A, B and C of a dot-product circuit, at most 3 * SC_MAX_INST heads, in launches of at most HEADS_PER_LAUNCH; the last
+              // one publishes the flag, after the earlier launches' values (stream order)
       std::vector<const u256*> hp;
       for (size_t i = 0; i < ninst; i++) {
         const dev::ScInst& in = sc.insts[i];
@@ -240,7 +241,13 @@ void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vector<DotpC
         if (i >= np) hp.push_back(in.t[2]);
       }
       dev::HostSig hs = ctx.next_sig();
-      dev::heads(d_heads.p, hp.data(), (int)hp.size(), ctx.stream, hs);
+      for (size_t at = 0; at < hp.size(); at += dev::HEADS_PER_LAUNCH) {
+        const size_t cnt = std::min<size_t>(dev::HEADS_PER_LAUNCH, hp.size() - at);
+        dev::HostSig part = hs;
+        part.host_out = hs.host_out + at;
+        if (at + cnt < hp.size()) part.flag = nullptr;
+        dev::heads(d_heads.p + at, hp.data() + at, (int)cnt, ctx.stream, part);
+      }
       if (layer_id > 0) build_eq(shape_of(layer_id - 1), rand_prod);
       ctx.wait_sig(hs);
       std::vector<Fq> got(hp.size());
@@ -277,9 +284,22 @@ void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vector<DotpC
 }
 
 // ================================================================================================ the caller's circuits (sp_prod_*)
-std::vector<Fq> prod_build(Ctx& ctx, std::vector<dev::ProdLeaves> leaves, size_t n, std::vector<std::unique_ptr<ProdCircuit>>& out) {
-  const size_t k = leaves.size();
+std::vector<Fq> prod_build(Ctx& ctx, std::vector<dev::ProdLeaves> leaves, std::vector<dev::DotpOperands> dotps, size_t n,
+                           std::vector<std::unique_ptr<ProdCircuit>>& out, ProdDotps& dout) {
+  const size_t k = leaves.size(), kd = dotps.size();
   out.clear();
+  dout = ProdDotps();
+  if (kd) {   // DotProductCircuit::split of each dot product d into its halves [0, n/2) and [n/2, n): circuits 2d and 2d + 1, the reference's order
+    dout.ops.alloc(3 * n * kd);
+    for (size_t d = 0; d < kd; d++) {
+      dotps[d].out = dout.ops.p + 3 * n * d;
+      for (size_t h = 0; h < 2; h++) {
+        u256* base = dotps[d].out + h * (n / 2);
+        dout.d.push_back(DotpCircuit{base, base + n, base + 2 * n, n / 2, false, Fq::zero()});
+      }
+    }
+    dev::dotp_operands(dotps.data(), (int)kd, n, ctx.small.p + layout::SMALL_BATCH.off, ctx.red.p, ctx.stream);
+  }
   for (size_t i = 0; i < k; i++) {
     out.emplace_back(new ProdCircuit);
     out[i]->alloc(ctx, n);   // no ShardScope: one rank's GPU, W = 1
@@ -296,22 +316,32 @@ std::vector<Fq> prod_build(Ctx& ctx, std::vector<dev::ProdLeaves> leaves, size_t
     build_circuits(ctx, grp, 1);
     first += cnt;
   }
-  // ProductCircuit::evaluate: the two entries of every last layer, with one synchronise
+  // ProductCircuit::evaluate: the two entries of every last layer, and DotProductCircuit::evaluate of every half, with one synchronise
   uint8_t* stage = ctx.pinned + layout::PIN_STAGE.off;
   for (size_t i = 0; i < k; i++) dev::d2h(stage + 64 * i, out[i]->layer(out[i]->num_layers - 1), 64, ctx.stream);
+  if (kd) dev::d2h(stage + 64 * k, ctx.small.p + layout::SMALL_BATCH.off, 2 * kd * sizeof(u256), ctx.stream);
   ctx.sync();
   std::vector<Fq> products(k);
   for (size_t i = 0; i < k; i++) { Fq v[2]; memcpy(static_cast<void*>(v), stage + 64 * i, 64); products[i] = v[0] * v[1]; }
+  for (size_t j = 0; j < 2 * kd; j++) memcpy(static_cast<void*>(&dout.d[j].claim), stage + 64 * k + sizeof(u256) * j, sizeof(u256));
   return products;
 }
 
-void prod_prove(Ctx& ctx, std::vector<ProdCircuit*>& cs, Transcript& T, ProductCircuitEvalProofBatched& out, std::vector<Fq>& rand, std::vector<Fq>& leaf_evals) {
-  std::vector<DotpCircuit> none;
-  batched_prove(ctx, cs, none, T, out, rand);
-  // the claims layer 0's proof leaves (product_tree.rs:373-375): left + r_layer (right - left), r_layer = rand[0]
+void prod_prove(Ctx& ctx, std::vector<ProdCircuit*>& cs, std::vector<DotpCircuit>& dotps, Transcript& T, ProductCircuitEvalProofBatched& out,
+                std::vector<Fq>& rand, std::vector<Fq>& leaf_evals, std::vector<Fq>& dotp_evals) {
+  batched_prove(ctx, cs, dotps, T, out, rand);
+  // the claims layer 0's proof leaves (product_tree.rs:373-375): left + r_layer (right - left), r_layer = rand[0]; for a dot product, its two
+  // halves' final claims combined the same way, as the verifier combines claims_dotp[2k] and [2k + 1] (:385-485)
   const LayerProofBatched& l0 = out.proof.back();
+  auto at_rand = [&](const Fq& lo, const Fq& hi) { return lo + rand[0] * (hi - lo); };
   leaf_evals.resize(cs.size());
-  for (size_t i = 0; i < cs.size(); i++) leaf_evals[i] = l0.claims_prod_left[i] + rand[0] * (l0.claims_prod_right[i] - l0.claims_prod_left[i]);
+  for (size_t i = 0; i < cs.size(); i++) leaf_evals[i] = at_rand(l0.claims_prod_left[i], l0.claims_prod_right[i]);
+  dotp_evals.clear();
+  for (size_t d = 0; d + 1 < dotps.size(); d += 2) {
+    dotp_evals.push_back(at_rand(out.dotp_left[d], out.dotp_left[d + 1]));
+    dotp_evals.push_back(at_rand(out.dotp_right[d], out.dotp_right[d + 1]));
+    dotp_evals.push_back(at_rand(out.dotp_weight[d], out.dotp_weight[d + 1]));
+  }
 }
 
 }  // namespace sp

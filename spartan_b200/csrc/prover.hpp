@@ -287,16 +287,22 @@ void batched_prove(Ctx& ctx, std::vector<ProdCircuit*>& prods, std::vector<DotpC
 // what ProductCircuitEvalProofBatched::verify (product_tree.rs:385-485; verifier.cpp: batched_verify) returns: the product circuits' claims about
 // their leaf polynomials at rand, three claims per pair of dot-product circuits, and rand
 struct BatchedOut { std::vector<Fq> claims, claims_dotp, rand; };
-// ProductCircuitEvalProofBatched::verify(products, [], 2^m, T) on bincode bytes (sp_prod_verify_t): SpError(SP_ERR_VERIFY) where the reference
-// asserts or the bytes do not decode
-BatchedOut prod_verify(const uint8_t* proof, size_t len, const std::vector<Fq>& products, size_t m, Transcript& T);
-// The caller's circuits (sp_prod_build): `leaves` without their layer pointers, k <= SP_PROD_MAX_CIRCUITS of them over tables of n = 2^m >= 2
-// entries, on this rank's GPU alone.  Allocates every circuit, writes the leaves and the first product layer in one launch (dev::prod_leaves),
-// the other layers with build_circuits in groups of at most 16, and returns the k products (ProductCircuit::evaluate)
-std::vector<Fq> prod_build(Ctx& ctx, std::vector<dev::ProdLeaves> leaves, size_t n, std::vector<std::unique_ptr<ProdCircuit>>& out);
-// ProductCircuitEvalProofBatched::prove(circuits, [], T) of the caller's circuits (no dot-product circuits), on this rank's GPU alone; leaf_evals:
-// each circuit's leaf polynomial at rand, the claims the verifier is left with
-void prod_prove(Ctx& ctx, std::vector<ProdCircuit*>& cs, Transcript& T, ProductCircuitEvalProofBatched& out, std::vector<Fq>& rand, std::vector<Fq>& leaf_evals);
+// ProductCircuitEvalProofBatched::verify(products, dotp_claims, 2^m, T) on bincode bytes (sp_prod_verify_t with no dotp claims,
+// sp_prod_verify_dotp_t): SpError(SP_ERR_VERIFY) where the reference asserts or the bytes do not decode
+BatchedOut prod_verify(const uint8_t* proof, size_t len, const std::vector<Fq>& products, const std::vector<Fq>& dotp_claims, size_t m, Transcript& T);
+// the caller's dot products, each split into two DotpCircuits (d[2i], d[2i + 1]: the halves of dot product i) whose tables live in `ops`,
+// [left | right | weight] of 2^m entries each per dot product; the claims are the halves' sums
+struct ProdDotps { DevBuf<u256> ops; std::vector<DotpCircuit> d; };
+// The caller's circuits (sp_prod_build, sp_prod_build_dotp): `leaves` without their layer pointers and `dotps` without their output pointers,
+// k + 2 kd <= SP_PROD_MAX_CIRCUITS of them over tables of n = 2^m >= 2 entries, on this rank's GPU alone.  Allocates every circuit, writes the
+// dot products' operands and half sums in one launch (dev::dotp_operands) when kd > 0, the leaves and the first product layer in one launch
+// (dev::prod_leaves), the other layers with build_circuits in groups of at most 16, and returns the k products (ProductCircuit::evaluate)
+std::vector<Fq> prod_build(Ctx& ctx, std::vector<dev::ProdLeaves> leaves, std::vector<dev::DotpOperands> dotps, size_t n,
+                           std::vector<std::unique_ptr<ProdCircuit>>& out, ProdDotps& dout);
+// ProductCircuitEvalProofBatched::prove(circuits, dotps, T) of the caller's circuits, on this rank's GPU alone; leaf_evals: each circuit's leaf
+// polynomial at rand, the claims the verifier is left with; dotp_evals: (left, right, weight) at rand of each dot product (dotps holds its halves)
+void prod_prove(Ctx& ctx, std::vector<ProdCircuit*>& cs, std::vector<DotpCircuit>& dotps, Transcript& T, ProductCircuitEvalProofBatched& out,
+                std::vector<Fq>& rand, std::vector<Fq>& leaf_evals, std::vector<Fq>& dotp_evals);
 
 // <x, G[0..n)> of one row of n scalars against the per-window table of `gs`, for latency.  For n >= 2 (even) it is the inner-product round kernel
 // with a = (1, 1) and blocks of two generators: its "L" (odd j) and "R" (even j) reach the host through the kernel's own publication and are added

@@ -743,9 +743,9 @@ void verify_batch(Ctx& ctx, std::vector<VerifyJob>& jobs, const uint8_t seed[32]
 
 }  // namespace
 
-BatchedOut prod_verify(const uint8_t* proof, size_t len, const std::vector<Fq>& products, size_t m, Transcript& T) {
+BatchedOut prod_verify(const uint8_t* proof, size_t len, const std::vector<Fq>& products, const std::vector<Fq>& dotp_claims, size_t m, Transcript& T) {
   const ProductCircuitEvalProofBatched p = from_bincode<ProductCircuitEvalProofBatched>(proof, len, SP_ERR_VERIFY, "product circuit proof");
-  return batched_verify(p, products, {}, (size_t)1 << m, T);
+  return batched_verify(p, products, dotp_claims, (size_t)1 << m, T);
 }
 
 Fq sumcheck_verify_bytes(const uint8_t* proof, size_t len, const Fq& claim, size_t num_rounds, size_t degree, Transcript& T, std::vector<Fq>& r) {
