@@ -267,7 +267,8 @@ int sp_pc_eval_verify_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t
  * commitment given to a verify that does not decompress.  The verifies return SP_OK when they accept, SP_ERR_VERIFY / SP_ERR_DECOMPRESS when they
  * reject (sp_last_error names the check), and leave the transcript where the reference's verify leaves it.  The sigma protocols commit on the
  * host; each set's host tables are built at its first such use.  On a connected multi-GPU context every entry runs on this rank's GPU alone. */
-/* DotProductProof is linear in n: n <= SP_DOTPROD_MAX_N (a ZK sumcheck's rounds need d + 1 <= 7); longer vectors belong to PolyEvalProof */
+/* DotProductProof is linear in n: n <= SP_DOTPROD_MAX_N (a ZK sumcheck's rounds need d + 1 <= 7); longer vectors belong to DotProductProofLog
+ * (sp_dotlog_prove_t) */
 #define SP_DOTPROD_MAX_N 64
 /* ZKSumcheckInstanceProof::prove_quad / prove_cubic_with_additive_term (sumcheck.rs:428-776) generalised to the composition of
  * sp_sumcheck_prove_t (same tables, terms, num_rounds and refusals; degree d = max nfactors, 1 <= d <= SP_SC_MAX_DEGREE).  The tape draws
@@ -312,6 +313,42 @@ int sp_dotproduct_prove_t(sp_ctx* ctx, const sp_gens* gens_1, const sp_gens* gen
                           uint8_t** proof, size_t* proof_len, uint8_t Cx_out32[32], uint8_t Cy_out32[32]);
 int sp_dotproduct_verify_t(sp_ctx* ctx, const sp_gens* gens_1, const sp_gens* gens_n, uint8_t* strobe_state, const uint64_t* a_vec_mont, size_t n,
                            const uint8_t Cx32[32], const uint8_t Cy32[32], const uint8_t* proof, size_t proof_len);
+
+/* ---- inner products of the caller's committed vectors in logarithmic size: DotProductProofLog (nizk/mod.rs:407-583, nizk/bullet.rs:32-225), the
+ * proof that Cx = <x, G> + blind_x * h commits to a vector x whose inner product with a public vector a is the y of Cy = y * G_n + blind_y * h.
+ * Conventions of the sigma protocols above (transcript and tape advanced and written back only when a prove succeeds, every argument checked
+ * before the first launch, tape draw or transcript write, this rank's GPU alone).  x and a are sp_poly handles of n entries, read and never
+ * modified: the prover folds copies.  Bytes equal the reference's for the same transcript, tape and vectors.
+ *
+ * Two layouts of the generators, chosen by n alone:
+ *   n <= SP_DOTLOG_TABLE_MAX_N: the set sp_pc_gens_create builds for this n (n + 2 points and 8-bit window tables, 393 KB per generator: at most
+ *     about 100 MB); the proof runs the inner-product rounds of PolyEvalProof over the unfolded generators.  256 is the largest n whose n + 2
+ *     generators stay under the 512 from which a set gets a row table and wider windows, gigabytes an inner-product proof never reads.
+ *   larger n: G[0..n) as affine niels points (96 B each, no window tables; 2^24 points take 1.6 GB) and a two-generator set {G_n, h}.  Every
+ *     round folds the generators on the device (H' = H_L + u^2 H_R with G = c * H, one variable-base multiplication per pair) and computes L and
+ *     R by MSMs over the folded halves.  A prove also holds copies of x and a and the round's MSM scalars (32 B per entry each), n/2 folded points
+ *     (96 B each) and the bucket MSM's scratch for n terms (about 100 B per term at n = 2^24): about 3 GB at n = 2^24; a verify holds the vector s
+ *     (32 B per entry) and the same MSM scratch.  All of it is released on return.  DESIGN.md ("Inner products of the caller's vectors") has the numbers. */
+#define SP_DOTLOG_MAX_N (1u << 24)
+#define SP_DOTLOG_TABLE_MAX_N 256
+typedef struct sp_dotlog_gens sp_dotlog_gens;
+/* DotProductProofGens::new(n, label) (nizk/mod.rs:414-419) = MultiCommitGens::new(n + 1, label).split_at(n): gens_n = G[0..n), gens_1 = G[n], both
+ * with h = G[n + 1].  SP_ERR_INVALID_ARG, before any allocation, unless n is a power of two with 1 <= n <= SP_DOTLOG_MAX_N. */
+int sp_dotlog_gens_create(sp_ctx* ctx, size_t n, const uint8_t* label, size_t label_len, sp_dotlog_gens** out);
+void sp_dotlog_gens_free(sp_dotlog_gens* g);
+/* DotProductProofLog::prove(gens, transcript, tape, x_vec, blind_x, a_vec, y, blind_y) -> (proof, Cx, Cy)   nizk/mod.rs:440-525.
+ * y NULL: y = <x, a>, computed on the device; a given y is not checked (neither does the reference): the verifier rejects the proof.  Out: *proof =
+ * bincode(DotProductProofLog) (free with sp_free), Cx, Cy and y_out = the y used.  SP_ERR_INVALID_ARG: a NULL argument, x or a of another context
+ * or of a length other than gens' n; SP_ERR_INVALID_SCALAR: blind_x, y or blind_y not reduced. */
+int sp_dotlog_prove_t(sp_ctx* ctx, const sp_dotlog_gens* gens, uint8_t* strobe_state /* in, out */, uint8_t* tape_state /* in, out */, const sp_poly* x,
+                      const uint64_t blind_x_mont[4], const sp_poly* a, const uint64_t* y_mont /* NULL: <x, a> */, const uint64_t blind_y_mont[4],
+                      uint8_t** proof, size_t* proof_len, uint8_t Cx_out32[32], uint8_t Cy_out32[32], uint64_t y_out[4]);
+/* DotProductProofLog::verify(n, gens, transcript, a, Cx, Cy) with BulletReductionProof::verify (nizk/mod.rs:527-583, bullet.rs:137-225): SP_OK =
+ * accepted; SP_ERR_VERIFY / SP_ERR_DECOMPRESS = rejected, sp_last_error names the check (an L_vec or R_vec of a length other than log2 n, or of 32
+ * or more, is SP_ERR_VERIFY), the transcript left where the reference's verify leaves it.  SP_ERR_INVALID_ARG: a NULL argument, n != gens' n, a of
+ * another context or length; SP_ERR_INVALID_POINT: Cx or Cy does not decompress; a refused call leaves the transcript untouched. */
+int sp_dotlog_verify_t(sp_ctx* ctx, const sp_dotlog_gens* gens, uint8_t* strobe_state /* in, out */, const sp_poly* a, size_t n, const uint8_t Cx32[32],
+                       const uint8_t Cy32[32], const uint8_t* proof, size_t proof_len);
 
 /* ---- product circuits over the caller's tables and the batched proof of their products: the grand-product argument of the reference's memory
  * check (ProductCircuit, ProductCircuitEvalProofBatched, product_tree.rs), bytes identical to the reference's for the same transcript.  Use, e.g.

@@ -10,7 +10,7 @@ from .api import (  # noqa: F401
     SNARKGens, SpartanB200Error, Transcript, VarsAssignment, default_context, device_bytes_live, kernel_launches, lib, random_tape_seed, release_cached_memory, scalar_from_bytes, scalar_to_bytes, tape_seed, prg_scalars,
     sumcheck_prove, sumcheck_verify, debug_memcheck, debug_memcheck_report, debug_memcheck_scan,
     PolyCommitmentGens, PolyCommitment, PolyEvalProof, RandomTape, poly_commit,
-    ZKSumcheckInstanceProof, KnowledgeProof, EqualityProof, ProductProof, DotProductProof,
+    ZKSumcheckInstanceProof, KnowledgeProof, EqualityProof, ProductProof, DotProductProof, DotProductProofGens, DotProductProofLog,
     ProductLeaves, ProductCircuits, ProductCircuitEvalProofBatched, product_leaf_eval,
     SparseMatPolyCommitmentGens, SparseMatPolyCommitment, SparseMatPolyDense, SparseMatPolynomial, SparseMatPolyEvalProof,
     SparseMatProducts,

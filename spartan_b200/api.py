@@ -849,6 +849,49 @@ class DotProductProof:
                                                     C.c_char_p(self.data), _sz(len(self.data))))
 
 
+class DotProductProofGens(_Handle):
+    """DotProductProofGens::new(n, label) (nizk/mod.rs:414-419): gens_n = G[0..n), gens_1 = G[n], h = G[n+1] of the label's stream, for a power of
+    two 1 <= n <= 2^24.  Up to SP_DOTLOG_TABLE_MAX_N (include/spartan_b200.h) the set holds window tables; above it only the points."""
+    _free = lib.sp_dotlog_gens_free
+
+    def __init__(self, n, label, ctx=None):
+        self.ctx = ctx or default_context()
+        self.n = n
+        h = _vp()
+        self.ctx.check(lib.sp_dotlog_gens_create(self.ctx.h, _sz(n), C.c_char_p(bytes(label)), _sz(len(label)), C.byref(h)))
+        self.h = h
+
+
+def _device_vec(v, ctx):
+    """a DensePolynomial as it is, a host array of Montgomery limbs uploaded"""
+    return v if isinstance(v, DensePolynomial) else DensePolynomial(v, ctx)
+
+
+class DotProductProofLog:
+    """nizk/mod.rs:407-583: Cx commits to x_vec, Cy to y = <a_vec, x_vec>, in a proof of O(log n) points (a bulletproofs inner-product argument).
+    x_vec and a_vec: DensePolynomials (read, never modified) or host arrays of Montgomery limbs.  `data` = bincode(DotProductProofLog)."""
+
+    def __init__(self, data):
+        self.data = bytes(data)
+
+    @staticmethod
+    def prove(gens, transcript, tape, x_vec, blind_x, a_vec, y, blind_y):
+        """returns (proof, Cx, Cy); y=None: y = <x_vec, a_vec>, computed on the device"""
+        ctx = gens.ctx
+        x, a = _device_vec(x_vec, ctx), _device_vec(a_vec, ctx)
+        out, n, cx, cy = C.POINTER(C.c_ubyte)(), _sz(), C.create_string_buffer(32), C.create_string_buffer(32)
+        y_out = np.zeros(4, dtype=np.uint64)
+        ctx.check(lib.sp_dotlog_prove_t(ctx.h, gens.h, transcript.state, tape.state, x.h, _scalar(blind_x), a.h, None if y is None else _scalar(y),
+                                        _scalar(blind_y), C.byref(out), C.byref(n), cx, cy, _p(y_out)))
+        return DotProductProofLog(_take_bytes(out, n)), cx.raw, cy.raw
+
+    def verify(self, n, gens, transcript, a, Cx, Cy):
+        """raises ProofVerifyError"""
+        ctx = gens.ctx
+        a = _device_vec(a, ctx)
+        ctx.check(lib.sp_dotlog_verify_t(ctx.h, gens.h, transcript.state, a.h, _sz(n), _point(Cx), _point(Cy), C.c_char_p(self.data), _sz(len(self.data))))
+
+
 # ----------------------------------------------------------------------------- product circuits of the caller's tables
 SP_PROD_MAX_CIRCUITS, SP_PROD_MAX_SOURCES = 24, 3
 

@@ -24,6 +24,7 @@ struct sp_pc_gens {
   size_t num_vars;
   PolyCommitmentGens g;
 };
+struct sp_dotlog_gens { Ctx* ctx; std::unique_ptr<DotLogGens> g; };
 struct sp_spark_gens { Ctx* ctx; size_t x, y, nz, b; SparkGens g; };
 struct sp_spark_dense { Ctx* ctx; SparkDense d; };
 struct sp_prod_circuits {
@@ -1548,6 +1549,71 @@ int sp_dotproduct_verify_t(sp_ctx* ctx, const sp_gens* gens_1, const sp_gens* ge
     Transcript T = ta.open();
     TranscriptClose close{ta, T};
     dotproduct_verify_bytes(ctx->c, g1, gn, T, fq_vec(a_vec, n), Cx, Cy, proof, proof_len);
+  });
+}
+
+// ---- DotProductProofLog of the caller's vectors (prover.cpp: dotlog_*)
+int sp_dotlog_gens_create(sp_ctx* ctx, size_t n, const uint8_t* label, size_t label_len, sp_dotlog_gens** out) {
+  return guarded(ctx, [&] {
+    const std::string what = "dotlog_gens_create";
+    if (!out || (!label && label_len)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    if (n < 1 || n > SP_DOTLOG_MAX_N || (n & (n - 1)))
+      throw SpError(SP_ERR_INVALID_ARG, what + ": n = " + std::to_string(n) + " is not a power of two in 1 .. SP_DOTLOG_MAX_N = " + std::to_string(SP_DOTLOG_MAX_N));
+    std::unique_ptr<sp_dotlog_gens> g(new sp_dotlog_gens{&ctx->c, nullptr});
+    g->g.reset(new DotLogGens(ctx->c, n, std::string((const char*)label, label_len)));
+    *out = g.release();
+  });
+}
+void sp_dotlog_gens_free(sp_dotlog_gens* g) { delete g; }
+// a vector of a DotProductProofLog: a handle of this context with gens' n entries
+static const u256* dotlog_vec(const sp_ctx* ctx, const sp_poly* p, size_t n, const std::string& what, const char* name) {
+  require_owned(ctx, p, what, name);
+  if (p->len != n) throw SpError(SP_ERR_INVALID_ARG, what + ": " + name + " has " + std::to_string(p->len) + " entries, gens have n = " + std::to_string(n));
+  return p->d.p;
+}
+int sp_dotlog_prove_t(sp_ctx* ctx, const sp_dotlog_gens* gens, uint8_t* strobe_state, uint8_t* tape_state, const sp_poly* x, const uint64_t blind_x[4],
+                      const sp_poly* a, const uint64_t* y, const uint64_t blind_y[4], uint8_t** proof, size_t* proof_len, uint8_t Cx_out32[32],
+                      uint8_t Cy_out32[32], uint64_t y_out[4]) {
+  return guarded(ctx, [&] {
+    const std::string what = "dotlog_prove";
+    const ProveStates st(strobe_state, tape_state, what);
+    if (!proof || !proof_len || !Cx_out32 || !Cy_out32 || !y_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    require_owned(ctx, gens, what, "gens");
+    const size_t n = gens->g->n;
+    const u256* dx = dotlog_vec(ctx, x, n, what, "x");
+    const u256* da = dotlog_vec(ctx, a, n, what, "a");
+    const Fq bx = scalar_in(blind_x, what + ": blind_x"), by = scalar_in(blind_y, what + ": blind_y");
+    const Fq fy = y ? scalar_in(y, what + ": y") : Fq::zero();
+    Transcript T = st.ta.open();
+    RandomTape tape(pc_tape_open(tape_state, what));
+    DotProductProofLog p;
+    Cp Cx, Cy;
+    Fq y_used;
+    dotlog_prove(ctx->c, *gens->g, T, tape, dx, bx, da, y ? &fy : nullptr, by, p, Cx, Cy, y_used);
+    st.ta.close(T);
+    tape.state().export_state(tape_state);
+    put_bytes(proof, proof_len, to_bincode(p));
+    cp_out(Cx_out32, Cx);
+    cp_out(Cy_out32, Cy);
+    fq_out(y_out, y_used);
+    flush_fine(ctx->c);
+  });
+}
+int sp_dotlog_verify_t(sp_ctx* ctx, const sp_dotlog_gens* gens, uint8_t* strobe_state, const sp_poly* a, size_t n, const uint8_t Cx32[32],
+                       const uint8_t Cy32[32], const uint8_t* proof, size_t proof_len) {
+  return guarded(ctx, [&] {
+    const std::string what = "dotlog_verify";
+    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
+    ta.check();
+    if (!proof && proof_len) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    require_owned(ctx, gens, what, "gens");
+    if (n != gens->g->n) throw SpError(SP_ERR_INVALID_ARG, what + ": n = " + std::to_string(n) + " but gens have n = " + std::to_string(gens->g->n));
+    const u256* da = dotlog_vec(ctx, a, n, what, "a");
+    const Cp Cx = cp_in(Cx32, what + ": Cx"), Cy = cp_in(Cy32, what + ": Cy");
+    Transcript T = ta.open();
+    TranscriptClose close{ta, T};
+    dotlog_verify_bytes(ctx->c, *gens->g, T, da, Cx, Cy, proof, proof_len);
+    flush_fine(ctx->c);
   });
 }
 

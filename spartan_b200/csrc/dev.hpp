@@ -196,7 +196,8 @@ void gather(u256* out, const u256* mem, const uint32_t* idx, size_t n, cudaStrea
 // addr == null: addr = index i;  ts == null: ts = 0;  ts_plus_one adds one.   d_rg = [r_hash, r_multiset]
 void spark_hash(u256* out, size_t n, const u256* addr, const u256* val, const u256* ts, int ts_plus_one, const u256* d_rg, cudaStream_t s);
 // the folds of an inner-product round (bullet.rs:105-108) in one launch: a[i] = a[i]*u + uinv*a[i+half], b[i] = b[i]*uinv + u*b[i+half], and the
-// running scalars s[j] of the unfolded generators (DESIGN.md "IPA without folding G") times uinv (left half of their block) or u (right half)
+// running scalars s[j] of the unfolded generators (DESIGN.md "IPA without folding G") times uinv (left half of their block) or u (right half);
+// svec null: a and b only
 void ipa_fold_update(u256* a, u256* b, u256* svec, size_t n_cur_half, size_t n_full, const u256& u, const u256& uinv, cudaStream_t s);
 void fill_one(u256* out, size_t n, cudaStream_t s);
 
@@ -355,6 +356,16 @@ struct IpaSRow {
   u256 u_sq[32];
 };
 void ipa_srow(const IpaSRow* d_items, size_t nitems, uint32_t max_lg_n, cudaStream_t s);
+
+// ---- the folding path of DotProductProofLog (prover.cpp: dotlog_fold_prove).  The generator vector G_k = c_k * H_k is kept as H_k and one common
+// scalar c_k, so a round folds H' = H_L + u^2 * H_R (bullet.rs:108 divided by c' = c * u^-1): one variable-base multiplication per pair.
+// A point buffer holds affine niels points (FOLD_NIELS, the input of msm_var) or extended points (FOLD_GE, the input of msm_var_segmented).
+enum FoldFmt { FOLD_NIELS = 0, FOLD_GE = 1 };
+constexpr int FOLD_WBITS = 4, FOLD_NWIN = (253 + FOLD_WBITS - 1) / FOLD_WBITS;   // signed 4-bit digits of the fold scalar
+// out[i] = in[i] + k * in[i + m] for i < m; k canonical (< q).  out may be in itself when both have the same format (thread i writes only entry i)
+void dotlog_fold(void* out, int out_fmt, const void* in, int in_fmt, size_t m, const u256& k, cudaStream_t s);
+// the scalars of a round's two MSMs, halves swapped: out = [c * a[m .. 2m) | c * a[0 .. m)], Montgomery form, or canonical integers (canonical = 1)
+void dotlog_scalars(u256* out, const u256* a, size_t m, const u256& c, int canonical, cudaStream_t s);
 
 }  // namespace dev
 }  // namespace sp

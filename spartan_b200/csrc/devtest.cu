@@ -827,6 +827,30 @@ int spd_msm_var_segmented(size_t K, size_t n, const ge* pts, const u256* scalars
     return (int)c.err;
   });
 }
+// dotlog_fold of 2m points given as extended points: out[i] = pts[i] + k * pts[i + m] (k canonical).  in_fmt FOLD_NIELS converts the points to
+// affine niels first (points_to_niels); a niels output comes back through niels_to_ge
+int spd_dotlog_fold(size_t m, int in_fmt, int out_fmt, const ge* pts, const u256* k, ge* out) {
+  return guarded([&] {
+    KCall c;
+    const ge* dp = c.in(pts, 2 * m);
+    ge_niels* dn = c.alloc<ge_niels>(2 * m);
+    ge_niels* don = c.alloc<ge_niels>(m);
+    ge* dout = c.alloc<ge>(m);
+    if (c.ok()) {
+      const void* in = dp;
+      if (in_fmt == FOLD_NIELS) { points_to_niels(dn, dp, 2 * m, c.s); in = dn; }
+      if (out_fmt == FOLD_NIELS) {
+        dotlog_fold(don, out_fmt, in, in_fmt, m, *k, c.s);
+        niels_to_ge(dout, don, m, c.s);
+      } else {
+        dotlog_fold(dout, out_fmt, in, in_fmt, m, *k, c.s);
+      }
+    }
+    c.sync();
+    c.out(out, dout, m);
+    return (int)c.err;
+  });
+}
 // the launch plan msm_var runs for n points (pip_plan, c_override = 0: the default window width):
 // out = {c, nwin, nb, tile, ntiles, G, S, max_items, pip_scratch_bytes}
 int spd_pip_plan(size_t n, int c_override, uint64_t out[9]) {

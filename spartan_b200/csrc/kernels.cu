@@ -596,7 +596,7 @@ void fill_one(u256* out, size_t n, cudaStream_t s) {
 __global__ void k_ipa_fold_update(u256* a, u256* b, u256* sv, size_t half, size_t n_full, const u256 u, const u256 ui) {
   const size_t t0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
   if (blockIdx.y == 0) {
-    for (size_t j = t0; j < n_full; j += step) {
+    for (size_t j = t0; sv && j < n_full; j += step) {
       const bool right = (j & (2 * half - 1)) >= half;
       st256(sv + j, fq_mul(ld256(sv + j), right ? u : ui));   // bullet.rs:108 on the unfolded generators
     }

@@ -433,5 +433,77 @@ void ipa_srow(const IpaSRow* d_items, size_t nitems, uint32_t max_lg_n, cudaStre
   check("ipa_srow");
 }
 
+// ---- the generator fold of DotProductProofLog's folding path.  Every thread multiplies its own point by the same scalar, so the signed digits are
+// recoded once on the host and every thread walks the same digit sequence: no divergence, and a table of the multiples 1..8 of the point.
+struct FoldDigits { int8_t d[FOLD_NWIN]; };
+template <int FMT> __device__ __forceinline__ ge fold_load(const void* p, size_t i) {
+  if (FMT == FOLD_GE) return ld_ge_p(static_cast<const ge*>(p) + i);
+  const ge_niels* q = static_cast<const ge_niels*>(p) + i;
+  ge_niels nl;
+  nl.ypx = ld256(&q->ypx); nl.ymx = ld256(&q->ymx); nl.t2d = ld256(&q->t2d);
+  return ge_madd(ge_identity(), nl, false);
+}
+template <int IN, int OUT>
+__global__ void __launch_bounds__(128) k_dotlog_fold(void* out, const void* in, size_t m, const FoldDigits dg) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  ge t[8];   // t[j] = (j + 1) * H_R[i]
+  t[0] = fold_load<IN>(in, i + m);
+  t[1] = ge_dbl(t[0]);
+  t[2] = ge_add(t[1], t[0]);
+  t[3] = ge_dbl(t[1]);
+  t[4] = ge_add(t[3], t[0]);
+  t[5] = ge_dbl(t[2]);
+  t[6] = ge_add(t[5], t[0]);
+  t[7] = ge_dbl(t[3]);
+  ge acc = ge_identity();
+  bool started = false;   // the same for every thread
+#pragma unroll 1
+  for (int w = FOLD_NWIN - 1; w >= 0; w--) {
+    if (started) { acc = ge_dbl(acc); acc = ge_dbl(acc); acc = ge_dbl(acc); acc = ge_dbl(acc); }
+    const int d = dg.d[w];
+    if (d) {
+      const ge& q = t[(d < 0 ? -d : d) - 1];
+      acc = started ? ge_add(acc, d < 0 ? ge_neg(q) : q) : (d < 0 ? ge_neg(q) : q);
+      started = true;
+    }
+  }
+  acc = ge_add(acc, fold_load<IN>(in, i));
+  if (OUT == FOLD_GE) {
+    st_ge_p(static_cast<ge*>(out) + i, acc);
+  } else {
+    const ge_niels q = ge_to_niels(acc);   // one inversion per point: about a tenth of the multiplication's field products
+    ge_niels* o = static_cast<ge_niels*>(out) + i;
+    st256(&o->ypx, q.ypx); st256(&o->ymx, q.ymx); st256(&o->t2d, q.t2d);
+  }
+}
+void dotlog_fold(void* out, int out_fmt, const void* in, int in_fmt, size_t m, const u256& k, cudaStream_t s) {
+  if (!m) return;
+  ProfScope ps("dotlog_fold", (in_fmt == FOLD_GE ? 256.0 : 192.0) * (double)m + (out_fmt == FOLD_GE ? 128.0 : 96.0) * (double)m, s);
+  FoldDigits dg;
+  uint32_t carry = 0;
+  for (int w = 0; w < FOLD_NWIN; w++) dg.d[w] = (int8_t)signed_digit(k, w, FOLD_WBITS, carry);
+  if (carry) throw std::runtime_error("spartan_b200: dotlog_fold: scalar not reduced");
+  const unsigned blocks = (unsigned)((m + 127) / 128);
+  if (in_fmt == FOLD_NIELS && out_fmt == FOLD_NIELS) k_dotlog_fold<FOLD_NIELS, FOLD_NIELS><<<blocks, 128, 0, s>>>(out, in, m, dg);
+  else if (in_fmt == FOLD_NIELS) k_dotlog_fold<FOLD_NIELS, FOLD_GE><<<blocks, 128, 0, s>>>(out, in, m, dg);
+  else if (out_fmt == FOLD_GE) k_dotlog_fold<FOLD_GE, FOLD_GE><<<blocks, 128, 0, s>>>(out, in, m, dg);
+  else throw std::runtime_error("spartan_b200: dotlog_fold: extended input needs extended output");
+  SP_LAUNCHED(); check("dotlog_fold");
+}
+
+__global__ void __launch_bounds__(256) k_dotlog_scalars(u256* __restrict__ out, const u256* __restrict__ a, size_t m, const u256 c, int canonical) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 2 * m) return;
+  const u256 v = fq_mul(c, ld256_ro(a + (i < m ? i + m : i - m)));
+  st256(out + i, canonical ? fq_from_mont(v) : v);
+}
+void dotlog_scalars(u256* out, const u256* a, size_t m, const u256& c, int canonical, cudaStream_t s) {
+  if (!m) return;
+  ProfScope ps("dotlog_scalars", 64.0 * (double)m, s);
+  k_dotlog_scalars<<<(unsigned)((2 * m + 255) / 256), 256, 0, s>>>(out, a, m, c, canonical);
+  SP_LAUNCHED(); check("dotlog_scalars");
+}
+
 }  // namespace dev
 }  // namespace sp

@@ -145,12 +145,16 @@ std::vector<Fq> Ctx::download(const u256* d, size_t n) {
   return v;
 }
 
-GenSet::GenSet(Ctx* c, const std::string& label_, size_t nbases_, const std::vector<size_t>& host_bases) : ctx(c), label(label_), nbases(nbases_) {
-  // MultiCommitGens::new (commitments.rs:15-33): SHAKE256(label || basepoint), 64 bytes per generator
+static std::vector<uint8_t> gens_seed(const std::string& label) {   // MultiCommitGens::new (commitments.rs:15-33): SHAKE256(label || basepoint)
   static const uint8_t basepoint[32] = {0xe2, 0xf2, 0xae, 0x0a, 0x6a, 0xbc, 0x4e, 0x71, 0xa8, 0x84, 0xa9, 0x61, 0xc5, 0x00, 0x51, 0x5f,
                                         0x58, 0xe3, 0x0b, 0x6a, 0xa5, 0x82, 0xdd, 0x8d, 0xb6, 0xa6, 0x59, 0x45, 0xe0, 0x8d, 0x2d, 0x76};
   std::vector<uint8_t> seed(label.begin(), label.end());
   seed.insert(seed.end(), basepoint, basepoint + 32);
+  return seed;
+}
+GenSet::GenSet(Ctx* c, const std::string& label_, size_t nbases_, const std::vector<size_t>& host_bases) : ctx(c), label(label_), nbases(nbases_) {
+  // 64 bytes of the label's stream per generator
+  const std::vector<uint8_t> seed = gens_seed(label);
   std::vector<uint8_t> uni(64 * nbases);
   shake256(uni.data(), uni.size(), seed.data(), seed.size());
   DevBuf<uint8_t> d_uni(uni.size());
@@ -815,25 +819,49 @@ static void bullet_prove(Ctx& ctx, Transcript& T, const PolyCommitmentGens& gens
   memcpy(&a_hat, stage, 32); memcpy(&b_hat, stage + 32, 32);
 }
 
+// the tape draws of DotProductProofLog::prove (nizk/mod.rs:452-467), in the reference's order
+struct DotLogTape { Fq d, r_delta, r_beta; std::vector<std::pair<Fq, Fq>> blinds_vec; };
+static DotLogTape dotlog_tape(RandomTape& tape, size_t n) {
+  DotLogTape t;
+  t.d = tape.random_scalar("d");
+  t.r_delta = tape.random_scalar("r_delta");
+  t.r_beta = tape.random_scalar("r_delta");  // sic: the reference reuses the label (nizk/mod.rs:459)
+  const size_t lg_n = log2_ceil(n);
+  std::vector<Fq> v1 = tape.random_vector("blinds_vec_1", lg_n), v2 = tape.random_vector("blinds_vec_2", lg_n);
+  for (size_t i = 0; i < lg_n; i++) t.blinds_vec.push_back({v1[i], v2[i]});
+  return t;
+}
+// DotProductProofLog::prove after the reduction (nizk/mod.rs:491-524), for both generator layouts: g1 = gens_1 (G_1 and h), the reduction's
+// x_hat, a_hat, g_hat and the final blind rhat_Gamma (blind_y's share included)
+static void dotlog_finish(Transcript& T, const CommitKey& g1, const DotLogTape& t, const Fq& r, const Fq& x_hat, const Fq& a_hat, const hge& g_hat,
+                          const Fq& rhat_Gamma, DotProductProofLog& proof) {
+  Fq y_hat = x_hat * a_hat;
+  // delta = d*g_hat + r_delta*h (gens_hat, nizk/mod.rs:497-505)
+  Term th[1] = {{g1.h, t.r_delta}};
+  proof.delta = compress(hge_add(hge_scalarmul(t.d.canonical(), g_hat), host_commit(*g1.set, th, 1)));
+  T.append_point("delta", proof.delta.b);
+  // beta = d*(r*G1) + r_beta*h (gens_1_scaled, nizk/mod.rs:507)
+  proof.beta = compress(commit1(g1, t.d * r, t.r_beta));
+  T.append_point("beta", proof.beta.b);
+  Fq c = T.challenge_scalar("c");
+  proof.z1 = t.d + c * y_hat;
+  proof.z2 = a_hat * (c * rhat_Gamma + t.r_beta) + t.r_delta;
+}
+
 // DotProductProofLog::prove (nizk/mod.rs:440-525).  d_x: device x_vec (n, consumed); a_vec on the host (it is absorbed by the transcript).
 // d_x: device x_vec (n, consumed); d_avec: device a_vec (n, consumed); a_canon: the canonical bytes of a_vec, which the transcript absorbs
 static void dotproduct_log_prove(Ctx& ctx, const PolyCommitmentGens& gens, Transcript& T, RandomTape& tape, u256* d_x, const Fq& blind_x,
-                                 u256* d_avec, const std::vector<uint8_t>& a_canon, const Fq& y, const Fq& blind_y, DotProductProofLog& proof, Cp& Cy_out) {
+                                 u256* d_avec, const std::vector<uint8_t>& a_canon, const Fq& y, const Fq& blind_y, DotProductProofLog& proof, Cp& Cy_out,
+                                 Cp* Cx_out = nullptr) {
   T.append_protocol_name("dot product proof (log)");
   FineTimer f0(ctx, "dotlog pre-ipa");
   size_t n = a_canon.size() / 32;
   if (gens.n != n) throw std::runtime_error("spartan_b200: DotProductProofLog size mismatch");
-  const GenSet& gs = *gens.gens_n.set;
-  Fq d = tape.random_scalar("d");
-  Fq r_delta = tape.random_scalar("r_delta");
-  Fq r_beta = tape.random_scalar("r_delta");  // sic: the reference reuses the label (nizk/mod.rs:459)
-  const size_t lg_n = log2_ceil(n);
-  std::vector<Fq> v1 = tape.random_vector("blinds_vec_1", lg_n), v2 = tape.random_vector("blinds_vec_2", lg_n);
-  std::vector<std::pair<Fq, Fq>> blinds_vec;
-  for (size_t i = 0; i < lg_n; i++) blinds_vec.push_back({v1[i], v2[i]});
+  const DotLogTape t = dotlog_tape(tape, n);
   std::vector<Cp> cx;
   commit_rows_and_compress(ctx, gens.gens_n, d_x, n, 1, n, &blind_x, cx);
   T.append_point("Cx", cx[0].b);
+  if (Cx_out) *Cx_out = cx[0];
   Cy_out = compress(commit1(gens.gens_1, y, blind_y));
   T.append_point("Cy", Cy_out.b);
   Fq r = Fq::zero();
@@ -846,20 +874,192 @@ static void dotproduct_log_prove(Ctx& ctx, const PolyCommitmentGens& gens, Trans
   hge g_hat;
   f0.stop();
   // blind_Gamma = blind_x + r*blind_y enters the reduction only through the final blind, which is linear in it: pass blind_x and add r*blind_y after
-  bullet_prove(ctx, T, gens, absorb_a, d_x, d_avec, n, blind_x, blinds_vec, proof.bullet_reduction_proof, x_hat, a_hat, g_hat, rhat_Gamma);
+  bullet_prove(ctx, T, gens, absorb_a, d_x, d_avec, n, blind_x, t.blinds_vec, proof.bullet_reduction_proof, x_hat, a_hat, g_hat, rhat_Gamma);
   rhat_Gamma = rhat_Gamma + r * blind_y;
   FineTimer f6(ctx, "dotlog post-ipa");
-  Fq y_hat = x_hat * a_hat;
-  // delta = d*g_hat + r_delta*h (gens_hat, nizk/mod.rs:497-505)
-  Term th[1] = {{gens.gens_1.h, r_delta}};
-  proof.delta = compress(hge_add(hge_scalarmul(d.canonical(), g_hat), host_commit(gs, th, 1)));
-  T.append_point("delta", proof.delta.b);
-  // beta = d*(r*G1) + r_beta*h (gens_1_scaled, nizk/mod.rs:507)
-  proof.beta = compress(commit1(gens.gens_1, d * r, r_beta));
-  T.append_point("beta", proof.beta.b);
-  Fq c = T.challenge_scalar("c");
-  proof.z1 = d + c * y_hat;
-  proof.z2 = a_hat * (c * rhat_Gamma + r_beta) + r_delta;
+  dotlog_finish(T, gens.gens_1, t, r, x_hat, a_hat, g_hat, rhat_Gamma, proof);
+}
+
+// ================================================================================================ DotProductProofLog of the caller's vectors
+DotLogGens::DotLogGens(Ctx& c, size_t n_, const std::string& label) : ctx(&c), n(n_) {
+  if (!folding()) {   // the set sp_pc_gens_create builds for n = 2^k (PolyCommitmentGens::new(2k, label) has this n)
+    set.reset(new GenSet(&c, label, n + 2, {n, n + 1}));
+    g = pc_gens_view(*set, 2 * log2_ceil(n));
+    return;
+  }
+  // the label's n + 2 points in slabs (so 2^24 points need no 1 GiB staging buffer): G[0..n) as niels into pts, G_n and h into the small set
+  const std::vector<uint8_t> seed = gens_seed(label);
+  Shake256 xof(seed.data(), seed.size());
+  pts.alloc(n);
+  const size_t total = n + 2, slab = std::min<size_t>((size_t)1 << 18, total);
+  std::vector<uint8_t> uni(64 * slab);
+  DevBuf<uint8_t> d_uni(uni.size());
+  DevBuf<ge> gbuf(slab), last(2);
+  for (size_t i0 = 0; i0 < total; i0 += slab) {
+    const size_t m = std::min(slab, total - i0), in_g = i0 < n ? std::min(m, n - i0) : 0;
+    xof.squeeze(uni.data(), 64 * m);
+    dev::h2d(d_uni.p, uni.data(), 64 * m, c.stream);
+    dev::gens_from_uniform(gbuf.p, d_uni.p, m, c.stream);
+    dev::points_to_niels(pts.p + i0, gbuf.p, in_g, c.stream);
+    if (m > in_g) dev::d2d(last.p + (i0 + in_g - n), gbuf.p + in_g, (m - in_g) * sizeof(ge), c.stream);
+    c.sync();
+  }
+  set.reset(new GenSet(&c, last.p, 2, {0, 1}));
+  g.n = n;
+  g.gens_1 = CommitKey{set.get(), 0, 1, 1};
+}
+
+std::vector<uint8_t> canonical_bytes(Ctx& ctx, const u256* d_a, size_t n) {
+  DevBuf<u256> c(n);
+  dev::to_canonical(c.p, d_a, n, ctx.stream);
+  std::vector<uint8_t> out(32 * n);
+  dev::d2h(out.data(), c.p, 32 * n, ctx.stream);
+  ctx.sync();
+  return out;
+}
+
+hge msm_var_host(Ctx& ctx, const ge_niels* pts, const u256* scalars, size_t n) {
+  const dev::PipPlan plan = dev::pip_plan(n, 0);
+  DevBuf<uint8_t> scratch(dev::pip_scratch_bytes(plan));
+  DevBuf<ge> out(1);
+  dev::msm_var(out.p, pts, scalars, plan, scratch.p, ctx.stream);
+  ge g;
+  dev::d2h(&g, out.p, sizeof(ge), ctx.stream);
+  ctx.sync();
+  return to_hge(g);
+}
+
+// BulletReductionProof::prove (nizk/bullet.rs:32-132) over generators folded on the device (the folding path of sp_dotlog_*), with Q = r*G_1 and H = h
+// folded into host fixed-base terms.  The folded vector is kept as G_k = c_k * H_k: a round folds H' = H_L + u^2 H_R (dev::dotlog_fold) and
+// c' = c * u^-1, and its MSMs take the scalars c * a.  Halves of at most DOTLOG_SEG_MAX_HALF terms run both MSMs as one segmented launch over
+// extended points; longer halves run the bucket MSM over niels points.  d_a / d_b are consumed (folded in place).
+static void bullet_fold_prove(Ctx& ctx, Transcript& T, const DotLogGens& gens, const std::function<Fq()>& get_r_scale, u256* d_a, u256* d_b, size_t n,
+                              const Fq& blind, const std::vector<std::pair<Fq, Fq>>& blinds_vec, BulletReductionProof& proof, Fq& a_hat, Fq& b_hat,
+                              hge& g_hat, Fq& blind_final) {
+  const CommitKey& g1 = gens.g.gens_1;
+  const size_t S = DOTLOG_SEG_MAX_HALF;
+  cudaStream_t s = ctx.stream;
+  // folded points: niels while the next round's halves take the bucket MSM (n/2 of them at most), extended from there on (and G itself when
+  // round 0 already takes the segmented MSM)
+  DevBuf<ge_niels> hn;
+  if (n / 2 > 2 * S) hn.alloc(n / 2);
+  DevBuf<ge> hg(std::min(n, 2 * S)), pts(2), seg_tmp(std::min(n, 2 * S));
+  DevBuf<u256> w(n);
+  size_t scratch_bytes = 0;
+  std::vector<uint32_t> seg;   // {0, m, 2m} of every segmented round
+  for (size_t m = n / 2; m >= 1; m /= 2)
+    if (m > S) scratch_bytes = std::max(scratch_bytes, dev::pip_scratch_bytes(dev::pip_plan(m, 0)));
+    else seg.insert(seg.end(), {0u, (uint32_t)m, (uint32_t)(2 * m)});
+  DevBuf<uint8_t> scratch(std::max<size_t>(scratch_bytes, 1));
+  DevBuf<uint32_t> d_seg(std::max<size_t>(seg.size(), 1));
+  dev::h2d(d_seg.p, seg.data(), seg.size() * sizeof(uint32_t), s);
+  const void* cur = gens.pts.p;
+  int fmt = dev::FOLD_NIELS;
+  if (n / 2 <= S) { dev::niels_to_ge(hg.p, gens.pts.p, n, s); cur = hg.p; fmt = dev::FOLD_GE; }
+  u256* c_dev = ctx.small.p + layout::SMALL_IPA_C.off;
+  uint8_t* stage = ctx.pinned + layout::PIN_STAGE.off;
+  blind_final = blind;
+  Fq c = Fq::one(), r_scale = Fq::zero();
+  size_t k = 0, seg_at = 0;
+  for (size_t m = n / 2; m >= 1; m /= 2, k++) {
+    FineTimer f1(ctx, "dotlog round launch");
+    dev::dot(c_dev, d_a, d_b + m, m, ctx.red.p, s);       // c_L = <a_L, b_R>
+    dev::dot(c_dev + 1, d_a + m, d_b, m, ctx.red.p, s);   // c_R = <a_R, b_L>
+    const bool segmented = m <= S;
+    dev::dotlog_scalars(w.p, d_a, m, c.m, segmented, s);   // [c a_R | c a_L]
+    if (segmented) {   // pts[0] = c <a_R, H_L> = R', pts[1] = c <a_L, H_R> = L'
+      dev::msm_var_segmented(pts.p, static_cast<const ge*>(cur), w.p, d_seg.p + seg_at, 2, 2 * m, seg_tmp.p, s);
+      seg_at += 3;
+    } else {
+      const dev::PipPlan plan = dev::pip_plan(m, 0);
+      const ge_niels* H = static_cast<const ge_niels*>(cur);
+      dev::msm_var(pts.p, H, w.p, plan, scratch.p, s);
+      dev::msm_var(pts.p + 1, H + m, w.p + m, plan, scratch.p, s);
+    }
+    dev::d2h(stage, c_dev, 2 * sizeof(u256), s);
+    dev::d2h(stage + 2 * sizeof(u256), pts.p, 2 * sizeof(ge), s);
+    f1.stop();
+    if (k == 0) {   // the transcript work that precedes the first round (absorbing a, deriving r) runs while the device computes round 0
+      FineTimer fa(ctx, "dotlog absorb a");
+      r_scale = get_r_scale();
+    }
+    FineTimer f2(ctx, "dotlog round wait");
+    ctx.sync();
+    f2.stop();
+    FineTimer f3(ctx, "dotlog round host");
+    Fq c_L, c_R;
+    ge Rg, Lg;
+    memcpy(&c_L, stage, 32); memcpy(&c_R, stage + 32, 32);
+    memcpy(&Rg, stage + 64, sizeof(ge)); memcpy(&Lg, stage + 64 + sizeof(ge), sizeof(ge));
+    // + c_L*Q + blind_L*H with Q = r*G_1 (nizk/mod.rs:479-480), H = h   (bullet.rs:83-97)
+    const Term tl[2] = {{g1.off, c_L * r_scale}, {g1.h, blinds_vec[k].first}};
+    const Term tr[2] = {{g1.off, c_R * r_scale}, {g1.h, blinds_vec[k].second}};
+    Cp Lc, Rc;
+    compress2(hge_add(to_hge(Lg), host_commit(*g1.set, tl, 2)), hge_add(to_hge(Rg), host_commit(*g1.set, tr, 2)), Lc, Rc);
+    T.append_point("L", Lc.b);
+    T.append_point("R", Rc.b);
+    const Fq u = T.challenge_scalar("u"), u_inv = u.inv();
+    f3.stop();
+    dev::ipa_fold_update(d_a, d_b, nullptr, m, 2 * m, u.m, u_inv.m, s);   // bullet.rs:106-107
+    const int out_fmt = m > 2 * S ? dev::FOLD_NIELS : dev::FOLD_GE;
+    void* out = out_fmt == dev::FOLD_NIELS ? static_cast<void*>(hn.p) : static_cast<void*>(hg.p);
+    dev::dotlog_fold(out, out_fmt, cur, fmt, m, (u * u).canonical(), s);   // bullet.rs:108 over H
+    cur = out;
+    fmt = out_fmt;
+    c = c * u_inv;
+    blind_final = blind_final + blinds_vec[k].first * u * u + blinds_vec[k].second * u_inv * u_inv;  // bullet.rs:111
+    proof.L_vec.push_back(Lc);
+    proof.R_vec.push_back(Rc);
+  }
+  // g_hat = G_final[0] = c * H_final[0]
+  dev::d2h(stage, d_a, 32, s);
+  dev::d2h(stage + 32, d_b, 32, s);
+  dev::d2h(stage + 64, cur, sizeof(ge), s);
+  ctx.sync();
+  ge h0;
+  memcpy(&a_hat, stage, 32); memcpy(&b_hat, stage + 32, 32); memcpy(&h0, stage + 64, sizeof(ge));
+  g_hat = hge_scalarmul(c.canonical(), to_hge(h0));
+}
+
+void dotlog_prove(Ctx& ctx, const DotLogGens& gens, Transcript& T, RandomTape& tape, const u256* d_x, const Fq& blind_x, const u256* d_a, const Fq* y,
+                  const Fq& blind_y, DotProductProofLog& proof, Cp& Cx, Cp& Cy, Fq& y_used) {
+  const size_t n = gens.n;
+  DevBuf<u256> x(n), a(n);   // the caller's vectors are read only: the rounds fold these copies
+  dev::d2d(x.p, d_x, n * sizeof(u256), ctx.stream);
+  dev::d2d(a.p, d_a, n * sizeof(u256), ctx.stream);
+  if (y) y_used = *y;
+  else {
+    dev::dot(ctx.small.p + layout::SMALL_DOT.off, x.p, a.p, n, ctx.red.p, ctx.stream);
+    ctx.get_small(layout::SMALL_DOT.off, &y_used, 1);
+  }
+  const std::vector<uint8_t> a_canon = canonical_bytes(ctx, a.p, n);
+  if (!gens.folding()) {
+    dotproduct_log_prove(ctx, gens.g, T, tape, x.p, blind_x, a.p, a_canon, y_used, blind_y, proof, Cy, &Cx);
+    return;
+  }
+  const CommitKey& g1 = gens.g.gens_1;
+  T.append_protocol_name("dot product proof (log)");
+  const DotLogTape t = dotlog_tape(tape, n);
+  FineTimer f0(ctx, "dotlog Cx");
+  const Term tb[1] = {{g1.h, blind_x}};
+  Cx = compress(hge_add(msm_var_host(ctx, gens.pts.p, x.p, n), host_commit(*g1.set, tb, 1)));
+  f0.stop();
+  T.append_point("Cx", Cx.b);
+  Cy = compress(commit1(g1, y_used, blind_y));
+  T.append_point("Cy", Cy.b);
+  Fq r = Fq::zero();
+  auto absorb_a = [&]() {   // nizk/mod.rs:475-477
+    T.append_scalar_bytes("a", a_canon.data(), n);
+    r = T.challenge_scalar("r");
+    return r;
+  };
+  Fq x_hat, a_hat, rhat_Gamma;
+  hge g_hat;
+  FineTimer f1(ctx, "dotlog rounds");
+  bullet_fold_prove(ctx, T, gens, absorb_a, x.p, a.p, n, blind_x, t.blinds_vec, proof.bullet_reduction_proof, x_hat, a_hat, g_hat, rhat_Gamma);
+  f1.stop();
+  rhat_Gamma = rhat_Gamma + r * blind_y;
+  dotlog_finish(T, g1, t, r, x_hat, a_hat, g_hat, rhat_Gamma, proof);
 }
 
 // PolyEvalProof::prove (dense_mlpoly.rs:312-365).  d_Z: device table of 2^|r| scalars (read-only).

@@ -163,6 +163,32 @@ Cp zk_sumcheck_verify_bytes(Ctx& ctx, const uint8_t* proof, size_t len, const Cp
 void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt, const std::vector<Fq>& r, const Fq* Zr, const Fq* blind_Zr_opt,
                     const PolyCommitmentGens& gens, Transcript& T, RandomTape& tape, PolyEvalProof& proof, Cp& C_Zr, Fq* Zr_out = nullptr);
 
+// ---- DotProductProofLog of the caller's vectors (sp_dotlog_*), on this rank's GPU alone
+// DotProductProofGens::new(n, label) (nizk/mod.rs:414-419).  n <= SP_DOTLOG_TABLE_MAX_N: `set` holds the n + 2 generators with the window tables of
+// sp_pc_gens_create's set and `g` views it, as PolyEvalProof's gens.  Larger n (folding()): `pts` holds G[0..n) as affine niels points, `set` the
+// two generators {G_n, h} (host tables for the sigma terms), and g.gens_1 views it; g.gens_n is unused.
+struct DotLogGens {
+  Ctx* ctx;
+  size_t n;
+  std::unique_ptr<GenSet> set;
+  PolyCommitmentGens g;
+  DevBuf<ge_niels> pts;
+  bool folding() const { return n > SP_DOTLOG_TABLE_MAX_N; }
+  DotLogGens(Ctx& ctx, size_t n, const std::string& label);
+};
+// the largest half length whose round MSMs run as one segmented launch (msm_var_segmented, one thread per term) instead of the bucket MSM
+constexpr size_t DOTLOG_SEG_MAX_HALF = 1024;
+// DotProductProofLog::prove (nizk/mod.rs:440-525): d_x, d_a (n each) are read only; y null: <x, a> on the device.  Out: the proof, Cx, Cy, y_used
+void dotlog_prove(Ctx& ctx, const DotLogGens& gens, Transcript& T, RandomTape& tape, const u256* d_x, const Fq& blind_x, const u256* d_a, const Fq* y,
+                  const Fq& blind_y, DotProductProofLog& proof, Cp& Cx, Cp& Cy, Fq& y_used);
+// DotProductProofLog::verify (nizk/mod.rs:527-583) on bincode bytes, with the Immediate checker (verifier.cpp): SpError(SP_ERR_VERIFY /
+// SP_ERR_DECOMPRESS) naming the failing check.  d_a: the n entries of a on the device
+void dotlog_verify_bytes(Ctx& ctx, const DotLogGens& gens, Transcript& T, const u256* d_a, const Cp& Cx, const Cp& Cy, const uint8_t* proof, size_t len);
+// sum_i scalars[i] * pts[i] of n >= 1 terms (bucket MSM, Montgomery scalars on the device), to the host; synchronises
+hge msm_var_host(Ctx& ctx, const ge_niels* pts, const u256* scalars, size_t n);
+// a's entries as the canonical bytes the transcript absorbs (32 per entry), through the device
+std::vector<uint8_t> canonical_bytes(Ctx& ctx, const u256* d_a, size_t n);
+
 // ---- the caller's own tables (sp_pc_*): k tables of 2^m entries each, committed and opened as DensePolynomial::merge of them (dense_mlpoly.rs:259-272),
 // on this rank's GPU alone
 // PolyCommitmentGens::new(num_vars, label) (dense_mlpoly.rs:29-36): gens_n.n = 2^(num_vars - num_vars/2), n + 2 points of the label's stream

@@ -371,17 +371,21 @@ Fq sumcheck_verify(const SumcheckInstanceProof& p, Fq e, size_t num_rounds, size
 }
 
 // ---- inner-product argument
-// DotProductProofLog::verify (nizk/mod.rs:527-583) with BulletReductionProof::verify (nizk/bullet.rs:137-225) inlined.  Its one caller opens
-// at a = eq(r_R, .), so a_hat = <a, s> is the O(lg n) product of ipa_a_hat.  Cy: the claimed evaluation's commitment as a term of coefficient
-// one (a point of the proof, or Zr * G_1), and its encoding
-void dotproduct_log_verify(Checker& chk, const DotProductProofLog& p, const PolyCommitmentGens& gens, Transcript& T, const std::vector<Fq>& r_R,
-                           const std::vector<Fq>& a, const hge& Cx, const Cp& Cx_c, const GTerm& Cy, const Cp& Cy_c) {
-  const size_t n = a.size();
-  if (gens.n != n) throw Reject("DotProductProofLog size");
+// how the public vector a of a DotProductProofLog enters its verify: absorbed by the transcript, and a_hat = <a, s> from the challenges u
+struct DotLogA {
+  std::function<void(Transcript&)> absorb;
+  std::function<Fq(const std::vector<Fq>& u, const std::vector<Fq>& u_inv, const IpaS& s)> a_hat;
+};
+// DotProductProofLog::verify (nizk/mod.rs:527-583) with BulletReductionProof::verify (nizk/bullet.rs:137-225) inlined, for vectors of n entries.
+// g1: gens_1 (G_1 and h).  gens_n set: g_hat = <s, G> is the Checker's IPA term over its tables; else g_hat_of(s) computes it.  Cy: the claimed
+// value's commitment as a term of coefficient one (a point of the proof, or Zr * G_1), and its encoding
+void dotproduct_log_verify(Checker& chk, const DotProductProofLog& p, const CommitKey& g1, const CommitKey* gens_n, size_t n, Transcript& T, const DotLogA& a,
+                           const hge& Cx, const Cp& Cx_c, const GTerm& Cy, const Cp& Cy_c, const std::function<hge(const IpaS&)>& g_hat_of = nullptr) {
+  if (gens_n && gens_n->n != n) throw Reject("DotProductProofLog size");
   T.append_protocol_name("dot product proof (log)");
   T.append_point("Cx", Cx_c.b);
   T.append_point("Cy", Cy_c.b);
-  T.append_scalars("a", a);
+  a.absorb(T);
   Fq r = T.challenge_scalar("r");
   const auto& L = p.bullet_reduction_proof.L_vec;
   const auto& R = p.bullet_reduction_proof.R_vec;
@@ -395,7 +399,8 @@ void dotproduct_log_verify(Checker& chk, const DotProductProofLog& p, const Poly
   }
   Fq allinv = Fq::one();
   for (size_t i = 0; i < lg_n; i++) { u_inv[i] = u[i].inv(); allinv *= u_inv[i]; u_sq[i] = u[i] * u[i]; u_inv_sq[i] = u_inv[i] * u_inv[i]; }
-  const Fq a_hat = ipa_a_hat(r_R.data(), u.data(), u_inv.data(), lg_n);
+  const IpaS s{gens_n, lg_n, u_sq, allinv, p.z1};
+  const Fq a_hat = a.a_hat(u, u_inv, s);
   T.append_point("delta", p.delta.b);
   T.append_point("beta", p.beta.b);
   Fq c = T.challenge_scalar("c");
@@ -406,10 +411,15 @@ void dotproduct_log_verify(Checker& chk, const DotProductProofLog& p, const Poly
   lhs.push_back(P(a_hat, p.beta, "beta"));
   lhs.push_back(P(Fq::one(), p.delta, "delta"));
   // rhs = (g_hat + a_hat*(r*G1))*z1 + h*z2, g_hat = <s, G>
-  const IpaS s{&gens.gens_n, lg_n, u_sq, allinv, p.z1};
-  chk.equal(lhs, {G(p.z1 * a_hat * r, gens.gens_1, gens.gens_1.off), G(p.z2, gens.gens_1, gens.gens_1.h)}, "DotProductProofLog", &s);
+  Side rhs = {G(p.z1 * a_hat * r, g1, g1.off), G(p.z2, g1, g1.h)};
+  if (gens_n) {
+    chk.equal(lhs, rhs, "DotProductProofLog", &s);
+    return;
+  }
+  rhs.push_back(H(p.z1, g_hat_of(s)));
+  chk.equal(lhs, rhs, "DotProductProofLog");
 }
-// PolyEvalProof::verify (dense_mlpoly.rs:367-389)
+// PolyEvalProof::verify (dense_mlpoly.rs:367-389).  It opens at a = eq(r_R, .), so a_hat = <a, s> is the O(lg n) product of ipa_a_hat
 void polyeval_verify(Checker& chk, const PolyEvalProof& p, const PolyCommitmentGens& gens, Transcript& T, const std::vector<Fq>& r, const GTerm& C_Zr,
                      const Cp& C_Zr_c, const PolyCommitment& comm) {
   T.append_protocol_name("polynomial evaluation proof");
@@ -418,7 +428,9 @@ void polyeval_verify(Checker& chk, const PolyEvalProof& p, const PolyCommitmentG
   std::vector<Fq> Lv = host_eq_evals(std::vector<Fq>(r.begin(), r.begin() + lv)), Rv = host_eq_evals(r_R);
   if (comm.C.size() != Lv.size()) throw Reject("polynomial commitment size");
   hge C_LZ = msm_points(chk, comm.C, Lv, "polynomial commitment share");
-  dotproduct_log_verify(chk, p.proof, gens, T, r_R, Rv, C_LZ, compress(C_LZ), C_Zr, C_Zr_c);
+  const DotLogA a{[&](Transcript& t) { t.append_scalars("a", Rv); },
+                  [&](const std::vector<Fq>& u, const std::vector<Fq>& u_inv, const IpaS& s) { return ipa_a_hat(r_R.data(), u.data(), u_inv.data(), s.lg_n); }};
+  dotproduct_log_verify(chk, p.proof, gens.gens_1, &gens.gens_n, Rv.size(), T, a, C_LZ, compress(C_LZ), C_Zr, C_Zr_c);
 }
 void polyeval_verify_plain(Checker& chk, const PolyEvalProof& p, const PolyCommitmentGens& gens, Transcript& T, const std::vector<Fq>& r, const Fq& Zr,
                            const PolyCommitment& comm) {   // dense_mlpoly.rs:391-404
@@ -820,6 +832,49 @@ void pc_eval_verify(Ctx& ctx, const PolyCommitmentGens& gens, const PolyCommitme
   Immediate chk(ctx);
   if (Zr) polyeval_verify_plain(chk, p, gens, T, r, *Zr, comm);
   else polyeval_verify(chk, p, gens, T, r, P(Fq::one(), *C_Zr, "C_Zr"), *C_Zr, comm);
+}
+// DotProductProofLog::verify of the caller's vectors (sp_dotlog_verify_t).  a_hat = <a, s>: on the host from n <= SP_DOTLOG_TABLE_MAX_N entries; on
+// the folding path s is built on the device (k_ipa_srow), where a_hat = <a, s> and g_hat = <s, G> (bucket MSM over the gens' points) follow
+void dotlog_verify_bytes(Ctx& ctx, const DotLogGens& gens, Transcript& T, const u256* d_a, const Cp& Cx, const Cp& Cy, const uint8_t* proof, size_t len) {
+  const DotProductProofLog p = from_bincode<DotProductProofLog>(proof, len, SP_ERR_VERIFY, "dot product proof (log)");
+  Immediate chk(ctx);
+  const size_t n = gens.n;
+  const std::vector<uint8_t> a_canon = canonical_bytes(ctx, d_a, n);
+  hge g_hat;
+  DotLogA a;
+  a.absorb = [&](Transcript& t) { t.append_scalar_bytes("a", a_canon.data(), n); };
+  if (!gens.folding()) {
+    a.a_hat = [&](const std::vector<Fq>&, const std::vector<Fq>&, const IpaS& s) {   // bullet.rs:160-177
+      const std::vector<Fq> av = ctx.download(d_a, n);
+      std::vector<Fq> sv(n);
+      sv[0] = s.allinv;
+      Fq acc = av[0] * sv[0];
+      for (size_t i = 1; i < n; i++) {
+        const size_t lg_i = 63 - (size_t)__builtin_clzll((unsigned long long)i);
+        sv[i] = sv[i - ((size_t)1 << lg_i)] * s.u_sq[s.lg_n - 1 - lg_i];
+        acc += av[i] * sv[i];
+      }
+      return acc;
+    };
+  } else {
+    a.a_hat = [&](const std::vector<Fq>&, const std::vector<Fq>&, const IpaS& s) {
+      FineTimer ft(ctx, "verify.dotlog_s");
+      DevBuf<u256> d_s(n);
+      DevBuf<dev::IpaSRow> d_it(1);
+      IpaS one = s;
+      one.scale = Fq::one();
+      const dev::IpaSRow it = srow_item(d_s.p, one, 0);
+      dev::h2d(d_it.p, &it, sizeof it, ctx.stream);
+      dev::ipa_srow(d_it.p, 1, (uint32_t)s.lg_n, ctx.stream);
+      dev::dot(ctx.small.p + layout::SMALL_DOT.off, d_a, d_s.p, n, ctx.red.p, ctx.stream);
+      g_hat = msm_var_host(ctx, gens.pts.p, d_s.p, n);   // synchronises
+      Fq a_hat;
+      ctx.get_small(layout::SMALL_DOT.off, &a_hat, 1);
+      return a_hat;
+    };
+  }
+  dotproduct_log_verify(chk, p, gens.g.gens_1, gens.folding() ? nullptr : &gens.g.gens_n, n, T, a, unpack(Cx, "Cx"), Cx, P(Fq::one(), Cy, "Cy"), Cy,
+                        [&](const IpaS&) { return g_hat; });
 }
 // DerefsEvalProof::verify_single (sparse_mlpoly.rs:149-176)
 void pc_eval_verify_joint(Ctx& ctx, const PolyCommitmentGens& gens, const PolyCommitment& comm, const std::vector<Fq>& r, const std::vector<Fq>& evals,
