@@ -1132,18 +1132,24 @@ class SparseMatPolynomial:
         return _SparkEntries(self.rows.ctypes.data, self.cols.ctypes.data, self.vals.ctypes.data, len(self.rows))
 
     @staticmethod
+    def _batch(polys, what):
+        """(device, num_vars_x, num_vars_y, _SparkEntries array) of a batch that is all host or all device matrices of one shape; what: the
+        method the refusals name"""
+        device = bool(polys) and polys[0].device
+        if any(p.device != device for p in polys):
+            raise SpartanB200Error(what + ": mix of host and device matrices")
+        if any((p.num_vars_x, p.num_vars_y) != (polys[0].num_vars_x, polys[0].num_vars_y) for p in polys):
+            raise SpartanB200Error(what + ": matrices of different shapes")
+        x, y = (polys[0].num_vars_x, polys[0].num_vars_y) if polys else (0, 0)
+        return device, x, y, (_SparkEntries * max(len(polys), 1))(*[p._entries() for p in polys])
+
+    @staticmethod
     def multi_commit(polys, gens):
         """SparseMatPolynomial::multi_commit (sparse_mlpoly.rs:483-503) of 1 .. SP_SPARK_MAX_BATCH matrices of one shape, all host or all device
         entries: returns (SparseMatPolyCommitment, SparseMatPolyDense)"""
         polys = list(polys)
         ctx = gens.ctx
-        device = bool(polys) and polys[0].device
-        if any(p.device != device for p in polys):
-            raise SpartanB200Error("multi_commit: mix of host and device matrices")
-        if any((p.num_vars_x, p.num_vars_y) != (polys[0].num_vars_x, polys[0].num_vars_y) for p in polys):
-            raise SpartanB200Error("multi_commit: matrices of different shapes")
-        x, y = (polys[0].num_vars_x, polys[0].num_vars_y) if polys else (0, 0)
-        arr = (_SparkEntries * max(len(polys), 1))(*[p._entries() for p in polys])
+        device, x, y, arr = SparseMatPolynomial._batch(polys, "multi_commit")
         if device:
             _sync_torch(ctx)
         h, out, n = _vp(), C.POINTER(C.c_ubyte)(), _sz()
@@ -1171,19 +1177,13 @@ class SparseMatPolynomial:
         """the device form of 1 .. SP_SPMAT_MAX_BATCH matrices of one shape, all host or all device entries, for their products with vectors
         (sp_spmat_create): a SparseMatProducts.  Host matrices go to ctx (default: the default context), device ones stay on theirs."""
         polys = list(polys)
-        device = bool(polys) and polys[0].device
-        if any(p.device != device for p in polys):
-            raise SpartanB200Error("multi_products: mix of host and device matrices")
-        if any((p.num_vars_x, p.num_vars_y) != (polys[0].num_vars_x, polys[0].num_vars_y) for p in polys):
-            raise SpartanB200Error("multi_products: matrices of different shapes")
+        device, x, y, arr = SparseMatPolynomial._batch(polys, "multi_products")
         if device:
             ctx = polys[0].ctx
             if any(p.ctx is not ctx for p in polys):
                 raise SpartanB200Error("multi_products: device matrices of different contexts")
             _sync_torch(ctx)
         ctx = ctx or default_context()
-        x, y = (polys[0].num_vars_x, polys[0].num_vars_y) if polys else (0, 0)
-        arr = (_SparkEntries * max(len(polys), 1))(*[p._entries() for p in polys])
         h = _vp()
         entry = lib.sp_spmat_create_device if device else lib.sp_spmat_create
         ctx.check(entry(ctx.h, arr, C.c_int(len(polys)), _sz(x), _sz(y), C.byref(h)))

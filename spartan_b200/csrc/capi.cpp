@@ -3,6 +3,7 @@
 #include "../../include/spartan_b200.h"
 #include <stdlib.h>
 #include <algorithm>
+#include <optional>
 #include <sstream>
 #include "prover.hpp"
 #include "snark.hpp"
@@ -104,18 +105,57 @@ static Tables caller_tables(const sp_ctx* ctx, sp_poly* const* polys, int k, con
   return t;
 }
 
-// ---- transcripts and witnesses of the proof entries
-// the caller's transcript: either a fresh Transcript::new(label) or (the _t entry points) the caller-owned STROBE state, updated in place
-struct TranscriptArg {
-  const uint8_t* label; size_t label_len; uint8_t* state; bool from_state;
-  static TranscriptArg fresh(const uint8_t* label, size_t label_len) { return {label, label_len, nullptr, false}; }
-  static TranscriptArg caller(uint8_t* state) { return {nullptr, 0, state, true}; }
-  void check() const { if (from_state && !state) throw SpError(SP_ERR_INVALID_ARG, "transcript state is NULL"); }
-  Transcript open() const { return from_state ? Transcript(Transcript::FromState(), state) : Transcript(std::string((const char*)label, label_len)); }
-  void close(const Transcript& T) const { if (from_state) T.export_state(state); }
+// ---- transcripts, tapes and witnesses of the proof entries
+// The transcript and tape of a proof entry.  The transcript is a fresh Transcript::new(label) or (the _t entry points) the caller's STROBE state,
+// updated in place; the tape, for the entries that draw from one, is the caller's tape state.  A NULL state is refused when this is made, before
+// the entry's other checks; open() reads the states after those checks, and refuses one that is not a STROBE state.  The entries that take their
+// tape later (the polynomial-evaluation and SPARK proofs, after their argument checks) pass it to open_tape() at that point instead, where a NULL or
+// bad tape state is refused.  A prove writes both back with proved(), on success alone, so a refused prove leaves them as they were.  A verify
+// opens with open_verify(): its transcript goes back to the caller on every exit, whether the proof is accepted or not.
+class ProofStates {
+ public:
+  struct Label { const uint8_t* p; size_t n; };
+  explicit ProofStates(Label label) : label_(label) {}
+  explicit ProofStates(uint8_t* strobe_state) : state_(strobe_state) {
+    if (!state_) throw SpError(SP_ERR_INVALID_ARG, "transcript state is NULL");
+  }
+  ProofStates(uint8_t* strobe_state, uint8_t* tape_state, const std::string& what) : ProofStates(strobe_state) {
+    tape_state_ = checked_tape(tape_state, what);
+  }
+  // no transcript, and the caller's tape when one is given (sp_pc_commit: NULL draws no blinds)
+  static ProofStates tape_only(uint8_t* tape_state) { return ProofStates(tape_state, false); }
+  ProofStates(const ProofStates&) = delete;
+  ~ProofStates() { if (verifying_) T_->export_state(state_); }
+
+  void open() {
+    if (transcript_) T_.emplace(state_ ? Transcript(Transcript::FromState(), state_) : Transcript(std::string((const char*)label_.p, label_.n)));
+    if (tape_state_ && !tape_) tape_.emplace(Transcript(Transcript::FromState(), tape_state_));
+  }
+  void open_tape(uint8_t* tape_state, const std::string& what) {
+    tape_state_ = checked_tape(tape_state, what);
+    tape_.emplace(Transcript(Transcript::FromState(), tape_state_));
+  }
+  void open_verify() { open(); verifying_ = state_ != nullptr; }
+  void proved() const {
+    if (state_) T_->export_state(state_);
+    if (tape_state_) tape_->state().export_state(tape_state_);
+  }
+  Transcript& T() { return *T_; }
+  RandomTape& tape() { return *tape_; }
+
+ private:
+  ProofStates(uint8_t* tape_state, bool transcript) : transcript_(transcript), tape_state_(tape_state) {}
+  static uint8_t* checked_tape(uint8_t* tape_state, const std::string& what) {
+    if (!tape_state) throw SpError(SP_ERR_INVALID_ARG, what + ": tape state is NULL");
+    return tape_state;
+  }
+  bool transcript_ = true, verifying_ = false;
+  Label label_{nullptr, 0};
+  uint8_t* state_ = nullptr;
+  uint8_t* tape_state_ = nullptr;
+  std::optional<Transcript> T_;
+  std::optional<RandomTape> tape_;
 };
-// the verifiers' _t forms update the caller's transcript state whether or not the proof is accepted (a _t prove writes it back only on success)
-struct TranscriptClose { const TranscriptArg& ta; const Transcript& T; ~TranscriptClose() { ta.close(T); } };
 static DevBuf<u256> upload_padded_vars(Ctx& c, const Instance& I, const uint64_t* vars, size_t nvars) {
   if (nvars > I.num_vars) throw SpError(SP_ERR_INVALID_INPUTS, "R1CSError::InvalidNumberOfInputs (vars)");
   DevBuf<u256> d(I.num_vars);
@@ -130,19 +170,20 @@ static const u256* vars_on_device(Ctx& c, const Instance& I, const VarsArg& v, D
   if (v.resident->len != I.num_vars) throw SpError(SP_ERR_INVALID_INPUTS, "resident vars must already be padded to num_vars");
   return v.resident->d.p;
 }
-// The body NIZK and SNARK proofs share.  `prove(d_vars, inputs, T, seed)` runs the statement's own prover and returns the proof's bincode.
-template <class Prove>
-static void prove_statement(Ctx& c, const Instance& I, const VarsArg& vars, const uint64_t* inputs, size_t ninputs, const TranscriptArg& ta,
+// The body NIZK and SNARK proofs share.  `transcript`: a ProofStates::Label or the caller's transcript state.  `prove(d_vars, inputs, T, seed)`
+// runs the statement's own prover and returns the proof's bincode.
+template <class Src, class Prove>
+static void prove_statement(Ctx& c, const Instance& I, const VarsArg& vars, const uint64_t* inputs, size_t ninputs, const Src& transcript,
                             const uint64_t seed[4], uint8_t** proof, size_t* proof_len, const Prove& prove) {
-  ta.check();
+  ProofStates st(transcript);
   DevBuf<u256> upload;
   const u256* d_vars = vars_on_device(c, I, vars, upload);
   if (ninputs != I.num_inputs) throw SpError(SP_ERR_INVALID_INPUTS, "R1CSError::InvalidNumberOfInputs");
   if (!seed) throw SpError(SP_ERR_INVALID_ARG, "tape seed is NULL: draw it from the OS RNG (random.rs:13-15); a fixed seed makes every blind public");
   require_reduced(inputs, ninputs, "inputs"); require_reduced(seed, 1, "tape seed");
-  Transcript T = ta.open();
-  const std::vector<uint8_t> bytes = prove(d_vars, fq_vec(inputs, ninputs), T, fq_in(seed));
-  ta.close(T);
+  st.open();
+  const std::vector<uint8_t> bytes = prove(d_vars, fq_vec(inputs, ninputs), st.T(), fq_in(seed));
+  st.proved();
   put_bytes(proof, proof_len, bytes);
 }
 // SP_FINE_TIMERS=1: the sub-phase timers of the last verify call (single or batch) replace sp_timings, as a prove call's do
@@ -153,16 +194,49 @@ static void flush_fine(Ctx& c) {
   c.fine.clear();
 }
 // The body NIZK and SNARK verification share.  `verify(inputs, T)` runs the statement's own verifier.
-template <class Verify>
-static int verify_statement(sp_ctx* ctx, const uint64_t* inputs, size_t ninputs, const TranscriptArg& ta, const Verify& verify) {
+template <class Src, class Verify>
+static int verify_statement(sp_ctx* ctx, const uint64_t* inputs, size_t ninputs, const Src& transcript, const Verify& verify) {
   return guarded(ctx, [&] {
-    ta.check();
+    ProofStates st(transcript);
     require_reduced(inputs, ninputs, "inputs");
-    Transcript T = ta.open();
-    TranscriptClose close{ta, T};
-    verify(fq_vec(inputs, ninputs), T);
+    st.open_verify();
+    verify(fq_vec(inputs, ninputs), st.T());
     flush_fine(ctx->c);
   });
+}
+
+template <class Src>
+static int nizk_prove_common(sp_ctx* ctx, const sp_instance* inst, const VarsArg& vars, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens,
+                             const Src& transcript, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
+  return guarded(ctx, [&] {
+    prove_statement(ctx->c, inst->inst, vars, inputs, ninputs, transcript, seed, proof, proof_len, [&](const u256* d_vars, const std::vector<Fq>& in, Transcript& T, const Fq& s) {
+      NizkProof P;
+      nizk_prove(ctx->c, inst->inst, d_vars, in, *gens->g, T, s, P);
+      return to_bincode(P);
+    });
+  });
+}
+template <class Src>
+static int snark_prove_common(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const VarsArg& vars, const uint64_t* inputs, size_t ninputs,
+                              const sp_snark_gens* gens, const Src& transcript, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
+  return guarded(ctx, [&] {
+    if (!enc->e->dense.comb_ops.p) throw SpError(SP_ERR_INVALID_ARG, "this handle holds a commitment only (sp_snark_commitment_load): proving needs sp_snark_encode");
+    prove_statement(ctx->c, inst->inst, vars, inputs, ninputs, transcript, seed, proof, proof_len, [&](const u256* d_vars, const std::vector<Fq>& in, Transcript& T, const Fq& s) {
+      SnarkProof P;
+      snark_prove(ctx->c, inst->inst, *enc->e, d_vars, in, *gens->g, T, s, P);
+      return to_bincode(P);
+    });
+  });
+}
+template <class Src>
+static int nizk_verify_common(sp_ctx* ctx, const sp_instance* inst, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens, const Src& transcript,
+                              const uint8_t* proof, size_t proof_len) {
+  return verify_statement(ctx, inputs, ninputs, transcript, [&](const std::vector<Fq>& in, Transcript& T) { nizk_verify(ctx->c, inst->inst, in, *gens->g, T, proof, proof_len); });
+}
+template <class Src>
+static int snark_verify_common(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t* inputs, size_t ninputs, const sp_snark_gens* gens,
+                               const Src& transcript, const uint8_t* proof, size_t proof_len) {
+  return verify_statement(ctx, inputs, ninputs, transcript, [&](const std::vector<Fq>& in, Transcript& T) { snark_verify(ctx->c, *comm->e, in, *gens->g, T, proof, proof_len); });
 }
 
 // ---- batch verifiers: proof i is checked as the single call would check it (statement i, inputs i, label i or caller transcript i); the group
@@ -226,10 +300,6 @@ static void pc_check_gens(const sp_ctx* ctx, const sp_pc_gens* g, size_t ell, co
                                           ", a table of 2^" + std::to_string(ell) + " entries needs n = R = " + std::to_string(pc_gens_n(ell)));
 }
 static const size_t PC_MAX_VARS = 60;
-static Transcript pc_tape_open(const uint8_t* tape_state, const std::string& what) {
-  if (!tape_state) throw SpError(SP_ERR_INVALID_ARG, what + ": tape state is NULL");
-  return Transcript(Transcript::FromState(), tape_state);
-}
 
 // ---- product circuits of the caller's tables
 static const size_t PROD_MAX_VARS = 60;
@@ -297,6 +367,50 @@ static dev::AffineForm device_form(const LeafForm& f, sp_poly* const* tables) {
   if (!f.idx.is_zero()) p.flags |= dev::PROD_IDX;
   if (!f.cst.is_zero()) p.flags |= dev::PROD_CST;
   return p;
+}
+
+// ---- the caller's sparse matrices
+static void require_device(const Ctx& c, const void* p, size_t n, const char* what) {
+  if (n && !dev::is_device_pointer(p, c.device))
+    throw SpError(SP_ERR_INVALID_ARG, std::string(what) + ": not device memory of the context's GPU (device " + std::to_string(c.device) + ")");
+}
+// the word a checking kernel leaves: ~0 before `launch(err)` runs on the stream, read back after it (~0: nothing failed)
+template <class Launch>
+static unsigned long long first_fault(Ctx& c, const Launch& launch) {
+  DevBuf<unsigned long long> err(1);
+  dev::set_max_u64(err.p, c.stream);
+  launch(err.p);
+  unsigned long long first = 0;
+  dev::d2h(&first, err.p, sizeof(first), c.stream);
+  c.sync();
+  return first;
+}
+// The entries of nmat matrices, host arrays (copied to the device as they are) or device arrays, through the ingestion kernel into out.  The caller's
+// arrays are read by those copies (host) or by the kernel (device) only, and both have finished when this returns or throws.  A bad entry:
+// refuse(matrix, entry, code) words the refusal of the first one in (matrix, entry) order, within it row, then column, then scalar (code:
+// dev::INGEST_*), and throws.
+template <class Refuse>
+static void ingest(Ctx& c, dev::CooIn in, int nmat, bool on_host, const dev::CooOut& out, size_t num_rows, size_t num_cols, size_t num_vars, size_t shift,
+                   const Refuse& refuse) {
+  DevBuf<uint64_t> d_row[dev::INGEST_MAX_MATRICES], d_col[dev::INGEST_MAX_MATRICES];
+  DevBuf<uint8_t> d_val[dev::INGEST_MAX_MATRICES];
+  for (int m = 0; on_host && m < nmat; m++) {
+    d_row[m].alloc(in.n[m]); d_col[m].alloc(in.n[m]); d_val[m].alloc(32 * in.n[m]);
+    dev::h2d(d_row[m].p, in.row[m], in.n[m] * sizeof(uint64_t), c.stream);
+    dev::h2d(d_col[m].p, in.col[m], in.n[m] * sizeof(uint64_t), c.stream);
+    dev::h2d(d_val[m].p, in.val[m], 32 * in.n[m], c.stream);
+    in.row[m] = d_row[m].p; in.col[m] = d_col[m].p; in.val[m] = d_val[m].p;
+  }
+  const unsigned long long first =
+      first_fault(c, [&](unsigned long long* err) { dev::inst_ingest(in, nmat, out, num_rows, num_cols, num_vars, shift, err, c.stream); });
+  if (first != ~0ull) refuse((size_t)(first >> 42), (size_t)((first >> 2) & ((1ull << 40) - 1)), (unsigned)(first & 3));
+}
+// the refusal of entry k of matrix m of a SPARK or product batch
+[[noreturn]] static void refuse_entry(const std::string& what, size_t m, size_t k, unsigned code) {
+  const std::string at = " (matrix " + std::to_string(m) + ", entry " + std::to_string(k) + ")";
+  if (code == dev::INGEST_ROW) throw SpError(SP_ERR_INVALID_INDEX, what + ": row out of range" + at);
+  if (code == dev::INGEST_COL) throw SpError(SP_ERR_INVALID_INDEX, what + ": col out of range" + at);
+  throw SpError(SP_ERR_INVALID_SCALAR, what + ": value not a canonical scalar" + at);
 }
 
 extern "C" {
@@ -760,27 +874,11 @@ int sp_points_upload(sp_ctx* ctx, const uint8_t* in32, size_t n, sp_points** out
 }
 int sp_points_derive(sp_ctx* ctx, const uint8_t* label, size_t label_len, size_t n, sp_points** out) {
   return guarded(ctx, [&] {
-    // the same SHAKE256(label || basepoint) stream as MultiCommitGens::new, squeezed and mapped in slabs so 2^24 points need no 1 GiB staging buffer
-    static const uint8_t basepoint[32] = {0xe2, 0xf2, 0xae, 0x0a, 0x6a, 0xbc, 0x4e, 0x71, 0xa8, 0x84, 0xa9, 0x61, 0xc5, 0x00, 0x51, 0x5f,
-                                          0x58, 0xe3, 0x0b, 0x6a, 0xa5, 0x82, 0xdd, 0x8d, 0xb6, 0xa6, 0x59, 0x45, 0xe0, 0x8d, 0x2d, 0x76};
-    std::vector<uint8_t> seed(label, label + label_len);
-    seed.insert(seed.end(), basepoint, basepoint + 32);
-    Shake256 xof(seed.data(), seed.size());
     std::unique_ptr<sp_points> P(new sp_points);
     P->ctx = &ctx->c; P->n = n;
     P->pts.alloc(n ? n : 1);
-    const size_t slab = (size_t)1 << 18;
-    std::vector<uint8_t> uni(64 * std::min(slab, n ? n : 1));
-    DevBuf<uint8_t> d_uni(uni.size());
-    DevBuf<ge> g(std::min(slab, n ? n : 1));
-    for (size_t i0 = 0; i0 < n; i0 += slab) {
-      size_t m = std::min(slab, n - i0);
-      xof.squeeze(uni.data(), 64 * m);
-      dev::h2d(d_uni.p, uni.data(), 64 * m, ctx->c.stream);
-      dev::gens_from_uniform(g.p, d_uni.p, m, ctx->c.stream);
-      dev::points_to_niels(P->pts.p + i0, g.p, m, ctx->c.stream);
-      ctx->c.sync();
-    }
+    label_gens(ctx->c, std::string((const char*)label, label_len), n, nullptr,
+               [&](size_t i0, size_t m, const ge* pts) { dev::points_to_niels(P->pts.p + i0, pts, m, ctx->c.stream); });
     *out = P.release();
   });
 }
@@ -846,9 +944,9 @@ int sp_msm_var_resident(sp_ctx* ctx, const sp_points* p, size_t offset, const sp
 }
 
 // ---- instances
-// Instance::new (lib.rs:129-198) from arrays in device memory: padding rules, checks, input-column remap and Montgomery form on the device, then
-// the CSR / CSC copies.  The caller's arrays are read by the ingestion kernel only, which has finished when this returns or throws.
-static sp_instance* instance_from_device(Ctx& c, size_t num_cons, size_t num_vars, size_t num_inputs, const dev::CooIn& in) {
+// Instance::new (lib.rs:129-198) from the caller's arrays: padding rules, checks, input-column remap and Montgomery form on the device, then the
+// CSR / CSC copies
+static sp_instance* instance_from_coo(Ctx& c, size_t num_cons, size_t num_vars, size_t num_inputs, const dev::CooIn& in, bool on_host) {
   size_t num_vars_padded = next_pow2(std::max(num_vars, num_inputs + 1));
   size_t num_cons_padded = num_cons;
   if (num_cons_padded == 0 || num_cons_padded == 1) num_cons_padded = 2;
@@ -863,18 +961,11 @@ static sp_instance* instance_from_device(Ctx& c, size_t num_cons, size_t num_var
     M.coo_row.alloc(M.nnz); M.coo_col.alloc(M.nnz); M.coo_val.alloc(M.nnz);
     co.row[m] = M.coo_row.p; co.col[m] = M.coo_col.p; co.val[m] = M.coo_val.p;
   }
-  DevBuf<unsigned long long> err(1);
-  dev::set_max_u64(err.p, c.stream);
-  dev::inst_ingest(in, 3, co, num_cons, num_vars + 1 + num_inputs, num_vars, num_vars_padded - num_vars, err.p, c.stream);
-  unsigned long long first = 0;
-  dev::d2h(&first, err.p, sizeof(first), c.stream);
-  c.sync();
-  if (first != ~0ull) {   // the first bad entry in (matrix, entry) order; within it row, then column, then scalar
-    const unsigned code = (unsigned)(first & 3);
+  ingest(c, in, 3, on_host, co, num_cons, num_vars + 1 + num_inputs, num_vars, num_vars_padded - num_vars, [](size_t, size_t, unsigned code) {
     if (code == dev::INGEST_ROW) throw SpError(SP_ERR_INVALID_INDEX, "R1CSError::InvalidIndex (row)");
     if (code == dev::INGEST_COL) throw SpError(SP_ERR_INVALID_INDEX, "R1CSError::InvalidIndex (col)");
     throw SpError(SP_ERR_INVALID_SCALAR, "R1CSError::InvalidScalar");
-  }
+  });
   for (int m = 0; m < 3; m++)
     if (pad) dev::inst_pad_rows(co.row[m], co.col[m], co.val[m], in.n[m], I->inst.M[m].nnz, (uint32_t)num_vars, c.stream);
   I->inst.finalize(&c);
@@ -885,28 +976,9 @@ int sp_instance_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num
                        size_t nA, const uint64_t* B_row, const uint64_t* B_col, const uint8_t* B_val, size_t nB, const uint64_t* C_row, const uint64_t* C_col,
                        const uint8_t* C_val, size_t nC, sp_instance** out) {
   return guarded(ctx, [&] {
-    // the host arrays go to the device as they are and meet the same checks as sp_instance_create_device's
-    const uint64_t* rows[3] = {A_row, B_row, C_row};
-    const uint64_t* cols[3] = {A_col, B_col, C_col};
-    const uint8_t* vals[3] = {A_val, B_val, C_val};
-    const size_t nn[3] = {nA, nB, nC};
-    DevBuf<uint64_t> d_row[3], d_col[3];
-    DevBuf<uint8_t> d_val[3];
-    dev::CooIn in;
-    for (int m = 0; m < 3; m++) {
-      d_row[m].alloc(nn[m]); d_col[m].alloc(nn[m]); d_val[m].alloc(32 * nn[m]);
-      dev::h2d(d_row[m].p, rows[m], nn[m] * sizeof(uint64_t), ctx->c.stream);
-      dev::h2d(d_col[m].p, cols[m], nn[m] * sizeof(uint64_t), ctx->c.stream);
-      dev::h2d(d_val[m].p, vals[m], 32 * nn[m], ctx->c.stream);
-      in.row[m] = d_row[m].p; in.col[m] = d_col[m].p; in.val[m] = d_val[m].p; in.n[m] = nn[m];
-    }
-    *out = instance_from_device(ctx->c, num_cons, num_vars, num_inputs, in);
+    const dev::CooIn in = {{A_row, B_row, C_row}, {A_col, B_col, C_col}, {A_val, B_val, C_val}, {nA, nB, nC}};
+    *out = instance_from_coo(ctx->c, num_cons, num_vars, num_inputs, in, true);
   });
-}
-
-static void require_device(const Ctx& c, const void* p, size_t n, const char* what) {
-  if (n && !dev::is_device_pointer(p, c.device))
-    throw SpError(SP_ERR_INVALID_ARG, std::string(what) + ": not device memory of the context's GPU (device " + std::to_string(c.device) + ")");
 }
 int sp_instance_create_device(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, const uint64_t* A_row, const uint64_t* A_col,
                               const uint8_t* A_val, size_t nA, const uint64_t* B_row, const uint64_t* B_col, const uint8_t* B_val, size_t nB,
@@ -919,7 +991,7 @@ int sp_instance_create_device(sp_ctx* ctx, size_t num_cons, size_t num_vars, siz
       require_device(ctx->c, in.col[m], in.n[m], names[m][1]);
       require_device(ctx->c, in.val[m], in.n[m], names[m][2]);
     }
-    *out = instance_from_device(ctx->c, num_cons, num_vars, num_inputs, in);
+    *out = instance_from_coo(ctx->c, num_cons, num_vars, num_inputs, in, false);
   });
 }
 
@@ -928,12 +1000,7 @@ int sp_poly_from_canonical_device(sp_ctx* ctx, const uint8_t* d_canonical32, siz
     Ctx& c = ctx->c;
     require_device(c, d_canonical32, n, "poly_from_canonical_device");
     std::unique_ptr<sp_poly> p(new sp_poly{&c, DevBuf<u256>(n), n});
-    DevBuf<unsigned long long> err(1);
-    dev::set_max_u64(err.p, c.stream);
-    dev::canonical_to_mont(p->d.p, d_canonical32, n, err.p, c.stream);
-    unsigned long long first = 0;
-    dev::d2h(&first, err.p, sizeof(first), c.stream);
-    c.sync();
+    const unsigned long long first = first_fault(c, [&](unsigned long long* err) { dev::canonical_to_mont(p->d.p, d_canonical32, n, err, c.stream); });
     if (first != ~0ull) throw SpError(SP_ERR_INVALID_SCALAR, "R1CSError::InvalidScalar (entry " + std::to_string(first) + ")");
     *out = p.release();
   });
@@ -1056,28 +1123,18 @@ int sp_nizk_gens_create_from(sp_ctx* ctx, const sp_gen_tables* tables, size_t nu
 }
 void sp_nizk_gens_free(sp_nizk_gens* g) { delete g; }
 
-static int nizk_prove_common(sp_ctx* ctx, const sp_instance* inst, const VarsArg& vars, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens,
-                             const TranscriptArg& ta, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  return guarded(ctx, [&] {
-    prove_statement(ctx->c, inst->inst, vars, inputs, ninputs, ta, seed, proof, proof_len, [&](const u256* d_vars, const std::vector<Fq>& in, Transcript& T, const Fq& s) {
-      NizkProof P;
-      nizk_prove(ctx->c, inst->inst, d_vars, in, *gens->g, T, s, P);
-      return to_bincode(P);
-    });
-  });
-}
 int sp_nizk_prove(sp_ctx* ctx, const sp_instance* inst, const uint64_t* vars, size_t nvars, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens,
                   const uint8_t* label, size_t label_len, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  return nizk_prove_common(ctx, inst, {vars, nvars, nullptr}, inputs, ninputs, gens, TranscriptArg::fresh(label, label_len), seed, proof, proof_len);
+  return nizk_prove_common(ctx, inst, {vars, nvars, nullptr}, inputs, ninputs, gens, ProofStates::Label{label, label_len}, seed, proof, proof_len);
 }
 // NIZK::prove(&inst, vars, &inputs, &gens, transcript: &mut Transcript) with the caller's transcript state in / out (lib.rs:501-508)
 int sp_nizk_prove_t(sp_ctx* ctx, const sp_instance* inst, const uint64_t* vars, size_t nvars, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens,
                     uint8_t* strobe_state, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  return nizk_prove_common(ctx, inst, {vars, nvars, nullptr}, inputs, ninputs, gens, TranscriptArg::caller(strobe_state), seed, proof, proof_len);
+  return nizk_prove_common(ctx, inst, {vars, nvars, nullptr}, inputs, ninputs, gens, strobe_state, seed, proof, proof_len);
 }
 int sp_nizk_prove_resident(sp_ctx* ctx, const sp_instance* inst, const sp_poly* vars, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens,
                            const uint8_t* label, size_t label_len, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  return nizk_prove_common(ctx, inst, {nullptr, 0, vars}, inputs, ninputs, gens, TranscriptArg::fresh(label, label_len), seed, proof, proof_len);
+  return nizk_prove_common(ctx, inst, {nullptr, 0, vars}, inputs, ninputs, gens, ProofStates::Label{label, label_len}, seed, proof, proof_len);
 }
 
 // ---- SNARK
@@ -1147,55 +1204,36 @@ int sp_snark_commitment_load(sp_ctx* ctx, const uint8_t* bytes, size_t len, sp_s
     *out = E.release();
   });
 }
-static int snark_prove_common(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const VarsArg& vars, const uint64_t* inputs, size_t ninputs,
-                              const sp_snark_gens* gens, const TranscriptArg& ta, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  return guarded(ctx, [&] {
-    if (!enc->e->dense.comb_ops.p) throw SpError(SP_ERR_INVALID_ARG, "this handle holds a commitment only (sp_snark_commitment_load): proving needs sp_snark_encode");
-    prove_statement(ctx->c, inst->inst, vars, inputs, ninputs, ta, seed, proof, proof_len, [&](const u256* d_vars, const std::vector<Fq>& in, Transcript& T, const Fq& s) {
-      SnarkProof P;
-      snark_prove(ctx->c, inst->inst, *enc->e, d_vars, in, *gens->g, T, s, P);
-      return to_bincode(P);
-    });
-  });
-}
 int sp_snark_prove(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const uint64_t* vars, size_t nvars, const uint64_t* inputs, size_t ninputs,
                    const sp_snark_gens* gens, const uint8_t* label, size_t label_len, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  return snark_prove_common(ctx, inst, enc, {vars, nvars, nullptr}, inputs, ninputs, gens, TranscriptArg::fresh(label, label_len), seed, proof, proof_len);
+  return snark_prove_common(ctx, inst, enc, {vars, nvars, nullptr}, inputs, ninputs, gens, ProofStates::Label{label, label_len}, seed, proof, proof_len);
 }
 // SNARK::prove(..., transcript: &mut Transcript) with the caller's transcript state in / out (lib.rs:339-347)
 int sp_snark_prove_t(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const uint64_t* vars, size_t nvars, const uint64_t* inputs, size_t ninputs,
                      const sp_snark_gens* gens, uint8_t* strobe_state, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  return snark_prove_common(ctx, inst, enc, {vars, nvars, nullptr}, inputs, ninputs, gens, TranscriptArg::caller(strobe_state), seed, proof, proof_len);
+  return snark_prove_common(ctx, inst, enc, {vars, nvars, nullptr}, inputs, ninputs, gens, strobe_state, seed, proof, proof_len);
 }
 int sp_snark_prove_resident(sp_ctx* ctx, const sp_instance* inst, const sp_snark_encoding* enc, const sp_poly* vars, const uint64_t* inputs, size_t ninputs,
                             const sp_snark_gens* gens, const uint8_t* label, size_t label_len, const uint64_t seed[4], uint8_t** proof, size_t* proof_len) {
-  return snark_prove_common(ctx, inst, enc, {nullptr, 0, vars}, inputs, ninputs, gens, TranscriptArg::fresh(label, label_len), seed, proof, proof_len);
+  return snark_prove_common(ctx, inst, enc, {nullptr, 0, vars}, inputs, ninputs, gens, ProofStates::Label{label, label_len}, seed, proof, proof_len);
 }
 
 // ---- verifiers.  The _t forms verify on the caller's transcript state (lib.rs:423-429, :549-555).
-static int nizk_verify_common(sp_ctx* ctx, const sp_instance* inst, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens, const TranscriptArg& ta,
-                              const uint8_t* proof, size_t proof_len) {
-  return verify_statement(ctx, inputs, ninputs, ta, [&](const std::vector<Fq>& in, Transcript& T) { nizk_verify(ctx->c, inst->inst, in, *gens->g, T, proof, proof_len); });
-}
-static int snark_verify_common(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t* inputs, size_t ninputs, const sp_snark_gens* gens,
-                               const TranscriptArg& ta, const uint8_t* proof, size_t proof_len) {
-  return verify_statement(ctx, inputs, ninputs, ta, [&](const std::vector<Fq>& in, Transcript& T) { snark_verify(ctx->c, *comm->e, in, *gens->g, T, proof, proof_len); });
-}
 int sp_nizk_verify(sp_ctx* ctx, const sp_instance* inst, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens, const uint8_t* label, size_t label_len,
                    const uint8_t* proof, size_t proof_len) {
-  return nizk_verify_common(ctx, inst, inputs, ninputs, gens, TranscriptArg::fresh(label, label_len), proof, proof_len);
+  return nizk_verify_common(ctx, inst, inputs, ninputs, gens, ProofStates::Label{label, label_len}, proof, proof_len);
 }
 int sp_snark_verify(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t* inputs, size_t ninputs, const sp_snark_gens* gens, const uint8_t* label,
                     size_t label_len, const uint8_t* proof, size_t proof_len) {
-  return snark_verify_common(ctx, comm, inputs, ninputs, gens, TranscriptArg::fresh(label, label_len), proof, proof_len);
+  return snark_verify_common(ctx, comm, inputs, ninputs, gens, ProofStates::Label{label, label_len}, proof, proof_len);
 }
 int sp_nizk_verify_t(sp_ctx* ctx, const sp_instance* inst, const uint64_t* inputs, size_t ninputs, const sp_nizk_gens* gens, uint8_t* strobe_state,
                      const uint8_t* proof, size_t proof_len) {
-  return nizk_verify_common(ctx, inst, inputs, ninputs, gens, TranscriptArg::caller(strobe_state), proof, proof_len);
+  return nizk_verify_common(ctx, inst, inputs, ninputs, gens, strobe_state, proof, proof_len);
 }
 int sp_snark_verify_t(sp_ctx* ctx, const sp_snark_encoding* comm, const uint64_t* inputs, size_t ninputs, const sp_snark_gens* gens, uint8_t* strobe_state,
                       const uint8_t* proof, size_t proof_len) {
-  return snark_verify_common(ctx, comm, inputs, ninputs, gens, TranscriptArg::caller(strobe_state), proof, proof_len);
+  return snark_verify_common(ctx, comm, inputs, ninputs, gens, strobe_state, proof, proof_len);
 }
 // ---- a whole sumcheck of a caller-defined polynomial (prover.cpp: poly_sumcheck_prove).  Every argument is checked before the first launch, so a
 // refused call leaves the tables as they were.
@@ -1241,50 +1279,50 @@ static CallerPoly caller_poly(const sp_ctx* ctx, sp_poly* const* tables, int k, 
   }
   return cp;
 }
-static int sumcheck_prove_common(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim[4],
-                                 size_t num_rounds, const TranscriptArg& ta, uint8_t** proof, size_t* proof_len, uint64_t* r_out, uint64_t* finals_out,
-                                 uint64_t e_out[4]) {
-  return guarded(ctx, [&] {
-    const std::string what = "sumcheck_prove";
-    ta.check();
-    if (!tables || !terms || !claim || !proof || !proof_len || !r_out || !finals_out || !e_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
-    const CallerPoly cp = caller_poly(ctx, tables, k, terms, nterms, num_rounds, what);
-    require_reduced(claim, 1, "sumcheck_prove: claim");
-    Transcript T = ta.open();
-    SumcheckInstanceProof pr;
-    std::vector<Fq> r, finals;
-    Fq e;
-    poly_sumcheck_prove(ctx->c, cp.P, cp.len, fq_in(claim), num_rounds, T, pr, r, finals, e);
-    for (sp_poly* p : cp.distinct) p->len >>= num_rounds;
-    ta.close(T);
-    put_bytes(proof, proof_len, to_bincode(pr));
-    put_scalars(r_out, r);
-    for (int i = 0; i < k; i++) fq_out(finals_out + 4 * i, finals[cp.slot[i]]);
-    fq_out(e_out, e);
-  });
+// the body of sp_sumcheck_prove(_t), run inside guarded: the entry makes st, the first check of the call
+static void sumcheck_prove_common(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim[4],
+                                  size_t num_rounds, ProofStates&& st, uint8_t** proof, size_t* proof_len, uint64_t* r_out, uint64_t* finals_out,
+                                  uint64_t e_out[4]) {
+  const std::string what = "sumcheck_prove";
+  if (!tables || !terms || !claim || !proof || !proof_len || !r_out || !finals_out || !e_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  const CallerPoly cp = caller_poly(ctx, tables, k, terms, nterms, num_rounds, what);
+  require_reduced(claim, 1, "sumcheck_prove: claim");
+  st.open();
+  SumcheckInstanceProof pr;
+  std::vector<Fq> r, finals;
+  Fq e;
+  poly_sumcheck_prove(ctx->c, cp.P, cp.len, fq_in(claim), num_rounds, st.T(), pr, r, finals, e);
+  for (sp_poly* p : cp.distinct) p->len >>= num_rounds;
+  st.proved();
+  put_bytes(proof, proof_len, to_bincode(pr));
+  put_scalars(r_out, r);
+  for (int i = 0; i < k; i++) fq_out(finals_out + 4 * i, finals[cp.slot[i]]);
+  fq_out(e_out, e);
 }
 int sp_sumcheck_prove_t(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim[4], size_t num_rounds,
                         uint8_t* strobe_state, uint8_t** proof, size_t* proof_len, uint64_t* r_out, uint64_t* finals_out, uint64_t e_out[4]) {
-  return sumcheck_prove_common(ctx, tables, k, terms, nterms, claim, num_rounds, TranscriptArg::caller(strobe_state), proof, proof_len, r_out, finals_out, e_out);
+  return guarded(ctx, [&] {
+    sumcheck_prove_common(ctx, tables, k, terms, nterms, claim, num_rounds, ProofStates(strobe_state), proof, proof_len, r_out, finals_out, e_out);
+  });
 }
 int sp_sumcheck_prove(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim[4], size_t num_rounds,
                       const uint8_t* label, size_t label_len, uint8_t** proof, size_t* proof_len, uint64_t* r_out, uint64_t* finals_out, uint64_t e_out[4]) {
-  return sumcheck_prove_common(ctx, tables, k, terms, nterms, claim, num_rounds, TranscriptArg::fresh(label, label_len), proof, proof_len, r_out, finals_out,
-                               e_out);
+  return guarded(ctx, [&] {
+    sumcheck_prove_common(ctx, tables, k, terms, nterms, claim, num_rounds, ProofStates(ProofStates::Label{label, label_len}), proof, proof_len, r_out,
+                          finals_out, e_out);
+  });
 }
 // host only: no device work, so ctx may be NULL (the message then goes where sp_last_error(NULL) reads it)
 int sp_sumcheck_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, const uint64_t claim[4], size_t num_rounds, size_t degree_bound,
                          uint8_t* strobe_state, uint64_t e_out[4], uint64_t* r_out) {
   return host_guarded(ctx, [&] {
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
+    ProofStates st(strobe_state);
     if (!claim || !e_out || (!r_out && num_rounds) || (!proof && proof_len)) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_verify: NULL argument");
     if (degree_bound < 1) throw SpError(SP_ERR_INVALID_ARG, "sumcheck_verify: degree_bound must be >= 1");
     require_reduced(claim, 1, "sumcheck_verify: claim");
-    Transcript T = ta.open();
-    TranscriptClose close{ta, T};
+    st.open_verify();
     std::vector<Fq> r;
-    fq_out(e_out, sumcheck_verify_bytes(proof, proof_len, fq_in(claim), num_rounds, degree_bound, T, r));
+    fq_out(e_out, sumcheck_verify_bytes(proof, proof_len, fq_in(claim), num_rounds, degree_bound, st.T(), r));
     put_scalars(r_out, r);
   });
 }
@@ -1319,22 +1357,13 @@ static Fq scalar_in(const uint64_t* l, const std::string& what) {
   return fq_in(l);
 }
 static void cp_out(uint8_t* out32, const Cp& c) { if (out32) memcpy(out32, c.b, 32); }
-// a prove entry's transcript and tape: both opened after the checks, both written back on success only
-struct ProveStates {
-  const TranscriptArg ta;
-  uint8_t* tape_state;
-  ProveStates(uint8_t* strobe_state, uint8_t* tape, const std::string& what) : ta(TranscriptArg::caller(strobe_state)), tape_state(tape) {
-    ta.check();
-    if (!tape_state) throw SpError(SP_ERR_INVALID_ARG, what + ": tape state is NULL");
-  }
-};
 
 int sp_zk_sumcheck_prove_t(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_sc_term* terms, int nterms, const uint64_t claim[4],
                            const uint64_t blind_claim[4], size_t num_rounds, const sp_gens* gens_1, const sp_gens* gens_n, uint8_t* strobe_state,
                            uint8_t* tape_state, uint8_t** proof, size_t* proof_len, uint64_t* r_out, uint64_t* finals_out, uint64_t blind_post_out[4]) {
   return guarded(ctx, [&] {
     const std::string what = "zk_sumcheck_prove";
-    const ProveStates st(strobe_state, tape_state, what);
+    ProofStates st(strobe_state, tape_state, what);
     if (!tables || !terms || !proof || !proof_len || !r_out || !finals_out || !blind_post_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     const CallerPoly cp = caller_poly(ctx, tables, k, terms, nterms, num_rounds, what);
     if (num_rounds > zk_sumcheck_max_rounds())
@@ -1346,15 +1375,13 @@ int sp_zk_sumcheck_prove_t(sp_ctx* ctx, sp_poly* const* tables, int k, const sp_
     const Fq c = scalar_in(claim, what + ": claim"), bc = scalar_in(blind_claim, what + ": blind_claim");
     gens_host_tables(gens_1);
     gens_host_tables(gens_n);
-    Transcript T = st.ta.open();
-    RandomTape tape(pc_tape_open(tape_state, what));
+    st.open();
     ZKSumcheckInstanceProof pr;
     std::vector<Fq> r, finals;
     Fq blind_post;
-    zk_poly_sumcheck_prove(ctx->c, cp.P, cp.len, c, bc, num_rounds, g1, gn, T, tape, pr, r, finals, blind_post);
+    zk_poly_sumcheck_prove(ctx->c, cp.P, cp.len, c, bc, num_rounds, g1, gn, st.T(), st.tape(), pr, r, finals, blind_post);
     for (sp_poly* p : cp.distinct) p->len >>= num_rounds;
-    st.ta.close(T);
-    tape.state().export_state(tape_state);
+    st.proved();
     put_bytes(proof, proof_len, to_bincode(pr));
     put_scalars(r_out, r);
     for (int i = 0; i < k; i++) fq_out(finals_out + 4 * i, finals[cp.slot[i]]);
@@ -1365,8 +1392,7 @@ int sp_zk_sumcheck_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len,
                             const sp_gens* gens_1, const sp_gens* gens_n, uint8_t* strobe_state, uint8_t comm_eval_out32[32], uint64_t* r_out) {
   return guarded(ctx, [&] {
     const std::string what = "zk_sumcheck_verify";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
+    ProofStates st(strobe_state);
     if ((!proof && proof_len) || !comm_eval_out32 || !r_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     if (num_rounds < 1) throw SpError(SP_ERR_INVALID_ARG, what + ": num_rounds must be >= 1");
     if (degree_bound < 1 || degree_bound + 1 > SP_DOTPROD_MAX_N)
@@ -1377,10 +1403,9 @@ int sp_zk_sumcheck_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len,
     const Cp cc = cp_in(comm_claim32, what + ": comm_claim");
     gens_host_tables(gens_1);
     gens_host_tables(gens_n);
-    Transcript T = ta.open();
-    TranscriptClose close{ta, T};
+    st.open_verify();
     std::vector<Fq> r;
-    cp_out(comm_eval_out32, zk_sumcheck_verify_bytes(ctx->c, proof, proof_len, cc, num_rounds, degree_bound, g1, gn, T, r));
+    cp_out(comm_eval_out32, zk_sumcheck_verify_bytes(ctx->c, proof, proof_len, cc, num_rounds, degree_bound, g1, gn, st.T(), r));
     put_scalars(r_out, r);
   });
 }
@@ -1389,18 +1414,16 @@ int sp_knowledge_prove_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_sta
                          uint8_t** proof, size_t* proof_len, uint8_t C_out32[32]) {
   return guarded(ctx, [&] {
     const std::string what = "knowledge_prove";
-    const ProveStates st(strobe_state, tape_state, what);
+    ProofStates st(strobe_state, tape_state, what);
     if (!proof || !proof_len || !C_out32) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     const CommitKey g = gens_key(ctx, gens_n, what, "gens_n");
     require_gens_n(g, 1, what, "gens_n", "a scalar's commitment");
     const Fq fx = scalar_in(x, what + ": x"), fr = scalar_in(r, what + ": r");
     gens_host_tables(gens_n);
-    Transcript T = st.ta.open();
-    RandomTape tape(pc_tape_open(tape_state, what));
+    st.open();
     Cp C;
-    const KnowledgeProof p = knowledge_prove(g, T, tape, fx, fr, C);
-    st.ta.close(T);
-    tape.state().export_state(tape_state);
+    const KnowledgeProof p = knowledge_prove(g, st.T(), st.tape(), fx, fr, C);
+    st.proved();
     put_bytes(proof, proof_len, to_bincode(p));
     cp_out(C_out32, C);
   });
@@ -1408,16 +1431,14 @@ int sp_knowledge_prove_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_sta
 int sp_knowledge_verify_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state, const uint8_t C32[32], const uint8_t* proof, size_t proof_len) {
   return guarded(ctx, [&] {
     const std::string what = "knowledge_verify";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
+    ProofStates st(strobe_state);
     if (!proof && proof_len) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     const CommitKey g = gens_key(ctx, gens_n, what, "gens_n");
     require_gens_n(g, 1, what, "gens_n", "a scalar's commitment");
     const Cp C = cp_in(C32, what + ": C");
     gens_host_tables(gens_n);
-    Transcript T = ta.open();
-    TranscriptClose close{ta, T};
-    knowledge_verify_bytes(ctx->c, g, T, C, proof, proof_len);
+    st.open_verify();
+    knowledge_verify_bytes(ctx->c, g, st.T(), C, proof, proof_len);
   });
 }
 
@@ -1425,18 +1446,16 @@ int sp_equality_prove_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_stat
                         const uint64_t v2[4], const uint64_t s2[4], uint8_t** proof, size_t* proof_len, uint8_t C1_out32[32], uint8_t C2_out32[32]) {
   return guarded(ctx, [&] {
     const std::string what = "equality_prove";
-    const ProveStates st(strobe_state, tape_state, what);
+    ProofStates st(strobe_state, tape_state, what);
     if (!proof || !proof_len || !C1_out32 || !C2_out32) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     const CommitKey g = gens_key(ctx, gens_n, what, "gens_n");
     require_gens_n(g, 1, what, "gens_n", "a scalar's commitment");
     const Fq a1 = scalar_in(v1, what + ": v1"), b1 = scalar_in(s1, what + ": s1"), a2 = scalar_in(v2, what + ": v2"), b2 = scalar_in(s2, what + ": s2");
     gens_host_tables(gens_n);
-    Transcript T = st.ta.open();
-    RandomTape tape(pc_tape_open(tape_state, what));
+    st.open();
     Cp C1, C2;
-    const EqualityProof p = equality_prove(g, T, tape, a1, b1, a2, b2, &C1, &C2);
-    st.ta.close(T);
-    tape.state().export_state(tape_state);
+    const EqualityProof p = equality_prove(g, st.T(), st.tape(), a1, b1, a2, b2, &C1, &C2);
+    st.proved();
     put_bytes(proof, proof_len, to_bincode(p));
     cp_out(C1_out32, C1);
     cp_out(C2_out32, C2);
@@ -1446,16 +1465,14 @@ int sp_equality_verify_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_sta
                          size_t proof_len) {
   return guarded(ctx, [&] {
     const std::string what = "equality_verify";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
+    ProofStates st(strobe_state);
     if (!proof && proof_len) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     const CommitKey g = gens_key(ctx, gens_n, what, "gens_n");
     require_gens_n(g, 1, what, "gens_n", "a scalar's commitment");
     const Cp C1 = cp_in(C1_32, what + ": C1"), C2 = cp_in(C2_32, what + ": C2");
     gens_host_tables(gens_n);
-    Transcript T = ta.open();
-    TranscriptClose close{ta, T};
-    equality_verify_bytes(ctx->c, g, T, C1, C2, proof, proof_len);
+    st.open_verify();
+    equality_verify_bytes(ctx->c, g, st.T(), C1, C2, proof, proof_len);
   });
 }
 
@@ -1464,19 +1481,17 @@ int sp_product_prove_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_state
                        uint8_t X_out32[32], uint8_t Y_out32[32], uint8_t Z_out32[32]) {
   return guarded(ctx, [&] {
     const std::string what = "product_prove";
-    const ProveStates st(strobe_state, tape_state, what);
+    ProofStates st(strobe_state, tape_state, what);
     if (!proof || !proof_len || !X_out32 || !Y_out32 || !Z_out32) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     const CommitKey g = gens_key(ctx, gens_n, what, "gens_n");
     require_gens_n(g, 1, what, "gens_n", "a scalar's commitment");
     const Fq fx = scalar_in(x, what + ": x"), frX = scalar_in(rX, what + ": rX"), fy = scalar_in(y, what + ": y"), frY = scalar_in(rY, what + ": rY"),
              fz = scalar_in(z, what + ": z"), frZ = scalar_in(rZ, what + ": rZ");
     gens_host_tables(gens_n);
-    Transcript T = st.ta.open();
-    RandomTape tape(pc_tape_open(tape_state, what));
+    st.open();
     Cp X, Y, Z;
-    const ProductProof p = product_prove(g, T, tape, fx, frX, fy, frY, fz, frZ, X, Y, Z);
-    st.ta.close(T);
-    tape.state().export_state(tape_state);
+    const ProductProof p = product_prove(g, st.T(), st.tape(), fx, frX, fy, frY, fz, frZ, X, Y, Z);
+    st.proved();
     put_bytes(proof, proof_len, to_bincode(p));
     cp_out(X_out32, X);
     cp_out(Y_out32, Y);
@@ -1487,16 +1502,14 @@ int sp_product_verify_t(sp_ctx* ctx, const sp_gens* gens_n, uint8_t* strobe_stat
                         const uint8_t* proof, size_t proof_len) {
   return guarded(ctx, [&] {
     const std::string what = "product_verify";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
+    ProofStates st(strobe_state);
     if (!proof && proof_len) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     const CommitKey g = gens_key(ctx, gens_n, what, "gens_n");
     require_gens_n(g, 1, what, "gens_n", "a scalar's commitment");
     const Cp X = cp_in(X32, what + ": X"), Y = cp_in(Y32, what + ": Y"), Z = cp_in(Z32, what + ": Z");
     gens_host_tables(gens_n);
-    Transcript T = ta.open();
-    TranscriptClose close{ta, T};
-    product_verify_bytes(ctx->c, g, T, X, Y, Z, proof, proof_len);
+    st.open_verify();
+    product_verify_bytes(ctx->c, g, st.T(), X, Y, Z, proof, proof_len);
   });
 }
 
@@ -1513,7 +1526,7 @@ int sp_dotproduct_prove_t(sp_ctx* ctx, const sp_gens* gens_1, const sp_gens* gen
                           size_t* proof_len, uint8_t Cx_out32[32], uint8_t Cy_out32[32]) {
   return guarded(ctx, [&] {
     const std::string what = "dotproduct_prove";
-    const ProveStates st(strobe_state, tape_state, what);
+    ProofStates st(strobe_state, tape_state, what);
     if (!proof || !proof_len || !Cx_out32 || !Cy_out32 || !x_vec || !a_vec) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     const CommitKey g1 = gens_key(ctx, gens_1, what, "gens_1"), gn = gens_key(ctx, gens_n, what, "gens_n");
     dotproduct_len(g1, gn, n, what);
@@ -1522,12 +1535,10 @@ int sp_dotproduct_prove_t(sp_ctx* ctx, const sp_gens* gens_1, const sp_gens* gen
     const Fq bx = scalar_in(blind_x, what + ": blind_x"), fy = scalar_in(y, what + ": y"), by = scalar_in(blind_y, what + ": blind_y");
     gens_host_tables(gens_1);
     gens_host_tables(gens_n);
-    Transcript T = st.ta.open();
-    RandomTape tape(pc_tape_open(tape_state, what));
+    st.open();
     Cp Cx, Cy;
-    const DotProductProof p = dotproduct_prove(g1, gn, T, tape, fq_vec(x_vec, n), bx, fq_vec(a_vec, n), fy, by, nullptr, nullptr, &Cx, &Cy);
-    st.ta.close(T);
-    tape.state().export_state(tape_state);
+    const DotProductProof p = dotproduct_prove(g1, gn, st.T(), st.tape(), fq_vec(x_vec, n), bx, fq_vec(a_vec, n), fy, by, nullptr, nullptr, &Cx, &Cy);
+    st.proved();
     put_bytes(proof, proof_len, to_bincode(p));
     cp_out(Cx_out32, Cx);
     cp_out(Cy_out32, Cy);
@@ -1537,8 +1548,7 @@ int sp_dotproduct_verify_t(sp_ctx* ctx, const sp_gens* gens_1, const sp_gens* ge
                            const uint8_t Cx32[32], const uint8_t Cy32[32], const uint8_t* proof, size_t proof_len) {
   return guarded(ctx, [&] {
     const std::string what = "dotproduct_verify";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
+    ProofStates st(strobe_state);
     if ((!proof && proof_len) || !a_vec) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     const CommitKey g1 = gens_key(ctx, gens_1, what, "gens_1"), gn = gens_key(ctx, gens_n, what, "gens_n");
     dotproduct_len(g1, gn, n, what);
@@ -1546,9 +1556,8 @@ int sp_dotproduct_verify_t(sp_ctx* ctx, const sp_gens* gens_1, const sp_gens* ge
     const Cp Cx = cp_in(Cx32, what + ": Cx"), Cy = cp_in(Cy32, what + ": Cy");
     gens_host_tables(gens_1);
     gens_host_tables(gens_n);
-    Transcript T = ta.open();
-    TranscriptClose close{ta, T};
-    dotproduct_verify_bytes(ctx->c, g1, gn, T, fq_vec(a_vec, n), Cx, Cy, proof, proof_len);
+    st.open_verify();
+    dotproduct_verify_bytes(ctx->c, g1, gn, st.T(), fq_vec(a_vec, n), Cx, Cy, proof, proof_len);
   });
 }
 
@@ -1576,7 +1585,7 @@ int sp_dotlog_prove_t(sp_ctx* ctx, const sp_dotlog_gens* gens, uint8_t* strobe_s
                       uint8_t Cy_out32[32], uint64_t y_out[4]) {
   return guarded(ctx, [&] {
     const std::string what = "dotlog_prove";
-    const ProveStates st(strobe_state, tape_state, what);
+    ProofStates st(strobe_state, tape_state, what);
     if (!proof || !proof_len || !Cx_out32 || !Cy_out32 || !y_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     require_owned(ctx, gens, what, "gens");
     const size_t n = gens->g->n;
@@ -1584,14 +1593,12 @@ int sp_dotlog_prove_t(sp_ctx* ctx, const sp_dotlog_gens* gens, uint8_t* strobe_s
     const u256* da = dotlog_vec(ctx, a, n, what, "a");
     const Fq bx = scalar_in(blind_x, what + ": blind_x"), by = scalar_in(blind_y, what + ": blind_y");
     const Fq fy = y ? scalar_in(y, what + ": y") : Fq::zero();
-    Transcript T = st.ta.open();
-    RandomTape tape(pc_tape_open(tape_state, what));
+    st.open();
     DotProductProofLog p;
     Cp Cx, Cy;
     Fq y_used;
-    dotlog_prove(ctx->c, *gens->g, T, tape, dx, bx, da, y ? &fy : nullptr, by, p, Cx, Cy, y_used);
-    st.ta.close(T);
-    tape.state().export_state(tape_state);
+    dotlog_prove(ctx->c, *gens->g, st.T(), st.tape(), dx, bx, da, y ? &fy : nullptr, by, p, Cx, Cy, y_used);
+    st.proved();
     put_bytes(proof, proof_len, to_bincode(p));
     cp_out(Cx_out32, Cx);
     cp_out(Cy_out32, Cy);
@@ -1603,16 +1610,14 @@ int sp_dotlog_verify_t(sp_ctx* ctx, const sp_dotlog_gens* gens, uint8_t* strobe_
                        const uint8_t Cy32[32], const uint8_t* proof, size_t proof_len) {
   return guarded(ctx, [&] {
     const std::string what = "dotlog_verify";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
+    ProofStates st(strobe_state);
     if (!proof && proof_len) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     require_owned(ctx, gens, what, "gens");
     if (n != gens->g->n) throw SpError(SP_ERR_INVALID_ARG, what + ": n = " + std::to_string(n) + " but gens have n = " + std::to_string(gens->g->n));
     const u256* da = dotlog_vec(ctx, a, n, what, "a");
     const Cp Cx = cp_in(Cx32, what + ": Cx"), Cy = cp_in(Cy32, what + ": Cy");
-    Transcript T = ta.open();
-    TranscriptClose close{ta, T};
-    dotlog_verify_bytes(ctx->c, *gens->g, T, da, Cx, Cy, proof, proof_len);
+    st.open_verify();
+    dotlog_verify_bytes(ctx->c, *gens->g, st.T(), da, Cx, Cy, proof, proof_len);
     flush_fine(ctx->c);
   });
 }
@@ -1663,13 +1668,11 @@ int sp_pc_commit(sp_ctx* ctx, const sp_pc_gens* gens, sp_poly* const* polys, int
     pc_check_gens(ctx, gens, ell, what);
     const size_t L = (size_t)1 << (ell / 2);
     std::vector<Fq> blinds(L, Fq::zero());
-    std::unique_ptr<RandomTape> tape;
-    if (tape_state) {
-      tape.reset(new RandomTape(pc_tape_open(tape_state, what)));
-      blinds = tape->random_vector("poly_blinds", L);   // dense_mlpoly.rs:185-189
-    }
-    const std::vector<uint8_t> bytes = to_bincode(pc_commit(ctx->c, gens->g, t.d.data(), k, m, tape ? blinds.data() : nullptr));
-    if (tape) tape->state().export_state(tape_state);
+    ProofStates st = ProofStates::tape_only(tape_state);
+    st.open();
+    if (tape_state) blinds = st.tape().random_vector("poly_blinds", L);   // dense_mlpoly.rs:185-189
+    const std::vector<uint8_t> bytes = to_bincode(pc_commit(ctx->c, gens->g, t.d.data(), k, m, tape_state ? blinds.data() : nullptr));
+    st.proved();
     put_bytes(comm, comm_len, bytes);
     if (blinds_out) put_scalars(blinds_out, blinds);
   });
@@ -1680,8 +1683,7 @@ int sp_pc_eval_prove_t(sp_ctx* ctx, const sp_pc_gens* gens, const sp_poly* poly,
                        uint64_t Zr_out[4]) {
   return guarded(ctx, [&] {
     const std::string what = "pc_eval_prove";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
+    ProofStates st(strobe_state);
     if (!poly || !proof || !proof_len || !C_Zr32 || !Zr_out || (!r && ell)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     sp_poly* const p = const_cast<sp_poly*>(poly);
     if (log2_ceil(caller_tables(ctx, &p, 1, what, 1).len) != ell || ell > PC_MAX_VARS)
@@ -1692,16 +1694,15 @@ int sp_pc_eval_prove_t(sp_ctx* ctx, const sp_pc_gens* gens, const sp_poly* poly,
     if (Zr) require_reduced(Zr, 1, "pc_eval_prove: Zr");
     if (blind_Zr) require_reduced(blind_Zr, 1, "pc_eval_prove: blind_Zr");
     if (blinds) require_reduced(blinds, L, "pc_eval_prove: blinds");
-    RandomTape tape(pc_tape_open(tape_state, what));
-    Transcript T = ta.open();
+    st.open_tape(tape_state, what);
+    st.open();
     const std::vector<Fq> bl = blinds ? fq_vec(blinds, L) : std::vector<Fq>();
     const Fq Zr_in = Zr ? fq_in(Zr) : Fq::zero(), bZr = blind_Zr ? fq_in(blind_Zr) : Fq::zero();
     PolyEvalProof P;
     Cp C;
     Fq zr;
-    polyeval_prove(ctx->c, poly->d.p, blinds ? &bl : nullptr, fq_vec(r, ell), Zr ? &Zr_in : nullptr, blind_Zr ? &bZr : nullptr, gens->g, T, tape, P, C, &zr);
-    ta.close(T);
-    tape.state().export_state(tape_state);
+    polyeval_prove(ctx->c, poly->d.p, blinds ? &bl : nullptr, fq_vec(r, ell), Zr ? &Zr_in : nullptr, blind_Zr ? &bZr : nullptr, gens->g, st.T(), st.tape(), P, C, &zr);
+    st.proved();
     put_bytes(proof, proof_len, to_bincode(P));
     memcpy(C_Zr32, C.b, 32);
     fq_out(Zr_out, zr);
@@ -1712,8 +1713,7 @@ int sp_pc_eval_verify_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t* comm
                         const uint64_t Zr[4], uint8_t* strobe_state, const uint8_t* proof, size_t proof_len) {
   return guarded(ctx, [&] {
     const std::string what = "pc_eval_verify";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
+    ProofStates st(strobe_state);
     if ((!comm && comm_len) || (!proof && proof_len) || (!r && ell)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     if (!C_Zr32 == !Zr) throw SpError(SP_ERR_INVALID_ARG, what + ": give exactly one of C_Zr and Zr");
     if (ell > PC_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(ell) + " > " + std::to_string(PC_MAX_VARS));
@@ -1724,9 +1724,8 @@ int sp_pc_eval_verify_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t* comm
     Cp c;
     if (C_Zr32) memcpy(c.b, C_Zr32, 32);
     const Fq zr = Zr ? fq_in(Zr) : Fq::zero();
-    Transcript T = ta.open();
-    TranscriptClose close{ta, T};
-    pc_eval_verify(ctx->c, gens->g, pc, fq_vec(r, ell), C_Zr32 ? &c : nullptr, Zr ? &zr : nullptr, T, proof, proof_len);
+    st.open_verify();
+    pc_eval_verify(ctx->c, gens->g, pc, fq_vec(r, ell), C_Zr32 ? &c : nullptr, Zr ? &zr : nullptr, st.T(), proof, proof_len);
   });
 }
 
@@ -1734,8 +1733,7 @@ int sp_pc_eval_prove_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, sp_poly* const
                              uint8_t* strobe_state, uint8_t* tape_state, uint8_t** proof, size_t* proof_len, uint64_t* evals_out) {
   return guarded(ctx, [&] {
     const std::string what = "pc_eval_prove_joint";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
+    ProofStates st(strobe_state);
     if (!proof || !proof_len || !evals_out || (!r && m)) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     require_count(what, k, "tables", "SP_PC_MAX_TABLES", SP_PC_MAX_TABLES);
     const Tables t = caller_tables(ctx, polys, k, what, 1);
@@ -1745,14 +1743,13 @@ int sp_pc_eval_prove_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, sp_poly* const
     pc_check_gens(ctx, gens, ell, what);
     require_reduced(r, m, "pc_eval_prove_joint: r");
     if (blinds) require_reduced(blinds, L, "pc_eval_prove_joint: blinds");
-    RandomTape tape(pc_tape_open(tape_state, what));
-    Transcript T = ta.open();
+    st.open_tape(tape_state, what);
+    st.open();
     const std::vector<Fq> bl = blinds ? fq_vec(blinds, L) : std::vector<Fq>();
     PolyEvalProof P;
     std::vector<Fq> evals;
-    pc_eval_prove_joint(ctx->c, gens->g, t.d.data(), k, fq_vec(r, m), blinds ? &bl : nullptr, T, tape, P, evals);
-    ta.close(T);
-    tape.state().export_state(tape_state);
+    pc_eval_prove_joint(ctx->c, gens->g, t.d.data(), k, fq_vec(r, m), blinds ? &bl : nullptr, st.T(), st.tape(), P, evals);
+    st.proved();
     put_bytes(proof, proof_len, to_bincode(P));
     put_scalars(evals_out, evals);
   });
@@ -1762,8 +1759,7 @@ int sp_pc_eval_verify_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t
                               int k, uint8_t* strobe_state, const uint8_t* proof, size_t proof_len) {
   return guarded(ctx, [&] {
     const std::string what = "pc_eval_verify_joint";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
+    ProofStates st(strobe_state);
     if ((!comm && comm_len) || (!proof && proof_len) || (!r && m) || !evals) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     require_count(what, k, "evaluations", "SP_PC_MAX_TABLES", SP_PC_MAX_TABLES);
     if (m > PC_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": |r| = " + std::to_string(m) + " > " + std::to_string(PC_MAX_VARS));
@@ -1771,9 +1767,8 @@ int sp_pc_eval_verify_joint_t(sp_ctx* ctx, const sp_pc_gens* gens, const uint8_t
     require_reduced(r, m, "pc_eval_verify_joint: r");
     require_reduced(evals, (size_t)k, "pc_eval_verify_joint: evals");
     const PolyCommitment pc = from_bincode<PolyCommitment>(comm, comm_len, SP_ERR_INVALID_ARG, "polynomial commitment");
-    Transcript T = ta.open();
-    TranscriptClose close{ta, T};
-    pc_eval_verify_joint(ctx->c, gens->g, pc, fq_vec(r, m), fq_vec(evals, (size_t)k), T, proof, proof_len);
+    st.open_verify();
+    pc_eval_verify_joint(ctx->c, gens->g, pc, fq_vec(r, m), fq_vec(evals, (size_t)k), st.T(), proof, proof_len);
   });
 }
 
@@ -1816,8 +1811,7 @@ int sp_prod_build_dotp(sp_ctx* ctx, sp_poly* const* tables, int ntables, const s
 // the body of sp_prod_prove_t (dotp_evals_out NULL: refuses a handle with dot products) and sp_prod_prove_dotp_t
 static void prod_prove_entry(sp_ctx* ctx, sp_prod_circuits* c, uint8_t* strobe_state, uint8_t** proof, size_t* proof_len, uint64_t* rand_out,
                              uint64_t* leaf_evals_out, uint64_t* dotp_evals_out, bool with_dotp, const std::string& what) {
-  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-  ta.check();
+  ProofStates st(strobe_state);
   if (!proof || !proof_len || !rand_out || !leaf_evals_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
   require_owned(ctx, c, what, "circuits handle");
   if (c->spent) throw SpError(SP_ERR_INVALID_ARG, what + ": the circuits were consumed by an earlier proof (their layers are bound in place)");
@@ -1826,14 +1820,14 @@ static void prod_prove_entry(sp_ctx* ctx, sp_prod_circuits* c, uint8_t* strobe_s
   if (!c->dotps.d.empty() && !dotp_evals_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
   std::vector<ProdCircuit*> cs;
   for (auto& p : c->cs) cs.push_back(p.get());
-  Transcript T = ta.open();
+  st.open();
   c->spent = true;
   ProductCircuitEvalProofBatched P;
   std::vector<Fq> rand, evals, dotp_evals;
-  prod_prove(ctx->c, cs, c->dotps.d, T, P, rand, evals, dotp_evals);
+  prod_prove(ctx->c, cs, c->dotps.d, st.T(), P, rand, evals, dotp_evals);
   c->cs.clear();
   c->dotps = ProdDotps();
-  ta.close(T);
+  st.proved();
   put_bytes(proof, proof_len, to_bincode(P));
   put_scalars(rand_out, rand);
   put_scalars(leaf_evals_out, evals);
@@ -1854,17 +1848,15 @@ void sp_prod_free(sp_prod_circuits* c) { delete c; }
 // the body of sp_prod_verify_t (kd = 0) and sp_prod_verify_dotp_t; host only
 static void prod_verify_entry(const uint8_t* proof, size_t proof_len, const uint64_t* products, int k, const uint64_t* dotp_claims, int kd, size_t m,
                               uint8_t* strobe_state, uint64_t* rand_out, uint64_t* leaf_claims_out, uint64_t* dotp_claims_out, const std::string& what) {
-  const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-  ta.check();
+  ProofStates st(strobe_state);
   if ((!proof && proof_len) || !products || !rand_out || !leaf_claims_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
   require_count(what, k, "products", "SP_PROD_MAX_CIRCUITS", SP_PROD_MAX_CIRCUITS);
   if (dotp_claims) dotp_counts(k, kd, what);
   if (m < 1 || m > PROD_MAX_VARS) throw SpError(SP_ERR_INVALID_ARG, what + ": m = " + std::to_string(m) + "; 1 .. " + std::to_string(PROD_MAX_VARS) + " supported");
   require_reduced(products, (size_t)k, (what + ": product").c_str());
   require_reduced(dotp_claims, 2 * (size_t)kd, (what + ": dotp claim").c_str());
-  Transcript T = ta.open();
-  TranscriptClose close{ta, T};
-  const BatchedOut o = prod_verify(proof, proof_len, fq_vec(products, (size_t)k), fq_vec(dotp_claims, 2 * (size_t)kd), m, T);
+  st.open_verify();
+  const BatchedOut o = prod_verify(proof, proof_len, fq_vec(products, (size_t)k), fq_vec(dotp_claims, 2 * (size_t)kd), m, st.T());
   put_scalars(rand_out, o.rand);
   put_scalars(leaf_claims_out, o.claims);
   if (dotp_claims_out) put_scalars(dotp_claims_out, o.claims_dotp);
@@ -1944,9 +1936,7 @@ static void spark_commit_common(sp_ctx* ctx, const sp_spark_gens* gens, const sp
   }
   if (N < 2) throw SpError(SP_ERR_INVALID_ARG, what + ": every matrix has at most one entry (num_ops = 1 leaves the product circuits without layers)");
   spark_check_gens(ctx, gens, x, y, N, (size_t)b, what);
-  // the caller's entries on the device (host arrays are copied as they are) meet the checks of sp_instance_create: row < 2^x, col < 2^y, val < q
-  DevBuf<uint64_t> d_row[SP_SPARK_MAX_BATCH], d_col[SP_SPARK_MAX_BATCH];
-  DevBuf<uint8_t> d_val[SP_SPARK_MAX_BATCH];
+  // the caller's entries meet the checks of sp_instance_create: row < 2^x, col < 2^y, val < q
   DevBuf<uint32_t> row[SP_SPARK_MAX_BATCH], col[SP_SPARK_MAX_BATCH];
   DevBuf<u256> val[SP_SPARK_MAX_BATCH];
   dev::CooIn in{};
@@ -1955,31 +1945,12 @@ static void spark_commit_common(sp_ctx* ctx, const sp_spark_gens* gens, const sp
   for (int m = 0; m < b; m++) {
     const sp_spark_entries& e = mats[m];
     in.row[m] = e.row; in.col[m] = e.col; in.val[m] = e.val32; in.n[m] = e.nnz;
-    if (!device) {
-      d_row[m].alloc(e.nnz); d_col[m].alloc(e.nnz); d_val[m].alloc(32 * e.nnz);
-      dev::h2d(d_row[m].p, e.row, e.nnz * sizeof(uint64_t), c.stream);
-      dev::h2d(d_col[m].p, e.col, e.nnz * sizeof(uint64_t), c.stream);
-      dev::h2d(d_val[m].p, e.val32, 32 * e.nnz, c.stream);
-      in.row[m] = d_row[m].p; in.col[m] = d_col[m].p; in.val[m] = d_val[m].p;
-    }
     row[m].alloc(e.nnz); col[m].alloc(e.nnz); val[m].alloc(e.nnz);
     co.row[m] = row[m].p; co.col[m] = col[m].p; co.val[m] = val[m].p;
     sm[m] = SparkMatrix{row[m].p, col[m].p, val[m].p, e.nnz};
   }
-  DevBuf<unsigned long long> err(1);
-  dev::set_max_u64(err.p, c.stream);
   const size_t ncols = (size_t)1 << y;
-  dev::inst_ingest(in, b, co, (size_t)1 << x, ncols, ncols, 0, err.p, c.stream);
-  unsigned long long first = 0;
-  dev::d2h(&first, err.p, sizeof(first), c.stream);
-  c.sync();
-  if (first != ~0ull) {   // the first bad entry in (matrix, entry) order; within it row, then column, then scalar
-    const unsigned code = (unsigned)(first & 3);
-    const std::string at = " (matrix " + std::to_string(first >> 42) + ", entry " + std::to_string((first >> 2) & (((unsigned long long)1 << 40) - 1)) + ")";
-    if (code == dev::INGEST_ROW) throw SpError(SP_ERR_INVALID_INDEX, what + ": row out of range" + at);
-    if (code == dev::INGEST_COL) throw SpError(SP_ERR_INVALID_INDEX, what + ": col out of range" + at);
-    throw SpError(SP_ERR_INVALID_SCALAR, what + ": value not a canonical scalar" + at);
-  }
+  ingest(c, in, b, !device, co, (size_t)1 << x, ncols, ncols, 0, [&](size_t m, size_t k, unsigned code) { refuse_entry(what, m, k, code); });
   std::unique_ptr<sp_spark_dense> d(new sp_spark_dense{&c, {}});
   SparseMatPolyCommitment cm;
   spark_commit(c, sm, (size_t)b, x, y, gens->g, d->d, cm);
@@ -2035,27 +2006,25 @@ int sp_spark_eval_prove_t(sp_ctx* ctx, const sp_spark_dense* dense, const sp_spa
                           const uint64_t* evals, uint8_t* strobe_state, uint8_t* tape_state, uint8_t** proof, size_t* proof_len, uint64_t* evals_out) {
   return guarded(ctx, [&] {
     const std::string what = "spark_eval_prove";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
+    ProofStates st(strobe_state);
     if (!proof || !proof_len || !evals_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     require_owned(ctx, dense, what, "dense handle");
     const SparkDense& d = dense->d;
     spark_check_gens(ctx, gens, d.x, d.y, d.N, d.b, what);
     spark_point(dense, rx, x, ry, y, what);
     if (evals) require_reduced(evals, d.b, (what + ": evals").c_str());
-    RandomTape tape(pc_tape_open(tape_state, what));
+    st.open_tape(tape_state, what);
     const std::vector<Fq> vx = fq_vec(rx, x), vy = fq_vec(ry, y);
     std::vector<Fq> ev(d.b);
     spark_evaluate(ctx->c, d, vx, vy, ev.data());
     if (evals)
       for (size_t m = 0; m < d.b; m++)
         if (!(fq_in(evals + 4 * m) == ev[m])) throw SpError(SP_ERR_INVALID_ARG, what + ": evals[" + std::to_string(m) + "] is not M_" + std::to_string(m) + "(rx, ry)");
-    Transcript T = ta.open();
+    st.open();
     ctx->c.timings.clear();
     SparseMatPolyEvalProof P;
-    spark_eval_prove(ctx->c, d, vx, vy, ev, gens->g, T, tape, P);
-    ta.close(T);
-    tape.state().export_state(tape_state);
+    spark_eval_prove(ctx->c, d, vx, vy, ev, gens->g, st.T(), st.tape(), P);
+    st.proved();
     put_bytes(proof, proof_len, to_bincode(P));
     put_scalars(evals_out, ev);
   });
@@ -2064,8 +2033,7 @@ int sp_spark_eval_verify_t(sp_ctx* ctx, const sp_spark_gens* gens, const uint8_t
                            size_t y, const uint64_t* evals, int b, uint8_t* strobe_state, const uint8_t* proof, size_t proof_len) {
   return guarded(ctx, [&] {
     const std::string what = "spark_eval_verify";
-    const TranscriptArg ta = TranscriptArg::caller(strobe_state);
-    ta.check();
+    ProofStates st(strobe_state);
     if ((!comm && comm_len) || (!proof && proof_len) || (!rx && x) || (!ry && y) || !evals) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
     require_count(what, b, "evaluations", "SP_SPARK_MAX_BATCH", SP_SPARK_MAX_BATCH);
     require_owned(ctx, gens, what, "gens handle");
@@ -2075,9 +2043,8 @@ int sp_spark_eval_verify_t(sp_ctx* ctx, const sp_spark_gens* gens, const uint8_t
     require_reduced(evals, (size_t)b, (what + ": evals").c_str());
     const SparseMatPolyCommitment cm = from_bincode<SparseMatPolyCommitment>(comm, comm_len, SP_ERR_VERIFY, "sparse polynomial commitment");
     check_spark_commitment(cm, (size_t)b, x, y, gens->g);
-    Transcript T = ta.open();
-    TranscriptClose close{ta, T};
-    spark_eval_verify(ctx->c, cm, fq_vec(rx, x), fq_vec(ry, y), fq_vec(evals, (size_t)b), gens->g, T, proof, proof_len);
+    st.open_verify();
+    spark_eval_verify(ctx->c, cm, fq_vec(rx, x), fq_vec(ry, y), fq_vec(evals, (size_t)b), gens->g, st.T(), proof, proof_len);
   });
 }
 
@@ -2127,32 +2094,12 @@ static void spmat_create_common(sp_ctx* ctx, const sp_spark_entries* mats, int b
     if (!n) continue;
     dev::CooIn in{};
     in.row[0] = e.row; in.col[0] = e.col; in.val[0] = e.val32; in.n[0] = n;
-    DevBuf<uint64_t> d_row, d_col;
-    DevBuf<uint8_t> d_val;
-    if (!device) {
-      d_row.alloc(n); d_col.alloc(n); d_val.alloc(32 * n);
-      dev::h2d(d_row.p, e.row, n * sizeof(uint64_t), c.stream);
-      dev::h2d(d_col.p, e.col, n * sizeof(uint64_t), c.stream);
-      dev::h2d(d_val.p, e.val32, 32 * n, c.stream);
-      in.row[0] = d_row.p; in.col[0] = d_col.p; in.val[0] = d_val.p;
-    }
     DevBuf<uint32_t> row(n), col(n);
     DevBuf<u256> val(n);
     dev::CooOut co{};
     co.row[0] = row.p; co.col[0] = col.p; co.val[0] = val.p;
-    DevBuf<unsigned long long> err(1);
-    dev::set_max_u64(err.p, c.stream);
-    dev::inst_ingest(in, 1, co, (size_t)1 << x, (size_t)1 << y, (size_t)1 << y, 0, err.p, c.stream);
-    unsigned long long first = 0;
-    dev::d2h(&first, err.p, sizeof(first), c.stream);
-    c.sync();
-    if (first != ~0ull) {   // the matrices are checked in order, so this is the first bad entry in (matrix, entry) order
-      const unsigned code = (unsigned)(first & 3);
-      const std::string at = " (matrix " + std::to_string(m) + ", entry " + std::to_string((first >> 2) & (((unsigned long long)1 << 40) - 1)) + ")";
-      if (code == dev::INGEST_ROW) throw SpError(SP_ERR_INVALID_INDEX, what + ": row out of range" + at);
-      if (code == dev::INGEST_COL) throw SpError(SP_ERR_INVALID_INDEX, what + ": col out of range" + at);
-      throw SpError(SP_ERR_INVALID_SCALAR, what + ": value not a canonical scalar" + at);
-    }
+    // the matrices are ingested in order, so a bad entry here is the first in (matrix, entry) order
+    ingest(c, in, 1, !device, co, (size_t)1 << x, (size_t)1 << y, (size_t)1 << y, 0, [&](size_t, size_t k, unsigned code) { refuse_entry(what, m, k, code); });
     DevBuf<uint8_t> scratch(dev::spmat_sort_scratch_bytes(n));
     SpmatOrder& R = S->by_row[m];
     SpmatOrder& C = S->by_col[m];

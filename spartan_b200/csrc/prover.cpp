@@ -145,22 +145,29 @@ std::vector<Fq> Ctx::download(const u256* d, size_t n) {
   return v;
 }
 
-static std::vector<uint8_t> gens_seed(const std::string& label) {   // MultiCommitGens::new (commitments.rs:15-33): SHAKE256(label || basepoint)
+void label_gens(Ctx& c, const std::string& label, size_t n, ge* out, const std::function<void(size_t i0, size_t m, const ge* pts)>& sink) {
   static const uint8_t basepoint[32] = {0xe2, 0xf2, 0xae, 0x0a, 0x6a, 0xbc, 0x4e, 0x71, 0xa8, 0x84, 0xa9, 0x61, 0xc5, 0x00, 0x51, 0x5f,
                                         0x58, 0xe3, 0x0b, 0x6a, 0xa5, 0x82, 0xdd, 0x8d, 0xb6, 0xa6, 0x59, 0x45, 0xe0, 0x8d, 0x2d, 0x76};
   std::vector<uint8_t> seed(label.begin(), label.end());
   seed.insert(seed.end(), basepoint, basepoint + 32);
-  return seed;
+  Shake256 xof(seed.data(), seed.size());
+  const size_t slab = std::min<size_t>((size_t)1 << 18, std::max<size_t>(n, 1));
+  std::vector<uint8_t> uni(64 * slab);
+  DevBuf<uint8_t> d_uni(uni.size());
+  DevBuf<ge> own(out ? 0 : slab);
+  for (size_t i0 = 0; i0 < n; i0 += slab) {
+    const size_t m = std::min(slab, n - i0);
+    ge* pts = out ? out + i0 : own.p;
+    xof.squeeze(uni.data(), 64 * m);
+    dev::h2d(d_uni.p, uni.data(), 64 * m, c.stream);
+    dev::gens_from_uniform(pts, d_uni.p, m, c.stream);
+    if (sink) sink(i0, m, pts);
+    c.sync();
+  }
 }
 GenSet::GenSet(Ctx* c, const std::string& label_, size_t nbases_, const std::vector<size_t>& host_bases) : ctx(c), label(label_), nbases(nbases_) {
-  // 64 bytes of the label's stream per generator
-  const std::vector<uint8_t> seed = gens_seed(label);
-  std::vector<uint8_t> uni(64 * nbases);
-  shake256(uni.data(), uni.size(), seed.data(), seed.size());
-  DevBuf<uint8_t> d_uni(uni.size());
-  dev::h2d(d_uni.p, uni.data(), uni.size(), ctx->stream);
   G.alloc(nbases);
-  dev::gens_from_uniform(G.p, d_uni.p, nbases, ctx->stream);
+  label_gens(*ctx, label, nbases, G.p, nullptr);
   finish(host_bases);
 }
 GenSet::GenSet(Ctx* c, const ge* d_points, size_t nbases_, const std::vector<size_t>& host_bases) : ctx(c), label("<uploaded>"), nbases(nbases_) {
@@ -887,23 +894,14 @@ DotLogGens::DotLogGens(Ctx& c, size_t n_, const std::string& label) : ctx(&c), n
     g = pc_gens_view(*set, 2 * log2_ceil(n));
     return;
   }
-  // the label's n + 2 points in slabs (so 2^24 points need no 1 GiB staging buffer): G[0..n) as niels into pts, G_n and h into the small set
-  const std::vector<uint8_t> seed = gens_seed(label);
-  Shake256 xof(seed.data(), seed.size());
+  // the label's n + 2 points: G[0..n) as niels into pts, G_n and h into the small set
   pts.alloc(n);
-  const size_t total = n + 2, slab = std::min<size_t>((size_t)1 << 18, total);
-  std::vector<uint8_t> uni(64 * slab);
-  DevBuf<uint8_t> d_uni(uni.size());
-  DevBuf<ge> gbuf(slab), last(2);
-  for (size_t i0 = 0; i0 < total; i0 += slab) {
-    const size_t m = std::min(slab, total - i0), in_g = i0 < n ? std::min(m, n - i0) : 0;
-    xof.squeeze(uni.data(), 64 * m);
-    dev::h2d(d_uni.p, uni.data(), 64 * m, c.stream);
-    dev::gens_from_uniform(gbuf.p, d_uni.p, m, c.stream);
-    dev::points_to_niels(pts.p + i0, gbuf.p, in_g, c.stream);
-    if (m > in_g) dev::d2d(last.p + (i0 + in_g - n), gbuf.p + in_g, (m - in_g) * sizeof(ge), c.stream);
-    c.sync();
-  }
+  DevBuf<ge> last(2);
+  label_gens(c, label, n + 2, nullptr, [&](size_t i0, size_t m, const ge* gbuf) {
+    const size_t in_g = i0 < n ? std::min(m, n - i0) : 0;
+    dev::points_to_niels(pts.p + i0, gbuf, in_g, c.stream);
+    if (m > in_g) dev::d2d(last.p + (i0 + in_g - n), gbuf + in_g, (m - in_g) * sizeof(ge), c.stream);
+  });
   set.reset(new GenSet(&c, last.p, 2, {0, 1}));
   g.n = n;
   g.gens_1 = CommitKey{set.get(), 0, 1, 1};

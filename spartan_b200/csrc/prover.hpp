@@ -163,6 +163,12 @@ Cp zk_sumcheck_verify_bytes(Ctx& ctx, const uint8_t* proof, size_t len, const Cp
 void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt, const std::vector<Fq>& r, const Fq* Zr, const Fq* blind_Zr_opt,
                     const PolyCommitmentGens& gens, Transcript& T, RandomTape& tape, PolyEvalProof& proof, Cp& C_Zr, Fq* Zr_out = nullptr);
 
+// MultiCommitGens::new(n, label) (commitments.rs:15-33): point i is gens_from_uniform of bytes [64 i, 64 i + 64) of SHAKE256(label || basepoint).
+// Points [0, n) are made in slabs of at most 2^18, so 2^24 points need no 1 GiB staging buffer.  They go to out[0, n) when out is given, else to
+// a slab buffer of this call's; sink(i0, m, pts), when given, then receives points [i0, i0 + m) at pts on the device, valid until the sink's work
+// on the context's stream has run.
+void label_gens(Ctx& c, const std::string& label, size_t n, ge* out, const std::function<void(size_t i0, size_t m, const ge* pts)>& sink);
+
 // ---- DotProductProofLog of the caller's vectors (sp_dotlog_*), on this rank's GPU alone
 // DotProductProofGens::new(n, label) (nizk/mod.rs:414-419).  n <= SP_DOTLOG_TABLE_MAX_N: `set` holds the n + 2 generators with the window tables of
 // sp_pc_gens_create's set and `g` views it, as PolyEvalProof's gens.  Larger n (folding()): `pts` holds G[0..n) as affine niels points, `set` the

@@ -10,6 +10,7 @@ from oracle.spartan_ref import core as oc
 
 LABEL = b"cabi-boundary"
 SP_ERR_INVALID_ARG = 3
+SP_ERR_INVALID_SCALAR = 5
 
 
 @pytest.fixture(scope="module")
@@ -132,3 +133,35 @@ def test_context_entries_refuse_a_bad_state(sb):
     rand, evals = np.zeros((m, 4), dtype=np.uint64), np.zeros((3, 4), dtype=np.uint64)
     refused(sb.lib.sp_prod_prove_t(ctx.h, circuits.h, t.state, C.byref(out), C.byref(ln), ptr(rand), ptr(evals)), st)
     sb.ProductCircuitEvalProofBatched.prove(circuits, sb.Transcript(LABEL))   # the refused call did not consume the circuits
+
+
+@pytest.mark.gpu
+def test_a_null_tape_is_refused_after_the_other_arguments(sb):
+    """sp_pc_eval_prove_t and sp_pc_eval_prove_joint_t check every other argument before they look at the tape: a NULL tape next to an
+    unreduced scalar reports the scalar, and alone it reports the tape, both leaving the transcript as it was"""
+    ctx = sb.default_context()
+    m, k = 4, 2
+    polys = [sb.DensePolynomial(oc.prg_scalars("cabi-null-tape-%d" % j, 1 << m)) for j in range(k)]
+    good_r = limbs(oc.prg_scalars("cabi-null-tape-r", m))
+    bad_r = good_r.copy()
+    bad_r[0] = np.frombuffer(oc.Q.to_bytes(32, "little"), dtype=np.uint64)
+    out, ln = C.POINTER(C.c_ubyte)(), C.c_size_t()
+    c_zr, zr, evals = C.create_string_buffer(32), np.zeros(4, dtype=np.uint64), np.zeros((k, 4), dtype=np.uint64)
+    gens, joint_gens = sb.PolyCommitmentGens(m, LABEL), sb.PolyCommitmentGens(m + 1, LABEL)
+    t = sb.Transcript(LABEL)
+    before = t.state.raw
+
+    def single(r):
+        return sb.lib.sp_pc_eval_prove_t(ctx.h, gens.h, polys[0].h, None, ptr(r), C.c_size_t(m), None, None, t.state, None, C.byref(out),
+                                         C.byref(ln), c_zr, ptr(zr))
+
+    def joint(r):
+        return sb.lib.sp_pc_eval_prove_joint_t(ctx.h, joint_gens.h, sb.api._handles(polys), C.c_int(k), None, ptr(r), C.c_size_t(m), t.state, None,
+                                               C.byref(out), C.byref(ln), ptr(evals))
+
+    for call, what in [(single, "pc_eval_prove"), (joint, "pc_eval_prove_joint")]:
+        assert call(bad_r) == SP_ERR_INVALID_SCALAR
+        assert sb.lib.sp_last_error(ctx.h).decode() == what + ": r: scalar limbs are not reduced modulo q"
+        assert call(good_r) == SP_ERR_INVALID_ARG
+        assert sb.lib.sp_last_error(ctx.h).decode() == what + ": tape state is NULL"
+        assert t.state.raw == before
