@@ -430,17 +430,50 @@ std::vector<Fq> ScRounds::wait() {
   return ev;
 }
 
+std::vector<Fq> ScRounds::finals() {
+  const dev::ScInst& in = insts[0];
+  int nt = 0;
+  while (nt < 4 && in.t[nt]) nt++;
+  uint8_t* stage = ctx.pinned + layout::PIN_STAGE.off;
+  for (int k = 0; k < nt; k++) dev::d2h(stage + 32 * k, in.t[k], 32, ctx.stream);   // the replicated copies after a shard exit
+  ctx.sync();
+  std::vector<Fq> f(nt);
+  memcpy(static_cast<void*>(f.data()), stage, 32 * nt);
+  return f;
+}
+
+// The device side of a sumcheck of a caller-defined polynomial: the operations of ScRounds over P (k_scp_eval, k_scp_fold_eval), single GPU
+struct ScPolyRounds {
+  Ctx& ctx;
+  const dev::ScPoly& P;
+  size_t len;
+  u256* d_out = ctx.small.p + layout::SMALL_ROUND.off;   // the d evaluations of a round
+  dev::HostSig sig;
+  void eval() { sig = ctx.next_sig(); dev::scp_eval(P, len, d_out, ctx.red.p, ctx.stream, sig); }
+  void fold_eval(const Fq& r) { sig = ctx.next_sig(); dev::scp_fold_eval(P, len, r.m, d_out, ctx.red.p, ctx.stream, sig); len >>= 1; }
+  void fold(const Fq& r) { dev::fold_top(P.t, P.ntables, len, r.m, ctx.stream); len >>= 1; }
+  std::vector<Fq> published(size_t k) {   // the first k results of the last launch
+    ctx.wait_sig(sig);
+    std::vector<Fq> v(k);
+    memcpy(static_cast<void*>(v.data()), ctx.host_res + layout::RES_OUT.off, k * sizeof(u256));
+    return v;
+  }
+  std::vector<Fq> wait() { return published(P.degree); }   // s(0), s(2) .. s(d)
+  std::vector<Fq> finals() {   // P.t[k][0] of every table, in one launch
+    sig = ctx.next_sig();
+    dev::heads(ctx.small.p + layout::SMALL_HEADS.off, P.t, P.ntables, ctx.stream, sig);
+    return published(P.ntables);
+  }
+};
+
 void poly_sumcheck_prove(Ctx& ctx, const dev::ScPoly& P, size_t len, const Fq& claim, size_t num_rounds, Transcript& T, SumcheckInstanceProof& proof,
                          std::vector<Fq>& r, std::vector<Fq>& finals, Fq& e) {
   const size_t d = (size_t)P.degree;
-  u256* d_out = ctx.small.p + layout::SMALL_ROUND.off;   // the d evaluations of a round
-  dev::HostSig sig = ctx.next_sig();
-  dev::scp_eval(P, len, d_out, ctx.red.p, ctx.stream, sig);
+  ScPolyRounds sc{ctx, P, len};
+  sc.eval();
   e = claim;
   for (size_t j = 0; j < num_rounds; j++) {
-    ctx.wait_sig(sig);
-    std::vector<Fq> ev(d);
-    memcpy(static_cast<void*>(ev.data()), ctx.host_res + layout::RES_OUT.off, d * sizeof(u256));
+    const std::vector<Fq> ev = sc.wait();
     std::vector<Fq> evals(d + 1);   // s_j(0), s_j(1) = e - s_j(0), s_j(2) .. s_j(d)
     evals[0] = ev[0];
     evals[1] = e - ev[0];
@@ -448,22 +481,13 @@ void poly_sumcheck_prove(Ctx& ctx, const dev::ScPoly& P, size_t len, const Fq& c
     UniPoly poly = UniPoly::from_evals(evals);
     poly.append_to_transcript("poly", T);
     const Fq r_j = T.challenge_scalar("challenge_nextround");
-    if (j + 1 < num_rounds) {   // bind and evaluate the next round while the host finishes this one
-      sig = ctx.next_sig();
-      dev::scp_fold_eval(P, len, r_j.m, d_out, ctx.red.p, ctx.stream, sig);
-    } else {
-      dev::fold_top(P.t, P.ntables, len, r_j.m, ctx.stream);
-    }
-    len >>= 1;
+    if (j + 1 < num_rounds) sc.fold_eval(r_j);   // bind and evaluate the next round while the host finishes this one
+    else sc.fold(r_j);
     e = poly.evaluate(r_j);
     proof.compressed_polys.push_back(poly.compress());
     r.push_back(r_j);
   }
-  sig = ctx.next_sig();
-  dev::heads(ctx.small.p + layout::SMALL_HEADS.off, P.t, P.ntables, ctx.stream, sig);
-  ctx.wait_sig(sig);
-  finals.resize(P.ntables);
-  memcpy(static_cast<void*>(finals.data()), ctx.host_res + layout::RES_OUT.off, P.ntables * sizeof(u256));
+  finals = sc.finals();
 }
 
 // ================================================================================================ ZK sumcheck on the device
@@ -472,8 +496,7 @@ void poly_sumcheck_prove(Ctx& ctx, const dev::ScPoly& P, size_t len, const Fq& c
 // Everything of a ZK sumcheck that depends on the random tape only (RandomTape is independent of the transcript): the blinds of the round polynomials and
 // evaluations, the per-round randomness of DotProductProof::prove (nizk/mod.rs:329-331) in the reference's order, and the commitments to them —
 //   delta_j = commit(d_vec_j; r_delta_j) and the blind halves blinds_poly[j]*h, blinds_evals[j]*h, r_beta_j*h — in four batched device MSMs.
-// enqueue() draws and launches (no synchronisation: the results travel to pinned host memory), finish() converts them once the stream has been synchronised;
-// r1cs_prove enqueues phase one's behind the witness commitment's MSM, so that neither the draws nor the launches sit on the critical path.
+// enqueue() draws and launches (no synchronisation: the results travel to pinned host memory), finish() converts them once the stream has been synchronised.
 // the staging area holds, per round, delta_j's encoding and three points
 size_t zk_sumcheck_max_rounds() { return layout::PIN_ZKPRE.cap / (32 + 3 * sizeof(ge)); }
 struct ZkPre {
@@ -485,7 +508,6 @@ struct ZkPre {
   DevBuf<ge> d_pts;
   DevBuf<uint8_t> d_c;
   uint8_t* stage = nullptr;   // pinned: 32*num_rounds encodings, then 3*num_rounds points
-  bool enqueued = false, finished = false;
   void enqueue(Ctx& ctx, int degree, size_t rounds, const CommitKey& g1, const CommitKey& gn, RandomTape& tape) {
     if (rounds > zk_sumcheck_max_rounds()) throw std::runtime_error("spartan_b200: ZK sumcheck with too many rounds for the staging area");
     num_rounds = rounds; nco = (size_t)degree + 1;
@@ -518,10 +540,8 @@ struct ZkPre {
     dev::msm_rows(d_pts.p + 3 * num_rounds, s1.table.p, s1.wbits, s1.rows(), d_s.p, 0, num_rounds, 0, d_b.p + 3 * num_rounds, g1.h, ctx.scratch.p, ctx.stream);  // blinds_evals[j] * h
     dev::d2h(stage, d_c.p, 32 * num_rounds, ctx.stream);
     dev::d2h(stage + 32 * num_rounds, d_pts.p + num_rounds, 3 * num_rounds * sizeof(ge), ctx.stream);
-    enqueued = true;
   }
-  void finish(Ctx& ctx) {   // the stream must have been synchronised after enqueue()
-    if (finished) return;
+  void finish() {   // the stream must have been synchronised after enqueue()
     bp_h.resize(num_rounds); be_h.resize(num_rounds);
     const ge* pts = reinterpret_cast<const ge*>(stage + 32 * num_rounds);
     for (size_t j = 0; j < num_rounds; j++) {
@@ -529,7 +549,6 @@ struct ZkPre {
       pre[j].r_beta_h = to_hge(pts[j]); bp_h[j] = to_hge(pts[num_rounds + j]); be_h[j] = to_hge(pts[2 * num_rounds + j]);
     }
     d_s.release(); d_b.release(); d_pts.release(); d_c.release();
-    finished = true;
   }
 };
 
@@ -584,35 +603,26 @@ struct ZkRounds {
   }
 };
 
-// sharded: `tables` are this rank's cyclic shards (length 2^num_rounds / world).  The first rounds then run on the shards — the fused
-// kernels exchange their partial sums over NVLink before handing the round's evaluations to the host — until the local tables drop below
-// streaming size; the shards are then all-gathered into replicated tables (in the window) and the latency-bound tail runs on every rank alike.
-static void zk_sumcheck_prove(Ctx& ctx, dev::ScKind kind, const Fq& claim, const Fq& blind_claim, size_t num_rounds, u256* const* tables, int nt,
-                              const CommitKey& g1, const CommitKey& gn, Transcript& T, RandomTape& tape, ZKSumcheckInstanceProof& proof,
-                              std::vector<Fq>& r, std::vector<Fq>& finals, Fq& blind_post, bool sharded = false, ZkPre* pre_in = nullptr) {
-  const bool sh = sharded && ctx.shard_world() > 1;
-  const int W = sh ? ctx.shard_world() : 1;
-  const int degree = kind == dev::SC_QUAD ? 2 : 3;
-  ZkPre pre_local;
-  ZkPre& zp = pre_in ? *pre_in : pre_local;
-  if (!zp.enqueued) zp.enqueue(ctx, degree, num_rounds, g1, gn, tape);
-  if (zp.num_rounds != num_rounds || zp.nco != (size_t)degree + 1) throw std::runtime_error("spartan_b200: ZK sumcheck pre-computation of the wrong shape");
-  if (!zp.finished) { ctx.sync(); zp.finish(ctx); }
-  ZkRounds zr(g1, gn, T, tape, zp, proof, (size_t)degree, claim, blind_claim);
-  dev::ScInst inst;
-  for (int t = 0; t < 4; t++) inst.t[t] = t < nt ? tables[t] : nullptr;
-  inst.c_out = inst.t[2];
-  inst.write_c = 1;
-  ScRounds sc{ctx, kind, {inst}, ((size_t)1 << num_rounds) / W, sh, ctx.small.p + layout::SMALL_ROUND.off};
+// The ZK sumcheck of degree `degree` over the device side `sc` (ScRounds or ScPolyRounds), its tables bound in place for num_rounds rounds.  The
+// tape-only commitments (ZkPre) are enqueued ahead of the first evaluation and converted once the stream has run them; then each round's bind
+// (fused with the next round's evaluation) is launched as soon as r_j is drawn, and the host runs the round's sigma protocol while it runs.
+// Out: the proof, r, finals = the tables' first entries after the last bind, blind_post = blinds_evals[num_rounds - 1].
+template <class Rounds>
+static void zk_sumcheck_prove(Ctx& ctx, Rounds& sc, size_t degree, const Fq& claim, const Fq& blind_claim, size_t num_rounds, const CommitKey& g1,
+                              const CommitKey& gn, Transcript& T, RandomTape& tape, ZKSumcheckInstanceProof& proof, std::vector<Fq>& r,
+                              std::vector<Fq>& finals, Fq& blind_post) {
+  ZkPre zp;
+  zp.enqueue(ctx, (int)degree, num_rounds, g1, gn, tape);
   sc.eval();
+  ctx.sync();
+  zp.finish();
+  ZkRounds zr(g1, gn, T, tape, zp, proof, degree, claim, blind_claim);
   for (size_t j = 0; j < num_rounds; j++) {
     FineTimer fw(ctx, "zk wait evals");
     const std::vector<Fq> e = sc.wait();
     fw.stop();
     FineTimer fh(ctx, "zk host commit_poly+challenge");
     const Fq r_j = zr.commit(j, e.data());
-    // bind the tables to r_j on the device right away (fused with the next round's evaluation); the host continues with the
-    // sigma protocol of this round while the kernel runs
     if (j + 1 < num_rounds) sc.fold_eval(r_j);
     else sc.fold(r_j);
     fh.stop();
@@ -620,47 +630,28 @@ static void zk_sumcheck_prove(Ctx& ctx, dev::ScKind kind, const Fq& claim, const
     zr.prove(j, r_j);
     r.push_back(r_j);
   }
-  finals.resize(nt);
-  uint8_t* stage = ctx.pinned + layout::PIN_STAGE.off;
-  for (int t = 0; t < nt; t++) dev::d2h(stage + 32 * t, sc.insts[0].t[t], 32, ctx.stream);   // the replicated copies after a shard exit
-  ctx.sync();
-  memcpy(finals.data(), stage, 32 * nt);
+  finals = sc.finals();
   blind_post = zp.blinds_evals[num_rounds - 1];
 }
 
 void zk_poly_sumcheck_prove(Ctx& ctx, const dev::ScPoly& P, size_t len, const Fq& claim, const Fq& blind_claim, size_t num_rounds, const CommitKey& g1,
                             const CommitKey& gn, Transcript& T, RandomTape& tape, ZKSumcheckInstanceProof& proof, std::vector<Fq>& r,
                             std::vector<Fq>& finals, Fq& blind_post) {
-  const size_t d = (size_t)P.degree;
-  ZkPre zp;
-  zp.enqueue(ctx, P.degree, num_rounds, g1, gn, tape);
-  u256* d_out = ctx.small.p + layout::SMALL_ROUND.off;   // the d evaluations of a round
-  dev::HostSig sig = ctx.next_sig();
-  dev::scp_eval(P, len, d_out, ctx.red.p, ctx.stream, sig);
-  ctx.sync();
-  zp.finish(ctx);
-  ZkRounds zr(g1, gn, T, tape, zp, proof, d, claim, blind_claim);
-  std::vector<Fq> ev(d);
-  for (size_t j = 0; j < num_rounds; j++) {
-    ctx.wait_sig(sig);
-    memcpy(static_cast<void*>(ev.data()), ctx.host_res + layout::RES_OUT.off, d * sizeof(u256));
-    const Fq r_j = zr.commit(j, ev.data());
-    if (j + 1 < num_rounds) {   // bind and evaluate the next round while the host runs this round's sigma protocol
-      sig = ctx.next_sig();
-      dev::scp_fold_eval(P, len, r_j.m, d_out, ctx.red.p, ctx.stream, sig);
-    } else {
-      dev::fold_top(P.t, P.ntables, len, r_j.m, ctx.stream);
-    }
-    len >>= 1;
-    zr.prove(j, r_j);
-    r.push_back(r_j);
-  }
-  sig = ctx.next_sig();
-  dev::heads(ctx.small.p + layout::SMALL_HEADS.off, P.t, P.ntables, ctx.stream, sig);
-  ctx.wait_sig(sig);
-  finals.resize(P.ntables);
-  memcpy(static_cast<void*>(finals.data()), ctx.host_res + layout::RES_OUT.off, P.ntables * sizeof(u256));
-  blind_post = zp.blinds_evals[num_rounds - 1];
+  ScPolyRounds sc{ctx, P, len};
+  zk_sumcheck_prove(ctx, sc, (size_t)P.degree, claim, blind_claim, num_rounds, g1, gn, T, tape, proof, r, finals, blind_post);
+}
+
+// One instance of a fixed-kind sumcheck over the nt tables (2^num_rounds entries, bound in place), for R1CS phase one (SC_CUBIC4) and two (SC_QUAD).
+// sharded: `tables` are this rank's cyclic shards (length 2^num_rounds / world).  The first rounds then run on the shards — the fused kernels
+// exchange their partial sums over NVLink before handing the round's evaluations to the host — until the local tables drop below streaming size;
+// the shards are then all-gathered into replicated tables (in the window) and the latency-bound tail runs on every rank alike.
+static ScRounds one_instance(Ctx& ctx, dev::ScKind kind, u256* const* tables, int nt, size_t num_rounds, bool sharded) {
+  const bool sh = sharded && ctx.shard_world() > 1;
+  dev::ScInst inst;
+  for (int t = 0; t < 4; t++) inst.t[t] = t < nt ? tables[t] : nullptr;
+  inst.c_out = inst.t[2];
+  inst.write_c = 1;
+  return ScRounds{ctx, kind, {inst}, ((size_t)1 << num_rounds) / (sh ? ctx.shard_world() : 1), sh, ctx.small.p + layout::SMALL_ROUND.off};
 }
 
 // ================================================================================================ polynomial commitment / evaluation proof
@@ -755,77 +746,7 @@ hge RowSum::collect() {
   return hge_add(to_hge(p[0]), to_hge(p[1]));
 }
 
-// BulletReductionProof::prove (nizk/bullet.rs:32-132) with Q = r*G1 and H = h folded into host fixed-base terms, and the
-// generator vector left unfolded (DESIGN.md "IPA without folding G").  d_a / d_b are consumed (folded in place).
-static void bullet_prove(Ctx& ctx, Transcript& T, const PolyCommitmentGens& gens, const std::function<Fq()>& get_r_scale, u256* d_a, u256* d_b, size_t n,
-                         const Fq& blind, const std::vector<std::pair<Fq, Fq>>& blinds_vec, BulletReductionProof& proof, Fq& a_hat, Fq& b_hat, hge& g_hat,
-                         Fq& blind_final) {
-  const GenSet& gs = *gens.gens_n.set;
-  const size_t rounds = blinds_vec.size();
-  DevBuf<u256> svec(n), lr(2 * n), d_bl(2 * rounds + 1);
-  DevBuf<ge> pts(2), d_bh(2 * rounds + 1);
-  dev::fill_one(svec.p, n, ctx.stream);
-  ctx.ensure_scratch(dev::msm_scratch_bytes(2 * rounds + 2, n) + 64);
-  // blind_L[k]*H and blind_R[k]*H depend on the tape only: one batched launch up front (rows with no generator terms, just the blind)
-  std::vector<ge> bh(2 * rounds);
-  if (rounds) {
-    std::vector<Fq> bl(2 * rounds);
-    for (size_t k = 0; k < rounds; k++) { bl[2 * k] = blinds_vec[k].first; bl[2 * k + 1] = blinds_vec[k].second; }
-    dev::h2d(d_bl.p, bl.data(), bl.size() * sizeof(u256), ctx.stream);
-    dev::msm_rows(d_bh.p, gs.table.p, gs.wbits, gs.rows(), lr.p, 0, 2 * rounds, 0, d_bl.p, gens.gens_n.h, ctx.scratch.p, ctx.stream);
-    dev::d2h(bh.data(), d_bh.p, bh.size() * sizeof(ge), ctx.stream);   // pageable target: completes before the call returns
-  }
-  IpaRound rd{ctx, gs, d_a, d_b, svec.p, n, pts.p};
-  blind_final = blind;
-  Fq r_scale = Fq::zero();
-  size_t cur = n, k = 0;
-  while (cur != 1) {
-    FineTimer f1(ctx, "ipa launch");
-    rd.launch(cur);
-    f1.stop();
-    // the transcript work that precedes the first round (absorbing a_vec, deriving r) runs while the device computes round 0
-    if (k == 0) r_scale = get_r_scale();
-    FineTimer f2(ctx, "ipa wait c");
-    Fq c_L, c_R;
-    rd.wait_c(c_L, c_R);
-    f2.stop();
-    FineTimer f3(ctx, "ipa host c*Q (overlaps MSM)");
-    // + c_L*Q + blind_L*H with Q = r*G1 (nizk/mod.rs:479-480), H = gens_n.h   (bullet.rs:83-97)
-    Term tl[1] = {{gens.gens_1.off, c_L * r_scale}};
-    Term tr[1] = {{gens.gens_1.off, c_R * r_scale}};
-    hge hl = hge_add(host_commit(gs, tl, 1), to_hge(bh[2 * k]));
-    hge hr = hge_add(host_commit(gs, tr, 1), to_hge(bh[2 * k + 1]));
-    f3.stop();
-    FineTimer f4(ctx, "ipa wait MSM");
-    ge Lg, Rg;
-    rd.wait_LR(Lg, Rg);
-    f4.stop();
-    FineTimer f5(ctx, "ipa host compress+transcript");
-    Cp Lc, Rc;
-    compress2(hge_add(to_hge(Lg), hl), hge_add(to_hge(Rg), hr), Lc, Rc);
-    T.append_point("L", Lc.b);
-    T.append_point("R", Rc.b);
-    Fq u = T.challenge_scalar("u");
-    Fq u_inv = u.inv();
-    f5.stop();
-    rd.fold(cur, u, u_inv);
-    blind_final = blind_final + blinds_vec[k].first * u * u + blinds_vec[k].second * u_inv * u_inv;  // bullet.rs:111
-    proof.L_vec.push_back(Lc);
-    proof.R_vec.push_back(Rc);
-    cur /= 2;
-    k++;
-  }
-  if (k == 0) r_scale = get_r_scale();
-  // g_hat = G_final[0] = <s, G>
-  FineTimer f6(ctx, "ipa final");
-  uint8_t* stage = ctx.pinned + layout::PIN_STAGE.off;
-  dev::d2h(stage, d_a, 32, ctx.stream);
-  dev::d2h(stage + 32, d_b, 32, ctx.stream);
-  g_hat = RowSum(ctx, gs, svec.p, n).collect();
-  ctx.sync();   // a_hat, b_hat
-  memcpy(&a_hat, stage, 32); memcpy(&b_hat, stage + 32, 32);
-}
-
+// ================================================================================================ DotProductProofLog
 // the tape draws of DotProductProofLog::prove (nizk/mod.rs:452-467), in the reference's order
 struct DotLogTape { Fq d, r_delta, r_beta; std::vector<std::pair<Fq, Fq>> blinds_vec; };
 static DotLogTape dotlog_tape(RandomTape& tape, size_t n) {
@@ -838,8 +759,8 @@ static DotLogTape dotlog_tape(RandomTape& tape, size_t n) {
   for (size_t i = 0; i < lg_n; i++) t.blinds_vec.push_back({v1[i], v2[i]});
   return t;
 }
-// DotProductProofLog::prove after the reduction (nizk/mod.rs:491-524), for both generator layouts: g1 = gens_1 (G_1 and h), the reduction's
-// x_hat, a_hat, g_hat and the final blind rhat_Gamma (blind_y's share included)
+// DotProductProofLog::prove after the reduction (nizk/mod.rs:491-524): g1 = gens_1 (G_1 and h), the reduction's x_hat, a_hat, g_hat and the
+// final blind rhat_Gamma (blind_y's share included)
 static void dotlog_finish(Transcript& T, const CommitKey& g1, const DotLogTape& t, const Fq& r, const Fq& x_hat, const Fq& a_hat, const hge& g_hat,
                           const Fq& rhat_Gamma, DotProductProofLog& proof) {
   Fq y_hat = x_hat * a_hat;
@@ -855,37 +776,123 @@ static void dotlog_finish(Transcript& T, const CommitKey& g1, const DotLogTape& 
   proof.z2 = a_hat * (c * rhat_Gamma + t.r_beta) + t.r_delta;
 }
 
-// DotProductProofLog::prove (nizk/mod.rs:440-525).  d_x: device x_vec (n, consumed); a_vec on the host (it is absorbed by the transcript).
-// d_x: device x_vec (n, consumed); d_avec: device a_vec (n, consumed); a_canon: the canonical bytes of a_vec, which the transcript absorbs
-static void dotproduct_log_prove(Ctx& ctx, const PolyCommitmentGens& gens, Transcript& T, RandomTape& tape, u256* d_x, const Fq& blind_x,
-                                 u256* d_avec, const std::vector<uint8_t>& a_canon, const Fq& y, const Fq& blind_y, DotProductProofLog& proof, Cp& Cy_out,
-                                 Cp* Cx_out = nullptr) {
+// DotProductProofLog::prove (nizk/mod.rs:440-525) with BulletReductionProof::prove (nizk/bullet.rs:32-132) inlined, Q = r*G_1 and H = h folded into
+// host fixed-base terms.  `dv` is the device side of one generator layout (DotLogTable, DotLogFold): it holds x and a (n each, folded in place) and
+// runs commit_x, the rounds' setup, each round's launch / wait_c / wait_LR / add_blinds / fold, and finish.  a_canon: the canonical bytes of a, which
+// the transcript absorbs while the device computes round 0 (same transcript order as nizk/mod.rs:475-477).
+template <class Dev>
+static void dotlog_body(Ctx& ctx, Dev& dv, const CommitKey& g1, Transcript& T, RandomTape& tape, const Fq& blind_x, const std::vector<uint8_t>& a_canon,
+                        const Fq& y, const Fq& blind_y, DotProductProofLog& proof, Cp& Cx, Cp& Cy) {
+  const size_t n = dv.n;
   T.append_protocol_name("dot product proof (log)");
-  FineTimer f0(ctx, "dotlog pre-ipa");
-  size_t n = a_canon.size() / 32;
-  if (gens.n != n) throw std::runtime_error("spartan_b200: DotProductProofLog size mismatch");
   const DotLogTape t = dotlog_tape(tape, n);
-  std::vector<Cp> cx;
-  commit_rows_and_compress(ctx, gens.gens_n, d_x, n, 1, n, &blind_x, cx);
-  T.append_point("Cx", cx[0].b);
-  if (Cx_out) *Cx_out = cx[0];
-  Cy_out = compress(commit1(gens.gens_1, y, blind_y));
-  T.append_point("Cy", Cy_out.b);
+  FineTimer f0(ctx, "dotlog Cx");
+  Cx = dv.commit_x(blind_x);
+  f0.stop();
+  T.append_point("Cx", Cx.b);
+  Cy = compress(commit1(g1, y, blind_y));
+  T.append_point("Cy", Cy.b);
   Fq r = Fq::zero();
-  auto absorb_a = [&]() {   // called by bullet_prove once round 0 is in flight on the device (same transcript order as nizk/mod.rs:475-477)
+  auto absorb_a = [&]() {
+    FineTimer fa(ctx, "dotlog absorb a");
     T.append_scalar_bytes("a", a_canon.data(), n);
     r = T.challenge_scalar("r");
-    return r;
   };
-  Fq x_hat, a_hat, rhat_Gamma;
+  FineTimer fr(ctx, "dotlog rounds");
+  dv.setup(t.blinds_vec);
+  // blind_Gamma = blind_x + r*blind_y enters the reduction only through the final blind, which is linear in it: start from blind_x, add r*blind_y after
+  Fq blind_final = blind_x;
+  BulletReductionProof& bullet = proof.bullet_reduction_proof;
+  size_t k = 0;
+  for (size_t m = n / 2; m >= 1; m /= 2, k++) {
+    FineTimer f1(ctx, "dotlog round launch");
+    dv.launch(m);
+    f1.stop();
+    if (k == 0) absorb_a();
+    Fq c_L, c_R;
+    ge Lg, Rg;
+    FineTimer f2(ctx, "dotlog round wait");
+    dv.wait_c(c_L, c_R);
+    f2.stop();
+    FineTimer f3(ctx, "dotlog round host");
+    // + c_L*Q + blind_L*H with Q = r*G_1 (nizk/mod.rs:479-480), H = h   (bullet.rs:83-97), while the
+    // table layout's MSM still computes L', R' (its wait counts as host time here)
+    const Term tl[1] = {{g1.off, c_L * r}}, tr[1] = {{g1.off, c_R * r}};
+    hge hl = host_commit(*g1.set, tl, 1), hr = host_commit(*g1.set, tr, 1);
+    dv.add_blinds(k, hl, hr);
+    dv.wait_LR(Lg, Rg);
+    Cp Lc, Rc;
+    compress2(hge_add(to_hge(Lg), hl), hge_add(to_hge(Rg), hr), Lc, Rc);
+    T.append_point("L", Lc.b);
+    T.append_point("R", Rc.b);
+    const Fq u = T.challenge_scalar("u"), u_inv = u.inv();
+    f3.stop();
+    dv.fold(m, u, u_inv);   // bullet.rs:105-108
+    blind_final = blind_final + t.blinds_vec[k].first * u * u + t.blinds_vec[k].second * u_inv * u_inv;  // bullet.rs:111
+    bullet.L_vec.push_back(Lc);
+    bullet.R_vec.push_back(Rc);
+  }
+  if (k == 0) absorb_a();
+  Fq x_hat, a_hat;
   hge g_hat;
-  f0.stop();
-  // blind_Gamma = blind_x + r*blind_y enters the reduction only through the final blind, which is linear in it: pass blind_x and add r*blind_y after
-  bullet_prove(ctx, T, gens, absorb_a, d_x, d_avec, n, blind_x, t.blinds_vec, proof.bullet_reduction_proof, x_hat, a_hat, g_hat, rhat_Gamma);
-  rhat_Gamma = rhat_Gamma + r * blind_y;
-  FineTimer f6(ctx, "dotlog post-ipa");
-  dotlog_finish(T, gens.gens_1, t, r, x_hat, a_hat, g_hat, rhat_Gamma, proof);
+  dv.finish(x_hat, a_hat, g_hat);
+  fr.stop();
+  dotlog_finish(T, g1, t, r, x_hat, a_hat, g_hat, blind_final + r * blind_y, proof);
 }
+
+// The table layout (PolyEvalProof's gens, and DotLogGens up to SP_DOTLOG_TABLE_MAX_N): Cx through commit_rows_and_compress's one-row path, the
+// rounds through IpaRound over the unfolded generators and their n running scalars svec (DESIGN.md "IPA without folding G"), every round's
+// blind_L*H and blind_R*H in one batched launch up front, and g_hat = <svec, G> at the end.  x, a: device x_vec and a_vec (n each, consumed).
+struct DotLogTable {
+  Ctx& ctx;
+  const PolyCommitmentGens& gens;
+  u256 *x, *a;
+  size_t n;
+  DevBuf<u256> svec, lr, d_bl;
+  DevBuf<ge> pts, d_bh;
+  std::vector<ge> bh;   // blind_L[k]*H, blind_R[k]*H
+  IpaRound rd;
+  DotLogTable(Ctx& c, const PolyCommitmentGens& g, u256* x_, u256* a_, size_t n_)
+      : ctx(c), gens(g), x(x_), a(a_), n(n_), rd{c, *g.gens_n.set, x_, a_, nullptr, n_, nullptr} {
+    if (gens.n != n) throw std::runtime_error("spartan_b200: DotProductProofLog size mismatch");
+  }
+  Cp commit_x(const Fq& blind_x) {
+    std::vector<Cp> cx;
+    return commit_rows_and_compress(ctx, gens.gens_n, x, n, 1, n, &blind_x, cx);
+  }
+  void setup(const std::vector<std::pair<Fq, Fq>>& blinds_vec) {
+    const GenSet& gs = *gens.gens_n.set;
+    const size_t rounds = blinds_vec.size();
+    svec.alloc(n); lr.alloc(2 * n); d_bl.alloc(2 * rounds + 1);
+    pts.alloc(2); d_bh.alloc(2 * rounds + 1);
+    dev::fill_one(svec.p, n, ctx.stream);
+    ctx.ensure_scratch(dev::msm_scratch_bytes(2 * rounds + 2, n) + 64);
+    // the blind terms depend on the tape only: rows with no generator terms, just the blind
+    bh.resize(2 * rounds);
+    if (rounds) {
+      std::vector<Fq> bl(2 * rounds);
+      for (size_t k = 0; k < rounds; k++) { bl[2 * k] = blinds_vec[k].first; bl[2 * k + 1] = blinds_vec[k].second; }
+      dev::h2d(d_bl.p, bl.data(), bl.size() * sizeof(u256), ctx.stream);
+      dev::msm_rows(d_bh.p, gs.table.p, gs.wbits, gs.rows(), lr.p, 0, 2 * rounds, 0, d_bl.p, gens.gens_n.h, ctx.scratch.p, ctx.stream);
+      dev::d2h(bh.data(), d_bh.p, bh.size() * sizeof(ge), ctx.stream);   // pageable target: completes before the call returns
+    }
+    rd.svec = svec.p;
+    rd.pts = pts.p;
+  }
+  void launch(size_t m) { rd.launch(2 * m); }
+  void wait_c(Fq& c_L, Fq& c_R) { rd.wait_c(c_L, c_R); }
+  void wait_LR(ge& L, ge& R) { rd.wait_LR(L, R); }
+  void add_blinds(size_t k, hge& hl, hge& hr) { hl = hge_add(hl, to_hge(bh[2 * k])); hr = hge_add(hr, to_hge(bh[2 * k + 1])); }
+  void fold(size_t m, const Fq& u, const Fq& u_inv) { rd.fold(2 * m, u, u_inv); }
+  void finish(Fq& x_hat, Fq& a_hat, hge& g_hat) {   // g_hat = G_final[0] = <s, G>
+    uint8_t* stage = ctx.pinned + layout::PIN_STAGE.off;
+    dev::d2h(stage, x, 32, ctx.stream);
+    dev::d2h(stage + 32, a, 32, ctx.stream);
+    g_hat = RowSum(ctx, *gens.gens_n.set, svec.p, n).collect();
+    ctx.sync();   // x_hat, a_hat
+    memcpy(&x_hat, stage, 32); memcpy(&a_hat, stage + 32, 32);
+  }
+};
 
 // ================================================================================================ DotProductProofLog of the caller's vectors
 DotLogGens::DotLogGens(Ctx& c, size_t n_, const std::string& label) : ctx(&c), n(n_) {
@@ -927,45 +934,57 @@ hge msm_var_host(Ctx& ctx, const ge_niels* pts, const u256* scalars, size_t n) {
   return to_hge(g);
 }
 
-// BulletReductionProof::prove (nizk/bullet.rs:32-132) over generators folded on the device (the folding path of sp_dotlog_*), with Q = r*G_1 and H = h
-// folded into host fixed-base terms.  The folded vector is kept as G_k = c_k * H_k: a round folds H' = H_L + u^2 H_R (dev::dotlog_fold) and
-// c' = c * u^-1, and its MSMs take the scalars c * a.  Halves of at most DOTLOG_SEG_MAX_HALF terms run both MSMs as one segmented launch over
-// extended points; longer halves run the bucket MSM over niels points.  d_a / d_b are consumed (folded in place).
-static void bullet_fold_prove(Ctx& ctx, Transcript& T, const DotLogGens& gens, const std::function<Fq()>& get_r_scale, u256* d_a, u256* d_b, size_t n,
-                              const Fq& blind, const std::vector<std::pair<Fq, Fq>>& blinds_vec, BulletReductionProof& proof, Fq& a_hat, Fq& b_hat,
-                              hge& g_hat, Fq& blind_final) {
-  const CommitKey& g1 = gens.g.gens_1;
-  const size_t S = DOTLOG_SEG_MAX_HALF;
-  cudaStream_t s = ctx.stream;
+// The folding layout (DotLogGens above SP_DOTLOG_TABLE_MAX_N): Cx is one bucket MSM over G[0..n).  The folded vector is kept as G_k = c_k * H_k:
+// a round folds H' = H_L + u^2 H_R (dev::dotlog_fold) and c' = c * u^-1, and its MSMs take the scalars c * x.  Halves of at most
+// DOTLOG_SEG_MAX_HALF terms run both MSMs as one segmented launch over extended points; longer halves run the bucket MSM over niels points.  The
+// blind terms are host fixed-base terms against h, and g_hat = c * H_final[0].  x, a: device x_vec and a_vec (n each, consumed).
+struct DotLogFold {
+  Ctx& ctx;
+  const DotLogGens& gens;
+  u256 *x, *a;
+  size_t n;
+  const std::vector<std::pair<Fq, Fq>>* blinds = nullptr;
   // folded points: niels while the next round's halves take the bucket MSM (n/2 of them at most), extended from there on (and G itself when
   // round 0 already takes the segmented MSM)
   DevBuf<ge_niels> hn;
-  if (n / 2 > 2 * S) hn.alloc(n / 2);
-  DevBuf<ge> hg(std::min(n, 2 * S)), pts(2), seg_tmp(std::min(n, 2 * S));
-  DevBuf<u256> w(n);
-  size_t scratch_bytes = 0;
-  std::vector<uint32_t> seg;   // {0, m, 2m} of every segmented round
-  for (size_t m = n / 2; m >= 1; m /= 2)
-    if (m > S) scratch_bytes = std::max(scratch_bytes, dev::pip_scratch_bytes(dev::pip_plan(m, 0)));
-    else seg.insert(seg.end(), {0u, (uint32_t)m, (uint32_t)(2 * m)});
-  DevBuf<uint8_t> scratch(std::max<size_t>(scratch_bytes, 1));
-  DevBuf<uint32_t> d_seg(std::max<size_t>(seg.size(), 1));
-  dev::h2d(d_seg.p, seg.data(), seg.size() * sizeof(uint32_t), s);
-  const void* cur = gens.pts.p;
+  DevBuf<ge> hg, pts, seg_tmp;
+  DevBuf<u256> w;
+  DevBuf<uint8_t> scratch;
+  DevBuf<uint32_t> d_seg;   // {0, m, 2m} of every segmented round
+  const void* cur = nullptr;
   int fmt = dev::FOLD_NIELS;
-  if (n / 2 <= S) { dev::niels_to_ge(hg.p, gens.pts.p, n, s); cur = hg.p; fmt = dev::FOLD_GE; }
-  u256* c_dev = ctx.small.p + layout::SMALL_IPA_C.off;
-  uint8_t* stage = ctx.pinned + layout::PIN_STAGE.off;
-  blind_final = blind;
-  Fq c = Fq::one(), r_scale = Fq::zero();
-  size_t k = 0, seg_at = 0;
-  for (size_t m = n / 2; m >= 1; m /= 2, k++) {
-    FineTimer f1(ctx, "dotlog round launch");
-    dev::dot(c_dev, d_a, d_b + m, m, ctx.red.p, s);       // c_L = <a_L, b_R>
-    dev::dot(c_dev + 1, d_a + m, d_b, m, ctx.red.p, s);   // c_R = <a_R, b_L>
-    const bool segmented = m <= S;
-    dev::dotlog_scalars(w.p, d_a, m, c.m, segmented, s);   // [c a_R | c a_L]
-    if (segmented) {   // pts[0] = c <a_R, H_L> = R', pts[1] = c <a_L, H_R> = L'
+  Fq c = Fq::one();
+  size_t seg_at = 0;
+  uint8_t* stage() const { return ctx.pinned + layout::PIN_STAGE.off; }
+  Cp commit_x(const Fq& blind_x) {
+    const Term tb[1] = {{gens.g.gens_1.h, blind_x}};
+    return compress(hge_add(msm_var_host(ctx, gens.pts.p, x, n), host_commit(*gens.g.gens_1.set, tb, 1)));
+  }
+  void setup(const std::vector<std::pair<Fq, Fq>>& blinds_vec) {
+    const size_t S = DOTLOG_SEG_MAX_HALF;
+    blinds = &blinds_vec;
+    if (n / 2 > 2 * S) hn.alloc(n / 2);
+    hg.alloc(std::min(n, 2 * S)); pts.alloc(2); seg_tmp.alloc(std::min(n, 2 * S));
+    w.alloc(n);
+    size_t scratch_bytes = 0;
+    std::vector<uint32_t> seg;
+    for (size_t m = n / 2; m >= 1; m /= 2)
+      if (m > S) scratch_bytes = std::max(scratch_bytes, dev::pip_scratch_bytes(dev::pip_plan(m, 0)));
+      else seg.insert(seg.end(), {0u, (uint32_t)m, (uint32_t)(2 * m)});
+    scratch.alloc(std::max<size_t>(scratch_bytes, 1));
+    d_seg.alloc(std::max<size_t>(seg.size(), 1));
+    dev::h2d(d_seg.p, seg.data(), seg.size() * sizeof(uint32_t), ctx.stream);
+    cur = gens.pts.p;
+    if (n / 2 <= S) { dev::niels_to_ge(hg.p, gens.pts.p, n, ctx.stream); cur = hg.p; fmt = dev::FOLD_GE; }
+  }
+  void launch(size_t m) {
+    cudaStream_t s = ctx.stream;
+    u256* c_dev = ctx.small.p + layout::SMALL_IPA_C.off;
+    dev::dot(c_dev, x, a + m, m, ctx.red.p, s);       // c_L = <x_L, a_R>
+    dev::dot(c_dev + 1, x + m, a, m, ctx.red.p, s);   // c_R = <x_R, a_L>
+    const bool segmented = m <= DOTLOG_SEG_MAX_HALF;
+    dev::dotlog_scalars(w.p, x, m, c.m, segmented, s);   // [c x_R | c x_L]
+    if (segmented) {   // pts[0] = c <x_R, H_L> = R', pts[1] = c <x_L, H_R> = L'
       dev::msm_var_segmented(pts.p, static_cast<const ge*>(cur), w.p, d_seg.p + seg_at, 2, 2 * m, seg_tmp.p, s);
       seg_at += 3;
     } else {
@@ -974,50 +993,38 @@ static void bullet_fold_prove(Ctx& ctx, Transcript& T, const DotLogGens& gens, c
       dev::msm_var(pts.p, H, w.p, plan, scratch.p, s);
       dev::msm_var(pts.p + 1, H + m, w.p + m, plan, scratch.p, s);
     }
-    dev::d2h(stage, c_dev, 2 * sizeof(u256), s);
-    dev::d2h(stage + 2 * sizeof(u256), pts.p, 2 * sizeof(ge), s);
-    f1.stop();
-    if (k == 0) {   // the transcript work that precedes the first round (absorbing a, deriving r) runs while the device computes round 0
-      FineTimer fa(ctx, "dotlog absorb a");
-      r_scale = get_r_scale();
-    }
-    FineTimer f2(ctx, "dotlog round wait");
+    dev::d2h(stage(), c_dev, 2 * sizeof(u256), s);
+    dev::d2h(stage() + 2 * sizeof(u256), pts.p, 2 * sizeof(ge), s);
+  }
+  void wait_c(Fq& c_L, Fq& c_R) {   // c_L, c_R, R', L' arrive together
     ctx.sync();
-    f2.stop();
-    FineTimer f3(ctx, "dotlog round host");
-    Fq c_L, c_R;
-    ge Rg, Lg;
-    memcpy(&c_L, stage, 32); memcpy(&c_R, stage + 32, 32);
-    memcpy(&Rg, stage + 64, sizeof(ge)); memcpy(&Lg, stage + 64 + sizeof(ge), sizeof(ge));
-    // + c_L*Q + blind_L*H with Q = r*G_1 (nizk/mod.rs:479-480), H = h   (bullet.rs:83-97)
-    const Term tl[2] = {{g1.off, c_L * r_scale}, {g1.h, blinds_vec[k].first}};
-    const Term tr[2] = {{g1.off, c_R * r_scale}, {g1.h, blinds_vec[k].second}};
-    Cp Lc, Rc;
-    compress2(hge_add(to_hge(Lg), host_commit(*g1.set, tl, 2)), hge_add(to_hge(Rg), host_commit(*g1.set, tr, 2)), Lc, Rc);
-    T.append_point("L", Lc.b);
-    T.append_point("R", Rc.b);
-    const Fq u = T.challenge_scalar("u"), u_inv = u.inv();
-    f3.stop();
-    dev::ipa_fold_update(d_a, d_b, nullptr, m, 2 * m, u.m, u_inv.m, s);   // bullet.rs:106-107
-    const int out_fmt = m > 2 * S ? dev::FOLD_NIELS : dev::FOLD_GE;
+    memcpy(&c_L, stage(), 32); memcpy(&c_R, stage() + 32, 32);
+  }
+  void wait_LR(ge& L, ge& R) { memcpy(&R, stage() + 64, sizeof(ge)); memcpy(&L, stage() + 64 + sizeof(ge), sizeof(ge)); }
+  void add_blinds(size_t k, hge& hl, hge& hr) {
+    const CommitKey& g1 = gens.g.gens_1;
+    host_fixed_mul_acc(hl, g1.set->tab(g1.h), (*blinds)[k].first);
+    host_fixed_mul_acc(hr, g1.set->tab(g1.h), (*blinds)[k].second);
+  }
+  void fold(size_t m, const Fq& u, const Fq& u_inv) {
+    dev::ipa_fold_update(x, a, nullptr, m, 2 * m, u.m, u_inv.m, ctx.stream);   // bullet.rs:106-107
+    const int out_fmt = m > 2 * DOTLOG_SEG_MAX_HALF ? dev::FOLD_NIELS : dev::FOLD_GE;
     void* out = out_fmt == dev::FOLD_NIELS ? static_cast<void*>(hn.p) : static_cast<void*>(hg.p);
-    dev::dotlog_fold(out, out_fmt, cur, fmt, m, (u * u).canonical(), s);   // bullet.rs:108 over H
+    dev::dotlog_fold(out, out_fmt, cur, fmt, m, (u * u).canonical(), ctx.stream);   // bullet.rs:108 over H
     cur = out;
     fmt = out_fmt;
     c = c * u_inv;
-    blind_final = blind_final + blinds_vec[k].first * u * u + blinds_vec[k].second * u_inv * u_inv;  // bullet.rs:111
-    proof.L_vec.push_back(Lc);
-    proof.R_vec.push_back(Rc);
   }
-  // g_hat = G_final[0] = c * H_final[0]
-  dev::d2h(stage, d_a, 32, s);
-  dev::d2h(stage + 32, d_b, 32, s);
-  dev::d2h(stage + 64, cur, sizeof(ge), s);
-  ctx.sync();
-  ge h0;
-  memcpy(&a_hat, stage, 32); memcpy(&b_hat, stage + 32, 32); memcpy(&h0, stage + 64, sizeof(ge));
-  g_hat = hge_scalarmul(c.canonical(), to_hge(h0));
-}
+  void finish(Fq& x_hat, Fq& a_hat, hge& g_hat) {   // g_hat = G_final[0] = c * H_final[0]
+    dev::d2h(stage(), x, 32, ctx.stream);
+    dev::d2h(stage() + 32, a, 32, ctx.stream);
+    dev::d2h(stage() + 64, cur, sizeof(ge), ctx.stream);
+    ctx.sync();
+    ge h0;
+    memcpy(&x_hat, stage(), 32); memcpy(&a_hat, stage() + 32, 32); memcpy(&h0, stage() + 64, sizeof(ge));
+    g_hat = hge_scalarmul(c.canonical(), to_hge(h0));
+  }
+};
 
 void dotlog_prove(Ctx& ctx, const DotLogGens& gens, Transcript& T, RandomTape& tape, const u256* d_x, const Fq& blind_x, const u256* d_a, const Fq* y,
                   const Fq& blind_y, DotProductProofLog& proof, Cp& Cx, Cp& Cy, Fq& y_used) {
@@ -1031,33 +1038,13 @@ void dotlog_prove(Ctx& ctx, const DotLogGens& gens, Transcript& T, RandomTape& t
     ctx.get_small(layout::SMALL_DOT.off, &y_used, 1);
   }
   const std::vector<uint8_t> a_canon = canonical_bytes(ctx, a.p, n);
-  if (!gens.folding()) {
-    dotproduct_log_prove(ctx, gens.g, T, tape, x.p, blind_x, a.p, a_canon, y_used, blind_y, proof, Cy, &Cx);
-    return;
+  if (gens.folding()) {
+    DotLogFold dv{ctx, gens, x.p, a.p, n};
+    dotlog_body(ctx, dv, gens.g.gens_1, T, tape, blind_x, a_canon, y_used, blind_y, proof, Cx, Cy);
+  } else {
+    DotLogTable dv(ctx, gens.g, x.p, a.p, n);
+    dotlog_body(ctx, dv, gens.g.gens_1, T, tape, blind_x, a_canon, y_used, blind_y, proof, Cx, Cy);
   }
-  const CommitKey& g1 = gens.g.gens_1;
-  T.append_protocol_name("dot product proof (log)");
-  const DotLogTape t = dotlog_tape(tape, n);
-  FineTimer f0(ctx, "dotlog Cx");
-  const Term tb[1] = {{g1.h, blind_x}};
-  Cx = compress(hge_add(msm_var_host(ctx, gens.pts.p, x.p, n), host_commit(*g1.set, tb, 1)));
-  f0.stop();
-  T.append_point("Cx", Cx.b);
-  Cy = compress(commit1(g1, y_used, blind_y));
-  T.append_point("Cy", Cy.b);
-  Fq r = Fq::zero();
-  auto absorb_a = [&]() {   // nizk/mod.rs:475-477
-    T.append_scalar_bytes("a", a_canon.data(), n);
-    r = T.challenge_scalar("r");
-    return r;
-  };
-  Fq x_hat, a_hat, rhat_Gamma;
-  hge g_hat;
-  FineTimer f1(ctx, "dotlog rounds");
-  bullet_fold_prove(ctx, T, gens, absorb_a, x.p, a.p, n, blind_x, t.blinds_vec, proof.bullet_reduction_proof, x_hat, a_hat, g_hat, rhat_Gamma);
-  f1.stop();
-  rhat_Gamma = rhat_Gamma + r * blind_y;
-  dotlog_finish(T, g1, t, r, x_hat, a_hat, g_hat, rhat_Gamma, proof);
 }
 
 // PolyEvalProof::prove (dense_mlpoly.rs:312-365).  d_Z: device table of 2^|r| scalars (read-only).
@@ -1091,7 +1078,9 @@ void polyeval_prove(Ctx& ctx, const u256* d_Z, const std::vector<Fq>* blinds_opt
   ctx.sync();
   Fq blind_Zr = blind_Zr_opt ? *blind_Zr_opt : Fq::zero();
   fp.stop();
-  dotproduct_log_prove(ctx, gens, T, tape, d_LZ.p, LZ_blind, d_R.p, a_canon, Zr_used, blind_Zr, proof.proof, C_Zr);
+  DotLogTable dv(ctx, gens, d_LZ.p, d_R.p, R_size);
+  Cp Cx;
+  dotlog_body(ctx, dv, gens.gens_1, T, tape, LZ_blind, a_canon, Zr_used, blind_Zr, proof.proof, Cx, C_Zr);
 }
 
 // ================================================================================================ the caller's tables (sp_pc_*)
@@ -1195,8 +1184,9 @@ void pc_eval_prove_joint(Ctx& ctx, const PolyCommitmentGens& gens, const u256* c
   std::vector<uint8_t> a_canon(32 * RJ);
   dev::d2h(a_canon.data(), d_Rc.p, 32 * RJ, ctx.stream);
   ctx.sync();
-  Cp C_Zr;
-  dotproduct_log_prove(ctx, gens, T, tape, d_LZ.p, LZ_blind, d_R.p, a_canon, joint, Fq::zero(), proof.proof, C_Zr);
+  DotLogTable dv(ctx, gens, d_LZ.p, d_R.p, RJ);
+  Cp Cx, C_Zr;
+  dotlog_body(ctx, dv, gens.gens_1, T, tape, LZ_blind, a_canon, joint, Fq::zero(), proof.proof, Cx, C_Zr);
 }
 
 // ================================================================================================ instance
@@ -1280,8 +1270,8 @@ void r1cs_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::v
   {
     PhaseTimer t(ctx, "polycommit");
     // dense_mlpoly.rs:193-196; the blinds are the tape's first draw and are made while the rows' MSM already runs
-    // (phase one's tape-only commitments are not queued here as well — ZkPre::enqueue behind the rows' MSM: their small kernels would
-    //  lengthen this commitment's chain by what they save phase one, whose rounds are host-bound anyway)
+    // (phase one's tape-only commitments are not queued behind the rows' MSM: their small kernels would lengthen this commitment's chain by
+    //  what they save phase one, whose rounds are host-bound anyway)
     commit_rows_and_compress(ctx, gens.gens_pc.gens_n, d_vars, R_size, L_size, R_size, nullptr, proof.comm_vars.C,
                              [&]() { blinds_vars = tape.random_vector("poly_blinds", L_size); return blinds_vars.data(); });
     append_poly_commitment(T, "poly_commitment", proof.comm_vars);
@@ -1319,8 +1309,9 @@ void r1cs_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::v
       for (int m = 0; m < 3; m++) dev::spmv(outs[m], num_cons, inst.M[m].csr_ptr.p, inst.M[m].csr_idx.p, inst.M[m].csr_val.p, d_z.p, ctx.stream);
     }
     u256* tabs[4] = {d_tau.p, d_Az.p, d_Bz.p, d_Cz.p};
-    zk_sumcheck_prove(ctx, dev::SC_CUBIC4, Fq::zero(), Fq::zero(), num_rounds_x, tabs, 4, gens.gens_1, gens.gens_4, T, tape, proof.sc_proof_phase1, rx, claims1,
-                      blind_claim_postsc1, sh1);
+    ScRounds sc = one_instance(ctx, dev::SC_CUBIC4, tabs, 4, num_rounds_x, sh1);
+    zk_sumcheck_prove(ctx, sc, 3, Fq::zero(), Fq::zero(), num_rounds_x, gens.gens_1, gens.gens_4, T, tape, proof.sc_proof_phase1, rx, claims1,
+                      blind_claim_postsc1);
   }
   if (hooks && hooks->on_rx) hooks->on_rx(rx);
   const Fq tau_claim = claims1[0], Az_claim = claims1[1], Bz_claim = claims1[2], Cz_claim = claims1[3];
@@ -1356,8 +1347,9 @@ void r1cs_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::v
     dev::lincomb3(d_ABC.p, eA.p, eB.p, eC.p, d_chal.p + 32, n2, ctx.stream);
     if (sh2) { d_zloc.alloc(n2); dev::take_cyclic(d_zloc.p, d_z.p, n2, rk, W, ctx.stream); }
     u256* tabs[2] = {sh2 ? d_zloc.p : d_z.p, d_ABC.p};
-    zk_sumcheck_prove(ctx, dev::SC_QUAD, claim_phase2, blind_claim_phase2, num_rounds_y, tabs, 2, gens.gens_1, gens.gens_3, T, tape, proof.sc_proof_phase2, ry, claims2,
-                      blind_claim_postsc2, sh2);
+    ScRounds sc = one_instance(ctx, dev::SC_QUAD, tabs, 2, num_rounds_y, sh2);
+    zk_sumcheck_prove(ctx, sc, 2, claim_phase2, blind_claim_phase2, num_rounds_y, gens.gens_1, gens.gens_3, T, tape, proof.sc_proof_phase2, ry, claims2,
+                      blind_claim_postsc2);
   }
   if (hooks && hooks->on_ry) hooks->on_ry(ry);
   {

@@ -226,7 +226,7 @@ Cp commit_rows_and_compress(Ctx& ctx, const CommitKey& key, const u256* d_scalar
                             std::vector<Cp>& out, const std::function<const Fq*()>& blinds_late = nullptr);
 
 // The device side of one inner-product round (bullet.rs:74-111) over the unfolded generators of `gs` (DESIGN.md "IPA without folding G"), run by
-// bullet_prove and by the operator-level sp_ipa_*.  launch() computes c_L = <a_L, b_R>, c_R = <a_R, b_L> and L' = <a_L, G_R>, R' = <a_R, G_L> in one
+// DotProductProofLog's table layout (prover.cpp: DotLogTable) and by the operator-level sp_ipa_*.  launch() computes c_L = <a_L, b_R>, c_R = <a_R, b_L> and L' = <a_L, G_R>, R' = <a_R, G_L> in one
 // kernel that publishes the two pairs to the host through separate flag words, so the host can work on c*Q while the MSM still runs.
 // Scratch: >= ipa_msm_scratch_points(n, gs.wbits) points.
 struct IpaRound {
@@ -259,6 +259,7 @@ struct ScRounds {
   void fold_eval(const Fq& r, u256* host_bound = nullptr);  // bind with r, evaluate the next round (host_bound: dev::sc_fold_eval)
   void fold(const Fq& r);                                   // bind the owned tables with r only
   std::vector<Fq> wait();                                   // the 3 ninst evaluations of the last launch
+  std::vector<Fq> finals();                                 // t[k][0] of the first instance's tables t[0], t[1], .. (synchronises)
   dev::XRank xr();                                          // the cross-rank exchange of the next launch (none once replicated)
 };
 

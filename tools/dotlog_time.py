@@ -7,7 +7,7 @@ synchronise), median of --reps runs after one warm-up call of each.  The prove i
   rounds      the log2 n rounds, absorb a excluded (host wall clock: launches, waits and the host's group work)
   fold        the generator-fold kernel (dotlog_fold), summed over the rounds
   msm         the round MSMs and Cx's (msm_var and msm_var_segmented)
-The table path has no fold and its rounds run the inner-product kernel: its split lines are those of the folding path only where they apply.
+The table path has no fold kernel and runs its MSMs in the inner-product kernel (ipa_msm): its fold and msm lines stay 0.
 
     python tools/dotlog_time.py [--logn 8 9 12 16 20 24] [--reps 5] [--out file.json]
 
