@@ -539,6 +539,43 @@ int sp_spmat_multiply_vec(sp_ctx* ctx, const sp_spmat* mats, size_t num_rows, si
 int sp_spmat_eval_table(sp_ctx* ctx, const sp_spmat* mats, const sp_poly* e, size_t num_rows, size_t num_cols, const uint64_t* weights_mont /* b x 4 or NULL */,
                         sp_poly** outs /* b, or 1 with weights */);
 
+/* ---- R1CSProof of the caller's matrices: R1CSGens::new (src/r1csproof.rs:61-74), R1CSProof::prove (:144-349) and ::verify (:351-489) on the
+ * caller's transcript and tape, on this rank's GPU alone (a connected multi-GPU context does not shard these calls).  The proof is the one
+ * NIZK::prove and SNARK::prove embed; the verifier takes the three claimed evaluations (A(rx, ry), B(rx, ry), C(rx, ry)) instead of the matrices,
+ * so a caller can prove those with its own argument (sp_spark_*, or a closed form of structured matrices).
+ *
+ * num_cons >= 2 and num_vars >= 1 are powers of two (the padded sizes), log2 num_cons and log2 (2 num_vars) at most 32.  z = vars || 1 || inputs ||
+ * 0.. has 2 num_vars entries, and |inputs| + 1 <= num_vars (r1csproof.rs:156). */
+typedef struct sp_r1cs_gens sp_r1cs_gens;
+/* R1CSGens::new(label, num_cons, num_vars): gens_pc = PolyCommitmentGens::new(log2 num_vars, label) and the sumcheck gens gens_1 (= gens_pc's),
+ * gens_3 and gens_4, all prefixes of the label's one stream: max(2^ceil(log2(num_vars) / 2) + 2, 5) generators with the device tables and
+ * footprint of sp_pc_gens_create's set.  NIZKGens / SNARKGens use the label "gens_r1cs_sat". */
+int sp_r1cs_gens_create(sp_ctx* ctx, const uint8_t* label, size_t label_len, size_t num_cons, size_t num_vars, sp_r1cs_gens** out);
+/* the same gens as a view of an existing gens_r1cs_sat set: of generator tables, of NIZK gens or of SNARK gens.  No device memory is added; the
+ * view keeps the set alive.  SP_ERR_INVALID_ARG: a set shorter than num_vars needs, or of another context */
+int sp_r1cs_gens_create_from(sp_ctx* ctx, const struct sp_gen_tables* tables /* sp_gen_tables, below */, size_t num_cons, size_t num_vars, sp_r1cs_gens** out);
+int sp_r1cs_gens_create_from_nizk(sp_ctx* ctx, const sp_nizk_gens* gens, size_t num_cons, size_t num_vars, sp_r1cs_gens** out);
+int sp_r1cs_gens_create_from_snark(sp_ctx* ctx, const sp_snark_gens* gens, size_t num_cons, size_t num_vars, sp_r1cs_gens** out);
+void sp_r1cs_gens_free(sp_r1cs_gens* g);
+/* R1CSProof::prove(inst, vars, inputs, gens, transcript, random_tape): the matrices are exactly one of
+ *   inst   an instance of num_cons x num_vars (padded): its products run as NIZK::prove's, one thread per row or column (k_spmv), so one row or
+ *          column holding most entries costs seconds at 2^20 (DESIGN.md "Products of the caller's matrices");
+ *   spmat  an sp_spmat of exactly 3 matrices A, B, C of 2^log2(num_cons) rows and 2^log2(2 num_vars) columns: the tiled products of
+ *          sp_spmat_multiply_vec / sp_spmat_eval_table, whose time does not depend on how the entries spread over rows and columns.
+ * vars: num_vars entries, read only.  The transcript and the tape (sp_random_tape_new) advance as the reference's do, and are written back only
+ * on success.  *proof = bincode(R1CSProof), released with sp_free; rx_out: log2 num_cons scalars, ry_out: log2 (2 num_vars).
+ * SP_ERR_INVALID_ARG, with nothing launched and the states untouched: dimensions as above, |inputs| + 1 > num_vars, both or neither of inst and
+ * spmat, an instance of other dimensions, an spmat of another shape, vars of another length, gens for another num_vars, NULL arguments, handles
+ * of another context; SP_ERR_INVALID_SCALAR: inputs not reduced. */
+int sp_r1cs_prove_t(sp_ctx* ctx, const sp_instance* inst, const sp_spmat* spmat, size_t num_cons, size_t num_vars, const sp_poly* vars,
+                    const uint64_t* inputs_mont, size_t ninputs, const sp_r1cs_gens* gens, uint8_t* strobe_state /* in, out */,
+                    uint8_t* tape_state /* in, out */, uint8_t** proof, size_t* proof_len, uint64_t* rx_out, uint64_t* ry_out);
+/* R1CSProof::verify(num_vars, num_cons, inputs, evals, transcript, gens) with evals = (Ar, Br, Cr): SP_ERR_VERIFY / SP_ERR_DECOMPRESS naming the
+ * failing check; the transcript is advanced as the reference's verify advances it, accepted or not.  rx_out / ry_out as sp_r1cs_prove_t's.
+ * Refusals as sp_r1cs_prove_t's, and SP_ERR_INVALID_SCALAR for evals not reduced; a refused call leaves the transcript untouched. */
+int sp_r1cs_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, size_t num_cons, size_t num_vars, const uint64_t* inputs_mont, size_t ninputs,
+                     const uint64_t evals_mont[12], const sp_r1cs_gens* gens, uint8_t* strobe_state /* in, out */, uint64_t* rx_out, uint64_t* ry_out);
+
 /* ---- inner-product argument, operator level: BulletReductionProof::prove (src/nizk/bullet.rs:32-132) for a host that keeps the transcript and
  * the orchestration.  sp_ipa_begin copies a_vec / b_vec; the generator vector G is `gens` (G[0..n)).  Each round: sp_ipa_round_LR returns the
  * compressed L, R of bullet.rs:83-97 (c_L, c_R are formed inside; Q and H are the caller's points), the host appends them and derives u
@@ -581,6 +618,9 @@ int sp_instance_bincode(const sp_instance* inst, uint8_t** out, size_t* len);
 int sp_instance_nnz(const sp_instance* inst, int matrix, size_t* nnz);
 int sp_instance_export(const sp_instance* inst, int matrix, uint64_t* row, uint64_t* col, uint64_t* val_mont);
 int sp_instance_is_sat(sp_ctx* ctx, const sp_instance* inst, const uint64_t* vars_mont, size_t nvars, const uint64_t* inputs_mont, size_t ninputs, int* sat);
+/* R1CSShape::evaluate(rx, ry) (r1cs.rs:300-303): out = (A(rx, ry), B(rx, ry), C(rx, ry)), the claims sp_r1cs_verify_t takes.  rx: log2 num_cons
+ * scalars, ry: log2 (2 num_vars), of the padded dimensions.  SP_ERR_INVALID_SCALAR: rx or ry not reduced. */
+int sp_instance_evaluate(sp_ctx* ctx, const sp_instance* inst, const uint64_t* rx_mont, const uint64_t* ry_mont, uint64_t out_mont[12]);
 
 /* ---- NIZK                                                                                lib.rs:468-591 */
 int sp_nizk_gens_create(sp_ctx* ctx, size_t num_cons, size_t num_vars, size_t num_inputs, sp_nizk_gens** out);

@@ -13,5 +13,5 @@ from .api import (  # noqa: F401
     ZKSumcheckInstanceProof, KnowledgeProof, EqualityProof, ProductProof, DotProductProof, DotProductProofGens, DotProductProofLog,
     ProductLeaves, ProductCircuits, ProductCircuitEvalProofBatched, product_leaf_eval,
     SparseMatPolyCommitmentGens, SparseMatPolyCommitment, SparseMatPolyDense, SparseMatPolynomial, SparseMatPolyEvalProof,
-    SparseMatProducts,
+    SparseMatProducts, R1CSGens, R1CSProof,
 )

@@ -1187,7 +1187,7 @@ class SparseMatPolynomial:
         h = _vp()
         entry = lib.sp_spmat_create_device if device else lib.sp_spmat_create
         ctx.check(entry(ctx.h, arr, C.c_int(len(polys)), _sz(x), _sz(y), C.byref(h)))
-        return SparseMatProducts(ctx, h, len(polys))
+        return SparseMatProducts(ctx, h, len(polys), x, y)
 
     def _products(self):
         if getattr(self, "_spmat", None) is None:
@@ -1211,8 +1211,9 @@ class SparseMatProducts(_Handle):
     compute_eval_table_sparse of all of them in one call"""
     _free = lib.sp_spmat_free
 
-    def __init__(self, ctx, h, batch_size):
+    def __init__(self, ctx, h, batch_size, num_vars_x=None, num_vars_y=None):
         self.ctx, self.h, self.batch_size = ctx, h, batch_size
+        self.num_vars_x, self.num_vars_y = num_vars_x, num_vars_y
 
     def _vector(self, v):
         if isinstance(v, DensePolynomial):
@@ -1388,6 +1389,17 @@ class Instance(_Handle):
         self.ctx.check(lib.sp_instance_is_sat(self.ctx.h, self.h, _p(vars.limbs), _sz(len(vars)), _p(inputs.limbs), _sz(len(inputs)), C.byref(sat)))
         return bool(sat.value)
 
+    def evaluate(self, rx, ry):
+        """R1CSShape::evaluate (r1cs.rs:300-303) on the device: (A(rx, ry), B(rx, ry), C(rx, ry)) as (3, 4) Montgomery limbs, the evals
+        R1CSProof.verify takes.  rx: log2 num_cons scalars, ry: log2 (2 num_vars), of the padded dimensions."""
+        rx, ry = _limbs(rx), _limbs(ry)
+        nx, ny = self.num_cons.bit_length() - 1, (2 * self.num_vars).bit_length() - 1
+        if len(rx) != nx or len(ry) != ny:
+            raise SpartanB200Error("Instance.evaluate: |rx| = %d, |ry| = %d; this instance needs %d and %d" % (len(rx), len(ry), nx, ny))
+        out = np.zeros((3, 4), dtype=np.uint64)
+        self.ctx.check(lib.sp_instance_evaluate(self.ctx.h, self.h, _p(rx), _p(ry), _p(out)))
+        return out
+
 
 def _take_bytes(out, n):
     b = C.string_at(out, n.value)
@@ -1442,6 +1454,89 @@ class NIZKGens(_Handle):
     @staticmethod
     def new(num_cons, num_vars, num_inputs, ctx=None):
         return NIZKGens(num_cons, num_vars, num_inputs, ctx)
+
+
+class R1CSGens(_Handle):
+    """R1CSGens::new(label, num_cons, num_vars) (r1csproof.rs:61-74): gens_pc = PolyCommitmentGens::new(log2 num_vars, label) and the sumcheck
+    gens gens_1, gens_3, gens_4 of the same label's stream, for a power-of-two num_vars.  view(gens, num_cons, num_vars) gives the same gens as a
+    view of the gens_r1cs_sat set of NIZKGens, SNARKGens or GeneratorTables, without device memory of its own."""
+    _free = lib.sp_r1cs_gens_free
+
+    def __init__(self, label, num_cons, num_vars, ctx=None):
+        self.ctx = ctx or default_context()
+        self.num_cons, self.num_vars = num_cons, num_vars
+        h = _vp()
+        self.ctx.check(lib.sp_r1cs_gens_create(self.ctx.h, C.c_char_p(bytes(label)), _sz(len(label)), _sz(num_cons), _sz(num_vars), C.byref(h)))
+        self.h = h
+
+    @classmethod
+    def view(cls, gens_or_tables, num_cons, num_vars):
+        entry = {NIZKGens: lib.sp_r1cs_gens_create_from_nizk, SNARKGens: lib.sp_r1cs_gens_create_from_snark,
+                 GeneratorTables: lib.sp_r1cs_gens_create_from}.get(type(gens_or_tables))
+        if entry is None:
+            raise SpartanB200Error("R1CSGens.view: expected NIZKGens, SNARKGens or GeneratorTables, got %s" % type(gens_or_tables).__name__)
+        o = cls.__new__(cls)
+        o.ctx, o.num_cons, o.num_vars = gens_or_tables.ctx, num_cons, num_vars
+        h = _vp()
+        o.ctx.check(entry(o.ctx.h, gens_or_tables.h, _sz(num_cons), _sz(num_vars), C.byref(h)))
+        o.h = h
+        return o
+
+
+def _input_limbs(inputs):
+    return inputs.limbs if isinstance(inputs, Assignment) else _limbs(inputs)
+
+
+class R1CSProof:
+    """r1csproof.rs:20-489: the proof NIZK and SNARK embed, on the caller's Transcript and RandomTape.  `data` = bincode(R1CSProof)."""
+
+    def __init__(self, data):
+        self.data = bytes(data)
+
+    def to_bytes(self):
+        return self.data
+
+    @classmethod
+    def from_bytes(cls, data):
+        return cls(data)
+
+    @staticmethod
+    def prove(matrices, vars, inputs, gens, transcript, tape):
+        """R1CSProof::prove(inst, vars, inputs, gens, transcript, random_tape): returns (proof, rx, ry) with rx, ry as Montgomery limbs.
+        matrices: an Instance (its products as NIZK.prove runs them) or a SparseMatProducts of A, B, C (2^log2 num_cons rows, 2^log2 (2 num_vars)
+        columns: the tiled products, whatever the rows' and columns' lengths).  vars: a DensePolynomial (read only) or host limbs, num_vars =
+        len(vars) entries (the padded count); inputs: an Assignment or host limbs."""
+        ctx = gens.ctx
+        v = _device_vec(vars.limbs if isinstance(vars, Assignment) else vars, ctx)
+        num_vars = v.len()
+        if isinstance(matrices, Instance):
+            inst, spmat, num_cons = matrices.h, None, matrices.num_cons
+        elif isinstance(matrices, SparseMatProducts):
+            if matrices.num_vars_x is None:
+                raise SpartanB200Error("R1CSProof.prove: a SparseMatProducts of unknown shape (make it with SparseMatPolynomial.multi_products)")
+            inst, spmat, num_cons = None, matrices.h, 1 << matrices.num_vars_x
+        else:
+            raise SpartanB200Error("R1CSProof.prove: matrices must be an Instance or a SparseMatProducts, got %s" % type(matrices).__name__)
+        x = _input_limbs(inputs)
+        out, n = C.POINTER(C.c_ubyte)(), _sz()
+        rx = np.zeros((max(num_cons.bit_length() - 1, 1), 4), dtype=np.uint64)
+        ry = np.zeros((max((2 * num_vars).bit_length() - 1, 1), 4), dtype=np.uint64)
+        ctx.check(lib.sp_r1cs_prove_t(ctx.h, inst, spmat, _sz(num_cons), _sz(num_vars), v.h, _p(x), _sz(len(x)), gens.h, transcript.state, tape.state,
+                                      C.byref(out), C.byref(n), _p(rx), _p(ry)))
+        return R1CSProof(_take_bytes(out, n)), rx[:num_cons.bit_length() - 1], ry[:(2 * num_vars).bit_length() - 1]
+
+    def verify(self, num_vars, num_cons, inputs, evals, transcript, gens):
+        """R1CSProof::verify(num_vars, num_cons, inputs, evals, transcript, gens) with evals = (Ar, Br, Cr) as (3, 4) limbs: returns (rx, ry),
+        raises ProofVerifyError"""
+        ctx = gens.ctx
+        x, ev = _input_limbs(inputs), _limbs(evals)
+        if len(ev) != 3:
+            raise SpartanB200Error("R1CSProof.verify: %d evals; (Ar, Br, Cr) expected" % len(ev))
+        nx, ny = max(num_cons, 1).bit_length() - 1, max(2 * num_vars, 1).bit_length() - 1
+        rx, ry = np.zeros((max(nx, 1), 4), dtype=np.uint64), np.zeros((max(ny, 1), 4), dtype=np.uint64)
+        ctx.check(lib.sp_r1cs_verify_t(ctx.h, C.c_char_p(self.data), _sz(len(self.data)), _sz(num_cons), _sz(num_vars), _p(x), _sz(len(x)), _p(ev),
+                                       gens.h, transcript.state, _p(rx), _p(ry)))
+        return rx[:nx], ry[:ny]
 
 
 class NIZK:

@@ -2116,6 +2116,29 @@ static void spmat_create_common(sp_ctx* ctx, const sp_spark_entries* mats, int b
   }
   *out = S.release();
 }
+// outs[m] = M_m x (row order) or M_m^T x (transpose: column order), nout entries each, for every matrix m of S
+static void spmat_run(Ctx& c, const sp_spmat& S, bool transpose, const u256* x, u256* const* outs, size_t nout) {
+  dev::SpmatBatch B{};
+  B.b = S.b;
+  for (int m = 0; m < S.b; m++) {
+    const SpmatOrder& o = transpose ? S.by_col[m] : S.by_row[m];
+    B.key[m] = o.key.p; B.src[m] = o.src.p; B.val[m] = o.val.p; B.nnz[m] = S.nnz[m];
+    B.out[m] = outs[m];
+  }
+  DevBuf<uint8_t> scratch(dev::spmat_products_scratch_bytes(S.total));
+  dev::spmat_products(B, x, nout, scratch.p, c.stream);
+}
+// out = sum_m w[m] M_m^T e (nout entries), from the b tables in scratch
+static void spmat_weighted(Ctx& c, const sp_spmat& S, const u256* e, const u256* w, u256* out, size_t nout) {
+  DevBuf<u256> tables(nout * S.b);
+  u256* t[SP_SPMAT_MAX_BATCH];
+  for (int m = 0; m < S.b; m++) t[m] = tables.p + nout * m;
+  spmat_run(c, S, true, e, t, nout);
+  dev::LincombTables lt{};
+  lt.b = S.b;
+  for (int m = 0; m < S.b; m++) { lt.t[m] = t[m]; lt.w[m] = w[m]; }
+  dev::lincomb_many(out, lt, nout, c.stream);
+}
 // M_m z (transpose = false: row order, z of num_cols entries, outputs of num_rows) or M_m^T e (column order, e of num_rows, outputs of num_cols)
 static void spmat_product(sp_ctx* ctx, const sp_spmat* S, const sp_poly* x, size_t num_rows, size_t num_cols, const uint64_t* weights, sp_poly** outs,
                           bool transpose) {
@@ -2138,24 +2161,15 @@ static void spmat_product(sp_ctx* ctx, const sp_spmat* S, const sp_poly* x, size
     throw SpError(SP_ERR_INVALID_ARG, what + ": num_cols = " + std::to_string(num_cols) + " but an entry has col " + std::to_string(S->max_col));
   if (weights) require_reduced(weights, (size_t)S->b, (what + ": weights").c_str());
   const size_t nout = transpose ? num_cols : num_rows;
-  dev::SpmatBatch B{};
-  B.b = S->b;
   const int nres = weights ? 1 : S->b;
   std::vector<std::unique_ptr<sp_poly>> res(nres);
   for (int i = 0; i < nres; i++) res[i].reset(new sp_poly{&c, DevBuf<u256>(nout), nout});
-  DevBuf<u256> tables(weights ? nout * S->b : 0);   // the per-matrix tables of the weighted sum
-  for (int m = 0; m < S->b; m++) {
-    const SpmatOrder& o = transpose ? S->by_col[m] : S->by_row[m];
-    B.key[m] = o.key.p; B.src[m] = o.src.p; B.val[m] = o.val.p; B.nnz[m] = S->nnz[m];
-    B.out[m] = weights ? tables.p + nout * m : res[m]->d.p;
-  }
-  DevBuf<uint8_t> scratch(dev::spmat_products_scratch_bytes(S->total));
-  dev::spmat_products(B, x->d.p, nout, scratch.p, c.stream);
   if (weights) {
-    dev::LincombTables lt{};
-    lt.b = S->b;
-    for (int m = 0; m < S->b; m++) { lt.t[m] = B.out[m]; memcpy(&lt.w[m], weights + 4 * m, 32); }
-    dev::lincomb_many(res[0]->d.p, lt, nout, c.stream);
+    spmat_weighted(c, *S, x->d.p, reinterpret_cast<const u256*>(weights), res[0]->d.p, nout);
+  } else {
+    u256* o[SP_SPMAT_MAX_BATCH];
+    for (int m = 0; m < S->b; m++) o[m] = res[m]->d.p;
+    spmat_run(c, *S, transpose, x->d.p, o, nout);
   }
   for (int i = 0; i < nres; i++) outs[i] = res[i].release();
 }
@@ -2172,6 +2186,167 @@ int sp_spmat_multiply_vec(sp_ctx* ctx, const sp_spmat* mats, size_t num_rows, si
 }
 int sp_spmat_eval_table(sp_ctx* ctx, const sp_spmat* mats, const sp_poly* e, size_t num_rows, size_t num_cols, const uint64_t* weights_mont, sp_poly** outs) {
   return guarded(ctx, [&] { spmat_product(ctx, mats, e, num_rows, num_cols, weights_mont, outs, true); });
+}
+
+// ---- R1CSProof of the caller's matrices (prover.cpp: r1cs_prove, verifier.cpp: r1cs_verify_bytes), on this rank's GPU alone
+struct sp_r1cs_gens { Ctx* ctx; size_t num_vars; std::unique_ptr<R1CSGens> g; };
+static const size_t R1CS_MAX_LOG = 32;   // num_cons and 2 num_vars: the tiled products index rows and columns with 32 bits
+static bool is_pow2(size_t x) { return x && !(x & (x - 1)); }
+// num_cons >= 2 and num_vars >= 1 powers of two (the verifier's check_dims), with both sumchecks short enough to stage
+static void r1cs_dims(size_t num_cons, size_t num_vars, const std::string& what) {
+  if (num_cons < 2 || !is_pow2(num_cons) || !is_pow2(num_vars))
+    throw SpError(SP_ERR_INVALID_ARG, what + ": num_cons = " + std::to_string(num_cons) + " and num_vars = " + std::to_string(num_vars) +
+                                          " must be powers of two, num_cons >= 2");
+  const size_t lx = log2_ceil(num_cons), ly = log2_ceil(2 * num_vars);
+  if (std::max(lx, ly) > std::min(R1CS_MAX_LOG, zk_sumcheck_max_rounds()))
+    throw SpError(SP_ERR_INVALID_ARG, what + ": log2 num_cons = " + std::to_string(lx) + " and log2 (2 num_vars) = " + std::to_string(ly) + "; at most " +
+                                          std::to_string(std::min(R1CS_MAX_LOG, zk_sumcheck_max_rounds())) + " supported");
+}
+// the view of `set` for num_vars, after the checks every gens entry shares
+static void r1cs_gens_out(sp_ctx* ctx, std::shared_ptr<GenSet> set, size_t num_vars, sp_r1cs_gens** out, const std::string& what) {
+  if (set->ctx != &ctx->c) throw SpError(SP_ERR_INVALID_ARG, what + ": the generators belong to another context");
+  const size_t need = R1CSGens::bases(num_vars);
+  if (set->nbases < need)
+    throw SpError(SP_ERR_INVALID_ARG, what + ": num_vars = " + std::to_string(num_vars) + " needs " + std::to_string(need) + " generators of " + set->label +
+                                          ", the set has " + std::to_string(set->nbases));
+  std::unique_ptr<sp_r1cs_gens> g(new sp_r1cs_gens{&ctx->c, num_vars, nullptr});
+  g->g.reset(new R1CSGens(std::move(set), num_vars));
+  *out = g.release();
+}
+static void r1cs_gens_args(sp_r1cs_gens** out, size_t num_cons, size_t num_vars, const std::string& what) {
+  if (!out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  r1cs_dims(num_cons, num_vars, what);
+}
+int sp_r1cs_gens_create(sp_ctx* ctx, const uint8_t* label, size_t label_len, size_t num_cons, size_t num_vars, sp_r1cs_gens** out) {
+  return guarded(ctx, [&] {
+    const std::string what = "r1cs_gens_create";
+    if (!label && label_len) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    r1cs_gens_args(out, num_cons, num_vars, what);
+    r1cs_gens_out(ctx, std::make_shared<GenSet>(&ctx->c, std::string((const char*)label, label_len), R1CSGens::bases(num_vars), R1CSGens::host_bases(num_vars)),
+                  num_vars, out, what);
+  });
+}
+int sp_r1cs_gens_create_from(sp_ctx* ctx, const sp_gen_tables* tables, size_t num_cons, size_t num_vars, sp_r1cs_gens** out) {
+  return guarded(ctx, [&] {
+    const std::string what = "r1cs_gens_create_from";
+    if (!tables) throw SpError(SP_ERR_INVALID_ARG, what + ": tables is NULL");
+    r1cs_gens_args(out, num_cons, num_vars, what);
+    r1cs_gens_out(ctx, tables->t->r1cs_sat, num_vars, out, what);
+  });
+}
+int sp_r1cs_gens_create_from_nizk(sp_ctx* ctx, const sp_nizk_gens* gens, size_t num_cons, size_t num_vars, sp_r1cs_gens** out) {
+  return guarded(ctx, [&] {
+    const std::string what = "r1cs_gens_create_from_nizk";
+    if (!gens) throw SpError(SP_ERR_INVALID_ARG, what + ": gens is NULL");
+    r1cs_gens_args(out, num_cons, num_vars, what);
+    r1cs_gens_out(ctx, gens->g->set, num_vars, out, what);
+  });
+}
+int sp_r1cs_gens_create_from_snark(sp_ctx* ctx, const sp_snark_gens* gens, size_t num_cons, size_t num_vars, sp_r1cs_gens** out) {
+  return guarded(ctx, [&] {
+    const std::string what = "r1cs_gens_create_from_snark";
+    if (!gens) throw SpError(SP_ERR_INVALID_ARG, what + ": gens is NULL");
+    r1cs_gens_args(out, num_cons, num_vars, what);
+    r1cs_gens_out(ctx, gens->g->gens_r1cs_sat->set, num_vars, out, what);
+  });
+}
+void sp_r1cs_gens_free(sp_r1cs_gens* g) { delete g; }
+
+// the dimensions, the gens and the inputs of a prove or verify call
+static void r1cs_common(const sp_ctx* ctx, size_t num_cons, size_t num_vars, const uint64_t* inputs, size_t ninputs, const sp_r1cs_gens* gens,
+                        const std::string& what) {
+  r1cs_dims(num_cons, num_vars, what);
+  if (!inputs && ninputs) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+  if (!(ninputs < num_vars))   // r1csproof.rs:156
+    throw SpError(SP_ERR_INVALID_ARG, what + ": |inputs| + 1 = " + std::to_string(ninputs + 1) + " > num_vars = " + std::to_string(num_vars));
+  require_owned(ctx, gens, what, "gens");
+  if (gens->g->gens_pc.n != R1CSGens::pc_n(num_vars))
+    throw SpError(SP_ERR_INVALID_ARG, what + ": gens for num_vars = " + std::to_string(gens->num_vars) + " do not fit num_vars = " + std::to_string(num_vars));
+  require_reduced(inputs, ninputs, (what + ": inputs").c_str());
+}
+// the three matrices of an sp_spmat as R1CS matrices: the tiled products of sp_spmat_multiply_vec / sp_spmat_eval_table, never sharded
+struct SpmatMatrices : R1csMatrices {
+  const sp_spmat& S;
+  SpmatMatrices(const sp_spmat& s, size_t nc, size_t nv) : R1csMatrices(nc, nv), S(s) {}
+  void multiply_vec(Ctx& ctx, const u256* d_z, u256* const outs[3], size_t n, bool sh) const override {
+    if (sh) throw SpError(SP_ERR_INTERNAL, "r1cs_prove: sp_spmat products do not shard");
+    spmat_run(ctx, S, false, d_z, outs, n);
+  }
+  void eval_table(Ctx& ctx, const u256* d_e, const Fq w[3], u256*, u256* out, size_t n, bool sh) const override {
+    if (sh) throw SpError(SP_ERR_INTERNAL, "r1cs_prove: sp_spmat products do not shard");
+    const u256 wm[3] = {w[0].m, w[1].m, w[2].m};
+    spmat_weighted(ctx, S, d_e, wm, out, n);
+  }
+};
+int sp_r1cs_prove_t(sp_ctx* ctx, const sp_instance* inst, const sp_spmat* spmat, size_t num_cons, size_t num_vars, const sp_poly* vars, const uint64_t* inputs,
+                    size_t ninputs, const sp_r1cs_gens* gens, uint8_t* strobe_state, uint8_t* tape_state, uint8_t** proof, size_t* proof_len, uint64_t* rx_out,
+                    uint64_t* ry_out) {
+  return guarded(ctx, [&] {
+    const std::string what = "r1cs_prove";
+    ProofStates st(strobe_state, tape_state, what);
+    if (!proof || !proof_len || !rx_out || !ry_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    if (!inst == !spmat) throw SpError(SP_ERR_INVALID_ARG, what + ": pass exactly one of inst and spmat");
+    r1cs_common(ctx, num_cons, num_vars, inputs, ninputs, gens, what);
+    std::optional<InstanceMatrices> im;
+    std::optional<SpmatMatrices> sm;
+    if (inst) {
+      const Instance& I = inst->inst;
+      require_device(ctx->c, I.M[0].csr_ptr.p, 1, (what + ": inst").c_str());   // the instance's matrices live on this context's device
+      if (I.num_cons != num_cons || I.num_vars != num_vars)
+        throw SpError(SP_ERR_INVALID_ARG, what + ": the instance is " + std::to_string(I.num_cons) + " x " + std::to_string(I.num_vars) + " (padded), not " +
+                                              std::to_string(num_cons) + " x " + std::to_string(num_vars));
+      im.emplace(I);
+    } else {
+      require_owned(ctx, spmat, what, "spmat");
+      const size_t x = log2_ceil(num_cons), y = log2_ceil(2 * num_vars);
+      if (spmat->b != 3 || spmat->x != x || spmat->y != y)
+        throw SpError(SP_ERR_INVALID_ARG, what + ": spmat holds " + std::to_string(spmat->b) + " matrices of 2^" + std::to_string(spmat->x) + " x 2^" +
+                                              std::to_string(spmat->y) + ", R1CS needs 3 of 2^" + std::to_string(x) + " x 2^" + std::to_string(y));
+      sm.emplace(*spmat, num_cons, num_vars);
+    }
+    require_owned(ctx, vars, what, "vars");
+    if (vars->len != num_vars)
+      throw SpError(SP_ERR_INVALID_ARG, what + ": vars has " + std::to_string(vars->len) + " entries, num_vars = " + std::to_string(num_vars));
+    st.open();
+    ctx->c.timings.clear();
+    R1CSProof P;
+    std::vector<Fq> rx, ry;
+    r1cs_prove(ctx->c, im ? static_cast<const R1csMatrices&>(*im) : *sm, vars->d.p, fq_vec(inputs, ninputs), *gens->g, st.T(), st.tape(), P, rx, ry);
+    st.proved();
+    put_bytes(proof, proof_len, to_bincode(P));
+    put_scalars(rx_out, rx);
+    put_scalars(ry_out, ry);
+  });
+}
+int sp_r1cs_verify_t(sp_ctx* ctx, const uint8_t* proof, size_t proof_len, size_t num_cons, size_t num_vars, const uint64_t* inputs, size_t ninputs,
+                     const uint64_t* evals, const sp_r1cs_gens* gens, uint8_t* strobe_state, uint64_t* rx_out, uint64_t* ry_out) {
+  return guarded(ctx, [&] {
+    const std::string what = "r1cs_verify";
+    ProofStates st(strobe_state);
+    if ((!proof && proof_len) || !evals || !rx_out || !ry_out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    r1cs_common(ctx, num_cons, num_vars, inputs, ninputs, gens, what);
+    require_reduced(evals, 3, (what + ": evals").c_str());
+    const std::vector<Fq> ev = fq_vec(evals, 3);
+    st.open_verify();
+    std::vector<Fq> rx, ry;
+    r1cs_verify_bytes(ctx->c, proof, proof_len, num_vars, num_cons, fq_vec(inputs, ninputs), ev.data(), *gens->g, st.T(), rx, ry);
+    put_scalars(rx_out, rx);
+    put_scalars(ry_out, ry);
+  });
+}
+// R1CSShape::evaluate (r1cs.rs:300-303) through the instance's COO on the device
+int sp_instance_evaluate(sp_ctx* ctx, const sp_instance* inst, const uint64_t* rx, const uint64_t* ry, uint64_t* out) {
+  return guarded(ctx, [&] {
+    const std::string what = "instance_evaluate";
+    if (!inst || !rx || !ry || !out) throw SpError(SP_ERR_INVALID_ARG, what + ": NULL argument");
+    const Instance& I = inst->inst;
+    const size_t x = log2_ceil(I.num_cons), y = log2_ceil(2 * I.num_vars);
+    require_reduced(rx, x, (what + ": rx").c_str());
+    require_reduced(ry, y, (what + ": ry").c_str());
+    Fq ev[3];
+    instance_evaluate(ctx->c, I, fq_vec(rx, x), fq_vec(ry, y), ev);
+    for (int m = 0; m < 3; m++) fq_out(out + 4 * m, ev[m]);
+  });
 }
 
 static int nizk_verify_batch_common(sp_ctx* ctx, const sp_instance* const* insts, const sp_nizk_gens* gens, const BatchArgs& a) {

@@ -241,9 +241,8 @@ size_t R1CSGens::pc_n(size_t num_vars) {
 size_t R1CSGens::bases(size_t num_vars) { return std::max<size_t>(pc_n(num_vars) + 2, 5); }   // gens_4 draws 5 points of the same stream
 std::vector<size_t> R1CSGens::host_bases(size_t num_vars) { const size_t n = pc_n(num_vars); return {0, 1, 2, 3, 4, n, n + 1}; }
 
-R1CSGens::R1CSGens(const Ctx* ctx, const GenTables& tables, size_t num_vars) {
-  tables.require(ctx, bases(num_vars), 0);
-  set = tables.r1cs_sat;
+R1CSGens::R1CSGens(const Ctx* ctx, const GenTables& tables, size_t num_vars) : R1CSGens((tables.require(ctx, bases(num_vars), 0), tables.r1cs_sat), num_vars) {}
+R1CSGens::R1CSGens(std::shared_ptr<GenSet> s, size_t num_vars) : set(std::move(s)) {
   set->add_host_tables(host_bases(num_vars));
   const size_t n = pc_n(num_vars);
   gens_pc.n = n;
@@ -1256,11 +1255,33 @@ struct PhaseTimer {
   ~PhaseTimer() { ctx.timings.push_back({name, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count()}); }
 };
 
-void r1cs_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::vector<Fq>& input, const R1CSGens& gens, Transcript& T,
+InstanceMatrices::InstanceMatrices(const Instance& i) : R1csMatrices(i.num_cons, i.num_vars), inst(i) {}
+void InstanceMatrices::multiply_vec(Ctx& ctx, const u256* d_z, u256* const outs[3], size_t n, bool sh) const {
+  const int W = ctx.shard_world(), rk = ctx.rank();
+  for (int m = 0; m < 3; m++) {
+    const SparseMatDev& S = inst.M[m];
+    if (sh) dev::spmv_cyclic(outs[m], n, rk, W, S.csr_ptr.p, S.csr_idx.p, S.csr_val.p, d_z, ctx.stream);   // this rank's rows
+    else dev::spmv(outs[m], n, S.csr_ptr.p, S.csr_idx.p, S.csr_val.p, d_z, ctx.stream);
+  }
+}
+void InstanceMatrices::eval_table(Ctx& ctx, const u256* d_e, const Fq w[3], u256* d_w, u256* out, size_t n, bool sh) const {
+  const int W = ctx.shard_world(), rk = ctx.rank();
+  DevBuf<u256> eA(n), eB(n), eC(n);
+  u256* outs[3] = {eA.p, eB.p, eC.p};
+  for (int m = 0; m < 3; m++) {
+    const SparseMatDev& S = inst.M[m];
+    if (sh) dev::spmv_cyclic(outs[m], n, rk, W, S.csc_ptr.p, S.csc_idx.p, S.csc_val.p, d_e, ctx.stream);   // this rank's columns
+    else dev::spmv(outs[m], n, S.csc_ptr.p, S.csc_idx.p, S.csc_val.p, d_e, ctx.stream);
+  }
+  dev::h2d(d_w, w, 3 * sizeof(u256), ctx.stream);
+  dev::lincomb3(out, eA.p, eB.p, eC.p, d_w, n, ctx.stream);
+}
+
+void r1cs_prove(Ctx& ctx, const R1csMatrices& mats, const u256* d_vars, const std::vector<Fq>& input, const R1CSGens& gens, Transcript& T,
                 RandomTape& tape, R1CSProof& proof, std::vector<Fq>& rx, std::vector<Fq>& ry, const R1csHooks* hooks) {
   PhaseTimer t_all(ctx, "R1CSProof::prove");
   T.append_protocol_name("R1CS proof");
-  const size_t num_vars = inst.num_vars, num_cons = inst.num_cons;
+  const size_t num_vars = mats.num_vars, num_cons = mats.num_cons;
   if (!(input.size() < num_vars)) throw std::runtime_error("spartan_b200: |input| + 1 must be at most the number of variables");  // r1csproof.rs:156
   T.append_scalars("input", input);
 
@@ -1297,17 +1318,16 @@ void r1cs_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::v
     dev::dzero(d_z.p + num_vars + tail.size(), (num_vars - tail.size()) * sizeof(u256), ctx.stream);
     std::vector<Fq> tau = T.challenge_vector("challenge_tau", num_rounds_x);
     dev::h2d(d_chal.p, tau.data(), tau.size() * sizeof(u256), ctx.stream);
-    // inst.multiply_vec (r1cs.rs:268-282)
-    u256* outs[3] = {d_Az.p, d_Bz.p, d_Cz.p};
     if (sh1) {
       // this rank's slice of eq(tau, .): eq over the leading variables times the factor its low index bits fix; its rows of A z, B z, C z
       dev::eq_evals(d_tau.p, d_chal.p, (int)num_rounds_x - logW, eq_small.p, ctx.stream);
       dev::scale(d_tau.p, shard_eq_scale(tau, W, rk).m, n1, ctx.stream);
-      for (int m = 0; m < 3; m++) dev::spmv_cyclic(outs[m], n1, rk, W, inst.M[m].csr_ptr.p, inst.M[m].csr_idx.p, inst.M[m].csr_val.p, d_z.p, ctx.stream);
     } else {
       dev::eq_evals(d_tau.p, d_chal.p, (int)num_rounds_x, eq_small.p, ctx.stream);
-      for (int m = 0; m < 3; m++) dev::spmv(outs[m], num_cons, inst.M[m].csr_ptr.p, inst.M[m].csr_idx.p, inst.M[m].csr_val.p, d_z.p, ctx.stream);
     }
+    // inst.multiply_vec (r1cs.rs:268-282)
+    u256* const outs[3] = {d_Az.p, d_Bz.p, d_Cz.p};
+    mats.multiply_vec(ctx, d_z.p, outs, n1, sh1);
     u256* tabs[4] = {d_tau.p, d_Az.p, d_Bz.p, d_Cz.p};
     ScRounds sc = one_instance(ctx, dev::SC_CUBIC4, tabs, 4, num_rounds_x, sh1);
     zk_sumcheck_prove(ctx, sc, 3, Fq::zero(), Fq::zero(), num_rounds_x, gens.gens_1, gens.gens_4, T, tape, proof.sc_proof_phase1, rx, claims1,
@@ -1337,14 +1357,8 @@ void r1cs_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::v
     // evals_rx = eq(rx, .), then the three transposed SpMVs of compute_eval_table_sparse (r1cs.rs:284-298), then r_A*A + r_B*B + r_C*C
     dev::h2d(d_chal.p, rx.data(), rx.size() * sizeof(u256), ctx.stream);
     dev::eq_evals(d_tau.p, d_chal.p, (int)num_rounds_x, eq_small.p, ctx.stream);
-    DevBuf<u256> eA(n2), eB(n2), eC(n2), d_ABC(n2), d_zloc;
-    u256* outs[3] = {eA.p, eB.p, eC.p};
-    for (int m = 0; m < 3; m++) {
-      if (sh2) dev::spmv_cyclic(outs[m], n2, rk, W, inst.M[m].csc_ptr.p, inst.M[m].csc_idx.p, inst.M[m].csc_val.p, d_tau.p, ctx.stream);   // this rank's columns
-      else dev::spmv(outs[m], zlen, inst.M[m].csc_ptr.p, inst.M[m].csc_idx.p, inst.M[m].csc_val.p, d_tau.p, ctx.stream);
-    }
-    dev::h2d(d_chal.p + 32, rabc, 3 * sizeof(u256), ctx.stream);
-    dev::lincomb3(d_ABC.p, eA.p, eB.p, eC.p, d_chal.p + 32, n2, ctx.stream);
+    DevBuf<u256> d_ABC(n2), d_zloc;
+    mats.eval_table(ctx, d_tau.p, rabc, d_chal.p + 32, d_ABC.p, n2, sh2);
     if (sh2) { d_zloc.alloc(n2); dev::take_cyclic(d_zloc.p, d_z.p, n2, rk, W, ctx.stream); }
     u256* tabs[2] = {sh2 ? d_zloc.p : d_z.p, d_ABC.p};
     ScRounds sc = one_instance(ctx, dev::SC_QUAD, tabs, 2, num_rounds_y, sh2);
@@ -1378,7 +1392,7 @@ void nizk_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::v
   PhaseTimer t(ctx, "NIZK::prove");
   RandomTape tape("proof", tape_seed);                                   // lib.rs:511
   append_nizk_head(T, inst);
-  r1cs_prove(ctx, inst, d_vars, input, gens, T, tape, out.r1cs_sat_proof, out.rx, out.ry);
+  r1cs_prove(ctx, InstanceMatrices(inst), d_vars, input, gens, T, tape, out.r1cs_sat_proof, out.rx, out.ry);
 }
 
 }  // namespace sp

@@ -14,11 +14,13 @@ struct PolyCommitmentGens {  // dense_mlpoly.rs:24-36 -> DotProductProofGens (ni
   CommitKey gens_n, gens_1;
 };
 struct R1CSGens {  // r1csproof.rs:39-74
-  std::shared_ptr<GenSet> set;   // gens_r1cs_sat of the tables this is a view into
+  std::shared_ptr<GenSet> set;   // the label's set this is a view into (gens_r1cs_sat of the tables, or a caller label's own set)
   PolyCommitmentGens gens_pc;
   CommitKey gens_1, gens_3, gens_4;
   // a view into tables.r1cs_sat for a num_vars (padded) circuit; SpError(SP_ERR_INVALID_ARG) when the set is too short or of another context
   R1CSGens(const Ctx* ctx, const GenTables& tables, size_t num_vars);
+  // a view into a set of at least bases(num_vars) generators (checked by the caller); adds the host tables it needs
+  R1CSGens(std::shared_ptr<GenSet> set, size_t num_vars);
   static size_t pc_n(size_t num_vars);                      // gens_pc.n
   static size_t bases(size_t num_vars);                     // generators of gens_r1cs_sat the view uses
   static std::vector<size_t> host_bases(size_t num_vars);   // the bases it needs host copies of
@@ -54,12 +56,36 @@ struct Instance {  // lib.rs:111-114 (R1CSShape + digest)
 
 std::vector<uint8_t> miniz_zlib_level6(const uint8_t* data, size_t len);   // deflate.cpp
 
+// The two products of the R1CS matrices A, B, C (num_cons x 2 num_vars, both powers of two) that R1CSProof::prove needs: inst.multiply_vec
+// (r1cs.rs:268-282) in phase one and the weighted compute_eval_table_sparse (r1cs.rs:284-298) in phase two.  `sh`: the prover runs that phase's
+// sumcheck on cyclic shards (Ctx::shard_table), and the outputs are this rank's n entries of each table.
+struct R1csMatrices {
+  size_t num_cons, num_vars;
+  R1csMatrices(size_t nc, size_t nv) : num_cons(nc), num_vars(nv) {}
+  virtual ~R1csMatrices() = default;
+  // outs[m] = M_m z, z of 2 num_vars entries
+  virtual void multiply_vec(Ctx& ctx, const u256* d_z, u256* const outs[3], size_t n, bool sh) const = 0;
+  // out = w[0] A^T e + w[1] B^T e + w[2] C^T e, e of num_cons entries; d_w: 3 scalars of device scratch the weights may be staged in
+  virtual void eval_table(Ctx& ctx, const u256* d_e, const Fq w[3], u256* d_w, u256* out, size_t n, bool sh) const = 0;
+};
+// an Instance's CSR / CSC copies through k_spmv (one thread per row or column), sharded when asked: the NIZK and SNARK provers' products
+struct InstanceMatrices : R1csMatrices {
+  const Instance& inst;
+  explicit InstanceMatrices(const Instance& i);
+  void multiply_vec(Ctx& ctx, const u256* d_z, u256* const outs[3], size_t n, bool sh) const override;
+  void eval_table(Ctx& ctx, const u256* d_e, const Fq w[3], u256* d_w, u256* out, size_t n, bool sh) const override;
+};
+
 // R1CSProof::prove (r1csproof.rs:144-349).  d_vars: device array of num_vars Montgomery scalars (consumed read-only).
 // hooks: called (when set) as soon as the first / the second sumcheck phase has produced its point, so that the caller can start work that
 // depends only on rx / ry on another stream while the rest of the proof runs (SNARK::prove: the dereferenced SPARK values and their commitment)
 struct R1csHooks { std::function<void(const std::vector<Fq>&)> on_rx, on_ry; };
-void r1cs_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::vector<Fq>& input, const R1CSGens& gens, Transcript& T,
+void r1cs_prove(Ctx& ctx, const R1csMatrices& mats, const u256* d_vars, const std::vector<Fq>& input, const R1CSGens& gens, Transcript& T,
                 RandomTape& tape, R1CSProof& proof, std::vector<Fq>& rx, std::vector<Fq>& ry, const R1csHooks* hooks = nullptr);
+// R1CSProof::verify (r1csproof.rs:351-489) on bincode bytes with the Immediate checker (verifier.cpp): SpError(SP_ERR_VERIFY / SP_ERR_DECOMPRESS)
+// naming the failing check.  evals: the claimed (A(rx, ry), B(rx, ry), C(rx, ry)).  Out: rx, ry
+void r1cs_verify_bytes(Ctx& ctx, const uint8_t* proof, size_t len, size_t num_vars, size_t num_cons, const std::vector<Fq>& input, const Fq evals[3],
+                       const R1CSGens& gens, Transcript& T, std::vector<Fq>& rx, std::vector<Fq>& ry);
 // NIZK::prove (lib.rs:501-546)
 void nizk_prove(Ctx& ctx, const Instance& inst, const u256* d_vars, const std::vector<Fq>& input, const R1CSGens& gens, Transcript& T,
                 const Fq& tape_seed, NizkProof& out);

@@ -482,7 +482,7 @@ void snark_prove(Ctx& ctx, const Instance& inst, const SnarkEncoding& enc, const
   }
 
   std::vector<Fq> rx, ry;
-  r1cs_prove(ctx, inst, d_vars, input, *gens.gens_r1cs_sat, T, tape, out.r1cs_sat_proof, rx, ry, early ? &hooks : nullptr);
+  r1cs_prove(ctx, InstanceMatrices(inst), d_vars, input, *gens.gens_r1cs_sat, T, tape, out.r1cs_sat_proof, rx, ry, early ? &hooks : nullptr);
 
   auto t0 = std::chrono::steady_clock::now();
   const std::array<Fq, 3>& inst_evals = out.inst_evals;

@@ -802,6 +802,14 @@ void nizk_verify(Ctx& ctx, const Instance& inst, const std::vector<Fq>& input, c
   nizk_replay(chk, inst, input, gens, T, p);
 }
 
+// R1CSProof::verify (r1csproof.rs:351-489) of a caller's proof; the dimensions are checked by the caller
+void r1cs_verify_bytes(Ctx& ctx, const uint8_t* proof, size_t len, size_t num_vars, size_t num_cons, const std::vector<Fq>& input, const Fq evals[3],
+                       const R1CSGens& gens, Transcript& T, std::vector<Fq>& rx, std::vector<Fq>& ry) {
+  const R1CSProof p = from_bincode<R1CSProof>(proof, len, SP_ERR_VERIFY, "R1CS proof");
+  Immediate chk(ctx);
+  r1cs_verify(chk, p, num_vars, num_cons, input, evals, T, gens, rx, ry);
+}
+
 // SNARK::verify (lib.rs:423-465); `enc` supplies the ComputationCommitment
 void snark_verify(Ctx& ctx, const SnarkEncoding& enc, const std::vector<Fq>& input, const SnarkGens& gens, Transcript& T, const uint8_t* proof, size_t len) {
   check_commitment(enc.comm);
