@@ -2,15 +2,14 @@
 import ctypes as C
 import hashlib
 import os
+import re
 import zlib
 
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "libspartan_b200.so")
-
-SP_OK, SP_ERR_NO_DEVICE, SP_ERR_CUDA, SP_ERR_INVALID_ARG, SP_ERR_INVALID_INDEX, SP_ERR_INVALID_SCALAR, SP_ERR_INVALID_INPUTS, SP_ERR_INTERNAL = range(8)
-SP_ERR_INVALID_POINT, SP_ERR_VERIFY, SP_ERR_DECOMPRESS = 8, 9, 10
+_HEADER = os.path.join(_HERE, os.pardir, "include", "spartan_b200.h")
 
 
 class SpartanB200Error(RuntimeError):
@@ -36,13 +35,36 @@ def _load():
     return C.CDLL(_LIB_PATH)
 
 
+_RESTYPES = {"int": C.c_int, "void": None, "size_t": C.c_size_t, "unsigned long long": C.c_ulonglong, "const char*": C.c_char_p}
+_ARGTYPES = {"int": C.c_int, "size_t": C.c_size_t, "uint64_t": C.c_uint64}
+
+
+def _declare(lib, header):
+    """Set restype and argtypes on `lib` for every sp_* function `header` declares, and return the header's `#define SP_<NAME> <decimal>`
+    constants.  Pointer and array parameters become c_void_p, by-value ones map through _ARGTYPES, return types through _RESTYPES; any
+    other type, or a declared name the library does not export, raises.  So ctypes refuses a call with too few arguments or an argument of
+    the wrong type.  Two gaps remain: a call with extra trailing arguments is not refused (ctypes passes them on to a cdecl function), and a
+    Python int too wide for a c_int parameter is truncated (2**40 arrives as 0), as C.c_int(2**40) truncates it."""
+    with open(header) as f:
+        text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", f.read(), flags=re.S)
+    consts = {m[1]: int(m[2]) for m in re.finditer(r"^[ \t]*#[ \t]*define[ \t]+(SP_\w+)[ \t]+(\d+)[ \t]*$", text, re.M)}
+    for decl in re.split(r"[;{}]", re.sub(r"^[ \t]*#.*$", " ", text, flags=re.M)):
+        decl = " ".join(decl.split())
+        if not re.search(r"\bsp_\w+ ?\(", decl):
+            continue   # a typedef, a struct member, extern "C"
+        m = re.fullmatch(r"(.+?) ?\b(sp_\w+) ?\((.*)\)", decl)
+        try:
+            fn = getattr(lib, m[2])
+            fn.restype = _RESTYPES[m[1].replace(" *", "*")]
+            params = [] if m[3] == "void" else [p.strip() for p in m[3].split(",")]
+            fn.argtypes = [C.c_void_p if "*" in p or "[" in p else _ARGTYPES[p.rpartition(" ")[0]] for p in params]
+        except (TypeError, KeyError, AttributeError):   # no match, a type outside the mapping, a name the library lacks
+            raise SpartanB200Error("%s: cannot bind `%s` to %s" % (header, decl, _LIB_PATH)) from None
+    return consts
+
+
 lib = _load()
-lib.sp_last_error.restype = C.c_char_p
-lib.sp_kernel_launches.restype = C.c_ulonglong
-lib.sp_release_cached_memory.restype = C.c_ulonglong
-lib.sp_device_bytes_live.restype = C.c_ulonglong
-lib.sp_poly_len.restype = C.c_size_t
-lib.sp_points_len.restype = C.c_size_t
+globals().update(_declare(lib, _HEADER))
 _vp, _sz = C.c_void_p, C.c_size_t
 
 
@@ -59,13 +81,10 @@ class _MemcheckCounts(C.Structure):
     _fields_ = [(n, C.c_ulonglong) for n in ("blocks_filled", "blocks_refilled", "context_refills", "guard_bytes_checked", "violations")]
 
 
-lib.sp_debug_memcheck_scan.restype = C.c_ulonglong
-
-
 def debug_memcheck(on=True):
     """process-wide memory-check mode (sp_debug_memcheck, single GPU): every device block filled when handed out and guarded past its end, the
     contexts' persistent scratch refilled at every call.  Switch it on before the first Context is created"""
-    lib.sp_debug_memcheck(C.c_int(1 if on else 0))
+    lib.sp_debug_memcheck(1 if on else 0)
 
 
 def debug_memcheck_scan():
@@ -80,7 +99,7 @@ def debug_memcheck_report():
     """the mode's counters since load, and the first and the latest violation's message ("" when there was none)"""
     c = _MemcheckCounts()
     buf = C.create_string_buffer(8192)
-    if lib.sp_debug_memcheck_report(C.byref(c), buf, _sz(len(buf))) != SP_OK:
+    if lib.sp_debug_memcheck_report(C.byref(c), buf, len(buf)) != SP_OK:
         raise SpartanB200Error("sp_debug_memcheck_report: message longer than the buffer")
     out = {n: int(getattr(c, n)) for n, _ in _MemcheckCounts._fields_}
     first, _, last = buf.value.decode().partition("\n")
@@ -119,6 +138,19 @@ def _check_host(rc):
         raise _status_error(rc, lib.sp_last_error(None).decode())
 
 
+def _string_out(check, entry, *args):
+    """the string entry(*args, buf, buflen) writes, with the buffer doubled while the entry refuses it as too short (SP_ERR_INVALID_ARG);
+    `check` raises for any other failure"""
+    n = 4096
+    while True:
+        buf = C.create_string_buffer(n)
+        rc = entry(*args, buf, n)
+        if rc != SP_ERR_INVALID_ARG:
+            check(rc)
+            return buf.value.decode()
+        n *= 2
+
+
 class _Handle:
     """owner of one library object `h`, released by the class's `_free` when the Python object goes"""
     _free = None
@@ -138,9 +170,7 @@ class Context(_Handle):
 
     def __init__(self, device=0):
         h = _vp()
-        rc = lib.sp_ctx_create(C.c_int(device), C.byref(h))
-        if rc != SP_OK:
-            raise SpartanB200Error("sp_ctx_create failed (%d): %s" % (rc, lib.sp_last_error(None).decode()))
+        _check_host(lib.sp_ctx_create(device, C.byref(h)))
         self.h = h
         self.device = device
 
@@ -152,28 +182,25 @@ class Context(_Handle):
         """Join `world` single-GPU processes into one sharded prover (sp_comm_export / sp_comm_connect).  `allgather(b: bytes) -> list[bytes]`
         is the host-side exchange (every rank contributes its handle, all get the list in rank order): spartan_b200.dist.allgather_bytes under
         torch.distributed.  Afterwards NIZK.prove / SNARK.prove must be called by every rank with the same arguments."""
-        lib.sp_comm_handle_bytes.restype = C.c_size_t
-        hb = int(lib.sp_comm_handle_bytes())
+        hb = lib.sp_comm_handle_bytes()
         mine = C.create_string_buffer(hb)
         self.check(lib.sp_comm_export(self.h, mine))
         handles = allgather(mine.raw)
         assert len(handles) == world and all(len(h) == hb for h in handles)
-        self.check(lib.sp_comm_connect(self.h, C.c_int(rank), C.c_int(world), C.c_char_p(b"".join(handles))))
+        self.check(lib.sp_comm_connect(self.h, rank, world, b"".join(handles)))
         self.rank, self.world = rank, world
 
     def set_sharding(self, enabled):
         """switch sharded proving off / on for a connected context (every rank must switch together)"""
-        lib.sp_comm_set_enabled(self.h, C.c_int(1 if enabled else 0))
+        self.check(lib.sp_comm_set_enabled(self.h, 1 if enabled else 0))
 
     def set_overlap(self, enabled):
         """background-stream commitment of the dereferenced values in SNARK.prove on / off (off: every kernel on one stream, for per-kernel profiling)"""
-        lib.sp_ctx_set_overlap(self.h, C.c_int(1 if enabled else 0))
+        self.check(lib.sp_ctx_set_overlap(self.h, 1 if enabled else 0))
 
     def timings(self):
-        buf = C.create_string_buffer(8192)
-        lib.sp_timings(self.h, buf, _sz(8192))
         out = {}
-        for item in buf.value.decode().split(";"):
+        for item in _string_out(self.check, lib.sp_timings, self.h).split(";"):
             if "=" in item:
                 k, v = item.split("=")
                 out[k] = float(v)
@@ -194,7 +221,7 @@ def default_context():
 def scalar_from_bytes(b):
     """Scalar::from_bytes (ristretto255.rs:391): canonical 32 bytes -> Montgomery limbs; raises on non-canonical input"""
     out = np.zeros(4, dtype=np.uint64)
-    if lib.sp_scalar_from_bytes(C.c_char_p(bytes(b)), _p(out)) != SP_OK:
+    if lib.sp_scalar_from_bytes(bytes(b), _p(out)) != SP_OK:
         raise R1CSError("InvalidScalar")
     return out
 
@@ -210,7 +237,7 @@ def prg_scalars(tag, n, seed=0):
     raw = hashlib.shake_256(b"spartan-b200/v1/" + tag.encode() + int(seed).to_bytes(8, "little")).digest(64 * n)
     out = np.zeros((n, 4), dtype=np.uint64)
     for i in range(n):
-        lib.sp_scalar_from_bytes_wide(C.c_char_p(raw[64 * i:64 * i + 64]), _p(out[i]))
+        lib.sp_scalar_from_bytes_wide(raw[64 * i:64 * i + 64], _p(out[i]))
     return out
 
 
@@ -223,7 +250,7 @@ def tape_seed(seed=0):
 def random_tape_seed():
     """the scalar RandomTape::new draws from OsRng (random.rs:13-15): 64 bytes of OS randomness -> Scalar::from_bytes_wide"""
     out = np.zeros(4, dtype=np.uint64)
-    lib.sp_scalar_from_bytes_wide(C.c_char_p(os.urandom(64)), _p(out))
+    lib.sp_scalar_from_bytes_wide(os.urandom(64), _p(out))
     return out
 
 
@@ -262,7 +289,7 @@ class DensePolynomial(_Handle):
         self.ctx = ctx or default_context()
         Z = _limbs(Z)
         h = _vp()
-        self.ctx.check(lib.sp_poly_upload(self.ctx.h, _p(Z), _sz(len(Z)), C.byref(h)))
+        self.ctx.check(lib.sp_poly_upload(self.ctx.h, _p(Z), len(Z), C.byref(h)))
         self.h = h
 
     @classmethod
@@ -279,7 +306,7 @@ class DensePolynomial(_Handle):
         vals = _device_tensor(vals, ctx, "vals", _torch().uint8, 32)
         _sync_torch(ctx)
         h = _vp()
-        ctx.check(lib.sp_poly_from_canonical_device(ctx.h, _vp(vals.data_ptr()), _sz(vals.shape[0]), C.byref(h)))
+        ctx.check(lib.sp_poly_from_canonical_device(ctx.h, _vp(vals.data_ptr()), vals.shape[0], C.byref(h)))
         return cls._wrap(ctx, h)
 
     def len(self):
@@ -287,23 +314,23 @@ class DensePolynomial(_Handle):
 
     def to_numpy(self):
         out = np.zeros((self.len(), 4), dtype=np.uint64)
-        self.ctx.check(lib.sp_poly_download(self.ctx.h, self.h, _p(out), _sz(len(out))))
+        self.ctx.check(lib.sp_poly_download(self.ctx.h, self.h, _p(out), len(out)))
         return out
 
     def bound_poly_var_top(self, r):
         arr = (_vp * 1)(self.h)
-        self.ctx.check(lib.sp_fold_top(self.ctx.h, arr, C.c_int(1), _p(np.ascontiguousarray(r, dtype=np.uint64))))
+        self.ctx.check(lib.sp_fold_top(self.ctx.h, arr, 1, _p(np.ascontiguousarray(r, dtype=np.uint64))))
 
     def evaluate(self, r):
         r = _limbs(r)
         out = np.zeros(4, dtype=np.uint64)
-        self.ctx.check(lib.sp_poly_evaluate(self.ctx.h, self.h, _p(r), _sz(len(r)), _p(out)))
+        self.ctx.check(lib.sp_poly_evaluate(self.ctx.h, self.h, _p(r), len(r), _p(out)))
         return out
 
     def bound(self, L):
         L = _limbs(L)
         h = _vp()
-        self.ctx.check(lib.sp_poly_bound_rows(self.ctx.h, self.h, _p(L), _sz(len(L)), C.byref(h)))
+        self.ctx.check(lib.sp_poly_bound_rows(self.ctx.h, self.h, _p(L), len(L), C.byref(h)))
         return DensePolynomial._wrap(self.ctx, h)
 
     def dot(self, other):
@@ -315,7 +342,7 @@ class DensePolynomial(_Handle):
         """DensePolynomial::commit_inner (dense_mlpoly.rs:148-177) -> list of L compressed points"""
         out = C.create_string_buffer(32 * L)
         bl = _limbs(blinds) if blinds is not None else None
-        self.ctx.check(lib.sp_commit_rows(self.ctx.h, gens.h, self.h, _sz(L), _sz(R), _p(bl) if bl is not None else None, out))
+        self.ctx.check(lib.sp_commit_rows(self.ctx.h, gens.h, self.h, L, R, _p(bl) if bl is not None else None, out))
         return [out.raw[32 * i:32 * i + 32] for i in range(L)]
 
     @staticmethod
@@ -323,7 +350,7 @@ class DensePolynomial(_Handle):
         ctx = ctx or default_context()
         r = _limbs(r)
         h = _vp()
-        ctx.check(lib.sp_eq_evals(ctx.h, _p(r), _sz(len(r)), C.byref(h)))
+        ctx.check(lib.sp_eq_evals(ctx.h, _p(r), len(r), C.byref(h)))
         return DensePolynomial._wrap(ctx, h)
 
 
@@ -331,7 +358,7 @@ def sumcheck_eval(kind, polys):
     ctx = polys[0].ctx
     arr = (_vp * len(polys))(*[p.h for p in polys])
     out = np.zeros((3, 4), dtype=np.uint64)
-    ctx.check(lib.sp_sumcheck_eval(ctx.h, C.c_int(kind), arr, _p(out)))
+    ctx.check(lib.sp_sumcheck_eval(ctx.h, kind, arr, _p(out)))
     return out
 
 
@@ -339,7 +366,7 @@ def sumcheck_fold_eval(kind, polys, r):
     ctx = polys[0].ctx
     arr = (_vp * len(polys))(*[p.h for p in polys])
     out = np.zeros((3, 4), dtype=np.uint64)
-    ctx.check(lib.sp_sumcheck_fold_eval(ctx.h, C.c_int(kind), arr, _p(np.ascontiguousarray(r, dtype=np.uint64)), _p(out)))
+    ctx.check(lib.sp_sumcheck_fold_eval(ctx.h, kind, arr, _p(np.ascontiguousarray(r, dtype=np.uint64)), _p(out)))
     return out
 
 
@@ -347,14 +374,14 @@ def sumcheck_eval_sharded(kind, polys):
     """sumcheck_eval on cyclic shards held by the ranks of a connected context: returns the evaluations of the whole tables on every rank"""
     ctx = polys[0].ctx
     out = np.zeros((3, 4), dtype=np.uint64)
-    ctx.check(lib.sp_sumcheck_eval_sharded(ctx.h, C.c_int(kind), (_vp * len(polys))(*[p.h for p in polys]), _p(out)))
+    ctx.check(lib.sp_sumcheck_eval_sharded(ctx.h, kind, (_vp * len(polys))(*[p.h for p in polys]), _p(out)))
     return out
 
 
 def sumcheck_fold_eval_sharded(kind, polys, r):
     ctx = polys[0].ctx
     out = np.zeros((3, 4), dtype=np.uint64)
-    ctx.check(lib.sp_sumcheck_fold_eval_sharded(ctx.h, C.c_int(kind), (_vp * len(polys))(*[p.h for p in polys]), _p(np.ascontiguousarray(r, dtype=np.uint64)), _p(out)))
+    ctx.check(lib.sp_sumcheck_fold_eval_sharded(ctx.h, kind, (_vp * len(polys))(*[p.h for p in polys]), _p(np.ascontiguousarray(r, dtype=np.uint64)), _p(out)))
     return out
 
 
@@ -366,7 +393,7 @@ def sumcheck_batched_eval(As, Bs, Cs):
     """prove_cubic_batched evaluation loops (sumcheck.rs:290-357) for len(As) instances of A*B*C; returns (ninst, 3, 4) limbs [e0, e2, e3]"""
     ctx = As[0].ctx
     out = np.zeros((len(As), 3, 4), dtype=np.uint64)
-    ctx.check(lib.sp_sumcheck_batched_eval(ctx.h, C.c_int(len(As)), _handles(As), _handles(Bs), _handles(Cs), _p(out)))
+    ctx.check(lib.sp_sumcheck_batched_eval(ctx.h, len(As), _handles(As), _handles(Bs), _handles(Cs), _p(out)))
     return out
 
 
@@ -374,17 +401,14 @@ def sumcheck_batched_fold_eval(As, Bs, Cs, r):
     """bind the top variable of every table with r (a C shared by several instances once) and evaluate the next round"""
     ctx = As[0].ctx
     out = np.zeros((len(As), 3, 4), dtype=np.uint64)
-    ctx.check(lib.sp_sumcheck_batched_fold_eval(ctx.h, C.c_int(len(As)), _handles(As), _handles(Bs), _handles(Cs), _p(np.ascontiguousarray(r, dtype=np.uint64)), _p(out)))
+    ctx.check(lib.sp_sumcheck_batched_fold_eval(ctx.h, len(As), _handles(As), _handles(Bs), _handles(Cs), _p(np.ascontiguousarray(r, dtype=np.uint64)), _p(out)))
     return out
 
 
 def fold_top(polys, r):
     ctx = polys[0].ctx
     arr = (_vp * len(polys))(*[p.h for p in polys])
-    ctx.check(lib.sp_fold_top(ctx.h, arr, C.c_int(len(polys)), _p(np.ascontiguousarray(r, dtype=np.uint64))))
-
-
-SP_SC_MAX_DEGREE, SP_SC_MAX_TABLES, SP_SC_MAX_TERMS = 6, 8, 32
+    ctx.check(lib.sp_fold_top(ctx.h, arr, len(polys), _p(np.ascontiguousarray(r, dtype=np.uint64))))
 
 
 class _ScTerm(C.Structure):
@@ -428,8 +452,8 @@ def sumcheck_prove(polys, comp, claim, num_rounds, transcript):
     r = np.zeros((num_rounds, 4), dtype=np.uint64)
     finals = np.zeros((len(polys), 4), dtype=np.uint64)
     e = np.zeros(4, dtype=np.uint64)
-    ctx.check(lib.sp_sumcheck_prove_t(ctx.h, _handles(polys), C.c_int(len(polys)), terms, C.c_int(len(comp.terms)),
-                                      _p(np.ascontiguousarray(claim, dtype=np.uint64)), _sz(num_rounds), t.state, C.byref(out), C.byref(n), _p(r),
+    ctx.check(lib.sp_sumcheck_prove_t(ctx.h, _handles(polys), len(polys), terms, len(comp.terms),
+                                      _p(np.ascontiguousarray(claim, dtype=np.uint64)), num_rounds, t.state, C.byref(out), C.byref(n), _p(r),
                                       _p(finals), _p(e)))
     return _take_bytes(out, n), r, finals, e
 
@@ -441,8 +465,8 @@ def sumcheck_verify(proof, claim, num_rounds, degree_bound, transcript):
     proof = bytes(proof)
     e = np.zeros(4, dtype=np.uint64)
     r = np.zeros((num_rounds, 4), dtype=np.uint64)
-    _check_host(lib.sp_sumcheck_verify_t(None, C.c_char_p(proof), _sz(len(proof)), _p(np.ascontiguousarray(claim, dtype=np.uint64)), _sz(num_rounds),
-                                         _sz(degree_bound), t.state, _p(e), _p(r)))
+    _check_host(lib.sp_sumcheck_verify_t(None, proof, len(proof), _p(np.ascontiguousarray(claim, dtype=np.uint64)), num_rounds,
+                                         degree_bound, t.state, _p(e), _p(r)))
     return e, r
 
 
@@ -454,7 +478,7 @@ class MultiCommitGens(_Handle):
         self.ctx = ctx or default_context()
         self.n = n
         h = _vp()
-        self.ctx.check(lib.sp_gens_create(self.ctx.h, C.c_char_p(label), _sz(len(label)), _sz(n), C.byref(h)))
+        self.ctx.check(lib.sp_gens_create(self.ctx.h, bytes(label), len(label), n, C.byref(h)))
         self.h = h
 
     @classmethod
@@ -464,7 +488,7 @@ class MultiCommitGens(_Handle):
         o.ctx = ctx or default_context()
         o.n = len(compressed) - 1
         h = _vp()
-        o.ctx.check(lib.sp_gens_upload(o.ctx.h, C.c_char_p(b"".join(compressed)), _sz(o.n), C.byref(h)))
+        o.ctx.check(lib.sp_gens_upload(o.ctx.h, b"".join(compressed), o.n, C.byref(h)))
         o.h = h
         return o
 
@@ -477,7 +501,7 @@ class MultiCommitGens(_Handle):
         """GroupElement::vartime_multiscalar_mul(scalars, G).compress()"""
         s = _limbs(scalars)
         out = C.create_string_buffer(32)
-        self.ctx.check(lib.sp_msm(self.ctx.h, self.h, _p(s), _sz(len(s)), out))
+        self.ctx.check(lib.sp_msm(self.ctx.h, self.h, _p(s), len(s), out))
         return out.raw
 
 
@@ -494,7 +518,7 @@ class BulletReduction(_Handle):
 
     def round_LR(self, Q, H, blind_L, blind_R):
         L, R = C.create_string_buffer(32), C.create_string_buffer(32)
-        self.ctx.check(lib.sp_ipa_round_LR(self.ctx.h, self.h, C.c_char_p(Q), C.c_char_p(H), _p(np.ascontiguousarray(blind_L, dtype=np.uint64)),
+        self.ctx.check(lib.sp_ipa_round_LR(self.ctx.h, self.h, bytes(Q), bytes(H), _p(np.ascontiguousarray(blind_L, dtype=np.uint64)),
                                            _p(np.ascontiguousarray(blind_R, dtype=np.uint64)), L, R))
         return L.raw, R.raw
 
@@ -515,7 +539,7 @@ class Points(_Handle):
         """compressed: list of 32-byte ristretto255 encodings; raises if any does not decompress"""
         self.ctx = ctx or default_context()
         h = _vp()
-        self.ctx.check(lib.sp_points_upload(self.ctx.h, C.c_char_p(b"".join(compressed)), _sz(len(compressed)), C.byref(h)))
+        self.ctx.check(lib.sp_points_upload(self.ctx.h, b"".join(compressed), len(compressed), C.byref(h)))
         self.h = h
 
     @classmethod
@@ -524,7 +548,7 @@ class Points(_Handle):
         o = cls.__new__(cls)
         o.ctx = ctx or default_context()
         h = _vp()
-        o.ctx.check(lib.sp_points_derive(o.ctx.h, C.c_char_p(label), _sz(len(label)), _sz(n), C.byref(h)))
+        o.ctx.check(lib.sp_points_derive(o.ctx.h, bytes(label), len(label), n, C.byref(h)))
         o.h = h
         return o
 
@@ -534,23 +558,23 @@ class Points(_Handle):
     def export(self, offset=0, n=None):
         n = len(self) - offset if n is None else n
         out = C.create_string_buffer(32 * n + 1)
-        self.ctx.check(lib.sp_points_export(self.ctx.h, self.h, _sz(offset), _sz(n), out))
+        self.ctx.check(lib.sp_points_export(self.ctx.h, self.h, offset, n, out))
         return [out.raw[32 * i:32 * i + 32] for i in range(n)]
 
     def msm(self, scalars, offset=0):
         """GroupElement::vartime_multiscalar_mul(scalars, points[offset:offset+len(scalars)]).compress()  (group.rs:98-117)"""
         out = C.create_string_buffer(32)
         if isinstance(scalars, DensePolynomial):
-            self.ctx.check(lib.sp_msm_var_resident(self.ctx.h, self.h, _sz(offset), scalars.h, out))
+            self.ctx.check(lib.sp_msm_var_resident(self.ctx.h, self.h, offset, scalars.h, out))
         else:
             s = _limbs(scalars)
-            self.ctx.check(lib.sp_msm_var(self.ctx.h, self.h, _sz(offset), _p(s), _sz(len(s)), out))
+            self.ctx.check(lib.sp_msm_var(self.ctx.h, self.h, offset, _p(s), len(s), out))
         return out.raw
 
     def msm_sharded(self, scalars, offset=0):
         """this rank's slice of a vector split by index range over the ranks of a connected context -> encoding of the whole sum (on every rank)"""
         out = C.create_string_buffer(32)
-        self.ctx.check(lib.sp_msm_var_sharded(self.ctx.h, self.h, _sz(offset), scalars.h, out))
+        self.ctx.check(lib.sp_msm_var_sharded(self.ctx.h, self.h, offset, scalars.h, out))
         return out.raw
 
 
@@ -558,7 +582,7 @@ def point_roundtrip(points, ctx=None):
     ctx = ctx or default_context()
     n = len(points)
     out = C.create_string_buffer(32 * n)
-    ctx.check(lib.sp_point_roundtrip(ctx.h, C.c_char_p(b"".join(points)), _sz(n), out))
+    ctx.check(lib.sp_point_roundtrip(ctx.h, b"".join(points), n, out))
     return [out.raw[32 * i:32 * i + 32] for i in range(n)]
 
 
@@ -566,7 +590,7 @@ def point_decompress_check(points, ctx=None):
     ctx = ctx or default_context()
     n = len(points)
     ok = (C.c_int * n)()
-    ctx.check(lib.sp_point_decompress_check(ctx.h, C.c_char_p(b"".join(points)), _sz(n), ok))
+    ctx.check(lib.sp_point_decompress_check(ctx.h, b"".join(points), n, ok))
     return [bool(x) for x in ok]
 
 
@@ -575,16 +599,16 @@ class Transcript:
     the 203-byte STROBE-128 state, advanced in place by NIZK.prove / SNARK.prove / verify when passed instead of a label."""
 
     def __init__(self, label):
-        self.state = C.create_string_buffer(203)
-        lib.sp_transcript_new(C.c_char_p(label), _sz(len(label)), self.state)
+        self.state = C.create_string_buffer(SP_TRANSCRIPT_STATE_BYTES)
+        _check_host(lib.sp_transcript_new(bytes(label), len(label), self.state))
 
     def append_message(self, label, msg):
         msg = bytes(msg)
-        _check_host(lib.sp_transcript_append_message(self.state, C.c_char_p(label), _sz(len(label)), C.c_char_p(msg), _sz(len(msg))))
+        _check_host(lib.sp_transcript_append_message(self.state, bytes(label), len(label), msg, len(msg)))
 
     def challenge_bytes(self, label, n):
         out = C.create_string_buffer(n)
-        _check_host(lib.sp_transcript_challenge_bytes(self.state, C.c_char_p(label), _sz(len(label)), out, _sz(n)))
+        _check_host(lib.sp_transcript_challenge_bytes(self.state, bytes(label), len(label), out, n))
         return out.raw
 
 
@@ -599,14 +623,14 @@ class PolyCommitmentGens(_Handle):
         self.ctx = ctx or default_context()
         self.num_vars, self.n = num_vars, 1 << (num_vars - num_vars // 2)
         h = _vp()
-        self.ctx.check(lib.sp_pc_gens_create(self.ctx.h, _sz(num_vars), C.c_char_p(bytes(label)), _sz(len(label)), C.byref(h)))
+        self.ctx.check(lib.sp_pc_gens_create(self.ctx.h, num_vars, bytes(label), len(label), C.byref(h)))
         self.h = h
 
     def view(self, num_vars):
         o = PolyCommitmentGens.__new__(PolyCommitmentGens)
         o.ctx, o.num_vars, o.n = self.ctx, num_vars, 1 << (num_vars - num_vars // 2)
         h = _vp()
-        self.ctx.check(lib.sp_pc_gens_create_from(self.ctx.h, self.h, _sz(num_vars), C.byref(h)))
+        self.ctx.check(lib.sp_pc_gens_create_from(self.ctx.h, self.h, num_vars, C.byref(h)))
         o.h = h
         return o
 
@@ -618,7 +642,7 @@ class RandomTape(Transcript):
 
     def __init__(self, seed=None):
         s = random_tape_seed() if seed is None else np.ascontiguousarray(seed, dtype=np.uint64).reshape(4)
-        self.state = C.create_string_buffer(203)
+        self.state = C.create_string_buffer(SP_TRANSCRIPT_STATE_BYTES)
         _check_host(lib.sp_random_tape_new(_p(s), self.state))
 
 
@@ -666,8 +690,7 @@ def poly_commit(polys, gens, tape=None):
     ell = (max(polys[0].len(), 1).bit_length() - 1 + (k - 1).bit_length()) if k else 0   # log2 of the merge's length
     blinds = np.zeros((1 << (ell // 2), 4), dtype=np.uint64)
     out, n = C.POINTER(C.c_ubyte)(), _sz()
-    ctx.check(lib.sp_pc_commit(ctx.h, gens.h, _handles(polys), C.c_int(k), tape.state if tape is not None else None, C.byref(out), C.byref(n),
-                               _p(blinds)))
+    ctx.check(lib.sp_pc_commit(ctx.h, gens.h, _handles(polys), k, tape.state if tape is not None else None, C.byref(out), C.byref(n), _p(blinds)))
     return PolyCommitment.from_bytes(_take_bytes(out, n)), blinds
 
 
@@ -685,13 +708,13 @@ class PolyEvalProof:
         t, r = _transcript_state(transcript), _limbs(r)
         out, n = C.POINTER(C.c_ubyte)(), _sz()
         c_zr, zr = C.create_string_buffer(32), np.zeros(4, dtype=np.uint64)
-        ctx.check(lib.sp_pc_eval_prove_t(ctx.h, gens.h, poly.h, _opt_limbs(blinds), _p(r), _sz(len(r)), _opt_limbs(Zr), _opt_limbs(blind_Zr), t.state,
+        ctx.check(lib.sp_pc_eval_prove_t(ctx.h, gens.h, poly.h, _opt_limbs(blinds), _p(r), len(r), _opt_limbs(Zr), _opt_limbs(blind_Zr), t.state,
                                          tape.state, C.byref(out), C.byref(n), c_zr, _p(zr)))
         return PolyEvalProof(_take_bytes(out, n)), c_zr.raw, zr
 
     def verify(self, gens, transcript, r, C_Zr, comm):
         """PolyEvalProof::verify against the commitment C_Zr (32 bytes); raises ProofVerifyError"""
-        self._verify(gens, transcript, r, C.c_char_p(bytes(C_Zr)), None, comm)
+        self._verify(gens, transcript, r, bytes(C_Zr), None, comm)
 
     def verify_plain(self, gens, transcript, r, Zr, comm):
         """PolyEvalProof::verify_plain against the evaluation Zr (limbs); raises ProofVerifyError"""
@@ -699,8 +722,7 @@ class PolyEvalProof:
 
     def _verify(self, gens, transcript, r, c_zr, zr, comm):
         t, r, cb = _transcript_state(transcript), _limbs(r), comm.to_bytes()
-        gens.ctx.check(lib.sp_pc_eval_verify_t(gens.ctx.h, gens.h, C.c_char_p(cb), _sz(len(cb)), _p(r), _sz(len(r)), c_zr, zr, t.state,
-                                               C.c_char_p(self.data), _sz(len(self.data))))
+        gens.ctx.check(lib.sp_pc_eval_verify_t(gens.ctx.h, gens.h, cb, len(cb), _p(r), len(r), c_zr, zr, t.state, self.data, len(self.data)))
 
     @staticmethod
     def prove_joint(polys, blinds, r, gens, transcript, tape):
@@ -710,21 +732,17 @@ class PolyEvalProof:
         t, r = _transcript_state(transcript), _limbs(r)
         out, n = C.POINTER(C.c_ubyte)(), _sz()
         evals = np.zeros((len(polys), 4), dtype=np.uint64)
-        ctx.check(lib.sp_pc_eval_prove_joint_t(ctx.h, gens.h, _handles(polys), C.c_int(len(polys)), _opt_limbs(blinds), _p(r), _sz(len(r)), t.state,
+        ctx.check(lib.sp_pc_eval_prove_joint_t(ctx.h, gens.h, _handles(polys), len(polys), _opt_limbs(blinds), _p(r), len(r), t.state,
                                                tape.state, C.byref(out), C.byref(n), _p(evals)))
         return PolyEvalProof(_take_bytes(out, n)), evals
 
     def verify_joint(self, gens, transcript, r, evals, comm):
         """DerefsEvalProof::verify_single for prove_joint's proof; raises ProofVerifyError"""
         t, r, ev, cb = _transcript_state(transcript), _limbs(r), _limbs(evals), comm.to_bytes()
-        gens.ctx.check(lib.sp_pc_eval_verify_joint_t(gens.ctx.h, gens.h, C.c_char_p(cb), _sz(len(cb)), _p(r), _sz(len(r)), _p(ev), C.c_int(len(ev)),
-                                                     t.state, C.c_char_p(self.data), _sz(len(self.data))))
+        gens.ctx.check(lib.sp_pc_eval_verify_joint_t(gens.ctx.h, gens.h, cb, len(cb), _p(r), len(r), _p(ev), len(ev), t.state, self.data, len(self.data)))
 
 
 # ----------------------------------------------------------------------------- zero-knowledge sumchecks and sigma protocols
-SP_DOTPROD_MAX_N = 64
-
-
 def _scalar(x):
     return _p(np.ascontiguousarray(x, dtype=np.uint64).reshape(4))
 
@@ -733,7 +751,7 @@ def _point(c):
     c = bytes(c)
     if len(c) != 32:
         raise SpartanB200Error("a commitment is 32 bytes, got %d" % len(c))
-    return C.c_char_p(c)
+    return c
 
 
 class ZKSumcheckInstanceProof:
@@ -754,8 +772,8 @@ class ZKSumcheckInstanceProof:
         r = np.zeros((num_rounds, 4), dtype=np.uint64)
         finals = np.zeros((len(polys), 4), dtype=np.uint64)
         blind_post = np.zeros(4, dtype=np.uint64)
-        ctx.check(lib.sp_zk_sumcheck_prove_t(ctx.h, _handles(polys), C.c_int(len(polys)), terms, C.c_int(len(comp.terms)), _scalar(claim),
-                                             _scalar(blind_claim), _sz(num_rounds), gens_1.h, gens_n.h, transcript.state, tape.state, C.byref(out),
+        ctx.check(lib.sp_zk_sumcheck_prove_t(ctx.h, _handles(polys), len(polys), terms, len(comp.terms), _scalar(claim),
+                                             _scalar(blind_claim), num_rounds, gens_1.h, gens_n.h, transcript.state, tape.state, C.byref(out),
                                              C.byref(n), _p(r), _p(finals), _p(blind_post)))
         return ZKSumcheckInstanceProof(_take_bytes(out, n)), r, finals, blind_post
 
@@ -764,7 +782,7 @@ class ZKSumcheckInstanceProof:
         ctx = gens_1.ctx
         comm_eval = C.create_string_buffer(32)
         r = np.zeros((max(num_rounds, 1), 4), dtype=np.uint64)
-        ctx.check(lib.sp_zk_sumcheck_verify_t(ctx.h, C.c_char_p(self.data), _sz(len(self.data)), _point(comm_claim), _sz(num_rounds), _sz(degree_bound),
+        ctx.check(lib.sp_zk_sumcheck_verify_t(ctx.h, self.data, len(self.data), _point(comm_claim), num_rounds, degree_bound,
                                               gens_1.h, gens_n.h, transcript.state, comm_eval, _p(r)))
         return comm_eval.raw, r[:num_rounds]
 
@@ -784,7 +802,7 @@ class KnowledgeProof:
         return KnowledgeProof(_take_bytes(out, n)), Cc.raw
 
     def verify(self, gens_n, transcript, C_):
-        gens_n.ctx.check(lib.sp_knowledge_verify_t(gens_n.ctx.h, gens_n.h, transcript.state, _point(C_), C.c_char_p(self.data), _sz(len(self.data))))
+        gens_n.ctx.check(lib.sp_knowledge_verify_t(gens_n.ctx.h, gens_n.h, transcript.state, _point(C_), self.data, len(self.data)))
 
 
 class EqualityProof:
@@ -802,8 +820,7 @@ class EqualityProof:
         return EqualityProof(_take_bytes(out, n)), c1.raw, c2.raw
 
     def verify(self, gens_n, transcript, C1, C2):
-        gens_n.ctx.check(lib.sp_equality_verify_t(gens_n.ctx.h, gens_n.h, transcript.state, _point(C1), _point(C2), C.c_char_p(self.data),
-                                                  _sz(len(self.data))))
+        gens_n.ctx.check(lib.sp_equality_verify_t(gens_n.ctx.h, gens_n.h, transcript.state, _point(C1), _point(C2), self.data, len(self.data)))
 
 
 class ProductProof:
@@ -822,8 +839,7 @@ class ProductProof:
         return ProductProof(_take_bytes(out, n)), X.raw, Y.raw, Z.raw
 
     def verify(self, gens_n, transcript, X, Y, Z):
-        gens_n.ctx.check(lib.sp_product_verify_t(gens_n.ctx.h, gens_n.h, transcript.state, _point(X), _point(Y), _point(Z), C.c_char_p(self.data),
-                                                 _sz(len(self.data))))
+        gens_n.ctx.check(lib.sp_product_verify_t(gens_n.ctx.h, gens_n.h, transcript.state, _point(X), _point(Y), _point(Z), self.data, len(self.data)))
 
 
 class DotProductProof:
@@ -840,13 +856,13 @@ class DotProductProof:
             raise SpartanB200Error("DotProductProof: x_vec has %d entries, a_vec %d" % (len(x), len(a)))
         out, n, cx, cy = C.POINTER(C.c_ubyte)(), _sz(), C.create_string_buffer(32), C.create_string_buffer(32)
         gens_1.ctx.check(lib.sp_dotproduct_prove_t(gens_1.ctx.h, gens_1.h, gens_n.h, transcript.state, tape.state, _p(x), _scalar(blind_x), _p(a),
-                                                   _sz(len(x)), _scalar(y), _scalar(blind_y), C.byref(out), C.byref(n), cx, cy))
+                                                   len(x), _scalar(y), _scalar(blind_y), C.byref(out), C.byref(n), cx, cy))
         return DotProductProof(_take_bytes(out, n)), cx.raw, cy.raw
 
     def verify(self, gens_1, gens_n, transcript, a, Cx, Cy):
         a = _limbs(a)
-        gens_1.ctx.check(lib.sp_dotproduct_verify_t(gens_1.ctx.h, gens_1.h, gens_n.h, transcript.state, _p(a), _sz(len(a)), _point(Cx), _point(Cy),
-                                                    C.c_char_p(self.data), _sz(len(self.data))))
+        gens_1.ctx.check(lib.sp_dotproduct_verify_t(gens_1.ctx.h, gens_1.h, gens_n.h, transcript.state, _p(a), len(a), _point(Cx), _point(Cy),
+                                                    self.data, len(self.data)))
 
 
 class DotProductProofGens(_Handle):
@@ -858,7 +874,7 @@ class DotProductProofGens(_Handle):
         self.ctx = ctx or default_context()
         self.n = n
         h = _vp()
-        self.ctx.check(lib.sp_dotlog_gens_create(self.ctx.h, _sz(n), C.c_char_p(bytes(label)), _sz(len(label)), C.byref(h)))
+        self.ctx.check(lib.sp_dotlog_gens_create(self.ctx.h, n, bytes(label), len(label), C.byref(h)))
         self.h = h
 
 
@@ -889,13 +905,10 @@ class DotProductProofLog:
         """raises ProofVerifyError"""
         ctx = gens.ctx
         a = _device_vec(a, ctx)
-        ctx.check(lib.sp_dotlog_verify_t(ctx.h, gens.h, transcript.state, a.h, _sz(n), _point(Cx), _point(Cy), C.c_char_p(self.data), _sz(len(self.data))))
+        ctx.check(lib.sp_dotlog_verify_t(ctx.h, gens.h, transcript.state, a.h, n, _point(Cx), _point(Cy), self.data, len(self.data)))
 
 
 # ----------------------------------------------------------------------------- product circuits of the caller's tables
-SP_PROD_MAX_CIRCUITS, SP_PROD_MAX_SOURCES = 24, 3
-
-
 class _ProdLeaves(C.Structure):
     _fields_ = [("nsources", C.c_uint32), ("source", C.c_uint32 * SP_PROD_MAX_SOURCES), ("coeff_mont", (C.c_uint64 * 4) * SP_PROD_MAX_SOURCES),
                 ("index_coeff_mont", C.c_uint64 * 4), ("const_mont", C.c_uint64 * 4)]
@@ -954,12 +967,11 @@ class ProductCircuits(_Handle):
         claims = np.zeros((max(self.kd, 1), 2, 4), dtype=np.uint64)
         h = _vp()
         if dotps is None:
-            self.ctx.check(lib.sp_prod_build(self.ctx.h, _handles(tables), C.c_int(len(tables)), _c_leaves(leaves), C.c_int(self.k), C.byref(h),
-                                             _p(products)))
+            self.ctx.check(lib.sp_prod_build(self.ctx.h, _handles(tables), len(tables), _c_leaves(leaves), self.k, C.byref(h), _p(products)))
         else:
             forms = _c_leaves([f for d in dotps for f in d])
-            self.ctx.check(lib.sp_prod_build_dotp(self.ctx.h, _handles(tables), C.c_int(len(tables)), _c_leaves(leaves), C.c_int(self.k), forms,
-                                                  C.c_int(self.kd), C.byref(h), _p(products), _p(claims)))
+            self.ctx.check(lib.sp_prod_build_dotp(self.ctx.h, _handles(tables), len(tables), _c_leaves(leaves), self.k, forms,
+                                                  self.kd, C.byref(h), _p(products), _p(claims)))
         self.h = h
         self.products = products[:self.k]
         self.dotp_claims = claims[:self.kd]
@@ -988,8 +1000,7 @@ class ProductCircuitEvalProofBatched:
         t, proof, prods = _transcript_state(transcript), bytes(proof), _limbs(products)
         rand = np.zeros((max(num_vars, 1), 4), dtype=np.uint64)
         claims = np.zeros((max(len(prods), 1), 4), dtype=np.uint64)
-        _check_host(lib.sp_prod_verify_t(None, C.c_char_p(proof), _sz(len(proof)), _p(prods), C.c_int(len(prods)), _sz(num_vars), t.state, _p(rand),
-                                         _p(claims)))
+        _check_host(lib.sp_prod_verify_t(None, proof, len(proof), _p(prods), len(prods), num_vars, t.state, _p(rand), _p(claims)))
         return rand[:num_vars], claims[:len(prods)]
 
     @staticmethod
@@ -1016,8 +1027,8 @@ class ProductCircuitEvalProofBatched:
         rand = np.zeros((max(num_vars, 1), 4), dtype=np.uint64)
         claims = np.zeros((max(len(prods), 1), 4), dtype=np.uint64)
         dotp = np.zeros((max(kd, 1), 3, 4), dtype=np.uint64)
-        _check_host(lib.sp_prod_verify_dotp_t(None, C.c_char_p(proof), _sz(len(proof)), _p(prods), C.c_int(len(prods)), _p(halves), C.c_int(kd),
-                                              _sz(num_vars), t.state, _p(rand), _p(claims), _p(dotp)))
+        _check_host(lib.sp_prod_verify_dotp_t(None, proof, len(proof), _p(prods), len(prods), _p(halves), kd,
+                                              num_vars, t.state, _p(rand), _p(claims), _p(dotp)))
         return rand[:num_vars], claims[:len(prods)], dotp[:kd]
 
 
@@ -1027,16 +1038,11 @@ def product_leaf_eval(leaves, table_evals, rand):
     ev, r = _limbs(table_evals), _limbs(rand)
     k = len(ev) if leaves is None else len(leaves)
     out = np.zeros((max(k, 1), 4), dtype=np.uint64)
-    _check_host(lib.sp_prod_leaf_eval(_c_leaves(leaves), C.c_int(k), _p(ev), C.c_int(len(ev)), _p(r), _sz(len(r)), _p(out)))
+    _check_host(lib.sp_prod_leaf_eval(_c_leaves(leaves), k, _p(ev), len(ev), _p(r), len(r), _p(out)))
     return out[:k]
 
 
 # ----------------------------------------------------------------------------- SPARK: the caller's sparse matrices
-SP_SPARK_MAX_BATCH = 4
-SP_SPMAT_MAX_BATCH = 8
-SP_SPMAT_PRODUCT_LAUNCHES = 3
-
-
 class _SparkEntries(C.Structure):
     _fields_ = [("row", _vp), ("col", _vp), ("val32", _vp), ("nnz", C.c_size_t)]
 
@@ -1051,8 +1057,7 @@ class SparseMatPolyCommitmentGens(_Handle):
         self.num_vars_x, self.num_vars_y, self.batch_size = num_vars_x, num_vars_y, batch_size
         label = bytes(label)
         h = _vp()
-        self.ctx.check(lib.sp_spark_gens_create(self.ctx.h, C.c_char_p(label), _sz(len(label)), _sz(num_vars_x), _sz(num_vars_y), _sz(num_nz_entries),
-                                                _sz(batch_size), C.byref(h)))
+        self.ctx.check(lib.sp_spark_gens_create(self.ctx.h, label, len(label), num_vars_x, num_vars_y, num_nz_entries, batch_size, C.byref(h)))
         self.h = h
 
 
@@ -1154,7 +1159,7 @@ class SparseMatPolynomial:
             _sync_torch(ctx)
         h, out, n = _vp(), C.POINTER(C.c_ubyte)(), _sz()
         entry = lib.sp_spark_commit_device if device else lib.sp_spark_commit
-        ctx.check(entry(ctx.h, gens.h, arr, C.c_int(len(polys)), _sz(x), _sz(y), C.byref(h), C.byref(out), C.byref(n)))
+        ctx.check(entry(ctx.h, gens.h, arr, len(polys), x, y, C.byref(h), C.byref(out), C.byref(n)))
         dense = SparseMatPolyDense(ctx, h, len(polys), x, y)
         return SparseMatPolyCommitment.from_bytes(_take_bytes(out, n)), dense
 
@@ -1169,7 +1174,7 @@ class SparseMatPolynomial:
             dense = SparseMatPolynomial.multi_commit(dense_or_polys, gens)[1]
         rx, ry = _limbs(rx), _limbs(ry)
         out = np.zeros((dense.batch_size, 4), dtype=np.uint64)
-        dense.ctx.check(lib.sp_spark_evaluate(dense.ctx.h, dense.h, _p(rx), _sz(len(rx)), _p(ry), _sz(len(ry)), _p(out)))
+        dense.ctx.check(lib.sp_spark_evaluate(dense.ctx.h, dense.h, _p(rx), len(rx), _p(ry), len(ry), _p(out)))
         return out
 
     @staticmethod
@@ -1186,7 +1191,7 @@ class SparseMatPolynomial:
         ctx = ctx or default_context()
         h = _vp()
         entry = lib.sp_spmat_create_device if device else lib.sp_spmat_create
-        ctx.check(entry(ctx.h, arr, C.c_int(len(polys)), _sz(x), _sz(y), C.byref(h)))
+        ctx.check(entry(ctx.h, arr, len(polys), x, y, C.byref(h)))
         return SparseMatProducts(ctx, h, len(polys), x, y)
 
     def _products(self):
@@ -1224,7 +1229,7 @@ class SparseMatProducts(_Handle):
         """[M_m z for every matrix m]: b DensePolynomials of num_rows entries; len(z) must be num_cols"""
         z = self._vector(z)
         outs = (_vp * self.batch_size)()
-        self.ctx.check(lib.sp_spmat_multiply_vec(self.ctx.h, self.h, _sz(num_rows), _sz(num_cols), z.h, outs))
+        self.ctx.check(lib.sp_spmat_multiply_vec(self.ctx.h, self.h, num_rows, num_cols, z.h, outs))
         return [DensePolynomial._wrap(self.ctx, _vp(outs[i])) for i in range(self.batch_size)]
 
     def compute_eval_table_sparse(self, rx, num_rows, num_cols, weights=None):
@@ -1236,7 +1241,7 @@ class SparseMatProducts(_Handle):
             raise SpartanB200Error("compute_eval_table_sparse: %d weights for %d matrices" % (len(w), self.batch_size))
         n = 1 if w is not None else self.batch_size
         outs = (_vp * n)()
-        self.ctx.check(lib.sp_spmat_eval_table(self.ctx.h, self.h, rx.h, _sz(num_rows), _sz(num_cols), None if w is None else _p(w), outs))
+        self.ctx.check(lib.sp_spmat_eval_table(self.ctx.h, self.h, rx.h, num_rows, num_cols, None if w is None else _p(w), outs))
         res = [DensePolynomial._wrap(self.ctx, _vp(outs[i])) for i in range(n)]
         return res[0] if w is not None else res
 
@@ -1256,7 +1261,7 @@ class SparseMatPolyEvalProof:
         rx, ry = _limbs(rx), _limbs(ry)
         out, n = C.POINTER(C.c_ubyte)(), _sz()
         ev = np.zeros((dense.batch_size, 4), dtype=np.uint64)
-        ctx.check(lib.sp_spark_eval_prove_t(ctx.h, dense.h, gens.h, _p(rx), _sz(len(rx)), _p(ry), _sz(len(ry)),
+        ctx.check(lib.sp_spark_eval_prove_t(ctx.h, dense.h, gens.h, _p(rx), len(rx), _p(ry), len(ry),
                                             None if evals is None else _p(_limbs(evals)), t.state, tape.state, C.byref(out), C.byref(n), _p(ev)))
         return SparseMatPolyEvalProof(_take_bytes(out, n)), ev
 
@@ -1264,8 +1269,8 @@ class SparseMatPolyEvalProof:
         """SparseMatPolyEvalProof::verify: raises ProofVerifyError; the transcript is advanced as the reference's verify advances it"""
         t, rx, ry, ev = _transcript_state(transcript), _limbs(rx), _limbs(ry), _limbs(evals)
         cb = comm.to_bytes() if isinstance(comm, SparseMatPolyCommitment) else bytes(comm)
-        gens.ctx.check(lib.sp_spark_eval_verify_t(gens.ctx.h, gens.h, C.c_char_p(cb), _sz(len(cb)), _p(rx), _sz(len(rx)), _p(ry), _sz(len(ry)), _p(ev),
-                                                  C.c_int(len(ev)), t.state, C.c_char_p(self.data), _sz(len(self.data))))
+        gens.ctx.check(lib.sp_spark_eval_verify_t(gens.ctx.h, gens.h, cb, len(cb), _p(rx), len(rx), _p(ry), len(ry), _p(ev),
+                                                  len(ev), t.state, self.data, len(self.data)))
 
 
 # ----------------------------------------------------------------------------- public API of lib.rs
@@ -1299,7 +1304,7 @@ class Instance(_Handle):
     def __init__(self, ctx, h):
         self.ctx, self.h = ctx, h
         nc, nv, ni = _sz(), _sz(), _sz()
-        lib.sp_instance_dims(h, C.byref(nc), C.byref(nv), C.byref(ni))
+        _check_host(lib.sp_instance_dims(h, C.byref(nc), C.byref(nv), C.byref(ni)))
         self.num_cons, self.num_vars, self.num_inputs = nc.value, nv.value, ni.value
         self._digest = None
 
@@ -1315,8 +1320,8 @@ class Instance(_Handle):
             return rows, cols, vals, len(t)
         a, b, c = split(A), split(B), split(Cm)
         h = _vp()
-        ctx.check(lib.sp_instance_create(ctx.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), _p(a[0]), _p(a[1]), C.c_char_p(a[2]), _sz(a[3]),
-                                         _p(b[0]), _p(b[1]), C.c_char_p(b[2]), _sz(b[3]), _p(c[0]), _p(c[1]), C.c_char_p(c[2]), _sz(c[3]), C.byref(h)))
+        ctx.check(lib.sp_instance_create(ctx.h, num_cons, num_vars, num_inputs, _p(a[0]), _p(a[1]), a[2], a[3],
+                                         _p(b[0]), _p(b[1]), b[2], b[3], _p(c[0]), _p(c[1]), c[2], c[3], C.byref(h)))
         return Instance(ctx, h)
 
     @staticmethod
@@ -1339,9 +1344,9 @@ class Instance(_Handle):
         _sync_torch(ctx)
         args = []
         for rows, cols, vals in mats:
-            args += [_vp(rows.data_ptr()), _vp(cols.data_ptr()), _vp(vals.data_ptr()), _sz(rows.shape[0])]
+            args += [_vp(rows.data_ptr()), _vp(cols.data_ptr()), _vp(vals.data_ptr()), rows.shape[0]]
         h = _vp()
-        ctx.check(lib.sp_instance_create_device(ctx.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), *args, C.byref(h)))
+        ctx.check(lib.sp_instance_create_device(ctx.h, num_cons, num_vars, num_inputs, *args, C.byref(h)))
         return Instance(ctx, h)
 
     @staticmethod
@@ -1351,42 +1356,40 @@ class Instance(_Handle):
         h = _vp()
         vars_out = np.zeros((num_vars, 4), dtype=np.uint64)
         inputs_out = np.zeros((num_inputs, 4), dtype=np.uint64)
-        ctx.check(lib.sp_instance_synthetic(ctx.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), C.c_uint64(seed), C.byref(h), _p(vars_out), _p(inputs_out)))
+        ctx.check(lib.sp_instance_synthetic(ctx.h, num_cons, num_vars, num_inputs, seed, C.byref(h), _p(vars_out), _p(inputs_out)))
         return Instance(ctx, h), Assignment(vars_out), Assignment(inputs_out)
 
     def bincode(self):
         out, n = C.POINTER(C.c_ubyte)(), _sz()
-        lib.sp_instance_bincode(self.h, C.byref(out), C.byref(n))
-        b = C.string_at(out, n.value)
-        lib.sp_free(out)
-        return b
+        _check_host(lib.sp_instance_bincode(self.h, C.byref(out), C.byref(n)))
+        return _take_bytes(out, n)
 
     @property
     def digest(self):
         """R1CSShape::get_digest (r1cs.rs:154-158): the caller-supplied bytes, else the library's miniz-level-6 zlib stream of bincode(shape)"""
         if self._digest is None:
             out, n = C.POINTER(C.c_ubyte)(), _sz()
-            lib.sp_instance_digest(self.h, C.byref(out), C.byref(n))
+            _check_host(lib.sp_instance_digest(self.h, C.byref(out), C.byref(n)))
             self._digest = _take_bytes(out, n)
         return self._digest
 
     def set_digest(self, digest):
         """absorb these bytes instead (e.g. the digest another compressor produced); b"" returns to the library's own"""
+        _check_host(lib.sp_instance_set_digest(self.h, bytes(digest), len(digest)))
         self._digest = bytes(digest) if digest else None
-        lib.sp_instance_set_digest(self.h, C.c_char_p(bytes(digest)), _sz(len(digest)))
 
     def export(self, matrix):
         n = _sz()
-        lib.sp_instance_nnz(self.h, C.c_int(matrix), C.byref(n))
+        _check_host(lib.sp_instance_nnz(self.h, matrix, C.byref(n)))
         row = np.zeros(n.value, dtype=np.uint64)
         col = np.zeros(n.value, dtype=np.uint64)
         val = np.zeros((n.value, 4), dtype=np.uint64)
-        lib.sp_instance_export(self.h, C.c_int(matrix), _p(row), _p(col), _p(val))
+        _check_host(lib.sp_instance_export(self.h, matrix, _p(row), _p(col), _p(val)))
         return row, col, val
 
     def is_sat(self, vars, inputs):
         sat = C.c_int()
-        self.ctx.check(lib.sp_instance_is_sat(self.ctx.h, self.h, _p(vars.limbs), _sz(len(vars)), _p(inputs.limbs), _sz(len(inputs)), C.byref(sat)))
+        self.ctx.check(lib.sp_instance_is_sat(self.ctx.h, self.h, _p(vars.limbs), len(vars), _p(inputs.limbs), len(inputs), C.byref(sat)))
         return bool(sat.value)
 
     def evaluate(self, rx, ry):
@@ -1421,13 +1424,13 @@ class GeneratorTables(_Handle):
     def __init__(self, num_cons, num_vars, num_inputs, num_nz_entries=0, ctx=None):
         self.ctx = ctx or default_context()
         h = _vp()
-        self.ctx.check(lib.sp_gen_tables_create(self.ctx.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), _sz(num_nz_entries), C.byref(h)))
+        self.ctx.check(lib.sp_gen_tables_create(self.ctx.h, num_cons, num_vars, num_inputs, num_nz_entries, C.byref(h)))
         self.h = h
 
     def info(self):
         """one dict per generator set: label, nbases, window_bits, has_row_table, device_bytes"""
         out, n = (_GenSetInfo * 2)(), _sz()
-        self.ctx.check(lib.sp_gen_tables_info(self.h, out, _sz(2), C.byref(n)))
+        self.ctx.check(lib.sp_gen_tables_info(self.h, out, 2, C.byref(n)))
         return [{"label": s.label.decode(), "nbases": int(s.nbases), "window_bits": int(s.window_bits), "has_row_table": bool(s.has_row_table),
                  "device_bytes": int(s.device_bytes)} for s in out[:n.value]]
 
@@ -1446,9 +1449,9 @@ class NIZKGens(_Handle):
         self.ctx = ctx or (tables.ctx if tables is not None else default_context())
         h = _vp()
         if tables is None:
-            self.ctx.check(lib.sp_nizk_gens_create(self.ctx.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), C.byref(h)))
+            self.ctx.check(lib.sp_nizk_gens_create(self.ctx.h, num_cons, num_vars, num_inputs, C.byref(h)))
         else:
-            self.ctx.check(lib.sp_nizk_gens_create_from(self.ctx.h, tables.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), C.byref(h)))
+            self.ctx.check(lib.sp_nizk_gens_create_from(self.ctx.h, tables.h, num_cons, num_vars, num_inputs, C.byref(h)))
         self.h = h
 
     @staticmethod
@@ -1466,7 +1469,7 @@ class R1CSGens(_Handle):
         self.ctx = ctx or default_context()
         self.num_cons, self.num_vars = num_cons, num_vars
         h = _vp()
-        self.ctx.check(lib.sp_r1cs_gens_create(self.ctx.h, C.c_char_p(bytes(label)), _sz(len(label)), _sz(num_cons), _sz(num_vars), C.byref(h)))
+        self.ctx.check(lib.sp_r1cs_gens_create(self.ctx.h, bytes(label), len(label), num_cons, num_vars, C.byref(h)))
         self.h = h
 
     @classmethod
@@ -1478,7 +1481,7 @@ class R1CSGens(_Handle):
         o = cls.__new__(cls)
         o.ctx, o.num_cons, o.num_vars = gens_or_tables.ctx, num_cons, num_vars
         h = _vp()
-        o.ctx.check(entry(o.ctx.h, gens_or_tables.h, _sz(num_cons), _sz(num_vars), C.byref(h)))
+        o.ctx.check(entry(o.ctx.h, gens_or_tables.h, num_cons, num_vars, C.byref(h)))
         o.h = h
         return o
 
@@ -1521,7 +1524,7 @@ class R1CSProof:
         out, n = C.POINTER(C.c_ubyte)(), _sz()
         rx = np.zeros((max(num_cons.bit_length() - 1, 1), 4), dtype=np.uint64)
         ry = np.zeros((max((2 * num_vars).bit_length() - 1, 1), 4), dtype=np.uint64)
-        ctx.check(lib.sp_r1cs_prove_t(ctx.h, inst, spmat, _sz(num_cons), _sz(num_vars), v.h, _p(x), _sz(len(x)), gens.h, transcript.state, tape.state,
+        ctx.check(lib.sp_r1cs_prove_t(ctx.h, inst, spmat, num_cons, num_vars, v.h, _p(x), len(x), gens.h, transcript.state, tape.state,
                                       C.byref(out), C.byref(n), _p(rx), _p(ry)))
         return R1CSProof(_take_bytes(out, n)), rx[:num_cons.bit_length() - 1], ry[:(2 * num_vars).bit_length() - 1]
 
@@ -1534,8 +1537,7 @@ class R1CSProof:
             raise SpartanB200Error("R1CSProof.verify: %d evals; (Ar, Br, Cr) expected" % len(ev))
         nx, ny = max(num_cons, 1).bit_length() - 1, max(2 * num_vars, 1).bit_length() - 1
         rx, ry = np.zeros((max(nx, 1), 4), dtype=np.uint64), np.zeros((max(ny, 1), 4), dtype=np.uint64)
-        ctx.check(lib.sp_r1cs_verify_t(ctx.h, C.c_char_p(self.data), _sz(len(self.data)), _sz(num_cons), _sz(num_vars), _p(x), _sz(len(x)), _p(ev),
-                                       gens.h, transcript.state, _p(rx), _p(ry)))
+        ctx.check(lib.sp_r1cs_verify_t(ctx.h, self.data, len(self.data), num_cons, num_vars, _p(x), len(x), _p(ev), gens.h, transcript.state, _p(rx), _p(ry)))
         return rx[:nx], ry[:ny]
 
 
@@ -1554,24 +1556,24 @@ class NIZK:
         out, n = C.POINTER(C.c_ubyte)(), _sz()
         if isinstance(transcript_label, Transcript):   # the caller's `&mut Transcript`: advanced in place
             v = vars.to_numpy() if isinstance(vars, DensePolynomial) else vars.limbs
-            ctx.check(lib.sp_nizk_prove_t(ctx.h, inst.h, _p(v), _sz(len(v)), _p(inputs.limbs), _sz(len(inputs)), gens.h, transcript_label.state, _p(seed),
+            ctx.check(lib.sp_nizk_prove_t(ctx.h, inst.h, _p(v), len(v), _p(inputs.limbs), len(inputs), gens.h, transcript_label.state, _p(seed),
                                           C.byref(out), C.byref(n)))
         elif isinstance(vars, DensePolynomial):
-            ctx.check(lib.sp_nizk_prove_resident(ctx.h, inst.h, vars.h, _p(inputs.limbs), _sz(len(inputs)), gens.h, C.c_char_p(transcript_label),
-                                                 _sz(len(transcript_label)), _p(seed), C.byref(out), C.byref(n)))
+            ctx.check(lib.sp_nizk_prove_resident(ctx.h, inst.h, vars.h, _p(inputs.limbs), len(inputs), gens.h, bytes(transcript_label),
+                                                 len(transcript_label), _p(seed), C.byref(out), C.byref(n)))
         else:
-            ctx.check(lib.sp_nizk_prove(ctx.h, inst.h, _p(vars.limbs), _sz(len(vars)), _p(inputs.limbs), _sz(len(inputs)), gens.h,
-                                        C.c_char_p(transcript_label), _sz(len(transcript_label)), _p(seed), C.byref(out), C.byref(n)))
+            ctx.check(lib.sp_nizk_prove(ctx.h, inst.h, _p(vars.limbs), len(vars), _p(inputs.limbs), len(inputs), gens.h,
+                                        bytes(transcript_label), len(transcript_label), _p(seed), C.byref(out), C.byref(n)))
         return NIZK(_take_bytes(out, n))
 
     def verify(self, inst, inputs, transcript_label, gens):
         """NIZK::verify(&self, &inst, &inputs, &mut Transcript::new(transcript_label), &gens): returns None, raises ProofVerifyError"""
         ctx = inst.ctx
         if isinstance(transcript_label, Transcript):
-            ctx.check(lib.sp_nizk_verify_t(ctx.h, inst.h, _p(inputs.limbs), _sz(len(inputs)), gens.h, transcript_label.state, C.c_char_p(bytes(self.bytes)), _sz(len(self.bytes))))
+            ctx.check(lib.sp_nizk_verify_t(ctx.h, inst.h, _p(inputs.limbs), len(inputs), gens.h, transcript_label.state, bytes(self.bytes), len(self.bytes)))
             return
-        ctx.check(lib.sp_nizk_verify(ctx.h, inst.h, _p(inputs.limbs), _sz(len(inputs)), gens.h, C.c_char_p(transcript_label), _sz(len(transcript_label)),
-                                     C.c_char_p(bytes(self.bytes)), _sz(len(self.bytes))))
+        ctx.check(lib.sp_nizk_verify(ctx.h, inst.h, _p(inputs.limbs), len(inputs), gens.h, bytes(transcript_label), len(transcript_label),
+                                     bytes(self.bytes), len(self.bytes)))
 
     @staticmethod
     def verify_batch(proofs, inst, inputs, transcript_label, gens, seed=None):
@@ -1591,10 +1593,9 @@ class SNARKGens(_Handle):
         self.ctx = ctx or (tables.ctx if tables is not None else default_context())
         h = _vp()
         if tables is None:
-            self.ctx.check(lib.sp_snark_gens_create(self.ctx.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), _sz(num_nz_entries), C.byref(h)))
+            self.ctx.check(lib.sp_snark_gens_create(self.ctx.h, num_cons, num_vars, num_inputs, num_nz_entries, C.byref(h)))
         else:
-            self.ctx.check(lib.sp_snark_gens_create_from(self.ctx.h, tables.h, _sz(num_cons), _sz(num_vars), _sz(num_inputs), _sz(num_nz_entries),
-                                                         C.byref(h)))
+            self.ctx.check(lib.sp_snark_gens_create_from(self.ctx.h, tables.h, num_cons, num_vars, num_inputs, num_nz_entries, C.byref(h)))
         self.h = h
 
     @staticmethod
@@ -1614,12 +1615,12 @@ class ComputationCommitment(_Handle):
         """a verifier's view: bincode(ComputationCommitment) only (cannot be used to prove)"""
         ctx = ctx or default_context()
         h = _vp()
-        ctx.check(lib.sp_snark_commitment_load(ctx.h, C.c_char_p(bytes(data)), _sz(len(data)), C.byref(h)))
+        ctx.check(lib.sp_snark_commitment_load(ctx.h, bytes(data), len(data), C.byref(h)))
         return cls(ctx, h)
 
     def commitment_bytes(self):
         out, n = C.POINTER(C.c_ubyte)(), _sz()
-        lib.sp_snark_commitment_bytes(self.h, C.byref(out), C.byref(n))
+        _check_host(lib.sp_snark_commitment_bytes(self.h, C.byref(out), C.byref(n)))
         return _take_bytes(out, n)
 
 
@@ -1645,24 +1646,24 @@ class SNARK:
         out, n = C.POINTER(C.c_ubyte)(), _sz()
         if isinstance(transcript_label, Transcript):   # the caller's `&mut Transcript`: advanced in place
             v = vars.to_numpy() if isinstance(vars, DensePolynomial) else vars.limbs
-            ctx.check(lib.sp_snark_prove_t(ctx.h, inst.h, comm.h, _p(v), _sz(len(v)), _p(inputs.limbs), _sz(len(inputs)), gens.h, transcript_label.state, _p(seed),
+            ctx.check(lib.sp_snark_prove_t(ctx.h, inst.h, comm.h, _p(v), len(v), _p(inputs.limbs), len(inputs), gens.h, transcript_label.state, _p(seed),
                                            C.byref(out), C.byref(n)))
         elif isinstance(vars, DensePolynomial):
-            ctx.check(lib.sp_snark_prove_resident(ctx.h, inst.h, comm.h, vars.h, _p(inputs.limbs), _sz(len(inputs)), gens.h, C.c_char_p(transcript_label),
-                                                  _sz(len(transcript_label)), _p(seed), C.byref(out), C.byref(n)))
+            ctx.check(lib.sp_snark_prove_resident(ctx.h, inst.h, comm.h, vars.h, _p(inputs.limbs), len(inputs), gens.h, bytes(transcript_label),
+                                                  len(transcript_label), _p(seed), C.byref(out), C.byref(n)))
         else:
-            ctx.check(lib.sp_snark_prove(ctx.h, inst.h, comm.h, _p(vars.limbs), _sz(len(vars)), _p(inputs.limbs), _sz(len(inputs)), gens.h,
-                                         C.c_char_p(transcript_label), _sz(len(transcript_label)), _p(seed), C.byref(out), C.byref(n)))
+            ctx.check(lib.sp_snark_prove(ctx.h, inst.h, comm.h, _p(vars.limbs), len(vars), _p(inputs.limbs), len(inputs), gens.h,
+                                         bytes(transcript_label), len(transcript_label), _p(seed), C.byref(out), C.byref(n)))
         return SNARK(_take_bytes(out, n))
 
     def verify(self, comm, inputs, transcript_label, gens):
         """SNARK::verify(&self, &comm, &inputs, &mut Transcript::new(transcript_label), &gens): returns None, raises ProofVerifyError"""
         ctx = comm.ctx
         if isinstance(transcript_label, Transcript):
-            ctx.check(lib.sp_snark_verify_t(ctx.h, comm.h, _p(inputs.limbs), _sz(len(inputs)), gens.h, transcript_label.state, C.c_char_p(bytes(self.bytes)), _sz(len(self.bytes))))
+            ctx.check(lib.sp_snark_verify_t(ctx.h, comm.h, _p(inputs.limbs), len(inputs), gens.h, transcript_label.state, bytes(self.bytes), len(self.bytes)))
             return
-        ctx.check(lib.sp_snark_verify(ctx.h, comm.h, _p(inputs.limbs), _sz(len(inputs)), gens.h, C.c_char_p(transcript_label), _sz(len(transcript_label)),
-                                      C.c_char_p(bytes(self.bytes)), _sz(len(self.bytes))))
+        ctx.check(lib.sp_snark_verify(ctx.h, comm.h, _p(inputs.limbs), len(inputs), gens.h, bytes(transcript_label), len(transcript_label),
+                                      bytes(self.bytes), len(self.bytes)))
 
     @staticmethod
     def verify_batch(proofs, comm, inputs, transcript_label, gens, seed=None):
@@ -1699,12 +1700,12 @@ def _verify_batch(ctx, entry, entry_t, handles, proofs, inputs, transcript_label
         raise SpartanB200Error("verify_batch: transcript_label mixes Transcript objects and labels")
     if all(isinstance(t, Transcript) for t in transcript_label):
         states = (_vp * k)(*[C.cast(t.state, _vp) for t in transcript_label])
-        rc = entry_t(ctx.h, _sz(k), hs, ins, nins, gens.h, states, pbuf, plens, C.c_char_p(seed), status)
+        rc = entry_t(ctx.h, k, hs, ins, nins, gens.h, states, pbuf, plens, seed, status)
     else:
         labels = [bytes(t) for t in transcript_label]
         lbuf = (C.c_char_p * k)(*labels)
         llens = (_sz * k)(*[len(t) for t in labels])
-        rc = entry(ctx.h, _sz(k), hs, ins, nins, gens.h, lbuf, llens, pbuf, plens, C.c_char_p(seed), status)
+        rc = entry(ctx.h, k, hs, ins, nins, gens.h, lbuf, llens, pbuf, plens, seed, status)
     if rc not in (SP_OK, SP_ERR_VERIFY):
         ctx.check(rc)
     out = []
@@ -1732,15 +1733,13 @@ def io_bytes():
 
 
 def prof_enable(on=True):
-    lib.sp_prof_enable(C.c_int(1 if on else 0))
+    lib.sp_prof_enable(1 if on else 0)
 
 
 def prof_report():
     """{kernel family: {"launches", "ms", "bytes"}} measured with CUDA events on the launching stream"""
-    buf = C.create_string_buffer(1 << 16)
-    lib.sp_prof_report(buf, _sz(1 << 16))
     out = {}
-    for item in buf.value.decode().split(";"):
+    for item in _string_out(_check_host, lib.sp_prof_report).split(";"):
         if item:
             name, n, ms, by, bb, bms = item.split(":")
             out[name] = {"launches": int(n), "ms": float(ms), "bytes": float(by), "largest_bytes": float(bb), "largest_ms": float(bms)}
